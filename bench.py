@@ -2,7 +2,7 @@
 """bench.py -- images/sec of the GAN train step (adversarial.lua loop body: 1 D iteration + 1 G iteration,
 both Adam updates) on synthetic 3x32x32 batches, batch 256 per GPU (BASELINE.json configs[1]; weak scaling).
 
-  python bench.py --gpus N --steps K --warmup W              our arm (libfg_b200.so through the C ABI)
+  python bench.py --gpus N --steps K --warmup W              our arm (libfg_b200.so through the C ABI, sm_90a)
   python bench.py --impl reference --gpus N --steps K ...    the reference's CPU math (oracle fp32 port; Torch7
                                                              itself cannot run in this image, see DESIGN.md)
 Prints ONE JSON line on rank 0.
@@ -58,7 +58,7 @@ def workload_config(world, B=256):
     """the `config` object both arms print (the reference arm runs our arm's config, bench contract)"""
     return {"workload": "train.lua color 3x32x32 batch=256 per GPU (BASELINE configs[1]), 1 D-iter + 1 G-iter, Adam",
             "global_batch": B * world, "per_gpu_batch": B, "parallelism": "dp%d" % world, "dropout": "in-kernel RNG",
-            "l2": "per-step working set (activations+grads ~1.5 GB) >> 126 MB L2, no explicit flush"}
+            "l2": "per-step working set (activations+grads ~1.5 GB) >> 50 MB L2, no explicit flush"}
 
 
 class CpuPort:
@@ -111,34 +111,8 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], bf16=d["bf16_tflops"], bf16_sus=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     src="measured")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sus=1400.0, src="fallback")
-
-
-def ncu_traffic(profile="r2_ncu_f16_tapconv.md"):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the G.C2 forward launch at batch 256 (the first kernel of the
-    committed `ncu --set full` summary; a number taken under the profiler, quoted only as traffic, never as time)."""
-    import re
-    try:
-        txt = open(os.path.join(ROOT, "profiles", profile)).read().split("\n## ")[1]
-        scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-        tot = 0.0
-        for key in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-            m = re.search(r"\| %s \| ([0-9.,]+) \| (\w+) \|" % re.escape(key), txt)
-            tot += float(m.group(1).replace(",", "")) * scale[m.group(2)]
-        return tot, "profiles/" + profile
-    except Exception:
-        return None, None
-
-
-def ncu_pipe_active(profile="r2_ncu_f16_tapconv.md"):
-    """sm__pipe_tensor_cycles_active (% of peak) of the G.C2 forward launch in the committed `ncu --set full` summary"""
-    import re
-    try:
-        txt = open(os.path.join(ROOT, "profiles", profile)).read().split("\n## ")[1]
-        m = re.search(r"\| sm__pipe_tensor_cycles_active\.avg\.pct_of_peak_sustained_active \| ([0-9.,]+) \|", txt)
-        return float(m.group(1).replace(",", "")), "profiles/" + profile
-    except Exception:
-        return None, None
+    # NVIDIA's data sheet for the H100 SXM (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- not reached figures
+    return dict(hbm=3350.0, bf16=989.0, bf16_sus=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -241,6 +215,17 @@ def secondary_configs(steps=5):
     return res
 
 
+def dump_outputs(ctx, out_dir):
+    """The state one train step leaves behind, as a caller of fg_train_step reads it back: updated parameters, the
+    step's gradients and the BatchNorm running statistics (~43 MB of float32 for the colour nets)."""
+    from face_generator_b200.lib import NET_D, NET_G
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"params_G": ctx.get_params(NET_G), "params_D": ctx.get_params(NET_D), "grads_G": ctx.get_grads(NET_G),
+              "grads_D": ctx.get_grads(NET_D), "bn_state_G": ctx.get_bn_state()}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -248,10 +233,13 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--batch", type=int, default=256, help="per-GPU batch (BASELINE configs[1]: 256)")
-    ap.add_argument("--conv-impl", type=int, default=-1, help="0 simt, 1 tcgen05 dense, 2 tcgen05 collapsed; -1 library default")
+    ap.add_argument("--conv-impl", type=int, default=-1, help="0 simt, 1 wgmma dense, 2 wgmma collapsed; -1 library default")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the configs[0]/[3]/[4] lines of the `secondary` block")
     ap.add_argument("--breakdown", action="store_true", help="per-layer kernel timings in kernel_ms_per_step")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (parameters, gradients and BatchNorm "
+                         "running state of rank 0) as DIR/<name>.npy in float32")
     args = ap.parse_args()
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local = int(os.environ.get("LOCAL_RANK", 0))
@@ -326,6 +314,8 @@ def main():
     ms = timed(step_resident, K)
     launches = ctx.launches() - l0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(ctx, args.dump_outputs)
     for _ in range(2):
         step_e2e()
     ms_e2e = timed(step_e2e, K)
@@ -368,7 +358,7 @@ def main():
     if rank == 0:
         try:
             tf32_peak = ctx.tf32_peak(20000)
-            os.environ["FG_TF32_PROBE_F16"] = "1"  # the same loop with kind::f16 instructions (128x256x16)
+            os.environ["FG_TF32_PROBE_F16"] = "1"  # the same loop with f16 instructions (m64n256k16)
             f16_peak = ctx.tf32_peak(20000)
             os.environ.pop("FG_TF32_PROBE_F16")
             os.environ["FG_TF32_PROBE_N"] = "128"  # the N=128 instruction shape
@@ -387,45 +377,41 @@ def main():
     t_c2 = (fam["G.C2.fwd"][0] + fam["G.C2.dgrad"][0] + fam["G.C2.wgrad"][0]) / 1e3
     tf_c2 = 3.5 * B * F_GC2 / t_c2 / 1e12 if t_c2 > 0 else 0.0
     f16 = bool(ctx.get_option("mma_f16")) and ctx.get_option("conv_impl") == 2
-    # kind::f16 MMAs run at the bf16 dense rate, kind::tf32 at half of it
+    # f16 MMAs run at the bf16 dense rate, tf32 at half of it
     peak = peaks["bf16_sus"] if f16 else peaks["bf16_sus"] / 2.0
     mma_peak = f16_peak if f16 else tf32_peak
-    traffic, traffic_src = ncu_traffic()
     # executed tensor-core work of that launch: 3 MMAs per logical MMA (3-term split), 9/25 of the taps (phase collapse)
     collapsed = ctx.get_option("conv_impl") == 2
     exec_ratio = 3.0 * (9.0 / 25.0 if collapsed else 1.0)
-    pipe_pct, pipe_src = ncu_pipe_active()
     out = {
         "metric": METRIC, "value": value, "unit": "images/s", "n_gpus": world, "steps": K, "warmup": W,
         "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
         "data": "synthetic",
         "config": workload_config(world, B),
         "config_detail": {"conv_impl": ctx.get_option("conv_impl"), "mma_f16": int(f16),
-                          "operand_split": "3xFP16 (kind::f16, fp32 accumulate)" if f16 else "3xTF32 (kind::tf32)"},
+                          "operand_split": "3xFP16 (f16 wgmma, fp32 accumulate)" if f16 else "3xTF32 (tf32 wgmma)"},
         "e2e": {"value": e2e, "unit": "images/s", "ms_per_step": ms_e2e / K,
                 "h2d_bytes_per_step": int(real.nbytes + nD.nbytes + nG.nbytes), "d2h_bytes_per_step": 40},
         "gpu_launches": int(launches),
         "clocks": clocks,
         "roofline": {"kernel": "G.C2 5x5 conv 256->128 @32x32 forward (implicit GEMM M=B*1024,N=128,K=6400)",
                      "bound": "tensor", "achieved": tf_fwd, "peak": peak, "unit": "TFLOP/s",
-                     "frac": tf_fwd / peak, "traffic": traffic,
-                     "traffic_note": "DRAM bytes of the batch-%d launch (%s); algorithmic bytes of that launch: "
-                                     "input hi+lo %s MB + output 134.2 MB + weights %s MB" % (
-                                         256, traffic_src, "2x33.6" if f16 else "2x67.1", "4.7" if f16 else "9.4"),
-                     "peak_source": ("%s bf16 sustained %.1f TF (kind::f16 runs at the bf16 rate); algorithmic fp32 FLOPs" if f16 else
-                                     "%s bf16 sustained %.1f TF / 2 (kind::tf32 is half rate); algorithmic fp32 FLOPs") % (
+                     "frac": tf_fwd / peak,
+                     "traffic_note": "algorithmic bytes of the batch-256 launch: input hi+lo %s MB + output 134.2 MB + "
+                                     "weights %s MB" % ("2x33.6" if f16 else "2x67.1", "4.7" if f16 else "9.4"),
+                     "peak_source": ("%s bf16 %.1f TF (f16 MMAs run at the bf16 rate); algorithmic fp32 FLOPs" if f16 else
+                                     "%s bf16 %.1f TF / 2 (tf32 MMAs run at half rate); algorithmic fp32 FLOPs") % (
                          peaks["src"], peaks["bf16_sus"]),
                      "executed_mma_tflops": tf_fwd * exec_ratio,
-                     "executed_note": "kind::%s MMAs actually issued: 3 per logical MMA (hi*hi + hi*lo + lo*hi)%s" % (
+                     "executed_note": "%s MMAs actually issued: 3 per logical MMA (hi*hi + hi*lo + lo*hi)%s" % (
                          "f16" if f16 else "tf32", " x 9/25 taps (upsample folded into four 3x3 phase convolutions)" if collapsed else ""),
                      "measured_f16_peak": f16_peak,
                      "measured_tf32_peak": tf32_peak,
                      "measured_tf32_peak_n128": tf32_peak_n128,
-                     "measured_tf32_peak_note": "fg_bench_tf32_peak: back-to-back tcgen05.mma.kind::tf32 128x256x8, cta_group::1, "
+                     "measured_tf32_peak_note": "fg_bench_tf32_peak: back-to-back tf32 wgmma m64n256k8, two warpgroups per SM, "
                                                 "smem-resident operands, all SMs, run at bench clocks right after the timed region",
                      "frac_executed_vs_measured_mma_peak": (tf_fwd * exec_ratio / mma_peak) if mma_peak else None,
                      "frac_algorithmic_vs_measured_mma_peak": (tf_fwd / mma_peak) if mma_peak else None,
-                     "pipe_active_pct": pipe_pct, "pipe_active_src": pipe_src,
                      "family_fwd_dgrad_wgrad_tflops": tf_c2,
                      "step_algorithmic_tflops": F_ITER_PER_IMG * B * K / (ms / 1e3) / 1e12},
         "hbm_kernels": [{"kernel": k[4:] if k.startswith("hbm.") else k, "bytes_per_step": int(nb), "ms_per_step": round(ms_k, 4),

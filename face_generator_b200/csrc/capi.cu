@@ -56,7 +56,7 @@ int to_user(fg_ctx* c, float* dst, const float* src_dev, size_t n) {
 
 extern "C" {
 
-const char* fg_version(void) { return "fg_b200 0.1 (sm_100a)"; }
+const char* fg_version(void) { return "fg_b200 0.1 (sm_90a)"; }
 const char* fg_last_error(void) { return g_err; }
 
 void fg_hyper_default(fg_hyper* h) {
@@ -83,8 +83,8 @@ int fg_create(fg_ctx** out, int device, int max_batch, int channels) {
   FG_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   FG_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    fg_set_error("fg_create: device %d is sm_%d%d; this library only contains sm_100a code", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    fg_set_error("fg_create: device %d is sm_%d%d; this library only contains sm_90a code", device, prop.major, prop.minor);
     return FG_ERR_UNSUPPORTED;
   }
   fg_ctx* c = new fg_ctx();
@@ -174,7 +174,7 @@ int fg_set_option(fg_ctx* c, const char* key, int64_t v) {
     c->bn_epilogue = v != 0;
     return FG_OK;
   }
-  if (!strcmp(key, "mma_f16")) {  // 1: K-major tensor-core kernels (forward, dgrad) use the 3xFP16 split + kind::f16 MMAs
+  if (!strcmp(key, "mma_f16")) {  // 1: K-major tensor-core kernels (forward, dgrad) use the 3xFP16 split + f16 MMAs
     c->mma_f16 = v != 0;
     c->G_packed = c->D_packed = false;
     return FG_OK;
@@ -551,13 +551,6 @@ int64_t fg_debug_tensor(fg_ctx* c, const char* name, float* dst, int64_t max_ele
   return -1;
 }
 
-// tests: tensor-core operand taken as a shifted window of a haloed, 128B-swizzled tile (see tc_umma_window_probe)
-int fg_debug_umma_window(fg_ctx* c, const float* x_dev, const float* ident_dev, int dy, int dx, int use_base_offset,
-                         float* out_dev) {
-  ENTER(c);
-  FG_REQUIRE(x_dev && ident_dev && out_dev && dy >= 0 && dy <= 2 && dx >= 0 && dx <= 7, "fg_debug_umma_window: bad arguments");
-  return tc_umma_window_probe(c, x_dev, ident_dev, dy, dx, use_base_offset, out_dev);
-}
 int fg_bench_tf32_peak(fg_ctx* c, int iters, double* tflops) {
   ENTER(c);
   FG_REQUIRE(tflops && iters > 0, "fg_bench_tf32_peak: bad arguments");

@@ -1,5 +1,5 @@
 // One convolution / Linear layer of the nets built outside nets.cu (coarse-to-fine nets, --scale 16 nets): weight
-// packs, TF32 splits and the forward / backward dispatch over the tcgen05, bandwidth-shaped and fp32 FFMA kernels.
+// packs, TF32 splits and the forward / backward dispatch over the wgmma, bandwidth-shaped and fp32 FFMA kernels.
 #pragma once
 #include <vector>
 

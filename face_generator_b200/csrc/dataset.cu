@@ -37,7 +37,7 @@ struct fg_dataset {
 };
 
 namespace {
-inline int grid_for(int64_t n, int block, int cap = 148 * 16) {
+inline int grid_for(int64_t n, int block, int cap = 132 * 16) {
   int64_t g = (n + block - 1) / block;
   return (int)std::max<int64_t>(1, std::min<int64_t>(g, cap));
 }

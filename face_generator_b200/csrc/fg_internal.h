@@ -37,7 +37,8 @@ void fg_set_error(const char* fmt, ...);
 constexpr int kMaskPerSample = 1984;  // 64+128+256+512 SpatialDropout + 512+512 Dropout keep flags
 constexpr int kNoiseDim = 100;
 constexpr int kSmallMaxParts = 2048;  // partial rows of the small-channel wgrad workspace
-constexpr int kGradTail = 8;          // extra floats behind each flat gradient (DP-reduced scalars)
+constexpr int kGradTail = 8;
+constexpr int kOptRedRows = 132 * 2;  // blocks of the penalty-loss reduction          // extra floats behind each flat gradient (DP-reduced scalars)
 
 // Geometry of one stride-1 "same" convolution seen as a sum over taps of shifted GEMMs.
 // Output pixels p = (b,y,x) in [0,B)x[0,H)x[0,W); the stored input is [B][H/ups][W/ups][Cin]
@@ -80,8 +81,8 @@ struct fg_ctx {
   cudaStream_t stream = nullptr;
   bool own_stream = true;
   int64_t launches = 0;
-  int conv_impl = FG_CONV_TC_COLLAPSED;  // default: tcgen05 path; FG_CONV_SIMT is the fp32 FFMA cross-check
-  int sm_count = 148;
+  int conv_impl = FG_CONV_TC_COLLAPSED;  // default: wgmma path; FG_CONV_SIMT is the fp32 FFMA cross-check
+  int sm_count = 132;
   // OPT.D_optmethod / OPT.G_optmethod (train.lua:38-39): FG_OPT_ADAM | FG_OPT_ADAGRAD | FG_OPT_SGD, and SGD momentum
   int opt_D = 0, opt_G = 0;
   float sgd_mom_D = 0.f, sgd_mom_G = 0.f;
@@ -108,6 +109,16 @@ struct fg_ctx {
   float* small_ws = nullptr;  // per-block partials of the small-channel wgrad (k_conv_small.cu)
   float* wgrad_ws = nullptr;  // packed weight-gradient workspace (largest layer)
   size_t wgrad_ws_elems = 0;
+  // Cross-block sums are never accumulated with float / double atomics, whose order varies from run to run: split-K
+  // weight gradients write one partial per split into splitk_ws and k_splitk_reduce adds them in split order; the
+  // reduction kernels write one row of partials per block into red_ws and the last block to finish (red_ticket)
+  // adds the rows in block order (k_ordered.cuh).  A step is bit-reproducible given its inputs and seed.
+  float* splitk_ws = nullptr;
+  size_t splitk_ws_elems = 0;
+  double* red_ws = nullptr;
+  size_t red_ws_elems = 0;
+  double* red_ws_opt = nullptr;  // [kOptRedRows]: the penalty-loss sum of the optimizer, which may run on comm_stream
+  unsigned* red_ticket = nullptr;  // [0]: red_ws, [1]: red_ws_opt
   // G activations (NHWC)
   int G_B = 0;
   bool G_train = true, G_fwd_valid = false;
@@ -117,7 +128,7 @@ struct fg_ctx {
   float* bn_parts = nullptr;  // [m-tile][2][C] BatchNorm partials written by the tensor-core conv epilogue
   int edge_impl = 1;          // option "edge_impl": 0 = the round-1 small-channel kernels (k_conv_small.cu) for G.C3 / D.C1
   int bn_epilogue = 1;        // option "bn_epilogue": 0 = separate statistics pass over z (the round-1 path)
-  int mma_f16 = 1;            // option "mma_f16": 1 (default) = tensor-core operands in the 3xFP16 split (kind::f16 MMAs); 0 = 3xTF32
+  int mma_f16 = 1;            // option "mma_f16": 1 (default) = tensor-core operands in the 3xFP16 split (f16 MMAs); 0 = 3xTF32
   float* amax_slot = nullptr; // [32] (max|x|, 1/scale) pairs on the device: power-of-two scales of the FP16-split operands
   unsigned* amax_out = nullptr;  // when set (nets.cu AmaxInto), the next elementwise producer also reduces max|output| there ...
   int amax_id = 0;               // ... and marks amax_valid[amax_id]: split_h_scaled then skips its own reduction pass
@@ -172,7 +183,7 @@ struct fg_ctx {
   cudaEvent_t events[16] = {};
   bool timing = false;
   std::map<std::string, TimerRec> timers;
-  // tcgen05 path: TF32 hi/lo splits of activations / gradients / packed weights (k_conv_tc.cu)
+  // tensor-core path: TF32 hi/lo splits of activations / gradients / packed weights (k_conv_tc.cu)
   struct TcBufs {
     float *G_h0_hi = nullptr, *G_h0_lo = nullptr, *G_h1_hi = nullptr, *G_h1_lo = nullptr;  // conv inputs (fwd -> wgrad)
     // G.L1 (nn.Linear 100 -> 8192, models.lua:59) as a 1x1 convolution with K padded 100 -> 128: zero-padded noise
@@ -307,6 +318,17 @@ int k_wgrad_small(fg_ctx* c, const float* in, const float* dY, float* dWp, ConvG
 // ---- k_conv_edge.cu: the same layers at width 32, weights in registers, TMA / smem staged (the default) ----------
 bool k_edge_eligible(const ConvGeom& g);
 int k_conv_edge(fg_ctx* c, const float* in, const float* Wp, const float* bias, float* out, ConvGeom g);
+
+// the ordered reductions of one launch need rows x n doubles of red_ws
+inline int red_check(fg_ctx* c, int64_t rows, int64_t n) {
+  if (rows * n > (int64_t)c->red_ws_elems) {
+    fg_set_error("ordered reduction of %lld x %lld partials exceeds its workspace", (long long)rows, (long long)n);
+    return FG_ERR_UNSUPPORTED;
+  }
+  return FG_OK;
+}
+// out[i] = sum over s in order of parts[s * n + i]  (split-K partials of a weight gradient, k_misc.cu)
+int k_splitk_reduce(fg_ctx* c, const float* parts, int splits, int64_t n, float* out);
 
 // ---- k_conv_tc.cu ----------------------------------------------------------------------------------
 int tc_init(fg_ctx* c);

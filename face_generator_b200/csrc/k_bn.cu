@@ -1,10 +1,11 @@
 // BatchNorm per-channel reductions at HBM speed (NHWC, C % 4 == 0): every thread owns 4 consecutive channels
 // (one float4 per pixel row), blockDim/(C/4) pixel rows are in flight per block iteration, accumulation in
-// double, one shared-memory tree + one double atomicAdd per channel per block.
+// double, one shared-memory tree per block, then the per-block partials are added in block order (k_ordered.cuh).
 //   stats   : acc[c] += sum z,            acc[C+c] += sum z^2                       (forward, models.lua:65,70)
 //   bwd     : acc[c] += sum g,            acc[C+c] += sum g*xhat,  *dslope += sum_{u<=0} dh*u
 //             with u = gamma*xhat+beta, g = dh*(u>0 ? 1 : a)                         (backward of BN+PReLU)
 #include "fg_internal.h"
+#include "k_ordered.cuh"
 
 #define LAUNCH_CHECK(c)                 \
   do {                                  \
@@ -19,7 +20,8 @@ __global__ void __launch_bounds__(256) bn_reduce4_kernel(const float* __restrict
                                                          const float* __restrict__ gamma, const float* __restrict__ beta,
                                                          const float* __restrict__ slope, double* __restrict__ acc,
                                                          float* __restrict__ dslope, int64_t P, int C,
-                                                         int64_t rows_per_block) {
+                                                         int64_t rows_per_block, double* __restrict__ ws,
+                                                         unsigned* __restrict__ ticket) {
   extern __shared__ double sm[];  // [2][lanes][C]
   const int C4 = C >> 2;
   const int lanes = blockDim.x / C4;
@@ -109,15 +111,18 @@ __global__ void __launch_bounds__(256) bn_reduce4_kernel(const float* __restrict
     }
   }
   __syncthreads();
+  // this block's row of partials: [sum | sum of squares / products | PReLU slope sum]
+  double* row = ws + (int64_t)blockIdx.x * (2 * C + 1);
   for (int i = threadIdx.x; i < C; i += blockDim.x) {
     double a0 = 0, a1 = 0;
     for (int l = 0; l < lanes; ++l) {
       a0 += s0[l * C + i];
       a1 += s1[l * C + i];
     }
-    atomicAdd(acc + i, a0);
-    atomicAdd(acc + C + i, a1);
+    row[i] = a0;
+    row[C + i] = a1;
   }
+  if (threadIdx.x == 0) row[2 * C] = 0.0;
   if (BWD && act && dslope) {
     // block-wide sum of ss
     __shared__ double red[32];
@@ -130,8 +135,13 @@ __global__ void __launch_bounds__(256) bn_reduce4_kernel(const float* __restrict
       double v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.0;
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if (threadIdx.x == 0) atomicAdd(dslope, (float)v);
+      if (threadIdx.x == 0) row[2 * C] = v;
     }
+  }
+  if (ordered_last_block(ticket)) {
+    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) acc[i] += ordered_sum(ws, gridDim.x, 2 * C + 1, i);
+    if (BWD && dslope && threadIdx.x == 0) *dslope += (float)ordered_sum(ws, gridDim.x, 2 * C + 1, 2 * C);
+    ordered_release(ticket);
   }
 }
 }  // namespace
@@ -144,8 +154,10 @@ int k_bn_stats4(fg_ctx* c, const float* z, double* acc, int64_t P, int C) {
   int grid = (int)std::min<int64_t>((int64_t)c->sm_count * 8, (P + lanes * 4 - 1) / (lanes * 4));
   if (grid < 1) grid = 1;
   const int64_t rpb = (P + grid - 1) / grid;
+  FG_TRY(red_check(c, grid, 2 * C + 1));
   bn_reduce4_kernel<false><<<grid, 256, sizeof(double) * 2 * lanes * C, c->stream>>>(z, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                                                                   nullptr, acc, nullptr, P, C, rpb);
+                                                                                   nullptr, acc, nullptr, P, C, rpb, c->red_ws,
+                                                                                   c->red_ticket);
   LAUNCH_CHECK(c);
   return FG_OK;
 }
@@ -156,8 +168,9 @@ int k_bn_bwd_reduce4(fg_ctx* c, const float* dh, const float* z, const float* me
   int grid = (int)std::min<int64_t>((int64_t)c->sm_count * 8, (P + lanes * 4 - 1) / (lanes * 4));
   if (grid < 1) grid = 1;
   const int64_t rpb = (P + grid - 1) / grid;
+  FG_TRY(red_check(c, grid, 2 * C + 1));
   bn_reduce4_kernel<true><<<grid, 256, sizeof(double) * 2 * lanes * C, c->stream>>>(z, dh, mean, istd, gamma, beta, slope, acc,
-                                                                                  dslope, P, C, rpb);
+                                                                                  dslope, P, C, rpb, c->red_ws, c->red_ticket);
   LAUNCH_CHECK(c);
   return FG_OK;
 }

@@ -251,9 +251,8 @@ __global__ void __launch_bounds__(256) wgrad_simt_kernel(const float* __restrict
     for (int j = 0; j < TN; ++j) {
       const int cc = c0 + tx * TN + j;
       if (cc < g.Cin) {
-        float* dst = dWp + ((int64_t)t * g.Cout + n) * g.Cin + cc;
-        if (splits > 1) atomicAdd(dst, acc[i][j]);
-        else *dst = acc[i][j];
+        // splits > 1: dWp holds one partial per split (k_splitk_reduce adds them in split order)
+        dWp[(int64_t)split * g.k * g.k * g.Cout * g.Cin + ((int64_t)t * g.Cout + n) * g.Cin + cc] = acc[i][j];
       }
     }
   }
@@ -302,12 +301,14 @@ int k_wgrad_simt(fg_ctx* c, const float* in, const float* dY, float* dWp, ConvGe
   const int max_splits = (P + 255) / 256;
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;
+  const int64_t size = (int64_t)KK * g.Cout * g.Cin;
+  while (splits > 1 && splits * size > (int64_t)c->splitk_ws_elems) --splits;  // partials must fit the split-K workspace
   int pps = (P + splits - 1) / splits;
   pps = (pps + BK - 1) / BK * BK;
   splits = (P + pps - 1) / pps;
-  if (splits > 1) FG_CUDA(cudaMemsetAsync(dWp, 0, sizeof(float) * (size_t)KK * g.Cout * g.Cin, c->stream));
+  float* dst = splits > 1 ? c->splitk_ws : dWp;
   dim3 grid(gx, gy, KK * splits);
-#define WG(TM_, TN_) wgrad_simt_kernel<TM_, TN_><<<grid, 256, 0, c->stream>>>(in, dY, dWp, g, splits, pps)
+#define WG(TM_, TN_) wgrad_simt_kernel<TM_, TN_><<<grid, 256, 0, c->stream>>>(in, dY, dst, g, splits, pps)
   if (tm == 8 && tn == 8) WG(8, 8);
   else if (tm == 8 && tn == 4) WG(8, 4);
   else if (tm == 8 && tn == 1) WG(8, 1);
@@ -319,5 +320,5 @@ int k_wgrad_simt(fg_ctx* c, const float* in, const float* dY, float* dWp, ConvGe
   else WG(1, 1);
 #undef WG
   LAUNCH_CHECK(c);
-  return FG_OK;
+  return splits > 1 ? k_splitk_reduce(c, c->splitk_ws, splits, size, dWp) : FG_OK;
 }

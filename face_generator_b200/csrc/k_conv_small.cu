@@ -204,8 +204,9 @@ __global__ void __launch_bounds__(128) wgrad_smallbig_kernel(const float* __rest
 #pragma unroll
     for (int c = 0; c < CS; ++c) dst[(t * CS + c) * Cb + cb] = acc[t][c];
 }
-// out (zeroed by the caller) += sum over a slice of the partial rows, mapped to the packed [t][n][c] layout.
-// grid.y slices the partial rows so the loads are not one long dependent chain per thread.
+// out[slice] = sum over a slice of the partial rows, mapped to the packed [t][n][c] layout (out holds gridDim.y slices
+// of `total`; k_splitk_reduce adds them in slice order).  grid.y slices the partial rows so the loads are not one long
+// dependent chain per thread.
 __global__ void wgrad_small_reduce_kernel(const float* __restrict__ part, float* __restrict__ out, int nparts, int CS, int Cb,
                                           int sign, int transposed) {
   const int total = 9 * CS * Cb;
@@ -224,7 +225,8 @@ __global__ void wgrad_small_reduce_kernel(const float* __restrict__ part, float*
   for (; i < i1; ++i) s0 += part[(size_t)i * total + j];
   const int idx = j / (CS * Cb), cs = (j / Cb) % CS, cb = j % Cb;
   const int t = sign > 0 ? idx : 8 - idx;
-  atomicAdd(out + (transposed ? ((size_t)t * Cb + cb) * CS + cs : ((size_t)t * CS + cs) * Cb + cb), (s0 + s1) + (s2 + s3));
+  out[(size_t)blockIdx.y * total + (transposed ? ((size_t)t * Cb + cb) * CS + cs : ((size_t)t * CS + cs) * Cb + cb)] =
+      (s0 + s1) + (s2 + s3);
 }
 }  // namespace
 
@@ -308,9 +310,9 @@ int k_wgrad_small(fg_ctx* c, const float* in, const float* dY, float* dWp, ConvG
 #undef WG
   LAUNCH_CHECK(c);
   const int total = 9 * Cs * Cb;
-  FG_CUDA(cudaMemsetAsync(dWp, 0, sizeof(float) * total, c->stream));
-  wgrad_small_reduce_kernel<<<dim3((total + 127) / 128, 32), 128, 0, c->stream>>>(c->small_ws, dWp, nblocks * lanes, Cs, Cb,
-                                                                                sign, transposed);
+  constexpr int kSlices = 32;
+  wgrad_small_reduce_kernel<<<dim3((total + 127) / 128, kSlices), 128, 0, c->stream>>>(c->small_ws, c->splitk_ws, nblocks * lanes,
+                                                                                     Cs, Cb, sign, transposed);
   LAUNCH_CHECK(c);
-  return FG_OK;
+  return k_splitk_reduce(c, c->splitk_ws, kSlices, total, dWp);
 }

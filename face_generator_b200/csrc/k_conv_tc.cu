@@ -1,5 +1,5 @@
-// tcgen05 / TMA implicit-GEMM convolutions for sm_100a with error-compensated 3xTF32
-// (hi*hi + hi*lo + lo*hi, fp32 accumulation in TMEM) so results stay within fp32 parity.
+// wgmma / TMA implicit-GEMM convolutions for sm_90a with error-compensated 3xTF32
+// (hi*hi + hi*lo + lo*hi, fp32 accumulation in registers) so results stay within fp32 parity.
 //
 // Both kernels view a stride-1 "same" convolution as a sum over filter taps of shifted GEMMs and feed
 // the tensor cores with plain TILED TMA boxes of the NHWC activation tensors (out-of-image rows /
@@ -15,9 +15,9 @@
 // only sees low-res offsets {-1,0,1}^2 (SURVEY.md 7.3), either with the 25 original taps ("dense")
 // or with the weights pre-summed to 9 taps per phase ("collapsed", 2.78x fewer MMAs).
 //
-// Pipeline per CTA (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + single-thread
-// tcgen05.mma issuer, warps 2..5 = epilogue (tcgen05.ld -> registers -> global).  3 smem stages of
-// {A_hi, A_lo, B_hi, B_lo}, 128B-swizzled, mbarrier full/empty rings, tcgen05.commit releases stages.
+// Pipeline per CTA (384 threads): warpgroups 0-1 = wgmma issue + epilogue (64 accumulator rows each),
+// warpgroup 2 = TMA producer.  3 smem stages of {A_hi, A_lo, B_hi, B_lo}, 128B-swizzled, mbarrier full/empty
+// rings (k_conv_tc_kernels.cuh).
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -28,6 +28,7 @@
 #include "fg_internal.h"
 #include "k_conv_tc.h"
 #include "k_f16split.cuh"
+#include "k_wgmma.cuh"
 
 namespace {
 
@@ -93,101 +94,16 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], kind::tf32, issued by ONE thread
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same with FP16 operands (kind::f16: 16 K elements per 32-byte slice, twice the TF32 rate), fp32 accumulation
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-template <bool F16>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if (F16) umma_f16(tmem_d, adesc, bdesc, idesc, accumulate);
-  else umma_tf32(tmem_d, adesc, bdesc, idesc, accumulate);
-}
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 columns of 32-bit: thread i of the warp receives row (lane-quadrant*32 + i)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// two 32x32 loads in flight, one wait: halves the exposed TMEM-load latency of the promotion loop
-__device__ __forceinline__ void tmem_ld_32x32_x2(uint32_t taddr_a, uint32_t taddr_b, uint32_t* a, uint32_t* b) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%64];\n\t"
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, [%65];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]), "=r"(a[4]), "=r"(a[5]), "=r"(a[6]), "=r"(a[7]), "=r"(a[8]), "=r"(a[9]), "=r"(a[10]), "=r"(a[11]), "=r"(a[12]), "=r"(a[13]), "=r"(a[14]), "=r"(a[15]), "=r"(a[16]), "=r"(a[17]), "=r"(a[18]), "=r"(a[19]), "=r"(a[20]), "=r"(a[21]), "=r"(a[22]), "=r"(a[23]), "=r"(a[24]), "=r"(a[25]), "=r"(a[26]), "=r"(a[27]), "=r"(a[28]), "=r"(a[29]), "=r"(a[30]), "=r"(a[31]),
-        "=r"(b[0]), "=r"(b[1]), "=r"(b[2]), "=r"(b[3]), "=r"(b[4]), "=r"(b[5]), "=r"(b[6]), "=r"(b[7]), "=r"(b[8]), "=r"(b[9]), "=r"(b[10]), "=r"(b[11]), "=r"(b[12]), "=r"(b[13]), "=r"(b[14]), "=r"(b[15]), "=r"(b[16]), "=r"(b[17]), "=r"(b[18]), "=r"(b[19]), "=r"(b[20]), "=r"(b[21]), "=r"(b[22]), "=r"(b[23]), "=r"(b[24]), "=r"(b[25]), "=r"(b[26]), "=r"(b[27]), "=r"(b[28]), "=r"(b[29]), "=r"(b[30]), "=r"(b[31])
-      : "r"(taddr_a), "r"(taddr_b)
-      : "memory");
-}
-
-// UMMA shared-memory descriptor (cute::UMMA::SmemDescriptor bit layout, version 1 = Blackwell):
-//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint64_t layout = 2) {
+// wgmma shared-memory matrix descriptor:
+//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base offset (0: every tile is 1024-aligned)
+//   | [62,64) layout (1 = SWIZZLE_128B)
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46) | (layout << 61);
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): D=f32, A=B=tf32 (format 2) or fp16 (format 0)
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, int a_mn_major, int b_mn_major, bool f16 = false) {
-  return (1u << 4) | ((f16 ? 0u : 2u) << 7) | ((f16 ? 0u : 2u) << 10) | ((uint32_t)a_mn_major << 15) |
-         ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// one lane of a fully active warp (the compiler knows the predicate selects exactly one lane, so code under it can
-// keep its operands in uniform registers)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 62);
 }
 
 constexpr int kStages = 3;
+constexpr int64_t kGridCap = 132 * 16;  // grid-stride elementwise kernels: 16 CTAs per SM of an H100
 constexpr uint32_t kABytes = 128 * 128;  // 128 rows x 32 fp32
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
@@ -200,7 +116,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // elementwise helpers of the tensor-core path
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
-  // hi: mantissa rounded to 10 bits (what kind::tf32 consumes exactly), lo: exact fp32 remainder
+  // hi: mantissa rounded to 10 bits (what a tf32 MMA consumes exactly), lo: exact fp32 remainder
   hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
   lo = x - hi;
 }
@@ -458,8 +374,8 @@ int make_map4(CUtensorMap* m, const float* base, int C, int W, int H, int B, int
   return FG_OK;
 }
 // 5-D map for the MN-major wgrad operands: dims (32 ch-in-group, W, H, B, C/32 groups); the box takes `ngroups`
-// channel groups of one 32-pixel box so the tile lands as [group][pixel][32 ch] (SWIZZLE_128B_ATOM_32B)
-// f16: groups of 64 fp16 channels (128 bytes), plain SWIZZLE_128B
+// channel groups of one 32-pixel box so the tile lands as [group][pixel][32 ch], unswizzled (the kernel transposes it)
+// f16: groups of 64 fp16 channels (128 bytes), SWIZZLE_128B (the canonical MN-major wgmma layout)
 int make_map5(CUtensorMap* m, const float* base, int C, int W, int H, int B, int64_t sW, int64_t sH, int64_t sB, int bw,
               int bh, int bb, int ngroups, bool f16 = false) {
   const int gch = f16 ? 64 : 32;
@@ -468,7 +384,7 @@ int make_map5(CUtensorMap* m, const float* base, int C, int W, int H, int B, int
   cuuint32_t box[5] = {(cuuint32_t)gch, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bb, (cuuint32_t)ngroups};
   cuuint32_t es[5] = {1, 1, 1, 1, 1};
   CUresult r = g_encode(m, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, (void*)base, dims, strides, box, es,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, f16 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, f16 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     fg_set_error("cuTensorMapEncodeTiled(5d) failed: %d (C=%d W=%d H=%d B=%d box %d,%d,%d x%d)", (int)r, C, W, H, B, bw, bh,
@@ -514,9 +430,10 @@ bool pick_box(int H, int W, int npix, int* bw, int* bh, int* bb) {
 }
 
 template <int BN>
-constexpr size_t fwd_smem() { return (size_t)kStages * (2 * kABytes + 2 * BN * 128) + 256 + 2 * 4 * BN * 4 + 1024; }
+constexpr size_t fwd_smem() { return (size_t)kStages * (2 * kABytes + 2 * BN * 128) + 256 + 2 * 8 * BN * 4 + 1024; }
+// F16: 3 TMA stages; TF32: 2 TMA stages + the K-major copy of one (same bytes per stage)
 template <int BN>
-constexpr size_t wg_smem() { return (size_t)kStages * (2 * 4 * 4096 + 2 * (BN / 32) * 4096) + 128 + 1024; }
+constexpr size_t wg_smem() { return (size_t)3 * (2 * 4 * 4096 + 2 * (BN / 32) * 4096) + 128 + 1024; }
 
 #define LAUNCH_CHECK(c)                 \
   do {                                  \
@@ -526,136 +443,49 @@ constexpr size_t wg_smem() { return (size_t)kStages * (2 * 4 * 4096 + 2 * (BN / 
 
 
 // ------------------------------------------------------------------------------------------------
-// tensor-pipe probe: the issue rate of tcgen05.mma.kind::tf32 (cta_group::1, M=128, N=256, K=8) with both operands
-// resident in shared memory -- no TMA, no epilogue.  bench.py runs it at bench clocks; the number is the measured
-// TF32 peak the 3xTF32 convolutions are normalised by (MEASURED_PEAKS.json only holds a bf16 figure).
+// tensor-pipe probe: the issue rate of back-to-back wgmmas (m64 x N x 8 tf32 or m64 x N x 16 f16, two warpgroups
+// per SM) with both operands resident in shared memory -- no TMA, no epilogue.  bench.py runs it at bench clocks;
+// the number is the measured MMA peak the 3-term convolutions are normalised by.
 // ------------------------------------------------------------------------------------------------
-template <int N, int NACC, bool F16 = false>
-__global__ void __launch_bounds__(128, 1) tf32_peak_kernel(int iters, int mode) {
-  // mode bits (experiments): 1 = a tcgen05.commit after every 4 MMAs; 2 = operands cycle through a 3 x 64 KB footprint
-  // like the stage ring of the convolution kernels; 4 = the accumulator changes with every instruction
+template <int N, bool F16 = false>
+__global__ void __launch_bounds__(256, 1) tf32_peak_kernel(int iters, float* sink) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr uint32_t kFoot = 3 * 65536;
-  uint64_t* done = reinterpret_cast<uint64_t*>(smem + kFoot);
-  uint64_t* dummy = done + 1;  // target of the intermediate commits (nobody waits on it)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done + 2);
-  for (uint32_t i = threadIdx.x; i < kFoot / 4; i += blockDim.x) reinterpret_cast<float*>(smem)[i] = 1.0f;
-  if (threadIdx.x == 0) {
-    mbar_init(done, 1);
-    mbar_init(dummy, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  constexpr uint32_t kFoot = (128 + N) * 128;  // A: 128 rows, B: N rows of 128 bytes
+  for (uint32_t i = threadIdx.x; i < kFoot / 4; i += blockDim.x) reinterpret_cast<float*>(smem)[i] = 1.f;
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy smem writes -> visible to the MMA
-  if (threadIdx.x < 32) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  if (*tmem_slot != 0) __trap();
-  constexpr uint32_t tmem_base = 0;
-  if (threadIdx.x < 32) {
-    constexpr uint32_t kIdesc = make_idesc(128, N, 0, 0, F16);
-    const uint32_t sa = smem_u32(smem);
-    for (int i = 0; i < iters; ++i) {
-      const uint32_t st = (mode & 2) ? (uint32_t)(i % 3) * 65536 : 0;
-      const uint64_t a = make_desc(sa + st, 16, 1024), b = make_desc(sa + st + 16384, 16, 1024);
-      const uint32_t acc = tmem_base + (uint32_t)(i % NACC) * N;  // NACC independent accumulators
-      if (elect_one()) {
+  const uint32_t sa = smem_u32(smem);
+  const uint64_t a = make_desc(sa + (threadIdx.x >> 7) * 64 * 128, 16, 1024), b = make_desc(sa + 128 * 128, 16, 1024);
+  float acc[N / 2];
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma<F16>((mode & 4) ? tmem_base + (uint32_t)((i + k) % NACC) * N : acc, a + (uint64_t)(k * 2), b + (uint64_t)(k * 2), kIdesc, 1);
-        if (mode & 1) umma_commit(dummy);
-      }
-      __syncwarp();
-    }
-    if (elect_one()) umma_commit(done);
-    mbar_wait(done, 0);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x < 32) tmem_dealloc<512>(tmem_base);
-}
-
-// ------------------------------------------------------------------------------------------------
-// descriptor probe (tests): an A operand that is a SHIFTED WINDOW of a larger 128B-swizzled tile.  The tile is a
-// "haloed" pixel block [18 rows][16 pixels][32 ch] (288 rows of 128 B) landed by TMA; the operand of tap (dy, dx) is
-// the 128 rows { (yi + dy) * 16 + xi + dx : yi < 16, xi < 8 }: 8-row core groups 2048 B apart (SBO), start address
-// base + (dy * 16 + dx) * 128 -- not 1024-aligned, so the descriptor's base-offset field must carry (addr >> 7) & 7.
-// With B = identity the accumulator is the gathered operand itself.
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) umma_window_probe_kernel(const __grid_constant__ CUtensorMap xmap,
-                                                                   const __grid_constant__ CUtensorMap bmap, int dy, int dx,
-                                                                   int use_base_offset, float* __restrict__ out) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr uint32_t kX = 288 * 128, kBb = 32 * 128;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kX + kBb);
-  uint64_t* done = full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done + 1);
-  if (threadIdx.x == 0) {
-    mbar_init(full, 1);
-    mbar_init(done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (threadIdx.x < 32) tmem_alloc<32>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (threadIdx.x == 0) {
-    mbar_expect_tx(full, kX + kBb);
-    tma_load_2d(smem, &xmap, full, 0, 0);
-    tma_load_2d(smem + 144 * 128, &xmap, full, 0, 144);
-    tma_load_2d(smem + kX, &bmap, full, 0, 0);
-    mbar_wait(full, 0);
-    tc_fence_after();
-    const int pitch = (use_base_offset >> 8) ? (use_base_offset >> 8) : 16;  // pixels per halo row (bits 8..)
-    const uint32_t sa = smem_u32(smem) + (uint32_t)(dy * pitch + dx) * 128;
-    uint64_t a = make_desc(sa, 16, (uint32_t)pitch * 128);
-    if (use_base_offset & 1) a |= (uint64_t)((sa >> 7) & 7) << 49;
-    const uint64_t b = make_desc(smem_u32(smem + kX), 16, 1024);
-    constexpr uint32_t kIdesc = make_idesc(128, 32, 0, 0);
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  for (int i = 0; i < iters; ++i) {
+    wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < 4; ++k) umma_tf32(tmem_base, a + (uint64_t)(k * 2), b + (uint64_t)(k * 2), kIdesc, k != 0);
-    umma_commit(done);
+    for (int k = 0; k < 4; ++k) wgmma_op<N, F16, false>(acc, a + (uint64_t)(k * 2), b + (uint64_t)(k * 2), 1);
+    wgmma_commit();
+    wgmma_wait<1>();
   }
-  mbar_wait(done, 0);
-  tc_fence_after();
-  uint32_t v[32];
-  tmem_ld_32x32(tmem_base + ((uint32_t)((threadIdx.x >> 5) * 32) << 16), v);
+  wgmma_wait<0>();
+  float s = 0.f;
 #pragma unroll
-  for (int i = 0; i < 32; ++i) out[threadIdx.x * 32 + i] = __uint_as_float(v[i]);
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x < 32) tmem_dealloc<32>(tmem_base);
+  for (int i = 0; i < N / 2; ++i) s += acc[i];
+  if (s == 1234.5f) *sink = s;  // never taken; keeps the accumulators live
 }
 
 }  // namespace
 
-// x: device [288][32] fp32 (tf32-exact values), ident: device [32][32] identity; out: device [128][32]
-int tc_umma_window_probe(fg_ctx* c, const float* x, const float* ident, int dy, int dx, int use_base_offset, float* out) {
-  FG_TRY(get_encode());
-  CUtensorMap xm, bm;
-  FG_TRY(make_map2(&xm, x, 32, 288, 32, 144));
-  FG_TRY(make_map2(&bm, ident, 32, 32, 32, 32));
-  constexpr int kSmem = 288 * 128 + 32 * 128 + 64 + 1024;
-  umma_window_probe_kernel<<<1, 128, kSmem, c->stream>>>(xm, bm, dy, dx, use_base_offset, out);
-  LAUNCH_CHECK(c);
-  return FG_OK;
-}
-
-// -> TFLOP/s of kind::tf32 MMAs (2*M*N*K per instruction) over all SMs, best of `reps` event-timed launches.
-// FG_TF32_PROBE_N=128 probes the N=128 instruction shape the convolution kernels issue (operand reads from shared
-// memory: 8 KB per 64-cycle MMA = the full 128 B/clk of one SM; N=256: 12 KB per 128 cycles)
+// -> TFLOP/s of the MMAs (2*M*N*K per instruction) over all SMs, best of `reps` event-timed launches.
+// FG_TF32_PROBE_N=128 probes the N=128 instruction shape; FG_TF32_PROBE_F16=1 the same loop with f16 operands
+// (K = 16 per instruction) -- the rate the 3xFP16 kernels run at
 int tc_tf32_peak(fg_ctx* c, int iters, int reps, double* tflops) {
-  constexpr int kSmem = 3 * 65536 + 64 + 1024;
   const char* env = getenv("FG_TF32_PROBE_N");
   const int N = env && atoi(env) == 128 ? 128 : 256;
-  const int mode = getenv("FG_TF32_PROBE_MODE") ? atoi(getenv("FG_TF32_PROBE_MODE")) : 0;
-  // FG_TF32_PROBE_F16=1: the same loop with kind::f16 (K = 16 per instruction) -- the rate the 3xFP16 kernels run at
   const bool f16 = getenv("FG_TF32_PROBE_F16") && atoi(getenv("FG_TF32_PROBE_F16"));
-  auto kern = f16 ? (N == 128 ? tf32_peak_kernel<128, 4, true> : tf32_peak_kernel<256, 2, true>)
-                  : (N == 128 ? tf32_peak_kernel<128, 4> : tf32_peak_kernel<256, 2>);
+  const int kSmem = (128 + N) * 128 + 1024;
+  auto kern = f16 ? (N == 128 ? tf32_peak_kernel<128, true> : tf32_peak_kernel<256, true>)
+                  : (N == 128 ? tf32_peak_kernel<128> : tf32_peak_kernel<256>);
   FG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
   cudaEvent_t e0, e1;
   FG_CUDA(cudaEventCreate(&e0));
@@ -663,7 +493,7 @@ int tc_tf32_peak(fg_ctx* c, int iters, int reps, double* tflops) {
   float best = 1e30f;
   for (int r = 0; r < reps + 1; ++r) {  // first launch = warm-up
     FG_CUDA(cudaEventRecord(e0, c->stream));
-    kern<<<c->sm_count, 128, kSmem, c->stream>>>(iters, mode);
+    kern<<<c->sm_count, 256, kSmem, c->stream>>>(iters, c->io_dev);
     LAUNCH_CHECK(c);
     FG_CUDA(cudaEventRecord(e1, c->stream));
     FG_CUDA(cudaEventSynchronize(e1));
@@ -707,7 +537,7 @@ int tc_split(fg_ctx* c, const float* x, float* hi, float* lo, int64_t n) {
     return FG_ERR_INVALID;
   }
   int64_t g = (n / 4 + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > kGridCap) g = kGridCap;
   if (reinterpret_cast<uintptr_t>(x) % 16 == 0) split_kernel<true><<<(int)g, 256, 0, c->stream>>>(x, hi, lo, n / 4);
   else split_kernel<false><<<(int)g, 256, 0, c->stream>>>(x, hi, lo, n / 4);  // e.g. a weight block inside the flat parameter vector
   LAUNCH_CHECK(c);
@@ -720,7 +550,7 @@ int tc_amax(fg_ctx* c, const float* x, int64_t n, float* amax_slot) {
   }
   FG_CUDA(cudaMemsetAsync(amax_slot, 0, 2 * sizeof(float), c->stream));
   int64_t g = (n / 4 + 255) / 256;
-  if (g > 148 * 8) g = 148 * 8;
+  if (g > kGridCap / 2) g = kGridCap / 2;
   amax_kernel<<<(int)g, 256, 0, c->stream>>>(x, n / 4, reinterpret_cast<unsigned*>(amax_slot));
   LAUNCH_CHECK(c);
   return FG_OK;
@@ -732,7 +562,7 @@ int tc_split_h(fg_ctx* c, const float* x, float* hh, float* hl, int64_t n, float
     return FG_ERR_INVALID;
   }
   int64_t g = (n / 4 + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > kGridCap) g = kGridCap;
   __half *h = reinterpret_cast<__half*>(hh), *l = reinterpret_cast<__half*>(hl);
   if (reinterpret_cast<uintptr_t>(x) % 16 == 0) split_h_kernel<true><<<(int)g, 256, 0, c->stream>>>(x, h, l, n / 4, amax_slot, inv_out);
   else split_h_kernel<false><<<(int)g, 256, 0, c->stream>>>(x, h, l, n / 4, amax_slot, inv_out);
@@ -747,7 +577,7 @@ int tc_pack_split_h(fg_ctx* c, const float* W, float* f_hi, float* f_lo, float* 
     return FG_OK;
   }
   int64_t g = ((int64_t)N * Cc * KK + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > kGridCap) g = kGridCap;
   pack_split_kernel<__half><<<(int)g, 256, 0, c->stream>>>(W, (__half*)f_hi, (__half*)f_lo, (__half*)d_hi, (__half*)d_lo, N, Cc, KK);
   LAUNCH_CHECK(c);
   return FG_OK;
@@ -760,7 +590,7 @@ int tc_pack_collapsed_h(fg_ctx* c, const float* W, float* f_hi, float* f_lo, flo
     return FG_OK;
   }
   int64_t g = ((int64_t)36 * N * Cc + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > kGridCap) g = kGridCap;
   pack_collapsed_kernel<__half><<<(int)g, 256, 0, c->stream>>>(W, (__half*)f_hi, (__half*)f_lo, (__half*)d_hi, (__half*)d_lo, N, Cc);
   LAUNCH_CHECK(c);
   return FG_OK;
@@ -772,7 +602,7 @@ int tc_pack_split(fg_ctx* c, const float* W, float* f_hi, float* f_lo, float* d_
     return FG_OK;
   }
   int64_t g = ((int64_t)N * Cc * KK + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > kGridCap) g = kGridCap;
   pack_split_kernel<float><<<(int)g, 256, 0, c->stream>>>(W, f_hi, f_lo, d_hi, d_lo, N, Cc, KK);
   LAUNCH_CHECK(c);
   return FG_OK;
@@ -784,25 +614,24 @@ int tc_pack_collapsed(fg_ctx* c, const float* W, float* f_hi, float* f_lo, float
     return FG_OK;
   }
   int64_t g = ((int64_t)36 * N * Cc + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > kGridCap) g = kGridCap;
   pack_collapsed_kernel<float><<<(int)g, 256, 0, c->stream>>>(W, f_hi, f_lo, d_hi, d_lo, N, Cc);
   LAUNCH_CHECK(c);
   return FG_OK;
 }
 int tc_combine_collapsed_wgrad(fg_ctx* c, const float* G, float* dW, int N, int Cc) {
   int64_t g = ((int64_t)N * Cc * 25 + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > kGridCap) g = kGridCap;
   combine_collapsed_wgrad_kernel<<<(int)g, 256, 0, c->stream>>>(G, dW, N, Cc);
   LAUNCH_CHECK(c);
   return FG_OK;
 }
 
-// K-blocks (32 channels of one tap) accumulated in TMEM before the epilogue promotes them into fp32 registers.
-// The truncation drift of a TMEM accumulator grows with the length of the run (DESIGN.md section 5), the hand-over
-// of an accumulator buffer costs the MMA warp a completion round trip (~1 us: commit -> epilogue -> release), so the
-// chunk is a trade: convolution forward / dgrad 12 (measured at batch 256: chunk 4 / 8 / 12 / 16 -> 41.2 / 42.6 / 42.9 /
-// 43.0 k img/s, every isolated launch still <= 1e-5 of fp64 at all four), wgrad and the Linear layers (K = pixels
-// resp. up to 16384 features) 8 resp. 4.  FG_TC_CHUNK / FG_TC_CHUNK_FWD override for experiments.
+// K-blocks (32 channels of one tap) accumulated in the wgmma accumulators before the consumers promote them into fp32
+// registers.  The drift of a tensor-core accumulation grows with the length of the run (DESIGN.md section 5), every
+// promotion drains the consumer's wgmma pipeline, so the chunk is a trade: convolution forward / dgrad 12, wgrad and
+// the Linear layers (K = pixels resp. up to 16384 features) 8 resp. 4.  FG_TC_CHUNK / FG_TC_CHUNK_FWD override for
+// experiments.
 static int tc_chunk(bool forward_type = false) {
   static int v[2] = {-1, -1};
   if (v[0] < 0) {
@@ -819,10 +648,10 @@ static int tc_chunk(bool forward_type = false) {
 static int launch_tapconv(fg_ctx* c, const TcFwdParams& p, int BN, int f16 = 0) {
   dim3 grid(std::min(p.ntiles, std::max(1, c->sm_count - c->reserve_sms)));
   if (f16) {
-    if (BN == 128) tapconv_tc_kernel<128, true><<<grid, 192, fwd_smem<128>(), c->stream>>>(p);
-    else tapconv_tc_kernel<64, true><<<grid, 192, fwd_smem<64>(), c->stream>>>(p);
-  } else if (BN == 128) tapconv_tc_kernel<128><<<grid, 192, fwd_smem<128>(), c->stream>>>(p);
-  else tapconv_tc_kernel<64><<<grid, 192, fwd_smem<64>(), c->stream>>>(p);
+    if (BN == 128) tapconv_tc_kernel<128, true><<<grid, kTcThreads, fwd_smem<128>(), c->stream>>>(p);
+    else tapconv_tc_kernel<64, true><<<grid, kTcThreads, fwd_smem<64>(), c->stream>>>(p);
+  } else if (BN == 128) tapconv_tc_kernel<128><<<grid, kTcThreads, fwd_smem<128>(), c->stream>>>(p);
+  else tapconv_tc_kernel<64><<<grid, kTcThreads, fwd_smem<64>(), c->stream>>>(p);
   LAUNCH_CHECK(c);
   return FG_OK;
 }
@@ -867,7 +696,7 @@ int tc_conv_fwd(fg_ctx* c, const float* x_hi, const float* x_lo, const float* w_
   const int64_t sW = (int64_t)g.Cin * es, sH = sW * Wl, sB = sH * Hl;
   FG_TRY(make_map4(&p.a_hi[0], x_hi, g.Cin, Wl, Hl, g.B, sW, sH, sB, ke, p.bw, p.bh, p.bb, CU_TENSOR_MAP_SWIZZLE_128B, false, h));
   FG_TRY(make_map4(&p.a_lo[0], x_lo, g.Cin, Wl, Hl, g.B, sW, sH, sB, ke, p.bw, p.bh, p.bb, CU_TENSOR_MAP_SWIZZLE_128B, false, h));
-  // N tile: 128 unless halving it keeps the same number of waves on the 148 SMs (few-tile layers such as
+  // N tile: 128 unless halving it keeps the same number of waves on the SMs (few-tile layers such as
   // D.C4's dgrad or the Linear layers): a BN=64 tile costs ~0.6 of a BN=128 tile
   int BN = g.Cout % 128 == 0 ? 128 : 64;
   if (BN == 128) {
@@ -927,7 +756,6 @@ int tc_conv_fwd(fg_ctx* c, const float* x_hi, const float* x_lo, const float* w_
   p.out_H = g.H; p.out_W = g.W;
   p.out_scale = g.ups;
   p.ntiles = p.tiles_per_phase * p.nphase * (g.Cout / BN);
-  p.dbg = getenv("FG_TC_DBG") ? atoi(getenv("FG_TC_DBG")) : 0;
   p.chunk = tc_chunk(g.H * g.W > 1);  // Linear layers (1x1 images, K up to 16384) keep the short chunk
   // fp16: a 128-byte K block holds twice the K elements, so the same chunk is a 2x longer accumulation run (K = 768 for
   // the convolutions); measured <= 1.3e-6 of fp64 on every isolated launch (the TF32 path's level) and 2 % faster than 6
@@ -982,7 +810,6 @@ int tc_conv_dgrad_ups(fg_ctx* c, const float* dy_hi, const float* dy_lo, const f
   p.out_H = Hl; p.out_W = Wl;
   p.out_scale = 1;
   p.ntiles = p.tiles_per_phase * (g.Cin / BN);
-  p.dbg = getenv("FG_TC_DBG") ? atoi(getenv("FG_TC_DBG")) : 0;
   p.chunk = tc_chunk(true);
   return launch_tapconv(c, p, BN, f16);
 }
@@ -1046,18 +873,23 @@ int tc_conv_wgrad(fg_ctx* c, const float* x_hi, const float* x_lo, const float* 
   if (splits > p.kblocks) splits = p.kblocks;
   p.kb_per_split = (p.kblocks + splits - 1) / splits;
   splits = (p.kblocks + p.kb_per_split - 1) / p.kb_per_split;
-  p.out = out;
+  const int64_t size = (int64_t)ntt * g.Cout * g.Cin;
+  p.out = splits > 1 ? c->splitk_ws : out;  // splits x base CTAs <= one per SM: fits splitk_ws
+  p.split_stride = size;
   p.oscale = oscale ? oscale : oscale2;
   p.oscale2 = oscale ? oscale2 : nullptr;
   p.chunk = tc_chunk() == 4 && !getenv("FG_TC_CHUNK") ? ((int64_t)g.H * g.W > 1 ? 8 : 4) : tc_chunk();  // wgrad of convolutions 8, of Linear layers 4
   if (h) p.chunk = std::max(1, p.chunk / 2);  // an fp16 K block holds 64 pixels
-  FG_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)ntt * g.Cout * g.Cin, c->stream));
+  if (splits * size > (int64_t)c->splitk_ws_elems) {
+    fg_set_error("tc_conv_wgrad: %d splits of %lld elements exceed the split-K workspace", splits, (long long)size);
+    return FG_ERR_UNSUPPORTED;
+  }
   dim3 grid(ntt, (g.Cout / 128) * (g.Cin / BN), splits);
   if (h) {
-    if (BN == 128) wgrad_tc_kernel<128, true><<<grid, 192, wg_smem<128>(), c->stream>>>(p);
-    else wgrad_tc_kernel<64, true><<<grid, 192, wg_smem<64>(), c->stream>>>(p);
-  } else if (BN == 128) wgrad_tc_kernel<128><<<grid, 192, wg_smem<128>(), c->stream>>>(p);
-  else wgrad_tc_kernel<64><<<grid, 192, wg_smem<64>(), c->stream>>>(p);
+    if (BN == 128) wgrad_tc_kernel<128, true><<<grid, kTcThreads, wg_smem<128>(), c->stream>>>(p);
+    else wgrad_tc_kernel<64, true><<<grid, kTcThreads, wg_smem<64>(), c->stream>>>(p);
+  } else if (BN == 128) wgrad_tc_kernel<128><<<grid, kTcThreads, wg_smem<128>(), c->stream>>>(p);
+  else wgrad_tc_kernel<64><<<grid, kTcThreads, wg_smem<64>(), c->stream>>>(p);
   LAUNCH_CHECK(c);
-  return FG_OK;
+  return splits > 1 ? k_splitk_reduce(c, c->splitk_ws, splits, size, out) : FG_OK;
 }

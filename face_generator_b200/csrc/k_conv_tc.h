@@ -1,4 +1,4 @@
-// Parameter blocks (passed as __grid_constant__) and host entry points of the tcgen05 conv path.
+// Parameter blocks (passed as __grid_constant__) and host entry points of the wgmma conv path.
 #pragma once
 #include <cuda.h>
 
@@ -22,8 +22,7 @@ struct alignas(64) TcFwdParams {
   float* stats;  // optional [m-tile][2][Cout]: per-tile column sums of the output and of its square (BatchNorm)
   int out_H, out_W, out_scale;
   const float *oscale, *oscale2;  // optional device scalars the accumulators are multiplied by (inverse operand scales)
-  int dbg;    // experiment switches (FG_TC_DBG): 1 = skip MMAs, 2 = skip TMA data movement
-  int chunk;  // K-blocks accumulated in TMEM before the epilogue promotes them to fp32 registers
+  int chunk;  // K-blocks accumulated in the wgmma accumulators before they are promoted to fp32 registers
 };
 
 struct alignas(64) TcWgParams {
@@ -35,6 +34,7 @@ struct alignas(64) TcWgParams {
   int tiles_x, tiles_y;
   int kblocks, kb_per_split;
   float* out;
+  int64_t split_stride;  // elements between the partial outputs of two K splits
   const float *oscale, *oscale2;  // optional device scalars multiplied into the result (inverse scales of dY and X)
   int chunk;
 };
@@ -46,7 +46,7 @@ int tc_pack_collapsed(fg_ctx* c, const float* W, float* f_hi, float* f_lo, float
 int tc_combine_collapsed_wgrad(fg_ctx* c, const float* G, float* dW, int N, int Cc);
 // stats / n_parts (optional): the kernel also writes per-tile BatchNorm partials [*n_parts][2][Cout] (see TcFwdParams)
 // f16 != 0: the four operand pointers are __half arrays holding the FP16 split (tc_split_h / tc_pack_*_h: hi = fp16(x),
-// lo = fp16((x - hi) * 2^11)) and the kernel issues kind::f16 MMAs (twice the tensor rate, half the operand bytes);
+// lo = fp16((x - hi) * 2^11)) and the kernel issues f16 MMAs (twice the tensor rate, half the operand bytes);
 // oscale: optional device scalar multiplied into the result (inverse of the power-of-two scale tc_split_h applied)
 int tc_conv_fwd(fg_ctx* c, const float* x_hi, const float* x_lo, const float* w_hi, const float* w_lo, const float* bias,
                 float* out, ConvGeom g, int mode, float* stats = nullptr, int* n_parts = nullptr, int f16 = 0,
@@ -65,4 +65,3 @@ int tc_conv_wgrad(fg_ctx* c, const float* x_hi, const float* x_lo, const float* 
                   ConvGeom g, int f16 = 0, const float* oscale = nullptr, const float* oscale2 = nullptr);
 int tc_tf32_peak(fg_ctx* c, int iters, int reps, double* tflops);
 int tc_encode_nhwc_box(CUtensorMap* m, const float* base, int C, int W, int H, int B, int bc, int bw, int bh, int bb);
-int tc_umma_window_probe(fg_ctx* c, const float* x, const float* ident, int dy, int dx, int use_base_offset, float* out);

@@ -2,12 +2,13 @@
 // layout changes at the ABI, weight packing, BatchNorm statistics/apply/backward, PReLU, pooling,
 // dropout, sigmoid+BCE, penalty+clamp+Adam.  All tensors NHWC fp32, channels fastest, so a warp
 // reads consecutive channels of one pixel (coalesced 128B lines); per-channel reductions keep
-// double accumulators and finish with one atomicAdd per block (warp-shuffle / smem trees).
+// double accumulators per block (warp-shuffle / smem trees) and add the per-block partials in block order.
 //
 // Reference semantics: SURVEY.md section 8a; nn.* classes named per kernel below.
 #include <cmath>
 
 #include "fg_internal.h"
+#include "k_ordered.cuh"
 
 #define LAUNCH_CHECK(c)                 \
   do {                                  \
@@ -15,7 +16,7 @@
     FG_CUDA(cudaGetLastError());        \
   } while (0)
 
-static inline int grid_for(int64_t n, int block, int cap = 148 * 16) {
+static inline int grid_for(int64_t n, int block, int cap = 132 * 16) {
   int64_t g = (n + block - 1) / block;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
@@ -156,7 +157,7 @@ int k_unpack_wgrad(fg_ctx* c, const float* dWp, float* dW, int N, int Cc, int KK
 
 // out[j] += sum_p X[p][perm(j)]   (bias gradients)
 __global__ void colsum_kernel(const float* __restrict__ X, float* __restrict__ out, int64_t P, int N, int nA, int nS,
-                              int64_t rows_per_block) {
+                              int64_t rows_per_block, double* __restrict__ ws, unsigned* __restrict__ ticket) {
   __shared__ double sm[8][33];
   const int col = blockIdx.x * 32 + threadIdx.x;
   const int64_t r0 = blockIdx.y * rows_per_block;
@@ -172,7 +173,12 @@ __global__ void colsum_kernel(const float* __restrict__ X, float* __restrict__ o
     for (int i = 0; i < 8; ++i) t += sm[i][threadIdx.x];
     // inverse permutation: column col == perm(j)  =>  j = perm^-1(col) = perm with (A,S) swapped
     const int j = nA == 0 ? col : (col % nA) * nS + (col / nA);
-    atomicAdd(out + j, (float)t);
+    ws[(int64_t)blockIdx.y * N + j] = t;  // row blockIdx.y: the blocks of one row slice cover all N columns
+  }
+  if (ordered_last_block(ticket)) {
+    for (int j = threadIdx.y * blockDim.x + threadIdx.x; j < N; j += blockDim.x * blockDim.y)
+      out[j] += (float)ordered_sum(ws, gridDim.y, N, j);
+    ordered_release(ticket);
   }
 }
 int k_colsum_add(fg_ctx* c, const float* X, float* out, int64_t P, int N, int nA, int nS) {
@@ -180,7 +186,8 @@ int k_colsum_add(fg_ctx* c, const float* X, float* out, int64_t P, int N, int nA
   if (gy < 1) gy = 1;
   const int64_t rpb = (P + gy - 1) / gy;
   dim3 grid((N + 31) / 32, gy), block(32, 8);
-  colsum_kernel<<<grid, block, 0, c->stream>>>(X, out, P, N, nA, nS, rpb);
+  FG_TRY(red_check(c, gy, N));
+  colsum_kernel<<<grid, block, 0, c->stream>>>(X, out, P, N, nA, nS, rpb, c->red_ws, c->red_ticket);
   LAUNCH_CHECK(c);
   return FG_OK;
 }
@@ -218,7 +225,8 @@ __device__ __forceinline__ float load_dh(const float* __restrict__ dh, int b, in
 
 __global__ void prelu_bwd_kernel(const float* __restrict__ dh, const float* __restrict__ z,
                                  const float* __restrict__ slope, float* __restrict__ dz, float* __restrict__ dslope, int B,
-                                 int H, int W, int C, int pool, unsigned* __restrict__ amax) {
+                                 int H, int W, int C, int pool, unsigned* __restrict__ amax, double* __restrict__ ws,
+                                 unsigned* __restrict__ ticket) {
   const float a = *slope;
   const int64_t n = (int64_t)B * H * W * C;
   double s = 0;
@@ -243,12 +251,18 @@ __global__ void prelu_bwd_kernel(const float* __restrict__ dh, const float* __re
   }
   amax_commit(amax, am);
   s = block_sum(s);
-  if (threadIdx.x == 0 && dslope) atomicAdd(dslope, (float)s);
+  if (!dslope) return;
+  if (threadIdx.x == 0) ws[blockIdx.x] = s;
+  if (ordered_last_block(ticket)) {
+    if (threadIdx.x == 0) *dslope += (float)ordered_sum(ws, gridDim.x, 1, 0);
+    ordered_release(ticket);
+  }
 }
 int k_prelu_bwd(fg_ctx* c, const float* dh, const float* z, const float* slope, float* dz, float* dslope, int B, int H,
                 int W, int C, int pool) {
   const int64_t n = (int64_t)B * H * W * C;
-  prelu_bwd_kernel<<<grid_for(n, 256, 148 * 8), 256, 0, c->stream>>>(dh, z, slope, dz, dslope, B, H, W, C, pool, take_amax(c));
+  prelu_bwd_kernel<<<grid_for(n, 256, 132 * 8), 256, 0, c->stream>>>(dh, z, slope, dz, dslope, B, H, W, C, pool, take_amax(c),
+                                                                    c->red_ws, c->red_ticket);
   LAUNCH_CHECK(c);
   return FG_OK;
 }
@@ -258,7 +272,7 @@ int k_prelu_bwd(fg_ctx* c, const float* dh, const float* z, const float* slope, 
 // ------------------------------------------------------------------------------------------------
 // acc[0..C) += sum_p z, acc[C..2C) += sum_p z^2   (double; caller zeroes acc)
 __global__ void bn_stats_kernel(const float* __restrict__ z, double* __restrict__ acc, int64_t P, int C,
-                                int64_t rows_per_block) {
+                                int64_t rows_per_block, double* __restrict__ ws, unsigned* __restrict__ ticket) {
   extern __shared__ double sm[];  // [2][blockDim]
   const int lanes = blockDim.x / C;
   const int ch = threadIdx.x % C, lane = threadIdx.x / C;
@@ -277,8 +291,12 @@ __global__ void bn_stats_kernel(const float* __restrict__ z, double* __restrict_
       s += sm[l * C + ch];
       s2 += sm[blockDim.x + l * C + ch];
     }
-    atomicAdd(acc + ch, s);
-    atomicAdd(acc + C + ch, s2);
+    ws[(int64_t)blockIdx.x * 2 * C + ch] = s;
+    ws[(int64_t)blockIdx.x * 2 * C + C + ch] = s2;
+  }
+  if (ordered_last_block(ticket)) {
+    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) acc[i] += ordered_sum(ws, gridDim.x, 2 * C, i);
+    ordered_release(ticket);
   }
 }
 static inline int bn_block(int C) {
@@ -297,7 +315,8 @@ int k_bn_stats(fg_ctx* c, const float* z, double* acc, int64_t P, int C) {
   int grid = (int)std::min<int64_t>(c->sm_count * 4, (P + 63) / 64);
   if (grid < 1) grid = 1;
   const int64_t rpb = (P + grid - 1) / grid;
-  bn_stats_kernel<<<grid, block, sizeof(double) * 2 * block, c->stream>>>(z, acc, P, C, rpb);
+  FG_TRY(red_check(c, grid, 2 * C));
+  bn_stats_kernel<<<grid, block, sizeof(double) * 2 * block, c->stream>>>(z, acc, P, C, rpb, c->red_ws, c->red_ticket);
   LAUNCH_CHECK(c);
   return FG_OK;
 }
@@ -481,7 +500,7 @@ __global__ void bn_prelu_bwd_reduce_kernel(const float* __restrict__ dh, const f
                                            const float* __restrict__ gamma, const float* __restrict__ beta,
                                            const float* __restrict__ slope, double* __restrict__ acc,
                                            float* __restrict__ dslope, int B, int H, int W, int C, int pool,
-                                           int64_t rows_per_block) {
+                                           int64_t rows_per_block, double* __restrict__ ws, unsigned* __restrict__ ticket) {
   extern __shared__ double sm[];
   const int lanes = blockDim.x / C;
   const int ch = threadIdx.x % C, lane = threadIdx.x / C;
@@ -521,12 +540,15 @@ __global__ void bn_prelu_bwd_reduce_kernel(const float* __restrict__ dh, const f
       sg += sm[l * C + ch];
       sgx += sm[blockDim.x + l * C + ch];
     }
-    atomicAdd(acc + ch, sg);
-    atomicAdd(acc + C + ch, sgx);
+    ws[(int64_t)blockIdx.x * (2 * C + 1) + ch] = sg;
+    ws[(int64_t)blockIdx.x * (2 * C + 1) + C + ch] = sgx;
   }
-  if (act) {
-    ss = block_sum(ss);
-    if (threadIdx.x == 0 && dslope) atomicAdd(dslope, (float)ss);
+  if (act) ss = block_sum(ss);
+  if (threadIdx.x == 0) ws[(int64_t)blockIdx.x * (2 * C + 1) + 2 * C] = ss;
+  if (ordered_last_block(ticket)) {
+    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) acc[i] += ordered_sum(ws, gridDim.x, 2 * C + 1, i);
+    if (act && dslope && threadIdx.x == 0) *dslope += (float)ordered_sum(ws, gridDim.x, 2 * C + 1, 2 * C);
+    ordered_release(ticket);
   }
 }
 int k_bn_prelu_bwd_reduce(fg_ctx* c, const float* dh, const float* z, const float* mean, const float* istd,
@@ -541,8 +563,10 @@ int k_bn_prelu_bwd_reduce(fg_ctx* c, const float* dh, const float* z, const floa
   int grid = (int)std::min<int64_t>(c->sm_count * 4, (P + 63) / 64);
   if (grid < 1) grid = 1;
   const int64_t rpb = (P + grid - 1) / grid;
+  FG_TRY(red_check(c, grid, 2 * C + 1));
   bn_prelu_bwd_reduce_kernel<<<grid, block, sizeof(double) * 2 * block, c->stream>>>(dh, z, mean, istd, gamma, beta, slope,
-                                                                                  acc, dslope, B, H, W, C, pool, rpb);
+                                                                                  acc, dslope, B, H, W, C, pool, rpb, c->red_ws,
+                                                                                  c->red_ticket);
   LAUNCH_CHECK(c);
   return FG_OK;
 }
@@ -588,20 +612,44 @@ __global__ void bn_prelu_bwd_apply_kernel(const float* __restrict__ dh, const fl
     dz[i] = ga * is * (g - mg[ch] - xh * mg[C + ch]);
   }
 }
+// Column sums of a 256-thread block whose thread t owns channels 4 (t % (C/4)) .. +3 (256 % (C/4) == 0): the block sums
+// its threads in thread order into row blockIdx.x of ws ([n] doubles: C channel sums, then an optional scalar `extra`
+// at index C), and the last block adds the rows in block order to dst[0..C) and, if given, to *extra_dst.
+__device__ void block_colsum_rows(const float (&bs)[4], int C, int n, double* ws, unsigned* ticket, float* dst,
+                                  float* extra_dst, double extra = 0.0) {
+  __shared__ float tb[256][4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) tb[threadIdx.x][j] = bs[j];
+  __syncthreads();
+  const int C4 = C / 4;
+  double* row = ws + (int64_t)blockIdx.x * n;
+  for (int i = threadIdx.x; i < C; i += blockDim.x) {
+    double s = 0;
+    for (int t = i / 4; t < (int)blockDim.x; t += C4) s += tb[t][i & 3];
+    row[i] = s;
+  }
+  if (n > C && threadIdx.x == 0) row[C] = extra;
+  if (ordered_last_block(ticket)) {
+    if (dst)
+      for (int i = threadIdx.x; i < C; i += blockDim.x) dst[i] += (float)ordered_sum(ws, gridDim.x, n, i);
+    if (extra_dst && threadIdx.x == 0) *extra_dst += (float)ordered_sum(ws, gridDim.x, n, C);
+    ordered_release(ticket);
+  }
+}
+
 // pool == 0 fast path: float4 along channels, no pixel decode
 __global__ void bn_prelu_bwd_apply4_kernel(const float* __restrict__ dh, const float* __restrict__ z,
                                            const float* __restrict__ mean, const float* __restrict__ istd,
                                            const float* __restrict__ gamma, const float* __restrict__ beta,
                                            const float* __restrict__ slope, const float* __restrict__ mg,
                                            float* __restrict__ dz, float* __restrict__ hi, float* __restrict__ lo,
-                                           float* __restrict__ dbias, int64_t n4, int C, unsigned* __restrict__ amax) {
+                                           float* __restrict__ dbias, int64_t n4, int C, unsigned* __restrict__ amax,
+                                           double* __restrict__ ws, unsigned* __restrict__ ticket) {
   float am = 0.f;
   // dbias (optional): += column sums of dz = the gradient of the convolution bias in front of the BatchNorm.  The grid
-  // stride is a multiple of C/4, so a thread always sees the same 4 channels: thread-local sums -> shared -> global
-  __shared__ float bsum[1024];
+  // stride is a multiple of C/4, so a thread always sees the same 4 channels: thread-local sums -> block sums in
+  // thread order -> per-block rows added in block order (block_colsum_rows)
   float bs[4] = {0.f, 0.f, 0.f, 0.f};
-  if (dbias)
-    for (int i = threadIdx.x; i < C; i += blockDim.x) bsum[i] = 0.f;
   const bool act = slope != nullptr;
   const float a = act ? *slope : 1.f;
   const float4* dh4 = reinterpret_cast<const float4*>(dh);
@@ -638,22 +686,17 @@ __global__ void bn_prelu_bwd_apply4_kernel(const float* __restrict__ dh, const f
     }
   }
   amax_commit(amax, am);
-  if (dbias) {
-    __syncthreads();
-    const int ch = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) % C4) * 4;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) atomicAdd(bsum + ch + j, bs[j]);
-    __syncthreads();
-    for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(dbias + i, bsum[i]);
-  }
+  if (dbias) block_colsum_rows(bs, C, C, ws, ticket, dbias, nullptr);
 }
 int k_bn_prelu_bwd_apply(fg_ctx* c, const float* dh, const float* z, const float* mean, const float* istd,
                          const float* gamma, const float* beta, const float* slope, const float* mg, float* dz, int B,
                          int H, int W, int C, int pool, float* hi, float* lo, float* dbias) {
   const int64_t n = (int64_t)B * H * W * C;
   if (!pool && C % 4 == 0 && C <= 1024 && 256 % (C / 4) == 0) {
-    bn_prelu_bwd_apply4_kernel<<<grid_for(n / 4, 256), 256, 0, c->stream>>>(dh, z, mean, istd, gamma, beta, slope, mg, dz,
-                                                                           hi, lo, dbias, n / 4, C, take_amax(c));
+    const int grid = grid_for(n / 4, 256);
+    FG_TRY(red_check(c, grid, C));
+    bn_prelu_bwd_apply4_kernel<<<grid, 256, 0, c->stream>>>(dh, z, mean, istd, gamma, beta, slope, mg, dz, hi, lo, dbias, n / 4,
+                                                           C, take_amax(c), c->red_ws, c->red_ticket);
     LAUNCH_CHECK(c);
     return FG_OK;
   }
@@ -802,15 +845,13 @@ __global__ void d_act_pool_bwd_kernel(const float* __restrict__ dp, const float*
                                       const float* __restrict__ slope, const float* __restrict__ masks, int moff,
                                       float eval_scale, float* __restrict__ dz, float* __restrict__ dslope,
                                       float4* __restrict__ hi, float4* __restrict__ lo, float* __restrict__ dbias, int B,
-                                      int H, int W, int C, unsigned* __restrict__ amax) {
+                                      int H, int W, int C, unsigned* __restrict__ amax, double* __restrict__ ws,
+                                      unsigned* __restrict__ ticket) {
   float am = 0.f;
   // one thread = one pooled pixel x 4 channels: reads dp once, handles its 2x2 window of z / dz.
   // dbias (optional): += column sums of dz (the conv bias gradient); a thread always sees the same 4 channels because the
   // grid stride is a multiple of C/4
-  __shared__ float bsum[512];
   float bs[4] = {0.f, 0.f, 0.f, 0.f};
-  if (dbias)
-    for (int i = threadIdx.x; i < C; i += blockDim.x) bsum[i] = 0.f;
   const float a = *slope;
   const uint32_t Ho = H / 2, Wo = W / 2, C4 = C / 4;
   const uint32_t n = (uint32_t)B * Ho * Wo * C4;
@@ -853,17 +894,7 @@ __global__ void d_act_pool_bwd_kernel(const float* __restrict__ dp, const float*
   }
   amax_commit(amax, am);
   sd = block_sum(sd);
-  if (threadIdx.x == 0 && dslope) atomicAdd(dslope, (float)sd);
-  if (dbias) {
-    __syncthreads();
-    const uint32_t ch = ((blockIdx.x * blockDim.x + threadIdx.x) % C4) * 4;
-    atomicAdd(bsum + ch, bs[0]);
-    atomicAdd(bsum + ch + 1, bs[1]);
-    atomicAdd(bsum + ch + 2, bs[2]);
-    atomicAdd(bsum + ch + 3, bs[3]);
-    __syncthreads();
-    for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(dbias + i, bsum[i]);
-  }
+  if (dbias || dslope) block_colsum_rows(bs, dbias ? (int)C : 0, (dbias ? (int)C : 0) + 1, ws, ticket, dbias, dslope, sd);
 }
 int k_d_act_pool_bwd(fg_ctx* c, const float* dp, const float* z, const float* slope, const float* masks, int moff,
                      float eval_scale, float* dz, float* dslope, int B, int H, int W, int C, float* hi, float* lo,
@@ -874,9 +905,11 @@ int k_d_act_pool_bwd(fg_ctx* c, const float* dp, const float* z, const float* sl
     return FG_ERR_UNSUPPORTED;
   }
   const bool fuse = dbias && C <= 512 && 256 % (C / 4) == 0;
-  d_act_pool_bwd_kernel<<<grid_for(n, 256, 148 * 8), 256, 0, c->stream>>>(dp, z, slope, masks, moff, eval_scale, dz, dslope,
-                                                                         reinterpret_cast<float4*>(hi), reinterpret_cast<float4*>(lo),
-                                                                         fuse ? dbias : nullptr, B, H, W, C, take_amax(c));
+  const int grid = grid_for(n, 256, 132 * 8);
+  FG_TRY(red_check(c, grid, C + 1));
+  d_act_pool_bwd_kernel<<<grid, 256, 0, c->stream>>>(dp, z, slope, masks, moff, eval_scale, dz, dslope,
+                                                    reinterpret_cast<float4*>(hi), reinterpret_cast<float4*>(lo),
+                                                    fuse ? dbias : nullptr, B, H, W, C, take_amax(c), c->red_ws, c->red_ticket);
   LAUNCH_CHECK(c);
   if (dbias && !fuse) return k_colsum_add(c, dz, dbias, (int64_t)B * H * W, C, 0, 0);
   return FG_OK;
@@ -908,7 +941,7 @@ int k_lin_act_drop_fwd(fg_ctx* c, const float* z, const float* slope, const floa
 __global__ void lin_act_drop_bwd_kernel(const float* __restrict__ dh, const float* __restrict__ z,
                                         const float* __restrict__ slope, const float* __restrict__ masks, int moff,
                                         float scale, float* __restrict__ dz, float* __restrict__ dslope, int B, int N,
-                                        unsigned* __restrict__ amax) {
+                                        unsigned* __restrict__ amax, double* __restrict__ ws, unsigned* __restrict__ ticket) {
   float am = 0.f;
   const float a = *slope;
   const int64_t n = (int64_t)B * N;
@@ -929,12 +962,18 @@ __global__ void lin_act_drop_bwd_kernel(const float* __restrict__ dh, const floa
   }
   amax_commit(amax, am);
   s = block_sum(s);
-  if (threadIdx.x == 0 && dslope) atomicAdd(dslope, (float)s);
+  if (!dslope) return;
+  if (threadIdx.x == 0) ws[blockIdx.x] = s;
+  if (ordered_last_block(ticket)) {
+    if (threadIdx.x == 0) *dslope += (float)ordered_sum(ws, gridDim.x, 1, 0);
+    ordered_release(ticket);
+  }
 }
 int k_lin_act_drop_bwd(fg_ctx* c, const float* dh, const float* z, const float* slope, const float* masks, int moff,
                        float scale, float* dz, float* dslope, int B, int N) {
-  lin_act_drop_bwd_kernel<<<grid_for((int64_t)B * N, 256, 148), 256, 0, c->stream>>>(dh, z, slope, masks, moff, scale, dz,
-                                                                                   dslope, B, N, take_amax(c));
+  lin_act_drop_bwd_kernel<<<grid_for((int64_t)B * N, 256, 132), 256, 0, c->stream>>>(dh, z, slope, masks, moff, scale, dz,
+                                                                                   dslope, B, N, take_amax(c), c->red_ws,
+                                                                                   c->red_ticket);
   LAUNCH_CHECK(c);
   return FG_OK;
 }
@@ -1013,7 +1052,8 @@ int k_bce_bwd(fg_ctx* c, const float* x, const float* t, int n, float* dx) {
 // penalty (loss part), gate + Adam step-size preparation, fused penalty+clamp+Adam
 // ------------------------------------------------------------------------------------------------
 // *loss += l1*||p||_1 + l2*||p||_2^2/2                                    (adversarial.lua:105-106)
-__global__ void penalty_loss_kernel(const float* __restrict__ p, int64_t n, float l1, float l2, float* __restrict__ loss) {
+__global__ void penalty_loss_kernel(const float* __restrict__ p, int64_t n, float l1, float l2, float* __restrict__ loss,
+                                    double* __restrict__ ws, unsigned* __restrict__ ticket) {
   double s1 = 0, s2 = 0;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const double v = p[i];
@@ -1022,10 +1062,16 @@ __global__ void penalty_loss_kernel(const float* __restrict__ p, int64_t n, floa
   }
   s1 = block_sum(s1);
   s2 = block_sum(s2);
-  if (threadIdx.x == 0) atomicAdd(loss, (float)(l1 * s1 + l2 * s2 * 0.5));
+  if (threadIdx.x == 0) ws[blockIdx.x] = l1 * s1 + l2 * s2 * 0.5;
+  if (ordered_last_block(ticket)) {
+    if (threadIdx.x == 0) *loss += (float)ordered_sum(ws, gridDim.x, 1, 0);
+    ordered_release(ticket);
+  }
 }
+// the optimizer of D may run on the communication stream next to the compute stream's reductions: own workspace
 int k_penalty_loss(fg_ctx* c, const float* p, int64_t n, float l1, float l2, float* loss_inout) {
-  penalty_loss_kernel<<<grid_for(n, 256, 148 * 2), 256, 0, c->stream>>>(p, n, l1, l2, loss_inout);
+  penalty_loss_kernel<<<grid_for(n, 256, kOptRedRows), 256, 0, c->stream>>>(p, n, l1, l2, loss_inout, c->red_ws_opt,
+                                                                           c->red_ticket + 1);
   LAUNCH_CHECK(c);
   return FG_OK;
 }
@@ -1165,7 +1211,7 @@ int k_adam(fg_ctx* c, float* p, const float* g, float* m, float* v, int64_t n, f
            float l1_grad, float l2, float clampv, float grad_scale, const float* step_dev, const int* flag_dev,
            float step_host, float* g_out) {
   (void)g_out;
-  adam_kernel<<<grid_for(n, 256, 148 * 8), 256, 0, c->stream>>>(p, const_cast<float*>(g), m, v, n, beta1, beta2, eps,
+  adam_kernel<<<grid_for(n, 256, 132 * 8), 256, 0, c->stream>>>(p, const_cast<float*>(g), m, v, n, beta1, beta2, eps,
                                                                l1_grad, l2, clampv, grad_scale, step_dev, flag_dev,
                                                                step_host, 1, FG_OPT_ADAM, 0.f, nullptr);
   LAUNCH_CHECK(c);
@@ -1174,7 +1220,7 @@ int k_adam(fg_ctx* c, float* p, const float* g, float* m, float* v, int64_t n, f
 int k_optim_update(fg_ctx* c, int mode, float* p, float* g, float* m, float* v, int64_t n, float beta1, float beta2, float eps,
                    float mom, float l1_grad, float l2, float clampv, float grad_scale, const float* step_dev,
                    const int* flag_dev, const int* t_dev) {
-  adam_kernel<<<grid_for(n, 256, 148 * 8), 256, 0, c->stream>>>(p, g, m, v, n, beta1, beta2, eps, l1_grad, l2, clampv, grad_scale,
+  adam_kernel<<<grid_for(n, 256, 132 * 8), 256, 0, c->stream>>>(p, g, m, v, n, beta1, beta2, eps, l1_grad, l2, clampv, grad_scale,
                                                                step_dev, flag_dev, 0.f, 1, mode, mom, t_dev);
   LAUNCH_CHECK(c);
   return FG_OK;

@@ -3,7 +3,7 @@
 #include <cuda_fp16.h>
 
 // 3xFP16 split: x ~= hi + lo * 2^-11 with hi = fp16(x), lo = fp16((x - hi) * 2^11): 22 significant bits like the TF32
-// split, operands of kind::f16 MMAs (2x the TF32 rate, 4 bytes per element for hi+lo instead of 8).  fp16 subnormals
+// split, operands of f16 MMAs (2x the TF32 rate, 4 bytes per element for hi+lo instead of 8).  fp16 subnormals
 // keep the ABSOLUTE error at 2^-36, so a tensor whose max is in [2^-13, 65504] is represented to 2^-23 of that max;
 // activations and weights are used as they are, gradients are first scaled by a power of two (tc_amax).
 __device__ __forceinline__ void split_f16(float x, __half& hi, __half& lo) {

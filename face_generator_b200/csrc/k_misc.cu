@@ -16,7 +16,7 @@
   } while (0)
 
 namespace {
-inline int grid_for(int64_t n, int block, int cap = 148 * 16) {
+inline int grid_for(int64_t n, int block, int cap = 132 * 16) {
   int64_t g = (n + block - 1) / block;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
@@ -406,6 +406,20 @@ int k_dropout_nchw(fg_ctx* c, const float* x, const float* mask, float scale, in
     dropout_nchw_kernel<<<grid_for(n, 256), 256, 0, c->stream>>>(x, mask, scale, inner, y, n);
   else
     scale_kernel<<<grid_for(n, 256), 256, 0, c->stream>>>(x, scale, y, n);
+  LAUNCH_CHECK(c);
+  return FG_OK;
+}
+
+// out[i] = sum over s of parts[s * n + i], always in split order (deterministic split-K reduction)
+__global__ void splitk_reduce_kernel(const float* __restrict__ parts, int splits, int64_t n, float* __restrict__ out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float s = parts[i];
+    for (int k = 1; k < splits; ++k) s += parts[(int64_t)k * n + i];
+    out[i] = s;
+  }
+}
+int k_splitk_reduce(fg_ctx* c, const float* parts, int splits, int64_t n, float* out) {
+  splitk_reduce_kernel<<<grid_for(n, 256), 256, 0, c->stream>>>(parts, splits, n, out);
   LAUNCH_CHECK(c);
   return FG_OK;
 }

@@ -119,6 +119,12 @@ int net_alloc(fg_ctx* c) {
   FG_TRY(dalloc(c, &c->D_L2pd, 512 * 512));
   c->wgrad_ws_elems = 9 * 512 * 256;
   FG_TRY(dalloc(c, &c->wgrad_ws, c->wgrad_ws_elems));
+  c->splitk_ws_elems = (size_t)c->sm_count * 4 * 128 * 128;  // >= splits x output of every split-K weight gradient
+  FG_TRY(dalloc(c, &c->splitk_ws, c->splitk_ws_elems));
+  c->red_ws_elems = (size_t)4 << 20;  // >= blocks x partials of every ordered reduction (checked at each launch)
+  FG_TRY(dalloc(c, reinterpret_cast<float**>(&c->red_ws), 2 * c->red_ws_elems));
+  FG_TRY(dalloc(c, reinterpret_cast<float**>(&c->red_ws_opt), 2 * kOptRedRows));
+  FG_TRY(dalloc(c, reinterpret_cast<float**>(&c->red_ticket), 2));  // zeroed; every ordered reduction resets its ticket
   FG_TRY(dalloc(c, &c->small_ws, (size_t)kSmallMaxParts * 9 * 4 * 128));
   // G activations
   FG_TRY(dalloc(c, &c->G_noise, B * kNoiseDim));
@@ -169,7 +175,7 @@ int net_alloc(fg_ctx* c) {
   c->io_dev_elems = std::max<size_t>(B * 1024 * C, B * kMaskPerSample);
   FG_TRY(dalloc(c, &c->io_dev, c->io_dev_elems));
   FG_TRY(dalloc(c, &c->io_dev2, c->io_dev_elems));
-  {  // tcgen05 path buffers
+  {  // tensor-core path buffers
     fg_ctx::TcBufs& t = c->tcb;
     FG_TRY(dalloc(c, &t.G_h0_hi, B * 8192));
     FG_TRY(dalloc(c, &t.G_h0_lo, B * 8192));
@@ -335,7 +341,7 @@ int net_pack_D(fg_ctx* c) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-// conv dispatch (SIMT now; tcgen05 variants are selected in k_conv_tc.cu)
+// conv dispatch (SIMT now; tensor-core variants are selected in k_conv_tc.cu)
 // ---------------------------------------------------------------------------------------------------
 static int conv_fwd(fg_ctx* c, const char* tag, const float* in, const float* Wp, const float* bias, float* out,
                     ConvGeom g) {
@@ -360,7 +366,7 @@ static inline bool use_tc_wgrad(const fg_ctx* c, const ConvGeom& g) {
   return use_tc(c, g) && g.Cout % 128 == 0 && g.Cin % 64 == 0;
 }
 
-// ---- option "mma_f16": every tensor-core operand in the 3xFP16 split (k_conv_tc.cu), kind::f16 MMAs -------------------
+// ---- option "mma_f16": every tensor-core operand in the 3xFP16 split (k_conv_tc.cu), f16 MMAs -----------------------
 // Activations and gradients are scaled into fp16's range by a power of two found on the device (tc_amax): slot i of
 // c->amax_slot holds (max|x|, 1/scale) of one tensor; the consuming kernels multiply their result by the inverse scales.
 // One slot per tensor and pass, so that a producer can reduce max|output| while it writes the tensor (AmaxInto) instead of
@@ -395,7 +401,7 @@ static int split_h_scaled(fg_ctx* c, const float* x, float* hh, float* hl, int64
 }
 
 // nn.Linear as a 1x1 convolution on a 1x1 image.  With only B rows the fp32 SIMT tiling leaves the GPU
-// idle (8 CTAs at B=256); the tcgen05 path splits the input on the fly and uses the pre-split weights.
+// idle (8 CTAs at B=256); the tensor-core path splits the input on the fly and uses the pre-split weights.
 // f16 mode: `in16` is the fp32 input (always given), split into keep16_h/l (or the dY scratch) under amax slot `slot`
 static int lin_fwd(fg_ctx* c, const char* tag, const float* in, const float* Wp, int wi, const float* bias, float* out,
                    ConvGeom g, float* keep_hi = nullptr, float* keep_lo = nullptr, const float* in16 = nullptr,
@@ -431,7 +437,7 @@ static int lin_wgrad_tc(fg_ctx* c, const char* tag, const float* x_hi, const flo
 }
 
 // G's two nn.SpatialUpSamplingNearest(2) -> 5x5 convolutions (li = 0: C1, li = 1: C2), forward.
-// tcgen05 path: split the low-res input into TF32 hi/lo once (kept for wgrad), then the phase conv.
+// tensor-core path: split the low-res input into TF32 hi/lo once (kept for wgrad), then the phase conv.
 // *stat_parts (optional, in: want BatchNorm partials; out: how many tiles wrote one into c->bn_parts, 0 = none)
 static int g_ups_fwd(fg_ctx* c, int li, const char* tag, const float* h, float* h_hi, float* h_lo, const float* Wp,
                      const float* bias, float* z, ConvGeom g, int* stat_parts = nullptr) {
@@ -454,7 +460,7 @@ static int g_ups_fwd(fg_ctx* c, int li, const char* tag, const float* h, float* 
   return tc_conv_fwd(c, h_hi, h_lo, t.G_Wf_hi[li], t.G_Wf_lo[li], bias, z, g, 2, st, st ? stat_parts : nullptr);
 }
 // backward of the same layer: dW += wgrad, dh = dgrad.  *pooled tells whether `dh` already is the gradient of
-// the LOW-RES input (tcgen05 path: the 2x2 sum of the upsample backward is folded into the dgrad GEMM) or the
+// the LOW-RES input (tensor-core path: the 2x2 sum of the upsample backward is folded into the dgrad GEMM) or the
 // full-resolution gradient that the consumer still has to sum 2x2 (SIMT path).
 static int g_ups_bwd(fg_ctx* c, int li, const char* wtag, const char* dtag, const float* h, const float* h_hi,
                      const float* h_lo, const float* dz, const float* Wpd, ConvGeom g, float* dW, float* dh, bool* pooled,
@@ -539,7 +545,7 @@ int net_G_forward(fg_ctx* c, const float* noise, int B, bool training) {
     FG_TRY(k_bn_eval_prep(c, c->bnG, c->bnG + 256, c->bn_mean1, c->bn_istd1, 256));
   }
   const ConvGeom gC2{B, 32, 32, 256, 128, 5, 2};
-  const bool h1_split = training && use_tc(c, gC2) && !f16_on(c);  // TF32 tcgen05 path consumes h1 only as TF32 hi/lo
+  const bool h1_split = training && use_tc(c, gC2) && !f16_on(c);  // TF32 tensor-core path consumes h1 only as TF32 hi/lo
   {
     AmaxInto am(c, kSlotH1);
     FG_TRY(k_bn_prelu_apply(c, c->G_z1, c->bn_mean1, c->bn_istd1, P + L.g1, P + L.be1, P + L.a2,
@@ -596,7 +602,7 @@ int net_G_backward(fg_ctx* c, const float* dy, float* dnoise) {
                                  G + L.a3, B, 32, 32, 128, 0));
   }
   FG_TRY(k_bn_bwd_finalize(c, c->bn_acc, c->bn_mg, G + L.g2, G + L.be2, (int64_t)B * 1024, 128));
-  // in tcgen05 mode the BN-backward kernels also emit the TF32 hi/lo split of dz (no separate split pass)
+  // in tensor-core mode the BN-backward kernels also emit the TF32 hi/lo split of dz (no separate split pass)
   const ConvGeom gC2{B, 32, 32, 256, 128, 5, 2}, gC1{B, 16, 16, 128, 256, 5, 2};
   const bool tc2 = use_tc_wgrad(c, gC2) && !f16_on(c), tc1 = use_tc_wgrad(c, gC1) && !f16_on(c);  // fused TF32 hi/lo of dz
   {

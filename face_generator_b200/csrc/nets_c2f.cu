@@ -7,7 +7,7 @@
 //   loop = adversarial_c2f.lua:121-187 (fevalD :40-81, fevalG_on_D :85-116, optim.adam)
 // cudnn.SpatialConvolutionUpsample with factor 1 (layers/cudnnSpatialConvolutionUpsample.lua:4-28) is a "same"
 // convolution whose output view is the identity, so every layer maps onto the tap-GEMM convolution kernels:
-// tcgen05 (3xTF32, chunk-promoted) where the channel counts make a dense contraction (64->64, 64->128,
+// wgmma (3xTF32, chunk-promoted) where the channel counts make a dense contraction (64->64, 64->128,
 // 128->256 and the 16384->512 Linear), the bandwidth-shaped small-channel kernels for (C+1)->64 / C->64 and the
 // fp32 FFMA tile kernel for the 256->C 7x7 output layer (N = 3 is not a tensor-core shape).
 #include <algorithm>

@@ -7,7 +7,7 @@
 //                       conv(512->1024,3,STRIDE 2) PReLU SpatialDropout() View(4096) Linear(4096,1024) PReLU
 //         dense branch: View(C*256) Linear(C*256,128) PReLU Dropout() Linear(128,128) PReLU
 //   loop = adversarial.lua:83-288 (the same fevalD / fevalG_on_D / accuracy gate / interruptable optimizers as the 32x32 nets)
-// Kernels: the two upsampled 5x5 layers use the phase-collapsed tcgen05 kernels of the 32x32 generator (forward with
+// Kernels: the two upsampled 5x5 layers use the phase-collapsed wgmma kernels of the 32x32 generator (forward with
 // BatchNorm partials from the epilogue, wgrad, dgrad with the upsample backward folded in); every other layer is a ConvL
 // (convl.h).  A stride-2 "same" 3x3 convolution is the stride-1 one sampled at the even pixels: forward = stride-1
 // kernel + subsample, backward = the stride-1 dgrad / wgrad of dY with zeros inserted at the odd pixels.  That is exact
@@ -31,7 +31,7 @@ namespace {
 constexpr int kS16Mask = 1024 + 128;  // nn.SpatialDropout() planes + nn.Dropout() of the dense branch, per sample
 constexpr int kSide = 16;
 
-inline int grid_for(int64_t n, int block, int cap = 148 * 16) {
+inline int grid_for(int64_t n, int block, int cap = 132 * 16) {
   int64_t g = (n + block - 1) / block;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
@@ -416,7 +416,7 @@ int ups_fwd(fg_s16* n, UpsL& U, const float* h, float* z, int B, int* parts) {
   return tc_conv_fwd(c, U.h_hi, U.h_lo, U.Wf_hi, U.Wf_lo, n->PG + U.b_off, z, g, 2, st, st ? parts : nullptr, h16,
                      h16 ? U.sx + 1 : nullptr);
 }
-// dW += wgrad; dh = dgrad.  *pooled: dh already is the gradient of the LOW-RES input (tcgen05 path folds the 2x2 sum of
+// dW += wgrad; dh = dgrad.  *pooled: dh already is the gradient of the LOW-RES input (tensor-core path folds the 2x2 sum of
 // the upsample backward into the dgrad GEMM); otherwise dh is the full-resolution gradient the consumer sums 2x2.
 int ups_bwd(fg_s16* n, UpsL& U, const float* h, const float* dz, float* dh, int B, bool* pooled) {
   fg_ctx* c = n->c;

@@ -165,7 +165,6 @@ SYMBOLS = {
     "fg_memcpy": (_I, [_P, _P, _P, _SZ]),
     "fg_kernel_launches": (_L, [_P]),
     "fg_debug_tensor": (_L, [_P, C.c_char_p, _P, _L]),
-    "fg_debug_umma_window": (_I, [_P, _P, _P, _I, _I, _I, _P]),
     "fg_bench_tf32_peak": (_I, [_P, _I, C.POINTER(C.c_double)]),
     "fg_event_record": (_I, [_P, _I]),
     "fg_event_elapsed_ms": (_I, [_P, _I, _I, C.POINTER(C.c_double)]),
@@ -401,7 +400,7 @@ class Context:
         self.lib.fg_dev_free(p)
 
     def tf32_peak(self, iters=20000):
-        """measured tcgen05 kind::tf32 issue rate in TFLOP/s (roofline denominator of the 3xTF32 convolutions)"""
+        """measured tf32 wgmma issue rate in TFLOP/s (roofline denominator of the 3xTF32 convolutions)"""
         v = C.c_double(0)
         _check(self.lib.fg_bench_tf32_peak(self.h, iters, C.byref(v)), "fg_bench_tf32_peak")
         return v.value

@@ -157,7 +157,6 @@ int fg_memcpy(fg_ctx* ctx, void* dst, const void* src, size_t bytes);
 int64_t fg_kernel_launches(fg_ctx* ctx);
 int64_t fg_debug_tensor(fg_ctx* ctx, const char* name, float* dst, int64_t max_elems);
 int fg_bench_tf32_peak(fg_ctx* ctx, int iters, double* tflops);
-int fg_debug_umma_window(fg_ctx* ctx, const float* x_dev, const float* ident_dev, int dy, int dx, int use_base_offset, float* out_dev);
 int fg_event_record(fg_ctx* ctx, int slot);
 int fg_event_elapsed_ms(fg_ctx* ctx, int slot_a, int slot_b, double* ms);
 int fg_timing_enable(fg_ctx* ctx, int on);

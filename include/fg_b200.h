@@ -1,4 +1,4 @@
-/* fg_b200.h -- C ABI of the B200-native GAN train-step hot path of aleju/face-generator.
+/* fg_b200.h -- C ABI of the H100-native GAN train-step hot path of aleju/face-generator.
  *
  * The reference (Lua/Torch7) has NO native FFI for this path: its "plugin surface" is Torch7's
  * Lua-level nn.Module protocol plus train.lua's globals (SURVEY.md section 8b).  This header is
@@ -40,8 +40,8 @@ enum { FG_NET_G = 0, FG_NET_D = 1 };
 /* Which implementation the big convolutions use (fg_set_option "conv_impl"). */
 enum {
   FG_CONV_SIMT = 0,         /* fp32 FFMA implicit GEMM (first correct path, any shape)          */
-  FG_CONV_TC_DENSE = 1,     /* tcgen05 3xTF32 implicit GEMM, dense 5x5 taps on the low-res input */
-  FG_CONV_TC_COLLAPSED = 2  /* tcgen05 3xTF32, upsample folded into four 3x3 phase convolutions  */
+  FG_CONV_TC_DENSE = 1,     /* wgmma 3xTF32 implicit GEMM, dense 5x5 taps on the low-res input   */
+  FG_CONV_TC_COLLAPSED = 2  /* wgmma 3-term split, upsample folded into four 3x3 phase convs    */
 };
 
 /* OPT.D_optmethod / OPT.G_optmethod (train.lua:38-39; adversarial.lua:259-285):
@@ -384,13 +384,9 @@ int64_t fg_debug_tensor(fg_ctx* ctx, const char* name, float* dst, int64_t max_e
 int fg_event_record(fg_ctx* ctx, int slot);
 int fg_event_elapsed_ms(fg_ctx* ctx, int slot_a, int slot_b, double* ms);
 int fg_timing_enable(fg_ctx* ctx, int on);
-/* tensor-pipe probe for the roofline: TFLOP/s of back-to-back tcgen05.mma.kind::tf32 (M=128,N=256,K=8, operands
- * resident in shared memory) on all SMs, best of 5 event-timed launches of `iters` x 4 MMAs per SM            */
+/* tensor-pipe probe for the roofline: TFLOP/s of back-to-back tf32 wgmmas (two warpgroups of M=64,N=256,K=8 per
+ * SM, operands resident in shared memory) on all SMs, best of 5 event-timed launches of `iters` x 4 MMAs per SM */
 int fg_bench_tf32_peak(fg_ctx* ctx, int iters, double* tflops);
-/* hardware probe used by tests/test_gpu_umma_window.py: D = A * I where A is the 128-row window
- * {(yi+dy)*16 + xi+dx} of a [288][32] fp32 tile (DEVICE pointers; x values must be TF32-exact)   */
-int fg_debug_umma_window(fg_ctx* ctx, const float* x_dev, const float* ident_dev, int dy, int dx, int use_base_offset,
-                         float* out_dev);
 int fg_timing_get(fg_ctx* ctx, const char* name, double* ms_total, int64_t* launches);
 
 #ifdef __cplusplus

@@ -5,7 +5,7 @@ stream, warm-up, synchronise on both sides); one JSON line per config.  Informat
   configs[4]  sample.lua 1024-image generation-only throughput (chunk 16 = script default, and 1024)
   configs[0]  gray batch 16 train step (the CPU-runnable case) on the GPU, for scale
 
-usage (GPU box):  python profiles/bench_configs.py [--steps 10] > gpurun_out/configs.jsonl
+usage:  python profiles/bench_configs.py [--steps 10] > configs.jsonl
 """
 import argparse
 import json

@@ -4,7 +4,7 @@ shapes of BASELINE configs[1] (batch 256), forward + input gradient + weight gra
 Measurement infrastructure only (PyTorch is not part of the product).  fp32 = TF32 disabled (the parity-equivalent
 setting); "tf32" = cuDNN allowed to use TF32 tensor cores (1e-3 relative error: would fail the 1e-4 bar).
 
-usage (GPU box):  python profiles/cudnn_bar.py > gpurun_out/cudnn_bar.jsonl"""
+usage:  python profiles/cudnn_bar.py > cudnn_bar.jsonl"""
 import json
 
 import torch

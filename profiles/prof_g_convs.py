@@ -1,8 +1,8 @@
 """ncu driver: 3 iterations of G forward+backward at B=256 (colour) so that
    tapconv launches per iteration = [G.C1 fwd, G.C2 fwd, G.C2 dgrad, G.C1 dgrad], wgrad = [G.C2 wgrad, G.C1 wgrad].
-Usage (under gpurun):
-   ncu --set full --clock-control none --import-source on -k regex:tapconv_tc -s 8 -c 4 -o gpurun_out/prof_tapconv python profiles/prof_g_convs.py
-   ncu --set full --clock-control none --import-source on -k regex:wgrad_tc  -s 4 -c 2 -o gpurun_out/prof_wgrad  python profiles/prof_g_convs.py
+Usage:
+   ncu --set full --clock-control none --import-source on -k regex:tapconv_tc -s 8 -c 4 -o /tmp/prof_tapconv python profiles/prof_g_convs.py
+   ncu --set full --clock-control none --import-source on -k regex:wgrad_tc  -s 4 -c 2 -o /tmp/prof_wgrad  python profiles/prof_g_convs.py
 """
 import os, sys
 import numpy as np

@@ -1,6 +1,6 @@
 """ncu driver: a few fg_train_step iterations at batch 256 (colour), everything resident on the device.
-   launch list :  ncu --metrics gpu__time_duration.sum --clock-control none -c 600 --csv --log-file gpurun_out/launches.csv python profiles/prof_step.py 2
-   one kernel  :  ncu --set full --clock-control none --import-source on -k regex:<name> -s <skip> -c <n> -o gpurun_out/prof_x python profiles/prof_step.py 2
+   launch list :  ncu --metrics gpu__time_duration.sum --clock-control none -c 600 --csv --log-file /tmp/launches.csv python profiles/prof_step.py 2
+   one kernel  :  ncu --set full --clock-control none --import-source on -k regex:<name> -s <skip> -c <n> -o /tmp/prof_x python profiles/prof_step.py 2
 """
 import os
 import sys

@@ -1,5 +1,5 @@
 """Summarise an .ncu-rep (ncu --set full) into the handful of metrics DESIGN.md / bench.py quote.
-usage: python profiles/summarize_ncu.py gpurun_out/prof.ncu-rep > profiles/<name>.md"""
+usage: python profiles/summarize_ncu.py /tmp/prof.ncu-rep > <name>.md"""
 import csv
 import io
 import subprocess

@@ -1,4 +1,4 @@
-"""times G's tcgen05 conv launches (CUDA events via fg_timing) for experiments: FG_TC_DBG=0/1/2"""
+"""times G's tensor-core conv launches (CUDA events via fg_timing); IMPL selects conv_impl"""
 import os, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -22,4 +22,4 @@ out = {}
 for k in ("G.C1.fwd", "G.C2.fwd", "G.C2.dgrad", "G.C1.dgrad", "G.C2.wgrad", "G.C1.wgrad"):
     ms, n = ctx.timing_get(k)
     out[k] = round(ms / max(n, 1), 4)
-print("DBG", os.environ.get("FG_TC_DBG", "0"), out)
+print("IMPL", os.environ.get("IMPL", "2"), out)

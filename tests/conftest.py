@@ -14,4 +14,4 @@ os.environ.setdefault("OMP_NUM_THREADS", str(max(1, min(32, os.cpu_count() or 1)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); select with -m gpu")

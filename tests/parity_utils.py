@@ -66,7 +66,7 @@ def oracle_iteration(case, B, C, hyper=None, state=None):
 # so a wrong x<=0 branch, a wrong slope gradient or a wrong mask shows up at the strict 1e-4 bar.  The tests also
 # assert that the ambiguous set is tiny (<= KINK_MAX_FRAC of a layer) and that the CUDA pre-activations of those
 # elements are indeed ~0 (which also proves the NCHW->NHWC index mapping).
-KINK_MARGIN = 2e-5      # single-net passes: the tcgen05 path is within ~5e-6 of the oracle (normwise)
+KINK_MARGIN = 2e-5      # single-net passes: the tensor-core path is within ~5e-6 of the oracle (normwise)
 KINK_MAX_FRAC = 2e-3
 
 

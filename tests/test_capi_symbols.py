@@ -21,7 +21,7 @@ def test_library_exports_every_declared_symbol():
     for n in names:
         assert hasattr(lib, n), "libfg_b200.so does not export %s" % n
     assert sorted(SYMBOLS) == names, "python binding and header disagree: %s" % (set(SYMBOLS) ^ set(names))
-    assert b"sm_100a" in lib.fg_version()
+    assert b"sm_90a" in lib.fg_version()
 
 
 def test_no_cpu_fallback_create_fails_loudly_without_gpu():

@@ -1,4 +1,4 @@
-"""Data-parallel parity on real GPUs (needs >= 2 B200s: run under `gpurun --gpus 2`; skipped on one GPU).
+"""Data-parallel parity on real GPUs (needs >= 2 GPUs; skipped on one GPU).
 Two processes, one per GPU, NCCL all-reduce inside fg_train_step; checked against the oracle-based DP
 restatement (tests/dp_ref.py) and for replica equality."""
 import os
@@ -52,7 +52,7 @@ def _worker(rank, world, port, impl, q):
 @pytest.mark.parametrize("impl", [0, 2])
 def test_dp_two_gpus_match_oracle_and_each_other(impl):
     if _gpu_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import threading
     import torch.multiprocessing as mp
     import parity_utils as PU
@@ -144,7 +144,7 @@ def _worker_c2f(rank, world, port, q):
 def test_dp_c2f_two_gpus_average_gradients():
     """adversarial_c2f loop under data parallelism: every rank ends with the mean of the per-shard gradients."""
     if _gpu_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     import parity_utils as PU
     world, port = 2, 29761
@@ -202,7 +202,7 @@ def test_dp_resume_broadcasts_step_counters():
     """fg_dp_broadcast_params carries t_D / t_G (Adam's bias correction depends on them): after a resume on rank 0
     only, replicas must stay bit-identical over the following steps."""
     if _gpu_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     world, port = 2, 29781
     mpc = mp.get_context("spawn")
@@ -259,7 +259,7 @@ def test_dp_overlap_matches_serial_schedule():
     runs -- three steps give the losses, confusion counts and (up to run-to-run rounding) parameters of the serial schedule,
     and the two ranks stay bit-identical."""
     if _gpu_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     world, port = 2, 29761
     mpc = mp.get_context("spawn")

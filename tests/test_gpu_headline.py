@@ -1,6 +1,6 @@
 """Parity at the HEADLINE size (BASELINE.json configs[1]: colour, batch 256 per GPU) and at a ragged batch (130).
 
-At B=256 the persistent tcgen05 kernels run ~14 tiles per CTA (TMEM ring wrap-around, cross-block phase waits,
+At B=256 the persistent wgmma kernels run many tiles per CTA (stage-ring wrap-around, cross-block phase waits,
 split-K sized to a wave, the BN=64/128 tile heuristic) -- code paths the small-batch parity tests never reach.
 The fp64 C++ oracle needs ~1 min per iteration at this size, so two checkers are used:
 
@@ -86,8 +86,8 @@ def test_G_at_headline_batch(fg, B):
     # ---- every forward launch on the CUDA path's own input ----
     up = lambda t: F.interpolate(t, scale_factor=2, mode="nearest")
     assert rel(T["z0"], F.linear(dev(noise), p["L1W"], p["L1b"]).view(B, 128, 8, 8)) < KTOL
-    assert rel(T["z1"], F.conv2d(up(T["h0"]), p["C1W"], p["C1b"], padding=2)) < KTOL  # tcgen05, collapsed phases
-    assert rel(T["z2"], F.conv2d(up(T["h1"]), p["C2W"], p["C2b"], padding=2)) < KTOL  # tcgen05, collapsed phases
+    assert rel(T["z1"], F.conv2d(up(T["h0"]), p["C1W"], p["C1b"], padding=2)) < KTOL  # tensor cores, collapsed phases
+    assert rel(T["z2"], F.conv2d(up(T["h1"]), p["C2W"], p["C2b"], padding=2)) < KTOL  # tensor cores, collapsed phases
     assert rel(T["z3"], F.conv2d(T["h2"], p["C3W"], p["C3b"], padding=1)) < KTOL
     for zn, hn, g, be, a in (("z1", "h1", "g1", "be1", "a2"), ("z2", "h2", "g2", "be2", "a3")):
         y = F.batch_norm(T[zn], None, None, p[g], p[be], training=True, eps=1e-5)

@@ -285,7 +285,7 @@ def test_modules_equal_fused_step(fg):
 @pytest.mark.parametrize("N,Cin,H,Cout,k", [(8, 64, 16, 128, 3), (3, 128, 8, 256, 3), (5, 256, 4, 512, 3),
                                             (2, 32, 32, 64, 5), (3, 64, 16, 128, 7), (1, 128, 32, 128, 1)])
 def test_tc_conv_lop(fg, N, Cin, H, Cout, k):
-    """tcgen05 3xTF32 implicit-GEMM kernels (fwd, dgrad, wgrad) in isolation through the L-op ABI; includes batch
+    """wgmma 3xTF32 implicit-GEMM kernels (fwd, dgrad, wgrad) in isolation through the L-op ABI; includes batch
     tails that do not fill a 128-pixel tile (TMA zero fill + predicated epilogue)."""
     from face_generator_b200.lib import _ptr
     rng = np.random.default_rng(100 + N + Cin)

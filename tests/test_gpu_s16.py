@@ -3,7 +3,7 @@ loop on them, plus cudnn.SpatialConvolutionUpsample with factor != 1 (layers/cud
 
 CPU: the C ABI reports the oracle's parameter counts.
 GPU (-m gpu): fg_s16_* / fg_scu_* through the C ABI against the fp64 oracle on the same seeded inputs, both conv
-implementations (0 = fp32 FFMA kernels, 2 = tcgen05 3xTF32).  Tolerance 1e-4 relative (BASELINE.json north_star).
+implementations (0 = fp32 FFMA kernels, 2 = wgmma 3-term split).  Tolerance 1e-4 relative (BASELINE.json north_star).
 Gradients are compared strictly on the "smooth" (PReLU slopes 1) and "near" (slopes 1 - k*1e-3, see s16_utils) inits;
 the "trained" init (slopes 0.25) holds the forward values to 1e-4 and the gradients to the kink bar."""
 import numpy as np
@@ -231,7 +231,7 @@ def test_gpu_s16_accuracy_gate_and_generated_masks():
 
 @pytest.mark.gpu
 def test_gpu_s16_batch_256_runs_on_the_tensor_cores():
-    """BASELINE batch size: finite losses, and the two stride-2 layers / Linear layers take the tcgen05 path
+    """BASELINE batch size: finite losses, and the two stride-2 layers / Linear layers take the tensor-core path
     (their timers are only attached to tensor-core launches' names, so compare impl 0 vs 2 outputs instead)."""
     from face_generator_b200.lib import NET_D, NET_G, hyper_default
     B, C = 256, 3

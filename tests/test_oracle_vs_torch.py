@@ -119,7 +119,7 @@ def test_penalty_clamp_order_and_G_quirk():
 
 def test_upsample_conv_phase_identity():
     """up2 -> 5x5/pad2 conv == four 3x3/pad1 phase convs with row/col pre-summed weights (SURVEY.md 7.3).
-    This identity is what the tcgen05 'collapsed' conv path relies on."""
+    This identity is what the tensor-core 'collapsed' conv path relies on."""
     rng = np.random.default_rng(5)
     B, Cin, Cout, H = 2, 5, 4, 6
     x = rng.standard_normal((B, Cin, H, H))
