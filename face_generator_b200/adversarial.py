@@ -98,7 +98,8 @@ def train(ctx, dataset, hyper, batch_size, n_epoch=-1, rng=None, epoch=1, rank=0
 
     ctx: a Context (the 32x32 nets) or an S16 built on one (train.lua --scale 16: the 16x16 nets, images [N][C][16][16]).
     dataset: array-like [N][C][32][32] float32 in [0,1] (what DATASET.loadImages returns, dataset.lua:43-75) or a
-    face_generator_b200.dataset.DeviceDataset (then batch assembly and noise happen on the device).
+    face_generator_b200.dataset.DeviceDataset (then batch assembly and noise happen on the device, at 16x16 through
+    fg_s16_train_step_dataset when ctx is an S16).
     hyper.D_maxAcc / hyper.accs_interval are the maxAccuracyD / accsInterval arguments.
     epoch / rank: the reference draws fresh math.random indices and uniform noise on every call
     (adversarial.lua:245, :276), so successive epochs must not replay the same draws: the step seeds (device-side
@@ -106,6 +107,7 @@ def train(ctx, dataset, hyper, batch_size, n_epoch=-1, rng=None, epoch=1, rank=0
     for host-resident datasets is derived from (epoch, rank) unless the caller passes (and keeps) its own `rng`.
     Returns (accuracy of D over the epoch = CONFUSION.totalValid (:316), confusion counts [4], batches that trained D)."""
     from .dataset import DeviceDataset
+    from .lib import S16
     seed0 = epoch_seed0(epoch, rank)
     rng = rng if rng is not None else np.random.default_rng([int(epoch), int(rank), 0x6661636573])
     on_device = isinstance(dataset, DeviceDataset)
@@ -115,7 +117,9 @@ def train(ctx, dataset, hyper, batch_size, n_epoch=-1, rng=None, epoch=1, rank=0
     trained = 0
     for i, (t, B) in enumerate(epoch_batches(n_epoch, batch_size)):
         seed = seed0 + i + 1
-        if on_device:
+        if on_device and isinstance(ctx, S16):
+            st = ctx.train_step_dataset(dataset, hyper, B, seed)               # the 16x16 real half, on the device
+        elif on_device:
             st = dataset.train_step(hyper, B, seed)
         else:
             real = np.ascontiguousarray(np.asarray(dataset)[rng.integers(0, N, B // 2)], np.float32)  # :244-249

@@ -100,6 +100,41 @@ __device__ __forceinline__ Span axis_span(int di, int src_len, int dst_len) {
 }
 __device__ __forceinline__ float span_w(const Span& s, int i) { return i == s.i0 ? s.w0 : (i == s.i1 ? s.w1 : 1.f); }
 
+// image.scale's output pixel (y, x) of an Ho x Wo image from an Hs x Ws source, src(yy, xx) = source value: pass 1
+// (width) then pass 2 (height), like image.scale's two-pass implementation.  Every rescale of the input side goes
+// through here, so the scaling rule lives in one place.
+template <class Src>
+__device__ __forceinline__ float scale_pixel(const Src& src, int y, int x, int Hs, int Ws, int Ho, int Wo) {
+  const Span sy = axis_span(y, Hs, Ho), sx = axis_span(x, Ws, Wo);
+  float acc_y = 0.f;
+  for (int yy = sy.i0; yy <= sy.i1; ++yy) {
+    float acc_x = 0.f;
+    for (int xx = sx.i0; xx <= sx.i1; ++xx) acc_x += span_w(sx, xx) * src(yy, xx);
+    acc_y += span_w(sy, yy) * (acc_x / sx.norm);
+  }
+  return acc_y / sy.norm;
+}
+// image.load(..., "float") of channel ch of one cached image: byte/255, image.rgb2y when gray
+struct U8Src {
+  const uint8_t* base;
+  int ch, Hs, Ws;
+  bool gray;
+  __device__ __forceinline__ float operator()(int yy, int xx) const {
+    if (gray) {
+      const float rr = base[(0 * Hs + yy) * Ws + xx] * (1.f / 255.f), gg = base[(1 * Hs + yy) * Ws + xx] * (1.f / 255.f),
+                  bb = base[(2 * Hs + yy) * Ws + xx] * (1.f / 255.f);
+      return 0.299f * rr + 0.587f * gg + 0.114f * bb;
+    }
+    return base[((int64_t)ch * Hs + yy) * Ws + xx] * (1.f / 255.f);
+  }
+};
+// one fp32 plane [H][W] (shared memory)
+struct PlaneSrc {
+  const float* p;
+  int W;
+  __device__ __forceinline__ float operator()(int yy, int xx) const { return p[yy * W + xx]; }
+};
+
 // out[b][c][y][x] (C channels, Ho x Wo) from u8 data[idx[b]][Cs][Hs][Ws]; gray = Cs==3 && C==1 (rgb2y)
 __global__ void gather_kernel(const uint8_t* __restrict__ data, const int32_t* __restrict__ idx, float* __restrict__ out,
                               int B, int C, int Cs, int Hs, int Ws, int Ho, int Wo, int64_t N) {
@@ -113,27 +148,48 @@ __global__ void gather_kernel(const uint8_t* __restrict__ data, const int32_t* _
     const int b = (int)(r / C);
     int64_t img = idx[b];
     img = img < 0 ? 0 : (img >= N ? N - 1 : img);
-    const Span sy = axis_span(y, Hs, Ho), sx = axis_span(x, Ws, Wo);
-    const bool gray = Cs == 3 && C == 1;
-    const uint8_t* base = data + img * (int64_t)Cs * Hs * Ws;
-    // pass 1 (width) then pass 2 (height), like image.scale's two-pass implementation
-    float acc_y = 0.f;
-    for (int yy = sy.i0; yy <= sy.i1; ++yy) {
-      float acc_x = 0.f;
-      for (int xx = sx.i0; xx <= sx.i1; ++xx) {
-        float v;
-        if (gray) {
-          const float rr = base[(0 * Hs + yy) * Ws + xx] * (1.f / 255.f), gg = base[(1 * Hs + yy) * Ws + xx] * (1.f / 255.f),
-                      bb = base[(2 * Hs + yy) * Ws + xx] * (1.f / 255.f);
-          v = 0.299f * rr + 0.587f * gg + 0.114f * bb;
-        } else {
-          v = base[((int64_t)ch * Hs + yy) * Ws + xx] * (1.f / 255.f);
-        }
-        acc_x += span_w(sx, xx) * v;
-      }
-      acc_y += span_w(sy, yy) * (acc_x / sx.norm);
-    }
-    out[i] = acc_y / sy.norm;
+    const U8Src src{data + img * (int64_t)Cs * Hs * Ws, ch, Hs, Ws, Cs == 3 && C == 1};
+    out[i] = scale_pixel(src, y, x, Hs, Ws, Ho, Wo);
+  }
+}
+// dataset_c2f.lua:49-62 _toResult at fineSize 32, one cached image per CTA:
+//   fine   = the 32x32 gather of the image (the per-pixel code of gather_kernel, so bit-identical to it), kept in
+//            shared memory as fp32 (the reference holds it in a FloatTensor before scaling it again)
+//   tmp    = image.scale(fine, cs, cs)            (shared memory)
+//   coarse = image.scale(tmp, 32, 32)
+//   diff   = fine - coarse                        (torch.add(fine, -1, coarse))
+// Outputs are NCHW [B][C][32][32]; any may be null.  Per image: Cs*Hs*Ws bytes read, up to 3 * C * 4 KB written.
+constexpr int kPairThreads = 256;
+__global__ void __launch_bounds__(kPairThreads) c2f_pairs_kernel(const uint8_t* __restrict__ data, const int32_t* __restrict__ idx,
+                                                                 float* __restrict__ fine, float* __restrict__ coarse,
+                                                                 float* __restrict__ diff, int C, int Cs, int Hs, int Ws, int cs,
+                                                                 int64_t N) {
+  __shared__ float sfine[3 * 1024];
+  __shared__ float stmp[3 * 1024];
+  const int b = blockIdx.x, n = C * 1024, m = cs * cs;
+  int64_t img = idx[b];
+  img = img < 0 ? 0 : (img >= N ? N - 1 : img);
+  const uint8_t* base = data + img * (int64_t)Cs * Hs * Ws;
+  const bool gray = Cs == 3 && C == 1;
+  const int64_t o = (int64_t)b * n;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const int x = i & 31, y = (i >> 5) & 31, ch = i >> 10;
+    const float v = scale_pixel(U8Src{base, ch, Hs, Ws, gray}, y, x, Hs, Ws, 32, 32);
+    sfine[i] = v;
+    if (fine) fine[o + i] = v;
+  }
+  if (!coarse && !diff) return;
+  __syncthreads();
+  for (int i = threadIdx.x; i < C * m; i += blockDim.x) {
+    const int ch = i / m, r = i - ch * m, y = r / cs, x = r - y * cs;
+    stmp[i] = scale_pixel(PlaneSrc{sfine + ch * 1024, 32}, y, x, 32, 32, cs, cs);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const int x = i & 31, y = (i >> 5) & 31, ch = i >> 10;
+    const float v = scale_pixel(PlaneSrc{stmp + ch * m, cs}, y, x, cs, cs, 32, 32);
+    if (coarse) coarse[o + i] = v;
+    if (diff) diff[o + i] = sfine[i] - v;
   }
 }
 __global__ void draw_indices_kernel(int32_t* __restrict__ idx, int B, uint64_t seed, int64_t N) {
@@ -228,11 +284,27 @@ bool is_dev(const void* p) {
   }
   return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
-int gather(fg_dataset* d, const int32_t* idx_dev, int B, float* out_dev) {
+int gather(fg_dataset* d, const int32_t* idx_dev, int B, float* out_dev, int size = 32) {
   fg_ctx* c = d->c;
-  gather_kernel<<<grid_for((int64_t)B * c->C * 1024, 256), 256, 0, c->stream>>>(d->data, idx_dev, out_dev, B, c->C, d->Cs, d->Hs,
-                                                                               d->Ws, 32, 32, d->N);
+  gather_kernel<<<grid_for((int64_t)B * c->C * size * size, 256), 256, 0, c->stream>>>(d->data, idx_dev, out_dev, B, c->C, d->Cs,
+                                                                                       d->Hs, d->Ws, size, size, d->N);
   LAUNCH_CHECK(c);
+  return FG_OK;
+}
+int gather_c2f(fg_dataset* d, const int32_t* idx_dev, int B, int cs, float* fine, float* coarse, float* diff) {
+  fg_ctx* c = d->c;
+  c2f_pairs_kernel<<<B, kPairThreads, 0, c->stream>>>(d->data, idx_dev, fine, coarse, diff, c->C, d->Cs, d->Hs, d->Ws, cs, d->N);
+  LAUNCH_CHECK(c);
+  return FG_OK;
+}
+// a host index list is range-checked and staged in d->idx; a device one is used as is (the kernels clamp it)
+int stage_indices(fg_dataset* d, const int32_t* idx, int B, const char* what, const int32_t** idx_dev) {
+  *idx_dev = idx;
+  if (is_dev(idx)) return FG_OK;
+  for (int i = 0; i < B; ++i)
+    FG_REQUIRE(idx[i] >= 0 && idx[i] < d->N, "%s: index %d out of range [0, %lld)", what, idx[i], (long long)d->N);
+  FG_CUDA(cudaMemcpyAsync(d->idx, idx, sizeof(int32_t) * B, cudaMemcpyHostToDevice, d->c->stream));
+  *idx_dev = d->idx;
   return FG_OK;
 }
 // queries [Q][D] (host or device); candidates either fp32 [N][D] (host or device) or the dataset cache.
@@ -354,23 +426,52 @@ int fg_dataset_upload(fg_dataset* d, int64_t first, int64_t count, const uint8_t
   return FG_OK;
 }
 // out [B][C][32][32] fp32 (host or device) = scale(load(image idx[b]));  idx: B int32 (host or device), 0-based
-int fg_dataset_gather(fg_dataset* d, const int32_t* idx, int B, float* out) {
+int fg_dataset_gather(fg_dataset* d, const int32_t* idx, int B, float* out) { return fg_dataset_gather_sized(d, idx, B, 32, out); }
+// the same at any square size in [1, 32] (dataset.lua setScale(size)); out [B][C][size][size]
+int fg_dataset_gather_sized(fg_dataset* d, const int32_t* idx, int B, int size, float* out) {
   ENTER(d);
   fg_ctx* c = d->c;
   FG_REQUIRE(idx && out && B >= 1 && B <= c->maxB, "fg_dataset_gather: bad arguments (B %d, max %d)", B, c->maxB);
-  const int32_t* idx_dev = idx;
-  if (!is_dev(idx)) {
-    for (int i = 0; i < B; ++i)
-      FG_REQUIRE(idx[i] >= 0 && idx[i] < d->N, "fg_dataset_gather: index %d out of range [0, %lld)", idx[i], (long long)d->N);
-    FG_CUDA(cudaMemcpyAsync(d->idx, idx, sizeof(int32_t) * B, cudaMemcpyHostToDevice, c->stream));
-    idx_dev = d->idx;
-  }
-  const size_t n = (size_t)B * c->C * 1024;
-  if (is_dev(out)) return gather(d, idx_dev, B, out);
-  FG_TRY(gather(d, idx_dev, B, c->io_dev));
+  FG_REQUIRE(size >= 1 && size <= 32, "fg_dataset_gather_sized: size %d outside [1, 32]", size);
+  const int32_t* idx_dev;
+  FG_TRY(stage_indices(d, idx, B, "fg_dataset_gather", &idx_dev));
+  const size_t n = (size_t)B * c->C * size * size;
+  if (is_dev(out)) return gather(d, idx_dev, B, out, size);
+  FG_TRY(gather(d, idx_dev, B, c->io_dev, size));
   FG_CUDA(cudaMemcpyAsync(out, c->io_dev, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
   FG_CUDA(cudaStreamSynchronize(c->stream));
   return FG_OK;
+}
+// dataset_c2f.lua:49-62 _toResult at fineSize 32 for B images: fine, coarse, diff [B][C][32][32] fp32, each host or
+// device or NULL.  Host outputs go through one temporary device buffer (this entry is not on a train step's path).
+int fg_dataset_gather_c2f(fg_dataset* d, const int32_t* idx, int B, int coarse_size, float* fine, float* coarse, float* diff) {
+  ENTER(d);
+  fg_ctx* c = d->c;
+  FG_REQUIRE(idx && B >= 1 && B <= c->maxB, "fg_dataset_gather_c2f: bad arguments (B %d, max %d)", B, c->maxB);
+  FG_REQUIRE(coarse_size >= 1 && coarse_size <= 32, "fg_dataset_gather_c2f: coarse size %d outside [1, 32]", coarse_size);
+  const int32_t* idx_dev;
+  FG_TRY(stage_indices(d, idx, B, "fg_dataset_gather_c2f", &idx_dev));
+  const size_t n = (size_t)B * c->C * 1024;
+  float* user[3] = {fine, coarse, diff};
+  float* dev[3] = {fine, coarse, diff};
+  int n_host = 0;
+  for (int k = 0; k < 3; ++k) n_host += user[k] && !is_dev(user[k]);
+  if (n_host == 0) return gather_c2f(d, idx_dev, B, coarse_size, fine, coarse, diff);
+  float* tmp = nullptr;
+  FG_CUDA(cudaMalloc((void**)&tmp, sizeof(float) * n * n_host));
+  for (int k = 0, j = 0; k < 3; ++k)
+    if (user[k] && !is_dev(user[k])) dev[k] = tmp + n * j++;
+  int rc = gather_c2f(d, idx_dev, B, coarse_size, dev[0], dev[1], dev[2]);
+  cudaError_t e = cudaSuccess;
+  for (int k = 0; k < 3 && rc == FG_OK && e == cudaSuccess; ++k)
+    if (dev[k] != user[k]) e = cudaMemcpyAsync(user[k], dev[k], n * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+  cudaFree(tmp);
+  if (rc == FG_OK && e != cudaSuccess) {
+    fg_set_error("fg_dataset_gather_c2f: %s", cudaGetErrorString(e));
+    rc = FG_ERR_CUDA;
+  }
+  return rc;
 }
 // the index stream fg_train_step_dataset uses: B draws of math.random(N)-1, counter-based (splitmix64)
 int fg_dataset_draw(fg_dataset* d, uint64_t seed, int B, int32_t* idx_out) {
@@ -477,3 +578,28 @@ int fg_train_step_dataset(fg_ctx* c, fg_dataset* d, const fg_hyper* h, int B, ui
 }
 
 }  // extern "C"
+
+// ---- batch assembly of the device-fed --scale 16 and coarse-to-fine steps (nets_s16.cu, nets_c2f.cu) ----------
+// Eager launches on the ctx stream into device buffers: no allocation, no host synchronisation.
+int dataset_check_feed(const fg_dataset* d, const fg_ctx* c, const char* what) {
+  FG_REQUIRE(d && d->c == c, "%s: the dataset belongs to another context", what);
+  FG_REQUIRE(!(d->Cs == 1 && c->C == 3), "%s: a grayscale cache cannot feed a colour context", what);
+  return FG_OK;
+}
+int dataset_draw_gather(fg_dataset* d, uint64_t seed, int B, int size, float* out_dev) {
+  fg_ctx* c = d->c;
+  draw_indices_kernel<<<(B + 127) / 128, 128, 0, c->stream>>>(d->idx, B, seed, d->N);
+  LAUNCH_CHECK(c);
+  return gather(d, d->idx, B, out_dev, size);
+}
+int dataset_draw_gather_c2f(fg_dataset* d, uint64_t seed, int B, int coarse_size, float* fine, float* coarse, float* diff) {
+  fg_ctx* c = d->c;
+  draw_indices_kernel<<<(B + 127) / 128, 128, 0, c->stream>>>(d->idx, B, seed, d->N);
+  LAUNCH_CHECK(c);
+  return gather_c2f(d, d->idx, B, coarse_size, fine, coarse, diff);
+}
+int noise_uniform_dev(fg_ctx* c, uint64_t seed, int64_t n, float* out_dev) {
+  uniform_pm1_kernel<<<grid_for(n, 256), 256, 0, c->stream>>>(out_dev, n, seed);
+  LAUNCH_CHECK(c);
+  return FG_OK;
+}

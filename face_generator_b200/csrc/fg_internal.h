@@ -355,3 +355,11 @@ int net_zero_grads(fg_ctx* c, int net);
 int net_allreduce_grads(fg_ctx* c, int net);  // flat gradient + its 8 tail scalars (one call when contiguous)
 int net_broadcast(fg_ctx* c, void* buf, size_t bytes);  // rank 0 -> all (dp.cu)
 int net_group(bool start);                                // ncclGroupStart / ncclGroupEnd
+
+// ---- dataset.cu: inputs of the device-fed --scale 16 / coarse-to-fine steps (eager launches on the ctx stream) ----
+int dataset_check_feed(const fg_dataset* d, const fg_ctx* c, const char* what);  // same ctx, compatible channels
+// out [B][C][size][size] (device) = gather at `size` of B indices drawn from stream `seed` (fg_dataset_draw)
+int dataset_draw_gather(fg_dataset* d, uint64_t seed, int B, int size, float* out_dev);
+// fine / coarse / diff [B][C][32][32] (device, any may be null) = fg_dataset_gather_c2f of B indices drawn from `seed`
+int dataset_draw_gather_c2f(fg_dataset* d, uint64_t seed, int B, int coarse_size, float* fine, float* coarse, float* diff);
+int noise_uniform_dev(fg_ctx* c, uint64_t seed, int64_t n, float* out_dev);  // fg_noise_uniform into device memory

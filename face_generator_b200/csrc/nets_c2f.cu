@@ -392,6 +392,37 @@ int train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_diff, cons
   FG_CUDA(cudaMemcpyAsync(n->hstats, n->dstats, sizeof(DeviceStats), cudaMemcpyDeviceToHost, c->stream));
   return FG_OK;
 }
+
+// train_step on device inputs: eager the first time, then a captured CUDA graph of the step (nets.cu net_graph_run);
+// the seed is read on the device
+int run_train_step(fg_c2f* n, const fg_hyper* h, int B, const float* rd, const float* cd, const float* nd, const float* cg,
+                   const float* ng, const float* md, const float* mg, uint64_t seed, fg_step_stats* stats) {
+  fg_ctx* c = n->c;
+  {
+    std::vector<uint8_t> key;
+    auto add = [&key](const void* p, size_t nb) { key.insert(key.end(), (const uint8_t*)p, (const uint8_t*)p + nb); };
+    const void* ptrs[] = {rd, cd, nd, cg, ng, md, mg, (const void*)c->stream, c->nccl_comm};
+    const int meta[3] = {c->graph_epoch, B, pack_key(c)};
+    add(meta, sizeof(meta));
+    add(h, sizeof(*h));
+    add(ptrs, sizeof(ptrs));
+    FG_TRY(net_graph_run(
+        c, n->graphs, key, seed, [&]() { return train_step(n, h, B, rd, cd, nd, cg, ng, md, mg, 0); },
+        [n]() { n->G_packed = n->D_packed = false; }, true));
+  }
+  if (stats) {
+    FG_CUDA(cudaStreamSynchronize(c->stream));
+    const DeviceStats& s = *n->hstats;
+    stats->loss_D = s.loss_D;
+    stats->loss_G = s.loss_G;
+    for (int i = 0; i < 4; ++i) stats->conf[i] = s.conf[i];
+    stats->trained_D = s.trained_D;
+    stats->t_D = s.t_D;
+    stats->t_G = s.t_G;
+    stats->acc_D = s.acc_D;
+  }
+  return FG_OK;
+}
 }  // namespace
 
 #define ENTER(n)                                         \
@@ -615,30 +646,32 @@ int fg_c2f_train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_dif
   FG_TRY(to_dev(c, noise_G, (size_t)B * 1024, n->in_e, &ng));
   if (masks_D) FG_TRY(to_dev(c, masks_D, (size_t)B * kC2fMask, n->in_m1, &md));
   if (masks_G) FG_TRY(to_dev(c, masks_G, (size_t)B * kC2fMask, n->in_m2, &mg));
-  {  // eager the first time, then a captured CUDA graph of the step (nets.cu net_graph_run); the seed is read on the device
-    std::vector<uint8_t> key;
-    auto add = [&key](const void* p, size_t nb) { key.insert(key.end(), (const uint8_t*)p, (const uint8_t*)p + nb); };
-    const void* ptrs[] = {rd, cd, nd, cg, ng, md, mg, (const void*)c->stream, c->nccl_comm};
-    const int meta[3] = {c->graph_epoch, B, pack_key(c)};
-    add(meta, sizeof(meta));
-    add(h, sizeof(*h));
-    add(ptrs, sizeof(ptrs));
-    FG_TRY(net_graph_run(
-        c, n->graphs, key, seed, [&]() { return train_step(n, h, B, rd, cd, nd, cg, ng, md, mg, 0); },
-        [n]() { n->G_packed = n->D_packed = false; }, true));
-  }
-  if (stats) {
-    FG_CUDA(cudaStreamSynchronize(c->stream));
-    const DeviceStats& s = *n->hstats;
-    stats->loss_D = s.loss_D;
-    stats->loss_G = s.loss_G;
-    for (int i = 0; i < 4; ++i) stats->conf[i] = s.conf[i];
-    stats->trained_D = s.trained_D;
-    stats->t_D = s.t_D;
-    stats->t_G = s.t_G;
-    stats->acc_D = s.acc_D;
-  }
-  return FG_OK;
+  return run_train_step(n, h, B, rd, cd, nd, cg, ng, md, mg, seed, stats);
+}
+
+// one adversarial_c2f.lua:121-187 loop body fed on the device (the draws of :124-141 and :168-174):
+//   real pairs  = gather_c2f(draw(8*seed,   B/2)) -> real_diff, cond_D rows [0, B/2)
+//   fake cond   = gather_c2f(draw(8*seed+1, B/2)) -> cond_D rows [B/2, B)
+//   G-step cond = gather_c2f(draw(8*seed+2, B))   -> cond_G
+//   noise_D = uniform(8*seed+3), noise_G = uniform(8*seed+4), dropout masks from `seed`.
+// The inputs land in the staging buffers a host-fed fg_c2f_train_step copies into, so both run the same step on the
+// same bits.
+int fg_c2f_train_step_dataset(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B, int coarse_size, uint64_t seed,
+                              fg_step_stats* stats) {
+  ENTER(n);
+  fg_ctx* c = n->c;
+  FG_TRY(dataset_check_feed(d, c, "fg_c2f_train_step_dataset"));
+  FG_REQUIRE(h && B >= 4 && B % 2 == 0 && B <= n->maxB, "fg_c2f_train_step_dataset: batch %d must be even, >= 4 and <= max_batch %d",
+             B, n->maxB);
+  FG_REQUIRE(coarse_size >= 1 && coarse_size <= 32, "fg_c2f_train_step_dataset: coarse size %d outside [1, 32]", coarse_size);
+  const int Bh = B / 2;
+  const size_t img = (size_t)n->C * 1024;
+  FG_TRY(dataset_draw_gather_c2f(d, seed * 8, Bh, coarse_size, nullptr, n->in_b, n->in_a));
+  FG_TRY(dataset_draw_gather_c2f(d, seed * 8 + 1, Bh, coarse_size, nullptr, n->in_b + Bh * img, nullptr));
+  FG_TRY(dataset_draw_gather_c2f(d, seed * 8 + 2, B, coarse_size, nullptr, n->in_d, nullptr));
+  FG_TRY(noise_uniform_dev(c, seed * 8 + 3, (int64_t)Bh * 1024, n->in_c));
+  FG_TRY(noise_uniform_dev(c, seed * 8 + 4, (int64_t)B * 1024, n->in_e));
+  return run_train_step(n, h, B, n->in_a, n->in_b, n->in_c, n->in_d, n->in_e, nullptr, nullptr, seed, stats);
 }
 
 }  // extern "C"

@@ -703,6 +703,37 @@ int train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const flo
   FG_CUDA(cudaMemcpyAsync(n->hstats, n->dstats, sizeof(DeviceStats), cudaMemcpyDeviceToHost, c->stream));
   return FG_OK;
 }
+
+// train_step on device inputs: eager the first time, then a captured CUDA graph of the step (nets.cu net_graph_run);
+// the seed is read on the device
+int run_train_step(fg_s16* n, const fg_hyper* h, int B, const float* rd, const float* nd, const float* ng, const float* md,
+                   const float* mg, uint64_t seed, fg_step_stats* stats) {
+  fg_ctx* c = n->c;
+  {
+    std::vector<uint8_t> key;
+    auto add = [&key](const void* p, size_t nb) { key.insert(key.end(), (const uint8_t*)p, (const uint8_t*)p + nb); };
+    const void* ptrs[] = {rd, nd, ng, md, mg, (const void*)c->stream, c->nccl_comm};
+    const int meta[3] = {c->graph_epoch, B, pack_key(c)};
+    add(meta, sizeof(meta));
+    add(h, sizeof(*h));
+    add(ptrs, sizeof(ptrs));
+    FG_TRY(net_graph_run(
+        c, n->graphs, key, seed, [&]() { return train_step(n, h, B, rd, nd, ng, md, mg, 0); },
+        [n]() { n->G_packed = n->D_packed = false; }, true));
+  }
+  if (stats) {
+    FG_CUDA(cudaStreamSynchronize(c->stream));
+    const DeviceStats& s = *n->hstats;
+    stats->loss_D = s.loss_D;
+    stats->loss_G = s.loss_G;
+    for (int i = 0; i < 4; ++i) stats->conf[i] = s.conf[i];
+    stats->trained_D = s.trained_D;
+    stats->t_D = s.t_D;
+    stats->t_G = s.t_G;
+    stats->acc_D = s.acc_D;
+  }
+  return FG_OK;
+}
 }  // namespace
 
 #define ENTER(n)                                         \
@@ -914,30 +945,22 @@ int fg_s16_train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, co
   FG_TRY(fg_to_dev(c, noise_G, (size_t)B * 100, n->in_c, &ng));
   if (masks_D) FG_TRY(fg_to_dev(c, masks_D, (size_t)B * kS16Mask, n->in_m1, &md));
   if (masks_G) FG_TRY(fg_to_dev(c, masks_G, (size_t)B * kS16Mask, n->in_m2, &mg));
-  {  // eager the first time, then a captured CUDA graph of the step (nets.cu net_graph_run); the seed is read on the device
-    std::vector<uint8_t> key;
-    auto add = [&key](const void* p, size_t nb) { key.insert(key.end(), (const uint8_t*)p, (const uint8_t*)p + nb); };
-    const void* ptrs[] = {rd, nd, ng, md, mg, (const void*)c->stream, c->nccl_comm};
-    const int meta[3] = {c->graph_epoch, B, pack_key(c)};
-    add(meta, sizeof(meta));
-    add(h, sizeof(*h));
-    add(ptrs, sizeof(ptrs));
-    FG_TRY(net_graph_run(
-        c, n->graphs, key, seed, [&]() { return train_step(n, h, B, rd, nd, ng, md, mg, 0); },
-        [n]() { n->G_packed = n->D_packed = false; }, true));
-  }
-  if (stats) {
-    FG_CUDA(cudaStreamSynchronize(c->stream));
-    const DeviceStats& s = *n->hstats;
-    stats->loss_D = s.loss_D;
-    stats->loss_G = s.loss_G;
-    for (int i = 0; i < 4; ++i) stats->conf[i] = s.conf[i];
-    stats->trained_D = s.trained_D;
-    stats->t_D = s.t_D;
-    stats->t_G = s.t_G;
-    stats->acc_D = s.acc_D;
-  }
-  return FG_OK;
+  return run_train_step(n, h, B, rd, nd, ng, md, mg, seed, stats);
+}
+
+// train.lua --scale 16 fed on the device: real = gather at 16x16 of draw(4*seed, B/2), noise_D = uniform(4*seed+1),
+// noise_G = uniform(4*seed+2), dropout masks from `seed` (the streams of fg_train_step_dataset).  The inputs land in
+// the staging buffers a host-fed fg_s16_train_step copies into, so both run the same step on the same bits.
+int fg_s16_train_step_dataset(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B, uint64_t seed, fg_step_stats* stats) {
+  ENTER(n);
+  fg_ctx* c = n->c;
+  FG_TRY(dataset_check_feed(d, c, "fg_s16_train_step_dataset"));
+  FG_REQUIRE(h && B >= 4 && B % 2 == 0 && B <= n->maxB, "fg_s16_train_step_dataset: batch %d must be even, >= 4 and <= max_batch %d",
+             B, n->maxB);
+  FG_TRY(dataset_draw_gather(d, seed * 4, B / 2, kSide, n->in_a));
+  FG_TRY(noise_uniform_dev(c, seed * 4 + 1, (int64_t)(B / 2) * 100, n->in_b));
+  FG_TRY(noise_uniform_dev(c, seed * 4 + 2, (int64_t)B * 100, n->in_c));
+  return run_train_step(n, h, B, n->in_a, n->in_b, n->in_c, nullptr, nullptr, seed, stats);
 }
 
 }  // extern "C"

@@ -3,7 +3,11 @@
 
     ds = DeviceDataset(ctx, images_u8)            # [N][Cs][Hs][Ws] uint8, e.g. the 64x64 faces of dataset.lua:10
     real = ds.gather(indices)                     # == image.scale(image.load(...), 32, 32) for those images
+    real16 = ds.gather(indices, 16)               # the same at 16x16 (train.lua --scale 16)
+    fine, coarse, diff = ds.gather_c2f(indices, 16)   # dataset_c2f.lua _toResult (train_c2f.lua --coarseSize 16)
     stats = ds.train_step(hyper, B, seed)         # adversarial.lua loop body with no host->device traffic
+    S16(ctx).train_step_dataset(ds, hyper, B, seed)            # the same for the --scale 16 nets
+    C2f(ctx).train_step_dataset(ds, hyper, B, 16, seed)        # and for the coarse-to-fine nets
 """
 import ctypes as C
 
@@ -40,12 +44,22 @@ class DeviceDataset:
     def size(self):
         return int(self.lib.fg_dataset_size(self.h))
 
-    def gather(self, indices):
+    def gather(self, indices, size=32):
+        """image.scale(image.load(...), size, size) of those images (dataset.lua setScale(size)), [B][C][size][size]."""
         idx = np.ascontiguousarray(indices, np.int32)
-        out = np.empty((idx.size, self.ctx.C, 32, 32), np.float32)
-        _check(self.lib.fg_dataset_gather(self.h, idx.ctypes.data_as(C.c_void_p), idx.size, out.ctypes.data_as(C.c_void_p)),
-               "fg_dataset_gather")
+        out = np.empty((idx.size, self.ctx.C, size, size), np.float32)
+        _check(self.lib.fg_dataset_gather_sized(self.h, idx.ctypes.data_as(C.c_void_p), idx.size, size,
+                                                out.ctypes.data_as(C.c_void_p)), "fg_dataset_gather_sized")
         return out
+
+    def gather_c2f(self, indices, coarse_size):
+        """dataset_c2f.lua _toResult of those images at fineSize 32: (fine, coarse, diff), each [B][C][32][32]."""
+        idx = np.ascontiguousarray(indices, np.int32)
+        fine, coarse, diff = (np.empty((idx.size, self.ctx.C, 32, 32), np.float32) for _ in range(3))
+        _check(self.lib.fg_dataset_gather_c2f(self.h, idx.ctypes.data_as(C.c_void_p), idx.size, coarse_size,
+                                              fine.ctypes.data_as(C.c_void_p), coarse.ctypes.data_as(C.c_void_p),
+                                              diff.ctypes.data_as(C.c_void_p)), "fg_dataset_gather_c2f")
+        return fine, coarse, diff
 
     def draw(self, seed, B):
         idx = np.empty(B, np.int32)

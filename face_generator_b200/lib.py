@@ -113,6 +113,10 @@ SYMBOLS = {
     "fg_dataset_draw": (_I, [_P, _U64, _I, _P]),
     "fg_noise_uniform": (_I, [_P, _U64, _L, _P]),
     "fg_train_step_dataset": (_I, [_P, _P, C.POINTER(Hyper), _I, _U64, C.POINTER(StepStats)]),
+    "fg_dataset_gather_sized": (_I, [_P, _P, _I, _I, _P]),
+    "fg_dataset_gather_c2f": (_I, [_P, _P, _I, _I, _P, _P, _P]),
+    "fg_s16_train_step_dataset": (_I, [_P, _P, C.POINTER(Hyper), _I, _U64, C.POINTER(StepStats)]),
+    "fg_c2f_train_step_dataset": (_I, [_P, _P, C.POINTER(Hyper), _I, _I, _U64, C.POINTER(StepStats)]),
     "fg_D_score": (_I, [_P, _P, _L, _I, _I, _U64, _P]),
     "fg_nearest": (_I, [_P, _P, _I, _P, _L, _I, _P, _P]),
     "fg_dataset_nearest": (_I, [_P, _P, _I, _P, _P]),
@@ -639,6 +643,16 @@ class C2f:
             return None
         return dict(loss_D=st.loss_D, loss_G=st.loss_G, conf=list(st.conf), t_D=st.t_D, t_G=st.t_G, acc_D=st.acc_D)
 
+    def train_step_dataset(self, dataset, hyper, B, coarse_size, seed, want_stats=True):
+        """train_step with the pairs, conditions and noise drawn on the device from a DeviceDataset of this ctx
+        (fg_c2f_train_step_dataset); coarse_size = train_c2f.lua --coarseSize."""
+        st = StepStats() if want_stats else None
+        _check(self.lib.fg_c2f_train_step_dataset(self.h, dataset.h, C.byref(hyper), B, coarse_size, seed,
+                                                  C.byref(st) if st is not None else None), "fg_c2f_train_step_dataset")
+        if st is None:
+            return None
+        return dict(loss_D=st.loss_D, loss_G=st.loss_G, conf=list(st.conf), t_D=st.t_D, t_G=st.t_G, acc_D=st.acc_D)
+
 
 S16_MASK_PER_SAMPLE = 1024 + 128
 
@@ -746,6 +760,17 @@ class S16:
         st = StepStats() if want_stats else None
         _check(self.lib.fg_s16_train_step(self.h, C.byref(hyper), B, _ptr(real), _ptr(noise_D), _ptr(noise_G), _ptr(masks_D),
                                           _ptr(masks_G), seed, C.byref(st) if st is not None else None), "fg_s16_train_step")
+        if st is None:
+            return None
+        return dict(loss_D=st.loss_D, loss_G=st.loss_G, conf=list(st.conf), trained_D=st.trained_D, t_D=st.t_D, t_G=st.t_G,
+                    acc_D=st.acc_D)
+
+    def train_step_dataset(self, dataset, hyper, B, seed, want_stats=True):
+        """train_step with the 16x16 real half and the noise drawn on the device from a DeviceDataset of this ctx
+        (fg_s16_train_step_dataset)."""
+        st = StepStats() if want_stats else None
+        _check(self.lib.fg_s16_train_step_dataset(self.h, dataset.h, C.byref(hyper), B, seed,
+                                                  C.byref(st) if st is not None else None), "fg_s16_train_step_dataset")
         if st is None:
             return None
         return dict(loss_D=st.loss_D, loss_G=st.loss_G, conf=list(st.conf), trained_D=st.trained_D, t_D=st.t_D, t_G=st.t_G,

@@ -99,6 +99,8 @@ int fg_dataset_gather(fg_dataset* d, const int32_t* idx, int B, float* out);
 int fg_dataset_draw(fg_dataset* d, uint64_t seed, int B, int32_t* idx_out);
 int fg_noise_uniform(fg_ctx* ctx, uint64_t seed, int64_t n, float* out);
 int fg_train_step_dataset(fg_ctx* ctx, fg_dataset* d, const fg_hyper* h, int B, uint64_t seed, fg_step_stats* stats);
+int fg_dataset_gather_sized(fg_dataset* d, const int32_t* idx, int B, int size, float* out);
+int fg_dataset_gather_c2f(fg_dataset* d, const int32_t* idx, int B, int coarse_size, float* fine, float* coarse, float* diff);
 int fg_D_score(fg_ctx* ctx, const float* images, int64_t N, int chunk, int training, uint64_t seed, float* preds_out);
 int fg_nearest(fg_ctx* ctx, const float* queries, int Q, const float* cands, int64_t N, int D, int32_t* idx_out, float* dist_out);
 int fg_dataset_nearest(fg_dataset* d, const float* queries, int Q, int32_t* idx_out, float* dist_out);
@@ -146,6 +148,9 @@ int fg_s16_D_forward(fg_s16* n, const float* img, int B, int training, const flo
 int fg_s16_D_backward(fg_s16* n, const float* d_out, int want_wgrad, float* d_img);
 int fg_s16_train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const float* noise_D, const float* noise_G,
                       const float* masks_D, const float* masks_G, uint64_t seed, fg_step_stats* stats);
+int fg_s16_train_step_dataset(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B, uint64_t seed, fg_step_stats* stats);
+int fg_c2f_train_step_dataset(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B, int coarse_size, uint64_t seed,
+                              fg_step_stats* stats);
 int fg_c2f_dp_broadcast_params(fg_c2f* n);
 int fg_s16_dp_broadcast_params(fg_s16* n);
 int fg_dp_world(fg_ctx* ctx);

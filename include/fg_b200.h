@@ -304,6 +304,27 @@ int fg_noise_uniform(fg_ctx* ctx, uint64_t seed, int64_t n, float* out);
 /* fg_train_step with every input produced on the device: real = gather(draw(4*seed, B/2)),
  * noise_D = uniform(4*seed+1), noise_G = uniform(4*seed+2), dropout masks from `seed`             */
 int fg_train_step_dataset(fg_ctx* ctx, fg_dataset* d, const fg_hyper* h, int B, uint64_t seed, fg_step_stats* stats);
+/* image.scale(image.load(...), size, size) (dataset.lua with setScale(size)) for B indices:
+ * out [B][C][size][size], 1 <= size <= 32; size 32 is fg_dataset_gather                           */
+int fg_dataset_gather_sized(fg_dataset* d, const int32_t* idx, int B, int size, float* out);
+/* dataset_c2f.lua:49-62 _toResult for B indices at fineSize 32: fine = fg_dataset_gather(idx),
+ * coarse = scale(scale(fine, cs, cs), 32, 32), diff = fine - coarse; [B][C][32][32] each, host or
+ * device, any may be NULL; 1 <= coarse_size (train_c2f.lua --coarseSize) <= 32                     */
+int fg_dataset_gather_c2f(fg_dataset* d, const int32_t* idx, int B, int coarse_size, float* fine, float* coarse,
+                          float* diff);
+/* fg_s16_train_step (train.lua --scale 16) with every input produced on the device:
+ * real = gather_sized(draw(4*seed, B/2), 16), noise_D = uniform(4*seed+1), noise_G = uniform(4*seed+2),
+ * dropout masks from `seed` (the streams of fg_train_step_dataset).  d must belong to n's ctx.     */
+int fg_s16_train_step_dataset(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B, uint64_t seed, fg_step_stats* stats);
+/* fg_c2f_train_step (one adversarial_c2f.lua:121-187 loop body) with every input produced on the device
+ * (the draws of adversarial_c2f.lua:124-141 and :168-174):
+ *   real pairs  = gather_c2f(draw(8*seed,   B/2)) -> real_diff, cond_D rows [0, B/2)
+ *   fake cond   = gather_c2f(draw(8*seed+1, B/2)) -> cond_D rows [B/2, B)
+ *   G-step cond = gather_c2f(draw(8*seed+2, B))   -> cond_G
+ *   noise_D = uniform(8*seed+3, B/2*1024), noise_G = uniform(8*seed+4, B*1024), dropout masks from `seed`.
+ * coarse_size = train_c2f.lua --coarseSize (1..32).  d must belong to n's ctx.                        */
+int fg_c2f_train_step_dataset(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B, int coarse_size, uint64_t seed,
+                              fg_step_stats* stats);
 
 /* ---- scoring helpers of the sampler / the c2f trainer ------------------------------------------ */
 /* device part of NN_UTILS.sortImagesByPrediction (utils/nn_utils.lua:90-98; sample.lua:84-85):

@@ -31,6 +31,10 @@ for C, B, impl in ((3, 12, 2), (1, 6, 0)):  # ragged batches on purpose (not mul
     ds = DeviceDataset(ctx, rng.integers(0, 256, (33, 3, 50, 45), dtype=np.uint8))
     ds.gather(ds.draw(6, 7))
     ds.train_step(hyper, B, 7)
+    for size in (16, 20, 1):
+        ds.gather(ds.draw(8, 5), size)
+    for cs in (16, 12, 1, 32):
+        ds.gather_c2f(ds.draw(9, 5), cs)
     S.find_closest_neighbours(ds, imgs[:3])
     S.nearest(ctx, rng.random((3, 100)).astype(np.float32), rng.random((20, 100)).astype(np.float32))
     x = rng.standard_normal((3, 5, 8, 8)).astype(np.float32)
@@ -49,6 +53,9 @@ for C, B, impl in ((3, 12, 2), (1, 6, 0)):  # ragged batches on purpose (not mul
                         rng.uniform(-1, 1, (B // 2, 1, 32, 32)).astype(np.float32), cg,
                         rng.uniform(-1, 1, (B, 1, 32, 32)).astype(np.float32), None, None, 9)
     assert np.isfinite(st["loss_D"]) and np.isfinite(st["loss_G"])
+    for i, cs in enumerate((16, 8, 16)):  # device-fed: eager, captured, replayed
+        st = net.train_step_dataset(ds, fg.hyper_default(D_L1=1e-7, D_L2=0.0), B, cs, 40 + i)
+        assert np.isfinite(st["loss_D"]) and np.isfinite(st["loss_G"])
     S.approx_parzen(net, diff[:2] + cr[:2], cr[:2], 5, rng)
     net.close()
     # the --scale 16 nets, three identical calls: eager, captured, replayed
@@ -59,6 +66,8 @@ for C, B, impl in ((3, 12, 2), (1, 6, 0)):  # ragged batches on purpose (not mul
     zD, zG = rng.uniform(-1, 1, (B // 2, 100)).astype(np.float32), rng.uniform(-1, 1, (B, 100)).astype(np.float32)
     for i in range(3):
         st = s16.train_step(fg.hyper_default(), B, r16, zD, zG, None, None, 20 + i)
+        assert np.isfinite(st["loss_D"]) and np.isfinite(st["loss_G"])
+        st = s16.train_step_dataset(ds, fg.hyper_default(), B, 50 + i)
         assert np.isfinite(st["loss_D"]) and np.isfinite(st["loss_G"])
     s16.close()
     # the 32x32 step through eager / capture / replay, on both operand splits
