@@ -24,8 +24,7 @@ void fg_set_error(const char* fmt, ...) {
     FG_CUDA(cudaSetDevice((c)->device));              \
   } while (0)
 
-namespace {
-bool is_device_ptr(const void* p) {
+bool fg_is_dev(const void* p) {
   cudaPointerAttributes a;
   if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
     cudaGetLastError();
@@ -33,9 +32,8 @@ bool is_device_ptr(const void* p) {
   }
   return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
-// returns a device pointer holding n floats of `p` (p itself when already on the device)
-int to_dev(fg_ctx* c, const float* p, size_t n, float* staging, const float** out) {
-  if (is_device_ptr(p)) {
+int fg_to_dev(fg_ctx* c, const float* p, size_t n, float* staging, const float** out) {
+  if (fg_is_dev(p)) {
     *out = p;
     return FG_OK;
   }
@@ -43,16 +41,14 @@ int to_dev(fg_ctx* c, const float* p, size_t n, float* staging, const float** ou
   *out = staging;
   return FG_OK;
 }
-// copy n floats from a device buffer to a user pointer (host => synchronise so it is valid on return)
-int to_user(fg_ctx* c, float* dst, const float* src_dev, size_t n) {
+int fg_to_user(fg_ctx* c, float* dst, const float* src_dev, size_t n) {
   if (dst == src_dev) return FG_OK;
-  const bool dev = is_device_ptr(dst);
+  const bool dev = fg_is_dev(dst);
   FG_CUDA(cudaMemcpyAsync(dst, src_dev, n * sizeof(float), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
                           c->stream));
   if (!dev) FG_CUDA(cudaStreamSynchronize(c->stream));
   return FG_OK;
 }
-}  // namespace
 
 extern "C" {
 
@@ -115,7 +111,6 @@ int fg_destroy(fg_ctx* c) {
   if (!c) return FG_OK;
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
-  net_graphs_clear(c);
   if (c->comm_stream) {
     cudaStreamSynchronize(c->comm_stream);
     cudaStreamDestroy(c->comm_stream);
@@ -159,11 +154,11 @@ int fg_set_option(fg_ctx* c, const char* key, int64_t v) {
   if (!strcmp(key, "conv_impl")) {
     FG_REQUIRE(v >= 0 && v <= 2, "conv_impl must be 0 (simt), 1 (tc dense) or 2 (tc collapsed)");
     c->conv_impl = (int)v;
-    c->G_packed = c->D_packed = false;
+    c->net.G_packed = c->net.D_packed = false;
     return FG_OK;
   }
   if (!strcmp(key, "params_dirty")) {
-    c->G_packed = c->D_packed = false;
+    c->net.G_packed = c->net.D_packed = false;
     return FG_OK;
   }
   if (!strcmp(key, "edge_impl")) {  // 1 (default): k_conv_edge.cu for the 3-channel-side convolutions; 0: k_conv_small.cu
@@ -176,7 +171,7 @@ int fg_set_option(fg_ctx* c, const char* key, int64_t v) {
   }
   if (!strcmp(key, "mma_f16")) {  // 1: K-major tensor-core kernels (forward, dgrad) use the 3xFP16 split + f16 MMAs
     c->mma_f16 = v != 0;
-    c->G_packed = c->D_packed = false;
+    c->net.G_packed = c->net.D_packed = false;
     return FG_OK;
   }
   if (!strcmp(key, "use_graph")) {  // 1 (default): fg_train_step replays a captured CUDA graph of the step
@@ -231,41 +226,25 @@ int64_t fg_param_count(int net, int channels) {
   if (channels != 1 && channels != 3) return -1;
   return net == FG_NET_G ? make_g_layout(channels).total : net == FG_NET_D ? make_d_layout(channels).total : -1;
 }
-static int net_bufs(fg_ctx* c, int net, float** p, float** g, float** m, float** v, int64_t* n) {
-  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
-  const bool d = net == FG_NET_D;
-  if (p) *p = d ? c->PD : c->PG;
-  if (g) *g = d ? c->gD : c->gG;
-  if (m) *m = d ? c->mD : c->mG;
-  if (v) *v = d ? c->vD : c->vG;
-  if (n) *n = d ? c->dl.total : c->gl.total;
-  return FG_OK;
-}
 int fg_set_params(fg_ctx* c, int net, const float* src) {
   ENTER(c);
-  float* p; int64_t n;
-  FG_TRY(net_bufs(c, net, &p, nullptr, nullptr, nullptr, &n));
-  FG_CUDA(cudaMemcpyAsync(p, src, n * sizeof(float), cudaMemcpyDefault, c->stream));
-  FG_CUDA(cudaStreamSynchronize(c->stream));
-  c->G_packed = c->D_packed = false;
-  return FG_OK;
+  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
+  return pair_set_params(c, c->net, net, src);
 }
 int fg_get_params(fg_ctx* c, int net, float* dst) {
   ENTER(c);
-  float* p; int64_t n;
-  FG_TRY(net_bufs(c, net, &p, nullptr, nullptr, nullptr, &n));
-  return to_user(c, dst, p, n);
+  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
+  return pair_get_params(c, c->net, net, dst);
 }
 int fg_get_grads(fg_ctx* c, int net, float* dst) {
   ENTER(c);
-  float* g; int64_t n;
-  FG_TRY(net_bufs(c, net, nullptr, &g, nullptr, nullptr, &n));
-  return to_user(c, dst, g, n);
+  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
+  return pair_get_grads(c, c->net, net, dst);
 }
 int fg_zero_grads(fg_ctx* c, int net) {
   ENTER(c);
   FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
-  return net_zero_grads(c, net);
+  return pair_zero_grads(c, c->net, net);
 }
 // Borrow caller-owned DEVICE buffers as the flat parameter / gradient vectors of `net` (see include/fg_b200.h).
 int fg_bind_params(fg_ctx* c, int net, float* params_dev, float* grads_dev) {
@@ -274,71 +253,53 @@ int fg_bind_params(fg_ctx* c, int net, float* params_dev, float* grads_dev) {
   FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
   for (const float* p : {params_dev, grads_dev}) {
     if (!p) continue;
-    cudaPointerAttributes a;
-    const bool dev = cudaPointerGetAttributes(&a, p) == cudaSuccess && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged);
-    if (!dev) cudaGetLastError();
-    FG_REQUIRE(dev, "fg_bind_params: buffers must be DEVICE memory (CudaTensor:data())");
+    FG_REQUIRE(fg_is_dev(p), "fg_bind_params: buffers must be DEVICE memory (CudaTensor:data())");
     FG_REQUIRE(reinterpret_cast<uintptr_t>(p) % 16 == 0, "fg_bind_params: buffers must be 16-byte aligned");
   }
   FG_CUDA(cudaStreamSynchronize(c->stream));
+  NetPair& np = c->net;
   const bool d = net == FG_NET_D;
-  (d ? c->PD : c->PG) = params_dev ? params_dev : (d ? c->ownPD : c->ownPG);
+  (d ? np.PD : np.PG) = params_dev ? params_dev : (d ? c->ownPD : c->ownPG);
   float* own_g = d ? c->ownGD : c->ownGG;
-  const int64_t n = d ? c->dl.total : c->gl.total;
-  (d ? c->gD : c->gG) = grads_dev ? grads_dev : own_g;
-  (d ? c->tailD : c->tailG) = grads_dev ? c->tail_sep + (d ? kGradTail : 0) : own_g + n;
-  c->G_packed = c->D_packed = false;
+  const int64_t n = d ? np.nD : np.nG;
+  (d ? np.gD : np.gG) = grads_dev ? grads_dev : own_g;
+  (d ? np.tailD : np.tailG) = grads_dev ? c->tail_sep + (d ? kGradTail : 0) : own_g + n;
+  np.G_packed = np.D_packed = false;
   return FG_OK;
 }
-float* fg_params_ptr(fg_ctx* c, int net) { return !c ? nullptr : net == FG_NET_D ? c->PD : net == FG_NET_G ? c->PG : nullptr; }
-float* fg_grads_ptr(fg_ctx* c, int net) { return !c ? nullptr : net == FG_NET_D ? c->gD : net == FG_NET_G ? c->gG : nullptr; }
+float* fg_params_ptr(fg_ctx* c, int net) { return !c ? nullptr : net == FG_NET_D ? c->net.PD : net == FG_NET_G ? c->net.PG : nullptr; }
+float* fg_grads_ptr(fg_ctx* c, int net) { return !c ? nullptr : net == FG_NET_D ? c->net.gD : net == FG_NET_G ? c->net.gG : nullptr; }
 
 int fg_set_adam_state(fg_ctx* c, int net, const float* m, const float* v, int t) {
   ENTER(c);
-  float *dm, *dv; int64_t n;
-  FG_TRY(net_bufs(c, net, nullptr, nullptr, &dm, &dv, &n));
-  if (m) FG_CUDA(cudaMemcpyAsync(dm, m, n * sizeof(float), cudaMemcpyDefault, c->stream));
-  if (v) FG_CUDA(cudaMemcpyAsync(dv, v, n * sizeof(float), cudaMemcpyDefault, c->stream));
-  int* tp = net == FG_NET_D ? &c->dstats->t_D : &c->dstats->t_G;
-  FG_CUDA(cudaMemcpyAsync(tp, &t, sizeof(int), cudaMemcpyHostToDevice, c->stream));
-  FG_CUDA(cudaStreamSynchronize(c->stream));
-  return FG_OK;
+  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
+  return pair_set_adam_state(c, c->net, net, m, v, t);
 }
 int fg_get_adam_state(fg_ctx* c, int net, float* m, float* v, int* t) {
   ENTER(c);
-  float *dm, *dv; int64_t n;
-  FG_TRY(net_bufs(c, net, nullptr, nullptr, &dm, &dv, &n));
-  if (m) FG_TRY(to_user(c, m, dm, n));
-  if (v) FG_TRY(to_user(c, v, dv, n));
-  if (t) {
-    const int* tp = net == FG_NET_D ? &c->dstats->t_D : &c->dstats->t_G;
-    FG_CUDA(cudaMemcpyAsync(t, tp, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    FG_CUDA(cudaStreamSynchronize(c->stream));
-  }
-  return FG_OK;
+  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
+  return pair_get_adam_state(c, c->net, net, m, v, t);
 }
 int fg_set_bn_state(fg_ctx* c, const float* src) {
   ENTER(c);
-  FG_CUDA(cudaMemcpyAsync(c->bnG, src, 768 * sizeof(float), cudaMemcpyDefault, c->stream));
-  FG_CUDA(cudaStreamSynchronize(c->stream));
-  return FG_OK;
+  return pair_set_bn_state(c, c->net, src);
 }
 int fg_get_bn_state(fg_ctx* c, float* dst) {
   ENTER(c);
-  return to_user(c, dst, c->bnG, 768);
+  return pair_get_bn_state(c, c->net, dst);
 }
 
 // ---- L-net ------------------------------------------------------------------------------------------
 int fg_G_forward(fg_ctx* c, const float* noise, int B, int training, float* images_out) {
   ENTER(c);
   FG_REQUIRE(noise && B >= 1 && B <= c->maxB, "fg_G_forward: bad arguments (B=%d, max %d)", B, c->maxB);
-  c->G_packed = false;  // parameters may have been edited through fg_params_ptr()
+  c->net.G_packed = false;  // parameters may have been edited through fg_params_ptr()
   const float* nd;
-  FG_TRY(to_dev(c, noise, (size_t)B * kNoiseDim, c->in_noiseG, &nd));
+  FG_TRY(fg_to_dev(c, noise, (size_t)B * kNoiseDim, c->in_noiseG, &nd));
   FG_TRY(net_G_forward(c, nd, B, training != 0));
   if (images_out) {
     FG_TRY(k_nhwc_to_nchw(c, c->G_y, c->io_dev, B, c->C, 1024));
-    FG_TRY(to_user(c, images_out, c->io_dev, (size_t)B * c->C * 1024));
+    FG_TRY(fg_to_user(c, images_out, c->io_dev, (size_t)B * c->C * 1024));
   }
   return FG_OK;
 }
@@ -347,22 +308,22 @@ int fg_G_backward(fg_ctx* c, const float* d_images, float* d_noise) {
   FG_REQUIRE(d_images, "fg_G_backward: d_images is null");
   const int B = c->G_B;
   const float* dd;
-  FG_TRY(to_dev(c, d_images, (size_t)B * c->C * 1024, c->io_dev, &dd));
+  FG_TRY(fg_to_dev(c, d_images, (size_t)B * c->C * 1024, c->io_dev, &dd));
   FG_TRY(k_nchw_to_nhwc(c, dd, c->io_dev2, B, c->C, 1024));
   float* dn = nullptr;
-  if (d_noise) dn = is_device_ptr(d_noise) ? d_noise : c->in_noiseD;
+  if (d_noise) dn = fg_is_dev(d_noise) ? d_noise : c->in_noiseD;
   FG_TRY(net_G_backward(c, c->io_dev2, dn));
-  if (d_noise && dn != d_noise) FG_TRY(to_user(c, d_noise, dn, (size_t)B * kNoiseDim));
+  if (d_noise && dn != d_noise) FG_TRY(fg_to_user(c, d_noise, dn, (size_t)B * kNoiseDim));
   return FG_OK;
 }
 int fg_D_forward(fg_ctx* c, const float* images, int B, int training, const float* masks, uint64_t seed, float* out) {
   ENTER(c);
   FG_REQUIRE(images && B >= 1 && B <= c->maxB, "fg_D_forward: bad arguments (B=%d, max %d)", B, c->maxB);
-  c->D_packed = false;
+  c->net.D_packed = false;
   fg_hyper h;
   fg_hyper_default(&h);
   const float* xd;
-  FG_TRY(to_dev(c, images, (size_t)B * c->C * 1024, c->io_dev, &xd));
+  FG_TRY(fg_to_dev(c, images, (size_t)B * c->C * 1024, c->io_dev, &xd));
   FG_TRY(k_nchw_to_nhwc(c, xd, c->D_x, B, c->C, 1024));
   if (training) {
     if (masks) {
@@ -373,7 +334,7 @@ int fg_D_forward(fg_ctx* c, const float* images, int B, int training, const floa
   }
   FG_TRY(net_D_forward(c, c->D_x, B, training != 0, &h));
   FG_TRY(k_sigmoid_fwd(c, c->D_logit, c->D_out, B));
-  if (out) FG_TRY(to_user(c, out, c->D_out, B));
+  if (out) FG_TRY(fg_to_user(c, out, c->D_out, B));
   return FG_OK;
 }
 int fg_D_backward(fg_ctx* c, const float* d_out, int want_wgrad, float* d_images) {
@@ -381,12 +342,12 @@ int fg_D_backward(fg_ctx* c, const float* d_out, int want_wgrad, float* d_images
   FG_REQUIRE(d_out, "fg_D_backward: d_out is null");
   const int B = c->D_B;
   const float* dd;
-  FG_TRY(to_dev(c, d_out, B, c->D_targets, &dd));
+  FG_TRY(fg_to_dev(c, d_out, B, c->D_targets, &dd));
   FG_TRY(k_sigmoid_grad_mul(c, dd, c->D_out, c->D_dlogit, B));
   FG_TRY(net_D_backward(c, c->D_dlogit, want_wgrad != 0, d_images != nullptr));
   if (d_images) {
     FG_TRY(k_nhwc_to_nchw(c, c->D_dx, c->io_dev, B, c->C, 1024));
-    FG_TRY(to_user(c, d_images, c->io_dev, (size_t)B * c->C * 1024));
+    FG_TRY(fg_to_user(c, d_images, c->io_dev, (size_t)B * c->C * 1024));
   }
   return FG_OK;
 }
@@ -394,19 +355,19 @@ int fg_bce_forward(fg_ctx* c, const float* x, const float* t, int n, float* loss
   ENTER(c);
   FG_REQUIRE(x && t && loss_out && n > 0 && n <= c->maxB, "fg_bce_forward: bad arguments");
   const float *xd, *td;
-  FG_TRY(to_dev(c, x, n, c->io_dev, &xd));
-  FG_TRY(to_dev(c, t, n, c->io_dev2, &td));
+  FG_TRY(fg_to_dev(c, x, n, c->io_dev, &xd));
+  FG_TRY(fg_to_dev(c, t, n, c->io_dev2, &td));
   FG_TRY(k_bce_fwd(c, xd, td, n, c->D_targets));
-  return to_user(c, loss_out, c->D_targets, 1);
+  return fg_to_user(c, loss_out, c->D_targets, 1);
 }
 int fg_bce_backward(fg_ctx* c, const float* x, const float* t, int n, float* dx) {
   ENTER(c);
   FG_REQUIRE(x && t && dx && n > 0 && n <= c->maxB, "fg_bce_backward: bad arguments");
   const float *xd, *td;
-  FG_TRY(to_dev(c, x, n, c->io_dev, &xd));
-  FG_TRY(to_dev(c, t, n, c->io_dev2, &td));
+  FG_TRY(fg_to_dev(c, x, n, c->io_dev, &xd));
+  FG_TRY(fg_to_dev(c, t, n, c->io_dev2, &td));
   FG_TRY(k_bce_bwd(c, xd, td, n, c->D_targets));
-  return to_user(c, dx, c->D_targets, n);
+  return fg_to_user(c, dx, c->D_targets, n);
 }
 int fg_optim_step(fg_ctx* c, int net, const fg_hyper* h, float grad_scale) {
   ENTER(c);
@@ -414,9 +375,8 @@ int fg_optim_step(fg_ctx* c, int net, const fg_hyper* h, float grad_scale) {
   // no accuracy information at this level: force the gate open by clearing the history influence
   fg_hyper hh = *h;
   hh.D_maxAcc = 2.0f;
-  float* g = net == FG_NET_D ? c->tailD : c->tailG;
-  FG_TRY(k_gate_and_prep(c, net, &hh, g, 1, 1.0f));
-  return net_optim(c, net, h, grad_scale, false);
+  FG_TRY(pair_gate(c, c->net, net, &hh, 1, 1.0f));
+  return pair_optim(c, c->net, net, h, grad_scale);
 }
 int fg_adam_step(fg_ctx* c, float* p, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2,
                  float eps, int t, float l1_grad, float l2, float clampv, float grad_scale) {
@@ -435,37 +395,26 @@ int fg_train_step(fg_ctx* c, const fg_hyper* h, int B, const float* real, const 
   FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= c->maxB, "fg_train_step: batch %d must be even, >= 4 and <= max_batch %d", B,
              c->maxB);
   const float *r, *nd, *ng, *md = nullptr, *mg = nullptr;
-  FG_TRY(to_dev(c, real, (size_t)(B / 2) * c->C * 1024, c->in_real, &r));
-  FG_TRY(to_dev(c, noise_D, (size_t)(B / 2) * kNoiseDim, c->in_noiseD, &nd));
-  FG_TRY(to_dev(c, noise_G, (size_t)B * kNoiseDim, c->in_noiseG, &ng));
-  if (masks_D) FG_TRY(to_dev(c, masks_D, (size_t)B * kMaskPerSample, c->in_masksD, &md));
-  if (masks_G) FG_TRY(to_dev(c, masks_G, (size_t)B * kMaskPerSample, c->in_masksG, &mg));
+  FG_TRY(fg_to_dev(c, real, (size_t)(B / 2) * c->C * 1024, c->in_real, &r));
+  FG_TRY(fg_to_dev(c, noise_D, (size_t)(B / 2) * kNoiseDim, c->in_noiseD, &nd));
+  FG_TRY(fg_to_dev(c, noise_G, (size_t)B * kNoiseDim, c->in_noiseG, &ng));
+  if (masks_D) FG_TRY(fg_to_dev(c, masks_D, (size_t)B * kMaskPerSample, c->in_masksD, &md));
+  if (masks_G) FG_TRY(fg_to_dev(c, masks_G, (size_t)B * kMaskPerSample, c->in_masksG, &mg));
   FG_TRY(net_train_step(c, h, B, r, nd, ng, md, mg, seed, true));
-  if (stats) {
-    FG_CUDA(cudaStreamSynchronize(c->stream));
-    const DeviceStats& s = *c->hstats;
-    stats->loss_D = s.loss_D;
-    stats->loss_G = s.loss_G;
-    for (int i = 0; i < 4; ++i) stats->conf[i] = s.conf[i];
-    stats->trained_D = s.trained_D;
-    stats->t_D = s.t_D;
-    stats->t_G = s.t_G;
-    stats->acc_D = s.acc_D;
-  }
-  return FG_OK;
+  return pair_step_stats(c, c->net, stats);
 }
 
 int fg_sample(fg_ctx* c, const float* noise, int N, int chunk, float* images_out) {
   ENTER(c);
   FG_REQUIRE(noise && images_out && N >= 1 && chunk >= 1 && chunk <= c->maxB, "fg_sample: bad arguments (chunk %d, max %d)",
              chunk, c->maxB);
-  const bool out_dev = is_device_ptr(images_out);
+  const bool out_dev = fg_is_dev(images_out);
   const size_t img = (size_t)c->C * 1024;
-  c->G_packed = false;
+  c->net.G_packed = false;
   for (int s = 0; s < N; s += chunk) {
     const int b = std::min(chunk, N - s);
     const float* nd;
-    FG_TRY(to_dev(c, noise + (size_t)s * kNoiseDim, (size_t)b * kNoiseDim, c->in_noiseG, &nd));
+    FG_TRY(fg_to_dev(c, noise + (size_t)s * kNoiseDim, (size_t)b * kNoiseDim, c->in_noiseG, &nd));
     // sample.lua never calls :evaluate() => BatchNorm uses the statistics of each chunk (SURVEY 3.4)
     FG_TRY(net_G_forward(c, nd, b, true));
     float* dst = images_out + (size_t)s * img;
@@ -543,7 +492,7 @@ int64_t fg_debug_tensor(fg_ctx* c, const char* name, float* dst, int64_t max_ele
       }
       if (dst) {
         if (n > max_elems) return -2;
-        if (to_user(c, dst, e.p, n) != FG_OK) return -3;
+        if (fg_to_user(c, dst, e.p, n) != FG_OK) return -3;
       }
       return n;
     }

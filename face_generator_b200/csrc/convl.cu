@@ -1,44 +1,10 @@
 // ConvL: layer-level dispatch shared by nets_c2f.cu and nets_s16.cu (see convl.h)
 #include "convl.h"
 
-#include <algorithm>
-
 #include "k_conv_tc.h"
 #include "k_misc.h"
 
-bool fg_is_dev(const void* p) {
-  cudaPointerAttributes a;
-  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-    cudaGetLastError();
-    return false;
-  }
-  return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-}
-int fg_to_dev(fg_ctx* c, const float* p, size_t n, float* staging, const float** out) {
-  if (fg_is_dev(p)) {
-    *out = p;
-    return FG_OK;
-  }
-  FG_CUDA(cudaMemcpyAsync(staging, p, n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  *out = staging;
-  return FG_OK;
-}
-int fg_to_user(fg_ctx* c, float* dst, const float* src_dev, size_t n) {
-  const bool dev = fg_is_dev(dst);
-  FG_CUDA(cudaMemcpyAsync(dst, src_dev, n * sizeof(float), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
-                          c->stream));
-  if (!dev) FG_CUDA(cudaStreamSynchronize(c->stream));
-  return FG_OK;
-}
-
-int convl_dalloc(ConvLEnv& e, float** p, size_t elems) {
-  void* q = nullptr;
-  FG_CUDA(cudaMalloc(&q, std::max<size_t>(elems, 1) * sizeof(float)));
-  FG_CUDA(cudaMemsetAsync(q, 0, std::max<size_t>(elems, 1) * sizeof(float), e.c->stream));
-  e.allocs->push_back(q);
-  *p = (float*)q;
-  return FG_OK;
-}
+int convl_dalloc(ConvLEnv& e, float** p, size_t elems) { return fg_dalloc(e.c, *e.allocs, p, elems); }
 
 namespace {
 // option "mma_f16": the hi/lo buffers of a layer hold the 3xFP16 split (halves, half of each buffer used), activations and

@@ -48,8 +48,3 @@ int convl_pack(fg_ctx* c, ConvL& L, const float* P);
 int convl_fwd(ConvLEnv& e, ConvL& L, const float* in, const float* P, float* out, int B);
 // G (may be null): dW += wgrad, db += colsum(dy).  din (may be null) = dgrad.
 int convl_bwd(ConvLEnv& e, ConvL& L, const float* in, const float* dy, float* G, float* din, int B);
-
-// host or device pointer -> device pointer (staged through `staging` when it is host memory); result -> user pointer
-bool fg_is_dev(const void* p);
-int fg_to_dev(fg_ctx* c, const float* p, size_t n, float* staging, const float** out);
-int fg_to_user(fg_ctx* c, float* dst, const float* src_dev, size_t n);

@@ -22,12 +22,6 @@
 
 #include "fg_internal.h"
 
-#define LAUNCH_CHECK(c)                 \
-  do {                                  \
-    (c)->launches++;                    \
-    FG_CUDA(cudaGetLastError());        \
-  } while (0)
-
 struct fg_dataset {
   fg_ctx* c = nullptr;
   int64_t N = 0;
@@ -37,10 +31,6 @@ struct fg_dataset {
 };
 
 namespace {
-inline int grid_for(int64_t n, int block, int cap = 132 * 16) {
-  int64_t g = (n + block - 1) / block;
-  return (int)std::max<int64_t>(1, std::min<int64_t>(g, cap));
-}
 __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
   x += 0x9E3779B97F4A7C15ull;
   x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
@@ -276,14 +266,6 @@ __global__ void nearest_unpack_kernel(const unsigned long long* __restrict__ bes
   }
 }
 
-bool is_dev(const void* p) {
-  cudaPointerAttributes a;
-  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-    cudaGetLastError();
-    return false;
-  }
-  return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-}
 int gather(fg_dataset* d, const int32_t* idx_dev, int B, float* out_dev, int size = 32) {
   fg_ctx* c = d->c;
   gather_kernel<<<grid_for((int64_t)B * c->C * size * size, 256), 256, 0, c->stream>>>(d->data, idx_dev, out_dev, B, c->C, d->Cs,
@@ -300,7 +282,7 @@ int gather_c2f(fg_dataset* d, const int32_t* idx_dev, int B, int cs, float* fine
 // a host index list is range-checked and staged in d->idx; a device one is used as is (the kernels clamp it)
 int stage_indices(fg_dataset* d, const int32_t* idx, int B, const char* what, const int32_t** idx_dev) {
   *idx_dev = idx;
-  if (is_dev(idx)) return FG_OK;
+  if (fg_is_dev(idx)) return FG_OK;
   for (int i = 0; i < B; ++i)
     FG_REQUIRE(idx[i] >= 0 && idx[i] < d->N, "%s: index %d out of range [0, %lld)", what, idx[i], (long long)d->N);
   FG_CUDA(cudaMemcpyAsync(d->idx, idx, sizeof(int32_t) * B, cudaMemcpyHostToDevice, d->c->stream));
@@ -326,13 +308,13 @@ int nearest_run(fg_ctx* c, const float* cands, const fg_dataset* d, int64_t N, i
   };
   do {
     const float* qd = queries;
-    if (!is_dev(queries)) {
+    if (!fg_is_dev(queries)) {
       if (fail(cudaMalloc((void**)&q_dev, sizeof(float) * (size_t)Q * D), "cudaMalloc")) break;
       if (fail(cudaMemcpyAsync(q_dev, queries, sizeof(float) * (size_t)Q * D, cudaMemcpyHostToDevice, c->stream), "H2D")) break;
       qd = q_dev;
     }
     const float* cd = cands;
-    if (cands && !is_dev(cands)) {
+    if (cands && !fg_is_dev(cands)) {
       if (fail(cudaMalloc((void**)&c_dev, sizeof(float) * (size_t)N * D), "cudaMalloc")) break;
       if (fail(cudaMemcpyAsync(c_dev, cands, sizeof(float) * (size_t)N * D, cudaMemcpyHostToDevice, c->stream), "H2D")) break;
       cd = c_dev;
@@ -436,7 +418,7 @@ int fg_dataset_gather_sized(fg_dataset* d, const int32_t* idx, int B, int size, 
   const int32_t* idx_dev;
   FG_TRY(stage_indices(d, idx, B, "fg_dataset_gather", &idx_dev));
   const size_t n = (size_t)B * c->C * size * size;
-  if (is_dev(out)) return gather(d, idx_dev, B, out, size);
+  if (fg_is_dev(out)) return gather(d, idx_dev, B, out, size);
   FG_TRY(gather(d, idx_dev, B, c->io_dev, size));
   FG_CUDA(cudaMemcpyAsync(out, c->io_dev, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
   FG_CUDA(cudaStreamSynchronize(c->stream));
@@ -455,12 +437,12 @@ int fg_dataset_gather_c2f(fg_dataset* d, const int32_t* idx, int B, int coarse_s
   float* user[3] = {fine, coarse, diff};
   float* dev[3] = {fine, coarse, diff};
   int n_host = 0;
-  for (int k = 0; k < 3; ++k) n_host += user[k] && !is_dev(user[k]);
+  for (int k = 0; k < 3; ++k) n_host += user[k] && !fg_is_dev(user[k]);
   if (n_host == 0) return gather_c2f(d, idx_dev, B, coarse_size, fine, coarse, diff);
   float* tmp = nullptr;
   FG_CUDA(cudaMalloc((void**)&tmp, sizeof(float) * n * n_host));
   for (int k = 0, j = 0; k < 3; ++k)
-    if (user[k] && !is_dev(user[k])) dev[k] = tmp + n * j++;
+    if (user[k] && !fg_is_dev(user[k])) dev[k] = tmp + n * j++;
   int rc = gather_c2f(d, idx_dev, B, coarse_size, dev[0], dev[1], dev[2]);
   cudaError_t e = cudaSuccess;
   for (int k = 0; k < 3 && rc == FG_OK && e == cudaSuccess; ++k)
@@ -478,7 +460,7 @@ int fg_dataset_draw(fg_dataset* d, uint64_t seed, int B, int32_t* idx_out) {
   ENTER(d);
   fg_ctx* c = d->c;
   FG_REQUIRE(idx_out && B >= 1 && B <= c->maxB, "fg_dataset_draw: bad arguments");
-  int32_t* dst = is_dev(idx_out) ? idx_out : d->idx;
+  int32_t* dst = fg_is_dev(idx_out) ? idx_out : d->idx;
   draw_indices_kernel<<<(B + 127) / 128, 128, 0, c->stream>>>(dst, B, seed, d->N);
   LAUNCH_CHECK(c);
   if (dst != idx_out) {
@@ -495,7 +477,7 @@ int fg_noise_uniform(fg_ctx* c, uint64_t seed, int64_t n, float* out) {
   }
   FG_CUDA(cudaSetDevice(c->device));
   FG_REQUIRE(out && n >= 1, "fg_noise_uniform: bad arguments");
-  if (is_dev(out)) {
+  if (fg_is_dev(out)) {
     uniform_pm1_kernel<<<grid_for(n, 256), 256, 0, c->stream>>>(out, n, seed);
     LAUNCH_CHECK(c);
     return FG_OK;
@@ -563,18 +545,7 @@ int fg_train_step_dataset(fg_ctx* c, fg_dataset* d, const fg_hyper* h, int B, ui
   uniform_pm1_kernel<<<grid_for((int64_t)B * kNoiseDim, 256), 256, 0, c->stream>>>(c->in_noiseG, (int64_t)B * kNoiseDim, seed * 4 + 2);
   LAUNCH_CHECK(c);
   FG_TRY(net_train_step(c, h, B, c->in_real, c->in_noiseD, c->in_noiseG, nullptr, nullptr, seed));
-  if (stats) {
-    FG_CUDA(cudaStreamSynchronize(c->stream));
-    const DeviceStats& s = *c->hstats;
-    stats->loss_D = s.loss_D;
-    stats->loss_G = s.loss_G;
-    for (int i = 0; i < 4; ++i) stats->conf[i] = s.conf[i];
-    stats->trained_D = s.trained_D;
-    stats->t_D = s.t_D;
-    stats->t_G = s.t_G;
-    stats->acc_D = s.acc_D;
-  }
-  return FG_OK;
+  return pair_step_stats(c, c->net, stats);
 }
 
 }  // extern "C"

@@ -97,7 +97,7 @@ int fg_dp_init(fg_ctx* c, const void* id128, int nranks, int rank) {
     return FG_ERR_INVALID;
   }
   FG_CUDA(cudaSetDevice(c->device));
-  net_graphs_clear(c);  // captured steps reference the old communicator
+  pair_clear_graphs(c->net);  // captured steps reference the old communicator
   c->graph_epoch++;
   if (c->nccl_comm) {
     g_nccl.CommDestroy((ncclComm_t)c->nccl_comm);
@@ -120,24 +120,7 @@ int fg_dp_broadcast_params(fg_ctx* c) {
   if (!c) return FG_ERR_INVALID;
   if (c->world <= 1) return FG_OK;
   FG_CUDA(cudaSetDevice(c->device));
-  // everything a replica's next step depends on: parameters, optimizer moments, BN running statistics AND the
-  // device-side step counters / accuracy history (the Adam bias correction uses t: a rank that resumed from a
-  // checkpoint at t > 0 while the others start at 0 would otherwise take a different step size and diverge)
-  FG_TRY(net_group(true));
-  const size_t nG = c->gl.total * sizeof(float), nD = c->dl.total * sizeof(float);
-  FG_TRY(net_broadcast(c, c->PG, nG));
-  FG_TRY(net_broadcast(c, c->PD, nD));
-  FG_TRY(net_broadcast(c, c->mG, nG));
-  FG_TRY(net_broadcast(c, c->vG, nG));
-  FG_TRY(net_broadcast(c, c->mD, nD));
-  FG_TRY(net_broadcast(c, c->vD, nD));
-  FG_TRY(net_broadcast(c, c->bnG, 768 * sizeof(float)));
-  FG_TRY(net_broadcast(c, c->dstats, sizeof(DeviceStats)));
-  FG_TRY(net_broadcast(c, c->acc_hist, kAccHistMax * sizeof(float)));
-  FG_TRY(net_group(false));
-  FG_CUDA(cudaStreamSynchronize(c->stream));
-  c->G_packed = c->D_packed = false;
-  return FG_OK;
+  return pair_broadcast(c, c->net);
 }
 int fg_dp_world(fg_ctx* c) { return c ? c->world : 0; }
 }

@@ -5,6 +5,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <functional>
+#include <initializer_list>
 #include <map>
 #include <string>
 #include <vector>
@@ -33,6 +34,21 @@ void fg_set_error(const char* fmt, ...);
       return FG_ERR_INVALID;          \
     }                                 \
   } while (0)
+// after every kernel launch on context c: count it and surface a launch error
+#define LAUNCH_CHECK(c)                 \
+  do {                                  \
+    (c)->launches++;                    \
+    FG_CUDA(cudaGetLastError());        \
+  } while (0)
+// grid of a grid-stride kernel over n elements: at most 16 blocks per SM of the H100's 132, at least 1
+inline int grid_for(int64_t n, int block, int cap = 132 * 16) {
+  int64_t g = (n + block - 1) / block;
+  if (g > cap) g = cap;
+  if (g < 1) g = 1;
+  return (int)g;
+}
+#define GRID_STRIDE(i, n) \
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < (n); i += (int64_t)gridDim.x * blockDim.x)
 
 constexpr int kMaskPerSample = 1984;  // 64+128+256+512 SpatialDropout + 512+512 Dropout keep flags
 constexpr int kNoiseDim = 100;
@@ -69,6 +85,30 @@ struct DeviceStats {  // lives in device memory; mirrored to fg_step_stats
   int do_train_D, do_train_G;
 };
 constexpr int kAccHistMax = 1024;
+constexpr int kBnState = 768;  // running mean / var of G's two BatchNorm layers: [mean1 256][var1 256][mean2 128][var2 128]
+
+// A captured train step (net_graph_run) and the key it was captured under
+struct StepGraph {
+  std::vector<uint8_t> key;
+  cudaGraphExec_t exec = nullptr;
+  int64_t launches = 0;
+  bool failed = false;
+};
+
+// The trainable state of one G/D pair (the 32x32 nets of fg_ctx, the coarse-to-fine nets, the --scale 16 nets)
+struct NetPair {
+  int64_t nG = 0, nD = 0;
+  float *PG = nullptr, *PD = nullptr, *gG = nullptr, *gD = nullptr;  // flat parameters and gradients
+  float *tailG = nullptr, *tailD = nullptr;  // the 8 DP-reduced scalars of each gradient: g + n, or elsewhere (fg_bind_params)
+  float *mG = nullptr, *vG = nullptr, *mD = nullptr, *vD = nullptr;  // optimizer moments
+  float* bnG = nullptr;  // [kBnState] G's BatchNorm running statistics; null when G has no BatchNorm
+  DeviceStats* dstats = nullptr;
+  DeviceStats* hstats = nullptr;  // pinned mirror
+  float* acc_hist = nullptr;      // [kAccHistMax]
+  bool G_packed = false, D_packed = false;  // the weight packs match the parameters
+  std::vector<StepGraph> graphs;
+  const char* optim_timer[2] = {nullptr, nullptr};  // ScopedTimer names of the G / D optimizer update (none: untimed)
+};
 
 struct TimerRec {
   double ms = 0;
@@ -89,23 +129,16 @@ struct fg_ctx {
   GLayout gl;
   DLayout dl;
   std::vector<void*> allocs;  // every cudaMalloc of net_alloc(), released by net_free()
-  // flat buffers (owned)
-  float *PG = nullptr, *PD = nullptr, *gG = nullptr, *gD = nullptr;
-  // the library's own allocations (PG.. point here unless fg_bind_params borrowed caller-owned buffers) and the 8
-  // DP-reduced scalars behind each gradient: contiguous with the own gradient buffer, separate for a bound one
+  NetPair net;
+  // the library's own allocations (net.PG.. point here unless fg_bind_params borrowed caller-owned buffers) and the 8
+  // DP-reduced scalars behind a bound gradient (behind the own gradient buffer they are contiguous with it)
   float *ownPG = nullptr, *ownPD = nullptr, *ownGG = nullptr, *ownGD = nullptr;
-  float *tailG = nullptr, *tailD = nullptr, *tail_sep = nullptr;
-  float *mG = nullptr, *vG = nullptr, *mD = nullptr, *vD = nullptr;
-  float* bnG = nullptr;  // [768] running stats
-  DeviceStats* dstats = nullptr;
-  float* acc_hist = nullptr;  // [kAccHistMax]
-  DeviceStats* hstats = nullptr;  // pinned mirror
+  float* tail_sep = nullptr;
   // packed weights (forward packs [tap][n][c], dgrad packs [tap'][c][n])
   float *G_L1p = nullptr, *G_L1pd = nullptr, *G_C1p = nullptr, *G_C1pd = nullptr, *G_C2p = nullptr, *G_C2pd = nullptr,
         *G_C3p = nullptr, *G_C3pd = nullptr;
   float *D_cp[4] = {nullptr, nullptr, nullptr, nullptr}, *D_cpd[4] = {nullptr, nullptr, nullptr, nullptr};
   float *D_L1p = nullptr, *D_L1pd = nullptr, *D_L2pd = nullptr, *D_L3pd = nullptr;
-  bool G_packed = false, D_packed = false;
   float* small_ws = nullptr;  // per-block partials of the small-channel wgrad (k_conv_small.cu)
   float* wgrad_ws = nullptr;  // packed weight-gradient workspace (largest layer)
   size_t wgrad_ws_elems = 0;
@@ -165,13 +198,6 @@ struct fg_ctx {
   // kernels); keyed on everything a captured step bakes in, the seed is read from device memory
   int use_graph = 1, graph_epoch = 0;
   uint64_t* seed_dev = nullptr;
-  struct StepGraph {
-    std::vector<uint8_t> key;
-    cudaGraphExec_t exec = nullptr;
-    int64_t launches = 0;
-    bool failed = false;
-  };
-  std::vector<StepGraph> graphs;
   cudaStream_t comm_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   // debug (tests): "debug_keep" = 1 keeps a copy of the D step's pre-activations of fg_train_step, which the G
@@ -216,8 +242,8 @@ struct ScopedTimer {
   fg_ctx* c;
   TimerRec* rec = nullptr;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
-  ScopedTimer(fg_ctx* c_, const char* name) : c(c_) {
-    if (c->timing) {
+  ScopedTimer(fg_ctx* c_, const char* name) : c(c_) {  // name == nullptr: not timed
+    if (c->timing && name) {
       rec = &c->timers[name];
       cudaEventCreate(&e0);
       cudaEventCreate(&e1);
@@ -292,7 +318,8 @@ int k_bce_bwd(fg_ctx* c, const float* x, const float* t, int n, float* dx);
 int k_sigmoid_grad_mul(fg_ctx* c, const float* dout, const float* out, float* dlogit, int n);
 // optimizer
 int k_penalty_loss(fg_ctx* c, const float* p, int64_t n, float l1, float l2, float* loss_inout);
-int k_gate_and_prep(fg_ctx* c, int net, const fg_hyper* h, const float* tail4, int B, float world);
+int k_gate_and_prep(fg_ctx* c, DeviceStats* st, float* acc_hist, int net, const fg_hyper* h, const float* tail4, int B,
+                    float world);
 int k_gemv_fwd(fg_ctx* c, const float* x, const float* w, const float* bias, float* out, int B, int K);
 int k_gemv_dgrad(fg_ctx* c, const float* dy, const float* w, float* dx, int B, int K);
 int k_gemv_wgrad_add(fg_ctx* c, const float* x, const float* dy, float* dw, float* db, int B, int K);
@@ -343,18 +370,46 @@ int net_G_forward(fg_ctx* c, const float* noise_dev, int B, bool training);     
 int net_G_backward(fg_ctx* c, const float* dy_nhwc, float* dnoise_dev);                      // accumulates c->gG
 int net_D_forward(fg_ctx* c, const float* x_nhwc, int B, bool training, const fg_hyper* h);  // masks in c->D_masks
 int net_D_backward(fg_ctx* c, const float* dlogit_dev, bool want_wgrad, bool want_dx);       // -> c->D_dx (NHWC)
-int net_optim(fg_ctx* c, int net, const fg_hyper* h, float grad_scale, bool gate);
-void net_graphs_clear(fg_ctx* c);
-int net_graph_run(fg_ctx* c, std::vector<fg_ctx::StepGraph>& cache, const std::vector<uint8_t>& key, uint64_t seed,
-                  const std::function<int()>& body, const std::function<void()>& repack, bool allow_graph);
 int net_train_step(fg_ctx* c, const fg_hyper* h, int B, const float* real_nchw_dev, const float* noiseD_dev,
                    const float* noiseG_dev, const float* masksD_dev, const float* masksG_dev, uint64_t seed,
                    bool allow_graph = false);
 int net_allreduce(fg_ctx* c, float* buf, int64_t n);
-int net_zero_grads(fg_ctx* c, int net);
-int net_allreduce_grads(fg_ctx* c, int net);  // flat gradient + its 8 tail scalars (one call when contiguous)
 int net_broadcast(fg_ctx* c, void* buf, size_t bytes);  // rank 0 -> all (dp.cu)
 int net_group(bool start);                                // ncclGroupStart / ncclGroupEnd
+
+// ---- netpair.cu: the lifecycle of a NetPair, on the ctx stream.  `net` is FG_NET_G or FG_NET_D (anything else: G) ----
+// zero-filled device buffer of n floats (at least one), released by whoever owns `allocs`
+int fg_dalloc(fg_ctx* c, std::vector<void*>& allocs, float** p, size_t n);
+// parameters, gradients (+ tails), moments, statistics, accuracy history and, with `bn`, BatchNorm running statistics
+// initialised as nn.SpatialBatchNormalization does (mean 0, var 1)
+int pair_alloc(fg_ctx* c, std::vector<void*>& allocs, NetPair& p, int64_t nG, int64_t nD, bool bn);
+void pair_clear_graphs(NetPair& p);
+void pair_free(NetPair& p);  // graphs and the pinned mirror; the device buffers belong to `allocs`
+int pair_zero_grads(fg_ctx* c, NetPair& p, int net);       // GRAD_PARAMETERS_x:zero() incl. the tail scalars
+int pair_allreduce_grads(fg_ctx* c, NetPair& p, int net);  // gradient + tail (one call when contiguous); world 1: nothing
+// the accuracy gate (D), t += 1 and the step size of `net` on the pair's own statistics
+int pair_gate(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, int B, float world);
+int pair_optim(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, float grad_scale);  // penalty -> clamp -> update
+int pair_broadcast(fg_ctx* c, NetPair& p);  // rank 0's parameters, moments, BatchNorm state, statistics, history
+int pair_step_stats(fg_ctx* c, const NetPair& p, fg_step_stats* stats);  // synchronise, then the last step's statistics
+int pair_set_params(fg_ctx* c, NetPair& p, int net, const float* src);
+int pair_get_params(fg_ctx* c, const NetPair& p, int net, float* dst);
+int pair_get_grads(fg_ctx* c, const NetPair& p, int net, float* dst);
+int pair_set_adam_state(fg_ctx* c, NetPair& p, int net, const float* m, const float* v, int t);
+int pair_get_adam_state(fg_ctx* c, const NetPair& p, int net, float* m, float* v, int* t);
+int pair_set_bn_state(fg_ctx* c, NetPair& p, const float* src);
+int pair_get_bn_state(fg_ctx* c, const NetPair& p, float* dst);
+// Runs `body` (launches on c->stream that read their seed from c->seed_dev) as a train step of pair p: eagerly, or as a
+// captured CUDA graph keyed on B, *h, `inputs`, the stream, the communicator, graph_epoch and pack_key
+int net_graph_run(fg_ctx* c, NetPair& p, int B, const fg_hyper* h, std::initializer_list<const void*> inputs, uint64_t seed,
+                  const std::function<int()>& body, bool allow_graph);
+
+// ---- capi.cu: host or device pointers at the C ABI ----
+bool fg_is_dev(const void* p);
+// device pointer holding n floats of p: p itself when it is device memory, else `staging` after an async copy
+int fg_to_dev(fg_ctx* c, const float* p, size_t n, float* staging, const float** out);
+// n floats from a device buffer to a user pointer (host: synchronised, so valid on return; dst == src: nothing)
+int fg_to_user(fg_ctx* c, float* dst, const float* src_dev, size_t n);
 
 // ---- dataset.cu: inputs of the device-fed --scale 16 / coarse-to-fine steps (eager launches on the ctx stream) ----
 int dataset_check_feed(const fg_dataset* d, const fg_ctx* c, const char* what);  // same ctx, compatible channels

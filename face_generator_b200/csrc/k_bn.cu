@@ -7,12 +7,6 @@
 #include "fg_internal.h"
 #include "k_ordered.cuh"
 
-#define LAUNCH_CHECK(c)                 \
-  do {                                  \
-    (c)->launches++;                    \
-    FG_CUDA(cudaGetLastError());        \
-  } while (0)
-
 namespace {
 template <bool BWD>
 __global__ void __launch_bounds__(256) bn_reduce4_kernel(const float* __restrict__ z, const float* __restrict__ dh,

@@ -21,12 +21,6 @@
 #include "fg_internal.h"
 #include "k_conv_tc.h"
 
-#define LAUNCH_CHECK(c)                 \
-  do {                                  \
-    (c)->launches++;                    \
-    FG_CUDA(cudaGetLastError());        \
-  } while (0)
-
 namespace {
 constexpr int kW = 32;  // image width these kernels are specialised for
 

@@ -11,12 +11,6 @@
 // Tiling: 256 threads as 16x16, each thread a TMxTN register tile; BK=16 staged through shared memory.
 #include "fg_internal.h"
 
-#define LAUNCH_CHECK(c)                 \
-  do {                                  \
-    (c)->launches++;                    \
-    FG_CUDA(cudaGetLastError());        \
-  } while (0)
-
 namespace {
 constexpr int BK = 16;
 

@@ -8,12 +8,6 @@
 // All tensors NHWC fp32; 3x3, stride 1, pad 1 (fully unrolled taps so the 9 loads are in flight together).
 #include "fg_internal.h"
 
-#define LAUNCH_CHECK(c)                 \
-  do {                                  \
-    (c)->launches++;                    \
-    FG_CUDA(cudaGetLastError());        \
-  } while (0)
-
 namespace {
 constexpr int kMaxSmallW = 36 * 128;  // 9 * Cs * Cb floats of weights in shared memory
 

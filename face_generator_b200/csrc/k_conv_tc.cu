@@ -435,12 +435,6 @@ constexpr size_t fwd_smem() { return (size_t)kStages * (2 * kABytes + 2 * BN * 1
 template <int BN>
 constexpr size_t wg_smem() { return (size_t)3 * (2 * 4 * 4096 + 2 * (BN / 32) * 4096) + 128 + 1024; }
 
-#define LAUNCH_CHECK(c)                 \
-  do {                                  \
-    (c)->launches++;                    \
-    FG_CUDA(cudaGetLastError());        \
-  } while (0)
-
 
 // ------------------------------------------------------------------------------------------------
 // tensor-pipe probe: the issue rate of back-to-back wgmmas (m64 x N x 8 tf32 or m64 x N x 16 f16, two warpgroups

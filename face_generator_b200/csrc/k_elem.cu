@@ -10,19 +10,6 @@
 #include "fg_internal.h"
 #include "k_ordered.cuh"
 
-#define LAUNCH_CHECK(c)                 \
-  do {                                  \
-    (c)->launches++;                    \
-    FG_CUDA(cudaGetLastError());        \
-  } while (0)
-
-static inline int grid_for(int64_t n, int block, int cap = 132 * 16) {
-  int64_t g = (n + block - 1) / block;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
 __device__ __forceinline__ int perm_idx(int j, int A, int S) {
   if (A == 0) return j;
   return (j % S) * A + (j / S);
@@ -1112,9 +1099,9 @@ __global__ void gate_prep_kernel(DeviceStats* st, float* acc_hist, int net, fg_h
     st->step_G = step_size(h, opt, h.lr_G, (double)st->t_G);
   }
 }
-int k_gate_and_prep(fg_ctx* c, int net, const fg_hyper* h, const float* tail4, int B, float world) {
-  gate_prep_kernel<<<1, 32, 0, c->stream>>>(c->dstats, c->acc_hist, net, *h, tail4, (float)B * world,
-                                            net == FG_NET_D ? c->opt_D : c->opt_G);
+int k_gate_and_prep(fg_ctx* c, DeviceStats* st, float* acc_hist, int net, const fg_hyper* h, const float* tail4, int B,
+                    float world) {
+  gate_prep_kernel<<<1, 32, 0, c->stream>>>(st, acc_hist, net, *h, tail4, (float)B * world, net == FG_NET_D ? c->opt_D : c->opt_G);
   LAUNCH_CHECK(c);
   return FG_OK;
 }

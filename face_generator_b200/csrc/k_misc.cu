@@ -9,22 +9,7 @@
 #include "k_f16split.cuh"
 #include "k_misc.h"
 
-#define LAUNCH_CHECK(c)                 \
-  do {                                  \
-    (c)->launches++;                    \
-    FG_CUDA(cudaGetLastError());        \
-  } while (0)
-
 namespace {
-inline int grid_for(int64_t n, int block, int cap = 132 * 16) {
-  int64_t g = (n + block - 1) / block;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-#define GRID_STRIDE(i, n) \
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < (n); i += (int64_t)gridDim.x * blockDim.x)
-
 // nn.JoinTable(2,2) of {noise [B][1][HW], cond [B][C][HW]} written as NHWC [B][HW][1+C]   (models_c2f.lua:116)
 __global__ void join_to_nhwc_kernel(const float* __restrict__ noise, const float* __restrict__ cond, float* __restrict__ out,
                                     int B, int C, int HW) {

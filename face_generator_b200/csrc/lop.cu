@@ -9,14 +9,6 @@
 #include "k_misc.h"
 
 namespace {
-bool is_dev(const void* p) {
-  cudaPointerAttributes a;
-  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-    cudaGetLastError();
-    return false;
-  }
-  return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-}
 int scratch(fg_ctx* c, int slot, size_t n, float** out) {
   if (c->scratch_elems[slot] < n) {
     FG_CUDA(cudaStreamSynchronize(c->stream));
@@ -31,7 +23,7 @@ int scratch(fg_ctx* c, int slot, size_t n, float** out) {
 }
 // device copy of a user tensor (slot used only for host pointers)
 int in_dev(fg_ctx* c, const float* p, size_t n, int slot, const float** out) {
-  if (is_dev(p)) {
+  if (fg_is_dev(p)) {
     *out = p;
     return FG_OK;
   }
@@ -43,7 +35,7 @@ int in_dev(fg_ctx* c, const float* p, size_t n, int slot, const float** out) {
 }
 // device buffer to produce a user output in; finish with out_done()
 int out_dev(fg_ctx* c, float* user, size_t n, int slot, float** dev, bool load) {
-  if (is_dev(user)) {
+  if (fg_is_dev(user)) {
     *dev = user;
     return FG_OK;
   }
@@ -440,7 +432,7 @@ int fg_dropout_backward(fg_ctx* c, const float* dy, const float* mask, float p, 
 }
 int fg_dropout_mask(fg_ctx* c, float* mask_dev, int64_t n, float p, uint64_t seed) {
   ENTER(c);
-  FG_REQUIRE(mask_dev && n > 0 && is_dev(mask_dev), "fg_dropout_mask: needs a device buffer");
+  FG_REQUIRE(mask_dev && n > 0 && fg_is_dev(mask_dev), "fg_dropout_mask: needs a device buffer");
   return k_bernoulli_keep(c, mask_dev, n, seed, p);
 }
 

@@ -1,0 +1,263 @@
+// The trainable state of a G/D pair (NetPair, fg_internal.h) and what every train step does with it: allocation,
+// zeroing and all-reducing the gradients, the accuracy gate and optimizer, the data-parallel broadcast, the statistics
+// mirror, the C ABI's set / get bodies and the CUDA-graph replay of the step.  Shared by the 32x32 nets (nets.cu), the
+// coarse-to-fine nets (nets_c2f.cu) and the --scale 16 nets (nets_s16.cu).
+#include <algorithm>
+#include <cstdlib>
+#include <cstring>
+
+#include "convl.h"
+#include "fg_internal.h"
+
+namespace {
+struct Half {  // one net of the pair
+  float *P, *g, *tail, *m, *v;
+  int64_t n;
+};
+Half half(const NetPair& p, int net) {
+  if (net == FG_NET_D) return Half{p.PD, p.gD, p.tailD, p.mD, p.vD, p.nD};
+  return Half{p.PG, p.gG, p.tailG, p.mG, p.vG, p.nG};
+}
+int* step_count(DeviceStats* s, int net) { return net == FG_NET_D ? &s->t_D : &s->t_G; }
+}  // namespace
+
+int fg_dalloc(fg_ctx* c, std::vector<void*>& allocs, float** p, size_t n) {
+  void* q = nullptr;
+  FG_CUDA(cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(float)));
+  FG_CUDA(cudaMemsetAsync(q, 0, std::max<size_t>(n, 1) * sizeof(float), c->stream));
+  allocs.push_back(q);
+  *p = (float*)q;
+  return FG_OK;
+}
+
+int pair_alloc(fg_ctx* c, std::vector<void*>& allocs, NetPair& p, int64_t nG, int64_t nD, bool bn) {
+  p.nG = nG;
+  p.nD = nD;
+  FG_TRY(fg_dalloc(c, allocs, &p.PG, nG));
+  FG_TRY(fg_dalloc(c, allocs, &p.PD, nD));
+  FG_TRY(fg_dalloc(c, allocs, &p.gG, nG + kGradTail));
+  FG_TRY(fg_dalloc(c, allocs, &p.gD, nD + kGradTail));
+  p.tailG = p.gG + nG;
+  p.tailD = p.gD + nD;
+  FG_TRY(fg_dalloc(c, allocs, &p.mG, nG));
+  FG_TRY(fg_dalloc(c, allocs, &p.vG, nG));
+  FG_TRY(fg_dalloc(c, allocs, &p.mD, nD));
+  FG_TRY(fg_dalloc(c, allocs, &p.vD, nD));
+  if (bn) {
+    FG_TRY(fg_dalloc(c, allocs, &p.bnG, kBnState));
+    float init[kBnState];
+    for (int i = 0; i < kBnState; ++i) init[i] = (i >= 256 && i < 512) || i >= 640 ? 1.f : 0.f;
+    FG_CUDA(cudaMemcpyAsync(p.bnG, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
+    FG_CUDA(cudaStreamSynchronize(c->stream));
+  }
+  float* tmp = nullptr;
+  FG_TRY(fg_dalloc(c, allocs, &tmp, (sizeof(DeviceStats) + 3) / 4));
+  p.dstats = (DeviceStats*)tmp;
+  FG_TRY(fg_dalloc(c, allocs, &p.acc_hist, kAccHistMax));
+  FG_CUDA(cudaMallocHost((void**)&p.hstats, sizeof(DeviceStats)));
+  memset(p.hstats, 0, sizeof(DeviceStats));
+  return FG_OK;
+}
+
+void pair_clear_graphs(NetPair& p) {
+  for (auto& g : p.graphs)
+    if (g.exec) cudaGraphExecDestroy(g.exec);
+  p.graphs.clear();
+}
+void pair_free(NetPair& p) {
+  pair_clear_graphs(p);
+  if (p.hstats) cudaFreeHost(p.hstats);
+  p.hstats = nullptr;
+}
+
+int pair_zero_grads(fg_ctx* c, NetPair& p, int net) {
+  const Half h = half(p, net);
+  if (h.tail == h.g + h.n) {
+    FG_CUDA(cudaMemsetAsync(h.g, 0, sizeof(float) * (h.n + kGradTail), c->stream));
+  } else {  // caller-owned gradient buffer (fg_bind_params): the tail lives in the library
+    FG_CUDA(cudaMemsetAsync(h.g, 0, sizeof(float) * h.n, c->stream));
+    FG_CUDA(cudaMemsetAsync(h.tail, 0, sizeof(float) * kGradTail, c->stream));
+  }
+  return FG_OK;
+}
+int pair_allreduce_grads(fg_ctx* c, NetPair& p, int net) {
+  if (c->world <= 1) return FG_OK;
+  const Half h = half(p, net);
+  if (h.tail == h.g + h.n) return net_allreduce(c, h.g, h.n + kGradTail);
+  FG_TRY(net_group(true));
+  FG_TRY(net_allreduce(c, h.g, h.n));
+  FG_TRY(net_allreduce(c, h.tail, kGradTail));
+  return net_group(false);
+}
+
+int pair_gate(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, int B, float world) {
+  return k_gate_and_prep(c, p.dstats, p.acc_hist, net, h, half(p, net).tail, B, world);
+}
+
+// penalty -> clamp -> interruptable optimizer on the flat vectors (adversarial.lua:219-231, interruptable_optimizers.lua)
+int pair_optim(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, float grad_scale) {
+  const bool isD = net == FG_NET_D;
+  const Half x = half(p, net);
+  DeviceStats* s = p.dstats;
+  const float l1 = isD ? h->D_L1 : h->G_L1, l2 = isD ? h->D_L2 : h->G_L2;
+  const bool pen = l1 != 0.f || l2 != 0.f;
+  // G quirk: the L1 gradient term is multiplied by G_L2 (adversarial.lua:223, adversarial_c2f.lua:108)
+  const float l1_grad = !pen ? 0.f : (isD ? l1 : l2);
+  if (pen) FG_TRY(k_penalty_loss(c, x.P, x.n, l1, l2, isD ? &s->loss_D : &s->loss_G));
+  ScopedTimer tm(c, p.optim_timer[isD]);
+  FG_TRY(k_optim_update(c, isD ? c->opt_D : c->opt_G, x.P, x.g, x.m, x.v, x.n, h->beta1, h->beta2, h->eps,
+                        isD ? c->sgd_mom_D : c->sgd_mom_G, l1_grad, pen ? l2 : 0.f, isD ? h->D_clamp : h->G_clamp, grad_scale,
+                        isD ? &s->step_D : &s->step_G, isD ? &s->do_train_D : &s->do_train_G, step_count(s, net)));
+  (isD ? p.D_packed : p.G_packed) = false;
+  return FG_OK;
+}
+
+// everything a replica's next step depends on: parameters, optimizer moments, BN running statistics AND the device-side
+// step counters / accuracy history (the Adam bias correction uses t: a rank that resumed from a checkpoint at t > 0
+// while the others start at 0 would otherwise take a different step size and diverge)
+int pair_broadcast(fg_ctx* c, NetPair& p) {
+  if (c->world <= 1) return FG_OK;
+  FG_TRY(net_group(true));
+  const size_t bG = p.nG * sizeof(float), bD = p.nD * sizeof(float);
+  FG_TRY(net_broadcast(c, p.PG, bG));
+  FG_TRY(net_broadcast(c, p.PD, bD));
+  FG_TRY(net_broadcast(c, p.mG, bG));
+  FG_TRY(net_broadcast(c, p.vG, bG));
+  FG_TRY(net_broadcast(c, p.mD, bD));
+  FG_TRY(net_broadcast(c, p.vD, bD));
+  if (p.bnG) FG_TRY(net_broadcast(c, p.bnG, kBnState * sizeof(float)));
+  FG_TRY(net_broadcast(c, p.dstats, sizeof(DeviceStats)));
+  FG_TRY(net_broadcast(c, p.acc_hist, kAccHistMax * sizeof(float)));
+  FG_TRY(net_group(false));
+  FG_CUDA(cudaStreamSynchronize(c->stream));
+  p.G_packed = p.D_packed = false;
+  return FG_OK;
+}
+
+int pair_step_stats(fg_ctx* c, const NetPair& p, fg_step_stats* stats) {
+  if (!stats) return FG_OK;
+  FG_CUDA(cudaStreamSynchronize(c->stream));
+  const DeviceStats& s = *p.hstats;
+  stats->loss_D = s.loss_D;
+  stats->loss_G = s.loss_G;
+  for (int i = 0; i < 4; ++i) stats->conf[i] = s.conf[i];
+  stats->trained_D = s.trained_D;
+  stats->t_D = s.t_D;
+  stats->t_G = s.t_G;
+  stats->acc_D = s.acc_D;
+  return FG_OK;
+}
+
+// ---- bodies of the set / get entry points (host or device pointers; a set synchronises) ------------------------------
+int pair_set_params(fg_ctx* c, NetPair& p, int net, const float* src) {
+  const Half h = half(p, net);
+  FG_CUDA(cudaMemcpyAsync(h.P, src, h.n * sizeof(float), cudaMemcpyDefault, c->stream));
+  FG_CUDA(cudaStreamSynchronize(c->stream));
+  (net == FG_NET_D ? p.D_packed : p.G_packed) = false;
+  return FG_OK;
+}
+int pair_get_params(fg_ctx* c, const NetPair& p, int net, float* dst) {
+  const Half h = half(p, net);
+  return fg_to_user(c, dst, h.P, h.n);
+}
+int pair_get_grads(fg_ctx* c, const NetPair& p, int net, float* dst) {
+  const Half h = half(p, net);
+  return fg_to_user(c, dst, h.g, h.n);
+}
+int pair_set_adam_state(fg_ctx* c, NetPair& p, int net, const float* m, const float* v, int t) {
+  const Half h = half(p, net);
+  if (m) FG_CUDA(cudaMemcpyAsync(h.m, m, h.n * sizeof(float), cudaMemcpyDefault, c->stream));
+  if (v) FG_CUDA(cudaMemcpyAsync(h.v, v, h.n * sizeof(float), cudaMemcpyDefault, c->stream));
+  FG_CUDA(cudaMemcpyAsync(step_count(p.dstats, net), &t, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  FG_CUDA(cudaStreamSynchronize(c->stream));
+  return FG_OK;
+}
+int pair_get_adam_state(fg_ctx* c, const NetPair& p, int net, float* m, float* v, int* t) {
+  const Half h = half(p, net);
+  if (m) FG_TRY(fg_to_user(c, m, h.m, h.n));
+  if (v) FG_TRY(fg_to_user(c, v, h.v, h.n));
+  if (t) {
+    FG_CUDA(cudaMemcpyAsync(t, step_count(p.dstats, net), sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    FG_CUDA(cudaStreamSynchronize(c->stream));
+  }
+  return FG_OK;
+}
+int pair_set_bn_state(fg_ctx* c, NetPair& p, const float* src) {
+  FG_CUDA(cudaMemcpyAsync(p.bnG, src, kBnState * sizeof(float), cudaMemcpyDefault, c->stream));
+  FG_CUDA(cudaStreamSynchronize(c->stream));
+  return FG_OK;
+}
+int pair_get_bn_state(fg_ctx* c, const NetPair& p, float* dst) { return fg_to_user(c, dst, p.bnG, kBnState); }
+
+// ---------------------------------------------------------------------------------------------------
+// CUDA-graph replay of the step.  A step is ~200 launches of mostly short kernels; replaying a captured graph removes
+// the launch gaps (measured 4.19 -> 3.87 ms at batch 256).  A graph bakes in every kernel argument, so it is keyed on all
+// of them: batch, hyper-parameters, input pointers, stream, communicator, option epoch (which every option, stream and
+// bound-buffer change bumps) and what the weight packs depend on.  The first step with a new key runs eagerly (it also
+// performs the lazy allocations), the second is captured, later ones are replayed.
+// ---------------------------------------------------------------------------------------------------
+namespace {
+template <class T>
+void key_add(std::vector<uint8_t>& k, const T& v) {
+  const uint8_t* q = reinterpret_cast<const uint8_t*>(&v);
+  k.insert(k.end(), q, q + sizeof(T));
+}
+}  // namespace
+
+// The packs are marked stale before the capture and after every replay: the captured sequence has to contain the pack
+// kernels whatever the flags said at capture time, and a replayed optimizer step invalidates them again.
+int net_graph_run(fg_ctx* c, NetPair& p, int B, const fg_hyper* h, std::initializer_list<const void*> inputs, uint64_t seed,
+                  const std::function<int()>& body, bool allow_graph) {
+  FG_TRY(k_set_u64(c, c->seed_dev, seed));
+  static const bool env_off = getenv("FG_GRAPH") && atoi(getenv("FG_GRAPH")) == 0;
+  if (!allow_graph || !c->use_graph || env_off || c->timing || c->debug_keep) return body();
+  std::vector<uint8_t> key;
+  key_add(key, c->graph_epoch);
+  key_add(key, B);
+  key_add(key, pack_key(c));
+  key_add(key, *h);
+  for (const void* q : inputs) key_add(key, q);
+  key_add(key, (const void*)c->stream);
+  key_add(key, c->nccl_comm);
+  std::vector<StepGraph>& cache = p.graphs;
+  StepGraph* e = nullptr;
+  for (auto& g : cache)
+    if (g.key == key) e = &g;
+  if (!e) {
+    if (cache.size() >= 8) {  // oldest out
+      if (cache.front().exec) cudaGraphExecDestroy(cache.front().exec);
+      cache.erase(cache.begin());
+    }
+    cache.emplace_back();
+    cache.back().key = key;
+    return body();  // eager: warms every lazy allocation
+  }
+  if (e->failed) return body();
+  if (!e->exec) {
+    p.G_packed = p.D_packed = false;
+    const int64_t l0 = c->launches;
+    FG_CUDA(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeRelaxed));
+    const int r = body();
+    cudaGraph_t g = nullptr;
+    const cudaError_t ce = cudaStreamEndCapture(c->stream, &g);
+    cudaGraphExec_t ex = nullptr;
+    if (r == FG_OK && ce == cudaSuccess && g && cudaGraphInstantiate(&ex, g, 0) == cudaSuccess) {
+      e->exec = ex;
+      e->launches = c->launches - l0;
+      c->launches = l0;
+    } else {
+      cudaGetLastError();
+      e->failed = true;
+    }
+    if (g) cudaGraphDestroy(g);
+    FG_TRY(r);
+    if (e->failed) {  // nothing ran during the failed capture
+      FG_TRY(k_set_u64(c, c->seed_dev, seed));
+      return body();
+    }
+  }
+  FG_CUDA(cudaGraphLaunch(e->exec, c->stream));
+  c->launches += e->launches;
+  p.G_packed = p.D_packed = false;
+  return FG_OK;
+}

@@ -52,48 +52,20 @@ const int kDcin[4] = {0 /*C*/, 64, 128, 256}, kDcout[4] = {64, 128, 256, 512}, k
 const int kDmoff[4] = {0, 64, 192, 448};
 inline int dcin(const fg_ctx* c, int i) { return i == 0 ? c->C : kDcin[i]; }
 
-inline std::vector<void*>& allocs(fg_ctx* c) { return c->allocs; }  // owned by the context: no process-wide state
-
-int dalloc(fg_ctx* c, float** p, size_t n) {
-  void* q = nullptr;
-  FG_CUDA(cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(float)));
-  FG_CUDA(cudaMemsetAsync(q, 0, std::max<size_t>(n, 1) * sizeof(float), c->stream));
-  allocs(c).push_back(q);
-  *p = (float*)q;
-  return FG_OK;
-}
+int dalloc(fg_ctx* c, float** p, size_t n) { return fg_dalloc(c, c->allocs, p, n); }
 }  // namespace
 
 int net_alloc(fg_ctx* c) {
   const size_t B = c->maxB, C = c->C;
   c->gl = make_g_layout(c->C);
   c->dl = make_d_layout(c->C);
-  const size_t nG = c->gl.total, nD = c->dl.total;
-  FG_TRY(dalloc(c, &c->PG, nG));
-  FG_TRY(dalloc(c, &c->PD, nD));
-  FG_TRY(dalloc(c, &c->gG, nG + kGradTail));
-  FG_TRY(dalloc(c, &c->gD, nD + kGradTail));
-  c->ownPG = c->PG; c->ownPD = c->PD; c->ownGG = c->gG; c->ownGD = c->gD;
-  c->tailG = c->gG + nG; c->tailD = c->gD + nD;
+  NetPair& p = c->net;
+  FG_TRY(pair_alloc(c, c->allocs, p, c->gl.total, c->dl.total, true));
+  p.optim_timer[0] = "hbm.optim.G";
+  p.optim_timer[1] = "hbm.optim.D";
+  c->ownPG = p.PG; c->ownPD = p.PD; c->ownGG = p.gG; c->ownGD = p.gD;
   FG_TRY(dalloc(c, &c->tail_sep, 2 * kGradTail));
-  FG_TRY(dalloc(c, &c->mG, nG));
-  FG_TRY(dalloc(c, &c->vG, nG));
-  FG_TRY(dalloc(c, &c->mD, nD));
-  FG_TRY(dalloc(c, &c->vD, nD));
-  FG_TRY(dalloc(c, &c->bnG, 768));
-  {  // running_mean = 0, running_var = 1 (nn.SpatialBatchNormalization init)
-    std::vector<float> init(768, 0.f);
-    for (int i = 256; i < 512; ++i) init[i] = 1.f;
-    for (int i = 640; i < 768; ++i) init[i] = 1.f;
-    FG_CUDA(cudaMemcpyAsync(c->bnG, init.data(), 768 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    FG_CUDA(cudaStreamSynchronize(c->stream));
-  }
   float* tmp = nullptr;
-  FG_TRY(dalloc(c, &tmp, (sizeof(DeviceStats) + 3) / 4));
-  c->dstats = (DeviceStats*)tmp;
-  FG_TRY(dalloc(c, &c->acc_hist, kAccHistMax));
-  FG_CUDA(cudaMallocHost((void**)&c->hstats, sizeof(DeviceStats)));
-  memset(c->hstats, 0, sizeof(DeviceStats));
   FG_TRY(dalloc(c, &c->amax_slot, 64));
   {
     float* sd = nullptr;
@@ -262,27 +234,27 @@ int net_alloc(fg_ctx* c) {
 }
 
 void net_free(fg_ctx* c) {
-  for (void* p : allocs(c)) cudaFree(p);
+  pair_free(c->net);
+  for (void* p : c->allocs) cudaFree(p);
   c->allocs.clear();
-  if (c->hstats) cudaFreeHost(c->hstats);
   if (c->stage_pinned) cudaFreeHost(c->stage_pinned);
   for (int i = 0; i < 8; ++i)
     if (c->scratch[i]) cudaFree(c->scratch[i]);
 }
 
 int net_pack_G(fg_ctx* c) {
-  if (c->G_packed) return FG_OK;
+  if (c->net.G_packed) return FG_OK;
   const GLayout& L = c->gl;
-  FG_TRY(k_pack_weights(c, c->PG + L.L1W, c->G_L1p, c->G_L1pd, 8192, 100, 1, 128, 64, 0, 0));
-  FG_TRY(k_pack_weights(c, c->PG + L.L1b, c->G_L1p + 8192 * 100, nullptr, 8192, 1, 1, 128, 64, 0, 0));
+  FG_TRY(k_pack_weights(c, c->net.PG + L.L1W, c->G_L1p, c->G_L1pd, 8192, 100, 1, 128, 64, 0, 0));
+  FG_TRY(k_pack_weights(c, c->net.PG + L.L1b, c->G_L1p + 8192 * 100, nullptr, 8192, 1, 1, 128, 64, 0, 0));
   // the tap-major fp32 packs of the two 5x5 layers only feed the SIMT kernels (fallback / cross-check path)
   const bool tc_g = c->conv_impl != FG_CONV_SIMT && tc_conv_eligible(ConvGeom{c->maxB, 16, 16, 128, 256, 5, 2}) &&
                     tc_conv_eligible(ConvGeom{c->maxB, 32, 32, 256, 128, 5, 2});
   if (!tc_g) {
-    FG_TRY(k_pack_weights(c, c->PG + L.C1W, c->G_C1p, c->G_C1pd, 256, 128, 25, 0, 0, 0, 0));
-    FG_TRY(k_pack_weights(c, c->PG + L.C2W, c->G_C2p, c->G_C2pd, 128, 256, 25, 0, 0, 0, 0));
+    FG_TRY(k_pack_weights(c, c->net.PG + L.C1W, c->G_C1p, c->G_C1pd, 256, 128, 25, 0, 0, 0, 0));
+    FG_TRY(k_pack_weights(c, c->net.PG + L.C2W, c->G_C2p, c->G_C2pd, 128, 256, 25, 0, 0, 0, 0));
   }
-  FG_TRY(k_pack_weights(c, c->PG + L.C3W, c->G_C3p, c->G_C3pd, c->C, 128, 9, 0, 0, 0, 0));
+  FG_TRY(k_pack_weights(c, c->net.PG + L.C3W, c->G_C3p, c->G_C3pd, c->C, 128, 9, 0, 0, 0, 0));
   if (c->conv_impl != FG_CONV_SIMT) {
     fg_ctx::TcBufs& t = c->tcb;
     // G.L1 on the tensor cores: [8192'][100] -> [8192'][128] (pad columns stay zero), then the TF32 split
@@ -291,52 +263,52 @@ int net_pack_G(fg_ctx* c) {
     if (c->mma_f16 && c->conv_impl == FG_CONV_TC_COLLAPSED) FG_TRY(tc_split_h(c, t.G_L1pad, t.G_L1w_hh, t.G_L1w_hl, 8192 * 128));
     else FG_TRY(tc_split(c, t.G_L1pad, t.G_L1w_hi, t.G_L1w_lo, 8192 * 128));
     if (c->mma_f16 && c->conv_impl == FG_CONV_TC_COLLAPSED) {  // forward and dgrad read the FP16 split; wgrad needs no weights
-      FG_TRY(tc_pack_collapsed_h(c, c->PG + L.C1W, t.G_Wf_hh[0], t.G_Wf_hl[0], t.G_Wd_hh[0], t.G_Wd_hl[0], 256, 128));
-      FG_TRY(tc_pack_collapsed_h(c, c->PG + L.C2W, t.G_Wf_hh[1], t.G_Wf_hl[1], t.G_Wd_hh[1], t.G_Wd_hl[1], 128, 256));
+      FG_TRY(tc_pack_collapsed_h(c, c->net.PG + L.C1W, t.G_Wf_hh[0], t.G_Wf_hl[0], t.G_Wd_hh[0], t.G_Wd_hl[0], 256, 128));
+      FG_TRY(tc_pack_collapsed_h(c, c->net.PG + L.C2W, t.G_Wf_hh[1], t.G_Wf_hl[1], t.G_Wd_hh[1], t.G_Wd_hl[1], 128, 256));
     } else {
-      FG_TRY(tc_pack_collapsed(c, c->PG + L.C1W, t.G_Wf_hi[0], t.G_Wf_lo[0], t.G_Wd_hi[0], t.G_Wd_lo[0], 256, 128));
-      FG_TRY(tc_pack_collapsed(c, c->PG + L.C2W, t.G_Wf_hi[1], t.G_Wf_lo[1], t.G_Wd_hi[1], t.G_Wd_lo[1], 128, 256));
+      FG_TRY(tc_pack_collapsed(c, c->net.PG + L.C1W, t.G_Wf_hi[0], t.G_Wf_lo[0], t.G_Wd_hi[0], t.G_Wd_lo[0], 256, 128));
+      FG_TRY(tc_pack_collapsed(c, c->net.PG + L.C2W, t.G_Wf_hi[1], t.G_Wf_lo[1], t.G_Wd_hi[1], t.G_Wd_lo[1], 128, 256));
     }
     if (c->conv_impl == FG_CONV_TC_DENSE) {
-      FG_TRY(tc_pack_split(c, c->PG + L.C1W, t.G_Wx_hi[0], t.G_Wx_lo[0], nullptr, nullptr, 256, 128, 25));
-      FG_TRY(tc_pack_split(c, c->PG + L.C2W, t.G_Wx_hi[1], t.G_Wx_lo[1], nullptr, nullptr, 128, 256, 25));
+      FG_TRY(tc_pack_split(c, c->net.PG + L.C1W, t.G_Wx_hi[0], t.G_Wx_lo[0], nullptr, nullptr, 256, 128, 25));
+      FG_TRY(tc_pack_split(c, c->net.PG + L.C2W, t.G_Wx_hi[1], t.G_Wx_lo[1], nullptr, nullptr, 128, 256, 25));
     }
   }
-  c->G_packed = true;
+  c->net.G_packed = true;
   return FG_OK;
 }
 int net_pack_D(fg_ctx* c) {
-  if (c->D_packed) return FG_OK;
+  if (c->net.D_packed) return FG_OK;
   const DLayout& L = c->dl;
   for (int i = 0; i < 4; ++i) {  // c2..c4 run on the tensor cores from their own TF32 packs (below) unless conv_impl = SIMT
     const ConvGeom gf{c->maxB, kDhw[i], kDhw[i], dcin(c, i), kDcout[i], 3, 1}, gd{c->maxB, kDhw[i], kDhw[i], kDcout[i], dcin(c, i), 3, 1};
     if (i > 0 && c->conv_impl != FG_CONV_SIMT && tc_conv_eligible(gf) && tc_conv_eligible(gd)) continue;
-    FG_TRY(k_pack_weights(c, c->PD + L.cW[i], c->D_cp[i], c->D_cpd[i], kDcout[i], dcin(c, i), 9, 0, 0, 0, 0));
+    FG_TRY(k_pack_weights(c, c->net.PD + L.cW[i], c->D_cp[i], c->D_cpd[i], kDcout[i], dcin(c, i), 9, 0, 0, 0, 0));
   }
   // View(2048) flattens [512][2][2] in (c,h,w) order; ours is NHWC (h,w,c): permute the columns
-  FG_TRY(k_pack_weights(c, c->PD + L.L1W, c->D_L1p, c->D_L1pd, 512, 2048, 1, 0, 0, 512, 4));
-  FG_TRY(k_pack_weights(c, c->PD + L.L2W, nullptr, c->D_L2pd, 512, 512, 1, 0, 0, 0, 0));
+  FG_TRY(k_pack_weights(c, c->net.PD + L.L1W, c->D_L1p, c->D_L1pd, 512, 2048, 1, 0, 0, 512, 4));
+  FG_TRY(k_pack_weights(c, c->net.PD + L.L2W, nullptr, c->D_L2pd, 512, 512, 1, 0, 0, 0, 0));
   if (c->conv_impl != FG_CONV_SIMT) {
     fg_ctx::TcBufs& t = c->tcb;
     for (int i = 1; i < 4; ++i) {
       if (c->mma_f16 && c->conv_impl == FG_CONV_TC_COLLAPSED)
-        FG_TRY(tc_pack_split_h(c, c->PD + L.cW[i], t.D_Wf_hh[i], t.D_Wf_hl[i], t.D_Wd_hh[i], t.D_Wd_hl[i], kDcout[i], kDcin[i], 9));
+        FG_TRY(tc_pack_split_h(c, c->net.PD + L.cW[i], t.D_Wf_hh[i], t.D_Wf_hl[i], t.D_Wd_hh[i], t.D_Wd_hl[i], kDcout[i], kDcin[i], 9));
       else
-        FG_TRY(tc_pack_split(c, c->PD + L.cW[i], t.D_Wf_hi[i], t.D_Wf_lo[i], t.D_Wd_hi[i], t.D_Wd_lo[i], kDcout[i], kDcin[i], 9));
+        FG_TRY(tc_pack_split(c, c->net.PD + L.cW[i], t.D_Wf_hi[i], t.D_Wf_lo[i], t.D_Wd_hi[i], t.D_Wd_lo[i], kDcout[i], kDcin[i], 9));
     }
     if (c->mma_f16 && c->conv_impl == FG_CONV_TC_COLLAPSED) {
       FG_TRY(tc_split_h(c, c->D_L1p, t.D_Lw_hh[0], t.D_Lw_hl[0], 512 * 2048));
       FG_TRY(tc_split_h(c, c->D_L1pd, t.D_Lw_hh[1], t.D_Lw_hl[1], 512 * 2048));
-      FG_TRY(tc_split_h(c, c->PD + L.L2W, t.D_Lw_hh[2], t.D_Lw_hl[2], 512 * 512));
+      FG_TRY(tc_split_h(c, c->net.PD + L.L2W, t.D_Lw_hh[2], t.D_Lw_hl[2], 512 * 512));
       FG_TRY(tc_split_h(c, c->D_L2pd, t.D_Lw_hh[3], t.D_Lw_hl[3], 512 * 512));
     } else {
       FG_TRY(tc_split(c, c->D_L1p, t.D_Lw_hi[0], t.D_Lw_lo[0], 512 * 2048));
       FG_TRY(tc_split(c, c->D_L1pd, t.D_Lw_hi[1], t.D_Lw_lo[1], 512 * 2048));
-      FG_TRY(tc_split(c, c->PD + L.L2W, t.D_Lw_hi[2], t.D_Lw_lo[2], 512 * 512));
+      FG_TRY(tc_split(c, c->net.PD + L.L2W, t.D_Lw_hi[2], t.D_Lw_lo[2], 512 * 512));
       FG_TRY(tc_split(c, c->D_L2pd, t.D_Lw_hi[3], t.D_Lw_lo[3], 512 * 512));
     }
   }
-  c->D_packed = true;
+  c->net.D_packed = true;
   return FG_OK;
 }
 
@@ -501,7 +473,7 @@ int net_G_forward(fg_ctx* c, const float* noise, int B, bool training) {
   FG_REQUIRE(B >= 1 && B <= c->maxB, "G forward: batch %d out of range [1,%d]", B, c->maxB);
   FG_TRY(net_pack_G(c));
   const GLayout& L = c->gl;
-  float* P = c->PG;
+  float* P = c->net.PG;
   if (noise != c->G_noise)
     FG_CUDA(cudaMemcpyAsync(c->G_noise, noise, sizeof(float) * B * kNoiseDim, cudaMemcpyDeviceToDevice, c->stream));
   c->G_B = B;
@@ -536,13 +508,13 @@ int net_G_forward(fg_ctx* c, const float* noise, int B, bool training) {
                    ConvGeom{B, 16, 16, 128, 256, 5, 2}, &parts));
   if (training) {
     if (parts) {
-      FG_TRY(k_bn_finalize_parts(c, c->bn_parts, parts, c->bn_mean1, c->bn_istd1, c->bnG, c->bnG + 256, (int64_t)B * 256, 256));
+      FG_TRY(k_bn_finalize_parts(c, c->bn_parts, parts, c->bn_mean1, c->bn_istd1, c->net.bnG, c->net.bnG + 256, (int64_t)B * 256, 256));
     } else {
       FG_TRY(k_bn_stats(c, c->G_z1, c->bn_acc, (int64_t)B * 256, 256));
-      FG_TRY(k_bn_finalize(c, c->bn_acc, c->bn_mean1, c->bn_istd1, c->bnG, c->bnG + 256, (int64_t)B * 256, 256));
+      FG_TRY(k_bn_finalize(c, c->bn_acc, c->bn_mean1, c->bn_istd1, c->net.bnG, c->net.bnG + 256, (int64_t)B * 256, 256));
     }
   } else {
-    FG_TRY(k_bn_eval_prep(c, c->bnG, c->bnG + 256, c->bn_mean1, c->bn_istd1, 256));
+    FG_TRY(k_bn_eval_prep(c, c->net.bnG, c->net.bnG + 256, c->bn_mean1, c->bn_istd1, 256));
   }
   const ConvGeom gC2{B, 32, 32, 256, 128, 5, 2};
   const bool h1_split = training && use_tc(c, gC2) && !f16_on(c);  // TF32 tensor-core path consumes h1 only as TF32 hi/lo
@@ -559,16 +531,16 @@ int net_G_forward(fg_ctx* c, const float* noise, int B, bool training) {
   if (training) {
     if (parts) {
       ScopedTimer tm(c, "G.bn2.finalize");
-      FG_TRY(k_bn_finalize_parts(c, c->bn_parts, parts, c->bn_mean2, c->bn_istd2, c->bnG + 512, c->bnG + 640, (int64_t)B * 1024, 128));
+      FG_TRY(k_bn_finalize_parts(c, c->bn_parts, parts, c->bn_mean2, c->bn_istd2, c->net.bnG + 512, c->net.bnG + 640, (int64_t)B * 1024, 128));
     } else {
       {
         ScopedTimer tm(c, "hbm.G.bn2.stats");
         FG_TRY(k_bn_stats(c, c->G_z2, c->bn_acc, (int64_t)B * 1024, 128));
       }
-      FG_TRY(k_bn_finalize(c, c->bn_acc, c->bn_mean2, c->bn_istd2, c->bnG + 512, c->bnG + 640, (int64_t)B * 1024, 128));
+      FG_TRY(k_bn_finalize(c, c->bn_acc, c->bn_mean2, c->bn_istd2, c->net.bnG + 512, c->net.bnG + 640, (int64_t)B * 1024, 128));
     }
   } else {
-    FG_TRY(k_bn_eval_prep(c, c->bnG + 512, c->bnG + 640, c->bn_mean2, c->bn_istd2, 128));
+    FG_TRY(k_bn_eval_prep(c, c->net.bnG + 512, c->net.bnG + 640, c->bn_mean2, c->bn_istd2, 128));
   }
   {
     ScopedTimer tm(c, "hbm.G.bn2.apply");
@@ -587,7 +559,7 @@ int net_G_backward(fg_ctx* c, const float* dy, float* dnoise) {
     return FG_ERR_STATE;
   }
   const GLayout& L = c->gl;
-  float *P = c->PG, *G = c->gG;
+  float *P = c->net.PG, *G = c->net.gG;
   const int B = c->G_B, C = c->C;
   FG_TRY(amax_reset(c));
   FG_TRY(k_sigmoid_bwd(c, dy, c->G_y, c->G_dz3, (int64_t)B * 1024 * C));
@@ -651,7 +623,7 @@ int net_G_backward(fg_ctx* c, const float* dy, float* dnoise) {
     FG_CUDA(cudaMemcpy2DAsync(c->wgrad_ws, 100 * sizeof(float), t.G_L1pad, 128 * sizeof(float), 100 * sizeof(float), 8192,
                               cudaMemcpyDeviceToDevice, c->stream));
     FG_TRY(k_unpack_wgrad(c, c->wgrad_ws, G + L.L1W, 8192, 100, 1, 128, 64, 0, 0));
-    c->G_packed = false;  // G_L1pad was used as scratch: the next forward re-packs (it does anyway after the optimizer step)
+    c->net.G_packed = false;  // G_L1pad was used as scratch: the next forward re-packs (it does anyway after the optimizer step)
   } else {
     FG_TRY(conv_wgrad(c, "G.L1.wgrad", c->G_noise, c->G_dz0, ConvGeom{B, 1, 1, 100, 8192, 1, 1}, G + L.L1W, 128, 64, 0, 0));
   }
@@ -669,7 +641,7 @@ int net_D_forward(fg_ctx* c, const float* x, int B, bool training, const fg_hype
   FG_TRY(net_pack_D(c));
   FG_TRY(amax_reset(c));
   const DLayout& L = c->dl;
-  float* P = c->PD;
+  float* P = c->net.PD;
   if (x != c->D_x)
     FG_CUDA(cudaMemcpyAsync(c->D_x, x, sizeof(float) * (size_t)B * 1024 * c->C, cudaMemcpyDeviceToDevice, c->stream));
   c->D_B = B;
@@ -740,7 +712,7 @@ int net_D_backward(fg_ctx* c, const float* dlogit, bool want_wgrad, bool want_dx
     return FG_ERR_STATE;
   }
   const DLayout& L = c->dl;
-  float *P = c->PD, *G = c->gD;
+  float *P = c->net.PD, *G = c->net.gD;
   const int B = c->D_B;
   const float* masks = c->D_train ? c->D_masks : nullptr;
   const float scale = c->D_drop_scale, eval_scale = c->D_spatial_eval;
@@ -835,52 +807,6 @@ int net_D_backward(fg_ctx* c, const float* dlogit, bool want_wgrad, bool want_dx
 }
 
 // ---------------------------------------------------------------------------------------------------
-// optimizer: penalty -> clamp -> interruptableAdam, all on device
-// ---------------------------------------------------------------------------------------------------
-int net_optim(fg_ctx* c, int net, const fg_hyper* h, float grad_scale, bool gate) {
-  (void)gate;
-  const bool isD = net == FG_NET_D;
-  float *p = isD ? c->PD : c->PG, *g = isD ? c->gD : c->gG, *m = isD ? c->mD : c->mG, *v = isD ? c->vD : c->vG;
-  const int64_t n = isD ? c->dl.total : c->gl.total;
-  const float l1 = isD ? h->D_L1 : h->G_L1, l2 = isD ? h->D_L2 : h->G_L2;
-  const bool pen = l1 != 0.f || l2 != 0.f;
-  // G quirk: the L1 gradient term is multiplied by G_L2 (adversarial.lua:223)
-  const float l1_grad = !pen ? 0.f : (isD ? l1 : l2);
-  if (pen) FG_TRY(k_penalty_loss(c, p, n, l1, l2, isD ? &c->dstats->loss_D : &c->dstats->loss_G));
-  ScopedTimer tm(c, isD ? "hbm.optim.D" : "hbm.optim.G");
-  FG_TRY(k_optim_update(c, isD ? c->opt_D : c->opt_G, p, g, m, v, n, h->beta1, h->beta2, h->eps,
-                        isD ? c->sgd_mom_D : c->sgd_mom_G, l1_grad, pen ? l2 : 0.f, isD ? h->D_clamp : h->G_clamp, grad_scale,
-                        isD ? &c->dstats->step_D : &c->dstats->step_G, isD ? &c->dstats->do_train_D : &c->dstats->do_train_G,
-                        isD ? &c->dstats->t_D : &c->dstats->t_G));
-  if (isD) c->D_packed = false; else c->G_packed = false;
-  return FG_OK;
-}
-
-// GRAD_PARAMETERS_x:zero() incl. the DP tail scalars
-int net_zero_grads(fg_ctx* c, int net) {
-  const bool d = net == FG_NET_D;
-  float *g = d ? c->gD : c->gG, *tail = d ? c->tailD : c->tailG;
-  const int64_t n = d ? c->dl.total : c->gl.total;
-  if (tail == g + n) {
-    FG_CUDA(cudaMemsetAsync(g, 0, sizeof(float) * (n + kGradTail), c->stream));
-  } else {  // caller-owned gradient buffer (fg_bind_params): the tail lives in the library
-    FG_CUDA(cudaMemsetAsync(g, 0, sizeof(float) * n, c->stream));
-    FG_CUDA(cudaMemsetAsync(tail, 0, sizeof(float) * kGradTail, c->stream));
-  }
-  return FG_OK;
-}
-int net_allreduce_grads(fg_ctx* c, int net) {
-  const bool d = net == FG_NET_D;
-  float *g = d ? c->gD : c->gG, *tail = d ? c->tailD : c->tailG;
-  const int64_t n = d ? c->dl.total : c->gl.total;
-  if (tail == g + n) return net_allreduce(c, g, n + kGradTail);
-  FG_TRY(net_group(true));
-  FG_TRY(net_allreduce(c, g, n));
-  FG_TRY(net_allreduce(c, tail, kGradTail));
-  return net_group(false);
-}
-
-// ---------------------------------------------------------------------------------------------------
 // one iteration of the adversarial.lua loop body (D_iterations = G_iterations = 1)
 // ---------------------------------------------------------------------------------------------------
 // the step proper; the seed of the device-drawn dropout masks is read from c->seed_dev
@@ -900,9 +826,9 @@ static int train_step_body(fg_ctx* c, const fg_hyper* h, int B, const float* rea
                             c->stream));
   else
     FG_TRY(k_masks_generate(c, c->D_masks, B, seed * 2 + 1, h->p_spatial, h->p_drop, seed_dev));
-  FG_TRY(net_zero_grads(c, FG_NET_D));
+  FG_TRY(pair_zero_grads(c, c->net, FG_NET_D));
   FG_TRY(net_D_forward(c, c->D_x, B, true, h));
-  FG_TRY(k_sigmoid_bce(c, c->D_logit, c->D_out, c->D_dlogit, &c->dstats->loss_D, c->tailD, B, Bh));
+  FG_TRY(k_sigmoid_bce(c, c->D_logit, c->D_out, c->D_dlogit, &c->net.dstats->loss_D, c->net.tailD, B, Bh));
   if (c->debug_keep) {  // tests: the G step's D forward overwrites these
     const float* src[8] = {c->D_z[0], c->D_z[1], c->D_z[2], c->D_z[3], c->D_zl1, c->D_zl2, c->D_logit, c->D_out};
     const size_t per[8] = {65536, 32768, 16384, 8192, 512, 512, 1, 1};
@@ -927,19 +853,19 @@ static int train_step_body(fg_ctx* c, const fg_hyper* h, int B, const float* rea
     FG_CUDA(cudaStreamWaitEvent(c->comm_stream, c->ev_fork, 0));
     cudaStream_t compute = c->stream;
     c->stream = c->comm_stream;
-    int r = net_allreduce_grads(c, FG_NET_D);
-    if (r == FG_OK) r = k_gate_and_prep(c, FG_NET_D, h, c->tailD, B, world);
-    if (r == FG_OK) r = net_optim(c, FG_NET_D, h, 1.0f / world, true);
+    int r = pair_allreduce_grads(c, c->net, FG_NET_D);
+    if (r == FG_OK) r = pair_gate(c, c->net, FG_NET_D, h, B, world);
+    if (r == FG_OK) r = pair_optim(c, c->net, FG_NET_D, h, 1.0f / world);
     if (r == FG_OK && cudaEventRecord(c->ev_join, c->comm_stream) != cudaSuccess) r = FG_ERR_CUDA;
     c->stream = compute;
     FG_TRY(r);
   } else {
-    if (c->world > 1) FG_TRY(net_allreduce_grads(c, FG_NET_D));
-    FG_TRY(k_gate_and_prep(c, FG_NET_D, h, c->tailD, B, world));
-    FG_TRY(net_optim(c, FG_NET_D, h, 1.0f / world, true));
+    FG_TRY(pair_allreduce_grads(c, c->net, FG_NET_D));
+    FG_TRY(pair_gate(c, c->net, FG_NET_D, h, B, world));
+    FG_TRY(pair_optim(c, c->net, FG_NET_D, h, 1.0f / world));
   }
   // ---- G step (adversarial.lua:275-288) ----
-  FG_TRY(net_zero_grads(c, FG_NET_G));
+  FG_TRY(pair_zero_grads(c, c->net, FG_NET_G));
   {
     // while the collective is in flight the persistent convolution kernels leave a few SMs to it (FG_DP_RESERVE_SMS)
     static const int reserve = getenv("FG_DP_RESERVE_SMS") ? atoi(getenv("FG_DP_RESERVE_SMS")) : 0;
@@ -955,96 +881,20 @@ static int train_step_body(fg_ctx* c, const fg_hyper* h, int B, const float* rea
   else
     FG_TRY(k_masks_generate(c, c->D_masks, B, seed * 2 + 2, h->p_spatial, h->p_drop, seed_dev));
   FG_TRY(net_D_forward(c, c->G_y, B, true, h));
-  FG_TRY(k_sigmoid_bce(c, c->D_logit, c->D_out, c->D_dlogit, &c->dstats->loss_G, c->tailG, B, B));
+  FG_TRY(k_sigmoid_bce(c, c->D_logit, c->D_out, c->D_dlogit, &c->net.dstats->loss_G, c->net.tailG, B, B));
   FG_TRY(net_D_backward(c, c->D_dlogit, false, true));  // D's weight grads are discarded by the reference (:209 vs :92)
   FG_TRY(net_G_backward(c, c->D_dx, nullptr));
-  if (c->world > 1) FG_TRY(net_allreduce_grads(c, FG_NET_G));
-  FG_TRY(k_gate_and_prep(c, FG_NET_G, h, c->tailG, B, world));
-  FG_TRY(net_optim(c, FG_NET_G, h, 1.0f / world, false));
-  FG_CUDA(cudaMemcpyAsync(c->hstats, c->dstats, sizeof(DeviceStats), cudaMemcpyDeviceToHost, c->stream));
-  return FG_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------
-// CUDA-graph replay of the step.  A step is ~200 launches of mostly short kernels; replaying a captured graph removes
-// the launch gaps (measured 4.19 -> 3.87 ms at batch 256).  A graph bakes in every kernel argument, so it is keyed on all
-// of them: batch, hyper-parameters, input / parameter pointers, option epoch.  The first step with a new key runs
-// eagerly (it also performs the lazy allocations), the second is captured, later ones are replayed.
-// ---------------------------------------------------------------------------------------------------
-void net_graphs_clear(fg_ctx* c) {
-  for (auto& g : c->graphs)
-    if (g.exec) cudaGraphExecDestroy(g.exec);
-  c->graphs.clear();
-}
-namespace {
-template <class T>
-void key_add(std::vector<uint8_t>& k, const T& v) {
-  const uint8_t* p = reinterpret_cast<const uint8_t*>(&v);
-  k.insert(k.end(), p, p + sizeof(T));
-}
-}  // namespace
-
-// Runs `body` (a sequence of launches on c->stream that reads its seed from c->seed_dev) eagerly the first time a key
-// is seen, captures it the second time and replays the captured graph afterwards.  `repack` is called before the
-// capture and after every replay: it must mark the weight packs stale (the captured sequence has to contain the pack
-// kernels whatever the flags said at capture time, and a replayed optimizer step invalidates them again).
-int net_graph_run(fg_ctx* c, std::vector<fg_ctx::StepGraph>& cache, const std::vector<uint8_t>& key, uint64_t seed,
-                  const std::function<int()>& body, const std::function<void()>& repack, bool allow_graph) {
-  FG_TRY(k_set_u64(c, c->seed_dev, seed));
-  static const bool env_off = getenv("FG_GRAPH") && atoi(getenv("FG_GRAPH")) == 0;
-  if (!allow_graph || !c->use_graph || env_off || c->timing || c->debug_keep) return body();
-  fg_ctx::StepGraph* e = nullptr;
-  for (auto& g : cache)
-    if (g.key == key) e = &g;
-  if (!e) {
-    if (cache.size() >= 8) {  // oldest out
-      if (cache.front().exec) cudaGraphExecDestroy(cache.front().exec);
-      cache.erase(cache.begin());
-    }
-    cache.emplace_back();
-    cache.back().key = key;
-    return body();  // eager: warms every lazy allocation
-  }
-  if (e->failed) return body();
-  if (!e->exec) {
-    repack();
-    const int64_t l0 = c->launches;
-    FG_CUDA(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeRelaxed));
-    const int r = body();
-    cudaGraph_t g = nullptr;
-    const cudaError_t ce = cudaStreamEndCapture(c->stream, &g);
-    cudaGraphExec_t ex = nullptr;
-    if (r == FG_OK && ce == cudaSuccess && g && cudaGraphInstantiate(&ex, g, 0) == cudaSuccess) {
-      e->exec = ex;
-      e->launches = c->launches - l0;
-      c->launches = l0;
-    } else {
-      cudaGetLastError();
-      e->failed = true;
-    }
-    if (g) cudaGraphDestroy(g);
-    FG_TRY(r);
-    if (e->failed) {  // nothing ran during the failed capture
-      FG_TRY(k_set_u64(c, c->seed_dev, seed));
-      return body();
-    }
-  }
-  FG_CUDA(cudaGraphLaunch(e->exec, c->stream));
-  c->launches += e->launches;
-  repack();
+  FG_TRY(pair_allreduce_grads(c, c->net, FG_NET_G));
+  FG_TRY(pair_gate(c, c->net, FG_NET_G, h, B, world));
+  FG_TRY(pair_optim(c, c->net, FG_NET_G, h, 1.0f / world));
+  FG_CUDA(cudaMemcpyAsync(c->net.hstats, c->net.dstats, sizeof(DeviceStats), cudaMemcpyDeviceToHost, c->stream));
   return FG_OK;
 }
 
 int net_train_step(fg_ctx* c, const fg_hyper* h, int B, const float* real, const float* noiseD, const float* noiseG,
                    const float* masksD, const float* masksG, uint64_t seed, bool allow_graph) {
   FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= c->maxB, "train step: batch %d must be even, >=4 and <= %d", B, c->maxB);
-  std::vector<uint8_t> key;
-  key_add(key, c->graph_epoch);
-  key_add(key, B);
-  key_add(key, *h);
-  const void* ptrs[] = {real, noiseD, noiseG, masksD, masksG, c->PG, c->PD, c->gG, c->gD, (const void*)c->stream, c->nccl_comm};
-  key_add(key, ptrs);
   return net_graph_run(
-      c, c->graphs, key, seed, [&]() { return train_step_body(c, h, B, real, noiseD, noiseG, masksD, masksG); },
-      [c]() { c->G_packed = c->D_packed = false; }, allow_graph);
+      c, c->net, B, h, {real, noiseD, noiseG, masksD, masksG}, seed,
+      [&]() { return train_step_body(c, h, B, real, noiseD, noiseG, masksD, masksG); }, allow_graph);
 }

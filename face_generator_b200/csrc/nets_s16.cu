@@ -14,31 +14,15 @@
 // (the inserted zeros contribute nothing) and keeps both layers on the tensor cores at 4x their minimal FLOPs, which
 // is 0.2 ms at batch 256.
 #include <algorithm>
-#include <cstring>
 
 #include "convl.h"
 #include "fg_internal.h"
 #include "k_conv_tc.h"
 #include "k_misc.h"
 
-#define LAUNCH_CHECK(c)                 \
-  do {                                  \
-    (c)->launches++;                    \
-    FG_CUDA(cudaGetLastError());        \
-  } while (0)
-
 namespace {
 constexpr int kS16Mask = 1024 + 128;  // nn.SpatialDropout() planes + nn.Dropout() of the dense branch, per sample
 constexpr int kSide = 16;
-
-inline int grid_for(int64_t n, int block, int cap = 132 * 16) {
-  int64_t g = (n + block - 1) / block;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-#define GRID_STRIDE(i, n) \
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < (n); i += (int64_t)gridDim.x * blockDim.x)
 
 // nn.SpatialAveragePooling(2,2,2,2), NHWC.  x [B][H][W][C] -> y [B][H/2][W/2][C]
 __global__ void avgpool2_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W, int C) {
@@ -137,12 +121,7 @@ struct UpsL {  // nn.SpatialUpSamplingNearest(2) -> 5x5 "same" convolution; H = 
 struct fg_s16 {
   fg_ctx* c = nullptr;
   int maxB = 0, C = 3;
-  int64_t nG = 0, nD = 0;
-  float *PG = nullptr, *PD = nullptr, *gG = nullptr, *gD = nullptr, *mG = nullptr, *vG = nullptr, *mD = nullptr,
-        *vD = nullptr;
-  float* bnG = nullptr;  // [768] running mean/var of the two BatchNorm layers (256 + 256 + 128 + 128)
-  DeviceStats *dstats = nullptr, *hstats = nullptr;
-  float* acc_hist = nullptr;
+  NetPair net;  // bnG: the running mean / var of G's two BatchNorm layers
   // G
   ConvL GL1, GC3;
   UpsL GU[2];
@@ -161,13 +140,11 @@ struct fg_s16 {
   // shared scratch
   float *ga = nullptr, *gb = nullptr, *dy_hi = nullptr, *dy_lo = nullptr, *ws = nullptr;
   float *in_a = nullptr, *in_b = nullptr, *in_c = nullptr, *in_m1 = nullptr, *in_m2 = nullptr, *io = nullptr;
-  bool G_packed = false, D_packed = false;
   int G_pack_impl = -1, D_pack_impl = -1;
   int G_B = 0, D_B = 0;
   bool G_valid = false, G_train = true, D_valid = false, D_train = true;
   std::vector<void*> allocs;
   ConvLEnv env;
-  std::vector<fg_ctx::StepGraph> graphs;  // captured train steps
 };
 
 namespace {
@@ -207,7 +184,7 @@ void make_layouts(fg_s16* n) {
     C3.w_off = o; o += (int64_t)C * 128 * 9;
     C3.b_off = o; o += C;
     C3.tf = "s16.G.C3.fwd"; C3.td = "s16.G.C3.dgrad"; C3.tw = "s16.G.C3.wgrad";
-    n->nG = o;
+    n->net.nG = o;
   }
   {  // D16Layout: conv branch, dense branch, joint Linear (ConcatTable order, models.lua:306-313)
     const int ci[4] = {C, 128, 128, 512}, co[4] = {128, 128, 512, 1024}, hw[4] = {16, 16, 8, 4};  // stride-1 sides
@@ -245,7 +222,7 @@ void make_layouts(fg_s16* n) {
     n->Dae2 = o; o += 1;
     n->DJW = o; o += 1152;
     n->DJb = o; o += 1;
-    n->nD = o;
+    n->net.nD = o;
   }
 }
 
@@ -255,27 +232,7 @@ int s16_alloc(fg_s16* n) {
   n->env.c = n->c;
   n->env.maxB = n->maxB;
   n->env.allocs = &n->allocs;
-  FG_TRY(dalloc(n, &n->PG, n->nG));
-  FG_TRY(dalloc(n, &n->PD, n->nD));
-  FG_TRY(dalloc(n, &n->gG, n->nG + kGradTail));
-  FG_TRY(dalloc(n, &n->gD, n->nD + kGradTail));
-  FG_TRY(dalloc(n, &n->mG, n->nG));
-  FG_TRY(dalloc(n, &n->vG, n->nG));
-  FG_TRY(dalloc(n, &n->mD, n->nD));
-  FG_TRY(dalloc(n, &n->vD, n->nD));
-  FG_TRY(dalloc(n, &n->bnG, 768));
-  {  // nn.SpatialBatchNormalization: running_mean = 0, running_var = 1
-    float init[768];
-    for (int i = 0; i < 768; ++i) init[i] = (i >= 256 && i < 512) || i >= 640 ? 1.f : 0.f;
-    FG_CUDA(cudaMemcpyAsync(n->bnG, init, sizeof(init), cudaMemcpyHostToDevice, n->c->stream));
-    FG_CUDA(cudaStreamSynchronize(n->c->stream));
-  }
-  float* tmp = nullptr;
-  FG_TRY(dalloc(n, &tmp, (sizeof(DeviceStats) + 3) / 4));
-  n->dstats = (DeviceStats*)tmp;
-  FG_TRY(dalloc(n, &n->acc_hist, kAccHistMax));
-  FG_CUDA(cudaMallocHost((void**)&n->hstats, sizeof(DeviceStats)));
-  memset(n->hstats, 0, sizeof(DeviceStats));
+  FG_TRY(pair_alloc(n->c, n->allocs, n->net, n->net.nG, n->net.nD, true));
   // ---- G ----
   FG_TRY(convl_alloc(n->env, n->GL1));
   FG_TRY(convl_alloc(n->env, n->GC3));
@@ -362,30 +319,30 @@ int s16_alloc(fg_s16* n) {
 
 int pack_G(fg_s16* n) {
   fg_ctx* c = n->c;
-  if (n->G_packed && n->G_pack_impl == pack_key(c)) return FG_OK;
-  FG_TRY(convl_pack(c, n->GL1, n->PG));
-  FG_TRY(convl_pack(c, n->GC3, n->PG));
+  if (n->net.G_packed && n->G_pack_impl == pack_key(c)) return FG_OK;
+  FG_TRY(convl_pack(c, n->GL1, n->net.PG));
+  FG_TRY(convl_pack(c, n->GC3, n->net.PG));
   for (int i = 0; i < 2; ++i) {
     UpsL& U = n->GU[i];
     if (use_tc_wgrad(c, U.geom(n->maxB)) && f16_on(c))
-      FG_TRY(tc_pack_collapsed_h(c, n->PG + U.w_off, U.Wf_hi, U.Wf_lo, U.Wd_hi, U.Wd_lo, U.Cout, U.Cin));
+      FG_TRY(tc_pack_collapsed_h(c, n->net.PG + U.w_off, U.Wf_hi, U.Wf_lo, U.Wd_hi, U.Wd_lo, U.Cout, U.Cin));
     else if (use_tc_wgrad(c, U.geom(n->maxB)))
-      FG_TRY(tc_pack_collapsed(c, n->PG + U.w_off, U.Wf_hi, U.Wf_lo, U.Wd_hi, U.Wd_lo, U.Cout, U.Cin));
+      FG_TRY(tc_pack_collapsed(c, n->net.PG + U.w_off, U.Wf_hi, U.Wf_lo, U.Wd_hi, U.Wd_lo, U.Cout, U.Cin));
     else
-      FG_TRY(k_pack_weights(c, n->PG + U.w_off, U.Wp, U.Wpd, U.Cout, U.Cin, 25, 0, 0, 0, 0));
+      FG_TRY(k_pack_weights(c, n->net.PG + U.w_off, U.Wp, U.Wpd, U.Cout, U.Cin, 25, 0, 0, 0, 0));
   }
-  n->G_packed = true;
+  n->net.G_packed = true;
   n->G_pack_impl = pack_key(c);
   return FG_OK;
 }
 int pack_D(fg_s16* n) {
   fg_ctx* c = n->c;
-  if (n->D_packed && n->D_pack_impl == pack_key(c)) return FG_OK;
-  for (int i = 0; i < 4; ++i) FG_TRY(convl_pack(c, n->Dc[i], n->PD));
-  FG_TRY(convl_pack(c, n->DF1, n->PD));
-  FG_TRY(convl_pack(c, n->DE1, n->PD));
-  FG_TRY(convl_pack(c, n->DE2, n->PD));
-  n->D_packed = true;
+  if (n->net.D_packed && n->D_pack_impl == pack_key(c)) return FG_OK;
+  for (int i = 0; i < 4; ++i) FG_TRY(convl_pack(c, n->Dc[i], n->net.PD));
+  FG_TRY(convl_pack(c, n->DF1, n->net.PD));
+  FG_TRY(convl_pack(c, n->DE1, n->net.PD));
+  FG_TRY(convl_pack(c, n->DE2, n->net.PD));
+  n->net.D_packed = true;
   n->D_pack_impl = pack_key(c);
   return FG_OK;
 }
@@ -401,7 +358,7 @@ int ups_fwd(fg_s16* n, UpsL& U, const float* h, float* z, int B, int* parts) {
   *parts = 0;
   if (!use_tc_wgrad(c, U.geom(n->maxB))) {
     ScopedTimer tm(c, U.tf);
-    return k_conv_simt(c, h, U.Wp, n->PG + U.b_off, z, g);
+    return k_conv_simt(c, h, U.Wp, n->net.PG + U.b_off, z, g);
   }
   const int64_t nh = (int64_t)B * (U.H / 2) * (U.H / 2) * U.Cin;
   const bool h16 = f16_on(c);
@@ -413,7 +370,7 @@ int ups_fwd(fg_s16* n, UpsL& U, const float* h, float* z, int B, int* parts) {
   }
   ScopedTimer tm(c, U.tf);
   float* st = want && c->bn_epilogue ? c->bn_parts : nullptr;
-  return tc_conv_fwd(c, U.h_hi, U.h_lo, U.Wf_hi, U.Wf_lo, n->PG + U.b_off, z, g, 2, st, st ? parts : nullptr, h16,
+  return tc_conv_fwd(c, U.h_hi, U.h_lo, U.Wf_hi, U.Wf_lo, n->net.PG + U.b_off, z, g, 2, st, st ? parts : nullptr, h16,
                      h16 ? U.sx + 1 : nullptr);
 }
 // dW += wgrad; dh = dgrad.  *pooled: dh already is the gradient of the LOW-RES input (tensor-core path folds the 2x2 sum of
@@ -426,7 +383,7 @@ int ups_bwd(fg_s16* n, UpsL& U, const float* h, const float* dz, float* dh, int 
       ScopedTimer tm(c, U.tw);
       FG_TRY(k_wgrad_simt(c, h, dz, n->ws, g));
     }
-    FG_TRY(k_unpack_wgrad(c, n->ws, n->gG + U.w_off, U.Cout, U.Cin, 25, 0, 0, 0, 0));
+    FG_TRY(k_unpack_wgrad(c, n->ws, n->net.gG + U.w_off, U.Cout, U.Cin, 25, 0, 0, 0, 0));
     *pooled = false;
     ScopedTimer tm(c, U.td);
     return k_conv_simt(c, dz, U.Wpd, nullptr, dh, ConvGeom{B, U.H, U.H, U.Cout, U.Cin, 5, 1});
@@ -444,7 +401,7 @@ int ups_bwd(fg_s16* n, UpsL& U, const float* h, const float* dz, float* dh, int 
     ScopedTimer tm(c, U.tw);
     FG_TRY(tc_conv_wgrad(c, U.h_hi, U.h_lo, n->dy_hi, n->dy_lo, n->ws, g, h16, h16 ? sdy + 1 : nullptr, h16 ? U.sx + 1 : nullptr));
   }
-  FG_TRY(tc_combine_collapsed_wgrad(c, n->ws, n->gG + U.w_off, U.Cout, U.Cin));
+  FG_TRY(tc_combine_collapsed_wgrad(c, n->ws, n->net.gG + U.w_off, U.Cout, U.Cin));
   *pooled = true;
   ScopedTimer tm(c, U.td);
   return tc_conv_dgrad_ups(c, n->dy_hi, n->dy_lo, U.Wd_hi, U.Wd_lo, dh, g, h16, h16 ? sdy + 1 : nullptr);
@@ -455,7 +412,7 @@ int bn_stats(fg_s16* n, int i, const float* z, int B, bool training, int parts) 
   fg_ctx* c = n->c;
   const int Cc = i == 0 ? 256 : 128;
   const int64_t P = (int64_t)B * (i == 0 ? 64 : 256);
-  float *rm = n->bnG + (i == 0 ? 0 : 512), *rv = rm + Cc;
+  float *rm = n->net.bnG + (i == 0 ? 0 : 512), *rv = rm + Cc;
   if (!training) return k_bn_eval_prep(c, rm, rv, n->bn_mean[i], n->bn_istd[i], Cc);
   if (parts) return k_bn_finalize_parts(c, c->bn_parts, parts, n->bn_mean[i], n->bn_istd[i], rm, rv, P, Cc);
   FG_TRY(k_bn_stats(c, z, c->bn_acc, P, Cc));
@@ -467,7 +424,7 @@ int G_forward(fg_s16* n, const float* noise, int B, bool training) {
   fg_ctx* c = n->c;
   FG_REQUIRE(B >= 1 && B <= n->maxB, "s16 G forward: batch %d out of range [1,%d]", B, n->maxB);
   FG_TRY(pack_G(n));
-  const float* P = n->PG;
+  const float* P = n->net.PG;
   if (noise != n->G_x) FG_CUDA(cudaMemcpyAsync(n->G_x, noise, sizeof(float) * B * 100, cudaMemcpyDeviceToDevice, c->stream));
   FG_TRY(convl_fwd(n->env, n->GL1, n->G_x, P, n->G_z0, B));
   FG_TRY(k_prelu_fwd(c, n->G_z0, P + n->Ga[0], n->G_h0, (int64_t)B * 2048));
@@ -496,8 +453,8 @@ int G_backward(fg_s16* n, const float* dy, float* dnoise) {
     return FG_ERR_STATE;
   }
   const int B = n->G_B;
-  const float* P = n->PG;
-  float* G = n->gG;
+  const float* P = n->net.PG;
+  float* G = n->net.gG;
   FG_TRY(k_sigmoid_bwd(c, dy, n->G_y, n->G_dz3, (int64_t)B * 256 * n->C));
   FG_TRY(convl_bwd(n->env, n->GC3, n->G_h2, n->G_dz3, G, n->G_dfull, B));
   bool pooled = false;
@@ -527,7 +484,7 @@ int D_forward(fg_s16* n, const float* x, int B, bool training) {
   fg_ctx* c = n->c;
   FG_REQUIRE(B >= 1 && B <= n->maxB, "s16 D forward: batch %d out of range [1,%d]", B, n->maxB);
   FG_TRY(pack_D(n));
-  const float* P = n->PD;
+  const float* P = n->net.PD;
   if (x != n->D_x) FG_CUDA(cudaMemcpyAsync(n->D_x, x, sizeof(float) * (size_t)B * 256 * n->C, cudaMemcpyDeviceToDevice, c->stream));
   const float* masks = training ? n->D_masks : nullptr;
   // ---- conv branch ----
@@ -577,8 +534,8 @@ int D_backward(fg_s16* n, const float* dlogit, bool want_wgrad, bool want_dx) {
     return FG_ERR_STATE;
   }
   const int B = n->D_B;
-  const float* P = n->PD;
-  float* G = want_wgrad ? n->gD : nullptr;
+  const float* P = n->net.PD;
+  float* G = want_wgrad ? n->net.gD : nullptr;
   const bool tr = n->D_train;
   const float* masks = tr ? n->D_masks : nullptr;
   if (G) FG_TRY(k_gemv_wgrad_add(c, n->D_joint, dlogit, G + n->DJW, G + n->DJb, B, 1152));
@@ -634,36 +591,6 @@ int D_backward(fg_s16* n, const float* dlogit, bool want_wgrad, bool want_dx) {
   return FG_OK;
 }
 
-// penalty -> clamp -> interruptable optimizer on the flat vectors (adversarial.lua:219-231, interruptable_optimizers.lua)
-int optim(fg_s16* n, int net, const fg_hyper* h, float grad_scale) {
-  fg_ctx* c = n->c;
-  const bool isD = net == FG_NET_D;
-  float *p = isD ? n->PD : n->PG, *g = isD ? n->gD : n->gG, *m = isD ? n->mD : n->mG, *v = isD ? n->vD : n->vG;
-  const int64_t cnt = isD ? n->nD : n->nG;
-  const float l1 = isD ? h->D_L1 : h->G_L1, l2 = isD ? h->D_L2 : h->G_L2;
-  const bool pen = l1 != 0.f || l2 != 0.f;
-  const float l1_grad = !pen ? 0.f : (isD ? l1 : l2);  // adversarial.lua:223 scales sign(p) by G_L2
-  if (pen) FG_TRY(k_penalty_loss(c, p, cnt, l1, l2, isD ? &n->dstats->loss_D : &n->dstats->loss_G));
-  FG_TRY(k_optim_update(c, isD ? c->opt_D : c->opt_G, p, g, m, v, cnt, h->beta1, h->beta2, h->eps,
-                        isD ? c->sgd_mom_D : c->sgd_mom_G, l1_grad, pen ? l2 : 0.f, isD ? h->D_clamp : h->G_clamp, grad_scale,
-                        isD ? &n->dstats->step_D : &n->dstats->step_G, isD ? &n->dstats->do_train_D : &n->dstats->do_train_G,
-                        isD ? &n->dstats->t_D : &n->dstats->t_G));
-  if (isD) n->D_packed = false; else n->G_packed = false;
-  return FG_OK;
-}
-// the accuracy gate, t += 1 and the step size, on this net's own statistics block (kernel shared with the 32x32 loop)
-int gate_prep(fg_s16* n, int net, const fg_hyper* h, const float* tail4, int B) {
-  fg_ctx* c = n->c;
-  DeviceStats* sd = c->dstats;
-  float* sa = c->acc_hist;
-  c->dstats = n->dstats;
-  c->acc_hist = n->acc_hist;
-  const int r = k_gate_and_prep(c, net, h, tail4, B, (float)c->world);
-  c->dstats = sd;
-  c->acc_hist = sa;
-  return r;
-}
-
 // one iteration of the adversarial.lua loop body (D_iterations = G_iterations = 1) on the 16x16 nets
 int train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const float* noiseD, const float* noiseG,
                const float* masksD, const float* masksG, uint64_t seed) {
@@ -679,60 +606,38 @@ int train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const flo
     FG_CUDA(cudaMemcpyAsync(n->D_masks, masksD, sizeof(float) * (size_t)B * kS16Mask, cudaMemcpyDeviceToDevice, c->stream));
   else
     FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * kS16Mask, 1, 0.5f, c->seed_dev));
-  FG_CUDA(cudaMemsetAsync(n->gD, 0, sizeof(float) * (n->nD + kGradTail), c->stream));
+  FG_TRY(pair_zero_grads(c, n->net, FG_NET_D));
   FG_TRY(D_forward(n, n->D_x, B, true));
-  FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->dstats->loss_D, n->gD + n->nD, B, Bh));
+  FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_D, n->net.tailD, B, Bh));
   FG_TRY(D_backward(n, n->D_dlogit, true, false));
-  if (c->world > 1) FG_TRY(net_allreduce(c, n->gD, n->nD + kGradTail));
-  FG_TRY(gate_prep(n, FG_NET_D, h, n->gD + n->nD, B));
-  FG_TRY(optim(n, FG_NET_D, h, inv_world));
+  FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_D));
+  FG_TRY(pair_gate(c, n->net, FG_NET_D, h, B, (float)c->world));
+  FG_TRY(pair_optim(c, n->net, FG_NET_D, h, inv_world));
   // ---- G step (adversarial.lua:275-288) ----
-  FG_CUDA(cudaMemsetAsync(n->gG, 0, sizeof(float) * (n->nG + kGradTail), c->stream));
+  FG_TRY(pair_zero_grads(c, n->net, FG_NET_G));
   FG_TRY(G_forward(n, noiseG, B, true));
   if (masksG)
     FG_CUDA(cudaMemcpyAsync(n->D_masks, masksG, sizeof(float) * (size_t)B * kS16Mask, cudaMemcpyDeviceToDevice, c->stream));
   else
     FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * kS16Mask, 2, 0.5f, c->seed_dev));
   FG_TRY(D_forward(n, n->G_y, B, true));
-  FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->dstats->loss_G, n->gG + n->nG, B, B));
+  FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_G, n->net.tailG, B, B));
   FG_TRY(D_backward(n, n->D_dlogit, false, true));  // D's weight grads are discarded by the reference (:209 vs :92)
   FG_TRY(G_backward(n, n->D_dx, nullptr));
-  if (c->world > 1) FG_TRY(net_allreduce(c, n->gG, n->nG + kGradTail));
-  FG_TRY(gate_prep(n, FG_NET_G, h, n->gG + n->nG, B));
-  FG_TRY(optim(n, FG_NET_G, h, inv_world));
-  FG_CUDA(cudaMemcpyAsync(n->hstats, n->dstats, sizeof(DeviceStats), cudaMemcpyDeviceToHost, c->stream));
+  FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_G));
+  FG_TRY(pair_gate(c, n->net, FG_NET_G, h, B, (float)c->world));
+  FG_TRY(pair_optim(c, n->net, FG_NET_G, h, inv_world));
+  FG_CUDA(cudaMemcpyAsync(n->net.hstats, n->net.dstats, sizeof(DeviceStats), cudaMemcpyDeviceToHost, c->stream));
   return FG_OK;
 }
 
-// train_step on device inputs: eager the first time, then a captured CUDA graph of the step (nets.cu net_graph_run);
-// the seed is read on the device
+// train_step on device inputs: eager the first time, then a captured CUDA graph of the step (net_graph_run); the seed
+// is read on the device
 int run_train_step(fg_s16* n, const fg_hyper* h, int B, const float* rd, const float* nd, const float* ng, const float* md,
                    const float* mg, uint64_t seed, fg_step_stats* stats) {
-  fg_ctx* c = n->c;
-  {
-    std::vector<uint8_t> key;
-    auto add = [&key](const void* p, size_t nb) { key.insert(key.end(), (const uint8_t*)p, (const uint8_t*)p + nb); };
-    const void* ptrs[] = {rd, nd, ng, md, mg, (const void*)c->stream, c->nccl_comm};
-    const int meta[3] = {c->graph_epoch, B, pack_key(c)};
-    add(meta, sizeof(meta));
-    add(h, sizeof(*h));
-    add(ptrs, sizeof(ptrs));
-    FG_TRY(net_graph_run(
-        c, n->graphs, key, seed, [&]() { return train_step(n, h, B, rd, nd, ng, md, mg, 0); },
-        [n]() { n->G_packed = n->D_packed = false; }, true));
-  }
-  if (stats) {
-    FG_CUDA(cudaStreamSynchronize(c->stream));
-    const DeviceStats& s = *n->hstats;
-    stats->loss_D = s.loss_D;
-    stats->loss_G = s.loss_G;
-    for (int i = 0; i < 4; ++i) stats->conf[i] = s.conf[i];
-    stats->trained_D = s.trained_D;
-    stats->t_D = s.t_D;
-    stats->t_G = s.t_G;
-    stats->acc_D = s.acc_D;
-  }
-  return FG_OK;
+  FG_TRY(net_graph_run(
+      n->c, n->net, B, h, {rd, nd, ng, md, mg}, seed, [&]() { return train_step(n, h, B, rd, nd, ng, md, mg, 0); }, true));
+  return pair_step_stats(n->c, n->net, stats);
 }
 }  // namespace
 
@@ -772,10 +677,8 @@ int fg_s16_destroy(fg_s16* n) {
     cudaSetDevice(n->c->device);
     cudaStreamSynchronize(n->c->stream);
   }
-  for (auto& g : n->graphs)
-    if (g.exec) cudaGraphExecDestroy(g.exec);
+  pair_free(n->net);
   for (void* p : n->allocs) cudaFree(p);
-  if (n->hstats) cudaFreeHost(n->hstats);
   delete n;
   return FG_OK;
 }
@@ -783,74 +686,50 @@ int64_t fg_s16_param_count(int net, int channels) {
   fg_s16 tmp;
   tmp.C = channels;
   make_layouts(&tmp);
-  return net == FG_NET_D ? tmp.nD : tmp.nG;
+  return net == FG_NET_D ? tmp.net.nD : tmp.net.nG;
 }
 int fg_s16_mask_per_sample(void) { return kS16Mask; }
 
 int fg_s16_set_params(fg_s16* n, int net, const float* src) {
   ENTER(n);
   FG_REQUIRE(src && (net == FG_NET_G || net == FG_NET_D), "fg_s16_set_params: bad arguments");
-  const bool isD = net == FG_NET_D;
-  FG_CUDA(cudaMemcpyAsync(isD ? n->PD : n->PG, src, sizeof(float) * (isD ? n->nD : n->nG), cudaMemcpyDefault, n->c->stream));
-  FG_CUDA(cudaStreamSynchronize(n->c->stream));
-  if (isD) n->D_packed = false; else n->G_packed = false;
-  return FG_OK;
+  return pair_set_params(n->c, n->net, net, src);
 }
 int fg_s16_get_params(fg_s16* n, int net, float* dst) {
   ENTER(n);
   FG_REQUIRE(dst && (net == FG_NET_G || net == FG_NET_D), "fg_s16_get_params: bad arguments");
-  const bool isD = net == FG_NET_D;
-  return fg_to_user(n->c, dst, isD ? n->PD : n->PG, isD ? n->nD : n->nG);
+  return pair_get_params(n->c, n->net, net, dst);
 }
 int fg_s16_get_grads(fg_s16* n, int net, float* dst) {
   ENTER(n);
   FG_REQUIRE(dst && (net == FG_NET_G || net == FG_NET_D), "fg_s16_get_grads: bad arguments");
-  const bool isD = net == FG_NET_D;
-  return fg_to_user(n->c, dst, isD ? n->gD : n->gG, isD ? n->nD : n->nG);
+  return pair_get_grads(n->c, n->net, net, dst);
 }
 int fg_s16_zero_grads(fg_s16* n, int net) {
   ENTER(n);
-  const bool isD = net == FG_NET_D;
-  FG_CUDA(cudaMemsetAsync(isD ? n->gD : n->gG, 0, sizeof(float) * ((isD ? n->nD : n->nG) + kGradTail), n->c->stream));
-  return FG_OK;
+  return pair_zero_grads(n->c, n->net, net);
 }
-float* fg_s16_params_ptr(fg_s16* n, int net) { return !n ? nullptr : (net == FG_NET_D ? n->PD : n->PG); }
-float* fg_s16_grads_ptr(fg_s16* n, int net) { return !n ? nullptr : (net == FG_NET_D ? n->gD : n->gG); }
+float* fg_s16_params_ptr(fg_s16* n, int net) { return !n ? nullptr : (net == FG_NET_D ? n->net.PD : n->net.PG); }
+float* fg_s16_grads_ptr(fg_s16* n, int net) { return !n ? nullptr : (net == FG_NET_D ? n->net.gD : n->net.gG); }
 
 int fg_s16_set_adam_state(fg_s16* n, int net, const float* m, const float* v, int t) {
   ENTER(n);
-  const bool isD = net == FG_NET_D;
-  const size_t cnt = isD ? n->nD : n->nG;
-  if (m) FG_CUDA(cudaMemcpyAsync(isD ? n->mD : n->mG, m, sizeof(float) * cnt, cudaMemcpyDefault, n->c->stream));
-  if (v) FG_CUDA(cudaMemcpyAsync(isD ? n->vD : n->vG, v, sizeof(float) * cnt, cudaMemcpyDefault, n->c->stream));
-  FG_CUDA(cudaMemcpyAsync(isD ? &n->dstats->t_D : &n->dstats->t_G, &t, sizeof(int), cudaMemcpyHostToDevice, n->c->stream));
-  FG_CUDA(cudaStreamSynchronize(n->c->stream));
-  return FG_OK;
+  return pair_set_adam_state(n->c, n->net, net, m, v, t);
 }
 int fg_s16_get_adam_state(fg_s16* n, int net, float* m, float* v, int* t) {
   ENTER(n);
-  const bool isD = net == FG_NET_D;
-  const size_t cnt = isD ? n->nD : n->nG;
-  if (m) FG_TRY(fg_to_user(n->c, m, isD ? n->mD : n->mG, cnt));
-  if (v) FG_TRY(fg_to_user(n->c, v, isD ? n->vD : n->vG, cnt));
-  if (t) {
-    FG_CUDA(cudaMemcpyAsync(t, isD ? &n->dstats->t_D : &n->dstats->t_G, sizeof(int), cudaMemcpyDeviceToHost, n->c->stream));
-    FG_CUDA(cudaStreamSynchronize(n->c->stream));
-  }
-  return FG_OK;
+  return pair_get_adam_state(n->c, n->net, net, m, v, t);
 }
 // running_mean / running_var of G's two nn.SpatialBatchNormalization layers: [mean1 256][var1 256][mean2 128][var2 128]
 int fg_s16_set_bn_state(fg_s16* n, const float* src768) {
   ENTER(n);
   FG_REQUIRE(src768, "fg_s16_set_bn_state: null source");
-  FG_CUDA(cudaMemcpyAsync(n->bnG, src768, sizeof(float) * 768, cudaMemcpyDefault, n->c->stream));
-  FG_CUDA(cudaStreamSynchronize(n->c->stream));
-  return FG_OK;
+  return pair_set_bn_state(n->c, n->net, src768);
 }
 int fg_s16_get_bn_state(fg_s16* n, float* dst768) {
   ENTER(n);
   FG_REQUIRE(dst768, "fg_s16_get_bn_state: null destination");
-  return fg_to_user(n->c, dst768, n->bnG, 768);
+  return pair_get_bn_state(n->c, n->net, dst768);
 }
 
 // noise [B][100] -> images [B][C][16][16] (NCHW; host or device pointers).  training != 0: batch statistics + running
@@ -913,23 +792,7 @@ int fg_s16_D_backward(fg_s16* n, const float* d_out, int want_wgrad, float* d_im
 // data parallel: rank 0's parameters, optimizer moments, step counters and BatchNorm running statistics to every rank
 int fg_s16_dp_broadcast_params(fg_s16* n) {
   ENTER(n);
-  fg_ctx* c = n->c;
-  if (c->world <= 1) return FG_OK;
-  FG_TRY(net_group(true));
-  const size_t bG = n->nG * sizeof(float), bD = n->nD * sizeof(float);
-  FG_TRY(net_broadcast(c, n->PG, bG));
-  FG_TRY(net_broadcast(c, n->PD, bD));
-  FG_TRY(net_broadcast(c, n->mG, bG));
-  FG_TRY(net_broadcast(c, n->vG, bG));
-  FG_TRY(net_broadcast(c, n->mD, bD));
-  FG_TRY(net_broadcast(c, n->vD, bD));
-  FG_TRY(net_broadcast(c, n->bnG, 768 * sizeof(float)));
-  FG_TRY(net_broadcast(c, n->dstats, sizeof(DeviceStats)));
-  FG_TRY(net_broadcast(c, n->acc_hist, kAccHistMax * sizeof(float)));
-  FG_TRY(net_group(false));
-  FG_CUDA(cudaStreamSynchronize(c->stream));
-  n->G_packed = n->D_packed = false;
-  return FG_OK;
+  return pair_broadcast(n->c, n->net);
 }
 
 int fg_s16_train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const float* noise_D, const float* noise_G,

@@ -13,7 +13,7 @@ import ctypes as C
 
 import numpy as np
 
-from .lib import Context, StepStats, _check
+from .lib import Context, StepStats, _check, _stats
 
 
 class DeviceDataset:
@@ -70,10 +70,7 @@ class DeviceDataset:
         st = StepStats() if want_stats else None
         _check(self.lib.fg_train_step_dataset(self.ctx.h, self.h, C.byref(hyper), B, seed,
                                               C.byref(st) if st is not None else None), "fg_train_step_dataset")
-        if st is None:
-            return None
-        return dict(loss_D=st.loss_D, loss_G=st.loss_G, conf=list(st.conf), trained_D=st.trained_D, t_D=st.t_D,
-                    t_G=st.t_G, acc_D=st.acc_D)
+        return _stats(st)
 
 
 def noise_uniform(ctx: Context, seed, shape):

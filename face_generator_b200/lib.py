@@ -243,7 +243,79 @@ class PinnedArray:
             self.addr = None
 
 
-class Context:
+def _stats(st):
+    """fg_step_stats -> dict (None when no statistics were asked for)"""
+    if st is None:
+        return None
+    return dict(loss_D=st.loss_D, loss_G=st.loss_G, conf=list(st.conf), trained_D=st.trained_D, t_D=st.t_D,
+                t_G=st.t_G, acc_D=st.acc_D)
+
+
+class _NetPair:
+    """What Context, C2f and S16 share: the flat parameters, gradients and optimizer state of one G/D pair, reached
+    through the C entry points _prefix + "set_params", _prefix + "get_grads", ..."""
+    _prefix = "fg_"  # "fg_", "fg_c2f_" or "fg_s16_"
+    _what = ""       # how errors of _sized name the nets: "", "c2f ", "s16 "
+
+    def _call(self, name, *args):
+        fn = self._prefix + name
+        _check(getattr(self.lib, fn)(self.h, *args), fn)
+
+    def count(self, net):
+        return self.nD if net == NET_D else self.nG
+
+    def _sized(self, what, a, n):
+        """the C ABI copies exactly n floats from the pointer it is given: a shorter buffer (a checkpoint written by a
+        1- vs 3-channel build, a truncated or hostile file) would be read out of bounds, so sizes are checked here
+        with a real error (asserts vanish under python -O)"""
+        a = f32(a)
+        if a.size != n:
+            raise FGError("%s%s: expected %d floats, got %d" % (self._what, what, n, a.size))
+        return a
+
+    def set_params(self, net, p):
+        self._call("set_params", net, _ptr(self._sized("set_params", p, self.count(net))))
+
+    def get_params(self, net):
+        out = np.empty(self.count(net), np.float32)
+        self._call("get_params", net, _ptr(out))
+        return out
+
+    def get_grads(self, net):
+        out = np.empty(self.count(net), np.float32)
+        self._call("get_grads", net, _ptr(out))
+        return out
+
+    def zero_grads(self, net):
+        self._call("zero_grads", net)
+
+    def set_adam_state(self, net, m, v, t):
+        m = None if m is None else self._sized("set_adam_state m", m, self.count(net))
+        v = None if v is None else self._sized("set_adam_state v", v, self.count(net))
+        self._call("set_adam_state", net, _ptr(m), _ptr(v), int(t))
+
+    def get_adam_state(self, net):
+        m, v, t = np.empty(self.count(net), np.float32), np.empty(self.count(net), np.float32), C.c_int(0)
+        self._call("get_adam_state", net, _ptr(m), _ptr(v), C.byref(t))
+        return m, v, t.value
+
+    def dp_broadcast_params(self):
+        self._call("dp_broadcast_params")
+
+
+class _BatchNormNetPair(_NetPair):
+    """A pair whose G has BatchNorm layers: their running statistics, [mean1 256][var1 256][mean2 128][var2 128]."""
+
+    def set_bn_state(self, s):
+        self._call("set_bn_state", _ptr(self._sized("set_bn_state", s, 768)))
+
+    def get_bn_state(self):
+        out = np.empty(768, np.float32)
+        self._call("get_bn_state", _ptr(out))
+        return out
+
+
+class Context(_BatchNormNetPair):
     """One fg_ctx (one GPU).  Mirrors face_generator_b200/lua/b200.lua's `b200.Context`."""
 
     def __init__(self, device=0, max_batch=256, channels=3):
@@ -264,54 +336,6 @@ class Context:
             self.close()
         except Exception:
             pass
-
-    # ---- parameters ----
-    def count(self, net):
-        return self.nD if net == NET_D else self.nG
-
-    def _sized(self, what, a, n):
-        """the C ABI copies exactly n floats from the pointer it is given: a shorter buffer (a checkpoint written by a
-        1- vs 3-channel build, a truncated or hostile file) would be read out of bounds, so sizes are checked here
-        with a real error (asserts vanish under python -O)"""
-        a = f32(a)
-        if a.size != n:
-            raise FGError("%s: expected %d floats, got %d" % (what, n, a.size))
-        return a
-
-    def set_params(self, net, p):
-        p = self._sized("set_params", p, self.count(net))
-        _check(self.lib.fg_set_params(self.h, net, _ptr(p)), "fg_set_params")
-
-    def get_params(self, net):
-        out = np.empty(self.count(net), np.float32)
-        _check(self.lib.fg_get_params(self.h, net, _ptr(out)), "fg_get_params")
-        return out
-
-    def get_grads(self, net):
-        out = np.empty(self.count(net), np.float32)
-        _check(self.lib.fg_get_grads(self.h, net, _ptr(out)), "fg_get_grads")
-        return out
-
-    def zero_grads(self, net):
-        _check(self.lib.fg_zero_grads(self.h, net), "fg_zero_grads")
-
-    def set_adam_state(self, net, m, v, t):
-        m = None if m is None else self._sized("set_adam_state m", m, self.count(net))
-        v = None if v is None else self._sized("set_adam_state v", v, self.count(net))
-        _check(self.lib.fg_set_adam_state(self.h, net, _ptr(m), _ptr(v), int(t)), "fg_set_adam_state")
-
-    def get_adam_state(self, net):
-        m, v, t = np.empty(self.count(net), np.float32), np.empty(self.count(net), np.float32), C.c_int(0)
-        _check(self.lib.fg_get_adam_state(self.h, net, _ptr(m), _ptr(v), C.byref(t)), "fg_get_adam_state")
-        return m, v, t.value
-
-    def set_bn_state(self, s):
-        _check(self.lib.fg_set_bn_state(self.h, _ptr(self._sized("set_bn_state", s, 768))), "fg_set_bn_state")
-
-    def get_bn_state(self):
-        out = np.empty(768, np.float32)
-        _check(self.lib.fg_get_bn_state(self.h, _ptr(out)), "fg_get_bn_state")
-        return out
 
     def set_option(self, key, value):
         _check(self.lib.fg_set_option(self.h, key.encode(), int(value)), "fg_set_option(%s)" % key)
@@ -379,10 +403,7 @@ class Context:
         _check(self.lib.fg_train_step(self.h, C.byref(hyper), B, _ptr(real), _ptr(noise_D), _ptr(noise_G),
                                       _ptr(masks_D), _ptr(masks_G), seed, C.byref(st) if st is not None else None),
                "fg_train_step")
-        if st is None:
-            return None
-        return dict(loss_D=st.loss_D, loss_G=st.loss_G, conf=list(st.conf), trained_D=st.trained_D, t_D=st.t_D,
-                    t_G=st.t_G, acc_D=st.acc_D)
+        return _stats(st)
 
     def sample(self, noise, chunk):
         noise = f32(noise)
@@ -447,9 +468,6 @@ class Context:
     def dp_init(self, id_bytes, nranks, rank):
         buf = (C.c_ubyte * 128).from_buffer_copy(id_bytes)
         _check(self.lib.fg_dp_init(self.h, buf, nranks, rank), "fg_dp_init")
-
-    def dp_broadcast_params(self):
-        _check(self.lib.fg_dp_broadcast_params(self.h), "fg_dp_broadcast_params")
 
     # ---- L-op: resampling / pooling / dropout / sigmoid at the nn.Module boundary (NCHW numpy in/out) ----
     def upsample2_forward(self, x):
@@ -545,8 +563,9 @@ class Context:
 C2F_MASK_PER_SAMPLE = 16384 + 512
 
 
-class C2f:
+class C2f(_NetPair):
     """Coarse-to-fine nets + loop (train_c2f.lua) on a Context.  Mirrors lua/adversarial_c2f_b200.lua."""
+    _prefix, _what = "fg_c2f_", "c2f "
 
     def __init__(self, ctx):
         self.ctx, self.lib, self.C = ctx, ctx.lib, ctx.C
@@ -567,42 +586,6 @@ class C2f:
                 self.close()
         except Exception:
             pass
-
-    def count(self, net):
-        return self.nD if net == NET_D else self.nG
-
-    def _sized(self, what, a, n):
-        a = f32(a)
-        if a.size != n:
-            raise FGError("%s: expected %d floats, got %d" % (what, n, a.size))
-        return a
-
-    def set_params(self, net, p):
-        p = self._sized("c2f set_params", p, self.count(net))
-        _check(self.lib.fg_c2f_set_params(self.h, net, _ptr(p)), "fg_c2f_set_params")
-
-    def get_params(self, net):
-        out = np.empty(self.count(net), np.float32)
-        _check(self.lib.fg_c2f_get_params(self.h, net, _ptr(out)), "fg_c2f_get_params")
-        return out
-
-    def get_grads(self, net):
-        out = np.empty(self.count(net), np.float32)
-        _check(self.lib.fg_c2f_get_grads(self.h, net, _ptr(out)), "fg_c2f_get_grads")
-        return out
-
-    def zero_grads(self, net):
-        _check(self.lib.fg_c2f_zero_grads(self.h, net), "fg_c2f_zero_grads")
-
-    def set_adam_state(self, net, m, v, t):
-        m = None if m is None else self._sized("c2f set_adam_state m", m, self.count(net))
-        v = None if v is None else self._sized("c2f set_adam_state v", v, self.count(net))
-        _check(self.lib.fg_c2f_set_adam_state(self.h, net, _ptr(m), _ptr(v), int(t)), "fg_c2f_set_adam_state")
-
-    def get_adam_state(self, net):
-        m, v, t = np.empty(self.count(net), np.float32), np.empty(self.count(net), np.float32), C.c_int(0)
-        _check(self.lib.fg_c2f_get_adam_state(self.h, net, _ptr(m), _ptr(v), C.byref(t)), "fg_c2f_get_adam_state")
-        return m, v, t.value
 
     def G_forward(self, noise, cond, want_diff=True):
         noise, cond = f32(noise), f32(cond)
@@ -629,9 +612,6 @@ class C2f:
         _check(self.lib.fg_c2f_D_backward(self.h, _ptr(d_out), int(want_wgrad), _ptr(dd)), "fg_c2f_D_backward")
         return dd
 
-    def dp_broadcast_params(self):
-        _check(self.lib.fg_c2f_dp_broadcast_params(self.h), "fg_c2f_dp_broadcast_params")
-
     def train_step(self, hyper, B, real_diff, cond_D, noise_D, cond_G, noise_G, masks_D=None, masks_G=None, seed=0,
                    want_stats=True):
         """Pointers may be numpy float32 arrays (host) or raw addresses (device / pinned)."""
@@ -639,9 +619,7 @@ class C2f:
         _check(self.lib.fg_c2f_train_step(self.h, C.byref(hyper), B, _ptr(real_diff), _ptr(cond_D), _ptr(noise_D),
                                           _ptr(cond_G), _ptr(noise_G), _ptr(masks_D), _ptr(masks_G), seed,
                                           C.byref(st) if st is not None else None), "fg_c2f_train_step")
-        if st is None:
-            return None
-        return dict(loss_D=st.loss_D, loss_G=st.loss_G, conf=list(st.conf), t_D=st.t_D, t_G=st.t_G, acc_D=st.acc_D)
+        return _stats(st)
 
     def train_step_dataset(self, dataset, hyper, B, coarse_size, seed, want_stats=True):
         """train_step with the pairs, conditions and noise drawn on the device from a DeviceDataset of this ctx
@@ -649,16 +627,15 @@ class C2f:
         st = StepStats() if want_stats else None
         _check(self.lib.fg_c2f_train_step_dataset(self.h, dataset.h, C.byref(hyper), B, coarse_size, seed,
                                                   C.byref(st) if st is not None else None), "fg_c2f_train_step_dataset")
-        if st is None:
-            return None
-        return dict(loss_D=st.loss_D, loss_G=st.loss_G, conf=list(st.conf), t_D=st.t_D, t_G=st.t_G, acc_D=st.acc_D)
+        return _stats(st)
 
 
 S16_MASK_PER_SAMPLE = 1024 + 128
 
 
-class S16:
+class S16(_BatchNormNetPair):
     """The --scale 16 nets (models.lua:27-51 G16, :279-316 D16_d) + the adversarial.lua loop on a Context."""
+    _prefix, _what = "fg_s16_", "s16 "
 
     def __init__(self, ctx):
         self.ctx, self.lib, self.C = ctx, ctx.lib, ctx.C
@@ -679,51 +656,6 @@ class S16:
                 self.close()
         except Exception:
             pass
-
-    def count(self, net):
-        return self.nD if net == NET_D else self.nG
-
-    def _sized(self, what, a, n):
-        a = f32(a)
-        if a.size != n:
-            raise FGError("%s: expected %d floats, got %d" % (what, n, a.size))
-        return a
-
-    def set_params(self, net, p):
-        p = self._sized("s16 set_params", p, self.count(net))
-        _check(self.lib.fg_s16_set_params(self.h, net, _ptr(p)), "fg_s16_set_params")
-
-    def get_params(self, net):
-        out = np.empty(self.count(net), np.float32)
-        _check(self.lib.fg_s16_get_params(self.h, net, _ptr(out)), "fg_s16_get_params")
-        return out
-
-    def get_grads(self, net):
-        out = np.empty(self.count(net), np.float32)
-        _check(self.lib.fg_s16_get_grads(self.h, net, _ptr(out)), "fg_s16_get_grads")
-        return out
-
-    def zero_grads(self, net):
-        _check(self.lib.fg_s16_zero_grads(self.h, net), "fg_s16_zero_grads")
-
-    def set_adam_state(self, net, m, v, t):
-        m = None if m is None else self._sized("s16 set_adam_state m", m, self.count(net))
-        v = None if v is None else self._sized("s16 set_adam_state v", v, self.count(net))
-        _check(self.lib.fg_s16_set_adam_state(self.h, net, _ptr(m), _ptr(v), int(t)), "fg_s16_set_adam_state")
-
-    def get_adam_state(self, net):
-        m, v, t = np.empty(self.count(net), np.float32), np.empty(self.count(net), np.float32), C.c_int(0)
-        _check(self.lib.fg_s16_get_adam_state(self.h, net, _ptr(m), _ptr(v), C.byref(t)), "fg_s16_get_adam_state")
-        return m, v, t.value
-
-    def set_bn_state(self, s):
-        s = self._sized("s16 set_bn_state", s, 768)
-        _check(self.lib.fg_s16_set_bn_state(self.h, _ptr(s)), "fg_s16_set_bn_state")
-
-    def get_bn_state(self):
-        out = np.empty(768, np.float32)
-        _check(self.lib.fg_s16_get_bn_state(self.h, _ptr(out)), "fg_s16_get_bn_state")
-        return out
 
     def G_forward(self, noise, training=True, want_img=True):
         noise = f32(noise)
@@ -752,18 +684,12 @@ class S16:
         _check(self.lib.fg_s16_D_backward(self.h, _ptr(d_out), int(want_wgrad), _ptr(dd)), "fg_s16_D_backward")
         return dd
 
-    def dp_broadcast_params(self):
-        _check(self.lib.fg_s16_dp_broadcast_params(self.h), "fg_s16_dp_broadcast_params")
-
     def train_step(self, hyper, B, real, noise_D, noise_G, masks_D=None, masks_G=None, seed=0, want_stats=True):
         """Pointers may be numpy float32 arrays (host) or raw addresses (device / pinned)."""
         st = StepStats() if want_stats else None
         _check(self.lib.fg_s16_train_step(self.h, C.byref(hyper), B, _ptr(real), _ptr(noise_D), _ptr(noise_G), _ptr(masks_D),
                                           _ptr(masks_G), seed, C.byref(st) if st is not None else None), "fg_s16_train_step")
-        if st is None:
-            return None
-        return dict(loss_D=st.loss_D, loss_G=st.loss_G, conf=list(st.conf), trained_D=st.trained_D, t_D=st.t_D, t_G=st.t_G,
-                    acc_D=st.acc_D)
+        return _stats(st)
 
     def train_step_dataset(self, dataset, hyper, B, seed, want_stats=True):
         """train_step with the 16x16 real half and the noise drawn on the device from a DeviceDataset of this ctx
@@ -771,7 +697,4 @@ class S16:
         st = StepStats() if want_stats else None
         _check(self.lib.fg_s16_train_step_dataset(self.h, dataset.h, C.byref(hyper), B, seed,
                                                   C.byref(st) if st is not None else None), "fg_s16_train_step_dataset")
-        if st is None:
-            return None
-        return dict(loss_D=st.loss_D, loss_G=st.loss_G, conf=list(st.conf), trained_D=st.trained_D, t_D=st.t_D, t_G=st.t_G,
-                    acc_D=st.acc_D)
+        return _stats(st)
