@@ -183,6 +183,16 @@ int fg_set_option(fg_ctx* c, const char* key, int64_t v) {
     c->dp_overlap = v != 0;
     return FG_OK;
   }
+  if (!strcmp(key, "bwd_merge")) {  // see fg_ctx::bwd_merge
+    FG_REQUIRE(v >= 0 && v <= 2, "bwd_merge must be 0 (two launches), 1 (merged where it is faster) or 2 (merged where possible)");
+    c->bwd_merge = (int)v;
+    return FG_OK;
+  }
+  if (!strcmp(key, "bwd_merge_ctas")) {
+    FG_REQUIRE(v >= 0, "bwd_merge_ctas must be >= 0 (0: one CTA per SM)");
+    c->bwd_merge_ctas = v > (1 << 20) ? (1 << 20) : (int)v;
+    return FG_OK;
+  }
   if (!strcmp(key, "debug_keep")) {  // keep the D step's pre-activations of fg_train_step ("Dstep.*" debug tensors)
     c->debug_keep = v != 0;
     return FG_OK;
@@ -217,6 +227,8 @@ int64_t fg_get_option(fg_ctx* c, const char* key) {
   if (!strcmp(key, "mma_f16")) return c->mma_f16;
   if (!strcmp(key, "dp_overlap")) return c->dp_overlap;
   if (!strcmp(key, "use_graph")) return c->use_graph;
+  if (!strcmp(key, "bwd_merge")) return c->bwd_merge;
+  if (!strcmp(key, "bwd_merge_ctas")) return c->bwd_merge_ctas;
   if (!strcmp(key, "optimizer_D")) return c->opt_D;
   if (!strcmp(key, "optimizer_G")) return c->opt_G;
   return -1;

@@ -194,6 +194,12 @@ struct fg_ctx {
   // stream already runs the G step's G forward (which only needs G's parameters); joined before D is used again
   int dp_overlap = 1;
   int reserve_sms = 0;  // SMs the persistent convolution kernels leave free while a collective runs next to them
+  // option "bwd_merge": the weight and data gradients of G's upsampled layers run as one persistent launch
+  // (k_conv_tc.cu tc_conv_bwd_ups).  1 (default): where its schedule estimate beats two launches (tc_bwd_pair_pays:
+  // G.C2 at batch 256, not G.C1); 2: wherever the shapes allow it; 0: two launches.  Option "bwd_merge_ctas"
+  // (0 = one per SM) caps the CTAs of the merged launch.
+  int bwd_merge = 1, bwd_merge_ctas = 0;
+  int* bwd_claim = nullptr;  // the work-item counter of the merged launch
   // option "use_graph" (default 1): fg_train_step replays a captured CUDA graph of the step (launch overhead of ~200
   // kernels); keyed on everything a captured step bakes in, the seed is read from device memory
   int use_graph = 1, graph_epoch = 0;

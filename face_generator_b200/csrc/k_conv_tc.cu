@@ -24,6 +24,9 @@
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
+#include <queue>
+#include <vector>
 
 #include "fg_internal.h"
 #include "k_conv_tc.h"
@@ -434,6 +437,9 @@ constexpr size_t fwd_smem() { return (size_t)kStages * (2 * kABytes + 2 * BN * 1
 // F16: 3 TMA stages; TF32: 2 TMA stages + the K-major copy of one (same bytes per stage)
 template <int BN>
 constexpr size_t wg_smem() { return (size_t)3 * (2 * 4 * 4096 + 2 * (BN / 32) * 4096) + 128 + 1024; }
+// 3 stages, then {full, empty}[3] and the id-slot ring (full, empty, ids) of bwd_pair_tc_kernel
+template <int BN>
+constexpr size_t bwd_smem() { return (size_t)kStages * fwd_stage_bytes<BN>() + 256 + 1024; }
 
 
 // ------------------------------------------------------------------------------------------------
@@ -521,6 +527,7 @@ int tc_init(fg_ctx* c) {
   FG_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg_smem<128>()));
   FG_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg_smem<64>()));
   FG_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg_smem<128>()));
+  FG_CUDA(cudaFuncSetAttribute(bwd_pair_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem<128>()));
   return FG_OK;
 }
 void tc_destroy(fg_ctx* c) { (void)c; }
@@ -757,12 +764,12 @@ int tc_conv_fwd(fg_ctx* c, const float* x_hi, const float* x_lo, const float* w_
   return launch_tapconv(c, p, BN, f16);
 }
 
+
 // dgrad of an up2+5x5 conv straight to the LOW-RES input gradient (the 2x2 sum of the upsample backward is
 // implicit: all 4 output phases accumulate into the same accumulator).  dy_hi/lo: [B][H][W][Cout] full-res;
 // wd_hi/lo: collapsed dgrad pack [36][Cin][Cout]; out: [B][H/2][W/2][Cin].
-int tc_conv_dgrad_ups(fg_ctx* c, const float* dy_hi, const float* dy_lo, const float* wd_hi, const float* wd_lo,
-                      float* out, ConvGeom g, int f16, const float* oscale) {
-  TcFwdParams p;
+static int dgrad_ups_params(const float* dy_hi, const float* dy_lo, const float* wd_hi, const float* wd_lo, float* out,
+                            ConvGeom g, int f16, const float* oscale, TcFwdParams& p, int* BN_out) {
   memset(&p, 0, sizeof(p));
   const int Hl = g.H / 2, Wl = g.W / 2;
   if (!pick_box(Hl, Wl, 128, &p.bw, &p.bh, &p.bb)) return FG_ERR_UNSUPPORTED;
@@ -805,14 +812,30 @@ int tc_conv_dgrad_ups(fg_ctx* c, const float* dy_hi, const float* dy_lo, const f
   p.out_scale = 1;
   p.ntiles = p.tiles_per_phase * (g.Cin / BN);
   p.chunk = tc_chunk(true);
+  *BN_out = BN;
+  return FG_OK;
+}
+int tc_conv_dgrad_ups(fg_ctx* c, const float* dy_hi, const float* dy_lo, const float* wd_hi, const float* wd_lo,
+                      float* out, ConvGeom g, int f16, const float* oscale) {
+  TcFwdParams p;
+  int BN;
+  FG_TRY(dgrad_ups_params(dy_hi, dy_lo, wd_hi, wd_lo, out, g, f16, oscale, p, &BN));
   return launch_tapconv(c, p, BN, f16);
+}
+
+// K splits of a weight gradient: about one wave of `base` CTAs per split
+static int wgrad_splits(const fg_ctx* c, int base, int kblocks) {
+  const int splits = std::min(std::max(1, c->sm_count / base), kblocks);
+  const int per = (kblocks + splits - 1) / splits;
+  return (kblocks + per - 1) / per;
 }
 
 // wgrad.  x_hi/lo: [B][H/ups][W/ups][Cin]; dy_hi/lo: [B][H][W][Cout]; out (overwritten):
 //   ups==1: [k*k][Cout][Cin]          ups==2: collapsed [36][Cout][Cin]
-int tc_conv_wgrad(fg_ctx* c, const float* x_hi, const float* x_lo, const float* dy_hi, const float* dy_lo, float* out,
-                  ConvGeom g, int f16, const float* oscale, const float* oscale2) {
-  TcWgParams p;
+// Fills p for `splits` K splits; the caller sets p.out / p.split_stride.  *ntt_out: tile-taps, *BN_out: Cin tile.
+static int wgrad_params(fg_ctx* c, const float* x_hi, const float* x_lo, const float* dy_hi, const float* dy_lo, ConvGeom g,
+                        int f16, const float* oscale, const float* oscale2, TcWgParams& p, int* BN_out, int* ntt_out,
+                        int* splits_out) {
   memset(&p, 0, sizeof(p));
   const int Hl = g.H / g.ups, Wl = g.W / g.ups;
   const bool h = f16 != 0;
@@ -862,28 +885,107 @@ int tc_conv_wgrad(fg_ctx* c, const float* x_hi, const float* x_lo, const float* 
   p.tiles_x = Wl / p.bw;
   p.tiles_y = Hl / p.bh;
   p.kblocks = p.bb == 1 ? g.B * p.tiles_x * p.tiles_y : (g.B + p.bb - 1) / p.bb;
-  const int base = ntt * (g.Cout / 128) * (g.Cin / BN);
-  int splits = std::max(1, c->sm_count / base);
-  if (splits > p.kblocks) splits = p.kblocks;
+  const int splits = wgrad_splits(c, ntt * (g.Cout / 128) * (g.Cin / BN), p.kblocks);
   p.kb_per_split = (p.kblocks + splits - 1) / splits;
-  splits = (p.kblocks + p.kb_per_split - 1) / p.kb_per_split;
-  const int64_t size = (int64_t)ntt * g.Cout * g.Cin;
-  p.out = splits > 1 ? c->splitk_ws : out;  // splits x base CTAs <= one per SM: fits splitk_ws
-  p.split_stride = size;
   p.oscale = oscale ? oscale : oscale2;
   p.oscale2 = oscale ? oscale2 : nullptr;
   p.chunk = tc_chunk() == 4 && !getenv("FG_TC_CHUNK") ? ((int64_t)g.H * g.W > 1 ? 8 : 4) : tc_chunk();  // wgrad of convolutions 8, of Linear layers 4
   if (h) p.chunk = std::max(1, p.chunk / 2);  // an fp16 K block holds 64 pixels
+  *BN_out = BN;
+  *ntt_out = ntt;
+  *splits_out = splits;
+  return FG_OK;
+}
+int tc_conv_wgrad(fg_ctx* c, const float* x_hi, const float* x_lo, const float* dy_hi, const float* dy_lo, float* out,
+                  ConvGeom g, int f16, const float* oscale, const float* oscale2) {
+  TcWgParams p;
+  int BN, ntt, splits;
+  FG_TRY(wgrad_params(c, x_hi, x_lo, dy_hi, dy_lo, g, f16, oscale, oscale2, p, &BN, &ntt, &splits));
+  const int64_t size = (int64_t)ntt * g.Cout * g.Cin;
+  p.out = splits > 1 ? c->splitk_ws : out;  // splits x base CTAs <= one per SM: fits splitk_ws
+  p.split_stride = size;
   if (splits * size > (int64_t)c->splitk_ws_elems) {
     fg_set_error("tc_conv_wgrad: %d splits of %lld elements exceed the split-K workspace", splits, (long long)size);
     return FG_ERR_UNSUPPORTED;
   }
   dim3 grid(ntt, (g.Cout / 128) * (g.Cin / BN), splits);
-  if (h) {
+  if (f16) {
     if (BN == 128) wgrad_tc_kernel<128, true><<<grid, kTcThreads, wg_smem<128>(), c->stream>>>(p);
     else wgrad_tc_kernel<64, true><<<grid, kTcThreads, wg_smem<64>(), c->stream>>>(p);
   } else if (BN == 128) wgrad_tc_kernel<128><<<grid, kTcThreads, wg_smem<128>(), c->stream>>>(p);
   else wgrad_tc_kernel<64><<<grid, kTcThreads, wg_smem<64>(), c->stream>>>(p);
   LAUNCH_CHECK(c);
   return splits > 1 ? k_splitk_reduce(c, c->splitk_ws, splits, size, out) : FG_OK;
+}
+
+// The merged launch covers the shapes where both halves run BN = 128 tiles and the weight gradient is not split
+// (fewer than two waves of its items fit on the GPU), so that every item is the unsplit tile of today's kernels.
+bool tc_bwd_pair_eligible(const fg_ctx* c, const ConvGeom& g) {
+  int bw, bh, bb;
+  const int Hl = g.H / 2, Wl = g.W / 2;
+  if (g.ups != 2 || g.k != 5 || g.Cin % 128 || g.Cout % 128) return false;
+  if (!pick_box(Hl, Wl, 128, &bw, &bh, &bb) || !pick_box(Hl, Wl, 64, &bw, &bh, &bb)) return false;
+  const int kblocks = bb == 1 ? g.B * (Wl / bw) * (Hl / bh) : (g.B + bb - 1) / bb;
+  return wgrad_splits(c, 36 * (g.Cout / 128) * (g.Cin / 128), kblocks) == 1;
+}
+
+static int bwd_pair_ctas(const fg_ctx* c, int nitems) {
+  int ctas = std::min(nitems, std::max(1, c->sm_count - c->reserve_sms));
+  return c->bwd_merge_ctas > 0 ? std::min(ctas, c->bwd_merge_ctas) : ctas;
+}
+
+// Does the merged launch finish sooner than the two launches?  Both schedules in K-block times: two launches = the
+// weight-gradient wave, then the dgrad tiles in waves; merged = the items handed out longest first to the CTA that
+// frees up first.  The merged estimate must win by 5 %: next to each other the two kinds share the L2 bandwidth that
+// the weight gradient had to itself (G.C1 at batch 256 ties at 400 K-block times and measured 5 % slower merged).
+bool tc_bwd_pair_pays(const fg_ctx* c, const ConvGeom& g) {
+  if (!tc_bwd_pair_eligible(c, g)) return false;
+  int bw, bh, bb, tw, th, tb;
+  const int Hl = g.H / 2, Wl = g.W / 2;
+  pick_box(Hl, Wl, 64, &bw, &bh, &bb);
+  pick_box(Hl, Wl, 128, &tw, &th, &tb);
+  const int64_t wlen = bb == 1 ? g.B * (Wl / bw) * (Hl / bh) : (g.B + bb - 1) / bb;  // K blocks of a wgrad item
+  const int64_t dlen = 36 * (g.Cout / 64);                                             // K blocks of a dgrad tile
+  const int nwg = 36 * (g.Cout / 128) * (g.Cin / 128);
+  const int ntiles = (tb == 1 ? g.B * (Wl / tw) * (Hl / th) : (g.B + tb - 1) / tb) * (g.Cin / 128);
+  const int sms = std::max(1, c->sm_count - c->reserve_sms);
+  const int64_t two = wlen + (int64_t)((ntiles + sms - 1) / sms) * dlen;
+  std::priority_queue<int64_t, std::vector<int64_t>, std::greater<int64_t>> free_at;  // when each CTA frees up
+  for (int i = 0, n = bwd_pair_ctas(c, nwg + ntiles); i < n; ++i) free_at.push(0);
+  int64_t merged = 0;
+  for (int id = 0; id < nwg + ntiles; ++id) {
+    const int64_t end = free_at.top() + (id < nwg ? wlen : dlen);
+    free_at.pop();
+    free_at.push(end);
+    merged = std::max(merged, end);
+  }
+  return merged * 20 < two * 19;
+}
+
+int tc_conv_bwd_ups(fg_ctx* c, const float* x_hi, const float* x_lo, const float* dy_hi, const float* dy_lo,
+                    const float* wd_hi, const float* wd_lo, float* wg_out, float* dh, ConvGeom g, const float* oscale_dy,
+                    const float* oscale_x) {
+  if (!tc_bwd_pair_eligible(c, g)) {
+    fg_set_error("tc_conv_bwd_ups: no merged backward for Cin %d, Cout %d at %dx%d, batch %d", g.Cin, g.Cout, g.H, g.W, g.B);
+    return FG_ERR_UNSUPPORTED;
+  }
+  TcBwdParams p;
+  memset(&p, 0, sizeof(p));
+  int wBN, ntt, splits, dBN;
+  FG_TRY(wgrad_params(c, x_hi, x_lo, dy_hi, dy_lo, g, 1, oscale_dy, oscale_x, p.wg, &wBN, &ntt, &splits));
+  FG_TRY(dgrad_ups_params(dy_hi, dy_lo, wd_hi, wd_lo, dh, g, 1, oscale_dy, p.dg, &dBN));
+  if (wBN != 128 || dBN != 128 || splits != 1) {
+    fg_set_error("tc_conv_bwd_ups: unexpected tiling (wgrad BN %d, %d splits, dgrad BN %d)", wBN, splits, dBN);
+    return FG_ERR_UNSUPPORTED;
+  }
+  p.wg.out = wg_out;
+  p.wg.split_stride = 0;
+  p.claim = c->bwd_claim;
+  p.nwg = ntt * (g.Cout / 128) * (g.Cin / 128);
+  p.nitems = p.nwg + p.dg.ntiles;
+  const int ctas = bwd_pair_ctas(c, p.nitems);
+  FG_CUDA(cudaMemsetAsync(c->bwd_claim, 0, sizeof(int), c->stream));  // part of a captured step: reset on every replay
+  bwd_pair_tc_kernel<128><<<ctas, kTcThreads, bwd_smem<128>(), c->stream>>>(p);
+  LAUNCH_CHECK(c);
+  return FG_OK;
 }

@@ -39,6 +39,14 @@ struct alignas(64) TcWgParams {
   int chunk;
 };
 
+// weight gradient + data gradient of one upsampled 5x5 layer in one persistent launch (bwd_pair_tc_kernel)
+struct alignas(64) TcBwdParams {
+  TcWgParams wg;
+  TcFwdParams dg;
+  int* claim;      // device counter of claimed work items, zeroed before every launch
+  int nwg, nitems;  // ids [0, nwg): weight-gradient items, [nwg, nitems): dgrad tiles
+};
+
 bool tc_conv_eligible(const ConvGeom& g);
 int tc_split(fg_ctx* c, const float* x, float* hi, float* lo, int64_t n);
 int tc_pack_split(fg_ctx* c, const float* W, float* f_hi, float* f_lo, float* d_hi, float* d_lo, int N, int Cc, int KK);
@@ -63,5 +71,13 @@ int tc_pack_split_h(fg_ctx* c, const float* W, float* f_hi, float* f_lo, float* 
 int tc_pack_collapsed_h(fg_ctx* c, const float* W, float* f_hi, float* f_lo, float* d_hi, float* d_lo, int N, int Cc);
 int tc_conv_wgrad(fg_ctx* c, const float* x_hi, const float* x_lo, const float* dy_hi, const float* dy_lo, float* out,
                   ConvGeom g, int f16 = 0, const float* oscale = nullptr, const float* oscale2 = nullptr);
+// tc_conv_wgrad (into the collapsed [36][Cout][Cin] `wg_out`) and tc_conv_dgrad_ups (into `dh`) of an upsampled 5x5
+// layer on the 3xFP16 split, as one launch of bwd_pair_tc_kernel with the same per-tile arithmetic, so the same bits.
+// Only for the shapes tc_bwd_pair_eligible accepts.  oscale_dy / oscale_x: inverse operand scales as for the two calls.
+bool tc_bwd_pair_eligible(const fg_ctx* c, const ConvGeom& g);
+bool tc_bwd_pair_pays(const fg_ctx* c, const ConvGeom& g);  // eligible, and its schedule estimate beats two launches
+int tc_conv_bwd_ups(fg_ctx* c, const float* x_hi, const float* x_lo, const float* dy_hi, const float* dy_lo,
+                    const float* wd_hi, const float* wd_lo, float* wg_out, float* dh, ConvGeom g, const float* oscale_dy,
+                    const float* oscale_x);
 int tc_tf32_peak(fg_ctx* c, int iters, int reps, double* tflops);
 int tc_encode_nhwc_box(CUtensorMap* m, const float* base, int C, int W, int H, int B, int bc, int bw, int bh, int bb);

@@ -94,12 +94,143 @@ __device__ __forceinline__ FwdTile fwd_decode(const TcFwdParams& p, int tile) {
 
 // ------------------------------------------------------------------------------------------------
 // tapconv: forward / dgrad.  Persistent: CTA i handles tiles i, i+gridDim.x, ...
+// The producer and consumer sides of one tile are device functions, shared with bwd_pair_tc_kernel; `kbg` is the
+// running K-block counter of the CTA's stage ring (stage kbg % kStages, phase kbg / kStages), carried across tiles.
 // ------------------------------------------------------------------------------------------------
+template <int BN>
+constexpr uint32_t fwd_stage_bytes() { return 2 * kABytes + 2 * BN * 128; }  // {a_hi, a_lo, b_hi, b_lo}
+
+template <int BN, bool F16>
+__device__ __forceinline__ void tapconv_load_tile(const TcFwdParams& p, int tile, uint8_t* smem, uint64_t* full,
+                                                  uint64_t* empty, uint32_t& kbg) {
+  constexpr uint32_t kBBytes = BN * 128;
+  constexpr uint32_t kStageBytes = fwd_stage_bytes<BN>();
+  constexpr int kKE = F16 ? 64 : 32;  // K elements of one 128-byte K block
+  const int nkb = p.ntaps * p.kpt;
+  const FwdTile t = fwd_decode<BN>(p, tile);
+  for (int kb = 0; kb < nkb; ++kb, ++kbg) {
+    const uint32_t s = kbg % kStages, it = kbg / kStages;
+    if (it > 0) mbar_wait_spin(empty + s, (it - 1) & 1);
+    const int tap = kb / p.kpt, c0 = (kb - tap * p.kpt) * kKE;
+    const int ti = t.ph * p.ntaps + tap;
+    const int am = p.amap[ti];
+    uint8_t* st = smem + s * kStageBytes;
+    mbar_expect_tx(full + s, kStageBytes);
+    tma_load_4d(st, &p.a_hi[am], full + s, c0, t.x0 + p.dx[ti], t.y0 + p.dy[ti], t.b0);
+    tma_load_4d(st + kABytes, &p.a_lo[am], full + s, c0, t.x0 + p.dx[ti], t.y0 + p.dy[ti], t.b0);
+    const int wrow = p.widx[ti] * p.Cout + t.n0;
+    tma_load_2d(st + 2 * kABytes, &p.b_hi, full + s, c0, wrow);
+    tma_load_2d(st + 2 * kABytes + kBBytes, &p.b_lo, full + s, c0, wrow);
+  }
+}
+
+// consumers: warpgroup wg owns accumulator rows [64 wg, 64 wg + 64) == tile pixels
+template <int BN, bool F16>
+__device__ __forceinline__ void tapconv_mma_tile(const TcFwdParams& p, int tile, uint8_t* smem, uint64_t* full,
+                                                 uint64_t* empty, float* stat_sm, uint32_t& kbg) {
+  constexpr uint32_t kBBytes = BN * 128;
+  constexpr uint32_t kStageBytes = fwd_stage_bytes<BN>();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = warp >> 2, g = lane >> 2, tq = lane & 3;
+  const uint32_t aoff = (uint32_t)wg * 64 * 128;  // the warpgroup's 64 rows of the A tile
+  const int nkb = p.ntaps * p.kpt;
+  const int kChunk = p.chunk;
+  const int nchunks = (nkb + kChunk - 1) / kChunk;
+  int rowpix[2];
+  for (int h = 0; h < 2; ++h) rowpix[h] = wg * 64 + (warp & 3) * 16 + g + 8 * h;
+  float acc[BN];
+  const FwdTile t = fwd_decode<BN>(p, tile);
+  float o[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) o[i] = 0.f;
+  for (int ch = 0; ch < nchunks; ++ch) {
+    const int nk = min(kChunk, nkb - ch * kChunk);
+    int prev = -1;
+    for (int j = 0; j < nk; ++j, ++kbg) {
+      const uint32_t s = kbg % kStages, it = kbg / kStages;
+      const uint32_t sa = smem_u32(smem + s * kStageBytes);
+      mbar_wait(full + s, it & 1);
+      mma_kblock<BN, F16, false>(acc, make_desc(sa + aoff, 16, 1024), make_desc(sa + kABytes + aoff, 16, 1024),
+                                 make_desc(sa + 2 * kABytes, 16, 1024), make_desc(sa + 2 * kABytes + kBBytes, 16, 1024),
+                                 2, j == 0);  // +32 bytes per K slice
+      wgmma_wait<1>();  // the previous block's group has read its stage
+      if (prev >= 0 && lane == 0) mbar_arrive(empty + prev);
+      prev = (int)s;
+    }
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(empty + prev);
+    promote<BN, F16>(o, acc);
+  }
+  if (p.oscale) {  // operands stored scaled by powers of two (FP16 split): undo it
+    const float os = *p.oscale * (p.oscale2 ? *p.oscale2 : 1.f);
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) o[i] *= os;
+  }
+  // fragment element i = 4 j + 2 h + e: row rowpix[h], column 8 j + 2 tq + e
+  int b[2];
+  float* orow[2];
+  for (int h = 0; h < 2; ++h) {
+    const int m = rowpix[h];
+    const int xi = m % p.bw, yi = (m / p.bw) % p.bh, bi = m / (p.bw * p.bh);
+    b[h] = t.b0 + bi;
+    const int Y = p.out_scale * (t.y0 + yi) + (t.ph >> 1) * (p.out_scale - 1);
+    const int X = p.out_scale * (t.x0 + xi) + (t.ph & 1) * (p.out_scale - 1);
+    orow[h] = p.out + (((int64_t)b[h] * p.out_H + Y) * p.out_W + X) * p.Cout + t.n0 + 2 * tq;
+  }
+  if (p.bias) {
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) o[i] += p.bias[t.n0 + 8 * (i >> 2) + 2 * tq + (i & 1)];
+  }
+  if (p.stats) {
+    // BatchNorm statistics from the convolution epilogue (nn.SpatialBatchNormalization, models.lua:65,70): per
+    // tile the column sums of z and z^2 over its (valid) 128 pixels.  Each warp reduces its 16 rows with shuffles,
+    // the 8 warps meet in shared memory and one thread per column writes the tile's partial.  Every sum has a fixed
+    // order => replicas stay identical.
+    const bool v0 = b[0] < p.B, v1 = b[1] < p.B;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float z0 = v0 ? o[4 * j + e] : 0.f, z1 = v1 ? o[4 * j + 2 + e] : 0.f;
+        float x = z0 + z1, y = z0 * z0 + z1 * z1;
+#pragma unroll
+        for (int sft = 4; sft < 32; sft <<= 1) {
+          x += __shfl_xor_sync(0xffffffffu, x, sft);
+          y += __shfl_xor_sync(0xffffffffu, y, sft);
+        }
+        if (g == 0) {
+          stat_sm[(0 * 8 + warp) * BN + 8 * j + 2 * tq + e] = x;
+          stat_sm[(1 * 8 + warp) * BN + 8 * j + 2 * tq + e] = y;
+        }
+      }
+    }
+    consumer_sync();
+    const int et = threadIdx.x;
+    if (et < BN) {
+      float s0 = 0.f, s1 = 0.f;
+      for (int w = 0; w < 8; ++w) {
+        s0 += stat_sm[(0 * 8 + w) * BN + et];
+        s1 += stat_sm[(1 * 8 + w) * BN + et];
+      }
+      const int mt = tile / (p.Cout / BN);
+      p.stats[((int64_t)mt * 2 + 0) * p.Cout + t.n0 + et] = s0;
+      p.stats[((int64_t)mt * 2 + 1) * p.Cout + t.n0 + et] = s1;
+    }
+    consumer_sync();
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (b[h] < p.B) {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+        *reinterpret_cast<float2*>(orow[h] + 8 * j) = make_float2(o[4 * j + 2 * h], o[4 * j + 2 * h + 1]);
+    }
+  }
+}
+
 template <int BN, bool F16 = false>
 __global__ void __launch_bounds__(kTcThreads, 1) tapconv_tc_kernel(const __grid_constant__ TcFwdParams p) {
-  constexpr uint32_t kBBytes = BN * 128;
-  constexpr uint32_t kStageBytes = 2 * kABytes + 2 * kBBytes;  // {a_hi, a_lo, b_hi, b_lo}
-  constexpr int kKE = F16 ? 64 : 32;                           // K elements of one 128-byte K block
+  constexpr uint32_t kStageBytes = fwd_stage_bytes<BN>();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
@@ -107,9 +238,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) tapconv_tc_kernel(const __grid_
   float* stat_sm = reinterpret_cast<float*>(smem + kStages * kStageBytes + 256);  // [2][8 warps][BN] (p.stats only)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nkb = p.ntaps * p.kpt;
-  const int kChunk = p.chunk;
-  const int nchunks = (nkb + kChunk - 1) / kChunk;
   const int ntiles = p.ntiles;
 
   if (threadIdx.x == 0) {
@@ -127,124 +255,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) tapconv_tc_kernel(const __grid_
       prefetch_tmap(&p.b_hi);
       prefetch_tmap(&p.b_lo);
       uint32_t kbg = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const FwdTile t = fwd_decode<BN>(p, tile);
-        for (int kb = 0; kb < nkb; ++kb, ++kbg) {
-          const uint32_t s = kbg % kStages, it = kbg / kStages;
-          if (it > 0) mbar_wait_spin(empty + s, (it - 1) & 1);
-          const int tap = kb / p.kpt, c0 = (kb - tap * p.kpt) * kKE;
-          const int ti = t.ph * p.ntaps + tap;
-          const int am = p.amap[ti];
-          uint8_t* st = smem + s * kStageBytes;
-          mbar_expect_tx(full + s, kStageBytes);
-          tma_load_4d(st, &p.a_hi[am], full + s, c0, t.x0 + p.dx[ti], t.y0 + p.dy[ti], t.b0);
-          tma_load_4d(st + kABytes, &p.a_lo[am], full + s, c0, t.x0 + p.dx[ti], t.y0 + p.dy[ti], t.b0);
-          const int wrow = p.widx[ti] * p.Cout + t.n0;
-          tma_load_2d(st + 2 * kABytes, &p.b_hi, full + s, c0, wrow);
-          tma_load_2d(st + 2 * kABytes + kBBytes, &p.b_lo, full + s, c0, wrow);
-        }
-      }
+      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) tapconv_load_tile<BN, F16>(p, tile, smem, full, empty, kbg);
     }
     return;
   }
 
-  // ---- consumers: warpgroup wg owns accumulator rows [64 wg, 64 wg + 64) == tile pixels ----
   consumer_regs();
-  const int wg = warp >> 2, g = lane >> 2, tq = lane & 3;
-  const uint32_t aoff = (uint32_t)wg * 64 * 128;  // the warpgroup's 64 rows of the A tile
-  int rowpix[2];
-  for (int h = 0; h < 2; ++h) rowpix[h] = wg * 64 + (warp & 3) * 16 + g + 8 * h;
   uint32_t kbg = 0;
-  float acc[BN];
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const FwdTile t = fwd_decode<BN>(p, tile);
-    float o[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) o[i] = 0.f;
-    for (int ch = 0; ch < nchunks; ++ch) {
-      const int nk = min(kChunk, nkb - ch * kChunk);
-      int prev = -1;
-      for (int j = 0; j < nk; ++j, ++kbg) {
-        const uint32_t s = kbg % kStages, it = kbg / kStages;
-        const uint32_t sa = smem_u32(smem + s * kStageBytes);
-        mbar_wait(full + s, it & 1);
-        mma_kblock<BN, F16, false>(acc, make_desc(sa + aoff, 16, 1024), make_desc(sa + kABytes + aoff, 16, 1024),
-                                   make_desc(sa + 2 * kABytes, 16, 1024), make_desc(sa + 2 * kABytes + kBBytes, 16, 1024),
-                                   2, j == 0);  // +32 bytes per K slice
-        wgmma_wait<1>();  // the previous block's group has read its stage
-        if (prev >= 0 && lane == 0) mbar_arrive(empty + prev);
-        prev = (int)s;
-      }
-      wgmma_wait<0>();
-      if (lane == 0) mbar_arrive(empty + prev);
-      promote<BN, F16>(o, acc);
-    }
-    if (p.oscale) {  // operands stored scaled by powers of two (FP16 split): undo it
-      const float os = *p.oscale * (p.oscale2 ? *p.oscale2 : 1.f);
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) o[i] *= os;
-    }
-    // fragment element i = 4 j + 2 h + e: row rowpix[h], column 8 j + 2 tq + e
-    int b[2];
-    float* orow[2];
-    for (int h = 0; h < 2; ++h) {
-      const int m = rowpix[h];
-      const int xi = m % p.bw, yi = (m / p.bw) % p.bh, bi = m / (p.bw * p.bh);
-      b[h] = t.b0 + bi;
-      const int Y = p.out_scale * (t.y0 + yi) + (t.ph >> 1) * (p.out_scale - 1);
-      const int X = p.out_scale * (t.x0 + xi) + (t.ph & 1) * (p.out_scale - 1);
-      orow[h] = p.out + (((int64_t)b[h] * p.out_H + Y) * p.out_W + X) * p.Cout + t.n0 + 2 * tq;
-    }
-    if (p.bias) {
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) o[i] += p.bias[t.n0 + 8 * (i >> 2) + 2 * tq + (i & 1)];
-    }
-    if (p.stats) {
-      // BatchNorm statistics from the convolution epilogue (nn.SpatialBatchNormalization, models.lua:65,70): per
-      // tile the column sums of z and z^2 over its (valid) 128 pixels.  Each warp reduces its 16 rows with shuffles,
-      // the 8 warps meet in shared memory and one thread per column writes the tile's partial.  Every sum has a fixed
-      // order => replicas stay identical.
-      const bool v0 = b[0] < p.B, v1 = b[1] < p.B;
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const float z0 = v0 ? o[4 * j + e] : 0.f, z1 = v1 ? o[4 * j + 2 + e] : 0.f;
-          float x = z0 + z1, y = z0 * z0 + z1 * z1;
-#pragma unroll
-          for (int sft = 4; sft < 32; sft <<= 1) {
-            x += __shfl_xor_sync(0xffffffffu, x, sft);
-            y += __shfl_xor_sync(0xffffffffu, y, sft);
-          }
-          if (g == 0) {
-            stat_sm[(0 * 8 + warp) * BN + 8 * j + 2 * tq + e] = x;
-            stat_sm[(1 * 8 + warp) * BN + 8 * j + 2 * tq + e] = y;
-          }
-        }
-      }
-      consumer_sync();
-      const int et = threadIdx.x;
-      if (et < BN) {
-        float s0 = 0.f, s1 = 0.f;
-        for (int w = 0; w < 8; ++w) {
-          s0 += stat_sm[(0 * 8 + w) * BN + et];
-          s1 += stat_sm[(1 * 8 + w) * BN + et];
-        }
-        const int mt = tile / (p.Cout / BN);
-        p.stats[((int64_t)mt * 2 + 0) * p.Cout + t.n0 + et] = s0;
-        p.stats[((int64_t)mt * 2 + 1) * p.Cout + t.n0 + et] = s1;
-      }
-      consumer_sync();
-    }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      if (b[h] < p.B) {
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j)
-          *reinterpret_cast<float2*>(orow[h] + 8 * j) = make_float2(o[4 * j + 2 * h], o[4 * j + 2 * h + 1]);
-      }
-    }
-  }
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) tapconv_mma_tile<BN, F16>(p, tile, smem, full, empty, stat_sm, kbg);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -278,86 +296,89 @@ __device__ __forceinline__ void transpose_block(const uint8_t* src, uint8_t* dst
   }
 }
 
-template <int BN, bool F16 = false>
-__global__ void __launch_bounds__(kTcThreads, 1) wgrad_tc_kernel(const __grid_constant__ TcWgParams p) {
-  constexpr int kS = wg_stages<F16>();
-  constexpr int kG = F16 ? 64 : 32;                  // channels per 128-byte group
-  constexpr uint32_t kBox = (F16 ? 64 : 32) * 128;   // one (group x K-block pixels) box: 32 px (tf32) / 64 px (fp16)
-  constexpr uint32_t kAB = (128 / kG) * kBox;        // M = 128 channels of dY
-  constexpr uint32_t kBB = (BN / kG) * kBox;
-  constexpr uint32_t kStageBytes = 2 * kAB + 2 * kBB;  // {dy_hi, dy_lo, x_hi, x_lo}
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* kbuf = smem + kS * kStageBytes;  // tf32: the K-major copy of one stage
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (kS + (F16 ? 0 : 1)) * kStageBytes);
-  uint64_t* empty = full + kS;
+template <int BN, bool F16>
+struct WgLayout {
+  static constexpr int kS = wg_stages<F16>();
+  static constexpr int kG = F16 ? 64 : 32;                  // channels per 128-byte group
+  static constexpr uint32_t kBox = (F16 ? 64 : 32) * 128;   // one (group x K-block pixels) box: 32 px (tf32) / 64 px (fp16)
+  static constexpr uint32_t kAB = (128 / kG) * kBox;        // M = 128 channels of dY
+  static constexpr uint32_t kBB = (BN / kG) * kBox;
+  static constexpr uint32_t kStageBytes = 2 * kAB + 2 * kBB;  // {dy_hi, dy_lo, x_hi, x_lo}
+};
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tt = blockIdx.x;
+// one weight-gradient work item: tile-tap tt, output block [m0, m0 + 128) x [c0, c0 + BN), K blocks
+// [kb_begin, kb_begin + nkb) of split z
+struct WgItem {
+  int tt, m0, c0, z, kb_begin, nkb;
+};
+template <int BN>
+__device__ __forceinline__ WgItem wg_decode(const TcWgParams& p, int tt, int mn, int z) {
   const int ntn = p.Cin / BN;
-  const int m0 = (blockIdx.y / ntn) * 128, c0 = (blockIdx.y % ntn) * BN;
-  const int kb_begin = blockIdx.z * p.kb_per_split;
-  const int kb_end = min(p.kblocks, kb_begin + p.kb_per_split);
-  const int nkb = kb_end - kb_begin;
+  WgItem w;
+  w.tt = tt;
+  w.m0 = (mn / ntn) * 128;
+  w.c0 = (mn % ntn) * BN;
+  w.z = z;
+  w.kb_begin = z * p.kb_per_split;
+  w.nkb = min(p.kblocks, w.kb_begin + p.kb_per_split) - w.kb_begin;
+  return w;
+}
+
+// producer side of one item (kbg: the running K-block counter of the stage ring, as in tapconv_load_tile)
+template <int BN, bool F16>
+__device__ __forceinline__ void wgrad_load_item(const TcWgParams& p, const WgItem& w, uint8_t* smem, uint64_t* full,
+                                                uint64_t* empty, uint32_t& kbg) {
+  using L = WgLayout<BN, F16>;
+  const int ph = p.phase[w.tt], dyo = p.dy[w.tt], dxo = p.dx[w.tt];
+  for (int i = 0; i < w.nkb; ++i, ++kbg) {
+    const int s = kbg % L::kS, it = kbg / L::kS;
+    if (it > 0) mbar_wait_spin(empty + s, (it - 1) & 1);
+    const int kb = w.kb_begin + i;
+    int b0, y0, x0;
+    if (p.bb == 1) {
+      const int per_img = p.tiles_x * p.tiles_y;
+      b0 = kb / per_img;
+      const int r = kb % per_img;
+      y0 = (r / p.tiles_x) * p.bh;
+      x0 = (r % p.tiles_x) * p.bw;
+    } else {
+      b0 = kb * p.bb;
+      y0 = 0;
+      x0 = 0;
+    }
+    uint8_t* st = smem + s * L::kStageBytes;
+    mbar_expect_tx(full + s, L::kStageBytes);
+    // 5-D maps (group channels, w, h, b, channel-group): ONE bulk copy lands [group][pixel][group channels] = all
+    // the boxes of an operand
+    tma_load_5d(st, &p.dy_hi[ph], full + s, 0, x0, y0, b0, w.m0 / L::kG);
+    tma_load_5d(st + L::kAB, &p.dy_lo[ph], full + s, 0, x0, y0, b0, w.m0 / L::kG);
+    tma_load_5d(st + 2 * L::kAB, &p.x_hi, full + s, 0, x0 + dxo, y0 + dyo, b0, w.c0 / L::kG);
+    tma_load_5d(st + 2 * L::kAB + L::kBB, &p.x_lo, full + s, 0, x0 + dxo, y0 + dyo, b0, w.c0 / L::kG);
+  }
+}
+
+// consumer side of one item: the K loop, the promotions and the store of the [n][c] block
+template <int BN, bool F16>
+__device__ __forceinline__ void wgrad_mma_item(const TcWgParams& p, const WgItem& w, uint8_t* smem, uint64_t* full,
+                                               uint64_t* empty, uint32_t& kbg) {
+  using L = WgLayout<BN, F16>;
+  constexpr uint32_t kBox = L::kBox, kAB = L::kAB, kBB = L::kBB;
+  uint8_t* kbuf = smem + L::kS * L::kStageBytes;  // tf32: the K-major copy of one stage
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = warp >> 2, g = lane >> 2, tq = lane & 3;
+  const int nkb = w.nkb;
   const int kChunk = p.chunk;
   const int nchunks = (nkb + kChunk - 1) / kChunk;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kS; ++s) {
-      mbar_init(full + s, 1);
-      mbar_init(empty + s, kConsumerThreads / 32);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (nkb <= 0) return;
-
-  if (warp >= kConsumerThreads / 32) {
-    producer_regs();
-    if (warp == kConsumerThreads / 32 && lane == 0) {
-      const int ph = p.phase[tt], dyo = p.dy[tt], dxo = p.dx[tt];
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % kS, it = i / kS;
-        if (it > 0) mbar_wait_spin(empty + s, (it - 1) & 1);
-        const int kb = kb_begin + i;
-        int b0, y0, x0;
-        if (p.bb == 1) {
-          const int per_img = p.tiles_x * p.tiles_y;
-          b0 = kb / per_img;
-          const int r = kb % per_img;
-          y0 = (r / p.tiles_x) * p.bh;
-          x0 = (r % p.tiles_x) * p.bw;
-        } else {
-          b0 = kb * p.bb;
-          y0 = 0;
-          x0 = 0;
-        }
-        uint8_t* st = smem + s * kStageBytes;
-        mbar_expect_tx(full + s, kStageBytes);
-        // 5-D maps (group channels, w, h, b, channel-group): ONE bulk copy lands [group][pixel][group channels] = all
-        // the boxes of an operand
-        tma_load_5d(st, &p.dy_hi[ph], full + s, 0, x0, y0, b0, m0 / kG);
-        tma_load_5d(st + kAB, &p.dy_lo[ph], full + s, 0, x0, y0, b0, m0 / kG);
-        tma_load_5d(st + 2 * kAB, &p.x_hi, full + s, 0, x0 + dxo, y0 + dyo, b0, c0 / kG);
-        tma_load_5d(st + 2 * kAB + kBB, &p.x_lo, full + s, 0, x0 + dxo, y0 + dyo, b0, c0 / kG);
-      }
-    }
-    return;
-  }
-
-  consumer_regs();
-  const int wg = warp >> 2, g = lane >> 2, tq = lane & 3;
   float acc[BN];
   float o[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) o[i] = 0.f;
-  int i = 0;
   for (int ch = 0; ch < nchunks; ++ch) {
     const int nk = min(kChunk, nkb - ch * kChunk);
     int prev = -1;
-    for (int j = 0; j < nk; ++j, ++i) {
-      const int s = i % kS, it = i / kS;
-      const uint32_t sa = smem_u32(smem + s * kStageBytes);
+    for (int j = 0; j < nk; ++j, ++kbg) {
+      const int s = kbg % L::kS, it = kbg / L::kS;
+      const uint32_t sa = smem_u32(smem + s * L::kStageBytes);
       mbar_wait(full + s, it & 1);
       if constexpr (F16) {
         // canonical MN-major SWIZZLE_128B layout: atoms of 64 channels x 8 pixels (1 KB), LBO = distance between
@@ -369,7 +390,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) wgrad_tc_kernel(const __grid_co
         if (prev >= 0 && lane == 0) mbar_arrive(empty + prev);
         prev = s;
       } else {
-        const uint8_t* st = smem + s * kStageBytes;
+        const uint8_t* st = smem + s * L::kStageBytes;
         transpose_block(st, kbuf, 128, threadIdx.x);                        // dy_hi -> rows [0, 128)
         transpose_block(st + kAB, kbuf + 128 * 128, 128, threadIdx.x);      // dy_lo -> rows [128, 256)
         transpose_block(st + 2 * kAB, kbuf + 256 * 128, BN, threadIdx.x);   // x_hi -> rows [256, 256 + BN)
@@ -398,12 +419,116 @@ __global__ void __launch_bounds__(kTcThreads, 1) wgrad_tc_kernel(const __grid_co
   }
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int n = m0 + wg * 64 + (warp & 3) * 16 + g + 8 * h;
-    float* orow = p.out + blockIdx.z * p.split_stride + ((int64_t)tt * p.Cout + n) * p.Cin + c0 + 2 * tq;
+    const int n = w.m0 + wg * 64 + (warp & 3) * 16 + g + 8 * h;
+    float* orow = p.out + w.z * p.split_stride + ((int64_t)w.tt * p.Cout + n) * p.Cin + w.c0 + 2 * tq;
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
       orow[8 * j] = o[4 * j + 2 * h];
       orow[8 * j + 1] = o[4 * j + 2 * h + 1];
     }
+  }
+}
+
+template <int BN, bool F16 = false>
+__global__ void __launch_bounds__(kTcThreads, 1) wgrad_tc_kernel(const __grid_constant__ TcWgParams p) {
+  using L = WgLayout<BN, F16>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (L::kS + (F16 ? 0 : 1)) * L::kStageBytes);
+  uint64_t* empty = full + L::kS;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const WgItem w = wg_decode<BN>(p, blockIdx.x, blockIdx.y, blockIdx.z);
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < L::kS; ++s) {
+      mbar_init(full + s, 1);
+      mbar_init(empty + s, kConsumerThreads / 32);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  if (w.nkb <= 0) return;
+
+  uint32_t kbg = 0;
+  if (warp >= kConsumerThreads / 32) {
+    producer_regs();
+    if (warp == kConsumerThreads / 32 && lane == 0) wgrad_load_item<BN, F16>(p, w, smem, full, empty, kbg);
+    return;
+  }
+  consumer_regs();
+  wgrad_mma_item<BN, F16>(p, w, smem, full, empty, kbg);
+}
+
+// ------------------------------------------------------------------------------------------------
+// bwd_pair: the weight gradient AND the data gradient of one upsampled 5x5 layer (3xFP16, collapsed) in one
+// persistent launch.  Work item ids [0, nwg) are unsplit weight-gradient items (tile-tap, Cout tile, Cin tile; the
+// whole K range), [nwg, nitems) the dgrad tiles of tc_conv_dgrad_ups: the long items go out first and the short
+// tiles fill in around them.  The producer lane claims the next id from a device counter and hands it to the
+// consumers through a small ring of id slots with its own full / empty mbarriers.  Both kinds use the same 64 KB
+// stages, so the stage ring runs on across items of either kind and the producer loads the next item while the
+// consumers run the current one's epilogue.  Each item runs the body of its own kernel: its result is bit for bit
+// what the two separate launches write.
+// ------------------------------------------------------------------------------------------------
+constexpr int kIdSlots = 2;
+
+template <int BN>
+__global__ void __launch_bounds__(kTcThreads, 1) bwd_pair_tc_kernel(const __grid_constant__ TcBwdParams p) {
+  using L = WgLayout<BN, true>;
+  static_assert(L::kS == kStages && L::kStageBytes == fwd_stage_bytes<BN>(), "one stage ring for both item kinds");
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * L::kStageBytes);
+  uint64_t* empty = full + kStages;
+  uint64_t* id_full = empty + kStages;
+  uint64_t* id_empty = id_full + kIdSlots;
+  volatile int* ids = reinterpret_cast<volatile int*>(id_empty + kIdSlots);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nmn = (p.wg.Cout / 128) * (p.wg.Cin / BN);  // weight-gradient output blocks per tile-tap
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(full + s, 1);
+      mbar_init(empty + s, kConsumerThreads / 32);
+    }
+    for (int s = 0; s < kIdSlots; ++s) {
+      mbar_init(id_full + s, 1);
+      mbar_init(id_empty + s, kConsumerThreads / 32);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  uint32_t kbg = 0;
+  if (warp >= kConsumerThreads / 32) {
+    producer_regs();
+    if (warp == kConsumerThreads / 32 && lane == 0) {
+      prefetch_tmap(&p.dg.b_hi);
+      prefetch_tmap(&p.dg.b_lo);
+      for (uint32_t n = 0;; ++n) {
+        const uint32_t slot = n % kIdSlots, use = n / kIdSlots;
+        if (use > 0) mbar_wait_spin(id_empty + slot, (use - 1) & 1);
+        const int id = atomicAdd(p.claim, 1);
+        ids[slot] = id;
+        mbar_arrive(id_full + slot);  // release: the consumers' wait on id_full acquires the id
+        if (id >= p.nitems) break;
+        if (id < p.nwg) wgrad_load_item<BN, true>(p.wg, wg_decode<BN>(p.wg, id / nmn, id % nmn, 0), smem, full, empty, kbg);
+        else tapconv_load_tile<BN, true>(p.dg, id - p.nwg, smem, full, empty, kbg);
+      }
+    }
+    return;
+  }
+
+  consumer_regs();
+  for (uint32_t n = 0;; ++n) {
+    const uint32_t slot = n % kIdSlots, use = n / kIdSlots;
+    mbar_wait(id_full + slot, use & 1);
+    const int id = ids[slot];
+    __syncwarp();
+    if (lane == 0) mbar_arrive(id_empty + slot);
+    if (id >= p.nitems) break;
+    if (id < p.nwg) wgrad_mma_item<BN, true>(p.wg, wg_decode<BN>(p.wg, id / nmn, id % nmn, 0), smem, full, empty, kbg);
+    else tapconv_mma_tile<BN, true>(p.dg, id - p.nwg, smem, full, empty, nullptr, kbg);
   }
 }

@@ -97,6 +97,7 @@ int net_alloc(fg_ctx* c) {
   FG_TRY(dalloc(c, reinterpret_cast<float**>(&c->red_ws), 2 * c->red_ws_elems));
   FG_TRY(dalloc(c, reinterpret_cast<float**>(&c->red_ws_opt), 2 * kOptRedRows));
   FG_TRY(dalloc(c, reinterpret_cast<float**>(&c->red_ticket), 2));  // zeroed; every ordered reduction resets its ticket
+  FG_TRY(dalloc(c, reinterpret_cast<float**>(&c->bwd_claim), 1));
   FG_TRY(dalloc(c, &c->small_ws, (size_t)kSmallMaxParts * 9 * 4 * 128));
   // G activations
   FG_TRY(dalloc(c, &c->G_noise, B * kNoiseDim));
@@ -434,9 +435,11 @@ static int g_ups_fwd(fg_ctx* c, int li, const char* tag, const float* h, float* 
 // backward of the same layer: dW += wgrad, dh = dgrad.  *pooled tells whether `dh` already is the gradient of
 // the LOW-RES input (tensor-core path: the 2x2 sum of the upsample backward is folded into the dgrad GEMM) or the
 // full-resolution gradient that the consumer still has to sum 2x2 (SIMT path).
-static int g_ups_bwd(fg_ctx* c, int li, const char* wtag, const char* dtag, const float* h, const float* h_hi,
-                     const float* h_lo, const float* dz, const float* Wpd, ConvGeom g, float* dW, float* dh, bool* pooled,
-                     const float* dz_f32 = nullptr, int dz_amax = -1) {
+// 3xFP16 path with option bwd_merge: wgrad and dgrad run as ONE persistent launch, timed as `btag` (G.C2's weight
+// gradient leaves 60 of 132 SMs idle for its whole duration, the dgrad tiles fill them; same bits as two launches).
+static int g_ups_bwd(fg_ctx* c, int li, const char* wtag, const char* dtag, const char* btag, const float* h,
+                     const float* h_hi, const float* h_lo, const float* dz, const float* Wpd, ConvGeom g, float* dW,
+                     float* dh, bool* pooled, const float* dz_f32 = nullptr, int dz_amax = -1) {
   if (!use_tc_wgrad(c, g)) {
     FG_TRY(conv_wgrad(c, wtag, h, dz, g, dW, 0, 0, 0, 0));
     *pooled = false;
@@ -445,13 +448,22 @@ static int g_ups_bwd(fg_ctx* c, int li, const char* wtag, const char* dtag, cons
   fg_ctx::TcBufs& t = c->tcb;
   if (f16_on(c) && dz_f32) {  // weight and data gradient on the FP16 split of the (scaled) gradient
     FG_TRY(split_h_scaled(c, dz_f32, t.dy_hh, t.dy_hl, (int64_t)g.B * g.H * g.W * g.Cout, kSlotDy, dz_amax));
+    *pooled = true;
+    if (c->bwd_merge == 2 ? tc_bwd_pair_eligible(c, g) : c->bwd_merge == 1 && tc_bwd_pair_pays(c, g)) {
+      {
+        ScopedTimer tm(c, btag);
+        FG_TRY(tc_conv_bwd_ups(c, li == 0 ? t.G_h0_hh : t.G_h1_hh, li == 0 ? t.G_h0_hl : t.G_h1_hl, t.dy_hh, t.dy_hl,
+                               t.G_Wd_hh[li], t.G_Wd_hl[li], c->wgrad_ws, dh, g, inv_scale(c, kSlotDy),
+                               inv_scale(c, li == 0 ? kSlotH0 : kSlotH1)));
+      }
+      return tc_combine_collapsed_wgrad(c, c->wgrad_ws, dW, g.Cout, g.Cin);
+    }
     {
       ScopedTimer tm(c, wtag);
       FG_TRY(tc_conv_wgrad(c, li == 0 ? t.G_h0_hh : t.G_h1_hh, li == 0 ? t.G_h0_hl : t.G_h1_hl, t.dy_hh, t.dy_hl, c->wgrad_ws, g, 1,
                            inv_scale(c, kSlotDy), inv_scale(c, li == 0 ? kSlotH0 : kSlotH1)));
     }
     FG_TRY(tc_combine_collapsed_wgrad(c, c->wgrad_ws, dW, g.Cout, g.Cin));
-    *pooled = true;
     ScopedTimer tm(c, dtag);
     return tc_conv_dgrad_ups(c, t.dy_hh, t.dy_hl, t.G_Wd_hh[li], t.G_Wd_hl[li], dh, g, 1, inv_scale(c, kSlotDy));
   }
@@ -586,7 +598,7 @@ int net_G_backward(fg_ctx* c, const float* dy, float* dnoise) {
   }
   // C2
   bool pooled = false;
-  FG_TRY(g_ups_bwd(c, 1, "G.C2.wgrad", "G.C2.dgrad", c->G_h1, c->tcb.G_h1_hi, c->tcb.G_h1_lo, tc2 ? nullptr : c->G_dz2,
+  FG_TRY(g_ups_bwd(c, 1, "G.C2.wgrad", "G.C2.dgrad", "G.C2.wgrad+dgrad", c->G_h1, c->tcb.G_h1_hi, c->tcb.G_h1_lo, tc2 ? nullptr : c->G_dz2,
                    c->G_C2pd, gC2, G + L.C2W, c->G_dfull, &pooled, c->G_dz2, kSlotGdz + 2));
   // BN1 + PReLU (the 2x2 sum = backward of the nearest upsample is folded into the loads)
   FG_TRY(k_bn_prelu_bwd_reduce(c, c->G_dfull, c->G_z1, c->bn_mean1, c->bn_istd1, P + L.g1, P + L.be1, P + L.a2, c->bn_acc,
@@ -600,7 +612,7 @@ int net_G_backward(fg_ctx* c, const float* dy, float* dnoise) {
                                 split1 ? c->tcb.dy_lo : nullptr, G + L.C1b));
   }
   // C1
-  FG_TRY(g_ups_bwd(c, 0, "G.C1.wgrad", "G.C1.dgrad", c->G_h0, c->tcb.G_h0_hi, c->tcb.G_h0_lo, split1 ? nullptr : c->G_dz1,
+  FG_TRY(g_ups_bwd(c, 0, "G.C1.wgrad", "G.C1.dgrad", "G.C1.wgrad+dgrad", c->G_h0, c->tcb.G_h0_hi, c->tcb.G_h0_lo, split1 ? nullptr : c->G_dz1,
                    c->G_C1pd,
                    ConvGeom{B, 16, 16, 128, 256, 5, 2}, G + L.C1W, c->G_dfull, &pooled, c->G_dz1, kSlotGdz + 1));
   {
