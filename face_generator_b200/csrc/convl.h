@@ -1,50 +1,35 @@
-// One convolution / Linear layer of the nets built outside nets.cu (coarse-to-fine nets, --scale 16 nets): weight
-// packs, TF32 splits and the forward / backward dispatch over the wgmma, bandwidth-shaped and fp32 FFMA kernels.
+// Layer-level dispatch of the layer types in fg_internal.h (TcOp, ConvL, UpsL, ConvLEnv): weight packs, tensor-core
+// operand splits and the forward / backward dispatch over the wgmma, bandwidth-shaped and fp32 FFMA kernels.  ConvL
+// serves the coarse-to-fine and --scale 16 nets; UpsL serves G's upsampled layers of the 32x32 and --scale 16 generators.
 #pragma once
 #include <vector>
 
 #include "fg_internal.h"
 
-struct ConvL {  // NHWC, stride 1, "same" padding (a strided layer runs at stride 1 and is subsampled by its net)
-  int Cin = 0, Cout = 0, k = 1, H = 1;
-  int64_t w_off = 0, b_off = 0;
-  int cA = 0, cS = 0;  // Linear after View([C][H][W]): column j=c*S+s of the reference <-> our NHWC column s*A+c
-  int nA = 0, nS = 0;  // Linear before View([C][H][W]): the same permutation on the output rows (weights, bias, gradients)
-  float *Wp = nullptr, *Wpd = nullptr;                                            // fp32 packs [t][n][c], [t'][c][n]
-  float* bp = nullptr;                                                            // bias in our row order (nA != 0)
-  float *Wf_hi = nullptr, *Wf_lo = nullptr, *Wd_hi = nullptr, *Wd_lo = nullptr;   // TF32 splits of the packs
-  float *x_hi = nullptr, *x_lo = nullptr;                                         // split of the input (fwd -> wgrad)
-  float* sx = nullptr;       // device (max|x|, 1/scale) of the input's FP16 split (option mma_f16)
-  bool packed_f16 = false;   // the hi/lo buffers currently hold the FP16 split (set by convl_pack)
-  // Layers whose output side is too narrow for a tensor-core tile still run there with zero-padded channels:
-  //   pad_out (Cout <= 4, e.g. the 256->C 7x7 output layer): forward with the weights padded to pad_out rows;
-  //           wgrad with the roles swapped (big channel count on the 128-row M side, padded dY on the N side)
-  //   pad_dy  (Cout == 64): wgrad with dY padded to the 128 rows the M side needs
-  int pad_out = 0, pad_dy = 0;
-  float *Wq_hi = nullptr, *Wq_lo = nullptr;  // [t][pad_out][Cin] TF32 hi/lo
-  bool need_dgrad = true;
-  const char *tf = "", *td = "", *tw = "";
-  ConvGeom geom(int B) const { return ConvGeom{B, H, H, Cin, Cout, k, 1}; }
-  ConvGeom geom_d(int B) const { return ConvGeom{B, H, H, Cout, Cin, k, 1}; }
-};
+// option "mma_f16": tensor-core operands in the 3xFP16 split (only with the phase-collapsed kernels)
+inline bool tc_f16(const fg_ctx* c) { return c->mma_f16 && c->conv_impl == FG_CONV_TC_COLLAPSED; }
 
-// what a layer needs from the net that owns it: the allocation list and the shared scratch buffers
-struct ConvLEnv {
-  fg_ctx* c = nullptr;
-  int maxB = 0;
-  std::vector<void*>* allocs = nullptr;
-  float *ga = nullptr;                          // padded forward output (pad_out layers): maxB * H*H * pad_out floats
-  float *dy_hi = nullptr, *dy_lo = nullptr;     // TF32 split of the current dY (largest layer output)
-  float *pad_hi = nullptr, *pad_lo = nullptr;   // channel-padded TF32 split of dY (pad_out / pad_dy layers)
-  float* ws = nullptr;                          // packed weight-gradient workspace (largest layer)
-  float* sdy = nullptr;                         // device (max|dY|, 1/scale) of the current dY's FP16 split
-};
+// the split of x (n elements) into op, in the format `f16` chooses, minus whatever the producer already did
+int tc_op_split(fg_ctx* c, TcOp& op, const float* x, int64_t n, bool f16);
 
 // what the weight packs depend on besides the parameters: re-pack when it changes
 inline int pack_key(const fg_ctx* c) { return c->conv_impl | (c->mma_f16 << 4); }
 int convl_dalloc(ConvLEnv& e, float** p, size_t elems);  // zero-filled device buffer, owned by *e.allocs
 int convl_alloc(ConvLEnv& e, ConvL& L);
+bool convl_tc_fwd(const fg_ctx* c, const ConvL& L);  // the forward runs on the tensor cores (it reads the input's split)
+bool convl_tc_bwd(const fg_ctx* c, const ConvL& L);  // ... and so does the data gradient
 int convl_pack(fg_ctx* c, ConvL& L, const float* P);
 int convl_fwd(ConvLEnv& e, ConvL& L, const float* in, const float* P, float* out, int B);
-// G (may be null): dW += wgrad, db += colsum(dy).  din (may be null) = dgrad.
+// G (may be null): dW += wgrad, db += colsum(dy).  din (may be null) = dgrad.  The flags of e.dy say what dY's producer
+// already did (split into e.dy, max|dY| into L.sdy, bias gradient added); they are cleared.
 int convl_bwd(ConvLEnv& e, ConvL& L, const float* in, const float* dy, float* G, float* din, int B);
+
+bool upsl_tc(const fg_ctx* c, const UpsL& U);  // the layer runs on the tensor cores
+int upsl_alloc(ConvLEnv& e, UpsL& U);
+int upsl_pack(fg_ctx* c, UpsL& U, const float* P);
+// *parts (optional, in: want BatchNorm partials; out: how many tiles wrote one into c->bn_parts, 0 = none)
+int upsl_fwd(ConvLEnv& e, UpsL& U, const float* h, const float* P, float* z, int B, int* parts = nullptr);
+// G: dW += wgrad (the bias gradient is the producer's: k_bn_prelu_bwd_apply's dbias); dh = dgrad; dy: the operand dz is
+// split into.  *pooled: dh already is the gradient of the LOW-RES input (the tensor-core dgrad folds in the 2x2 sum of
+// the upsample backward); otherwise dh is the full-resolution gradient the consumer still sums 2x2.
+int upsl_bwd(ConvLEnv& e, UpsL& U, TcOp& dy, const float* h, const float* dz, float* G, float* dh, int B, bool* pooled);

@@ -110,6 +110,69 @@ struct NetPair {
   const char* optim_timer[2] = {nullptr, nullptr};  // ScopedTimer names of the G / D optimizer update (none: untimed)
 };
 
+// ---- layer types (dispatch in convl.cu) ------------------------------------------------------------------
+// One tensor-core operand: the hi/lo split of a tensor and its device (max|x|, 1/scale) pair.  Each buffer is sized for
+// the 3xTF32 split; the 3xFP16 split uses its first half.  A producer kernel that already did part of the work says so:
+//   split_ready  it wrote the TF32 split into hi/lo (3xTF32 path)
+//   amax_ready   it reduced max|x| into s[0] (3xFP16 path; AmaxInto in nets.cu)
+//   bias_ready   it added the bias gradient (the column sums of a dY) into the gradient (ConvLEnv::dy only)
+// The consuming layer then skips that pass and clears the flag.
+struct TcOp {
+  float *hi = nullptr, *lo = nullptr;
+  float* s = nullptr;
+  bool split_ready = false, amax_ready = false, bias_ready = false;
+};
+struct ConvL {  // NHWC, stride 1, "same" padding (a strided layer runs at stride 1 and is subsampled by its net)
+  int Cin = 0, Cout = 0, k = 1, H = 1;
+  int64_t w_off = 0, b_off = 0;
+  int cA = 0, cS = 0;  // Linear after View([C][H][W]): column j=c*S+s of the reference <-> our NHWC column s*A+c
+  int nA = 0, nS = 0;  // Linear before View([C][H][W]): the same permutation on the output rows (weights, bias, gradients)
+  float *Wp = nullptr, *Wpd = nullptr;                                            // fp32 packs [t][n][c], [t'][c][n]
+  float* bp = nullptr;                                                            // bias in our row order (nA != 0)
+  float *Wf_hi = nullptr, *Wf_lo = nullptr, *Wd_hi = nullptr, *Wd_lo = nullptr;   // TF32 splits of the packs
+  TcOp x;                    // split of the input (fwd -> wgrad); x.s may be set before convl_alloc
+  float* sdy = nullptr;      // (max|dY|, 1/scale) of this layer's dY split; nullptr: the shared ConvLEnv::dy.s
+  // kpad (Linear only): K zero-padded Cin -> kpad so that the layer runs on the tensor cores (xpad: [B][kpad] input,
+  // Wpad: [Cout][kpad] weights, both with zero pad columns); its weight gradient needs Cout * (kpad + Cin) floats of ws
+  int kpad = 0;
+  float *xpad = nullptr, *Wpad = nullptr;
+  bool packed_f16 = false;   // the hi/lo buffers currently hold the FP16 split (set by convl_pack)
+  // Layers whose output side is too narrow for a tensor-core tile still run there with zero-padded channels:
+  //   pad_out (Cout <= 4, e.g. the 256->C 7x7 output layer): forward with the weights padded to pad_out rows;
+  //           wgrad with the roles swapped (big channel count on the 128-row M side, padded dY on the N side)
+  //   pad_dy  (Cout == 64): wgrad with dY padded to the 128 rows the M side needs
+  int pad_out = 0, pad_dy = 0;
+  float *Wq_hi = nullptr, *Wq_lo = nullptr;  // [t][pad_out][Cin] TF32 hi/lo
+  bool need_dgrad = true;
+  const char *tf = "", *td = "", *tw = "";
+  ConvGeom geom(int B) const { return ConvGeom{B, H, H, Cin, Cout, k, 1}; }
+  ConvGeom geom_k(int B) const { return ConvGeom{B, H, H, kpad ? kpad : Cin, Cout, k, 1}; }  // the tensor-core shape
+  ConvGeom geom_d(int B) const { return ConvGeom{B, H, H, Cout, Cin, k, 1}; }
+};
+
+struct UpsL {  // nn.SpatialUpSamplingNearest(2) -> 5x5 "same" convolution; H = output side
+  int Cin = 0, Cout = 0, H = 0;
+  int64_t w_off = 0, b_off = 0;
+  float *Wp = nullptr, *Wpd = nullptr;                                            // fp32 tap-major packs (FFMA path)
+  float *Wf_hi = nullptr, *Wf_lo = nullptr, *Wd_hi = nullptr, *Wd_lo = nullptr;   // phase-collapsed packs [36][..][..]
+  float *Wx_hi = nullptr, *Wx_lo = nullptr;                                       // dense forward pack [25][n][c] (conv_impl 1)
+  TcOp x;  // split of the low-res input (fwd -> wgrad); x.s may be set before upsl_alloc to keep the pair elsewhere
+  // tb: timer of the merged weight-and-data-gradient launch (tc_conv_bwd_ups, option bwd_merge); nullptr: never merged
+  const char *tf = "", *td = "", *tw = "", *tb = nullptr;
+  ConvGeom geom(int B) const { return ConvGeom{B, H, H, Cin, Cout, 5, 2}; }
+};
+
+// what a layer needs from the net that owns it: the allocation list and the shared scratch buffers
+struct ConvLEnv {
+  fg_ctx* c = nullptr;
+  int maxB = 0;
+  std::vector<void*>* allocs = nullptr;
+  float *ga = nullptr;  // padded forward output (pad_out layers): maxB * H*H * pad_out floats
+  TcOp dy;              // split of the current dY (largest layer output); dy.s: (max|dY|, 1/scale) of its FP16 split
+  TcOp pad;             // channel-padded split of dY (pad_out / pad_dy layers); scaled by dy.s
+  float* ws = nullptr;  // packed weight-gradient workspace (largest layer)
+};
+
 struct TimerRec {
   double ms = 0;
   int64_t launches = 0;
@@ -135,10 +198,6 @@ struct fg_ctx {
   float *ownPG = nullptr, *ownPD = nullptr, *ownGG = nullptr, *ownGD = nullptr;
   float* tail_sep = nullptr;
   // packed weights (forward packs [tap][n][c], dgrad packs [tap'][c][n])
-  float *G_L1p = nullptr, *G_L1pd = nullptr, *G_C1p = nullptr, *G_C1pd = nullptr, *G_C2p = nullptr, *G_C2pd = nullptr,
-        *G_C3p = nullptr, *G_C3pd = nullptr;
-  float *D_cp[4] = {nullptr, nullptr, nullptr, nullptr}, *D_cpd[4] = {nullptr, nullptr, nullptr, nullptr};
-  float *D_L1p = nullptr, *D_L1pd = nullptr, *D_L2pd = nullptr, *D_L3pd = nullptr;
   float* small_ws = nullptr;  // per-block partials of the small-channel wgrad (k_conv_small.cu)
   float* wgrad_ws = nullptr;  // packed weight-gradient workspace (largest layer)
   size_t wgrad_ws_elems = 0;
@@ -164,8 +223,7 @@ struct fg_ctx {
   int mma_f16 = 1;            // option "mma_f16": 1 (default) = tensor-core operands in the 3xFP16 split (f16 MMAs); 0 = 3xTF32
   float* amax_slot = nullptr; // [32] (max|x|, 1/scale) pairs on the device: power-of-two scales of the FP16-split operands
   unsigned* amax_out = nullptr;  // when set (nets.cu AmaxInto), the next elementwise producer also reduces max|output| there ...
-  int amax_id = 0;               // ... and marks amax_valid[amax_id]: split_h_scaled then skips its own reduction pass
-  bool amax_valid[32] = {};
+  bool* amax_done = nullptr;     // ... and sets *amax_done (a TcOp's amax_ready): its consumer skips its own reduction
   double* bn_acc = nullptr;  // [4][256] double accumulators (sum, sumsq / sum g, sum g xhat)
   float *bn_mean1 = nullptr, *bn_istd1 = nullptr, *bn_mean2 = nullptr, *bn_istd2 = nullptr, *bn_mg = nullptr;
   float *G_dz3 = nullptr, *G_dfull = nullptr, *G_dz2 = nullptr, *G_dz1 = nullptr, *G_dz0 = nullptr;
@@ -215,33 +273,12 @@ struct fg_ctx {
   cudaEvent_t events[16] = {};
   bool timing = false;
   std::map<std::string, TimerRec> timers;
-  // tensor-core path: TF32 hi/lo splits of activations / gradients / packed weights (k_conv_tc.cu)
-  struct TcBufs {
-    float *G_h0_hi = nullptr, *G_h0_lo = nullptr, *G_h1_hi = nullptr, *G_h1_lo = nullptr;  // conv inputs (fwd -> wgrad)
-    // G.L1 (nn.Linear 100 -> 8192, models.lua:59) as a 1x1 convolution with K padded 100 -> 128: zero-padded noise
-    // [B][128] and its split, packed weights [8192'][128] (rows permuted for the View) and their split
-    float *G_xpad = nullptr, *G_x_hi = nullptr, *G_x_lo = nullptr, *G_L1pad = nullptr, *G_L1w_hi = nullptr, *G_L1w_lo = nullptr;
-    float *dy_hi = nullptr, *dy_lo = nullptr;                                             // current dY (dgrad + wgrad)
-    float *G_Wf_hi[2] = {nullptr, nullptr}, *G_Wf_lo[2] = {nullptr, nullptr};  // C1,C2 collapsed fwd [36][n][c]
-    float *G_Wd_hi[2] = {nullptr, nullptr}, *G_Wd_lo[2] = {nullptr, nullptr};  // collapsed dgrad [36][c][n]
-    float *G_Wx_hi[2] = {nullptr, nullptr}, *G_Wx_lo[2] = {nullptr, nullptr};  // dense fwd [25][n][c]
-    float *D_p_hi[3] = {nullptr, nullptr, nullptr}, *D_p_lo[3] = {nullptr, nullptr, nullptr};  // pooled inputs of c2..c4
-    float *D_Wf_hi[4] = {nullptr, nullptr, nullptr, nullptr}, *D_Wf_lo[4] = {nullptr, nullptr, nullptr, nullptr};
-    float *D_Wd_hi[4] = {nullptr, nullptr, nullptr, nullptr}, *D_Wd_lo[4] = {nullptr, nullptr, nullptr, nullptr};
-    // D's Linear layers: [0] L1 fwd [512][2048'], [1] L1 dgrad [2048'][512], [2] L2 fwd, [3] L2 dgrad
-    float *D_Lw_hi[4] = {nullptr, nullptr, nullptr, nullptr}, *D_Lw_lo[4] = {nullptr, nullptr, nullptr, nullptr};
-    float *D_lin_hi[2] = {nullptr, nullptr}, *D_lin_lo[2] = {nullptr, nullptr};  // splits of p4 / hl1 kept for wgrad
-    // 3xFP16 split twins (option mma_f16) of the K-major operands: n halves = n/2 floats per buffer
-    float *G_h0_hh = nullptr, *G_h0_hl = nullptr, *G_h1_hh = nullptr, *G_h1_hl = nullptr, *dy_hh = nullptr, *dy_hl = nullptr;
-    float *G_Wf_hh[2] = {nullptr, nullptr}, *G_Wf_hl[2] = {nullptr, nullptr}, *G_Wd_hh[2] = {nullptr, nullptr},
-          *G_Wd_hl[2] = {nullptr, nullptr};
-    float *D_p_hh[3] = {nullptr, nullptr, nullptr}, *D_p_hl[3] = {nullptr, nullptr, nullptr};
-    float *D_Wf_hh[4] = {nullptr, nullptr, nullptr, nullptr}, *D_Wf_hl[4] = {nullptr, nullptr, nullptr, nullptr};
-    float *D_Wd_hh[4] = {nullptr, nullptr, nullptr, nullptr}, *D_Wd_hl[4] = {nullptr, nullptr, nullptr, nullptr};
-    float *G_x_hh = nullptr, *G_x_hl = nullptr, *G_L1w_hh = nullptr, *G_L1w_hl = nullptr;
-    float *D_lin_hh[2] = {nullptr, nullptr}, *D_lin_hl[2] = {nullptr, nullptr};
-    float *D_Lw_hh[4] = {nullptr, nullptr, nullptr, nullptr}, *D_Lw_hl[4] = {nullptr, nullptr, nullptr, nullptr};
-  } tcb;
+  // the layers of G and D (D.L3 runs on the GEMV kernels) and the scratch they share: env.dy is the split of the current
+  // dY, env.ws = wgrad_ws.  Their FP16 scale pairs all live in amax_slot.
+  ConvLEnv env;
+  ConvL GL1, GC3, Dc[4], DL1, DL2;
+  UpsL GU[2];  // G.C1, G.C2
+  float* G_sdz[2] = {nullptr, nullptr};  // scale pairs of their dz (TcOp::s of the dz operand)
 };
 
 struct ScopedTimer {

@@ -52,10 +52,10 @@ __device__ __forceinline__ void amax_commit(unsigned* amax, float m) {
 __device__ __forceinline__ float amax4(float m, float a, float b, float c, float d) {
   return fmaxf(fmaxf(m, fmaxf(fabsf(a), fabsf(b))), fmaxf(fabsf(c), fabsf(d)));
 }
-// host side: the producer launched next reports into c->amax_out (set by nets.cu) and marks the slot valid
+// host side: the producer launched next reports into c->amax_out (set by nets.cu) and says so in *c->amax_done
 static inline unsigned* take_amax(fg_ctx* c) {
   unsigned* p = c->amax_out;
-  if (p) c->amax_valid[c->amax_id] = true;
+  if (p) *c->amax_done = true;
   return p;
 }
 

@@ -32,8 +32,7 @@ struct fg_c2f {
   float *D_x = nullptr, *D_cond = nullptr, *D_z[4] = {}, *D_h[4] = {}, *D_p2 = nullptr, *D_p4 = nullptr, *D_d4 = nullptr;
   float *D_zl1 = nullptr, *D_al1 = nullptr, *D_hl1 = nullptr, *D_logit = nullptr, *D_out = nullptr, *D_masks = nullptr,
         *D_dlogit = nullptr, *D_dx = nullptr;
-  float *ga = nullptr, *gb = nullptr, *dy_hi = nullptr, *dy_lo = nullptr, *ws = nullptr;
-  float *pad_hi = nullptr, *pad_lo = nullptr;  // channel-padded TF32 split of dY (ConvL::pad_out / pad_dy)
+  float *ga = nullptr, *gb = nullptr, *ws = nullptr;
   float *in_a = nullptr, *in_b = nullptr, *in_c = nullptr, *in_d = nullptr, *in_e = nullptr, *in_m1 = nullptr,
         *in_m2 = nullptr, *io = nullptr;
   int G_B = 0, D_B = 0;
@@ -136,13 +135,12 @@ int c2f_alloc(fg_c2f* n) {
   const size_t big = B * 1024 * 256;  // largest activation: G conv4 output
   FG_TRY(dalloc(n, &n->ga, big));
   FG_TRY(dalloc(n, &n->gb, big));
-  FG_TRY(dalloc(n, &n->dy_hi, big));
-  FG_TRY(dalloc(n, &n->dy_lo, big));
-  FG_TRY(dalloc(n, &n->pad_hi, big / 2));  // up to 128 padded channels at 32x32
-  FG_TRY(dalloc(n, &n->pad_lo, big / 2));
+  FG_TRY(dalloc(n, &n->env.dy.hi, big));
+  FG_TRY(dalloc(n, &n->env.dy.lo, big));
+  FG_TRY(dalloc(n, &n->env.pad.hi, big / 2));  // up to 128 padded channels at 32x32
+  FG_TRY(dalloc(n, &n->env.pad.lo, big / 2));
   FG_TRY(dalloc(n, &n->ws, std::max<size_t>((size_t)512 * 16384, (size_t)25 * 256 * 128)));
-  n->env.ga = n->ga; n->env.dy_hi = n->dy_hi; n->env.dy_lo = n->dy_lo;
-  n->env.pad_hi = n->pad_hi; n->env.pad_lo = n->pad_lo; n->env.ws = n->ws;
+  n->env.ga = n->ga; n->env.ws = n->ws;
   FG_TRY(dalloc(n, &n->in_a, B * 1024 * C));
   FG_TRY(dalloc(n, &n->in_b, B * 1024 * C));
   FG_TRY(dalloc(n, &n->in_c, B * 1024));

@@ -7,17 +7,15 @@
 //                       conv(512->1024,3,STRIDE 2) PReLU SpatialDropout() View(4096) Linear(4096,1024) PReLU
 //         dense branch: View(C*256) Linear(C*256,128) PReLU Dropout() Linear(128,128) PReLU
 //   loop = adversarial.lua:83-288 (the same fevalD / fevalG_on_D / accuracy gate / interruptable optimizers as the 32x32 nets)
-// Kernels: the two upsampled 5x5 layers use the phase-collapsed wgmma kernels of the 32x32 generator (forward with
-// BatchNorm partials from the epilogue, wgrad, dgrad with the upsample backward folded in); every other layer is a ConvL
-// (convl.h).  A stride-2 "same" 3x3 convolution is the stride-1 one sampled at the even pixels: forward = stride-1
-// kernel + subsample, backward = the stride-1 dgrad / wgrad of dY with zeros inserted at the odd pixels.  That is exact
-// (the inserted zeros contribute nothing) and keeps both layers on the tensor cores at 4x their minimal FLOPs, which
-// is 0.2 ms at batch 256.
+// Kernels: the two upsampled 5x5 layers are UpsL layers like the 32x32 generator's (forward with BatchNorm partials
+// from the epilogue, wgrad, dgrad with the upsample backward folded in); every other layer is a ConvL (convl.h).  A
+// stride-2 "same" 3x3 convolution is the stride-1 one sampled at the even pixels: forward = stride-1 kernel + subsample,
+// backward = the stride-1 dgrad / wgrad of dY with zeros inserted at the odd pixels.  That is exact (the inserted zeros
+// contribute nothing) and keeps both layers on the tensor cores at 4x their minimal FLOPs, which is 0.2 ms at batch 256.
 #include <algorithm>
 
 #include "convl.h"
 #include "fg_internal.h"
-#include "k_conv_tc.h"
 #include "k_misc.h"
 
 namespace {
@@ -105,17 +103,6 @@ __global__ void split2_kernel(const float* __restrict__ in, float* __restrict__ 
     if (j < Na) a[r * Na + j] = in[i]; else b[r * Nb + (j - Na)] = in[i];
   }
 }
-
-struct UpsL {  // nn.SpatialUpSamplingNearest(2) -> 5x5 "same" convolution; H = output side
-  int Cin = 0, Cout = 0, H = 0;
-  int64_t w_off = 0, b_off = 0;
-  float *Wp = nullptr, *Wpd = nullptr;                                            // fp32 tap-major packs (FFMA path)
-  float *Wf_hi = nullptr, *Wf_lo = nullptr, *Wd_hi = nullptr, *Wd_lo = nullptr;   // phase-collapsed TF32 packs [36][..][..]
-  float *h_hi = nullptr, *h_lo = nullptr;                                         // split of the low-res input (fwd -> wgrad)
-  float* sx = nullptr;                                                            // (max|h|, 1/scale) of its FP16 split
-  const char *tf = "", *td = "", *tw = "";
-  ConvGeom geom(int B) const { return ConvGeom{B, H, H, Cin, Cout, 5, 2}; }
-};
 }  // namespace
 
 struct fg_s16 {
@@ -138,7 +125,7 @@ struct fg_s16 {
         *D_joint = nullptr, *D_logit = nullptr, *D_out = nullptr, *D_masks = nullptr, *D_dlogit = nullptr, *D_dx = nullptr,
         *D_dx2 = nullptr, *D_djoint = nullptr, *D_dhf = nullptr, *D_dhe2 = nullptr;
   // shared scratch
-  float *ga = nullptr, *gb = nullptr, *dy_hi = nullptr, *dy_lo = nullptr, *ws = nullptr;
+  float *ga = nullptr, *gb = nullptr, *ws = nullptr;
   float *in_a = nullptr, *in_b = nullptr, *in_c = nullptr, *in_m1 = nullptr, *in_m2 = nullptr, *io = nullptr;
   int G_pack_impl = -1, D_pack_impl = -1;
   int G_B = 0, D_B = 0;
@@ -149,10 +136,6 @@ struct fg_s16 {
 
 namespace {
 int dalloc(fg_s16* n, float** p, size_t elems) { return convl_dalloc(n->env, p, elems); }
-inline bool use_tc(const fg_ctx* c, const ConvGeom& g) { return c->conv_impl != FG_CONV_SIMT && tc_conv_eligible(g); }
-inline bool use_tc_wgrad(const fg_ctx* c, const ConvGeom& g) { return use_tc(c, g) && g.Cout % 128 == 0 && g.Cin % 64 == 0; }
-// option "mma_f16": the upsampled layers' hi/lo buffers hold the 3xFP16 split (see convl.cu)
-inline bool f16_on(const fg_ctx* c) { return c->mma_f16 && c->conv_impl == FG_CONV_TC_COLLAPSED; }
 
 void make_layouts(fg_s16* n) {
   const int C = n->C;
@@ -236,20 +219,7 @@ int s16_alloc(fg_s16* n) {
   // ---- G ----
   FG_TRY(convl_alloc(n->env, n->GL1));
   FG_TRY(convl_alloc(n->env, n->GC3));
-  for (int i = 0; i < 2; ++i) {
-    UpsL& U = n->GU[i];
-    const size_t nw25 = (size_t)25 * U.Cout * U.Cin, nw36 = (size_t)36 * U.Cout * U.Cin;
-    FG_TRY(dalloc(n, &U.Wp, nw25));
-    FG_TRY(dalloc(n, &U.Wpd, nw25));
-    FG_TRY(dalloc(n, &U.Wf_hi, nw36));
-    FG_TRY(dalloc(n, &U.Wf_lo, nw36));
-    FG_TRY(dalloc(n, &U.Wd_hi, nw36));
-    FG_TRY(dalloc(n, &U.Wd_lo, nw36));
-    const size_t nx = B * (U.H / 2) * (U.H / 2) * U.Cin;
-    FG_TRY(dalloc(n, &U.h_hi, nx));
-    FG_TRY(dalloc(n, &U.h_lo, nx));
-    FG_TRY(dalloc(n, &U.sx, 2));
-  }
+  for (int i = 0; i < 2; ++i) FG_TRY(upsl_alloc(n->env, n->GU[i]));
   FG_TRY(dalloc(n, &n->G_x, B * 100));
   FG_TRY(dalloc(n, &n->G_z0, B * 2048));
   FG_TRY(dalloc(n, &n->G_h0, B * 2048));
@@ -303,10 +273,10 @@ int s16_alloc(fg_s16* n) {
   const size_t big = B * 256 * 128;  // largest activation: [B][16][16][128] = [B][8][8][512]
   FG_TRY(dalloc(n, &n->ga, big));
   FG_TRY(dalloc(n, &n->gb, big));
-  FG_TRY(dalloc(n, &n->dy_hi, big));
-  FG_TRY(dalloc(n, &n->dy_lo, big));
+  FG_TRY(dalloc(n, &n->env.dy.hi, big));
+  FG_TRY(dalloc(n, &n->env.dy.lo, big));
   FG_TRY(dalloc(n, &n->ws, (size_t)9 * 1024 * 512));  // largest weight tensor (c4); F1 is 4096*1024, the 5x5 packs 36*256*128
-  n->env.ga = n->ga; n->env.dy_hi = n->dy_hi; n->env.dy_lo = n->dy_lo; n->env.ws = n->ws;
+  n->env.ga = n->ga; n->env.ws = n->ws;
   FG_TRY(dalloc(n, &n->in_a, B * 256 * C));
   FG_TRY(dalloc(n, &n->in_b, B * 100));
   FG_TRY(dalloc(n, &n->in_c, B * 100));
@@ -322,15 +292,7 @@ int pack_G(fg_s16* n) {
   if (n->net.G_packed && n->G_pack_impl == pack_key(c)) return FG_OK;
   FG_TRY(convl_pack(c, n->GL1, n->net.PG));
   FG_TRY(convl_pack(c, n->GC3, n->net.PG));
-  for (int i = 0; i < 2; ++i) {
-    UpsL& U = n->GU[i];
-    if (use_tc_wgrad(c, U.geom(n->maxB)) && f16_on(c))
-      FG_TRY(tc_pack_collapsed_h(c, n->net.PG + U.w_off, U.Wf_hi, U.Wf_lo, U.Wd_hi, U.Wd_lo, U.Cout, U.Cin));
-    else if (use_tc_wgrad(c, U.geom(n->maxB)))
-      FG_TRY(tc_pack_collapsed(c, n->net.PG + U.w_off, U.Wf_hi, U.Wf_lo, U.Wd_hi, U.Wd_lo, U.Cout, U.Cin));
-    else
-      FG_TRY(k_pack_weights(c, n->net.PG + U.w_off, U.Wp, U.Wpd, U.Cout, U.Cin, 25, 0, 0, 0, 0));
-  }
+  for (int i = 0; i < 2; ++i) FG_TRY(upsl_pack(c, n->GU[i], n->net.PG));
   n->net.G_packed = true;
   n->G_pack_impl = pack_key(c);
   return FG_OK;
@@ -350,63 +312,6 @@ int pack_D(fg_s16* n) {
 // ---------------------------------------------------------------------------------------------------
 // G16
 // ---------------------------------------------------------------------------------------------------
-// *parts (in: want BatchNorm partials; out: how many tiles wrote one into c->bn_parts, 0 = none)
-int ups_fwd(fg_s16* n, UpsL& U, const float* h, float* z, int B, int* parts) {
-  fg_ctx* c = n->c;
-  const ConvGeom g = U.geom(B);
-  const bool want = *parts != 0;
-  *parts = 0;
-  if (!use_tc_wgrad(c, U.geom(n->maxB))) {
-    ScopedTimer tm(c, U.tf);
-    return k_conv_simt(c, h, U.Wp, n->net.PG + U.b_off, z, g);
-  }
-  const int64_t nh = (int64_t)B * (U.H / 2) * (U.H / 2) * U.Cin;
-  const bool h16 = f16_on(c);
-  if (h16) {
-    FG_TRY(tc_amax(c, h, nh, U.sx));
-    FG_TRY(tc_split_h(c, h, U.h_hi, U.h_lo, nh, U.sx));
-  } else {
-    FG_TRY(tc_split(c, h, U.h_hi, U.h_lo, nh));  // kept for the weight gradient
-  }
-  ScopedTimer tm(c, U.tf);
-  float* st = want && c->bn_epilogue ? c->bn_parts : nullptr;
-  return tc_conv_fwd(c, U.h_hi, U.h_lo, U.Wf_hi, U.Wf_lo, n->net.PG + U.b_off, z, g, 2, st, st ? parts : nullptr, h16,
-                     h16 ? U.sx + 1 : nullptr);
-}
-// dW += wgrad; dh = dgrad.  *pooled: dh already is the gradient of the LOW-RES input (tensor-core path folds the 2x2 sum of
-// the upsample backward into the dgrad GEMM); otherwise dh is the full-resolution gradient the consumer sums 2x2.
-int ups_bwd(fg_s16* n, UpsL& U, const float* h, const float* dz, float* dh, int B, bool* pooled) {
-  fg_ctx* c = n->c;
-  const ConvGeom g = U.geom(B);
-  if (!use_tc_wgrad(c, U.geom(n->maxB))) {
-    {
-      ScopedTimer tm(c, U.tw);
-      FG_TRY(k_wgrad_simt(c, h, dz, n->ws, g));
-    }
-    FG_TRY(k_unpack_wgrad(c, n->ws, n->net.gG + U.w_off, U.Cout, U.Cin, 25, 0, 0, 0, 0));
-    *pooled = false;
-    ScopedTimer tm(c, U.td);
-    return k_conv_simt(c, dz, U.Wpd, nullptr, dh, ConvGeom{B, U.H, U.H, U.Cout, U.Cin, 5, 1});
-  }
-  const int64_t ndz = (int64_t)B * U.H * U.H * U.Cout;
-  const bool h16 = f16_on(c);
-  float* sdy = n->env.sdy;
-  if (h16) {
-    FG_TRY(tc_amax(c, dz, ndz, sdy));
-    FG_TRY(tc_split_h(c, dz, n->dy_hi, n->dy_lo, ndz, sdy));
-  } else {
-    FG_TRY(tc_split(c, dz, n->dy_hi, n->dy_lo, ndz));
-  }
-  {
-    ScopedTimer tm(c, U.tw);
-    FG_TRY(tc_conv_wgrad(c, U.h_hi, U.h_lo, n->dy_hi, n->dy_lo, n->ws, g, h16, h16 ? sdy + 1 : nullptr, h16 ? U.sx + 1 : nullptr));
-  }
-  FG_TRY(tc_combine_collapsed_wgrad(c, n->ws, n->net.gG + U.w_off, U.Cout, U.Cin));
-  *pooled = true;
-  ScopedTimer tm(c, U.td);
-  return tc_conv_dgrad_ups(c, n->dy_hi, n->dy_lo, U.Wd_hi, U.Wd_lo, dh, g, h16, h16 ? sdy + 1 : nullptr);
-}
-
 // BatchNorm statistics of layer i (0: 256 channels at 8x8, 1: 128 channels at 16x16) -> bn_mean / bn_istd
 int bn_stats(fg_s16* n, int i, const float* z, int B, bool training, int parts) {
   fg_ctx* c = n->c;
@@ -429,12 +334,12 @@ int G_forward(fg_s16* n, const float* noise, int B, bool training) {
   FG_TRY(convl_fwd(n->env, n->GL1, n->G_x, P, n->G_z0, B));
   FG_TRY(k_prelu_fwd(c, n->G_z0, P + n->Ga[0], n->G_h0, (int64_t)B * 2048));
   int parts = training ? 1 : 0;
-  FG_TRY(ups_fwd(n, n->GU[0], n->G_h0, n->G_z1, B, &parts));
+  FG_TRY(upsl_fwd(n->env, n->GU[0], n->G_h0, P, n->G_z1, B, &parts));
   FG_TRY(bn_stats(n, 0, n->G_z1, B, training, parts));
   FG_TRY(k_bn_prelu_apply(c, n->G_z1, n->bn_mean[0], n->bn_istd[0], P + n->Gg[0], P + n->Gbe[0], P + n->Ga[1], n->G_h1,
                           (int64_t)B * 64, 256));
   parts = training ? 1 : 0;
-  FG_TRY(ups_fwd(n, n->GU[1], n->G_h1, n->G_z2, B, &parts));
+  FG_TRY(upsl_fwd(n->env, n->GU[1], n->G_h1, P, n->G_z2, B, &parts));
   FG_TRY(bn_stats(n, 1, n->G_z2, B, training, parts));
   FG_TRY(k_bn_prelu_apply(c, n->G_z2, n->bn_mean[1], n->bn_istd[1], P + n->Gg[1], P + n->Gbe[1], P + n->Ga[2], n->G_h2,
                           (int64_t)B * 256, 128));
@@ -464,14 +369,14 @@ int G_backward(fg_s16* n, const float* dy, float* dnoise) {
   FG_TRY(k_bn_bwd_finalize(c, c->bn_acc, n->bn_mg, G + n->Gg[1], G + n->Gbe[1], (int64_t)B * 256, 128));
   FG_TRY(k_bn_prelu_bwd_apply(c, n->G_dfull, n->G_z2, n->bn_mean[1], n->bn_istd[1], P + n->Gg[1], P + n->Gbe[1], P + n->Ga[2],
                               n->bn_mg, n->G_dz, B, 16, 16, 128, 0, nullptr, nullptr, G + n->GU[1].b_off));
-  FG_TRY(ups_bwd(n, n->GU[1], n->G_h1, n->G_dz, n->G_dfull, B, &pooled));
+  FG_TRY(upsl_bwd(n->env, n->GU[1], n->env.dy, n->G_h1, n->G_dz, G, n->G_dfull, B, &pooled));
   // BN1 + PReLU, C1 (the 2x2 sum = backward of the nearest upsample is folded into the loads when not pooled yet)
   FG_TRY(k_bn_prelu_bwd_reduce(c, n->G_dfull, n->G_z1, n->bn_mean[0], n->bn_istd[0], P + n->Gg[0], P + n->Gbe[0], P + n->Ga[1],
                                c->bn_acc, G + n->Ga[1], B, 8, 8, 256, pooled ? 0 : 1));
   FG_TRY(k_bn_bwd_finalize(c, c->bn_acc, n->bn_mg, G + n->Gg[0], G + n->Gbe[0], (int64_t)B * 64, 256));
   FG_TRY(k_bn_prelu_bwd_apply(c, n->G_dfull, n->G_z1, n->bn_mean[0], n->bn_istd[0], P + n->Gg[0], P + n->Gbe[0], P + n->Ga[1],
                               n->bn_mg, n->G_dz, B, 8, 8, 256, pooled ? 0 : 1, nullptr, nullptr, G + n->GU[0].b_off));
-  FG_TRY(ups_bwd(n, n->GU[0], n->G_h0, n->G_dz, n->G_dfull, B, &pooled));
+  FG_TRY(upsl_bwd(n->env, n->GU[0], n->env.dy, n->G_h0, n->G_dz, G, n->G_dfull, B, &pooled));
   FG_TRY(k_prelu_bwd(c, n->G_dfull, n->G_z0, P + n->Ga[0], n->G_dz0, G + n->Ga[0], B, 4, 4, 128, pooled ? 0 : 1));
   return convl_bwd(n->env, n->GL1, n->G_x, n->G_dz0, G, dnoise, B);
 }

@@ -150,7 +150,7 @@ def test_gpu_s16_D_forward_backward(C, impl, init):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("C,B", [(3, 8), (1, 12)])
-@pytest.mark.parametrize("impl", [0, 2])
+@pytest.mark.parametrize("impl", [0, 1, 2])
 def test_gpu_s16_train_step_matches_oracle(C, B, impl):
     """fg_s16_train_step == the adversarial.lua iteration composed from the fp64 oracle: losses, confusion counts,
     both clamped gradients (recovered from Adam's first moment: m = (1-beta1) g at t = 1), parameters, BN state."""
