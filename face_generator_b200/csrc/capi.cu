@@ -49,6 +49,25 @@ int fg_to_user(fg_ctx* c, float* dst, const float* src_dev, size_t n) {
   if (!dev) FG_CUDA(cudaStreamSynchronize(c->stream));
   return FG_OK;
 }
+int64_t debug_tensor_copy(fg_ctx* c, const char* what, const DebugTensor* ents, size_t n_ents, const char* name, float* dst,
+                          int64_t max_elems) {
+  for (size_t i = 0; i < n_ents; ++i) {
+    const DebugTensor& e = ents[i];
+    if (strcmp(e.name, name)) continue;
+    const int64_t n = e.per * e.B;
+    if (!e.p) {
+      fg_set_error("%s: '%s' has not been produced (Dstep.*: option \"debug_keep\" + a train step)", what, name);
+      return -1;
+    }
+    if (dst) {
+      if (n > max_elems) return -2;
+      if (fg_to_user(c, dst, e.p, n) != FG_OK) return -3;
+    }
+    return n;
+  }
+  fg_set_error("%s: unknown tensor '%s'", what, name);
+  return -1;
+}
 
 extern "C" {
 
@@ -479,9 +498,8 @@ int64_t fg_kernel_launches(fg_ctx* c) { return c ? c->launches : -1; }
 int64_t fg_debug_tensor(fg_ctx* c, const char* name, float* dst, int64_t max_elems) {
   if (!c || !name) return -1;
   cudaSetDevice(c->device);
-  struct Ent { const char* n; const float* p; int64_t per; int B; };
   const int gb = c->G_B, db = c->D_B;
-  const Ent ents[] = {
+  const DebugTensor ents[] = {
       {"G.z0", c->G_z0, 8192, gb}, {"G.h0", c->G_h0, 8192, gb}, {"G.z1", c->G_z1, 65536, gb}, {"G.h1", c->G_h1, 65536, gb},
       {"G.z2", c->G_z2, 131072, gb}, {"G.h2", c->G_h2, 131072, gb}, {"G.z3", c->G_z3, 1024 * c->C, gb},
       {"G.y", c->G_y, 1024 * c->C, gb}, {"G.dz2", c->G_dz2, 131072, gb}, {"G.dz1", c->G_dz1, 65536, gb},
@@ -495,21 +513,7 @@ int64_t fg_debug_tensor(fg_ctx* c, const char* name, float* dst, int64_t max_ele
       {"Dstep.z3", c->keep_D[2], 16384, c->keep_B}, {"Dstep.z4", c->keep_D[3], 8192, c->keep_B},
       {"Dstep.zl1", c->keep_D[4], 512, c->keep_B}, {"Dstep.zl2", c->keep_D[5], 512, c->keep_B},
       {"Dstep.logit", c->keep_D[6], 1, c->keep_B}, {"Dstep.out", c->keep_D[7], 1, c->keep_B}};
-  for (const Ent& e : ents)
-    if (!strcmp(e.n, name)) {
-      const int64_t n = e.per * e.B;
-      if (!e.p) {
-        fg_set_error("fg_debug_tensor: '%s' has not been produced (option \"debug_keep\" + fg_train_step)", name);
-        return -1;
-      }
-      if (dst) {
-        if (n > max_elems) return -2;
-        if (fg_to_user(c, dst, e.p, n) != FG_OK) return -3;
-      }
-      return n;
-    }
-  fg_set_error("fg_debug_tensor: unknown tensor '%s'", name);
-  return -1;
+  return debug_tensor_copy(c, "fg_debug_tensor", ents, sizeof(ents) / sizeof(ents[0]), name, dst, max_elems);
 }
 
 int fg_bench_tf32_peak(fg_ctx* c, int iters, double* tflops) {

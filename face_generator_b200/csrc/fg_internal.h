@@ -453,6 +453,16 @@ bool fg_is_dev(const void* p);
 int fg_to_dev(fg_ctx* c, const float* p, size_t n, float* staging, const float** out);
 // n floats from a device buffer to a user pointer (host: synchronised, so valid on return; dst == src: nothing)
 int fg_to_user(fg_ctx* c, float* dst, const float* src_dev, size_t n);
+// the fg_*debug_tensor contract over a table of named device tensors (per * B floats each; p == nullptr: not produced
+// yet): dst == nullptr -> the element count; -2: dst too small; -1 + fg_last_error: unknown or not produced
+struct DebugTensor {
+  const char* name;
+  const float* p;
+  int64_t per;
+  int B;
+};
+int64_t debug_tensor_copy(fg_ctx* c, const char* what, const DebugTensor* ents, size_t n_ents, const char* name, float* dst,
+                          int64_t max_elems);
 
 // ---- dataset.cu: inputs of the device-fed --scale 16 / coarse-to-fine steps (eager launches on the ctx stream) ----
 int dataset_check_feed(const fg_dataset* d, const fg_ctx* c, const char* what);  // same ctx, compatible channels

@@ -38,6 +38,9 @@ struct fg_c2f {
   int G_B = 0, D_B = 0;
   bool G_valid = false, D_valid = false, D_train = true;
   float D_scale = 2.f;
+  // option "debug_keep" (tests): the D step's D_z[0..3], D_zl1, D_logit, D_out, which the G step's D forward overwrites
+  float* keep_D[7] = {};
+  int keep_B = 0;
   std::vector<void*> allocs;
   ConvLEnv env;  // shared scratch of the ConvL layers (filled by c2f_alloc)
 };
@@ -303,6 +306,20 @@ int prep(fg_c2f* n, int net, const fg_hyper* h, int B) {
   return pair_gate(n->c, n->net, net, &hh, B, (float)n->c->world);
 }
 
+// option "debug_keep": copy the D step's pre-activations and outputs to keep_D ("Dstep.*" debug tensors)
+int keep_dstep(fg_c2f* n, int B) {
+  fg_ctx* c = n->c;
+  const float* src[7] = {n->D_z[0], n->D_z[1], n->D_z[2], n->D_z[3], n->D_zl1, n->D_logit, n->D_out};
+  size_t per[7] = {0, 0, 0, 0, 512, 1, 1};
+  for (int i = 0; i < 4; ++i) per[i] = (size_t)n->Dc[i].H * n->Dc[i].H * n->Dc[i].Cout;
+  for (int i = 0; i < 7; ++i) {
+    if (!n->keep_D[i]) FG_TRY(dalloc(n, &n->keep_D[i], (size_t)n->maxB * per[i]));
+    FG_CUDA(cudaMemcpyAsync(n->keep_D[i], src[i], sizeof(float) * B * per[i], cudaMemcpyDeviceToDevice, c->stream));
+  }
+  n->keep_B = B;
+  return FG_OK;
+}
+
 int train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_diff, const float* condD, const float* noiseD,
                const float* condG, const float* noiseG, const float* masksD, const float* masksG, uint64_t seed) {
   fg_ctx* c = n->c;
@@ -321,6 +338,7 @@ int train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_diff, cons
   FG_TRY(pair_zero_grads(c, n->net, FG_NET_D));
   FG_TRY(D_forward(n, n->io, n->D_cond, B, true, h->p_drop));
   FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_D, n->net.tailD, B, Bh));
+  if (c->debug_keep) FG_TRY(keep_dstep(n, B));
   FG_TRY(D_backward(n, n->D_dlogit, true, false));
   FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_D));
   FG_TRY(prep(n, FG_NET_D, h, B));
@@ -565,6 +583,28 @@ int fg_c2f_train_step_dataset(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B
   FG_TRY(noise_uniform_dev(c, seed * 8 + 3, (int64_t)Bh * 1024, n->in_c));
   FG_TRY(noise_uniform_dev(c, seed * 8 + 4, (int64_t)B * 1024, n->in_e));
   return run_train_step(n, h, B, n->in_a, n->in_b, n->in_c, n->in_d, n->in_e, nullptr, nullptr, seed, stats);
+}
+
+int64_t fg_c2f_debug_tensor(fg_c2f* n, const char* name, float* dst, int64_t max_elems) {
+  if (!n || !n->c || !name) {
+    fg_set_error("fg_c2f_debug_tensor: null argument");
+    return -1;
+  }
+  cudaSetDevice(n->c->device);
+  const int gb = n->G_B, db = n->D_B, kb = n->keep_B, C = n->C;
+  auto g = [&](const float* p) { return n->G_valid ? p : nullptr; };
+  auto d = [&](const float* p) { return n->D_valid ? p : nullptr; };
+  auto dz = [&](int i) { return (int64_t)n->Dc[i].H * n->Dc[i].H * n->Dc[i].Cout; };
+  const DebugTensor ents[] = {
+      {"G.x", g(n->G_x), 1024 * (C + 1), gb}, {"G.z1", g(n->G_z[0]), 1024 * 64, gb}, {"G.z2", g(n->G_z[1]), 1024 * 64, gb},
+      {"G.z3", g(n->G_z[2]), 1024 * 128, gb}, {"G.z4", g(n->G_z[3]), 1024 * 256, gb}, {"G.z5", g(n->G_z[4]), 1024 * C, gb},
+      {"D.x", d(n->D_x), 1024 * C, db}, {"D.z1", d(n->D_z[0]), dz(0), db}, {"D.z2", d(n->D_z[1]), dz(1), db},
+      {"D.z3", d(n->D_z[2]), dz(2), db}, {"D.z4", d(n->D_z[3]), dz(3), db}, {"D.p2", d(n->D_p2), 256 * 64, db},
+      {"D.p4", d(n->D_p4), 16384, db}, {"D.zl1", d(n->D_zl1), 512, db}, {"D.logit", d(n->D_logit), 1, db},
+      {"D.out", d(n->D_out), 1, db}, {"Dstep.z1", n->keep_D[0], dz(0), kb}, {"Dstep.z2", n->keep_D[1], dz(1), kb},
+      {"Dstep.z3", n->keep_D[2], dz(2), kb}, {"Dstep.z4", n->keep_D[3], dz(3), kb}, {"Dstep.zl1", n->keep_D[4], 512, kb},
+      {"Dstep.logit", n->keep_D[5], 1, kb}, {"Dstep.out", n->keep_D[6], 1, kb}};
+  return debug_tensor_copy(n->c, "fg_c2f_debug_tensor", ents, sizeof(ents) / sizeof(ents[0]), name, dst, max_elems);
 }
 
 }  // extern "C"

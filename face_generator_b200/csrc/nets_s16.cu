@@ -130,6 +130,10 @@ struct fg_s16 {
   int G_pack_impl = -1, D_pack_impl = -1;
   int G_B = 0, D_B = 0;
   bool G_valid = false, G_train = true, D_valid = false, D_train = true;
+  // option "debug_keep" (tests): the D step's D_z[0..3], D_zf, D_ze1, D_ze2, D_logit, D_out, which the G step's D
+  // forward overwrites
+  float* keep_D[9] = {};
+  int keep_B = 0;
   std::vector<void*> allocs;
   ConvLEnv env;
 };
@@ -496,6 +500,19 @@ int D_backward(fg_s16* n, const float* dlogit, bool want_wgrad, bool want_dx) {
   return FG_OK;
 }
 
+// option "debug_keep": copy the D step's pre-activations and outputs to keep_D ("Dstep.*" debug tensors)
+int keep_dstep(fg_s16* n, int B) {
+  fg_ctx* c = n->c;
+  const float* src[9] = {n->D_z[0], n->D_z[1], n->D_z[2], n->D_z[3], n->D_zf, n->D_ze1, n->D_ze2, n->D_logit, n->D_out};
+  const size_t per[9] = {256 * 128, 256 * 128, 16 * 512, 4 * 1024, 1024, 128, 128, 1, 1};
+  for (int i = 0; i < 9; ++i) {
+    if (!n->keep_D[i]) FG_TRY(dalloc(n, &n->keep_D[i], (size_t)n->maxB * per[i]));
+    FG_CUDA(cudaMemcpyAsync(n->keep_D[i], src[i], sizeof(float) * B * per[i], cudaMemcpyDeviceToDevice, c->stream));
+  }
+  n->keep_B = B;
+  return FG_OK;
+}
+
 // one iteration of the adversarial.lua loop body (D_iterations = G_iterations = 1) on the 16x16 nets
 int train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const float* noiseD, const float* noiseG,
                const float* masksD, const float* masksG, uint64_t seed) {
@@ -514,6 +531,7 @@ int train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const flo
   FG_TRY(pair_zero_grads(c, n->net, FG_NET_D));
   FG_TRY(D_forward(n, n->D_x, B, true));
   FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_D, n->net.tailD, B, Bh));
+  if (c->debug_keep) FG_TRY(keep_dstep(n, B));
   FG_TRY(D_backward(n, n->D_dlogit, true, false));
   FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_D));
   FG_TRY(pair_gate(c, n->net, FG_NET_D, h, B, (float)c->world));
@@ -729,6 +747,29 @@ int fg_s16_train_step_dataset(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B
   FG_TRY(noise_uniform_dev(c, seed * 4 + 1, (int64_t)(B / 2) * 100, n->in_b));
   FG_TRY(noise_uniform_dev(c, seed * 4 + 2, (int64_t)B * 100, n->in_c));
   return run_train_step(n, h, B, n->in_a, n->in_b, n->in_c, nullptr, nullptr, seed, stats);
+}
+
+int64_t fg_s16_debug_tensor(fg_s16* n, const char* name, float* dst, int64_t max_elems) {
+  if (!n || !n->c || !name) {
+    fg_set_error("fg_s16_debug_tensor: null argument");
+    return -1;
+  }
+  cudaSetDevice(n->c->device);
+  const int gb = n->G_B, db = n->D_B, kb = n->keep_B, sb = n->G_valid ? 1 : 0;
+  auto g = [&](const float* p) { return n->G_valid ? p : nullptr; };
+  auto d = [&](const float* p) { return n->D_valid ? p : nullptr; };
+  const DebugTensor ents[] = {
+      {"G.z0", g(n->G_z0), 2048, gb}, {"G.z1", g(n->G_z1), 64 * 256, gb}, {"G.z2", g(n->G_z2), 256 * 128, gb},
+      {"G.z3", g(n->G_z3), 256 * n->C, gb}, {"G.bn_mean1", g(n->bn_mean[0]), 256, sb}, {"G.bn_istd1", g(n->bn_istd[0]), 256, sb},
+      {"G.bn_mean2", g(n->bn_mean[1]), 128, sb}, {"G.bn_istd2", g(n->bn_istd[1]), 128, sb},
+      {"D.z1", d(n->D_z[0]), 256 * 128, db}, {"D.z2", d(n->D_z[1]), 256 * 128, db}, {"D.z3", d(n->D_z[2]), 16 * 512, db},
+      {"D.z4", d(n->D_z[3]), 4 * 1024, db}, {"D.p1", d(n->D_p1), 64 * 128, db}, {"D.zf", d(n->D_zf), 1024, db},
+      {"D.ze1", d(n->D_ze1), 128, db}, {"D.ze2", d(n->D_ze2), 128, db}, {"D.logit", d(n->D_logit), 1, db},
+      {"D.out", d(n->D_out), 1, db}, {"Dstep.z1", n->keep_D[0], 256 * 128, kb}, {"Dstep.z2", n->keep_D[1], 256 * 128, kb},
+      {"Dstep.z3", n->keep_D[2], 16 * 512, kb}, {"Dstep.z4", n->keep_D[3], 4 * 1024, kb}, {"Dstep.zf", n->keep_D[4], 1024, kb},
+      {"Dstep.ze1", n->keep_D[5], 128, kb}, {"Dstep.ze2", n->keep_D[6], 128, kb}, {"Dstep.logit", n->keep_D[7], 1, kb},
+      {"Dstep.out", n->keep_D[8], 1, kb}};
+  return debug_tensor_copy(n->c, "fg_s16_debug_tensor", ents, sizeof(ents) / sizeof(ents[0]), name, dst, max_elems);
 }
 
 }  // extern "C"

@@ -169,6 +169,8 @@ SYMBOLS = {
     "fg_memcpy": (_I, [_P, _P, _P, _SZ]),
     "fg_kernel_launches": (_L, [_P]),
     "fg_debug_tensor": (_L, [_P, C.c_char_p, _P, _L]),
+    "fg_c2f_debug_tensor": (_L, [_P, C.c_char_p, _P, _L]),
+    "fg_s16_debug_tensor": (_L, [_P, C.c_char_p, _P, _L]),
     "fg_bench_tf32_peak": (_I, [_P, _I, C.POINTER(C.c_double)]),
     "fg_event_record": (_I, [_P, _I]),
     "fg_event_elapsed_ms": (_I, [_P, _I, _I, C.POINTER(C.c_double)]),
@@ -302,6 +304,18 @@ class _NetPair:
     def dp_broadcast_params(self):
         self._call("dp_broadcast_params")
 
+    def debug_tensor(self, name):
+        """an internal tensor of the last forward / train step as stored (NHWC), flat float32 (tests)"""
+        fn = getattr(self.lib, self._prefix + "debug_tensor")
+        n = fn(self.h, name.encode(), None, 0)
+        if n < 0:
+            raise FGError("%sdebug_tensor(%s): %d: %s" % (self._prefix, name, n, self.lib.fg_last_error().decode()))
+        out = np.empty(n, np.float32)
+        r = fn(self.h, name.encode(), _ptr(out), n)
+        if r < 0:
+            raise FGError("%sdebug_tensor(%s): %d" % (self._prefix, name, r))
+        return out
+
 
 class _BatchNormNetPair(_NetPair):
     """A pair whose G has BatchNorm layers: their running statistics, [mean1 256][var1 256][mean2 128][var2 128]."""
@@ -429,16 +443,6 @@ class Context(_BatchNormNetPair):
         v = C.c_double(0)
         _check(self.lib.fg_bench_tf32_peak(self.h, iters, C.byref(v)), "fg_bench_tf32_peak")
         return v.value
-
-    def debug_tensor(self, name):
-        n = self.lib.fg_debug_tensor(self.h, name.encode(), None, 0)
-        if n < 0:
-            raise FGError("fg_debug_tensor(%s): %d" % (name, n))
-        out = np.empty(n, np.float32)
-        r = self.lib.fg_debug_tensor(self.h, name.encode(), _ptr(out), n)
-        if r < 0:
-            raise FGError("fg_debug_tensor(%s): %d" % (name, r))
-        return out
 
     def launches(self):
         return int(self.lib.fg_kernel_launches(self.h))

@@ -161,6 +161,8 @@ int fg_host_free_pinned(void* p);
 int fg_memcpy(fg_ctx* ctx, void* dst, const void* src, size_t bytes);
 int64_t fg_kernel_launches(fg_ctx* ctx);
 int64_t fg_debug_tensor(fg_ctx* ctx, const char* name, float* dst, int64_t max_elems);
+int64_t fg_c2f_debug_tensor(fg_c2f* n, const char* name, float* dst, int64_t max_elems);
+int64_t fg_s16_debug_tensor(fg_s16* n, const char* name, float* dst, int64_t max_elems);
 int fg_bench_tf32_peak(fg_ctx* ctx, int iters, double* tflops);
 int fg_event_record(fg_ctx* ctx, int slot);
 int fg_event_elapsed_ms(fg_ctx* ctx, int slot_a, int slot_b, double* ms);

@@ -399,6 +399,14 @@ int fg_memcpy(fg_ctx* ctx, void* dst, const void* src, size_t bytes);   /* any d
 int64_t fg_kernel_launches(fg_ctx* ctx);                  /* kernels launched by this ctx so far   */
 /* copy an internal activation (NHWC) to dst: names "G.z0","G.h0","G.z1","G.h1","G.z2","G.h2","G.z3" */
 int64_t fg_debug_tensor(fg_ctx* ctx, const char* name, float* dst, int64_t max_elems);
+/* the same for the coarse-to-fine and --scale 16 nets: dst == NULL returns the element count, -2 when
+ * dst is too small, -1 (fg_last_error) for an unknown name or one not produced yet.  "Dstep.*" are the
+ * D step's tensors of the last train step with option "debug_keep".
+ *   c2f: G.x G.z1..G.z5  D.x D.z1..D.z4 D.p2 D.p4 D.zl1 D.logit D.out  Dstep.z1..z4 .zl1 .logit .out
+ *   s16: G.z0..G.z3 G.bn_mean1/2 G.bn_istd1/2  D.z1..D.z4 (after the stride-2 sampling) D.p1 D.zf
+ *        D.ze1 D.ze2 D.logit D.out  Dstep.z1..z4 .zf .ze1 .ze2 .logit .out                            */
+int64_t fg_c2f_debug_tensor(fg_c2f* n, const char* name, float* dst, int64_t max_elems);
+int64_t fg_s16_debug_tensor(fg_s16* n, const char* name, float* dst, int64_t max_elems);
 /* timing of the dominant kernel family inside the last fg_train_step (CUDA events on the ctx
  * stream): returns ms in out[0..n) for the names in fg_timing_names(); 0 when not enabled.       */
 /* whole-step timing on the ctx stream: record CUDA event `slot` (0..15), elapsed ms between two. */

@@ -70,6 +70,16 @@ def kink_branch(gpu_pos, counts, margin=PU.KINK_MARGIN):
 
 @pytest.mark.parametrize("B", [256, 130])
 def test_G_at_headline_batch(fg, B):
+    _G_at_headline_batch(fg, B, 2)
+
+
+@pytest.mark.parametrize("B", [256, 130])
+def test_G_dense_forward_at_headline_batch(fg, B):
+    """conv_impl = 1: C1 / C2 forward on the dense 25-tap pack of the upsampled 5x5 layers (same checks)"""
+    _G_at_headline_batch(fg, B, 1)
+
+
+def _G_at_headline_batch(fg, B, impl):
     import torch_ref as R
     F = torch.nn.functional
     from face_generator_b200.lib import NET_G
@@ -78,6 +88,7 @@ def test_G_at_headline_batch(fg, B):
     noise = case["noise_G"][:B]
     dout = np.random.default_rng(B).standard_normal((B, C, 32, 32)).astype(np.float32)
     ctx = fg.Context(0, max_batch=B, channels=C)
+    ctx.set_option("conv_impl", impl)
     ctx.set_params(NET_G, case["PG"])
     out = ctx.G_forward(noise)
     p = R._split(dev(case["PG"]), O.G_layout(C))

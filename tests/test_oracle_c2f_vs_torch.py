@@ -32,6 +32,31 @@ def test_maxpool_first_max_wins():
     assert dx[0, 0].tolist() == [[0, 7, 3, 0], [0, 0, 0, 0]]
 
 
+def test_routed_restatement_matches_oracle():
+    """D_forward with the branch / max-pool routing hooks making their own decisions (the hooks of the batch-256 GPU
+    checks) is the same function as the oracle, values and gradients; forcing another window element moves the value"""
+    rng = np.random.default_rng(45)
+    B, C = 3, 3
+    P = RC.trained_like_D(C, rng)
+    diff, cond = RC.make_pairs(B, C, rng)
+    masks = RC.make_masks(B, rng)
+    dout = rng.standard_normal(B)
+    d = OC.f64.D()
+    out = d.forward(P, diff, cond, masks)
+    dP, dd = d.backward(dout)
+    own = lambda name, x: x > 0
+    route = lambda name, win: win.argmax(-1)
+    Pt = torch.tensor(P, requires_grad=True)
+    dt = torch.tensor(diff, requires_grad=True)
+    out_t = RC.D_forward(Pt, dt, torch.tensor(cond), torch.tensor(masks), C, branch=own, route=route)
+    out_t.backward(torch.tensor(dout))
+    assert rel(out, out_t.detach().numpy()) < 1e-12
+    assert rel(dP, Pt.grad.numpy()) < 1e-9 and rel(dd, dt.grad.numpy()) < 1e-9
+    x = torch.tensor(rng.standard_normal((2, 4, 6, 8)))
+    assert torch.equal(RC.maxpool2(x, route, "p"), torch.nn.functional.max_pool2d(x, 2, 2))
+    assert (RC.maxpool2(x, lambda n, w: w.argmin(-1), "p") < RC.maxpool2(x)).all()
+
+
 @pytest.mark.parametrize("C", [3, 1])
 def test_G_fwd_bwd_matches_torch(C):
     rng = np.random.default_rng(30 + C)

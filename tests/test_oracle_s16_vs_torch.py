@@ -1,16 +1,14 @@
 """CPU: the --scale 16 nets of the oracle (models.lua:26-51 create_G_decoder_upsampling16, :279-316 create_D16_d with
-its stride-2 convolutions and ConcatTable/JoinTable) against PyTorch-CPU autograd in fp64.  No CUDA counterpart yet
-(SURVEY.md 8(f).4): this is the checker it will be held to."""
+its stride-2 convolutions and ConcatTable/JoinTable) against PyTorch-CPU autograd in fp64 (tests/torch_ref_s16.py,
+the checker tests/test_gpu_c2f_s16_headline.py holds the CUDA path to at batch 256)."""
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-from torch_ref import d_sigmoid
-
 from oracle import oracle_s16 as OS
-from torch_ref import _split, prelu
 from torch_ref_c2f import trained_like
+from torch_ref_s16 import torch_D16, torch_G16
 
 torch.set_num_threads(8)
 
@@ -32,32 +30,6 @@ def test_strided_conv_matches_torch(stride, pad, H, k):
     yt.backward(torch.tensor(dy))
     dx, dw, db = OS.f64.convs_bwd(x, w, dy, stride, pad)
     assert rel(dx, xt.grad.numpy()) < 1e-12 and rel(dw, wt.grad.numpy()) < 1e-12 and rel(db, bt.grad.numpy()) < 1e-12
-
-
-def torch_G16(P, noise, C):
-    p = _split(P, OS.G_layout(C))
-    B = noise.shape[0]
-    h = prelu(F.linear(noise, p["L1W"], p["L1b"]).view(B, 128, 4, 4), p["a1"])
-    h = F.conv2d(F.interpolate(h, scale_factor=2, mode="nearest"), p["C1W"], p["C1b"], padding=2)
-    h = prelu(F.batch_norm(h, None, None, p["g1"], p["be1"], training=True, eps=1e-5), p["a2"])
-    h = F.conv2d(F.interpolate(h, scale_factor=2, mode="nearest"), p["C2W"], p["C2b"], padding=2)
-    h = prelu(F.batch_norm(h, None, None, p["g2"], p["be2"], training=True, eps=1e-5), p["a3"])
-    return torch.sigmoid(F.conv2d(h, p["C3W"], p["C3b"], padding=1))
-
-
-def torch_D16(P, img, masks, C):
-    p = _split(P, OS.D_layout(C))
-    B = img.shape[0]
-    h = prelu(F.conv2d(img, p["c1W"], p["c1b"], padding=1), p["a1"])
-    h = prelu(F.conv2d(h, p["c2W"], p["c2b"], padding=1), p["a2"])
-    h = F.avg_pool2d(h, 2, 2)
-    h = prelu(F.conv2d(h, p["c3W"], p["c3b"], stride=2, padding=1), p["a3"])
-    h = prelu(F.conv2d(h, p["c4W"], p["c4b"], stride=2, padding=1), p["a4"])
-    h = h * masks[:, :1024].reshape(B, 1024, 1, 1)  # SpatialDropout: no rescale
-    fine = prelu(F.linear(h.reshape(B, 4096), p["F1W"], p["F1b"]), p["af"])
-    e = prelu(F.linear(img.reshape(B, -1), p["E1W"], p["E1b"]), p["ae1"]) * masks[:, 1024:] * 2.0
-    e = prelu(F.linear(e, p["E2W"], p["E2b"]), p["ae2"])
-    return d_sigmoid(F.linear(torch.cat([fine, e], dim=1), p["JW"], p["Jb"])).reshape(B)
 
 
 def test_param_counts():
@@ -90,6 +62,21 @@ def test_G16_fwd_bwd_matches_torch(C):
             assert np.abs(dP[o:o + n]).max() < 1e-9 * np.abs(gt).max()
             continue
         assert rel(dP[o:o + n], gt[o:o + n]) < 1e-8, k
+
+
+def test_G16_running_statistics_match_torch():
+    """the BatchNorm running statistics of two training-mode forwards (the D and the G step of one iteration)"""
+    import s16_utils as SU
+    rng = np.random.default_rng(64)
+    C = 3
+    P = trained_like(OS.G_layout(C), OS.G_param_count(C), rng, gain=1.0)
+    bn = SU.bn_init()
+    running = torch.tensor(bn)
+    for B in (3, 5):
+        noise = rng.uniform(-1, 1, (B, 100))
+        OS.f64.G().forward(P, noise, C, bn)
+        torch_G16(torch.tensor(P), torch.tensor(noise), C, running=running)
+    assert rel(bn, running.numpy()) < 1e-12
 
 
 @pytest.mark.parametrize("C", [3, 1])
