@@ -4,6 +4,7 @@
 #include <cstdlib>
 #include <cstring>
 
+#include "convl.h"
 #include "fg_internal.h"
 #include "k_conv_tc.h"
 
@@ -255,7 +256,7 @@ int64_t fg_get_option(fg_ctx* c, const char* key) {
 
 int64_t fg_param_count(int net, int channels) {
   if (channels != 1 && channels != 3) return -1;
-  return net == FG_NET_G ? make_g_layout(channels).total : net == FG_NET_D ? make_d_layout(channels).total : -1;
+  return net == FG_NET_G ? make_g_layout(channels, 32).total : net == FG_NET_D ? make_d_layout(channels).total : -1;
 }
 int fg_set_params(fg_ctx* c, int net, const float* src) {
   ENTER(c);
@@ -327,9 +328,9 @@ int fg_G_forward(fg_ctx* c, const float* noise, int B, int training, float* imag
   c->net.G_packed = false;  // parameters may have been edited through fg_params_ptr()
   const float* nd;
   FG_TRY(fg_to_dev(c, noise, (size_t)B * kNoiseDim, c->in_noiseG, &nd));
-  FG_TRY(net_G_forward(c, nd, B, training != 0));
+  FG_TRY(gen_forward(c->env, c->G, c->net, nd, B, training != 0));
   if (images_out) {
-    FG_TRY(k_nhwc_to_nchw(c, c->G_y, c->io_dev, B, c->C, 1024));
+    FG_TRY(k_nhwc_to_nchw(c, c->G.y, c->io_dev, B, c->C, 1024));
     FG_TRY(fg_to_user(c, images_out, c->io_dev, (size_t)B * c->C * 1024));
   }
   return FG_OK;
@@ -337,13 +338,13 @@ int fg_G_forward(fg_ctx* c, const float* noise, int B, int training, float* imag
 int fg_G_backward(fg_ctx* c, const float* d_images, float* d_noise) {
   ENTER(c);
   FG_REQUIRE(d_images, "fg_G_backward: d_images is null");
-  const int B = c->G_B;
+  const int B = c->G.B;
   const float* dd;
   FG_TRY(fg_to_dev(c, d_images, (size_t)B * c->C * 1024, c->io_dev, &dd));
   FG_TRY(k_nchw_to_nhwc(c, dd, c->io_dev2, B, c->C, 1024));
   float* dn = nullptr;
   if (d_noise) dn = fg_is_dev(d_noise) ? d_noise : c->in_noiseD;
-  FG_TRY(net_G_backward(c, c->io_dev2, dn));
+  FG_TRY(gen_backward(c->env, c->G, c->net, c->io_dev2, dn));
   if (d_noise && dn != d_noise) FG_TRY(fg_to_user(c, d_noise, dn, (size_t)B * kNoiseDim));
   return FG_OK;
 }
@@ -447,12 +448,12 @@ int fg_sample(fg_ctx* c, const float* noise, int N, int chunk, float* images_out
     const float* nd;
     FG_TRY(fg_to_dev(c, noise + (size_t)s * kNoiseDim, (size_t)b * kNoiseDim, c->in_noiseG, &nd));
     // sample.lua never calls :evaluate() => BatchNorm uses the statistics of each chunk (SURVEY 3.4)
-    FG_TRY(net_G_forward(c, nd, b, true));
+    FG_TRY(gen_forward(c->env, c->G, c->net, nd, b, true));
     float* dst = images_out + (size_t)s * img;
     if (out_dev) {
-      FG_TRY(k_nhwc_to_nchw(c, c->G_y, dst, b, c->C, 1024));
+      FG_TRY(k_nhwc_to_nchw(c, c->G.y, dst, b, c->C, 1024));
     } else {
-      FG_TRY(k_nhwc_to_nchw(c, c->G_y, c->io_dev, b, c->C, 1024));
+      FG_TRY(k_nhwc_to_nchw(c, c->G.y, c->io_dev, b, c->C, 1024));
       FG_CUDA(cudaMemcpyAsync(dst, c->io_dev, b * img * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
       if (s + chunk < N) FG_CUDA(cudaStreamSynchronize(c->stream));  // io_dev is reused by the next chunk
     }
@@ -498,22 +499,18 @@ int64_t fg_kernel_launches(fg_ctx* c) { return c ? c->launches : -1; }
 int64_t fg_debug_tensor(fg_ctx* c, const char* name, float* dst, int64_t max_elems) {
   if (!c || !name) return -1;
   cudaSetDevice(c->device);
-  const int gb = c->G_B, db = c->D_B;
-  const DebugTensor ents[] = {
-      {"G.z0", c->G_z0, 8192, gb}, {"G.h0", c->G_h0, 8192, gb}, {"G.z1", c->G_z1, 65536, gb}, {"G.h1", c->G_h1, 65536, gb},
-      {"G.z2", c->G_z2, 131072, gb}, {"G.h2", c->G_h2, 131072, gb}, {"G.z3", c->G_z3, 1024 * c->C, gb},
-      {"G.y", c->G_y, 1024 * c->C, gb}, {"G.dz2", c->G_dz2, 131072, gb}, {"G.dz1", c->G_dz1, 65536, gb},
-      {"G.dz0", c->G_dz0, 8192, gb}, {"D.z1", c->D_z[0], 65536, db}, {"D.z2", c->D_z[1], 32768, db},
-      {"D.z3", c->D_z[2], 16384, db}, {"D.z4", c->D_z[3], 8192, db}, {"D.p4", c->D_p[3], 2048, db},
-      {"D.logit", c->D_logit, 1, db}, {"D.out", c->D_out, 1, db}, {"D.dx", c->D_dx, 1024 * c->C, db},
-      {"D.masks", c->D_masks, kMaskPerSample, db}, {"G.bn_mean1", c->bn_mean1, 256, 1}, {"G.bn_istd1", c->bn_istd1, 256, 1},
-      {"G.bn_mean2", c->bn_mean2, 128, 1}, {"G.bn_istd2", c->bn_istd2, 128, 1},
+  const int db = c->D_B;
+  std::vector<DebugTensor> ents = {
+      {"D.z1", c->D_z[0], 65536, db}, {"D.z2", c->D_z[1], 32768, db}, {"D.z3", c->D_z[2], 16384, db},
+      {"D.z4", c->D_z[3], 8192, db}, {"D.p4", c->D_p[3], 2048, db}, {"D.logit", c->D_logit, 1, db},
+      {"D.out", c->D_out, 1, db}, {"D.dx", c->D_dx, 1024 * c->C, db}, {"D.masks", c->D_masks, kMaskPerSample, db},
       {"D.zl1", c->D_zl1, 512, db}, {"D.zl2", c->D_zl2, 512, db},
       {"Dstep.z1", c->keep_D[0], 65536, c->keep_B}, {"Dstep.z2", c->keep_D[1], 32768, c->keep_B},
       {"Dstep.z3", c->keep_D[2], 16384, c->keep_B}, {"Dstep.z4", c->keep_D[3], 8192, c->keep_B},
       {"Dstep.zl1", c->keep_D[4], 512, c->keep_B}, {"Dstep.zl2", c->keep_D[5], 512, c->keep_B},
       {"Dstep.logit", c->keep_D[6], 1, c->keep_B}, {"Dstep.out", c->keep_D[7], 1, c->keep_B}};
-  return debug_tensor_copy(c, "fg_debug_tensor", ents, sizeof(ents) / sizeof(ents[0]), name, dst, max_elems);
+  gen_debug_rows(c->G, ents);
+  return debug_tensor_copy(c, "fg_debug_tensor", ents.data(), ents.size(), name, dst, max_elems);
 }
 
 int fg_bench_tf32_peak(fg_ctx* c, int iters, double* tflops) {

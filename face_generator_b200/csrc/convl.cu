@@ -6,6 +6,25 @@
 
 int convl_dalloc(ConvLEnv& e, float** p, size_t elems) { return fg_dalloc(e.c, *e.allocs, p, elems); }
 
+int ScalePairs::alloc(fg_ctx* c, std::vector<void*>& allocs, int pairs) {
+  n = pairs;
+  used = 0;
+  return fg_dalloc(c, allocs, &base, 2 * (size_t)pairs);
+}
+int ScalePairs::take(float** pair) {
+  if (used == n) {
+    fg_set_error("a block of %d FP16 scale pairs is full", n);
+    return FG_ERR_UNSUPPORTED;
+  }
+  *pair = base + 2 * used++;
+  return FG_OK;
+}
+int ScalePairs::reset(fg_ctx* c) const {
+  if (!tc_f16(c)) return FG_OK;
+  FG_CUDA(cudaMemset2DAsync(base, 2 * sizeof(float), 0, sizeof(float), n, c->stream));
+  return FG_OK;
+}
+
 namespace {
 // option "mma_f16": the hi/lo buffers of a layer hold the 3xFP16 split (halves, half of each buffer used), activations and
 // gradients scaled into fp16's range by a device-side power of two (TcOp::s: (max|x|, 1/scale) pairs); the tensor

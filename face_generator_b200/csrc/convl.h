@@ -9,6 +9,20 @@
 // option "mma_f16": tensor-core operands in the 3xFP16 split (only with the phase-collapsed kernels)
 inline bool tc_f16(const fg_ctx* c) { return c->mma_f16 && c->conv_impl == FG_CONV_TC_COLLAPSED; }
 
+// The ONE elementwise producer launched inside the scope also reduces max|output| into `pair` (with the FP16 split) and
+// sets *done, so that the consuming layer skips its own read pass.  The pair's max word must be zero (ScalePairs::reset).
+struct AmaxInto {
+  fg_ctx* c;
+  AmaxInto(fg_ctx* c_, TcOp& op) : AmaxInto(c_, op.s, &op.amax_ready) {}
+  AmaxInto(fg_ctx* c_, float* pair, bool* done) : c(c_) {
+    if (tc_f16(c)) {
+      c->amax_out = reinterpret_cast<unsigned*>(pair);
+      c->amax_done = done;
+    }
+  }
+  ~AmaxInto() { c->amax_out = nullptr; }
+};
+
 // the split of x (n elements) into op, in the format `f16` chooses, minus whatever the producer already did
 int tc_op_split(fg_ctx* c, TcOp& op, const float* x, int64_t n, bool f16);
 
@@ -33,3 +47,12 @@ int upsl_fwd(ConvLEnv& e, UpsL& U, const float* h, const float* P, float* z, int
 // split into.  *pooled: dh already is the gradient of the LOW-RES input (the tensor-core dgrad folds in the 2x2 sum of
 // the upsample backward); otherwise dh is the full-resolution gradient the consumer still sums 2x2.
 int upsl_bwd(ConvLEnv& e, UpsL& U, TcOp& dy, const float* h, const float* dz, float* G, float* dh, int B, bool* pooled);
+
+// ---- gen.cu: UpsGen on the owner's layer scratch (ConvLEnv) and parameters (NetPair: PG, gG, bnG, G_packed) ----
+int gen_alloc(ConvLEnv& e, UpsGen& G, const GenDesc& d);
+int gen_pack(fg_ctx* c, UpsGen& G, NetPair& p);  // unless p.G_packed under the current pack_key()
+// noise: device [B][100] -> G.y (NHWC [B][S][S][C]).  training: batch statistics + running statistics update
+int gen_forward(ConvLEnv& e, UpsGen& G, NetPair& p, const float* noise, int B, bool training);
+// dy: NHWC [B][S][S][C] of the last (training-mode) forward; accumulates into p.gG; dnoise (device [B][100]) may be null
+int gen_backward(ConvLEnv& e, UpsGen& G, NetPair& p, const float* dy, float* dnoise);
+void gen_debug_rows(const UpsGen& G, std::vector<DebugTensor>& rows);  // "G.*" of fg_*debug_tensor

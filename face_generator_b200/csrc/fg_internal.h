@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
+#include <deque>
 #include <functional>
 #include <initializer_list>
 #include <map>
@@ -70,7 +71,7 @@ struct GLayout {
 struct DLayout {
   int64_t cW[4], cb[4], ca[4], L1W, L1b, a5, L2W, L2b, a6, L3W, L3b, total;
 };
-GLayout make_g_layout(int C);
+GLayout make_g_layout(int C, int side);  // the generator of models.lua at side 32 (upsampling32) or 16 (upsampling16)
 DLayout make_d_layout(int C);
 
 struct DeviceStats {  // lives in device memory; mirrored to fg_step_stats
@@ -111,10 +112,22 @@ struct NetPair {
 };
 
 // ---- layer types (dispatch in convl.cu) ------------------------------------------------------------------
+// A block of device (max|x|, 1/scale) pairs: the power-of-two scales of one net's FP16-split operands (option mma_f16).
+// The owner takes one pair per operand at alloc and resets the block at the start of each of its passes.
+struct ScalePairs {
+  float* base = nullptr;
+  int n = 0, used = 0;
+  int alloc(fg_ctx* c, std::vector<void*>& allocs, int pairs);
+  int take(float** pair);  // the next pair; an error when the block is full
+  // with the FP16 split only: zero the max words, which producers reduce into by atomicMax (AmaxInto).  The inverse
+  // scales stay: the weight gradients of a later pass still read them.
+  int reset(fg_ctx* c) const;
+};
+
 // One tensor-core operand: the hi/lo split of a tensor and its device (max|x|, 1/scale) pair.  Each buffer is sized for
 // the 3xTF32 split; the 3xFP16 split uses its first half.  A producer kernel that already did part of the work says so:
 //   split_ready  it wrote the TF32 split into hi/lo (3xTF32 path)
-//   amax_ready   it reduced max|x| into s[0] (3xFP16 path; AmaxInto in nets.cu)
+//   amax_ready   it reduced max|x| into s[0] (3xFP16 path; AmaxInto in convl.h)
 //   bias_ready   it added the bias gradient (the column sums of a dY) into the gradient (ConvLEnv::dy only)
 // The consuming layer then skips that pass and clears the flag.
 struct TcOp {
@@ -173,6 +186,36 @@ struct ConvLEnv {
   float* ws = nullptr;  // packed weight-gradient workspace (largest layer)
 };
 
+// What differs between the generator sizes, as data: the generator code never asks which net it serves
+struct GenDesc {
+  int side;            // 32 or 16; every size follows from it
+  const char* prefix;  // of every timer name: "" keeps the 32x32 names that bench.py and profiles/ read
+  int l1_kpad;         // ConvL::kpad of G.L1 (0: no padding, G.L1 stays on the FFMA kernels)
+  bool bwd_merge;      // G.C1 / G.C2 name a merged-launch timer (UpsL::tb), so option bwd_merge may merge them
+};
+
+// The generator of models.lua at side S (create_G_decoder_upsampling32 / 16; gen.cu): Linear(100 -> 128 (S/4)^2) View
+// PReLU | Up2 conv(128->256,5) BN PReLU | Up2 conv(256->128,5) BN PReLU | conv(128->C,3) Sigmoid
+struct UpsGen {
+  int S = 32, C = 3;
+  GLayout gl;
+  ConvL GL1, GC3;
+  UpsL GU[2];                          // G.C1, G.C2
+  ScalePairs pairs;                    // the scale pairs of every FP16 operand below
+  float* sdz[2] = {nullptr, nullptr};  // ... among them those of G.C1 / G.C2's dz
+  // activations and gradients (NHWC)
+  float *noise = nullptr, *z0 = nullptr, *h0 = nullptr, *z1 = nullptr, *h1 = nullptr, *z2 = nullptr, *h2 = nullptr,
+        *z3 = nullptr, *y = nullptr;
+  float *dz3 = nullptr, *dfull = nullptr, *dz2 = nullptr, *dz1 = nullptr, *dz0 = nullptr;
+  float *bn_mean[2] = {nullptr, nullptr}, *bn_istd[2] = {nullptr, nullptr}, *bn_mg = nullptr;
+  int B = 0;
+  bool train = true, valid = false;
+  int pack_key = -1;  // pack_key() of the weight packs
+  std::deque<std::string> names;  // prefixed timer names (stable storage: the layers point into it)
+  const char *t_bn2_finalize = nullptr, *t_bn2_stats = nullptr, *t_bn2_apply = nullptr, *t_bn2_bwd_reduce = nullptr,
+             *t_bn2_bwd_apply = nullptr;
+};
+
 struct TimerRec {
   double ms = 0;
   int64_t launches = 0;
@@ -189,7 +232,6 @@ struct fg_ctx {
   // OPT.D_optmethod / OPT.G_optmethod (train.lua:38-39): FG_OPT_ADAM | FG_OPT_ADAGRAD | FG_OPT_SGD, and SGD momentum
   int opt_D = 0, opt_G = 0;
   float sgd_mom_D = 0.f, sgd_mom_G = 0.f;
-  GLayout gl;
   DLayout dl;
   std::vector<void*> allocs;  // every cudaMalloc of net_alloc(), released by net_free()
   NetPair net;
@@ -211,22 +253,17 @@ struct fg_ctx {
   size_t red_ws_elems = 0;
   double* red_ws_opt = nullptr;  // [kOptRedRows]: the penalty-loss sum of the optimizer, which may run on comm_stream
   unsigned* red_ticket = nullptr;  // [0]: red_ws, [1]: red_ws_opt
-  // G activations (NHWC)
-  int G_B = 0;
-  bool G_train = true, G_fwd_valid = false;
-  float *G_noise = nullptr, *G_z0 = nullptr, *G_h0 = nullptr, *G_z1 = nullptr, *G_h1 = nullptr, *G_z2 = nullptr,
-        *G_h2 = nullptr, *G_z3 = nullptr, *G_y = nullptr;
+  // workspaces of the BatchNorm kernels, shared by the generators on this ctx's stream
   double* bn_slice_acc = nullptr;  // workspace of k_bn_finalize_parts: 32 slices x 2 x 256 doubles + tickets
   float* bn_parts = nullptr;  // [m-tile][2][C] BatchNorm partials written by the tensor-core conv epilogue
   int edge_impl = 1;          // option "edge_impl": 0 = the round-1 small-channel kernels (k_conv_small.cu) for G.C3 / D.C1
   int bn_epilogue = 1;        // option "bn_epilogue": 0 = separate statistics pass over z (the round-1 path)
   int mma_f16 = 1;            // option "mma_f16": 1 (default) = tensor-core operands in the 3xFP16 split (f16 MMAs); 0 = 3xTF32
-  float* amax_slot = nullptr; // [32] (max|x|, 1/scale) pairs on the device: power-of-two scales of the FP16-split operands
-  unsigned* amax_out = nullptr;  // when set (nets.cu AmaxInto), the next elementwise producer also reduces max|output| there ...
+  float* lop_sx = nullptr;  // (max|x|, 1/scale) pair of the L-op convolutions' FP16-split input (lop.cu) ...
+  float* lop_sy = nullptr;  // ... and of their dY
+  unsigned* amax_out = nullptr;  // when set (AmaxInto, convl.h), the next elementwise producer also reduces max|output| there ...
   bool* amax_done = nullptr;     // ... and sets *amax_done (a TcOp's amax_ready): its consumer skips its own reduction
   double* bn_acc = nullptr;  // [4][256] double accumulators (sum, sumsq / sum g, sum g xhat)
-  float *bn_mean1 = nullptr, *bn_istd1 = nullptr, *bn_mean2 = nullptr, *bn_istd2 = nullptr, *bn_mg = nullptr;
-  float *G_dz3 = nullptr, *G_dfull = nullptr, *G_dz2 = nullptr, *G_dz1 = nullptr, *G_dz0 = nullptr;
   // D activations (NHWC)
   int D_B = 0;
   bool D_train = true, D_fwd_valid = false;
@@ -273,12 +310,12 @@ struct fg_ctx {
   cudaEvent_t events[16] = {};
   bool timing = false;
   std::map<std::string, TimerRec> timers;
-  // the layers of G and D (D.L3 runs on the GEMV kernels) and the scratch they share: env.dy is the split of the current
-  // dY, env.ws = wgrad_ws.  Their FP16 scale pairs all live in amax_slot.
+  // G, the layers of D (D.L3 runs on the GEMV kernels) and the scratch they share: env.dy is the split of the current
+  // dY, env.ws = wgrad_ws.  D's FP16 scale pairs, env.dy's included, live in D_pairs.
   ConvLEnv env;
-  ConvL GL1, GC3, Dc[4], DL1, DL2;
-  UpsL GU[2];  // G.C1, G.C2
-  float* G_sdz[2] = {nullptr, nullptr};  // scale pairs of their dz (TcOp::s of the dz operand)
+  UpsGen G;
+  ConvL Dc[4], DL1, DL2;
+  ScalePairs D_pairs;
 };
 
 struct ScopedTimer {
@@ -407,10 +444,7 @@ void tc_destroy(fg_ctx* c);
 // ---- nets.cu ---------------------------------------------------------------------------------------
 int net_alloc(fg_ctx* c);
 void net_free(fg_ctx* c);
-int net_pack_G(fg_ctx* c);
 int net_pack_D(fg_ctx* c);
-int net_G_forward(fg_ctx* c, const float* noise_dev, int B, bool training);                 // -> c->G_y (NHWC)
-int net_G_backward(fg_ctx* c, const float* dy_nhwc, float* dnoise_dev);                      // accumulates c->gG
 int net_D_forward(fg_ctx* c, const float* x_nhwc, int B, bool training, const fg_hyper* h);  // masks in c->D_masks
 int net_D_backward(fg_ctx* c, const float* dlogit_dev, bool want_wgrad, bool want_dx);       // -> c->D_dx (NHWC)
 int net_train_step(fg_ctx* c, const fg_hyper* h, int B, const float* real_nchw_dev, const float* noiseD_dev,

@@ -82,10 +82,10 @@ int fg_conv2d_forward(fg_ctx* c, const float* x, const float* w, const float* b,
     float *xs, *ws;  // FP16 split: nx (nw) halves each for hi and lo = nx (nw) floats of scratch
     FG_TRY(scratch(c, 4, nx, &xs));
     FG_TRY(scratch(c, 7, nw, &ws));
-    FG_TRY(tc_amax(c, xn, (int64_t)nx, c->amax_slot + 60));  // activations are scaled into fp16's range as well
-    FG_TRY(tc_split_h(c, xn, xs, xs + nx / 2, (int64_t)nx, c->amax_slot + 60));
+    FG_TRY(tc_amax(c, xn, (int64_t)nx, c->lop_sx));  // activations are scaled into fp16's range as well
+    FG_TRY(tc_split_h(c, xn, xs, xs + nx / 2, (int64_t)nx, c->lop_sx));
     FG_TRY(tc_pack_split_h(c, wd, ws, ws + nw / 2, nullptr, nullptr, Cout, Cin, k * k));
-    FG_TRY(tc_conv_fwd(c, xs, xs + nx / 2, ws, ws + nw / 2, bd, yn, g, 0, nullptr, nullptr, 1, c->amax_slot + 61));
+    FG_TRY(tc_conv_fwd(c, xs, xs + nx / 2, ws, ws + nw / 2, bd, yn, g, 0, nullptr, nullptr, 1, c->lop_sx + 1));
   } else if (c->conv_impl != FG_CONV_SIMT && tc_conv_eligible(g)) {
     float *xs, *ws;
     FG_TRY(scratch(c, 4, 2 * nx, &xs));
@@ -121,10 +121,10 @@ int fg_conv2d_backward_data(fg_ctx* c, const float* dy, const float* w, float* d
     float *ys, *ws;  // the gradient is scaled by a power of two into fp16's range first (tc_amax), the kernel undoes it
     FG_TRY(scratch(c, 2, ny, &ys));
     FG_TRY(scratch(c, 7, 2 * nw, &ws));
-    FG_TRY(tc_amax(c, dyn, (int64_t)ny, c->amax_slot + 62));
-    FG_TRY(tc_split_h(c, dyn, ys, ys + ny / 2, (int64_t)ny, c->amax_slot + 62));
+    FG_TRY(tc_amax(c, dyn, (int64_t)ny, c->lop_sy));
+    FG_TRY(tc_split_h(c, dyn, ys, ys + ny / 2, (int64_t)ny, c->lop_sy));
     FG_TRY(tc_pack_split_h(c, wd, ws, ws + nw / 2, ws + nw, ws + nw + nw / 2, Cout, Cin, k * k));
-    FG_TRY(tc_conv_fwd(c, ys, ys + ny / 2, ws + nw, ws + nw + nw / 2, nullptr, dxn, gd, 0, nullptr, nullptr, 1, c->amax_slot + 63));
+    FG_TRY(tc_conv_fwd(c, ys, ys + ny / 2, ws + nw, ws + nw + nw / 2, nullptr, dxn, gd, 0, nullptr, nullptr, 1, c->lop_sy + 1));
   } else if (c->conv_impl != FG_CONV_SIMT && tc_conv_eligible(gd)) {
     float *ys, *ws;
     FG_TRY(scratch(c, 2, 2 * ny, &ys));
@@ -162,11 +162,11 @@ int fg_conv2d_backward_filter(fg_ctx* c, const float* x, const float* dy, float*
     float *xs, *ys;  // FP16 split; dY scaled into range by a power of two that the kernel undoes
     FG_TRY(scratch(c, 2, nx, &xs));
     FG_TRY(scratch(c, 7, ny, &ys));
-    FG_TRY(tc_amax(c, xn, (int64_t)nx, c->amax_slot + 60));
-    FG_TRY(tc_split_h(c, xn, xs, xs + nx / 2, (int64_t)nx, c->amax_slot + 60));
-    FG_TRY(tc_amax(c, dyn, (int64_t)ny, c->amax_slot + 62));
-    FG_TRY(tc_split_h(c, dyn, ys, ys + ny / 2, (int64_t)ny, c->amax_slot + 62));
-    FG_TRY(tc_conv_wgrad(c, xs, xs + nx / 2, ys, ys + ny / 2, ws, gw, 1, c->amax_slot + 63, c->amax_slot + 61));
+    FG_TRY(tc_amax(c, xn, (int64_t)nx, c->lop_sx));
+    FG_TRY(tc_split_h(c, xn, xs, xs + nx / 2, (int64_t)nx, c->lop_sx));
+    FG_TRY(tc_amax(c, dyn, (int64_t)ny, c->lop_sy));
+    FG_TRY(tc_split_h(c, dyn, ys, ys + ny / 2, (int64_t)ny, c->lop_sy));
+    FG_TRY(tc_conv_wgrad(c, xs, xs + nx / 2, ys, ys + ny / 2, ws, gw, 1, c->lop_sy + 1, c->lop_sx + 1));
   } else if (c->conv_impl != FG_CONV_SIMT && tc_conv_eligible(gw) && Cout % 128 == 0 && Cin % 64 == 0) {
     float *xs, *ys;
     FG_TRY(scratch(c, 2, 2 * nx, &xs));

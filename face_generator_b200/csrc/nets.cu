@@ -1,4 +1,4 @@
-// Orchestration of G (models.lua:57-81), D (models.lua:382-416) and the adversarial.lua loop body
+// Orchestration of G (models.lua:57-81; gen.cu), D (models.lua:382-416) and the adversarial.lua loop body
 // (adversarial.lua:54-300) on one stream.  Kernels live in k_elem.cu / k_conv_simt.cu / k_conv_tc.cu.
 #include <algorithm>
 
@@ -6,27 +6,6 @@
 #include "fg_internal.h"
 #include "k_conv_tc.h"
 
-GLayout make_g_layout(int C) {
-  GLayout L;
-  int64_t o = 0;
-  L.L1W = o; o += 8192 * 100;
-  L.L1b = o; o += 8192;
-  L.a1 = o; o += 1;
-  L.C1W = o; o += 256 * 128 * 25;
-  L.C1b = o; o += 256;
-  L.g1 = o; o += 256;
-  L.be1 = o; o += 256;
-  L.a2 = o; o += 1;
-  L.C2W = o; o += 128 * 256 * 25;
-  L.C2b = o; o += 128;
-  L.g2 = o; o += 128;
-  L.be2 = o; o += 128;
-  L.a3 = o; o += 1;
-  L.C3W = o; o += (int64_t)C * 128 * 9;
-  L.C3b = o; o += C;
-  L.total = o;
-  return L;
-}
 DLayout make_d_layout(int C) {
   DLayout L;
   const int cin[4] = {C, 64, 128, 256}, cout[4] = {64, 128, 256, 512};
@@ -52,23 +31,22 @@ namespace {
 const int kDcin[4] = {0 /*C*/, 64, 128, 256}, kDcout[4] = {64, 128, 256, 512}, kDhw[4] = {32, 16, 8, 4};
 const int kDmoff[4] = {0, 64, 192, 448};
 inline int dcin(const fg_ctx* c, int i) { return i == 0 ? c->C : kDcin[i]; }
-constexpr int kScalePairs = 32;  // (max|x|, 1/scale) pairs in c->amax_slot, handed out in net_alloc (see amax_reset)
 
 int dalloc(fg_ctx* c, float** p, size_t n) { return fg_dalloc(c, c->allocs, p, n); }
 }  // namespace
 
 int net_alloc(fg_ctx* c) {
   const size_t B = c->maxB, C = c->C;
-  c->gl = make_g_layout(c->C);
   c->dl = make_d_layout(c->C);
   NetPair& p = c->net;
-  FG_TRY(pair_alloc(c, c->allocs, p, c->gl.total, c->dl.total, true));
+  FG_TRY(pair_alloc(c, c->allocs, p, make_g_layout(c->C, 32).total, c->dl.total, true));
   p.optim_timer[0] = "hbm.optim.G";
   p.optim_timer[1] = "hbm.optim.D";
   c->ownPG = p.PG; c->ownPD = p.PD; c->ownGG = p.gG; c->ownGD = p.gD;
   FG_TRY(dalloc(c, &c->tail_sep, 2 * kGradTail));
   float* tmp = nullptr;
-  FG_TRY(dalloc(c, &c->amax_slot, 2 * kScalePairs));
+  FG_TRY(dalloc(c, &c->lop_sx, 2));
+  FG_TRY(dalloc(c, &c->lop_sy, 2));
   {
     float* sd = nullptr;
     FG_TRY(dalloc(c, &sd, 2));
@@ -85,31 +63,11 @@ int net_alloc(fg_ctx* c) {
   FG_TRY(dalloc(c, reinterpret_cast<float**>(&c->red_ticket), 2));  // zeroed; every ordered reduction resets its ticket
   FG_TRY(dalloc(c, reinterpret_cast<float**>(&c->bwd_claim), 1));
   FG_TRY(dalloc(c, &c->small_ws, (size_t)kSmallMaxParts * 9 * 4 * 128));
-  // G activations
-  FG_TRY(dalloc(c, &c->G_noise, B * kNoiseDim));
-  FG_TRY(dalloc(c, &c->G_z0, B * 8192));
-  FG_TRY(dalloc(c, &c->G_h0, B * 8192));
-  FG_TRY(dalloc(c, &c->G_z1, B * 65536));
-  FG_TRY(dalloc(c, &c->G_h1, B * 65536));
-  FG_TRY(dalloc(c, &c->G_z2, B * 131072));
-  FG_TRY(dalloc(c, &c->G_h2, B * 131072));
-  FG_TRY(dalloc(c, &c->G_z3, B * 1024 * C));
-  FG_TRY(dalloc(c, &c->G_y, B * 1024 * C));
   FG_TRY(dalloc(c, &tmp, 4 * 256 * 2));  // doubles
   c->bn_acc = (double*)tmp;
   FG_TRY(dalloc(c, &tmp, 32 * 2 * 256 * 2 + 64));  // doubles + tickets (zero-initialised)
   c->bn_slice_acc = (double*)tmp;
   FG_TRY(dalloc(c, &c->bn_parts, B * 2048));  // G.C2: 8 tiles/image x 2 x 128 ch; G.C1: 2 tiles/image x 2 x 256 ch
-  FG_TRY(dalloc(c, &c->bn_mean1, 256));
-  FG_TRY(dalloc(c, &c->bn_istd1, 256));
-  FG_TRY(dalloc(c, &c->bn_mean2, 128));
-  FG_TRY(dalloc(c, &c->bn_istd2, 128));
-  FG_TRY(dalloc(c, &c->bn_mg, 512));
-  FG_TRY(dalloc(c, &c->G_dz3, B * 1024 * C));
-  FG_TRY(dalloc(c, &c->G_dfull, B * 262144));
-  FG_TRY(dalloc(c, &c->G_dz2, B * 131072));
-  FG_TRY(dalloc(c, &c->G_dz1, B * 65536));
-  FG_TRY(dalloc(c, &c->G_dz0, B * 8192));
   // D activations
   FG_TRY(dalloc(c, &c->D_x, B * 1024 * C));
   for (int i = 0; i < 4; ++i) {
@@ -142,23 +100,18 @@ int net_alloc(fg_ctx* c) {
     e.ws = c->wgrad_ws;
     FG_TRY(dalloc(c, &e.dy.hi, B * 131072));
     FG_TRY(dalloc(c, &e.dy.lo, B * 131072));
-    int pairs = 0;  // every FP16-split operand gets its own scale pair in amax_slot
-    auto pair = [&]() { return c->amax_slot + 2 * pairs++; };
-    e.dy.s = pair();
-    const GLayout& gl = c->gl;
+    static const GenDesc g32{32, "", 128, true};  // G.L1 padded to K = 128 for the tensor cores; G.C1 / G.C2 may merge
+    FG_TRY(gen_alloc(e, c->G, g32));
+    ScalePairs& sp = c->D_pairs;  // every FP16-split operand of D gets its own scale pair
+    FG_TRY(sp.alloc(c, c->allocs, 1 + 2 * 6));
+    FG_TRY(sp.take(&e.dy.s));
     const DLayout& dl = c->dl;
     auto conv = [&](ConvL& L, int Cin, int Cout, int k, int H, int64_t w_off, int64_t b_off, const char* tf, const char* td,
                     const char* tw) {
       L.Cin = Cin; L.Cout = Cout; L.k = k; L.H = H;
       L.w_off = w_off; L.b_off = b_off;
       L.tf = tf; L.td = td; L.tw = tw;
-      L.x.s = pair();
-      L.sdy = pair();
     };
-    conv(c->GL1, kNoiseDim, 8192, 1, 1, gl.L1W, gl.L1b, "G.L1.fwd", "G.L1.dgrad", "G.L1.wgrad");
-    c->GL1.nA = 128; c->GL1.nS = 64;  // View(128,8,8): reference row c*64+s <-> our NHWC row s*128+c
-    c->GL1.kpad = 128;                 // K = 100 is no multiple of 32: zero-padded for the tensor cores
-    conv(c->GC3, 128, c->C, 3, 32, gl.C3W, gl.C3b, "G.C3.fwd", "G.C3.dgrad", "G.C3.wgrad");
     static const char* tf[4] = {"D.C1.fwd", "D.C2.fwd", "D.C3.fwd", "D.C4.fwd"};
     static const char* td[4] = {"D.C1.dgrad", "D.C2.dgrad", "D.C3.dgrad", "D.C4.dgrad"};
     static const char* tw[4] = {"D.C1.wgrad", "D.C2.wgrad", "D.C3.wgrad", "D.C4.wgrad"};
@@ -166,21 +119,10 @@ int net_alloc(fg_ctx* c) {
     conv(c->DL1, 2048, 512, 1, 1, dl.L1W, dl.L1b, "D.L1.fwd", "D.L1.dgrad", "D.L1.wgrad");
     c->DL1.cA = 512; c->DL1.cS = 4;  // View(2048) flattens [512][2][2] in (c,h,w) order; ours is NHWC (h,w,c)
     conv(c->DL2, 512, 512, 1, 1, dl.L2W, dl.L2b, "D.L2.fwd", "D.L2.dgrad", "D.L2.wgrad");
-    for (ConvL* L : {&c->GL1, &c->GC3, &c->Dc[0], &c->Dc[1], &c->Dc[2], &c->Dc[3], &c->DL1, &c->DL2}) FG_TRY(convl_alloc(e, *L));
-    const int ci[2] = {128, 256}, co[2] = {256, 128}, hs[2] = {16, 32};
-    static const char* uf[2] = {"G.C1.fwd", "G.C2.fwd"};
-    static const char* ud[2] = {"G.C1.dgrad", "G.C2.dgrad"};
-    static const char* uw[2] = {"G.C1.wgrad", "G.C2.wgrad"};
-    static const char* ub[2] = {"G.C1.wgrad+dgrad", "G.C2.wgrad+dgrad"};
-    const int64_t wo[2] = {gl.C1W, gl.C2W}, bo[2] = {gl.C1b, gl.C2b};
-    for (int i = 0; i < 2; ++i) {
-      UpsL& U = c->GU[i];
-      U.Cin = ci[i]; U.Cout = co[i]; U.H = hs[i];
-      U.w_off = wo[i]; U.b_off = bo[i];
-      U.tf = uf[i]; U.td = ud[i]; U.tw = uw[i]; U.tb = ub[i];
-      U.x.s = pair();
-      c->G_sdz[i] = pair();
-      FG_TRY(upsl_alloc(e, U));
+    for (ConvL* L : {&c->Dc[0], &c->Dc[1], &c->Dc[2], &c->Dc[3], &c->DL1, &c->DL2}) {
+      FG_TRY(sp.take(&L->x.s));
+      FG_TRY(sp.take(&L->sdy));
+      FG_TRY(convl_alloc(e, *L));
     }
   }
   FG_TRY(dalloc(c, &c->in_real, B * 1024 * C));
@@ -201,14 +143,6 @@ void net_free(fg_ctx* c) {
     if (c->scratch[i]) cudaFree(c->scratch[i]);
 }
 
-int net_pack_G(fg_ctx* c) {
-  if (c->net.G_packed) return FG_OK;
-  FG_TRY(convl_pack(c, c->GL1, c->net.PG));
-  for (int i = 0; i < 2; ++i) FG_TRY(upsl_pack(c, c->GU[i], c->net.PG));
-  FG_TRY(convl_pack(c, c->GC3, c->net.PG));
-  c->net.G_packed = true;
-  return FG_OK;
-}
 int net_pack_D(fg_ctx* c) {
   if (c->net.D_packed) return FG_OK;
   for (int i = 0; i < 4; ++i) FG_TRY(convl_pack(c, c->Dc[i], c->net.PD));
@@ -218,158 +152,13 @@ int net_pack_D(fg_ctx* c) {
   return FG_OK;
 }
 
-// ---- option "mma_f16": every tensor-core operand in the 3xFP16 split (k_conv_tc.cu), f16 MMAs -----------------------
-// Activations and gradients are scaled into fp16's range by a power of two found on the device: each operand (TcOp::s,
-// ConvL::sdy, G_sdz) has its own (max|x|, 1/scale) pair in c->amax_slot; the consuming kernels multiply their result by
-// the inverse scales.  A producer can reduce max|output| into the pair while it writes the tensor (AmaxInto) instead of a
-// separate read pass; amax_reset() zeroes the max words (not the inverse scales, which the weight-gradient kernels of a
-// later pass still need) at the start of every forward / backward pass.
-static int amax_reset(fg_ctx* c) {
-  if (!tc_f16(c)) return FG_OK;
-  FG_CUDA(cudaMemset2DAsync(c->amax_slot, 2 * sizeof(float), 0, sizeof(float), kScalePairs, c->stream));
-  return FG_OK;
-}
-struct AmaxInto {  // the ONE elementwise producer launched inside the scope reports max|output| into `pair` and sets *done
-  fg_ctx* c;
-  AmaxInto(fg_ctx* c_, TcOp& op) : AmaxInto(c_, op.s, &op.amax_ready) {}
-  AmaxInto(fg_ctx* c_, float* pair, bool* done) : c(c_) {
-    if (tc_f16(c)) {
-      c->amax_out = reinterpret_cast<unsigned*>(pair);
-      c->amax_done = done;
-    }
-  }
-  ~AmaxInto() { c->amax_out = nullptr; }
-};
-
-// ---------------------------------------------------------------------------------------------------
-// G
-// ---------------------------------------------------------------------------------------------------
-int net_G_forward(fg_ctx* c, const float* noise, int B, bool training) {
-  FG_REQUIRE(B >= 1 && B <= c->maxB, "G forward: batch %d out of range [1,%d]", B, c->maxB);
-  FG_TRY(net_pack_G(c));
-  const GLayout& L = c->gl;
-  float* P = c->net.PG;
-  if (noise != c->G_noise)
-    FG_CUDA(cudaMemcpyAsync(c->G_noise, noise, sizeof(float) * B * kNoiseDim, cudaMemcpyDeviceToDevice, c->stream));
-  c->G_B = B;
-  c->G_train = training;
-  FG_TRY(amax_reset(c));
-  FG_TRY(convl_fwd(c->env, c->GL1, c->G_noise, P, c->G_z0, B));
-  {
-    AmaxInto am(c, c->GU[0].x);
-    FG_TRY(k_prelu_fwd(c, c->G_z0, P + L.a1, c->G_h0, (int64_t)B * 8192));
-  }
-  // training: the BatchNorm statistics come out of the convolution's epilogue (per-tile partials) when it ran on
-  // the tensor cores; otherwise a separate pass over z computes them
-  int parts = training ? 1 : 0;
-  FG_TRY(upsl_fwd(c->env, c->GU[0], c->G_h0, P, c->G_z1, B, &parts));
-  if (training) {
-    if (parts) {
-      FG_TRY(k_bn_finalize_parts(c, c->bn_parts, parts, c->bn_mean1, c->bn_istd1, c->net.bnG, c->net.bnG + 256, (int64_t)B * 256, 256));
-    } else {
-      FG_TRY(k_bn_stats(c, c->G_z1, c->bn_acc, (int64_t)B * 256, 256));
-      FG_TRY(k_bn_finalize(c, c->bn_acc, c->bn_mean1, c->bn_istd1, c->net.bnG, c->net.bnG + 256, (int64_t)B * 256, 256));
-    }
-  } else {
-    FG_TRY(k_bn_eval_prep(c, c->net.bnG, c->net.bnG + 256, c->bn_mean1, c->bn_istd1, 256));
-  }
-  UpsL& C2 = c->GU[1];
-  C2.x.split_ready = training && upsl_tc(c, C2) && !tc_f16(c);  // the TF32 tensor-core path reads h1 only as its split
-  {
-    AmaxInto am(c, C2.x);
-    FG_TRY(k_bn_prelu_apply(c, c->G_z1, c->bn_mean1, c->bn_istd1, P + L.g1, P + L.be1, P + L.a2,
-                            c->G_h1, (int64_t)B * 256, 256, C2.x.split_ready ? C2.x.hi : nullptr,
-                            C2.x.split_ready ? C2.x.lo : nullptr));
-  }
-  parts = training ? 1 : 0;
-  FG_TRY(upsl_fwd(c->env, C2, c->G_h1, P, c->G_z2, B, &parts));
-  // "hbm.*" timers: the bandwidth-bound kernels bench.py reports against the measured HBM peak
-  if (training) {
-    if (parts) {
-      ScopedTimer tm(c, "G.bn2.finalize");
-      FG_TRY(k_bn_finalize_parts(c, c->bn_parts, parts, c->bn_mean2, c->bn_istd2, c->net.bnG + 512, c->net.bnG + 640, (int64_t)B * 1024, 128));
-    } else {
-      {
-        ScopedTimer tm(c, "hbm.G.bn2.stats");
-        FG_TRY(k_bn_stats(c, c->G_z2, c->bn_acc, (int64_t)B * 1024, 128));
-      }
-      FG_TRY(k_bn_finalize(c, c->bn_acc, c->bn_mean2, c->bn_istd2, c->net.bnG + 512, c->net.bnG + 640, (int64_t)B * 1024, 128));
-    }
-  } else {
-    FG_TRY(k_bn_eval_prep(c, c->net.bnG + 512, c->net.bnG + 640, c->bn_mean2, c->bn_istd2, 128));
-  }
-  {
-    ScopedTimer tm(c, "hbm.G.bn2.apply");
-    FG_TRY(k_bn_prelu_apply(c, c->G_z2, c->bn_mean2, c->bn_istd2, P + L.g2, P + L.be2, P + L.a3, c->G_h2, (int64_t)B * 1024,
-                            128));
-  }
-  FG_TRY(convl_fwd(c->env, c->GC3, c->G_h2, P, c->G_z3, B));
-  FG_TRY(k_sigmoid_fwd(c, c->G_z3, c->G_y, (int64_t)B * 1024 * c->C));
-  c->G_fwd_valid = true;
-  return FG_OK;
-}
-
-int net_G_backward(fg_ctx* c, const float* dy, float* dnoise) {
-  if (!c->G_fwd_valid || !c->G_train) {
-    fg_set_error("G backward needs a preceding training-mode G forward");
-    return FG_ERR_STATE;
-  }
-  const GLayout& L = c->gl;
-  float *P = c->net.PG, *G = c->net.gG;
-  const int B = c->G_B, C = c->C;
-  FG_TRY(amax_reset(c));
-  FG_TRY(k_sigmoid_bwd(c, dy, c->G_y, c->G_dz3, (int64_t)B * 1024 * C));
-  FG_TRY(convl_bwd(c->env, c->GC3, c->G_h2, c->G_dz3, G, c->G_dfull, B));
-  // BN2 + PReLU
-  {
-    ScopedTimer tm(c, "hbm.G.bn2.bwd_reduce");
-    FG_TRY(k_bn_prelu_bwd_reduce(c, c->G_dfull, c->G_z2, c->bn_mean2, c->bn_istd2, P + L.g2, P + L.be2, P + L.a3, c->bn_acc,
-                                 G + L.a3, B, 32, 32, 128, 0));
-  }
-  FG_TRY(k_bn_bwd_finalize(c, c->bn_acc, c->bn_mg, G + L.g2, G + L.be2, (int64_t)B * 1024, 128));
-  // in tensor-core mode the BN-backward kernels also emit the TF32 hi/lo split of dz (no separate split pass); with the
-  // FP16 split they reduce max|dz| into dz's own scale pair
-  const bool tf32 = !tc_f16(c);
-  TcOp dz2{c->env.dy.hi, c->env.dy.lo, c->G_sdz[1]};
-  dz2.split_ready = upsl_tc(c, c->GU[1]) && tf32;
-  {
-    ScopedTimer tm(c, "hbm.G.bn2.bwd_apply");
-    AmaxInto am(c, dz2);
-    FG_TRY(k_bn_prelu_bwd_apply(c, c->G_dfull, c->G_z2, c->bn_mean2, c->bn_istd2, P + L.g2, P + L.be2, P + L.a3, c->bn_mg,
-                                c->G_dz2, B, 32, 32, 128, 0, dz2.split_ready ? dz2.hi : nullptr, dz2.split_ready ? dz2.lo : nullptr,
-                                G + L.C2b));  // + the bias gradient of C2 (column sums of dz2) in the same pass
-  }
-  // C2
-  bool pooled = false;
-  FG_TRY(upsl_bwd(c->env, c->GU[1], dz2, c->G_h1, c->G_dz2, G, c->G_dfull, B, &pooled));
-  // BN1 + PReLU (the 2x2 sum = backward of the nearest upsample is folded into the loads)
-  FG_TRY(k_bn_prelu_bwd_reduce(c, c->G_dfull, c->G_z1, c->bn_mean1, c->bn_istd1, P + L.g1, P + L.be1, P + L.a2, c->bn_acc,
-                               G + L.a2, B, 16, 16, 256, pooled ? 0 : 1));
-  FG_TRY(k_bn_bwd_finalize(c, c->bn_acc, c->bn_mg, G + L.g1, G + L.be1, (int64_t)B * 256, 256));
-  TcOp dz1{c->env.dy.hi, c->env.dy.lo, c->G_sdz[0]};
-  dz1.split_ready = upsl_tc(c, c->GU[0]) && tf32 && pooled;
-  {
-    AmaxInto am(c, dz1);
-    FG_TRY(k_bn_prelu_bwd_apply(c, c->G_dfull, c->G_z1, c->bn_mean1, c->bn_istd1, P + L.g1, P + L.be1, P + L.a2, c->bn_mg,
-                                c->G_dz1, B, 16, 16, 256, pooled ? 0 : 1, dz1.split_ready ? dz1.hi : nullptr,
-                                dz1.split_ready ? dz1.lo : nullptr, G + L.C1b));
-  }
-  // C1
-  FG_TRY(upsl_bwd(c->env, c->GU[0], dz1, c->G_h0, c->G_dz1, G, c->G_dfull, B, &pooled));
-  {
-    AmaxInto am(c, c->GL1.sdy, &c->env.dy.amax_ready);
-    FG_TRY(k_prelu_bwd(c, c->G_dfull, c->G_z0, P + L.a1, c->G_dz0, G + L.a1, B, 8, 8, 128, pooled ? 0 : 1));
-  }
-  return convl_bwd(c->env, c->GL1, c->G_noise, c->G_dz0, G, dnoise, B);
-}
-
 // ---------------------------------------------------------------------------------------------------
 // D
 // ---------------------------------------------------------------------------------------------------
 int net_D_forward(fg_ctx* c, const float* x, int B, bool training, const fg_hyper* h) {
   FG_REQUIRE(B >= 1 && B <= c->maxB, "D forward: batch %d out of range [1,%d]", B, c->maxB);
   FG_TRY(net_pack_D(c));
-  FG_TRY(amax_reset(c));
+  FG_TRY(c->D_pairs.reset(c));
   const DLayout& L = c->dl;
   float* P = c->net.PD;
   if (x != c->D_x)
@@ -419,7 +208,7 @@ int net_D_backward(fg_ctx* c, const float* dlogit, bool want_wgrad, bool want_dx
   const int B = c->D_B;
   const float* masks = c->D_train ? c->D_masks : nullptr;
   const float scale = c->D_drop_scale, eval_scale = c->D_spatial_eval;
-  FG_TRY(amax_reset(c));
+  FG_TRY(c->D_pairs.reset(c));
   // L3
   if (want_wgrad) {
     ScopedTimer tm(c, "D.L3.wgrad");
@@ -472,9 +261,9 @@ static int train_step_body(fg_ctx* c, const fg_hyper* h, int B, const float* rea
   const size_t img = (size_t)C * 1024;
   const float world = (float)c->world;
   // ---- D step (adversarial.lua:240-268) ----
-  FG_TRY(net_G_forward(c, noiseD, Bh, true));  // createImages: G in training mode (nn_utils.lua:52)
+  FG_TRY(gen_forward(c->env, c->G, c->net, noiseD, Bh, true));  // createImages: G in training mode (nn_utils.lua:52)
   FG_TRY(k_nchw_to_nhwc(c, real, c->D_x, Bh, C, 1024));
-  FG_CUDA(cudaMemcpyAsync(c->D_x + Bh * img, c->G_y, sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
+  FG_CUDA(cudaMemcpyAsync(c->D_x + Bh * img, c->G.y, sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
   if (masksD)
     FG_CUDA(cudaMemcpyAsync(c->D_masks, masksD, sizeof(float) * (size_t)B * kMaskPerSample, cudaMemcpyDeviceToDevice,
                             c->stream));
@@ -524,7 +313,7 @@ static int train_step_body(fg_ctx* c, const fg_hyper* h, int B, const float* rea
     // while the collective is in flight the persistent convolution kernels leave a few SMs to it (FG_DP_RESERVE_SMS)
     static const int reserve = getenv("FG_DP_RESERVE_SMS") ? atoi(getenv("FG_DP_RESERVE_SMS")) : 0;
     c->reserve_sms = overlap ? reserve : 0;
-    const int r = net_G_forward(c, noiseG, B, true);
+    const int r = gen_forward(c->env, c->G, c->net, noiseG, B, true);
     c->reserve_sms = 0;
     FG_TRY(r);
   }
@@ -534,10 +323,10 @@ static int train_step_body(fg_ctx* c, const fg_hyper* h, int B, const float* rea
                             c->stream));
   else
     FG_TRY(k_masks_generate(c, c->D_masks, B, seed * 2 + 2, h->p_spatial, h->p_drop, seed_dev));
-  FG_TRY(net_D_forward(c, c->G_y, B, true, h));
+  FG_TRY(net_D_forward(c, c->G.y, B, true, h));
   FG_TRY(k_sigmoid_bce(c, c->D_logit, c->D_out, c->D_dlogit, &c->net.dstats->loss_G, c->net.tailG, B, B));
   FG_TRY(net_D_backward(c, c->D_dlogit, false, true));  // D's weight grads are discarded by the reference (:209 vs :92)
-  FG_TRY(net_G_backward(c, c->D_dx, nullptr));
+  FG_TRY(gen_backward(c->env, c->G, c->net, c->D_dx, nullptr));
   FG_TRY(pair_allreduce_grads(c, c->net, FG_NET_G));
   FG_TRY(pair_gate(c, c->net, FG_NET_G, h, B, world));
   FG_TRY(pair_optim(c, c->net, FG_NET_G, h, 1.0f / world));

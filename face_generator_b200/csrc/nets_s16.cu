@@ -7,8 +7,7 @@
 //                       conv(512->1024,3,STRIDE 2) PReLU SpatialDropout() View(4096) Linear(4096,1024) PReLU
 //         dense branch: View(C*256) Linear(C*256,128) PReLU Dropout() Linear(128,128) PReLU
 //   loop = adversarial.lua:83-288 (the same fevalD / fevalG_on_D / accuracy gate / interruptable optimizers as the 32x32 nets)
-// Kernels: the two upsampled 5x5 layers are UpsL layers like the 32x32 generator's (forward with BatchNorm partials
-// from the epilogue, wgrad, dgrad with the upsample backward folded in); every other layer is a ConvL (convl.h).  A
+// Kernels: G16 is the 32x32 nets' generator type at side 16 (UpsGen, gen.cu); every layer of D16 is a ConvL (convl.h).  A
 // stride-2 "same" 3x3 convolution is the stride-1 one sampled at the even pixels: forward = stride-1 kernel + subsample,
 // backward = the stride-1 dgrad / wgrad of dY with zeros inserted at the odd pixels.  That is exact (the inserted zeros
 // contribute nothing) and keeps both layers on the tensor cores at 4x their minimal FLOPs, which is 0.2 ms at batch 256.
@@ -109,14 +108,7 @@ struct fg_s16 {
   fg_ctx* c = nullptr;
   int maxB = 0, C = 3;
   NetPair net;  // bnG: the running mean / var of G's two BatchNorm layers
-  // G
-  ConvL GL1, GC3;
-  UpsL GU[2];
-  int64_t Ga[3] = {0, 0, 0}, Gg[2] = {0, 0}, Gbe[2] = {0, 0};
-  float *G_x = nullptr, *G_z0 = nullptr, *G_h0 = nullptr, *G_z1 = nullptr, *G_h1 = nullptr, *G_z2 = nullptr, *G_h2 = nullptr,
-        *G_z3 = nullptr, *G_y = nullptr;
-  float *bn_mean[2] = {nullptr, nullptr}, *bn_istd[2] = {nullptr, nullptr}, *bn_mg = nullptr;
-  float *G_dz3 = nullptr, *G_dfull = nullptr, *G_dz = nullptr, *G_dz0 = nullptr;
+  UpsGen G;
   // D
   ConvL Dc[4], DF1, DE1, DE2;
   int64_t Dca[4] = {0, 0, 0, 0}, Daf = 0, Dae1 = 0, Dae2 = 0, DJW = 0, DJb = 0;
@@ -127,9 +119,9 @@ struct fg_s16 {
   // shared scratch
   float *ga = nullptr, *gb = nullptr, *ws = nullptr;
   float *in_a = nullptr, *in_b = nullptr, *in_c = nullptr, *in_m1 = nullptr, *in_m2 = nullptr, *io = nullptr;
-  int G_pack_impl = -1, D_pack_impl = -1;
-  int G_B = 0, D_B = 0;
-  bool G_valid = false, G_train = true, D_valid = false, D_train = true;
+  int D_pack_impl = -1;
+  int D_B = 0;
+  bool D_valid = false, D_train = true;
   // option "debug_keep" (tests): the D step's D_z[0..3], D_zf, D_ze1, D_ze2, D_logit, D_out, which the G step's D
   // forward overwrites
   float* keep_D[9] = {};
@@ -141,38 +133,8 @@ struct fg_s16 {
 namespace {
 int dalloc(fg_s16* n, float** p, size_t elems) { return convl_dalloc(n->env, p, elems); }
 
-void make_layouts(fg_s16* n) {
+void make_d16_layout(fg_s16* n) {
   const int C = n->C;
-  {  // G16Layout: getParameters() order of models.lua:27-51
-    int64_t o = 0;
-    ConvL& L1 = n->GL1;
-    L1.Cin = 100; L1.Cout = 2048; L1.k = 1; L1.H = 1;
-    L1.nA = 128; L1.nS = 16;  // View(128,4,4): reference row c*16+s <-> our NHWC row s*128+c
-    L1.w_off = o; o += 2048 * 100;
-    L1.b_off = o; o += 2048;
-    L1.tf = "s16.G.L1.fwd"; L1.td = "s16.G.L1.dgrad"; L1.tw = "s16.G.L1.wgrad";
-    n->Ga[0] = o; o += 1;
-    const int ci[2] = {128, 256}, co[2] = {256, 128}, hs[2] = {8, 16};
-    static const char* tf[2] = {"s16.G.C1.fwd", "s16.G.C2.fwd"};
-    static const char* td[2] = {"s16.G.C1.dgrad", "s16.G.C2.dgrad"};
-    static const char* tw[2] = {"s16.G.C1.wgrad", "s16.G.C2.wgrad"};
-    for (int i = 0; i < 2; ++i) {
-      UpsL& U = n->GU[i];
-      U.Cin = ci[i]; U.Cout = co[i]; U.H = hs[i];
-      U.w_off = o; o += (int64_t)co[i] * ci[i] * 25;
-      U.b_off = o; o += co[i];
-      n->Gg[i] = o; o += co[i];
-      n->Gbe[i] = o; o += co[i];
-      n->Ga[i + 1] = o; o += 1;
-      U.tf = tf[i]; U.td = td[i]; U.tw = tw[i];
-    }
-    ConvL& C3 = n->GC3;
-    C3.Cin = 128; C3.Cout = C; C3.k = 3; C3.H = kSide;
-    C3.w_off = o; o += (int64_t)C * 128 * 9;
-    C3.b_off = o; o += C;
-    C3.tf = "s16.G.C3.fwd"; C3.td = "s16.G.C3.dgrad"; C3.tw = "s16.G.C3.wgrad";
-    n->net.nG = o;
-  }
   {  // D16Layout: conv branch, dense branch, joint Linear (ConcatTable order, models.lua:306-313)
     const int ci[4] = {C, 128, 128, 512}, co[4] = {128, 128, 512, 1024}, hw[4] = {16, 16, 8, 4};  // stride-1 sides
     static const char* tf[4] = {"s16.D.c1.fwd", "s16.D.c2.fwd", "s16.D.c3.fwd", "s16.D.c4.fwd"};
@@ -215,33 +177,11 @@ void make_layouts(fg_s16* n) {
 
 int s16_alloc(fg_s16* n) {
   const size_t B = n->maxB, C = n->C;
-  make_layouts(n);
+  make_d16_layout(n);
   n->env.c = n->c;
   n->env.maxB = n->maxB;
   n->env.allocs = &n->allocs;
-  FG_TRY(pair_alloc(n->c, n->allocs, n->net, n->net.nG, n->net.nD, true));
-  // ---- G ----
-  FG_TRY(convl_alloc(n->env, n->GL1));
-  FG_TRY(convl_alloc(n->env, n->GC3));
-  for (int i = 0; i < 2; ++i) FG_TRY(upsl_alloc(n->env, n->GU[i]));
-  FG_TRY(dalloc(n, &n->G_x, B * 100));
-  FG_TRY(dalloc(n, &n->G_z0, B * 2048));
-  FG_TRY(dalloc(n, &n->G_h0, B * 2048));
-  FG_TRY(dalloc(n, &n->G_z1, B * 64 * 256));
-  FG_TRY(dalloc(n, &n->G_h1, B * 64 * 256));
-  FG_TRY(dalloc(n, &n->G_z2, B * 256 * 128));
-  FG_TRY(dalloc(n, &n->G_h2, B * 256 * 128));
-  FG_TRY(dalloc(n, &n->G_z3, B * 256 * C));
-  FG_TRY(dalloc(n, &n->G_y, B * 256 * C));
-  for (int i = 0; i < 2; ++i) {
-    FG_TRY(dalloc(n, &n->bn_mean[i], 256));
-    FG_TRY(dalloc(n, &n->bn_istd[i], 256));
-  }
-  FG_TRY(dalloc(n, &n->bn_mg, 512));
-  FG_TRY(dalloc(n, &n->G_dz3, B * 256 * C));
-  FG_TRY(dalloc(n, &n->G_dfull, B * 256 * 256));  // full-resolution dgrad of C2 on the FFMA path: [B][16][16][256]
-  FG_TRY(dalloc(n, &n->G_dz, B * 256 * 128));
-  FG_TRY(dalloc(n, &n->G_dz0, B * 2048));
+  FG_TRY(pair_alloc(n->c, n->allocs, n->net, make_g_layout(n->C, kSide).total, n->net.nD, true));
   // ---- D ----
   for (int i = 0; i < 4; ++i) FG_TRY(convl_alloc(n->env, n->Dc[i]));
   FG_TRY(convl_alloc(n->env, n->DF1));
@@ -281,6 +221,9 @@ int s16_alloc(fg_s16* n) {
   FG_TRY(dalloc(n, &n->env.dy.lo, big));
   FG_TRY(dalloc(n, &n->ws, (size_t)9 * 1024 * 512));  // largest weight tensor (c4); F1 is 4096*1024, the 5x5 packs 36*256*128
   n->env.ga = n->ga; n->env.ws = n->ws;
+  // G.L1 keeps K = 100 (on the FFMA kernels): padding it would change its bits.  Two backward launches per 5x5 layer.
+  static const GenDesc g16{kSide, "s16.", 0, false};
+  FG_TRY(gen_alloc(n->env, n->G, g16));
   FG_TRY(dalloc(n, &n->in_a, B * 256 * C));
   FG_TRY(dalloc(n, &n->in_b, B * 100));
   FG_TRY(dalloc(n, &n->in_c, B * 100));
@@ -291,16 +234,6 @@ int s16_alloc(fg_s16* n) {
   return FG_OK;
 }
 
-int pack_G(fg_s16* n) {
-  fg_ctx* c = n->c;
-  if (n->net.G_packed && n->G_pack_impl == pack_key(c)) return FG_OK;
-  FG_TRY(convl_pack(c, n->GL1, n->net.PG));
-  FG_TRY(convl_pack(c, n->GC3, n->net.PG));
-  for (int i = 0; i < 2; ++i) FG_TRY(upsl_pack(c, n->GU[i], n->net.PG));
-  n->net.G_packed = true;
-  n->G_pack_impl = pack_key(c);
-  return FG_OK;
-}
 int pack_D(fg_s16* n) {
   fg_ctx* c = n->c;
   if (n->net.D_packed && n->D_pack_impl == pack_key(c)) return FG_OK;
@@ -311,78 +244,6 @@ int pack_D(fg_s16* n) {
   n->net.D_packed = true;
   n->D_pack_impl = pack_key(c);
   return FG_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------
-// G16
-// ---------------------------------------------------------------------------------------------------
-// BatchNorm statistics of layer i (0: 256 channels at 8x8, 1: 128 channels at 16x16) -> bn_mean / bn_istd
-int bn_stats(fg_s16* n, int i, const float* z, int B, bool training, int parts) {
-  fg_ctx* c = n->c;
-  const int Cc = i == 0 ? 256 : 128;
-  const int64_t P = (int64_t)B * (i == 0 ? 64 : 256);
-  float *rm = n->net.bnG + (i == 0 ? 0 : 512), *rv = rm + Cc;
-  if (!training) return k_bn_eval_prep(c, rm, rv, n->bn_mean[i], n->bn_istd[i], Cc);
-  if (parts) return k_bn_finalize_parts(c, c->bn_parts, parts, n->bn_mean[i], n->bn_istd[i], rm, rv, P, Cc);
-  FG_TRY(k_bn_stats(c, z, c->bn_acc, P, Cc));
-  return k_bn_finalize(c, c->bn_acc, n->bn_mean[i], n->bn_istd[i], rm, rv, P, Cc);
-}
-
-// noise: device [B][100]; the image lands in G_y (NHWC [B][16][16][C])
-int G_forward(fg_s16* n, const float* noise, int B, bool training) {
-  fg_ctx* c = n->c;
-  FG_REQUIRE(B >= 1 && B <= n->maxB, "s16 G forward: batch %d out of range [1,%d]", B, n->maxB);
-  FG_TRY(pack_G(n));
-  const float* P = n->net.PG;
-  if (noise != n->G_x) FG_CUDA(cudaMemcpyAsync(n->G_x, noise, sizeof(float) * B * 100, cudaMemcpyDeviceToDevice, c->stream));
-  FG_TRY(convl_fwd(n->env, n->GL1, n->G_x, P, n->G_z0, B));
-  FG_TRY(k_prelu_fwd(c, n->G_z0, P + n->Ga[0], n->G_h0, (int64_t)B * 2048));
-  int parts = training ? 1 : 0;
-  FG_TRY(upsl_fwd(n->env, n->GU[0], n->G_h0, P, n->G_z1, B, &parts));
-  FG_TRY(bn_stats(n, 0, n->G_z1, B, training, parts));
-  FG_TRY(k_bn_prelu_apply(c, n->G_z1, n->bn_mean[0], n->bn_istd[0], P + n->Gg[0], P + n->Gbe[0], P + n->Ga[1], n->G_h1,
-                          (int64_t)B * 64, 256));
-  parts = training ? 1 : 0;
-  FG_TRY(upsl_fwd(n->env, n->GU[1], n->G_h1, P, n->G_z2, B, &parts));
-  FG_TRY(bn_stats(n, 1, n->G_z2, B, training, parts));
-  FG_TRY(k_bn_prelu_apply(c, n->G_z2, n->bn_mean[1], n->bn_istd[1], P + n->Gg[1], P + n->Gbe[1], P + n->Ga[2], n->G_h2,
-                          (int64_t)B * 256, 128));
-  FG_TRY(convl_fwd(n->env, n->GC3, n->G_h2, P, n->G_z3, B));
-  FG_TRY(k_sigmoid_fwd(c, n->G_z3, n->G_y, (int64_t)B * 256 * n->C));
-  n->G_B = B;
-  n->G_train = training;
-  n->G_valid = true;
-  return FG_OK;
-}
-// dy: NHWC [B][16][16][C]; accumulates into gG; dnoise (device [B][100]) may be null
-int G_backward(fg_s16* n, const float* dy, float* dnoise) {
-  fg_ctx* c = n->c;
-  if (!n->G_valid || !n->G_train) {
-    fg_set_error("s16 G backward needs a preceding training-mode G forward");
-    return FG_ERR_STATE;
-  }
-  const int B = n->G_B;
-  const float* P = n->net.PG;
-  float* G = n->net.gG;
-  FG_TRY(k_sigmoid_bwd(c, dy, n->G_y, n->G_dz3, (int64_t)B * 256 * n->C));
-  FG_TRY(convl_bwd(n->env, n->GC3, n->G_h2, n->G_dz3, G, n->G_dfull, B));
-  bool pooled = false;
-  // BN2 + PReLU, C2
-  FG_TRY(k_bn_prelu_bwd_reduce(c, n->G_dfull, n->G_z2, n->bn_mean[1], n->bn_istd[1], P + n->Gg[1], P + n->Gbe[1], P + n->Ga[2],
-                               c->bn_acc, G + n->Ga[2], B, 16, 16, 128, 0));
-  FG_TRY(k_bn_bwd_finalize(c, c->bn_acc, n->bn_mg, G + n->Gg[1], G + n->Gbe[1], (int64_t)B * 256, 128));
-  FG_TRY(k_bn_prelu_bwd_apply(c, n->G_dfull, n->G_z2, n->bn_mean[1], n->bn_istd[1], P + n->Gg[1], P + n->Gbe[1], P + n->Ga[2],
-                              n->bn_mg, n->G_dz, B, 16, 16, 128, 0, nullptr, nullptr, G + n->GU[1].b_off));
-  FG_TRY(upsl_bwd(n->env, n->GU[1], n->env.dy, n->G_h1, n->G_dz, G, n->G_dfull, B, &pooled));
-  // BN1 + PReLU, C1 (the 2x2 sum = backward of the nearest upsample is folded into the loads when not pooled yet)
-  FG_TRY(k_bn_prelu_bwd_reduce(c, n->G_dfull, n->G_z1, n->bn_mean[0], n->bn_istd[0], P + n->Gg[0], P + n->Gbe[0], P + n->Ga[1],
-                               c->bn_acc, G + n->Ga[1], B, 8, 8, 256, pooled ? 0 : 1));
-  FG_TRY(k_bn_bwd_finalize(c, c->bn_acc, n->bn_mg, G + n->Gg[0], G + n->Gbe[0], (int64_t)B * 64, 256));
-  FG_TRY(k_bn_prelu_bwd_apply(c, n->G_dfull, n->G_z1, n->bn_mean[0], n->bn_istd[0], P + n->Gg[0], P + n->Gbe[0], P + n->Ga[1],
-                              n->bn_mg, n->G_dz, B, 8, 8, 256, pooled ? 0 : 1, nullptr, nullptr, G + n->GU[0].b_off));
-  FG_TRY(upsl_bwd(n->env, n->GU[0], n->env.dy, n->G_h0, n->G_dz, G, n->G_dfull, B, &pooled));
-  FG_TRY(k_prelu_bwd(c, n->G_dfull, n->G_z0, P + n->Ga[0], n->G_dz0, G + n->Ga[0], B, 4, 4, 128, pooled ? 0 : 1));
-  return convl_bwd(n->env, n->GL1, n->G_x, n->G_dz0, G, dnoise, B);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -521,9 +382,9 @@ int train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const flo
   const size_t img = (size_t)C * 256;
   const float inv_world = 1.0f / (float)c->world;
   // ---- D step (adversarial.lua:240-268) ----
-  FG_TRY(G_forward(n, noiseD, Bh, true));  // createImages: G in training mode (nn_utils.lua:52)
+  FG_TRY(gen_forward(n->env, n->G, n->net, noiseD, Bh, true));  // createImages: G in training mode (nn_utils.lua:52)
   FG_TRY(k_nchw_to_nhwc(c, real, n->D_x, Bh, C, 256));
-  FG_CUDA(cudaMemcpyAsync(n->D_x + Bh * img, n->G_y, sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
+  FG_CUDA(cudaMemcpyAsync(n->D_x + Bh * img, n->G.y, sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
   if (masksD)
     FG_CUDA(cudaMemcpyAsync(n->D_masks, masksD, sizeof(float) * (size_t)B * kS16Mask, cudaMemcpyDeviceToDevice, c->stream));
   else
@@ -538,15 +399,15 @@ int train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const flo
   FG_TRY(pair_optim(c, n->net, FG_NET_D, h, inv_world));
   // ---- G step (adversarial.lua:275-288) ----
   FG_TRY(pair_zero_grads(c, n->net, FG_NET_G));
-  FG_TRY(G_forward(n, noiseG, B, true));
+  FG_TRY(gen_forward(n->env, n->G, n->net, noiseG, B, true));
   if (masksG)
     FG_CUDA(cudaMemcpyAsync(n->D_masks, masksG, sizeof(float) * (size_t)B * kS16Mask, cudaMemcpyDeviceToDevice, c->stream));
   else
     FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * kS16Mask, 2, 0.5f, c->seed_dev));
-  FG_TRY(D_forward(n, n->G_y, B, true));
+  FG_TRY(D_forward(n, n->G.y, B, true));
   FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_G, n->net.tailG, B, B));
   FG_TRY(D_backward(n, n->D_dlogit, false, true));  // D's weight grads are discarded by the reference (:209 vs :92)
-  FG_TRY(G_backward(n, n->D_dx, nullptr));
+  FG_TRY(gen_backward(n->env, n->G, n->net, n->D_dx, nullptr));
   FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_G));
   FG_TRY(pair_gate(c, n->net, FG_NET_G, h, B, (float)c->world));
   FG_TRY(pair_optim(c, n->net, FG_NET_G, h, inv_world));
@@ -606,10 +467,11 @@ int fg_s16_destroy(fg_s16* n) {
   return FG_OK;
 }
 int64_t fg_s16_param_count(int net, int channels) {
+  if (net != FG_NET_D) return make_g_layout(channels, kSide).total;
   fg_s16 tmp;
   tmp.C = channels;
-  make_layouts(&tmp);
-  return net == FG_NET_D ? tmp.net.nD : tmp.net.nG;
+  make_d16_layout(&tmp);
+  return tmp.net.nD;
 }
 int fg_s16_mask_per_sample(void) { return kS16Mask; }
 
@@ -662,9 +524,9 @@ int fg_s16_G_forward(fg_s16* n, const float* noise, int B, int training, float* 
   FG_REQUIRE(noise && B >= 1 && B <= n->maxB, "fg_s16_G_forward: bad arguments (batch %d, max %d)", B, n->maxB);
   const float* nd;
   FG_TRY(fg_to_dev(n->c, noise, (size_t)B * 100, n->in_b, &nd));
-  FG_TRY(G_forward(n, nd, B, training != 0));
+  FG_TRY(gen_forward(n->env, n->G, n->net, nd, B, training != 0));
   if (img_out) {
-    FG_TRY(k_nhwc_to_nchw(n->c, n->G_y, n->io, B, n->C, 256));
+    FG_TRY(k_nhwc_to_nchw(n->c, n->G.y, n->io, B, n->C, 256));
     FG_TRY(fg_to_user(n->c, img_out, n->io, (size_t)B * n->C * 256));
   }
   return FG_OK;
@@ -673,10 +535,10 @@ int fg_s16_G_backward(fg_s16* n, const float* d_img, float* d_noise) {
   ENTER(n);
   FG_REQUIRE(d_img, "fg_s16_G_backward: null gradient");
   const float* dd;
-  FG_TRY(fg_to_dev(n->c, d_img, (size_t)n->G_B * n->C * 256, n->in_a, &dd));
-  FG_TRY(k_nchw_to_nhwc(n->c, dd, n->io, n->G_B, n->C, 256));
-  FG_TRY(G_backward(n, n->io, d_noise ? n->in_c : nullptr));
-  if (d_noise) FG_TRY(fg_to_user(n->c, d_noise, n->in_c, (size_t)n->G_B * 100));
+  FG_TRY(fg_to_dev(n->c, d_img, (size_t)n->G.B * n->C * 256, n->in_a, &dd));
+  FG_TRY(k_nchw_to_nhwc(n->c, dd, n->io, n->G.B, n->C, 256));
+  FG_TRY(gen_backward(n->env, n->G, n->net, n->io, d_noise ? n->in_c : nullptr));
+  if (d_noise) FG_TRY(fg_to_user(n->c, d_noise, n->in_c, (size_t)n->G.B * 100));
   return FG_OK;
 }
 int fg_s16_D_forward(fg_s16* n, const float* img, int B, int training, const float* masks, uint64_t seed, float* out) {
@@ -755,13 +617,9 @@ int64_t fg_s16_debug_tensor(fg_s16* n, const char* name, float* dst, int64_t max
     return -1;
   }
   cudaSetDevice(n->c->device);
-  const int gb = n->G_B, db = n->D_B, kb = n->keep_B, sb = n->G_valid ? 1 : 0;
-  auto g = [&](const float* p) { return n->G_valid ? p : nullptr; };
+  const int db = n->D_B, kb = n->keep_B;
   auto d = [&](const float* p) { return n->D_valid ? p : nullptr; };
-  const DebugTensor ents[] = {
-      {"G.z0", g(n->G_z0), 2048, gb}, {"G.z1", g(n->G_z1), 64 * 256, gb}, {"G.z2", g(n->G_z2), 256 * 128, gb},
-      {"G.z3", g(n->G_z3), 256 * n->C, gb}, {"G.bn_mean1", g(n->bn_mean[0]), 256, sb}, {"G.bn_istd1", g(n->bn_istd[0]), 256, sb},
-      {"G.bn_mean2", g(n->bn_mean[1]), 128, sb}, {"G.bn_istd2", g(n->bn_istd[1]), 128, sb},
+  std::vector<DebugTensor> ents = {
       {"D.z1", d(n->D_z[0]), 256 * 128, db}, {"D.z2", d(n->D_z[1]), 256 * 128, db}, {"D.z3", d(n->D_z[2]), 16 * 512, db},
       {"D.z4", d(n->D_z[3]), 4 * 1024, db}, {"D.p1", d(n->D_p1), 64 * 128, db}, {"D.zf", d(n->D_zf), 1024, db},
       {"D.ze1", d(n->D_ze1), 128, db}, {"D.ze2", d(n->D_ze2), 128, db}, {"D.logit", d(n->D_logit), 1, db},
@@ -769,7 +627,8 @@ int64_t fg_s16_debug_tensor(fg_s16* n, const char* name, float* dst, int64_t max
       {"Dstep.z3", n->keep_D[2], 16 * 512, kb}, {"Dstep.z4", n->keep_D[3], 4 * 1024, kb}, {"Dstep.zf", n->keep_D[4], 1024, kb},
       {"Dstep.ze1", n->keep_D[5], 128, kb}, {"Dstep.ze2", n->keep_D[6], 128, kb}, {"Dstep.logit", n->keep_D[7], 1, kb},
       {"Dstep.out", n->keep_D[8], 1, kb}};
-  return debug_tensor_copy(n->c, "fg_s16_debug_tensor", ents, sizeof(ents) / sizeof(ents[0]), name, dst, max_elems);
+  gen_debug_rows(n->G, ents);
+  return debug_tensor_copy(n->c, "fg_s16_debug_tensor", ents.data(), ents.size(), name, dst, max_elems);
 }
 
 }  // extern "C"

@@ -1,0 +1,262 @@
+"""Bit-for-bit A/B of two builds of libfg_b200.so.
+
+`run` loads the library at --lib, and for each case (net, batch, options) runs 3 host-fed and 3 device-fed seeded train
+steps, then one G forward / G backward / D forward / D backward call.  It writes every piece of state as .npy under
+--out/<case>/: parameters, gradients, optimizer m / v / t, BatchNorm running state, the step statistics, the outputs
+of those calls and the generator's debug tensors, plus the kernel launches of each step (launches.json).  The L-op
+convolutions (fg_conv2d_*) with the 3xFP16 split are one more case.  `compare A B` reports, per case, the first array
+that differs and the launches per step of both builds.
+
+One build per process: both libraries export the same symbols.
+
+usage:  python profiles/ab_state.py run --lib face_generator_b200/libfg_b200.so --out /tmp/ab/new [--only 32,s16,c2f,lop]
+        python profiles/ab_state.py compare /tmp/ab/old /tmp/ab/new
+"""
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+
+C = 3
+OPTS_32 = [("default", {}), ("mma_f16=0", {"mma_f16": 0}), ("conv_impl=0", {"conv_impl": 0}),
+           ("conv_impl=1", {"conv_impl": 1}), ("bn_epilogue=0", {"bn_epilogue": 0}), ("edge_impl=0", {"edge_impl": 0}),
+           ("bwd_merge=0", {"bwd_merge": 0}), ("bwd_merge=2", {"bwd_merge": 2}), ("use_graph=0", {"use_graph": 0})]
+OPTS_S16 = OPTS_32[:4]
+G_DEBUG_32 = ["G." + n for n in ("z0", "h0", "z1", "h1", "z2", "h2", "z3", "y", "dz2", "dz1", "dz0",
+                                 "bn_mean1", "bn_istd1", "bn_mean2", "bn_istd2")]
+G_DEBUG_S16 = ["G." + n for n in ("z0", "z1", "z2", "z3", "bn_mean1", "bn_istd1", "bn_mean2", "bn_istd2")]
+
+
+def f32(a):
+    return np.ascontiguousarray(a, np.float32)
+
+
+def pair_state(net, bn):
+    from face_generator_b200.lib import NET_D, NET_G
+    out = {}
+    for k, w in ((NET_G, "G"), (NET_D, "D")):
+        m, v, t = net.get_adam_state(k)
+        out.update({"params_" + w: net.get_params(k), "grads_" + w: net.get_grads(k), "adam_m_" + w: m, "adam_v_" + w: v,
+                    "adam_t_" + w: np.array([t])})
+    if bn:
+        out["bn_state"] = net.get_bn_state()
+    return out
+
+
+def stats_array(st):
+    return np.concatenate([np.ravel(np.asarray(st[k], np.float64)) for k in sorted(st)])
+
+
+def steps(ctx, out, host_step, dev_step):
+    """3 host-fed, then 3 device-fed steps (eager, captured, replayed where the net captures graphs)"""
+    launches = []
+    for i in range(6):
+        l0 = ctx.launches()
+        st = host_step(10 + i) if i < 3 else dev_step(10 + i)
+        ctx.sync()
+        launches.append(ctx.launches() - l0)
+        out["stats_%d" % i] = stats_array(st)
+    return launches
+
+
+def case_32(B, opts, imgs):
+    import face_generator_b200 as fg
+    from face_generator_b200 import layouts as LY
+    from face_generator_b200.dataset import DeviceDataset
+    from face_generator_b200.lib import NET_D, NET_G
+    rng = np.random.default_rng(7)
+    ctx = fg.Context(0, max_batch=B, channels=C)
+    for k, v in opts.items():
+        ctx.set_option(k, v)
+    ctx.set_params(NET_G, LY.trained_like_init(LY.G_layout(C), rng))
+    ctx.set_params(NET_D, LY.trained_like_init(LY.D_layout(C), rng, 1.4))
+    ds = DeviceDataset(ctx, imgs)
+    h = fg.hyper_default()
+    out = {}
+
+    def host(seed):
+        real = f32(rng.random((B // 2, C, 32, 32)))
+        return ctx.train_step(h, B, real, f32(rng.uniform(-1, 1, (B // 2, 100))), f32(rng.uniform(-1, 1, (B, 100))),
+                              None, None, seed)
+
+    launches = steps(ctx, out, host, lambda seed: ds.train_step(h, B, seed))
+    out.update(pair_state(ctx, True))
+    out["G_forward"] = ctx.G_forward(f32(rng.uniform(-1, 1, (B, 100))), training=True)
+    out["G_backward.dnoise"] = ctx.G_backward(f32(rng.standard_normal((B, C, 32, 32)) * 1e-2), want_dnoise=True)
+    for n in G_DEBUG_32:
+        out["debug." + n] = ctx.debug_tensor(n)
+    out["D_forward"] = ctx.D_forward(f32(rng.random((B, C, 32, 32))), None, True, 3)
+    out["D_backward.dimages"] = ctx.D_backward(f32(rng.standard_normal(B)), True, True)
+    out["grads_G_after_calls"], out["grads_D_after_calls"] = ctx.get_grads(NET_G), ctx.get_grads(NET_D)
+    out["sample_chunk16"] = ctx.sample(f32(rng.uniform(-1, 1, (40, 100))), 16)
+    ds.close()
+    ctx.close()
+    return out, launches
+
+
+def case_s16(B, opts, imgs):
+    import face_generator_b200 as fg
+    from face_generator_b200.dataset import DeviceDataset
+    from face_generator_b200.lib import NET_D, NET_G
+    rng = np.random.default_rng(41)
+    ctx = fg.Context(0, max_batch=B, channels=C)
+    for k, v in opts.items():
+        ctx.set_option(k, v)
+    net = fg.S16(ctx)
+    net.set_params(NET_G, f32(rng.standard_normal(net.count(NET_G)) * 0.02))
+    net.set_params(NET_D, f32(rng.standard_normal(net.count(NET_D)) * 0.02))
+    ds = DeviceDataset(ctx, imgs)
+    h = fg.hyper_default()
+    out = {}
+
+    def host(seed):
+        real = f32(rng.random((B // 2, C, 16, 16)))
+        return net.train_step(h, B, real, f32(rng.uniform(-1, 1, (B // 2, 100))), f32(rng.uniform(-1, 1, (B, 100))),
+                              None, None, seed)
+
+    launches = steps(ctx, out, host, lambda seed: net.train_step_dataset(ds, h, B, seed))
+    out.update(pair_state(net, True))
+    out["G_forward"] = net.G_forward(f32(rng.uniform(-1, 1, (B, 100))), training=True)
+    out["G_backward.dnoise"] = net.G_backward(f32(rng.standard_normal((B, C, 16, 16)) * 1e-2), want_dnoise=True)
+    for n in G_DEBUG_S16:
+        out["debug." + n] = net.debug_tensor(n)
+    out["D_forward"] = net.D_forward(f32(rng.random((B, C, 16, 16))), None, True, 3)
+    out["D_backward.dimg"] = net.D_backward(f32(rng.standard_normal(B)), True, True)
+    out["grads_G_after_calls"], out["grads_D_after_calls"] = net.get_grads(NET_G), net.get_grads(NET_D)
+    ds.close()
+    net.close()
+    ctx.close()
+    return out, launches
+
+
+def case_c2f(B, imgs, cs=16):
+    import face_generator_b200 as fg
+    from face_generator_b200 import layouts as LY
+    from face_generator_b200.dataset import DeviceDataset, noise_uniform
+    from face_generator_b200.lib import NET_D, NET_G
+    rng = np.random.default_rng(51)
+    ctx = fg.Context(0, max_batch=B, channels=C)
+    net = fg.C2f(ctx)
+    net.set_params(NET_G, LY.trained_like_init(LY.c2f_G_layout(C), rng, 1.2))
+    net.set_params(NET_D, LY.trained_like_init(LY.c2f_D_layout(C), rng, 1.0))
+    ds = DeviceDataset(ctx, imgs)
+    h = fg.hyper_default()
+    out = {}
+    Bh = B // 2
+
+    def host(seed):
+        _, cr, dr = ds.gather_c2f(ds.draw(8 * seed, Bh), cs)
+        _, cf, _ = ds.gather_c2f(ds.draw(8 * seed + 1, Bh), cs)
+        _, cg, _ = ds.gather_c2f(ds.draw(8 * seed + 2, B), cs)
+        nD, nG = noise_uniform(ctx, 8 * seed + 3, (Bh, 1, 32, 32)), noise_uniform(ctx, 8 * seed + 4, (B, 1, 32, 32))
+        return net.train_step(h, B, dr, np.concatenate([cr, cf]), nD, cg, nG, None, None, seed)
+
+    launches = steps(ctx, out, host, lambda seed: net.train_step_dataset(ds, h, B, cs, seed))
+    out.update(pair_state(net, False))
+    _, cond, diff = ds.gather_c2f(ds.draw(99, B), cs)
+    out["G_forward"] = net.G_forward(f32(rng.uniform(-1, 1, (B, 1, 32, 32))), cond)
+    net.G_backward(f32(rng.standard_normal((B, C, 32, 32)) * 1e-2))
+    out["D_forward"] = net.D_forward(diff, cond, None, True, 3)
+    out["D_backward.ddiff"] = net.D_backward(f32(rng.standard_normal(B)), True, True)
+    out["grads_G_after_calls"], out["grads_D_after_calls"] = net.get_grads(NET_G), net.get_grads(NET_D)
+    ds.close()
+    net.close()
+    ctx.close()
+    return out, launches
+
+
+def case_lop(N=16, Cin=128, H=16, Cout=128, k=3):
+    """fg_conv2d_* with mma_f16 1 at a shape that takes the 3xFP16 tensor-core path"""
+    import face_generator_b200 as fg
+    from face_generator_b200.lib import _check, _ptr
+    rng = np.random.default_rng(3)
+    ctx = fg.Context(0, max_batch=N, channels=C)
+    ctx.set_option("mma_f16", 1)
+    lib, hd = ctx.lib, ctx.h
+    x, w = f32(rng.standard_normal((N, Cin, H, H))), f32(rng.standard_normal((Cout, Cin, k, k)) * 0.05)
+    b, dy = f32(rng.standard_normal(Cout)), f32(rng.standard_normal((N, Cout, H, H)) * 1e-3)
+    y, dx = np.empty((N, Cout, H, H), np.float32), np.empty((N, Cin, H, H), np.float32)
+    dw, db = np.zeros((Cout, Cin, k, k), np.float32), np.zeros(Cout, np.float32)
+    l0 = ctx.launches()
+    _check(lib.fg_conv2d_forward(hd, _ptr(x), _ptr(w), _ptr(b), _ptr(y), N, Cin, H, H, Cout, k), "fg_conv2d_forward")
+    _check(lib.fg_conv2d_backward_data(hd, _ptr(dy), _ptr(w), _ptr(dx), N, Cin, H, H, Cout, k), "fg_conv2d_backward_data")
+    _check(lib.fg_conv2d_backward_filter(hd, _ptr(x), _ptr(dy), _ptr(dw), _ptr(db), N, Cin, H, H, Cout, k),
+           "fg_conv2d_backward_filter")
+    launches = [ctx.launches() - l0]
+    ctx.close()
+    return {"y": y, "dx": dx, "dw": dw, "db": db}, launches
+
+
+def run(args):
+    from face_generator_b200.lib import load_library
+    load_library(os.path.abspath(args.lib))
+    only = set(args.only.split(","))
+    imgs = np.random.default_rng(50).integers(0, 256, (600, C, 64, 64), dtype=np.uint8)
+    cases = []
+    for B in (256, 130):
+        if "32" in only:
+            cases += [("32.B%d.%s" % (B, n), lambda B=B, o=o: case_32(B, o, imgs)) for n, o in OPTS_32]
+        if "s16" in only:
+            cases += [("s16.B%d.%s" % (B, n), lambda B=B, o=o: case_s16(B, o, imgs)) for n, o in OPTS_S16]
+    if "c2f" in only:
+        cases.append(("c2f.B256.default", lambda: case_c2f(256, imgs)))
+    if "lop" in only:
+        cases.append(("lop.conv2d_f16", case_lop))
+    for name, fn in cases:
+        out, launches = fn()
+        d = os.path.join(args.out, name)
+        os.makedirs(d, exist_ok=True)
+        for k, a in out.items():
+            np.save(os.path.join(d, k + ".npy"), a)
+        with open(os.path.join(d, "launches.json"), "w") as f:
+            json.dump(launches, f)
+        print("%-28s %3d arrays  launches/step %s" % (name, len(out), launches), flush=True)
+
+
+def compare(args):
+    bad = 0
+    for name in sorted(os.listdir(args.A)):
+        da, db = os.path.join(args.A, name), os.path.join(args.B, name)
+        la, lb = (json.load(open(os.path.join(d, "launches.json"))) for d in (da, db))
+        keys = sorted(f[:-4] for f in os.listdir(da) if f.endswith(".npy"))
+        first = None
+        for k in keys:
+            pb = os.path.join(db, k + ".npy")
+            a = np.load(os.path.join(da, k + ".npy"))
+            if not os.path.exists(pb):
+                first = "%s: missing in B" % k
+                break
+            b = np.load(pb)
+            if a.dtype != b.dtype or a.shape != b.shape or a.tobytes() != b.tobytes():
+                n = int(np.sum(a != b)) if a.shape == b.shape else -1
+                first = "%s: %d elements differ" % (k, n)
+                break
+        bad += first is not None
+        print("%-28s %-34s launches/step A %s  B %s" % (name, first or "identical (%d arrays)" % len(keys), la, lb))
+    print("%d case(s) differ" % bad)
+    return 1 if bad else 0
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    sub = ap.add_subparsers(dest="cmd", required=True)
+    r = sub.add_parser("run")
+    r.add_argument("--lib", required=True)
+    r.add_argument("--out", required=True)
+    r.add_argument("--only", default="32,s16,c2f,lop")
+    c = sub.add_parser("compare")
+    c.add_argument("A")
+    c.add_argument("B")
+    args = ap.parse_args()
+    if args.cmd == "run":
+        run(args)
+        return 0
+    return compare(args)
+
+
+if __name__ == "__main__":
+    sys.exit(main())
