@@ -145,7 +145,7 @@ __global__ void amax_kernel(const float* __restrict__ x, int64_t n4, unsigned* _
   float m = 0.f;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
     const float4 v = x4[i];
-    m = fmaxf(fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
+    m = fmaxf(fmaxf(m, fmaxf(finite_abs(v.x), finite_abs(v.y))), fmaxf(finite_abs(v.z), finite_abs(v.w)));
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));

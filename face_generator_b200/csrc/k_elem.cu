@@ -8,6 +8,7 @@
 #include <cmath>
 
 #include "fg_internal.h"
+#include "k_f16split.cuh"
 #include "k_ordered.cuh"
 
 __device__ __forceinline__ int perm_idx(int j, int A, int S) {
@@ -35,8 +36,8 @@ __device__ __forceinline__ double block_sum(double v) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// max|output| of an elementwise producer into a device word (option mma_f16: the power-of-two scale of the FP16 split
-// is derived from it, k_conv_tc.cu).  Non-negative floats order like their bit patterns, so atomicMax on the bits is exact
+// max|output| over the finite outputs of an elementwise producer (finite_abs) into a device word (option mma_f16: the
+// power-of-two scale of the FP16 split is derived from it, k_conv_tc.cu).  Non-negative floats order like their bit patterns, so atomicMax on the bits is exact
 // and order-independent (replicas stay identical).  Must be reached by all 32 lanes.
 __device__ __forceinline__ void amax_commit(unsigned* amax, float m) {
   if (!amax) return;
@@ -50,7 +51,7 @@ __device__ __forceinline__ void amax_commit(unsigned* amax, float m) {
   }
 }
 __device__ __forceinline__ float amax4(float m, float a, float b, float c, float d) {
-  return fmaxf(fmaxf(m, fmaxf(fabsf(a), fabsf(b))), fmaxf(fabsf(c), fabsf(d)));
+  return fmaxf(fmaxf(m, fmaxf(finite_abs(a), finite_abs(b))), fmaxf(finite_abs(c), finite_abs(d)));
 }
 // host side: the producer launched next reports into c->amax_out (set by nets.cu) and says so in *c->amax_done
 static inline unsigned* take_amax(fg_ctx* c) {
@@ -190,7 +191,7 @@ __global__ void prelu_fwd_kernel(const float* __restrict__ z, const float* __res
     const float v = z[i];
     const float o = v > 0.f ? v : a * v;
     h[i] = o;
-    am = fmaxf(am, fabsf(o));
+    am = fmaxf(am, finite_abs(o));
   }
   amax_commit(amax, am);
 }
@@ -229,10 +230,10 @@ __global__ void prelu_bwd_kernel(const float* __restrict__ dh, const float* __re
     const float v = z[i];
     if (v > 0.f) {
       dz[i] = g;
-      am = fmaxf(am, fabsf(g));
+      am = fmaxf(am, finite_abs(g));
     } else {
       dz[i] = a * g;
-      am = fmaxf(am, fabsf(a * g));
+      am = fmaxf(am, finite_abs(a * g));
       s += (double)g * (double)v;
     }
   }
@@ -915,7 +916,7 @@ __global__ void lin_act_drop_fwd_kernel(const float* __restrict__ z, const float
     const float act = v > 0.f ? v : a * v;
     const float o = masks ? act * masks[(int64_t)b * kMaskPerSample + moff + j] * scale : act;
     h[i] = o;
-    am = fmaxf(am, fabsf(o));
+    am = fmaxf(am, finite_abs(o));
   }
   amax_commit(amax, am);
 }
@@ -940,10 +941,10 @@ __global__ void lin_act_drop_bwd_kernel(const float* __restrict__ dh, const floa
     const float v = z[i];
     if (v > 0.f) {
       dz[i] = g;
-      am = fmaxf(am, fabsf(g));
+      am = fmaxf(am, finite_abs(g));
     } else {
       dz[i] = a * g;
-      am = fmaxf(am, fabsf(a * g));
+      am = fmaxf(am, finite_abs(a * g));
       s += (double)g * (double)v;
     }
   }

@@ -4,12 +4,20 @@
 
 // 3xFP16 split: x ~= hi + lo * 2^-11 with hi = fp16(x), lo = fp16((x - hi) * 2^11): 22 significant bits like the TF32
 // split, operands of f16 MMAs (2x the TF32 rate, 4 bytes per element for hi+lo instead of 8).  fp16 subnormals
-// keep the ABSOLUTE error at 2^-36, so a tensor whose max is in [2^-13, 65504] is represented to 2^-23 of that max;
-// activations and weights are used as they are, gradients are first scaled by a power of two (tc_amax).
+// keep the ABSOLUTE error at 2^-36, so a tensor whose max is in [2^-13, 65504] is represented to 2^-23 of that max.
+// Activations and gradients are first scaled by the power of two of their own max|x| (scale_for_amax); weights are
+// used as they are.  NaN and +-Inf pass through unclamped (hi = x, lo = 0), so that the MMA propagates them as the
+// fp32 path does; the clamp only bounds finite values.
 __device__ __forceinline__ void split_f16(float x, __half& hi, __half& lo) {
-  const float xc = fminf(fmaxf(x, -65504.f), 65504.f);
-  hi = __float2half_rn(xc);
-  lo = __float2half_rn(fminf(fmaxf((x - __half2float(hi)) * 2048.f, -65504.f), 65504.f));
+  const bool fin = fabsf(x) <= 3.402823466e38f;  // false for NaN and +-Inf
+  hi = __float2half_rn(fin ? fminf(fmaxf(x, -65504.f), 65504.f) : x);
+  lo = __float2half_rn(fin ? fminf(fmaxf((x - __half2float(hi)) * 2048.f, -65504.f), 65504.f) : 0.f);
+}
+// |x| as the max|x| reductions that set a tensor's scale see it: NaN and +-Inf count as 0, so that one non-finite
+// element does not take the scaling away from the rest of its tensor (split_f16 passes that element through as it is)
+__device__ __forceinline__ float finite_abs(float x) {
+  const float a = fabsf(x);
+  return a <= 3.402823466e38f ? a : 0.f;
 }
 // power of two that brings amax into [2^14, 2^15) (1 for an all-zero tensor); exponent clamped so that s and 1/s are normal
 __device__ __forceinline__ float scale_for_amax(float amax) {
