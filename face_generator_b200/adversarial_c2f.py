@@ -9,9 +9,9 @@ import numpy as np
 from .lib import C2f, NET_D, NET_G
 
 
-def create_noise_inputs(n, rng):
+def create_noise_inputs(n, rng, fine_size=32):
     """noiseInputs:uniform(-1, 1) over NOISE_DIM = {1, fineSize, fineSize} (train_c2f.lua:80, adversarial_c2f.lua:135)."""
-    return rng.uniform(-1.0, 1.0, (n, 1, 32, 32)).astype(np.float32)
+    return rng.uniform(-1.0, 1.0, (n, 1, fine_size, fine_size)).astype(np.float32)
 
 
 def train_batch(net: C2f, hyper, real_diff, cond_D, noise_D, cond_G, noise_G, masks_D=None, masks_G=None, seed=0,

@@ -142,29 +142,32 @@ __global__ void gather_kernel(const uint8_t* __restrict__ data, const int32_t* _
     out[i] = scale_pixel(src, y, x, Hs, Ws, Ho, Wo);
   }
 }
-// dataset_c2f.lua:49-62 _toResult at fineSize 32, one cached image per CTA:
-//   fine   = the 32x32 gather of the image (the per-pixel code of gather_kernel, so bit-identical to it), kept in
+// dataset_c2f.lua:49-62 _toResult at fineSize S, one cached image per CTA:
+//   fine   = the S x S gather of the image (the per-pixel code of gather_kernel, so bit-identical to it), kept in
 //            shared memory as fp32 (the reference holds it in a FloatTensor before scaling it again)
 //   tmp    = image.scale(fine, cs, cs)            (shared memory)
-//   coarse = image.scale(tmp, 32, 32)
+//   coarse = image.scale(tmp, S, S)
 //   diff   = fine - coarse                        (torch.add(fine, -1, coarse))
-// Outputs are NCHW [B][C][32][32]; any may be null.  Per image: Cs*Hs*Ws bytes read, up to 3 * C * 4 KB written.
+// Outputs are NCHW [B][C][S][S]; any may be null.  Per image: Cs*Hs*Ws bytes read, up to 3 * C * S*S * 4 bytes
+// written.  Dynamic shared memory: C*S*S floats of fine, then C*cs*cs of tmp (c2f_pairs_smem; 96 KB at S = cs = 64).
 constexpr int kPairThreads = 256;
+size_t c2f_pairs_smem(int C, int S, int cs) { return sizeof(float) * ((size_t)C * S * S + (size_t)C * cs * cs); }
 __global__ void __launch_bounds__(kPairThreads) c2f_pairs_kernel(const uint8_t* __restrict__ data, const int32_t* __restrict__ idx,
                                                                  float* __restrict__ fine, float* __restrict__ coarse,
-                                                                 float* __restrict__ diff, int C, int Cs, int Hs, int Ws, int cs,
-                                                                 int64_t N) {
-  __shared__ float sfine[3 * 1024];
-  __shared__ float stmp[3 * 1024];
-  const int b = blockIdx.x, n = C * 1024, m = cs * cs;
+                                                                 float* __restrict__ diff, int C, int Cs, int Hs, int Ws, int S,
+                                                                 int cs, int64_t N) {
+  extern __shared__ float pair_smem[];
+  const int b = blockIdx.x, SS = S * S, n = C * SS, m = cs * cs;
+  float* sfine = pair_smem;
+  float* stmp = pair_smem + n;
   int64_t img = idx[b];
   img = img < 0 ? 0 : (img >= N ? N - 1 : img);
   const uint8_t* base = data + img * (int64_t)Cs * Hs * Ws;
   const bool gray = Cs == 3 && C == 1;
   const int64_t o = (int64_t)b * n;
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    const int x = i & 31, y = (i >> 5) & 31, ch = i >> 10;
-    const float v = scale_pixel(U8Src{base, ch, Hs, Ws, gray}, y, x, Hs, Ws, 32, 32);
+    const int ch = i / SS, r = i - ch * SS, y = r / S, x = r - y * S;
+    const float v = scale_pixel(U8Src{base, ch, Hs, Ws, gray}, y, x, Hs, Ws, S, S);
     sfine[i] = v;
     if (fine) fine[o + i] = v;
   }
@@ -172,12 +175,12 @@ __global__ void __launch_bounds__(kPairThreads) c2f_pairs_kernel(const uint8_t* 
   __syncthreads();
   for (int i = threadIdx.x; i < C * m; i += blockDim.x) {
     const int ch = i / m, r = i - ch * m, y = r / cs, x = r - y * cs;
-    stmp[i] = scale_pixel(PlaneSrc{sfine + ch * 1024, 32}, y, x, 32, 32, cs, cs);
+    stmp[i] = scale_pixel(PlaneSrc{sfine + ch * SS, S}, y, x, S, S, cs, cs);
   }
   __syncthreads();
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    const int x = i & 31, y = (i >> 5) & 31, ch = i >> 10;
-    const float v = scale_pixel(PlaneSrc{stmp + ch * m, cs}, y, x, cs, cs, 32, 32);
+    const int ch = i / SS, r = i - ch * SS, y = r / S, x = r - y * S;
+    const float v = scale_pixel(PlaneSrc{stmp + ch * m, cs}, y, x, cs, cs, S, S);
     if (coarse) coarse[o + i] = v;
     if (diff) diff[o + i] = sfine[i] - v;
   }
@@ -273,9 +276,11 @@ int gather(fg_dataset* d, const int32_t* idx_dev, int B, float* out_dev, int siz
   LAUNCH_CHECK(c);
   return FG_OK;
 }
-int gather_c2f(fg_dataset* d, const int32_t* idx_dev, int B, int cs, float* fine, float* coarse, float* diff) {
+int gather_c2f(fg_dataset* d, const int32_t* idx_dev, int B, int S, int cs, float* fine, float* coarse, float* diff) {
   fg_ctx* c = d->c;
-  c2f_pairs_kernel<<<B, kPairThreads, 0, c->stream>>>(d->data, idx_dev, fine, coarse, diff, c->C, d->Cs, d->Hs, d->Ws, cs, d->N);
+  const size_t smem = c2f_pairs_smem(c->C, S, cs);
+  if (smem > 48 * 1024) FG_CUDA(cudaFuncSetAttribute(c2f_pairs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  c2f_pairs_kernel<<<B, kPairThreads, smem, c->stream>>>(d->data, idx_dev, fine, coarse, diff, c->C, d->Cs, d->Hs, d->Ws, S, cs, d->N);
   LAUNCH_CHECK(c);
   return FG_OK;
 }
@@ -293,8 +298,8 @@ int stage_indices(fg_dataset* d, const int32_t* idx, int B, const char* what, co
 // idx_out / dist_out: host or device, Q entries each.
 int nearest_run(fg_ctx* c, const float* cands, const fg_dataset* d, int64_t N, int D, const float* queries, int Q,
                 int32_t* idx_out, float* dist_out) {
-  FG_REQUIRE(queries && idx_out && dist_out && Q >= 1 && N >= 1 && D >= 1 && D <= 3072 && N < ((int64_t)1 << 32),
-             "nearest: need 1 <= D <= 3072 (3x32x32), Q >= 1, 1 <= N < 2^32");
+  FG_REQUIRE(queries && idx_out && dist_out && Q >= 1 && N >= 1 && D >= 1 && D <= 12288 && N < ((int64_t)1 << 32),
+             "nearest: need 1 <= D <= 12288 (3x64x64), Q >= 1, 1 <= N < 2^32");
   float *q_dev = nullptr, *c_dev = nullptr, *dist_dev = nullptr;
   int32_t* idx_dev = nullptr;
   unsigned long long* best = nullptr;
@@ -326,6 +331,10 @@ int nearest_run(fg_ctx* c, const float* cands, const fg_dataset* d, int64_t N, i
     const int warps = 8;
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((N + warps - 1) / warps, (int64_t)c->sm_count * 4));
     const size_t smem = sizeof(float) * kQG * D;
+    if (smem > 48 * 1024) {  // above 3x32x32: opt in to the larger dynamic shared memory
+      auto fn = d ? nearest_kernel<true> : nearest_kernel<false>;
+      if (fail(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) break;
+    }
     if (d)
       nearest_kernel<true><<<grid, 32 * warps, smem, c->stream>>>(nullptr, d->data, N, D, c->C, d->Cs, d->Hs, d->Ws, qd, Q, best);
     else
@@ -424,26 +433,36 @@ int fg_dataset_gather_sized(fg_dataset* d, const int32_t* idx, int B, int size, 
   FG_CUDA(cudaStreamSynchronize(c->stream));
   return FG_OK;
 }
-// dataset_c2f.lua:49-62 _toResult at fineSize 32 for B images: fine, coarse, diff [B][C][32][32] fp32, each host or
-// device or NULL.  Host outputs go through one temporary device buffer (this entry is not on a train step's path).
+// dataset_c2f.lua:49-62 _toResult at fineSize 32 (fg_dataset_gather_c2f_sized at 32)
 int fg_dataset_gather_c2f(fg_dataset* d, const int32_t* idx, int B, int coarse_size, float* fine, float* coarse, float* diff) {
+  return fg_dataset_gather_c2f_sized(d, idx, B, 32, coarse_size, fine, coarse, diff);
+}
+// _toResult at fineSize S in {16, 32, 64} for B images: fine, coarse, diff [B][C][S][S] fp32, each host or device or
+// NULL.  Host outputs go through one temporary device buffer (this entry is not on a train step's path).
+int fg_dataset_gather_c2f_sized(fg_dataset* d, const int32_t* idx, int B, int fine_size, int coarse_size, float* fine,
+                                float* coarse, float* diff) {
   ENTER(d);
   fg_ctx* c = d->c;
   FG_REQUIRE(idx && B >= 1 && B <= c->maxB, "fg_dataset_gather_c2f: bad arguments (B %d, max %d)", B, c->maxB);
-  FG_REQUIRE(coarse_size >= 1 && coarse_size <= 32, "fg_dataset_gather_c2f: coarse size %d outside [1, 32]", coarse_size);
+  if (!(fine_size == 16 || fine_size == 32 || fine_size == 64)) {
+    fg_set_error("fg_dataset_gather_c2f_sized: fine size %d is not supported (16, 32 or 64)", fine_size);
+    return FG_ERR_UNSUPPORTED;
+  }
+  FG_REQUIRE(coarse_size >= 1 && coarse_size <= fine_size, "fg_dataset_gather_c2f: coarse size %d outside [1, %d]", coarse_size,
+             fine_size);
   const int32_t* idx_dev;
   FG_TRY(stage_indices(d, idx, B, "fg_dataset_gather_c2f", &idx_dev));
-  const size_t n = (size_t)B * c->C * 1024;
+  const size_t n = (size_t)B * c->C * fine_size * fine_size;
   float* user[3] = {fine, coarse, diff};
   float* dev[3] = {fine, coarse, diff};
   int n_host = 0;
   for (int k = 0; k < 3; ++k) n_host += user[k] && !fg_is_dev(user[k]);
-  if (n_host == 0) return gather_c2f(d, idx_dev, B, coarse_size, fine, coarse, diff);
+  if (n_host == 0) return gather_c2f(d, idx_dev, B, fine_size, coarse_size, fine, coarse, diff);
   float* tmp = nullptr;
   FG_CUDA(cudaMalloc((void**)&tmp, sizeof(float) * n * n_host));
   for (int k = 0, j = 0; k < 3; ++k)
     if (user[k] && !fg_is_dev(user[k])) dev[k] = tmp + n * j++;
-  int rc = gather_c2f(d, idx_dev, B, coarse_size, dev[0], dev[1], dev[2]);
+  int rc = gather_c2f(d, idx_dev, B, fine_size, coarse_size, dev[0], dev[1], dev[2]);
   cudaError_t e = cudaSuccess;
   for (int k = 0; k < 3 && rc == FG_OK && e == cudaSuccess; ++k)
     if (dev[k] != user[k]) e = cudaMemcpyAsync(user[k], dev[k], n * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
@@ -563,11 +582,12 @@ int dataset_draw_gather(fg_dataset* d, uint64_t seed, int B, int size, float* ou
   LAUNCH_CHECK(c);
   return gather(d, d->idx, B, out_dev, size);
 }
-int dataset_draw_gather_c2f(fg_dataset* d, uint64_t seed, int B, int coarse_size, float* fine, float* coarse, float* diff) {
+int dataset_draw_gather_c2f(fg_dataset* d, uint64_t seed, int B, int fine_size, int coarse_size, float* fine, float* coarse,
+                            float* diff) {
   fg_ctx* c = d->c;
   draw_indices_kernel<<<(B + 127) / 128, 128, 0, c->stream>>>(d->idx, B, seed, d->N);
   LAUNCH_CHECK(c);
-  return gather_c2f(d, d->idx, B, coarse_size, fine, coarse, diff);
+  return gather_c2f(d, d->idx, B, fine_size, coarse_size, fine, coarse, diff);
 }
 int noise_uniform_dev(fg_ctx* c, uint64_t seed, int64_t n, float* out_dev) {
   uniform_pm1_kernel<<<grid_for(n, 256), 256, 0, c->stream>>>(out_dev, n, seed);

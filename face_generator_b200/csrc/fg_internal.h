@@ -502,6 +502,7 @@ int64_t debug_tensor_copy(fg_ctx* c, const char* what, const DebugTensor* ents, 
 int dataset_check_feed(const fg_dataset* d, const fg_ctx* c, const char* what);  // same ctx, compatible channels
 // out [B][C][size][size] (device) = gather at `size` of B indices drawn from stream `seed` (fg_dataset_draw)
 int dataset_draw_gather(fg_dataset* d, uint64_t seed, int B, int size, float* out_dev);
-// fine / coarse / diff [B][C][32][32] (device, any may be null) = fg_dataset_gather_c2f of B indices drawn from `seed`
-int dataset_draw_gather_c2f(fg_dataset* d, uint64_t seed, int B, int coarse_size, float* fine, float* coarse, float* diff);
+// fine / coarse / diff [B][C][S][S] (device, any may be null) = fg_dataset_gather_c2f_sized of B indices drawn from `seed`
+int dataset_draw_gather_c2f(fg_dataset* d, uint64_t seed, int B, int fine_size, int coarse_size, float* fine, float* coarse,
+                            float* diff);
 int noise_uniform_dev(fg_ctx* c, uint64_t seed, int64_t n, float* out_dev);  // fg_noise_uniform into device memory

@@ -904,7 +904,7 @@ int tc_conv_wgrad(fg_ctx* c, const float* x_hi, const float* x_lo, const float* 
   const int64_t size = (int64_t)ntt * g.Cout * g.Cin;
   p.out = splits > 1 ? c->splitk_ws : out;  // splits x base CTAs <= one per SM: fits splitk_ws
   p.split_stride = size;
-  if (splits * size > (int64_t)c->splitk_ws_elems) {
+  if (splits > 1 && splits * size > (int64_t)c->splitk_ws_elems) {  // an unsplit gradient goes straight to `out`
     fg_set_error("tc_conv_wgrad: %d splits of %lld elements exceed the split-K workspace", splits, (long long)size);
     return FG_ERR_UNSUPPORTED;
   }

@@ -1,16 +1,19 @@
-// Coarse-to-fine GAN (BASELINE configs[3], train_c2f.lua) on the same kernels as the 32x32 nets:
-//   G = models_c2f.lua:113-145 create_G_d : JoinTable{noise[1x32x32], coarse[Cx32x32]} -> SCU(C+1->64,3) PReLU
-//       SCU(64->64,3) PReLU SCU(64->128,5) PReLU SCU(128->256,5) PReLU SCU(256->C,7)            (all at 32x32)
+// Coarse-to-fine GAN (BASELINE configs[3], train_c2f.lua) on the same kernels as the 32x32 nets, at fine size
+// S = train_c2f.lua --fineSize in {16, 32, 64} (the pyramid levels a 64x64 training set feeds):
+//   G = models_c2f.lua:113-145 create_G_d : JoinTable{noise[1xSxS], coarse[CxSxS]} -> SCU(C+1->64,3) PReLU
+//       SCU(64->64,3) PReLU SCU(64->128,5) PReLU SCU(128->256,5) PReLU SCU(256->C,7)            (all at SxS)
 //   D = models_c2f.lua:237-278 create_D_c : CAddTable{diff, coarse} -> conv(C->64,3) PReLU conv(64->64,3) PReLU
-//       MaxPool2 conv(64->128,3) PReLU conv(128->256,3) PReLU MaxPool2 Dropout View(16384) Linear(512) PReLU
+//       MaxPool2 conv(64->128,3) PReLU conv(128->256,3) PReLU MaxPool2 Dropout View(256*(S/4)^2) Linear(512) PReLU
 //       Dropout Linear(1) Sigmoid
 //   loop = adversarial_c2f.lua:121-187 (fevalD :40-81, fevalG_on_D :85-116, optim.adam)
 // cudnn.SpatialConvolutionUpsample with factor 1 (layers/cudnnSpatialConvolutionUpsample.lua:4-28) is a "same"
 // convolution whose output view is the identity, so every layer maps onto the tap-GEMM convolution kernels:
 // wgmma (3xTF32, chunk-promoted) where the channel counts make a dense contraction (64->64, 64->128,
-// 128->256 and the 16384->512 Linear), the bandwidth-shaped small-channel kernels for (C+1)->64 / C->64 and the
+// 128->256 and the 256*(S/4)^2 -> 512 Linear), the bandwidth-shaped small-channel kernels for (C+1)->64 / C->64 and the
 // fp32 FFMA tile kernel for the 256->C 7x7 output layer (N = 3 is not a tensor-core shape).
 #include <algorithm>
+#include <deque>
+#include <string>
 
 #include "convl.h"
 #include "fg_internal.h"
@@ -18,15 +21,25 @@
 #include "k_misc.h"
 
 namespace {
-constexpr int kC2fMask = 16384 + 512;  // nn.Dropout keep flags per sample: [256][8][8] then [512]
+bool c2f_size_ok(int S) { return S == 16 || S == 32 || S == 64; }
+// View(256*(S/4)^2) of D's last pooled map [256][S/4][S/4]: D.L1's input width
+int c2f_flat(int S) { return 256 * (S / 4) * (S / 4); }
+// nn.Dropout keep flags per sample: [256][S/4][S/4] then [512]
+int c2f_mask(int S) { return c2f_flat(S) + 512; }
 }  // namespace
 
 struct fg_c2f {
   fg_ctx* c = nullptr;
   int maxB = 0, C = 3;
+  int S = 32;           // fine size: every image, noise and activation of G and D's first stage is S x S
+  int HW = 1024;        // S * S
+  int flat = 16384;     // c2f_flat(S)
+  int mask = 16896;     // c2f_mask(S)
+  std::deque<std::string> names;  // timer names (stable storage: the layers point into it)
   NetPair net;  // no BatchNorm
   int64_t Gca[4] = {0, 0, 0, 0}, Dca[4] = {0, 0, 0, 0}, Da5 = 0, DL2W = 0, DL2b = 0;
   ConvL Gc[5], Dc[4], DL1;
+  const char* D_L2_timer = "";
   int G_pack_impl = -1, D_pack_impl = -1;
   float *G_x = nullptr, *G_z[5] = {}, *G_h[4] = {};
   float *D_x = nullptr, *D_cond = nullptr, *D_z[4] = {}, *D_h[4] = {}, *D_p2 = nullptr, *D_p4 = nullptr, *D_d4 = nullptr;
@@ -53,32 +66,38 @@ inline int convl_bwd(fg_c2f* n, ConvL& L, const float* in, const float* dy, floa
   return ::convl_bwd(n->env, L, in, dy, G, din, B);
 }
 
+// "c2f.<layer>" at S = 32 (the names profiles/bench_configs.py reads), "c2f16.<layer>" / "c2f64.<layer>" otherwise, so
+// that nets of two sizes on one ctx keep their timings apart
+const char* timer_name(fg_c2f* n, const char* layer) {
+  n->names.push_back((n->S == 32 ? std::string("c2f.") : "c2f" + std::to_string(n->S) + ".") + layer);
+  return n->names.back().c_str();
+}
+
 void make_layouts(fg_c2f* n) {
-  const int C = n->C;
+  const int C = n->C, S = n->S;
+  n->HW = S * S;
+  n->flat = c2f_flat(S);
+  n->mask = c2f_mask(S);
+  n->names.clear();
   {
     const int ci[5] = {C + 1, 64, 64, 128, 256}, co[5] = {64, 64, 128, 256, C}, kk[5] = {3, 3, 5, 5, 7};
-    static const char* tf[5] = {"c2f.G.c1.fwd", "c2f.G.c2.fwd", "c2f.G.c3.fwd", "c2f.G.c4.fwd", "c2f.G.c5.fwd"};
-    static const char* td[5] = {"c2f.G.c1.dgrad", "c2f.G.c2.dgrad", "c2f.G.c3.dgrad", "c2f.G.c4.dgrad", "c2f.G.c5.dgrad"};
-    static const char* tw[5] = {"c2f.G.c1.wgrad", "c2f.G.c2.wgrad", "c2f.G.c3.wgrad", "c2f.G.c4.wgrad", "c2f.G.c5.wgrad"};
     int64_t o = 0;
     for (int i = 0; i < 5; ++i) {
       ConvL& L = n->Gc[i];
-      L.Cin = ci[i]; L.Cout = co[i]; L.k = kk[i]; L.H = 32;
+      L.Cin = ci[i]; L.Cout = co[i]; L.k = kk[i]; L.H = S;
       L.w_off = o; o += (int64_t)co[i] * ci[i] * kk[i] * kk[i];
       L.b_off = o; o += co[i];
       if (i < 4) { n->Gca[i] = o; o += 1; }
       L.need_dgrad = i > 0;
-      L.tf = tf[i]; L.td = td[i]; L.tw = tw[i];
+      const std::string l = "G.c" + std::to_string(i + 1);
+      L.tf = timer_name(n, (l + ".fwd").c_str()); L.td = timer_name(n, (l + ".dgrad").c_str()); L.tw = timer_name(n, (l + ".wgrad").c_str());
       if (co[i] <= 4 && ci[i] % 128 == 0) L.pad_out = 64;  // c5: 256 -> C, 7x7
       if (co[i] == 64 && ci[i] % 64 == 0) L.pad_dy = 128;  // c2: 64 -> 64
     }
     n->net.nG = o;
   }
   {
-    const int ci[4] = {C, 64, 64, 128}, co[4] = {64, 64, 128, 256}, hw[4] = {32, 32, 16, 16};
-    static const char* tf[4] = {"c2f.D.c1.fwd", "c2f.D.c2.fwd", "c2f.D.c3.fwd", "c2f.D.c4.fwd"};
-    static const char* td[4] = {"c2f.D.c1.dgrad", "c2f.D.c2.dgrad", "c2f.D.c3.dgrad", "c2f.D.c4.dgrad"};
-    static const char* tw[4] = {"c2f.D.c1.wgrad", "c2f.D.c2.wgrad", "c2f.D.c3.wgrad", "c2f.D.c4.wgrad"};
+    const int ci[4] = {C, 64, 64, 128}, co[4] = {64, 64, 128, 256}, hw[4] = {S, S, S / 2, S / 2};
     int64_t o = 0;
     for (int i = 0; i < 4; ++i) {
       ConvL& L = n->Dc[i];
@@ -86,15 +105,17 @@ void make_layouts(fg_c2f* n) {
       L.w_off = o; o += (int64_t)co[i] * ci[i] * 9;
       L.b_off = o; o += co[i];
       n->Dca[i] = o; o += 1;
-      L.tf = tf[i]; L.td = td[i]; L.tw = tw[i];
+      const std::string l = "D.c" + std::to_string(i + 1);
+      L.tf = timer_name(n, (l + ".fwd").c_str()); L.td = timer_name(n, (l + ".dgrad").c_str()); L.tw = timer_name(n, (l + ".wgrad").c_str());
       if (co[i] == 64 && ci[i] % 64 == 0) L.pad_dy = 128;  // c2: 64 -> 64
     }
     ConvL& L = n->DL1;
-    L.Cin = 16384; L.Cout = 512; L.k = 1; L.H = 1;
-    L.cA = 256; L.cS = 64;  // View(16384) flattens [256][8][8]; ours is [8][8][256]
-    L.w_off = o; o += (int64_t)512 * 16384;
+    L.Cin = n->flat; L.Cout = 512; L.k = 1; L.H = 1;
+    L.cA = 256; L.cS = (S / 4) * (S / 4);  // View(256*(S/4)^2) flattens [256][S/4][S/4]; ours is [S/4][S/4][256]
+    L.w_off = o; o += (int64_t)512 * n->flat;
     L.b_off = o; o += 512;
-    L.tf = "c2f.D.L1.fwd"; L.td = "c2f.D.L1.dgrad"; L.tw = "c2f.D.L1.wgrad";
+    L.tf = timer_name(n, "D.L1.fwd"); L.td = timer_name(n, "D.L1.dgrad"); L.tw = timer_name(n, "D.L1.wgrad");
+    n->D_L2_timer = timer_name(n, "D.L2.fwd");
     n->Da5 = o; o += 1;
     n->DL2W = o; o += 512;
     n->DL2b = o; o += 1;
@@ -103,8 +124,8 @@ void make_layouts(fg_c2f* n) {
 }
 
 int c2f_alloc(fg_c2f* n) {
-  const size_t B = n->maxB, C = n->C;
   make_layouts(n);
+  const size_t B = n->maxB, C = n->C, HW = n->HW, flat = n->flat, mask = n->mask;
   n->env.c = n->c;
   n->env.maxB = n->maxB;
   n->env.allocs = &n->allocs;
@@ -112,46 +133,46 @@ int c2f_alloc(fg_c2f* n) {
   for (int i = 0; i < 5; ++i) FG_TRY(convl_alloc(n, n->Gc[i]));
   for (int i = 0; i < 4; ++i) FG_TRY(convl_alloc(n, n->Dc[i]));
   FG_TRY(convl_alloc(n, n->DL1));
-  FG_TRY(dalloc(n, &n->G_x, B * 1024 * (C + 1)));
+  FG_TRY(dalloc(n, &n->G_x, B * HW * (C + 1)));
   for (int i = 0; i < 5; ++i) {
-    FG_TRY(dalloc(n, &n->G_z[i], B * 1024 * n->Gc[i].Cout));
-    if (i < 4) FG_TRY(dalloc(n, &n->G_h[i], B * 1024 * n->Gc[i].Cout));
+    FG_TRY(dalloc(n, &n->G_z[i], B * HW * n->Gc[i].Cout));
+    if (i < 4) FG_TRY(dalloc(n, &n->G_h[i], B * HW * n->Gc[i].Cout));
   }
-  FG_TRY(dalloc(n, &n->D_x, B * 1024 * C));
-  FG_TRY(dalloc(n, &n->D_cond, B * 1024 * C));
+  FG_TRY(dalloc(n, &n->D_x, B * HW * C));
+  FG_TRY(dalloc(n, &n->D_cond, B * HW * C));
   for (int i = 0; i < 4; ++i) {
     const size_t e = B * (size_t)n->Dc[i].H * n->Dc[i].H * n->Dc[i].Cout;
     FG_TRY(dalloc(n, &n->D_z[i], e));
     FG_TRY(dalloc(n, &n->D_h[i], e));
   }
-  FG_TRY(dalloc(n, &n->D_p2, B * 256 * 64));
-  FG_TRY(dalloc(n, &n->D_p4, B * 16384));
-  FG_TRY(dalloc(n, &n->D_d4, B * 16384));
+  FG_TRY(dalloc(n, &n->D_p2, B * (HW / 4) * 64));
+  FG_TRY(dalloc(n, &n->D_p4, B * flat));
+  FG_TRY(dalloc(n, &n->D_d4, B * flat));
   FG_TRY(dalloc(n, &n->D_zl1, B * 512));
   FG_TRY(dalloc(n, &n->D_al1, B * 512));
   FG_TRY(dalloc(n, &n->D_hl1, B * 512));
   FG_TRY(dalloc(n, &n->D_logit, B));
   FG_TRY(dalloc(n, &n->D_out, B));
   FG_TRY(dalloc(n, &n->D_dlogit, B));
-  FG_TRY(dalloc(n, &n->D_masks, B * kC2fMask));
-  FG_TRY(dalloc(n, &n->D_dx, B * 1024 * C));
-  const size_t big = B * 1024 * 256;  // largest activation: G conv4 output
+  FG_TRY(dalloc(n, &n->D_masks, B * mask));
+  FG_TRY(dalloc(n, &n->D_dx, B * HW * C));
+  const size_t big = B * HW * 256;  // largest activation: G conv4 output
   FG_TRY(dalloc(n, &n->ga, big));
   FG_TRY(dalloc(n, &n->gb, big));
   FG_TRY(dalloc(n, &n->env.dy.hi, big));
   FG_TRY(dalloc(n, &n->env.dy.lo, big));
-  FG_TRY(dalloc(n, &n->env.pad.hi, big / 2));  // up to 128 padded channels at 32x32
+  FG_TRY(dalloc(n, &n->env.pad.hi, big / 2));  // up to 128 padded channels at S x S
   FG_TRY(dalloc(n, &n->env.pad.lo, big / 2));
-  FG_TRY(dalloc(n, &n->ws, std::max<size_t>((size_t)512 * 16384, (size_t)25 * 256 * 128)));
+  FG_TRY(dalloc(n, &n->ws, std::max<size_t>((size_t)512 * flat, (size_t)25 * 256 * 128)));
   n->env.ga = n->ga; n->env.ws = n->ws;
-  FG_TRY(dalloc(n, &n->in_a, B * 1024 * C));
-  FG_TRY(dalloc(n, &n->in_b, B * 1024 * C));
-  FG_TRY(dalloc(n, &n->in_c, B * 1024));
-  FG_TRY(dalloc(n, &n->in_d, B * 1024 * C));
-  FG_TRY(dalloc(n, &n->in_e, B * 1024));
-  FG_TRY(dalloc(n, &n->in_m1, B * kC2fMask));
-  FG_TRY(dalloc(n, &n->in_m2, B * kC2fMask));
-  FG_TRY(dalloc(n, &n->io, B * 1024 * C));
+  FG_TRY(dalloc(n, &n->in_a, B * HW * C));
+  FG_TRY(dalloc(n, &n->in_b, B * HW * C));
+  FG_TRY(dalloc(n, &n->in_c, B * HW));
+  FG_TRY(dalloc(n, &n->in_d, B * HW * C));
+  FG_TRY(dalloc(n, &n->in_e, B * HW));
+  FG_TRY(dalloc(n, &n->in_m1, B * mask));
+  FG_TRY(dalloc(n, &n->in_m2, B * mask));
+  FG_TRY(dalloc(n, &n->io, B * HW * C));
   FG_CUDA(cudaStreamSynchronize(n->c->stream));
   return FG_OK;
 }
@@ -174,17 +195,17 @@ int pack_D(fg_c2f* n) {
   return FG_OK;
 }
 
-// noise [B][1][32][32] and cond [B][C][32][32] are NCHW device pointers; the diff lands in G_z[4] (NHWC)
+// noise [B][1][S][S] and cond [B][C][S][S] are NCHW device pointers; the diff lands in G_z[4] (NHWC)
 int G_forward(fg_c2f* n, const float* noise, const float* cond, int B) {
   fg_ctx* c = n->c;
   FG_REQUIRE(B >= 1 && B <= n->maxB, "c2f G forward: batch %d out of range [1,%d]", B, n->maxB);
   FG_TRY(pack_G(n));
-  FG_TRY(k_join_to_nhwc(c, noise, cond, n->G_x, B, n->C, 1024));
+  FG_TRY(k_join_to_nhwc(c, noise, cond, n->G_x, B, n->C, n->HW));
   const float* cur = n->G_x;
   for (int i = 0; i < 5; ++i) {
     FG_TRY(convl_fwd(n, n->Gc[i], cur, n->net.PG, n->G_z[i], B));
     if (i < 4) {
-      FG_TRY(k_prelu_fwd(c, n->G_z[i], n->net.PG + n->Gca[i], n->G_h[i], (int64_t)B * 1024 * n->Gc[i].Cout));
+      FG_TRY(k_prelu_fwd(c, n->G_z[i], n->net.PG + n->Gca[i], n->G_h[i], (int64_t)B * n->HW * n->Gc[i].Cout));
       cur = n->G_h[i];
     }
   }
@@ -192,7 +213,7 @@ int G_forward(fg_c2f* n, const float* noise, const float* cond, int B) {
   n->G_valid = true;
   return FG_OK;
 }
-// ddiff: NHWC [B][32][32][C]; accumulates into gG
+// ddiff: NHWC [B][S][S][C]; accumulates into gG
 int G_backward(fg_c2f* n, const float* ddiff) {
   fg_ctx* c = n->c;
   if (!n->G_valid) {
@@ -205,7 +226,7 @@ int G_backward(fg_c2f* n, const float* ddiff) {
     const float* in = i == 0 ? n->G_x : n->G_h[i - 1];
     FG_TRY(convl_bwd(n, n->Gc[i], in, dcur, n->net.gG, i > 0 ? n->ga : nullptr, B));
     if (i > 0) {
-      FG_TRY(k_prelu_bwd(c, n->ga, n->G_z[i - 1], n->net.PG + n->Gca[i - 1], n->gb, n->net.gG + n->Gca[i - 1], B, 32, 32,
+      FG_TRY(k_prelu_bwd(c, n->ga, n->G_z[i - 1], n->net.PG + n->Gca[i - 1], n->gb, n->net.gG + n->Gca[i - 1], B, n->S, n->S,
                          n->Gc[i - 1].Cout, 0));
       dcur = n->gb;
     }
@@ -219,7 +240,7 @@ int D_forward(fg_c2f* n, const float* diff, const float* cond, int B, bool train
   FG_REQUIRE(B >= 1 && B <= n->maxB, "c2f D forward: batch %d out of range [1,%d]", B, n->maxB);
   FG_TRY(pack_D(n));
   const float* P = n->net.PD;
-  FG_TRY(k_add(c, diff, cond, n->D_x, (int64_t)B * 1024 * n->C));  // nn.CAddTable
+  FG_TRY(k_add(c, diff, cond, n->D_x, (int64_t)B * n->HW * n->C));  // nn.CAddTable
   const float* cur = n->D_x;
   for (int i = 0; i < 4; ++i) {
     const ConvL& L = n->Dc[i];
@@ -227,27 +248,27 @@ int D_forward(fg_c2f* n, const float* diff, const float* cond, int B, bool train
     FG_TRY(k_prelu_fwd(c, n->D_z[i], P + n->Dca[i], n->D_h[i], (int64_t)B * L.H * L.H * L.Cout));
     cur = n->D_h[i];
     if (i == 1) {
-      FG_TRY(k_maxpool2_fwd(c, n->D_h[1], n->D_p2, B, 32, 32, 64));
+      FG_TRY(k_maxpool2_fwd(c, n->D_h[1], n->D_p2, B, n->S, n->S, 64));
       cur = n->D_p2;
     } else if (i == 3) {
-      FG_TRY(k_maxpool2_fwd(c, n->D_h[3], n->D_p4, B, 16, 16, 256));
+      FG_TRY(k_maxpool2_fwd(c, n->D_h[3], n->D_p4, B, n->S / 2, n->S / 2, 256));
     }
   }
   n->D_scale = 1.0f / (1.0f - p_drop);
   const float* d4 = n->D_p4;
   if (training) {  // nn.Dropout (v2): mask/(1-p) in training, identity in evaluation
-    FG_TRY(k_dropout_nhwc(c, n->D_p4, n->D_masks, kC2fMask, 0, 64, 256, n->D_scale, n->D_d4, B));
+    FG_TRY(k_dropout_nhwc(c, n->D_p4, n->D_masks, n->mask, 0, n->HW / 16, 256, n->D_scale, n->D_d4, B));
     d4 = n->D_d4;
   }
   FG_TRY(convl_fwd(n, n->DL1, d4, P, n->D_zl1, B));
   FG_TRY(k_prelu_fwd(c, n->D_zl1, P + n->Da5, n->D_al1, (int64_t)B * 512));
   const float* hl1 = n->D_al1;
   if (training) {
-    FG_TRY(k_dropout_nhwc(c, n->D_al1, n->D_masks, kC2fMask, 16384, 1, 512, n->D_scale, n->D_hl1, B));
+    FG_TRY(k_dropout_nhwc(c, n->D_al1, n->D_masks, n->mask, n->flat, 1, 512, n->D_scale, n->D_hl1, B));
     hl1 = n->D_hl1;
   }
   {
-    ScopedTimer tm(c, "c2f.D.L2.fwd");
+    ScopedTimer tm(c, n->D_L2_timer);
     FG_TRY(k_gemv_fwd(c, hl1, P + n->DL2W, P + n->DL2b, n->D_logit, B, 512));
   }
   n->D_B = B;
@@ -272,15 +293,15 @@ int D_backward(fg_c2f* n, const float* dlogit, bool want_wgrad, bool want_dx) {
   float *cur = n->ga, *oth = n->gb;  // gradient ping-pong: every stage reads `cur`, writes `oth`, then they swap
   FG_TRY(k_gemv_dgrad(c, dlogit, P + n->DL2W, cur, B, 512));
   if (tr) {
-    FG_TRY(k_dropout_nhwc(c, cur, n->D_masks, kC2fMask, 16384, 1, 512, n->D_scale, oth, B));
+    FG_TRY(k_dropout_nhwc(c, cur, n->D_masks, n->mask, n->flat, 1, 512, n->D_scale, oth, B));
     std::swap(cur, oth);
   }
   FG_TRY(k_prelu_bwd(c, cur, n->D_zl1, P + n->Da5, oth, G ? G + n->Da5 : nullptr, B, 1, 1, 512, 0));
   std::swap(cur, oth);
-  FG_TRY(convl_bwd(n, n->DL1, d4, cur, G, oth, B));  // -> gradient of the View(16384) input, [B][8][8][256]
+  FG_TRY(convl_bwd(n, n->DL1, d4, cur, G, oth, B));  // -> gradient of the View input, [B][S/4][S/4][256]
   std::swap(cur, oth);
   if (tr) {
-    FG_TRY(k_dropout_nhwc(c, cur, n->D_masks, kC2fMask, 0, 64, 256, n->D_scale, oth, B));
+    FG_TRY(k_dropout_nhwc(c, cur, n->D_masks, n->mask, 0, n->HW / 16, 256, n->D_scale, oth, B));
     std::swap(cur, oth);
   }
   for (int i = 3; i >= 0; --i) {
@@ -324,17 +345,17 @@ int train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_diff, cons
                const float* condG, const float* noiseG, const float* masksD, const float* masksG, uint64_t seed) {
   fg_ctx* c = n->c;
   const int Bh = B / 2, C = n->C;
-  const size_t img = (size_t)C * 1024;
+  const size_t img = (size_t)C * n->HW;
   const float inv_world = 1.0f / (float)c->world;
   // ---- D step (adversarial_c2f.lua:121-163) ----
   FG_TRY(G_forward(n, noiseD, condD + Bh * img, Bh));
-  FG_TRY(k_nchw_to_nhwc(c, real_diff, n->io, Bh, C, 1024));
+  FG_TRY(k_nchw_to_nhwc(c, real_diff, n->io, Bh, C, n->HW));
   FG_CUDA(cudaMemcpyAsync(n->io + Bh * img, n->G_z[4], sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
-  FG_TRY(k_nchw_to_nhwc(c, condD, n->D_cond, B, C, 1024));
+  FG_TRY(k_nchw_to_nhwc(c, condD, n->D_cond, B, C, n->HW));
   if (masksD)
-    FG_CUDA(cudaMemcpyAsync(n->D_masks, masksD, sizeof(float) * (size_t)B * kC2fMask, cudaMemcpyDeviceToDevice, c->stream));
+    FG_CUDA(cudaMemcpyAsync(n->D_masks, masksD, sizeof(float) * (size_t)B * n->mask, cudaMemcpyDeviceToDevice, c->stream));
   else
-    FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * kC2fMask, 1, h->p_drop, c->seed_dev));
+    FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * n->mask, 1, h->p_drop, c->seed_dev));
   FG_TRY(pair_zero_grads(c, n->net, FG_NET_D));
   FG_TRY(D_forward(n, n->io, n->D_cond, B, true, h->p_drop));
   FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_D, n->net.tailD, B, Bh));
@@ -347,11 +368,11 @@ int train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_diff, cons
   // ---- G step (adversarial_c2f.lua:167-187) ----
   FG_TRY(pair_zero_grads(c, n->net, FG_NET_G));
   FG_TRY(G_forward(n, noiseG, condG, B));
-  FG_TRY(k_nchw_to_nhwc(c, condG, n->D_cond, B, C, 1024));
+  FG_TRY(k_nchw_to_nhwc(c, condG, n->D_cond, B, C, n->HW));
   if (masksG)
-    FG_CUDA(cudaMemcpyAsync(n->D_masks, masksG, sizeof(float) * (size_t)B * kC2fMask, cudaMemcpyDeviceToDevice, c->stream));
+    FG_CUDA(cudaMemcpyAsync(n->D_masks, masksG, sizeof(float) * (size_t)B * n->mask, cudaMemcpyDeviceToDevice, c->stream));
   else
-    FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * kC2fMask, 2, h->p_drop, c->seed_dev));
+    FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * n->mask, 2, h->p_drop, c->seed_dev));
   FG_TRY(D_forward(n, n->G_z[4], n->D_cond, B, true, h->p_drop));
   FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_G, n->net.tailG, B, B));
   FG_TRY(D_backward(n, n->D_dlogit, false, true));  // D's weight grads are zeroed before use (:45) -> skipped
@@ -385,15 +406,21 @@ int run_train_step(fg_c2f* n, const fg_hyper* h, int B, const float* rd, const f
 
 extern "C" {
 
-int fg_c2f_create(fg_ctx* ctx, fg_c2f** out) {
+int fg_c2f_create(fg_ctx* ctx, fg_c2f** out) { return fg_c2f_create_sized(ctx, 32, out); }
+int fg_c2f_create_sized(fg_ctx* ctx, int fine_size, fg_c2f** out) {
   if (!ctx || !out) {
-    fg_set_error("fg_c2f_create: null argument");
+    fg_set_error("fg_c2f_create_sized: null argument");
     return FG_ERR_INVALID;
   }
   *out = nullptr;
+  if (!c2f_size_ok(fine_size)) {
+    fg_set_error("fg_c2f_create_sized: fine size %d is not supported (16, 32 or 64)", fine_size);
+    return FG_ERR_UNSUPPORTED;
+  }
   FG_CUDA(cudaSetDevice(ctx->device));
   fg_c2f* n = new fg_c2f();
   n->c = ctx;
+  n->S = fine_size;
   n->maxB = ctx->maxB;
   n->C = ctx->C;
   const int r = c2f_alloc(n);
@@ -415,13 +442,18 @@ int fg_c2f_destroy(fg_c2f* n) {
   delete n;
   return FG_OK;
 }
-int64_t fg_c2f_param_count(int net, int channels) {
+int64_t fg_c2f_param_count(int net, int channels) { return fg_c2f_param_count_sized(net, channels, 32); }
+int64_t fg_c2f_param_count_sized(int net, int channels, int fine_size) {
+  if (!c2f_size_ok(fine_size)) return -1;
   fg_c2f tmp;
   tmp.C = channels;
+  tmp.S = fine_size;
   make_layouts(&tmp);
   return net == FG_NET_D ? tmp.net.nD : tmp.net.nG;
 }
-int fg_c2f_mask_per_sample(void) { return kC2fMask; }
+int fg_c2f_mask_per_sample(void) { return c2f_mask(32); }
+int fg_c2f_mask_per_sample_sized(int fine_size) { return c2f_size_ok(fine_size) ? c2f_mask(fine_size) : -1; }
+int fg_c2f_fine_size(fg_c2f* n) { return n ? n->S : 0; }
 
 int fg_c2f_set_params(fg_c2f* n, int net, const float* src) {
   ENTER(n);
@@ -458,12 +490,12 @@ int fg_c2f_G_forward(fg_c2f* n, const float* noise, const float* cond, int B, fl
   ENTER(n);
   FG_REQUIRE(noise && cond && B >= 1 && B <= n->maxB, "fg_c2f_G_forward: bad arguments (batch %d, max %d)", B, n->maxB);
   const float *nd, *cd;
-  FG_TRY(fg_to_dev(n->c, noise, (size_t)B * 1024, n->in_c, &nd));
-  FG_TRY(fg_to_dev(n->c, cond, (size_t)B * n->C * 1024, n->in_b, &cd));
+  FG_TRY(fg_to_dev(n->c, noise, (size_t)B * n->HW, n->in_c, &nd));
+  FG_TRY(fg_to_dev(n->c, cond, (size_t)B * n->C * n->HW, n->in_b, &cd));
   FG_TRY(G_forward(n, nd, cd, B));
   if (diff_out) {
-    FG_TRY(k_nhwc_to_nchw(n->c, n->G_z[4], n->io, B, n->C, 1024));
-    FG_TRY(fg_to_user(n->c, diff_out, n->io, (size_t)B * n->C * 1024));
+    FG_TRY(k_nhwc_to_nchw(n->c, n->G_z[4], n->io, B, n->C, n->HW));
+    FG_TRY(fg_to_user(n->c, diff_out, n->io, (size_t)B * n->C * n->HW));
   }
   return FG_OK;
 }
@@ -471,8 +503,8 @@ int fg_c2f_G_backward(fg_c2f* n, const float* d_diff) {
   ENTER(n);
   FG_REQUIRE(d_diff, "fg_c2f_G_backward: null gradient");
   const float* dd;
-  FG_TRY(fg_to_dev(n->c, d_diff, (size_t)n->G_B * n->C * 1024, n->in_a, &dd));
-  FG_TRY(k_nchw_to_nhwc(n->c, dd, n->io, n->G_B, n->C, 1024));
+  FG_TRY(fg_to_dev(n->c, d_diff, (size_t)n->G_B * n->C * n->HW, n->in_a, &dd));
+  FG_TRY(k_nchw_to_nhwc(n->c, dd, n->io, n->G_B, n->C, n->HW));
   return G_backward(n, n->io);
 }
 int fg_c2f_D_forward(fg_c2f* n, const float* diff, const float* cond, int B, int training, const float* masks,
@@ -481,15 +513,15 @@ int fg_c2f_D_forward(fg_c2f* n, const float* diff, const float* cond, int B, int
   FG_REQUIRE(diff && cond && B >= 1 && B <= n->maxB, "fg_c2f_D_forward: bad arguments (batch %d, max %d)", B, n->maxB);
   fg_ctx* c = n->c;
   const float *dd, *cd;
-  FG_TRY(fg_to_dev(c, diff, (size_t)B * n->C * 1024, n->in_a, &dd));
-  FG_TRY(fg_to_dev(c, cond, (size_t)B * n->C * 1024, n->in_b, &cd));
-  FG_TRY(k_nchw_to_nhwc(c, dd, n->io, B, n->C, 1024));
-  FG_TRY(k_nchw_to_nhwc(c, cd, n->D_cond, B, n->C, 1024));
+  FG_TRY(fg_to_dev(c, diff, (size_t)B * n->C * n->HW, n->in_a, &dd));
+  FG_TRY(fg_to_dev(c, cond, (size_t)B * n->C * n->HW, n->in_b, &cd));
+  FG_TRY(k_nchw_to_nhwc(c, dd, n->io, B, n->C, n->HW));
+  FG_TRY(k_nchw_to_nhwc(c, cd, n->D_cond, B, n->C, n->HW));
   if (training) {
     if (masks)
-      FG_CUDA(cudaMemcpyAsync(n->D_masks, masks, sizeof(float) * (size_t)B * kC2fMask, cudaMemcpyDefault, c->stream));
+      FG_CUDA(cudaMemcpyAsync(n->D_masks, masks, sizeof(float) * (size_t)B * n->mask, cudaMemcpyDefault, c->stream));
     else
-      FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * kC2fMask, seed, 0.5f));
+      FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * n->mask, seed, 0.5f));
   }
   FG_TRY(D_forward(n, n->io, n->D_cond, B, training != 0, 0.5f));
   FG_TRY(k_sigmoid_fwd(c, n->D_logit, n->D_out, B));
@@ -505,30 +537,30 @@ int fg_c2f_D_backward(fg_c2f* n, const float* d_out, int want_wgrad, float* d_di
   FG_TRY(k_sigmoid_bwd(c, dd, n->D_out, n->D_dlogit, n->D_B));
   FG_TRY(D_backward(n, n->D_dlogit, want_wgrad != 0, d_diff != nullptr));
   if (d_diff) {
-    FG_TRY(k_nhwc_to_nchw(c, n->D_dx, n->io, n->D_B, n->C, 1024));
-    FG_TRY(fg_to_user(c, d_diff, n->io, (size_t)n->D_B * n->C * 1024));
+    FG_TRY(k_nhwc_to_nchw(c, n->D_dx, n->io, n->D_B, n->C, n->HW));
+    FG_TRY(fg_to_user(c, d_diff, n->io, (size_t)n->D_B * n->C * n->HW));
   }
   return FG_OK;
 }
 
 // adversarial_c2f.lua:305-325 approxParzen, one sample: K generations G({noise_k, coarse}) + coarse for the SAME
-// coarse image, the smallest torch.dist to the ground-truth fine image.  noise [K][1][32][32], coarse / fine
-// [C][32][32] (host or device); *dist_out (host).
+// coarse image, the smallest torch.dist to the ground-truth fine image.  noise [K][1][S][S], coarse / fine
+// [C][S][S] (host or device); *dist_out (host).
 int fg_c2f_parzen_dist(fg_c2f* n, const float* noise, const float* coarse, const float* fine, int K, float* dist_out) {
   ENTER(n);
   FG_REQUIRE(noise && coarse && fine && dist_out && K >= 1 && K <= n->maxB, "fg_c2f_parzen_dist: bad arguments (K %d, max %d)", K,
              n->maxB);
   fg_ctx* c = n->c;
-  const size_t img = (size_t)n->C * 1024;
+  const size_t img = (size_t)n->C * n->HW;
   const float *nd, *fd;
-  FG_TRY(fg_to_dev(c, noise, (size_t)K * 1024, n->in_c, &nd));
+  FG_TRY(fg_to_dev(c, noise, (size_t)K * n->HW, n->in_c, &nd));
   for (int k = 0; k < K; ++k)  // condInputs[i] = condInput:clone()  (:318-320)
     FG_CUDA(cudaMemcpyAsync(n->in_b + (size_t)k * img, coarse, img * sizeof(float), cudaMemcpyDefault, c->stream));
   FG_TRY(G_forward(n, nd, n->in_b, K));
-  FG_TRY(k_nchw_to_nhwc(c, n->in_b, n->D_cond, K, n->C, 1024));
+  FG_TRY(k_nchw_to_nhwc(c, n->in_b, n->D_cond, K, n->C, n->HW));
   FG_TRY(k_add(c, n->G_z[4], n->D_cond, n->io, (int64_t)K * img));  // neighbors:add(condInputs)  (:322)
   FG_TRY(fg_to_dev(c, fine, img, n->in_a, &fd));
-  FG_TRY(k_nchw_to_nhwc(c, fd, n->in_d, 1, n->C, 1024));
+  FG_TRY(k_nchw_to_nhwc(c, fd, n->in_d, 1, n->C, n->HW));
   int32_t idx = 0;
   return fg_nearest(c, n->in_d, 1, n->io, K, (int)img, &idx, dist_out);
 }
@@ -548,15 +580,15 @@ int fg_c2f_train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_dif
   FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= n->maxB, "fg_c2f_train_step: batch %d must be even, >= 4 and <= max_batch %d", B,
              n->maxB);
   fg_ctx* c = n->c;
-  const size_t img = (size_t)n->C * 1024;
+  const size_t img = (size_t)n->C * n->HW;
   const float *rd, *cd, *nd, *cg, *ng, *md = nullptr, *mg = nullptr;
   FG_TRY(fg_to_dev(c, real_diff, (size_t)(B / 2) * img, n->in_a, &rd));
   FG_TRY(fg_to_dev(c, cond_D, (size_t)B * img, n->in_b, &cd));
-  FG_TRY(fg_to_dev(c, noise_D, (size_t)(B / 2) * 1024, n->in_c, &nd));
+  FG_TRY(fg_to_dev(c, noise_D, (size_t)(B / 2) * n->HW, n->in_c, &nd));
   FG_TRY(fg_to_dev(c, cond_G, (size_t)B * img, n->in_d, &cg));
-  FG_TRY(fg_to_dev(c, noise_G, (size_t)B * 1024, n->in_e, &ng));
-  if (masks_D) FG_TRY(fg_to_dev(c, masks_D, (size_t)B * kC2fMask, n->in_m1, &md));
-  if (masks_G) FG_TRY(fg_to_dev(c, masks_G, (size_t)B * kC2fMask, n->in_m2, &mg));
+  FG_TRY(fg_to_dev(c, noise_G, (size_t)B * n->HW, n->in_e, &ng));
+  if (masks_D) FG_TRY(fg_to_dev(c, masks_D, (size_t)B * n->mask, n->in_m1, &md));
+  if (masks_G) FG_TRY(fg_to_dev(c, masks_G, (size_t)B * n->mask, n->in_m2, &mg));
   return run_train_step(n, h, B, rd, cd, nd, cg, ng, md, mg, seed, stats);
 }
 
@@ -574,14 +606,14 @@ int fg_c2f_train_step_dataset(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B
   FG_TRY(dataset_check_feed(d, c, "fg_c2f_train_step_dataset"));
   FG_REQUIRE(h && B >= 4 && B % 2 == 0 && B <= n->maxB, "fg_c2f_train_step_dataset: batch %d must be even, >= 4 and <= max_batch %d",
              B, n->maxB);
-  FG_REQUIRE(coarse_size >= 1 && coarse_size <= 32, "fg_c2f_train_step_dataset: coarse size %d outside [1, 32]", coarse_size);
-  const int Bh = B / 2;
-  const size_t img = (size_t)n->C * 1024;
-  FG_TRY(dataset_draw_gather_c2f(d, seed * 8, Bh, coarse_size, nullptr, n->in_b, n->in_a));
-  FG_TRY(dataset_draw_gather_c2f(d, seed * 8 + 1, Bh, coarse_size, nullptr, n->in_b + Bh * img, nullptr));
-  FG_TRY(dataset_draw_gather_c2f(d, seed * 8 + 2, B, coarse_size, nullptr, n->in_d, nullptr));
-  FG_TRY(noise_uniform_dev(c, seed * 8 + 3, (int64_t)Bh * 1024, n->in_c));
-  FG_TRY(noise_uniform_dev(c, seed * 8 + 4, (int64_t)B * 1024, n->in_e));
+  FG_REQUIRE(coarse_size >= 1 && coarse_size <= n->S, "fg_c2f_train_step_dataset: coarse size %d outside [1, %d]", coarse_size, n->S);
+  const int Bh = B / 2, S = n->S;
+  const size_t img = (size_t)n->C * n->HW;
+  FG_TRY(dataset_draw_gather_c2f(d, seed * 8, Bh, S, coarse_size, nullptr, n->in_b, n->in_a));
+  FG_TRY(dataset_draw_gather_c2f(d, seed * 8 + 1, Bh, S, coarse_size, nullptr, n->in_b + Bh * img, nullptr));
+  FG_TRY(dataset_draw_gather_c2f(d, seed * 8 + 2, B, S, coarse_size, nullptr, n->in_d, nullptr));
+  FG_TRY(noise_uniform_dev(c, seed * 8 + 3, (int64_t)Bh * n->HW, n->in_c));
+  FG_TRY(noise_uniform_dev(c, seed * 8 + 4, (int64_t)B * n->HW, n->in_e));
   return run_train_step(n, h, B, n->in_a, n->in_b, n->in_c, n->in_d, n->in_e, nullptr, nullptr, seed, stats);
 }
 
@@ -591,16 +623,16 @@ int64_t fg_c2f_debug_tensor(fg_c2f* n, const char* name, float* dst, int64_t max
     return -1;
   }
   cudaSetDevice(n->c->device);
-  const int gb = n->G_B, db = n->D_B, kb = n->keep_B, C = n->C;
+  const int gb = n->G_B, db = n->D_B, kb = n->keep_B, C = n->C, HW = n->HW;
   auto g = [&](const float* p) { return n->G_valid ? p : nullptr; };
   auto d = [&](const float* p) { return n->D_valid ? p : nullptr; };
   auto dz = [&](int i) { return (int64_t)n->Dc[i].H * n->Dc[i].H * n->Dc[i].Cout; };
   const DebugTensor ents[] = {
-      {"G.x", g(n->G_x), 1024 * (C + 1), gb}, {"G.z1", g(n->G_z[0]), 1024 * 64, gb}, {"G.z2", g(n->G_z[1]), 1024 * 64, gb},
-      {"G.z3", g(n->G_z[2]), 1024 * 128, gb}, {"G.z4", g(n->G_z[3]), 1024 * 256, gb}, {"G.z5", g(n->G_z[4]), 1024 * C, gb},
-      {"D.x", d(n->D_x), 1024 * C, db}, {"D.z1", d(n->D_z[0]), dz(0), db}, {"D.z2", d(n->D_z[1]), dz(1), db},
-      {"D.z3", d(n->D_z[2]), dz(2), db}, {"D.z4", d(n->D_z[3]), dz(3), db}, {"D.p2", d(n->D_p2), 256 * 64, db},
-      {"D.p4", d(n->D_p4), 16384, db}, {"D.zl1", d(n->D_zl1), 512, db}, {"D.logit", d(n->D_logit), 1, db},
+      {"G.x", g(n->G_x), HW * (C + 1), gb}, {"G.z1", g(n->G_z[0]), HW * 64, gb}, {"G.z2", g(n->G_z[1]), HW * 64, gb},
+      {"G.z3", g(n->G_z[2]), HW * 128, gb}, {"G.z4", g(n->G_z[3]), HW * 256, gb}, {"G.z5", g(n->G_z[4]), HW * C, gb},
+      {"D.x", d(n->D_x), HW * C, db}, {"D.z1", d(n->D_z[0]), dz(0), db}, {"D.z2", d(n->D_z[1]), dz(1), db},
+      {"D.z3", d(n->D_z[2]), dz(2), db}, {"D.z4", d(n->D_z[3]), dz(3), db}, {"D.p2", d(n->D_p2), HW / 4 * 64, db},
+      {"D.p4", d(n->D_p4), n->flat, db}, {"D.zl1", d(n->D_zl1), 512, db}, {"D.logit", d(n->D_logit), 1, db},
       {"D.out", d(n->D_out), 1, db}, {"Dstep.z1", n->keep_D[0], dz(0), kb}, {"Dstep.z2", n->keep_D[1], dz(1), kb},
       {"Dstep.z3", n->keep_D[2], dz(2), kb}, {"Dstep.z4", n->keep_D[3], dz(3), kb}, {"Dstep.zl1", n->keep_D[4], 512, kb},
       {"Dstep.logit", n->keep_D[5], 1, kb}, {"Dstep.out", n->keep_D[6], 1, kb}};

@@ -8,6 +8,7 @@
     stats = ds.train_step(hyper, B, seed)         # adversarial.lua loop body with no host->device traffic
     S16(ctx).train_step_dataset(ds, hyper, B, seed)            # the same for the --scale 16 nets
     C2f(ctx).train_step_dataset(ds, hyper, B, 16, seed)        # and for the coarse-to-fine nets
+    C2f(ctx, 64).train_step_dataset(ds, hyper, B, 32, seed)    # the pyramid level 32x32 -> 64x64 (--fineSize 64)
 """
 import ctypes as C
 
@@ -52,13 +53,15 @@ class DeviceDataset:
                                                 out.ctypes.data_as(C.c_void_p)), "fg_dataset_gather_sized")
         return out
 
-    def gather_c2f(self, indices, coarse_size):
-        """dataset_c2f.lua _toResult of those images at fineSize 32: (fine, coarse, diff), each [B][C][32][32]."""
+    def gather_c2f(self, indices, coarse_size, fine_size=32):
+        """dataset_c2f.lua _toResult of those images at fineSize S = fine_size (16, 32 or 64): (fine, coarse, diff),
+        each [B][C][S][S]."""
         idx = np.ascontiguousarray(indices, np.int32)
-        fine, coarse, diff = (np.empty((idx.size, self.ctx.C, 32, 32), np.float32) for _ in range(3))
-        _check(self.lib.fg_dataset_gather_c2f(self.h, idx.ctypes.data_as(C.c_void_p), idx.size, coarse_size,
-                                              fine.ctypes.data_as(C.c_void_p), coarse.ctypes.data_as(C.c_void_p),
-                                              diff.ctypes.data_as(C.c_void_p)), "fg_dataset_gather_c2f")
+        S = fine_size
+        fine, coarse, diff = (np.empty((idx.size, self.ctx.C, S, S), np.float32) for _ in range(3))
+        _check(self.lib.fg_dataset_gather_c2f_sized(self.h, idx.ctypes.data_as(C.c_void_p), idx.size, S, coarse_size,
+                                                    fine.ctypes.data_as(C.c_void_p), coarse.ctypes.data_as(C.c_void_p),
+                                                    diff.ctypes.data_as(C.c_void_p)), "fg_dataset_gather_c2f_sized")
         return fine, coarse, diff
 
     def draw(self, seed, B):

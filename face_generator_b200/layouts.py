@@ -73,13 +73,13 @@ def c2f_G_layout(c):
     return out, o
 
 
-def c2f_D_layout(c):
-    """create_D_c (models_c2f.lua:237-278)."""
+def c2f_D_layout(c, fine_size=32):
+    """create_D_c (models_c2f.lua:237-278) at fine size S: the Linear reads View(256*(S/4)^2)."""
     cin, cout = [c, 64, 64, 128], [64, 64, 128, 256]
     items = []
     for i in range(4):
         items += [("c%dW" % (i + 1), (cout[i], cin[i], 3, 3)), ("c%db" % (i + 1), (cout[i],)), ("a%d" % (i + 1), (1,))]
-    items += [("L1W", (512, 16384)), ("L1b", (512,)), ("a5", (1,)), ("L2W", (1, 512)), ("L2b", (1,))]
+    items += [("L1W", (512, 256 * (fine_size // 4) ** 2)), ("L1b", (512,)), ("a5", (1,)), ("L2W", (1, 512)), ("L2b", (1,))]
     out, o = {}, 0
     for name, shape in items:
         out[name] = (o, shape)
@@ -87,10 +87,11 @@ def c2f_D_layout(c):
     return out, o
 
 
-def c2f_pairs(B, c, rng):
+def c2f_pairs(B, c, rng, fine_size=32):
     """Synthetic stand-in for dataset_c2f.lua:54-60: fine ~ U[0,1), coarse = 2x average-down then 2x nearest-up,
-    diff = fine - coarse.  Returns (diff, coarse), both [B][c][32][32] float32."""
-    fine = rng.random((B, c, 32, 32))
-    small = fine.reshape(B, c, 16, 2, 16, 2).mean(axis=(3, 5))
+    diff = fine - coarse.  Returns (diff, coarse), both [B][c][S][S] float32 (S = fine_size)."""
+    S = fine_size
+    fine = rng.random((B, c, S, S))
+    small = fine.reshape(B, c, S // 2, 2, S // 2, 2).mean(axis=(3, 5))
     coarse = np.repeat(np.repeat(small, 2, axis=2), 2, axis=3)
     return (fine - coarse).astype(np.float32), coarse.astype(np.float32)

@@ -89,6 +89,10 @@ SYMBOLS = {
     "fg_sigmoid_forward": (_I, [_P, _P, _P, _L]),
     "fg_sigmoid_backward": (_I, [_P, _P, _P, _P, _L]),
     "fg_c2f_create": (_I, [_P, C.POINTER(_P)]),
+    "fg_c2f_create_sized": (_I, [_P, _I, C.POINTER(_P)]),
+    "fg_c2f_fine_size": (_I, [_P]),
+    "fg_c2f_param_count_sized": (_L, [_I, _I, _I]),
+    "fg_c2f_mask_per_sample_sized": (_I, [_I]),
     "fg_c2f_destroy": (_I, [_P]),
     "fg_c2f_param_count": (_L, [_I, _I]),
     "fg_c2f_mask_per_sample": (_I, []),
@@ -115,6 +119,7 @@ SYMBOLS = {
     "fg_train_step_dataset": (_I, [_P, _P, C.POINTER(Hyper), _I, _U64, C.POINTER(StepStats)]),
     "fg_dataset_gather_sized": (_I, [_P, _P, _I, _I, _P]),
     "fg_dataset_gather_c2f": (_I, [_P, _P, _I, _I, _P, _P, _P]),
+    "fg_dataset_gather_c2f_sized": (_I, [_P, _P, _I, _I, _I, _P, _P, _P]),
     "fg_s16_train_step_dataset": (_I, [_P, _P, C.POINTER(Hyper), _I, _U64, C.POINTER(StepStats)]),
     "fg_c2f_train_step_dataset": (_I, [_P, _P, C.POINTER(Hyper), _I, _I, _U64, C.POINTER(StepStats)]),
     "fg_D_score": (_I, [_P, _P, _L, _I, _I, _U64, _P]),
@@ -565,19 +570,28 @@ class Context(_BatchNormNetPair):
 
 
 C2F_MASK_PER_SAMPLE = 16384 + 512
+C2F_FINE_SIZES = (16, 32, 64)
+
+
+def c2f_mask_per_sample(fine_size=32):
+    """nn.Dropout keep flags per sample of the coarse-to-fine D at fine size S: [256][S/4][S/4] then [512]"""
+    return 256 * (fine_size // 4) ** 2 + 512
 
 
 class C2f(_NetPair):
-    """Coarse-to-fine nets + loop (train_c2f.lua) on a Context.  Mirrors lua/adversarial_c2f_b200.lua."""
+    """Coarse-to-fine nets + loop (train_c2f.lua) on a Context at fine size S = train_c2f.lua --fineSize (16, 32 or
+    64).  Mirrors lua/adversarial_c2f_b200.lua."""
     _prefix, _what = "fg_c2f_", "c2f "
 
-    def __init__(self, ctx):
+    def __init__(self, ctx, fine_size=32):
         self.ctx, self.lib, self.C = ctx, ctx.lib, ctx.C
         h = C.c_void_p()
-        _check(self.lib.fg_c2f_create(ctx.h, C.byref(h)), "fg_c2f_create")
+        _check(self.lib.fg_c2f_create_sized(ctx.h, fine_size, C.byref(h)), "fg_c2f_create_sized")
         self.h = h
-        self.nG = int(self.lib.fg_c2f_param_count(NET_G, self.C))
-        self.nD = int(self.lib.fg_c2f_param_count(NET_D, self.C))
+        self.S = int(self.lib.fg_c2f_fine_size(h))
+        self.mask_per_sample = int(self.lib.fg_c2f_mask_per_sample_sized(self.S))
+        self.nG = int(self.lib.fg_c2f_param_count_sized(NET_G, self.C, self.S))
+        self.nD = int(self.lib.fg_c2f_param_count_sized(NET_D, self.C, self.S))
 
     def close(self):
         if self.h:
@@ -594,7 +608,7 @@ class C2f(_NetPair):
     def G_forward(self, noise, cond, want_diff=True):
         noise, cond = f32(noise), f32(cond)
         B = cond.shape[0]
-        out = np.empty((B, self.C, 32, 32), np.float32) if want_diff else None
+        out = np.empty((B, self.C, self.S, self.S), np.float32) if want_diff else None
         _check(self.lib.fg_c2f_G_forward(self.h, _ptr(noise), _ptr(cond), B, _ptr(out)), "fg_c2f_G_forward")
         return out
 
@@ -612,7 +626,7 @@ class C2f(_NetPair):
 
     def D_backward(self, d_out, want_wgrad=True, want_ddiff=True):
         d_out = f32(d_out)
-        dd = np.empty((d_out.shape[0], self.C, 32, 32), np.float32) if want_ddiff else None
+        dd = np.empty((d_out.shape[0], self.C, self.S, self.S), np.float32) if want_ddiff else None
         _check(self.lib.fg_c2f_D_backward(self.h, _ptr(d_out), int(want_wgrad), _ptr(dd)), "fg_c2f_D_backward")
         return dd
 

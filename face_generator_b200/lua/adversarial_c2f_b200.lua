@@ -17,7 +17,8 @@ local net = nil   -- fg_c2f*, created on first use, parameters uploaded from PAR
 local function c2f(ctx)
   if net == nil then
     local out = ffi.new('fg_c2f*[1]')
-    F.check(C.fg_c2f_create(ctx, out), 'fg_c2f_create')
+    -- train_c2f.lua --fineSize (16, 32 or 64) sizes both nets; IMG_DIMENSIONS / NOISE_DIM / COND_DIM follow it
+    F.check(C.fg_c2f_create_sized(ctx, OPT.fineSize, out), 'fg_c2f_create_sized')
     net = out[0]
     -- flat vectors are already in getParameters() order (train_c2f.lua:131-132)
     F.check(C.fg_c2f_set_params(net, 0, F.ptr(PARAMETERS_G)), 'fg_c2f_set_params(G)')

@@ -72,6 +72,10 @@ int fg_sigmoid_forward(fg_ctx* ctx, const float* x, float* y, int64_t n);
 int fg_sigmoid_backward(fg_ctx* ctx, const float* y, const float* dy, float* dx, int64_t n);
 typedef struct fg_c2f fg_c2f;
 int fg_c2f_create(fg_ctx* ctx, fg_c2f** out);
+int fg_c2f_create_sized(fg_ctx* ctx, int fine_size, fg_c2f** out);
+int fg_c2f_fine_size(fg_c2f* n);
+int64_t fg_c2f_param_count_sized(int net, int channels, int fine_size);
+int fg_c2f_mask_per_sample_sized(int fine_size);
 int fg_c2f_destroy(fg_c2f* n);
 int64_t fg_c2f_param_count(int net, int channels);
 int fg_c2f_mask_per_sample(void);
@@ -101,6 +105,8 @@ int fg_noise_uniform(fg_ctx* ctx, uint64_t seed, int64_t n, float* out);
 int fg_train_step_dataset(fg_ctx* ctx, fg_dataset* d, const fg_hyper* h, int B, uint64_t seed, fg_step_stats* stats);
 int fg_dataset_gather_sized(fg_dataset* d, const int32_t* idx, int B, int size, float* out);
 int fg_dataset_gather_c2f(fg_dataset* d, const int32_t* idx, int B, int coarse_size, float* fine, float* coarse, float* diff);
+int fg_dataset_gather_c2f_sized(fg_dataset* d, const int32_t* idx, int B, int fine_size, int coarse_size, float* fine, float* coarse,
+                                float* diff);
 int fg_D_score(fg_ctx* ctx, const float* images, int64_t N, int chunk, int training, uint64_t seed, float* preds_out);
 int fg_nearest(fg_ctx* ctx, const float* queries, int Q, const float* cands, int64_t N, int D, int32_t* idx_out, float* dist_out);
 int fg_dataset_nearest(fg_dataset* d, const float* queries, int Q, int32_t* idx_out, float* dist_out);

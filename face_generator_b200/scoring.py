@@ -53,7 +53,7 @@ def approx_parzen(net, fine, coarse, nneighbors, rng):
     out = np.empty(fine.shape[0], np.float32)
     d = np.empty(1, np.float32)
     for i in range(fine.shape[0]):
-        noise = rng.uniform(-1, 1, (nneighbors, 1, 32, 32)).astype(np.float32)
+        noise = rng.uniform(-1, 1, (nneighbors, 1, net.S, net.S)).astype(np.float32)
         _check(net.lib.fg_c2f_parzen_dist(net.h, noise.ctypes.data_as(C.c_void_p), coarse[i].ctypes.data_as(C.c_void_p),
                                           fine[i].ctypes.data_as(C.c_void_p), nneighbors, d.ctypes.data_as(C.c_void_p)),
                "fg_c2f_parzen_dist")

@@ -212,17 +212,26 @@ int fg_train_step(fg_ctx* ctx, const fg_hyper* h, int B, const float* real, cons
 int fg_sample(fg_ctx* ctx, const float* noise, int N, int chunk, float* images_out);
 
 /* ---- coarse-to-fine GAN (train_c2f.lua; BASELINE configs[3]) --------------------------------- */
-/* G = models_c2f.lua:113-145 create_G_d, D = models_c2f.lua:237-278 create_D_c, both at 32x32 on
- * the ctx's channel count; cudnn.SpatialConvolutionUpsample with factor 1
+/* G = models_c2f.lua:113-145 create_G_d, D = models_c2f.lua:237-278 create_D_c, both at the fine
+ * size S = train_c2f.lua --fineSize (16, 32 or 64; fg_c2f_create: 32) on the ctx's channel count.
+ * Every image, noise and mask buffer below is at the net's S: images [B][C][S][S], noise
+ * [B][1][S][S], masks [B][fg_c2f_mask_per_sample_sized(S)].  cudnn.SpatialConvolutionUpsample with factor 1
  * (layers/cudnnSpatialConvolutionUpsample.lua) is a "same" convolution.  The object borrows the
  * ctx (stream, device, DP communicator, "conv_impl"); destroy it before the ctx.  Flat parameter
  * vectors follow getParameters() order: G [c1W c1b a1 ... c4W c4b a4 c5W c5b], D [c1W c1b a1 ...
  * c4W c4b a4 L1W L1b a5 L2W L2b].                                                                 */
 typedef struct fg_c2f fg_c2f;
-int fg_c2f_create(fg_ctx* ctx, fg_c2f** out);
+int fg_c2f_create(fg_ctx* ctx, fg_c2f** out);            /* fg_c2f_create_sized(ctx, 32, out)      */
+/* any fine size other than 16, 32, 64 -> FG_ERR_UNSUPPORTED before anything is allocated          */
+int fg_c2f_create_sized(fg_ctx* ctx, int fine_size, fg_c2f** out);
+int fg_c2f_fine_size(fg_c2f* n);
 int fg_c2f_destroy(fg_c2f* n);
 int64_t fg_c2f_param_count(int net, int channels);        /* 1 101 319 / 8 797 382 for colour      */
 int fg_c2f_mask_per_sample(void);                         /* 16896 = [256][8][8] + [512] nn.Dropout */
+/* at fine size S: G unchanged, D's Linear 256*(S/4)^2 -> 512 (colour D: 2 505 926 at 16, 33 963 206
+ * at 64); keep flags [256][S/4][S/4] + [512] (4608 / 16896 / 66048); -1 for an unsupported size    */
+int64_t fg_c2f_param_count_sized(int net, int channels, int fine_size);
+int fg_c2f_mask_per_sample_sized(int fine_size);
 int fg_c2f_set_params(fg_c2f* n, int net, const float* src);
 int fg_c2f_get_params(fg_c2f* n, int net, float* dst);
 int fg_c2f_get_grads(fg_c2f* n, int net, float* dst);
@@ -231,19 +240,19 @@ float* fg_c2f_params_ptr(fg_c2f* n, int net);
 float* fg_c2f_grads_ptr(fg_c2f* n, int net);
 int fg_c2f_set_adam_state(fg_c2f* n, int net, const float* m, const float* v, int t);
 int fg_c2f_get_adam_state(fg_c2f* n, int net, float* m, float* v, int* t);
-/* MODEL_G:forward({noise, cond}): noise [B][1][32][32], cond (coarse image) [B][C][32][32]
- * -> generated diff [B][C][32][32] (may be NULL).  backward accumulates into G's grad buffer.    */
+/* MODEL_G:forward({noise, cond}): noise [B][1][S][S], cond (coarse image) [B][C][S][S]
+ * -> generated diff [B][C][S][S] (may be NULL).  backward accumulates into G's grad buffer.    */
 int fg_c2f_G_forward(fg_c2f* n, const float* noise, const float* cond, int B, float* diff_out);
 int fg_c2f_G_backward(fg_c2f* n, const float* d_diff);
-/* MODEL_D:forward({diff, cond}) -> [B] sigmoid outputs; masks [B][16896] nn.Dropout keep flags
+/* MODEL_D:forward({diff, cond}) -> [B] sigmoid outputs; masks [B][mask_per_sample] keep flags
  * or NULL (drawn from seed); training=0 => evaluate().  d_diff = MODEL_D.gradInput[1].           */
 int fg_c2f_D_forward(fg_c2f* n, const float* diff, const float* cond, int B, int training, const float* masks,
                      uint64_t seed, float* out);
 int fg_c2f_D_backward(fg_c2f* n, const float* d_out, int want_wgrad, float* d_diff);
 /* one adversarial_c2f.lua:121-187 loop body (1 D iteration + 1 G iteration, optim.adam for both):
- * real_diff [B/2][C][32][32] (fine - coarse of the real half), cond_D [B][C][32][32] (rows < B/2
- * go with the real half, the rest feed G), noise_D [B/2][1][32][32], cond_G / noise_G [B] redrawn
- * for the G step, masks_* [B][16896] or NULL.  h->D_maxAcc / accs_interval are ignored (the c2f
+ * real_diff [B/2][C][S][S] (fine - coarse of the real half), cond_D [B][C][S][S] (rows < B/2
+ * go with the real half, the rest feed G), noise_D [B/2][1][S][S], cond_G / noise_G [B] redrawn
+ * for the G step, masks_* [B][mask_per_sample] or NULL.  h->D_maxAcc / accs_interval are ignored (the c2f
  * loop has no accuracy gate).                                                                     */
 int fg_c2f_train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_diff, const float* cond_D,
                       const float* noise_D, const float* cond_G, const float* noise_G, const float* masks_D,
@@ -312,17 +321,22 @@ int fg_dataset_gather_sized(fg_dataset* d, const int32_t* idx, int B, int size, 
  * device, any may be NULL; 1 <= coarse_size (train_c2f.lua --coarseSize) <= 32                     */
 int fg_dataset_gather_c2f(fg_dataset* d, const int32_t* idx, int B, int coarse_size, float* fine, float* coarse,
                           float* diff);
+/* the same at fineSize S in {16, 32, 64} (others: FG_ERR_UNSUPPORTED): fine = scale(image, S, S),
+ * coarse = scale(scale(fine, cs, cs), S, S), diff = fine - coarse, [B][C][S][S] each; 1 <= cs <= S.
+ * fine_size 32 is fg_dataset_gather_c2f.                                                           */
+int fg_dataset_gather_c2f_sized(fg_dataset* d, const int32_t* idx, int B, int fine_size, int coarse_size, float* fine,
+                                float* coarse, float* diff);
 /* fg_s16_train_step (train.lua --scale 16) with every input produced on the device:
  * real = gather_sized(draw(4*seed, B/2), 16), noise_D = uniform(4*seed+1), noise_G = uniform(4*seed+2),
  * dropout masks from `seed` (the streams of fg_train_step_dataset).  d must belong to n's ctx.     */
 int fg_s16_train_step_dataset(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B, uint64_t seed, fg_step_stats* stats);
 /* fg_c2f_train_step (one adversarial_c2f.lua:121-187 loop body) with every input produced on the device
  * (the draws of adversarial_c2f.lua:124-141 and :168-174):
- *   real pairs  = gather_c2f(draw(8*seed,   B/2)) -> real_diff, cond_D rows [0, B/2)
- *   fake cond   = gather_c2f(draw(8*seed+1, B/2)) -> cond_D rows [B/2, B)
- *   G-step cond = gather_c2f(draw(8*seed+2, B))   -> cond_G
- *   noise_D = uniform(8*seed+3, B/2*1024), noise_G = uniform(8*seed+4, B*1024), dropout masks from `seed`.
- * coarse_size = train_c2f.lua --coarseSize (1..32).  d must belong to n's ctx.                        */
+ *   real pairs  = gather_c2f_sized(draw(8*seed,   B/2), S) -> real_diff, cond_D rows [0, B/2)
+ *   fake cond   = gather_c2f_sized(draw(8*seed+1, B/2), S) -> cond_D rows [B/2, B)
+ *   G-step cond = gather_c2f_sized(draw(8*seed+2, B), S)   -> cond_G
+ *   noise_D = uniform(8*seed+3, B/2*S*S), noise_G = uniform(8*seed+4, B*S*S), dropout masks from `seed`.
+ * coarse_size = train_c2f.lua --coarseSize (1..S).  d must belong to n's ctx.                         */
 int fg_c2f_train_step_dataset(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B, int coarse_size, uint64_t seed,
                               fg_step_stats* stats);
 
@@ -332,13 +346,13 @@ int fg_c2f_train_step_dataset(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B
  * what sample.lua does (it never calls evaluate(): dropout live, masks from seed), 0 = evaluate(). */
 int fg_D_score(fg_ctx* ctx, const float* images, int64_t N, int chunk, int training, uint64_t seed, float* preds_out);
 /* brute-force nearest neighbour by torch.dist (2-norm): for each of Q queries [Q][D] the index of
- * the closest of N candidates [N][D] and the distance (D <= 3072); ties -> lowest index            */
+ * the closest of N candidates [N][D] and the distance (D <= 12288 = 3x64x64); ties -> lowest index */
 int fg_nearest(fg_ctx* ctx, const float* queries, int Q, const float* cands, int64_t N, int D, int32_t* idx_out,
                float* dist_out);
 /* findClosestNeighboursOf (sample.lua:141-159) against the device-resident training set            */
 int fg_dataset_nearest(fg_dataset* d, const float* queries, int Q, int32_t* idx_out, float* dist_out);
 /* one sample of adversarial_c2f.lua:305-325 approxParzen: min_k || G({noise_k, coarse}) + coarse - fine ||,
- * noise [K][1][32][32], coarse / fine [C][32][32]                                                   */
+ * noise [K][1][S][S], coarse / fine [C][S][S]                                                       */
 int fg_c2f_parzen_dist(fg_c2f* n, const float* noise, const float* coarse, const float* fine, int K, float* dist_out);
 
 /* ---- Torch7 checkpoint files (host only, no GPU needed) --------------------------------------- */
