@@ -435,6 +435,26 @@ int fg_train_step(fg_ctx* c, const fg_hyper* h, int B, const float* real, const 
   FG_TRY(net_train_step(c, h, B, r, nd, ng, md, mg, seed, true));
   return pair_step_stats(c, c->net, stats);
 }
+// d_iters D iterations + g_iters G iterations of the loop body on inputs stacked per iteration
+int fg_train_step_iters(fg_ctx* c, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,
+                        const float* noise_D, const float* noise_G, const float* masks_D, const float* masks_G, uint64_t seed,
+                        fg_step_stats* stats) {
+  ENTER(c);
+  FG_TRY(iters_check(d_iters, g_iters, "fg_train_step_iters"));
+  FG_REQUIRE(h && real && noise_D && noise_G, "fg_train_step_iters: null input");
+  FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= c->maxB, "fg_train_step_iters: batch %d must be even, >= 4 and <= max_batch %d", B,
+             c->maxB);
+  const size_t nd = d_iters, ng = g_iters, Bh = B / 2, M = c->maxB, img = (size_t)c->C * 1024;
+  IterStage& s = c->iter_stage;
+  const float *r, *zd, *zg, *md, *mg;
+  FG_TRY(s.in(c, c->allocs, 0, real, nd * Bh * img, nd * M / 2 * img, &r));
+  FG_TRY(s.in(c, c->allocs, 1, noise_D, nd * Bh * kNoiseDim, nd * M / 2 * kNoiseDim, &zd));
+  FG_TRY(s.in(c, c->allocs, 2, noise_G, ng * B * kNoiseDim, ng * M * kNoiseDim, &zg));
+  FG_TRY(s.in(c, c->allocs, 3, masks_D, nd * B * kMaskPerSample, nd * M * kMaskPerSample, &md));
+  FG_TRY(s.in(c, c->allocs, 4, masks_G, ng * B * kMaskPerSample, ng * M * kMaskPerSample, &mg));
+  FG_TRY(net_train_step_iters(c, h, B, d_iters, g_iters, r, zd, zg, md, mg, seed, nullptr, nullptr));
+  return pair_step_stats(c, c->net, stats);
+}
 
 int fg_sample(fg_ctx* c, const float* noise, int N, int chunk, float* images_out) {
   ENTER(c);

@@ -185,11 +185,17 @@ __global__ void __launch_bounds__(kPairThreads) c2f_pairs_kernel(const uint8_t* 
     if (diff) diff[o + i] = sfine[i] - v;
   }
 }
-__global__ void draw_indices_kernel(int32_t* __restrict__ idx, int B, uint64_t seed, int64_t N) {
+// root (optional): the stream is *root * kinds + seed, read on the device (the per-iteration stream roots of a captured
+// multi-iteration step, k_seed_roots)
+__global__ void draw_indices_kernel(int32_t* __restrict__ idx, int B, uint64_t seed, int64_t N, const uint64_t* root = nullptr,
+                                    uint64_t kinds = 0) {
+  if (root) seed += *root * kinds;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < B) idx[i] = (int32_t)(splitmix64(seed * 0x100000001B3ull + (uint64_t)i) % (uint64_t)N);
 }
-__global__ void uniform_pm1_kernel(float* __restrict__ out, int64_t n, uint64_t seed) {
+__global__ void uniform_pm1_kernel(float* __restrict__ out, int64_t n, uint64_t seed, const uint64_t* root = nullptr,
+                                   uint64_t kinds = 0) {
+  if (root) seed += *root * kinds;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const uint64_t r = splitmix64(seed * 0x100000001B3ull + (uint64_t)i);
     out[i] = (float)(r >> 40) * (2.0f / 16777216.0f) - 1.0f;  // 24-bit uniform in [-1, 1)
@@ -399,6 +405,10 @@ int fg_dataset_destroy(fg_dataset* d) {
   if (d->c) {
     cudaSetDevice(d->c->device);
     cudaStreamSynchronize(d->c->stream);
+    // the device-fed multi-iteration steps capture the draws and gathers, i.e. d->data, d->idx and d->N, into the
+    // step graphs of this ctx (32x32, --scale 16 and c2f alike): none of them may be replayed once these are freed,
+    // even if a later dataset is allocated at the same host address
+    d->c->graph_epoch++;
   }
   cudaFree(d->data);
   cudaFree(d->idx);
@@ -567,6 +577,36 @@ int fg_train_step_dataset(fg_ctx* c, fg_dataset* d, const fg_hyper* h, int B, ui
   return pair_step_stats(c, c->net, stats);
 }
 
+// fg_train_step_iters fed on the device: the inputs of D iteration j are gather(draw(4*r_j)) and uniform(4*r_j+1), those
+// of G iteration j uniform(4*r_j+2), r_j the stream root of iteration j (fg_b200.h).  The draws run inside the step
+// (one graph launch per call once captured), each reading its root from c->seed_dev.
+int fg_train_step_dataset_iters(fg_ctx* c, fg_dataset* d, const fg_hyper* h, int B, int d_iters, int g_iters, uint64_t seed,
+                                fg_step_stats* stats) {
+  ENTER(d);
+  FG_TRY(iters_check(d_iters, g_iters, "fg_train_step_dataset_iters"));
+  FG_TRY(dataset_check_feed(d, c, "fg_train_step_dataset_iters"));
+  FG_REQUIRE(h && B >= 4 && B % 2 == 0 && B <= c->maxB,
+             "fg_train_step_dataset_iters: batch %d must be even, >= 4 and <= max_batch %d", B, c->maxB);
+  const int Bh = B / 2;
+  const size_t M = c->maxB, img = (size_t)c->C * 1024;
+  IterStage& s = c->iter_stage;
+  FG_TRY(s.reserve(c, c->allocs, 0, d_iters * M / 2 * img));
+  FG_TRY(s.reserve(c, c->allocs, 1, d_iters * M / 2 * kNoiseDim));
+  FG_TRY(s.reserve(c, c->allocs, 2, g_iters * M * kNoiseDim));
+  float *real = s.p[0], *zd = s.p[1], *zg = s.p[2];
+  const std::function<int()> feed = [&]() -> int {
+    for (int j = 0; j < d_iters; ++j) {
+      FG_TRY(dataset_draw_gather(d, 0, Bh, 32, real + (size_t)j * Bh * img, c->seed_dev + j, 4));
+      FG_TRY(noise_uniform_dev(c, 1, (int64_t)Bh * kNoiseDim, zd + (size_t)j * Bh * kNoiseDim, c->seed_dev + j, 4));
+    }
+    for (int j = 0; j < g_iters; ++j)
+      FG_TRY(noise_uniform_dev(c, 2, (int64_t)B * kNoiseDim, zg + (size_t)j * B * kNoiseDim, c->seed_dev + j, 4));
+    return FG_OK;
+  };
+  FG_TRY(net_train_step_iters(c, h, B, d_iters, g_iters, real, zd, zg, nullptr, nullptr, seed, feed, d));
+  return pair_step_stats(c, c->net, stats);
+}
+
 }  // extern "C"
 
 // ---- batch assembly of the device-fed --scale 16 and coarse-to-fine steps (nets_s16.cu, nets_c2f.cu) ----------
@@ -576,21 +616,21 @@ int dataset_check_feed(const fg_dataset* d, const fg_ctx* c, const char* what) {
   FG_REQUIRE(!(d->Cs == 1 && c->C == 3), "%s: a grayscale cache cannot feed a colour context", what);
   return FG_OK;
 }
-int dataset_draw_gather(fg_dataset* d, uint64_t seed, int B, int size, float* out_dev) {
+int dataset_draw_gather(fg_dataset* d, uint64_t seed, int B, int size, float* out_dev, const uint64_t* root, uint64_t kinds) {
   fg_ctx* c = d->c;
-  draw_indices_kernel<<<(B + 127) / 128, 128, 0, c->stream>>>(d->idx, B, seed, d->N);
+  draw_indices_kernel<<<(B + 127) / 128, 128, 0, c->stream>>>(d->idx, B, seed, d->N, root, kinds);
   LAUNCH_CHECK(c);
   return gather(d, d->idx, B, out_dev, size);
 }
 int dataset_draw_gather_c2f(fg_dataset* d, uint64_t seed, int B, int fine_size, int coarse_size, float* fine, float* coarse,
-                            float* diff) {
+                            float* diff, const uint64_t* root, uint64_t kinds) {
   fg_ctx* c = d->c;
-  draw_indices_kernel<<<(B + 127) / 128, 128, 0, c->stream>>>(d->idx, B, seed, d->N);
+  draw_indices_kernel<<<(B + 127) / 128, 128, 0, c->stream>>>(d->idx, B, seed, d->N, root, kinds);
   LAUNCH_CHECK(c);
   return gather_c2f(d, d->idx, B, fine_size, coarse_size, fine, coarse, diff);
 }
-int noise_uniform_dev(fg_ctx* c, uint64_t seed, int64_t n, float* out_dev) {
-  uniform_pm1_kernel<<<grid_for(n, 256), 256, 0, c->stream>>>(out_dev, n, seed);
+int noise_uniform_dev(fg_ctx* c, uint64_t seed, int64_t n, float* out_dev, const uint64_t* root, uint64_t kinds) {
+  uniform_pm1_kernel<<<grid_for(n, 256), 256, 0, c->stream>>>(out_dev, n, seed, root, kinds);
   LAUNCH_CHECK(c);
   return FG_OK;
 }

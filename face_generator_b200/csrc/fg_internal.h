@@ -86,6 +86,9 @@ struct DeviceStats {  // lives in device memory; mirrored to fg_step_stats
   int do_train_D, do_train_G;
 };
 constexpr int kAccHistMax = 1024;
+// the most D or G iterations one train step runs (train.lua --D_iterations / --G_iterations); c->seed_dev holds one
+// stream root per iteration (k_seed_roots)
+constexpr int kMaxIters = 16;
 constexpr int kBnState = 768;  // running mean / var of G's two BatchNorm layers: [mean1 256][var1 256][mean2 128][var2 128]
 
 // A captured train step (net_graph_run) and the key it was captured under
@@ -222,6 +225,17 @@ struct TimerRec {
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pending;
 };
 
+// the staging buffers of the stacked inputs of a multi-iteration step: one device buffer per input kind, grown on
+// demand (the old buffer is released, so a grown buffer gets a new address and with it a new graph key)
+struct IterStage {
+  float* p[8] = {};
+  size_t cap[8] = {};
+  int reserve(fg_ctx* c, std::vector<void*>& allocs, int k, size_t n);
+  // *out = the n floats at p on the device: p itself (device memory or null), else buffer k (at least `cap_n` floats)
+  // after an async copy
+  int in(fg_ctx* c, std::vector<void*>& allocs, int k, const float* p, size_t n, size_t cap_n, const float** out);
+};
+
 struct fg_ctx {
   int device = 0, maxB = 0, C = 3;
   cudaStream_t stream = nullptr;
@@ -280,6 +294,7 @@ struct fg_ctx {
   size_t io_dev_elems = 0;
   float* io_dev2 = nullptr;
   float *in_real = nullptr, *in_noiseD = nullptr, *in_noiseG = nullptr, *in_masksD = nullptr, *in_masksG = nullptr;
+  IterStage iter_stage;  // the stacked inputs of fg_train_step_iters / fg_train_step_dataset_iters
   float* scratch[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   size_t scratch_elems[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   // data parallel
@@ -379,6 +394,9 @@ int k_sigmoid_bwd(fg_ctx* c, const float* dy, const float* y, float* dz, int64_t
 int k_masks_generate(fg_ctx* c, float* masks, int B, uint64_t seed, float p_spatial, float p_drop,
                      const uint64_t* seed_dev = nullptr);  // seed_dev: effective seed = *seed_dev * 2 + seed
 int k_set_u64(fg_ctx* c, uint64_t* dst, uint64_t v);
+// roots[j] = 2^60 | roots[0] << 8 | j for 1 <= j < n: the stream root of iteration j of a multi-iteration step
+// (fg_b200.h, "Several D and G iterations per call"); roots[0] is the step seed
+int k_seed_roots(fg_ctx* c, uint64_t* roots, int n);
 // hi / lo (optional): also emit the TF32 split of the result (16-byte aligned buffers of the output's size)
 int k_d_act_pool_fwd(fg_ctx* c, const float* z, const float* slope, const float* masks, int moff, float eval_scale,
                      float* p, int B, int H, int W, int C, float* hi = nullptr, float* lo = nullptr);
@@ -398,8 +416,9 @@ int k_bce_bwd(fg_ctx* c, const float* x, const float* t, int n, float* dx);
 int k_sigmoid_grad_mul(fg_ctx* c, const float* dout, const float* out, float* dlogit, int n);
 // optimizer
 int k_penalty_loss(fg_ctx* c, const float* p, int64_t n, float l1, float l2, float* loss_inout);
+// accumulate: conf and trained_D add to the values of the earlier D iterations of the same step instead of replacing them
 int k_gate_and_prep(fg_ctx* c, DeviceStats* st, float* acc_hist, int net, const fg_hyper* h, const float* tail4, int B,
-                    float world);
+                    float world, bool accumulate = false);
 int k_gemv_fwd(fg_ctx* c, const float* x, const float* w, const float* bias, float* out, int B, int K);
 int k_gemv_dgrad(fg_ctx* c, const float* dy, const float* w, float* dx, int B, int K);
 int k_gemv_wgrad_add(fg_ctx* c, const float* x, const float* dy, float* dw, float* db, int B, int K);
@@ -450,6 +469,14 @@ int net_D_backward(fg_ctx* c, const float* dlogit_dev, bool want_wgrad, bool wan
 int net_train_step(fg_ctx* c, const fg_hyper* h, int B, const float* real_nchw_dev, const float* noiseD_dev,
                    const float* noiseG_dev, const float* masksD_dev, const float* masksG_dev, uint64_t seed,
                    bool allow_graph = false);
+// nd D iterations + ng G iterations on inputs stacked per iteration (fg_train_step_iters).  feed (may be empty) runs
+// first inside the step, after the stream roots are set: the device-fed step draws its inputs there; feed_key names
+// what the feed reads (the dataset), for the graph key.
+int net_train_step_iters(fg_ctx* c, const fg_hyper* h, int B, int nd, int ng, const float* real, const float* noiseD,
+                         const float* noiseG, const float* masksD, const float* masksG, uint64_t seed,
+                         const std::function<int()>& feed, const void* feed_key);
+// 1 <= nd, ng <= kMaxIters, else FG_ERR_UNSUPPORTED
+int iters_check(int nd, int ng, const char* what);
 int net_allreduce(fg_ctx* c, float* buf, int64_t n);
 int net_broadcast(fg_ctx* c, void* buf, size_t bytes);  // rank 0 -> all (dp.cu)
 int net_group(bool start);                                // ncclGroupStart / ncclGroupEnd
@@ -465,7 +492,7 @@ void pair_free(NetPair& p);  // graphs and the pinned mirror; the device buffers
 int pair_zero_grads(fg_ctx* c, NetPair& p, int net);       // GRAD_PARAMETERS_x:zero() incl. the tail scalars
 int pair_allreduce_grads(fg_ctx* c, NetPair& p, int net);  // gradient + tail (one call when contiguous); world 1: nothing
 // the accuracy gate (D), t += 1 and the step size of `net` on the pair's own statistics
-int pair_gate(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, int B, float world);
+int pair_gate(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, int B, float world, bool accumulate = false);
 int pair_optim(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, float grad_scale);  // penalty -> clamp -> update
 int pair_broadcast(fg_ctx* c, NetPair& p);  // rank 0's parameters, moments, BatchNorm state, statistics, history
 int pair_step_stats(fg_ctx* c, const NetPair& p, fg_step_stats* stats);  // synchronise, then the last step's statistics
@@ -477,9 +504,10 @@ int pair_get_adam_state(fg_ctx* c, const NetPair& p, int net, float* m, float* v
 int pair_set_bn_state(fg_ctx* c, NetPair& p, const float* src);
 int pair_get_bn_state(fg_ctx* c, const NetPair& p, float* dst);
 // Runs `body` (launches on c->stream that read their seed from c->seed_dev) as a train step of pair p: eagerly, or as a
-// captured CUDA graph keyed on B, *h, `inputs`, the stream, the communicator, graph_epoch and pack_key
+// captured CUDA graph keyed on B, *h, `inputs`, the stream, the communicator, graph_epoch, pack_key and the iteration
+// counts nd / ng
 int net_graph_run(fg_ctx* c, NetPair& p, int B, const fg_hyper* h, std::initializer_list<const void*> inputs, uint64_t seed,
-                  const std::function<int()>& body, bool allow_graph);
+                  const std::function<int()>& body, bool allow_graph, int nd = 1, int ng = 1);
 
 // ---- capi.cu: host or device pointers at the C ABI ----
 bool fg_is_dev(const void* p);
@@ -498,11 +526,14 @@ struct DebugTensor {
 int64_t debug_tensor_copy(fg_ctx* c, const char* what, const DebugTensor* ents, size_t n_ents, const char* name, float* dst,
                           int64_t max_elems);
 
-// ---- dataset.cu: inputs of the device-fed --scale 16 / coarse-to-fine steps (eager launches on the ctx stream) ----
+// ---- dataset.cu: inputs of the device-fed --scale 16 / coarse-to-fine steps (launches on the ctx stream) ----
+// root (optional): the stream is *root * kinds + seed, read on the device (a captured step replays with a new seed)
 int dataset_check_feed(const fg_dataset* d, const fg_ctx* c, const char* what);  // same ctx, compatible channels
 // out [B][C][size][size] (device) = gather at `size` of B indices drawn from stream `seed` (fg_dataset_draw)
-int dataset_draw_gather(fg_dataset* d, uint64_t seed, int B, int size, float* out_dev);
+int dataset_draw_gather(fg_dataset* d, uint64_t seed, int B, int size, float* out_dev, const uint64_t* root = nullptr,
+                        uint64_t kinds = 0);
 // fine / coarse / diff [B][C][S][S] (device, any may be null) = fg_dataset_gather_c2f_sized of B indices drawn from `seed`
 int dataset_draw_gather_c2f(fg_dataset* d, uint64_t seed, int B, int fine_size, int coarse_size, float* fine, float* coarse,
-                            float* diff);
-int noise_uniform_dev(fg_ctx* c, uint64_t seed, int64_t n, float* out_dev);  // fg_noise_uniform into device memory
+                            float* diff, const uint64_t* root = nullptr, uint64_t kinds = 0);
+// fg_noise_uniform into device memory
+int noise_uniform_dev(fg_ctx* c, uint64_t seed, int64_t n, float* out_dev, const uint64_t* root = nullptr, uint64_t kinds = 0);

@@ -756,6 +756,15 @@ int k_set_u64(fg_ctx* c, uint64_t* dst, uint64_t v) {
   LAUNCH_CHECK(c);
   return FG_OK;
 }
+__global__ void seed_roots_kernel(uint64_t* roots, int n) {
+  const int j = threadIdx.x;
+  if (j >= 1 && j < n) roots[j] = (1ull << 60) | (roots[0] << 8) | (uint64_t)j;
+}
+int k_seed_roots(fg_ctx* c, uint64_t* roots, int n) {
+  seed_roots_kernel<<<1, 32, 0, c->stream>>>(roots, n);
+  LAUNCH_CHECK(c);
+  return FG_OK;
+}
 int k_masks_generate(fg_ctx* c, float* masks, int B, uint64_t seed, float p_spatial, float p_drop, const uint64_t* seed_dev) {
   masks_generate_kernel<<<grid_for((int64_t)B * kMaskPerSample, 256), 256, 0, c->stream>>>(masks, B, seed, p_spatial,
                                                                                           p_drop, seed_dev);
@@ -1071,7 +1080,10 @@ __device__ __forceinline__ float step_size(const fg_hyper& h, int opt, float lr,
   if (opt != FG_OPT_ADAM) return lr;
   return (float)((double)lr * sqrt(1.0 - pow((double)h.beta2, t)) / (1.0 - pow((double)h.beta1, t)));
 }
-__global__ void gate_prep_kernel(DeviceStats* st, float* acc_hist, int net, fg_hyper h, const float* tail4, float total, int opt) {
+// accumulate: a later D iteration of the same step -- CONFUSION:add runs in every fevalD (adversarial.lua:115) and
+// countTrainedD counts every iteration that stepped (:170), so conf and trained_D add up over the step's iterations
+__global__ void gate_prep_kernel(DeviceStats* st, float* acc_hist, int net, fg_hyper h, const float* tail4, float total, int opt,
+                                 int accumulate) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   if (net == FG_NET_D) {
     int interval = h.accs_interval;
@@ -1079,7 +1091,7 @@ __global__ void gate_prep_kernel(DeviceStats* st, float* acc_hist, int net, fg_h
     if (interval > kAccHistMax) interval = kAccHistMax;
     const float correct = tail4[0] + tail4[3];
     const float tV = correct / total;
-    for (int i = 0; i < 4; ++i) st->conf[i] = (int)(tail4[i] + 0.5f);
+    for (int i = 0; i < 4; ++i) st->conf[i] = (accumulate ? st->conf[i] : 0) + (int)(tail4[i] + 0.5f);
     st->acc_D = tV;
     acc_hist[st->acc_head] = tV;
     st->acc_head = (st->acc_head + 1) % interval;
@@ -1089,7 +1101,7 @@ __global__ void gate_prep_kernel(DeviceStats* st, float* acc_hist, int net, fg_h
     m /= st->acc_count;
     const int go = m < (double)h.D_maxAcc ? 1 : 0;
     st->do_train_D = go;
-    st->trained_D = go;
+    st->trained_D = (accumulate ? st->trained_D : 0) + go;
     if (go) {
       st->t_D += 1;
       st->step_D = step_size(h, opt, h.lr_D, (double)st->t_D);
@@ -1101,8 +1113,9 @@ __global__ void gate_prep_kernel(DeviceStats* st, float* acc_hist, int net, fg_h
   }
 }
 int k_gate_and_prep(fg_ctx* c, DeviceStats* st, float* acc_hist, int net, const fg_hyper* h, const float* tail4, int B,
-                    float world) {
-  gate_prep_kernel<<<1, 32, 0, c->stream>>>(st, acc_hist, net, *h, tail4, (float)B * world, net == FG_NET_D ? c->opt_D : c->opt_G);
+                    float world, bool accumulate) {
+  gate_prep_kernel<<<1, 32, 0, c->stream>>>(st, acc_hist, net, *h, tail4, (float)B * world, net == FG_NET_D ? c->opt_D : c->opt_G,
+                                            accumulate ? 1 : 0);
   LAUNCH_CHECK(c);
   return FG_OK;
 }

@@ -90,8 +90,37 @@ int pair_allreduce_grads(fg_ctx* c, NetPair& p, int net) {
   return net_group(false);
 }
 
-int pair_gate(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, int B, float world) {
-  return k_gate_and_prep(c, p.dstats, p.acc_hist, net, h, half(p, net).tail, B, world);
+int pair_gate(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, int B, float world, bool accumulate) {
+  return k_gate_and_prep(c, p.dstats, p.acc_hist, net, h, half(p, net).tail, B, world, accumulate);
+}
+
+int IterStage::reserve(fg_ctx* c, std::vector<void*>& allocs, int k, size_t n) {
+  if (cap[k] >= n) return FG_OK;
+  if (p[k]) {
+    FG_CUDA(cudaStreamSynchronize(c->stream));  // an earlier step may still read the old buffer
+    allocs.erase(std::find(allocs.begin(), allocs.end(), (void*)p[k]));
+    cudaFree(p[k]);
+    p[k] = nullptr;
+    cap[k] = 0;
+  }
+  FG_TRY(fg_dalloc(c, allocs, &p[k], n));
+  cap[k] = n;
+  return FG_OK;
+}
+
+int IterStage::in(fg_ctx* c, std::vector<void*>& allocs, int k, const float* q, size_t n, size_t cap_n, const float** out) {
+  *out = q;
+  if (!q || fg_is_dev(q)) return FG_OK;
+  FG_TRY(reserve(c, allocs, k, std::max(n, cap_n)));
+  return fg_to_dev(c, q, n, p[k], out);
+}
+
+int iters_check(int nd, int ng, const char* what) {
+  if (nd < 1 || nd > kMaxIters || ng < 1 || ng > kMaxIters) {
+    fg_set_error("%s: %d D and %d G iterations; each count must lie in [1, %d]", what, nd, ng, kMaxIters);
+    return FG_ERR_UNSUPPORTED;
+  }
+  return FG_OK;
 }
 
 // penalty -> clamp -> interruptable optimizer on the flat vectors (adversarial.lua:219-231, interruptable_optimizers.lua)
@@ -207,13 +236,15 @@ void key_add(std::vector<uint8_t>& k, const T& v) {
 // The packs are marked stale before the capture and after every replay: the captured sequence has to contain the pack
 // kernels whatever the flags said at capture time, and a replayed optimizer step invalidates them again.
 int net_graph_run(fg_ctx* c, NetPair& p, int B, const fg_hyper* h, std::initializer_list<const void*> inputs, uint64_t seed,
-                  const std::function<int()>& body, bool allow_graph) {
+                  const std::function<int()>& body, bool allow_graph, int nd, int ng) {
   FG_TRY(k_set_u64(c, c->seed_dev, seed));
   static const bool env_off = getenv("FG_GRAPH") && atoi(getenv("FG_GRAPH")) == 0;
   if (!allow_graph || !c->use_graph || env_off || c->timing || c->debug_keep) return body();
   std::vector<uint8_t> key;
   key_add(key, c->graph_epoch);
   key_add(key, B);
+  key_add(key, nd);
+  key_add(key, ng);
   key_add(key, pack_key(c));
   key_add(key, *h);
   for (const void* q : inputs) key_add(key, q);

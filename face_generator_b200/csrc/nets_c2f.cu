@@ -48,6 +48,7 @@ struct fg_c2f {
   float *ga = nullptr, *gb = nullptr, *ws = nullptr;
   float *in_a = nullptr, *in_b = nullptr, *in_c = nullptr, *in_d = nullptr, *in_e = nullptr, *in_m1 = nullptr,
         *in_m2 = nullptr, *io = nullptr;
+  IterStage iter_stage;  // the stacked inputs of fg_c2f_train_step_iters / fg_c2f_train_step_dataset_iters
   int G_B = 0, D_B = 0;
   bool G_valid = false, D_valid = false, D_train = true;
   float D_scale = 2.f;
@@ -321,10 +322,10 @@ int D_backward(fg_c2f* n, const float* dlogit, bool want_wgrad, bool want_dx) {
 }
 
 // t += 1 and the Adam step size on the device (shares the kernel of the 32x32 loop; no accuracy gate here)
-int prep(fg_c2f* n, int net, const fg_hyper* h, int B) {
+int prep(fg_c2f* n, int net, const fg_hyper* h, int B, bool accumulate = false) {
   fg_hyper hh = *h;
   hh.D_maxAcc = 1e30f;
-  return pair_gate(n->c, n->net, net, &hh, B, (float)n->c->world);
+  return pair_gate(n->c, n->net, net, &hh, B, (float)n->c->world, accumulate);
 }
 
 // option "debug_keep": copy the D step's pre-activations and outputs to keep_D ("Dstep.*" debug tensors)
@@ -341,45 +342,57 @@ int keep_dstep(fg_c2f* n, int B) {
   return FG_OK;
 }
 
-int train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_diff, const float* condD, const float* noiseD,
-               const float* condG, const float* noiseG, const float* masksD, const float* masksG, uint64_t seed) {
+// nD D iterations (adversarial_c2f.lua:121-163), then nG G iterations (:167-187), on inputs stacked per iteration; the
+// dropout masks of iteration j come from the stream root c->seed_dev[j] (k_seed_roots).  feed (may be null) draws the
+// inputs on the device first.
+int train_step(fg_c2f* n, const fg_hyper* h, int B, int nD, int nG, const float* real_diff, const float* condD,
+               const float* noiseD, const float* condG, const float* noiseG, const float* masksD, const float* masksG,
+               const std::function<int()>* feed) {
   fg_ctx* c = n->c;
   const int Bh = B / 2, C = n->C;
-  const size_t img = (size_t)C * n->HW;
+  const size_t img = (size_t)C * n->HW, mask = (size_t)B * n->mask;
   const float inv_world = 1.0f / (float)c->world;
-  // ---- D step (adversarial_c2f.lua:121-163) ----
-  FG_TRY(G_forward(n, noiseD, condD + Bh * img, Bh));
-  FG_TRY(k_nchw_to_nhwc(c, real_diff, n->io, Bh, C, n->HW));
-  FG_CUDA(cudaMemcpyAsync(n->io + Bh * img, n->G_z[4], sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
-  FG_TRY(k_nchw_to_nhwc(c, condD, n->D_cond, B, C, n->HW));
-  if (masksD)
-    FG_CUDA(cudaMemcpyAsync(n->D_masks, masksD, sizeof(float) * (size_t)B * n->mask, cudaMemcpyDeviceToDevice, c->stream));
-  else
-    FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * n->mask, 1, h->p_drop, c->seed_dev));
-  FG_TRY(pair_zero_grads(c, n->net, FG_NET_D));
-  FG_TRY(D_forward(n, n->io, n->D_cond, B, true, h->p_drop));
-  FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_D, n->net.tailD, B, Bh));
-  if (c->debug_keep) FG_TRY(keep_dstep(n, B));
-  FG_TRY(D_backward(n, n->D_dlogit, true, false));
-  FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_D));
-  FG_TRY(prep(n, FG_NET_D, h, B));
-  // optim.adam / optim.adagrad / optim.sgd (adversarial_c2f.lua:153-161, :177-185): same rules as the interruptable ones
-  FG_TRY(pair_optim(c, n->net, FG_NET_D, h, inv_world));
-  // ---- G step (adversarial_c2f.lua:167-187) ----
-  FG_TRY(pair_zero_grads(c, n->net, FG_NET_G));
-  FG_TRY(G_forward(n, noiseG, condG, B));
-  FG_TRY(k_nchw_to_nhwc(c, condG, n->D_cond, B, C, n->HW));
-  if (masksG)
-    FG_CUDA(cudaMemcpyAsync(n->D_masks, masksG, sizeof(float) * (size_t)B * n->mask, cudaMemcpyDeviceToDevice, c->stream));
-  else
-    FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * n->mask, 2, h->p_drop, c->seed_dev));
-  FG_TRY(D_forward(n, n->G_z[4], n->D_cond, B, true, h->p_drop));
-  FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_G, n->net.tailG, B, B));
-  FG_TRY(D_backward(n, n->D_dlogit, false, true));  // D's weight grads are zeroed before use (:45) -> skipped
-  FG_TRY(G_backward(n, n->D_dx));
-  FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_G));
-  FG_TRY(prep(n, FG_NET_G, h, B));
-  FG_TRY(pair_optim(c, n->net, FG_NET_G, h, inv_world));
+  if (nD > 1 || nG > 1) FG_TRY(k_seed_roots(c, c->seed_dev, std::max(nD, nG)));
+  if (feed && *feed) FG_TRY((*feed)());
+  for (int j = 0; j < nD; ++j) {
+    // ---- D iteration j (adversarial_c2f.lua:121-163) ----
+    const float* cd = condD + (size_t)j * B * img;
+    FG_TRY(G_forward(n, noiseD + (size_t)j * Bh * n->HW, cd + Bh * img, Bh));
+    FG_TRY(k_nchw_to_nhwc(c, real_diff + (size_t)j * Bh * img, n->io, Bh, C, n->HW));
+    FG_CUDA(cudaMemcpyAsync(n->io + Bh * img, n->G_z[4], sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
+    FG_TRY(k_nchw_to_nhwc(c, cd, n->D_cond, B, C, n->HW));
+    if (masksD)
+      FG_CUDA(cudaMemcpyAsync(n->D_masks, masksD + j * mask, sizeof(float) * mask, cudaMemcpyDeviceToDevice, c->stream));
+    else
+      FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)mask, 1, h->p_drop, c->seed_dev + j));
+    FG_TRY(pair_zero_grads(c, n->net, FG_NET_D));
+    FG_TRY(D_forward(n, n->io, n->D_cond, B, true, h->p_drop));
+    FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_D, n->net.tailD, B, Bh));
+    if (c->debug_keep) FG_TRY(keep_dstep(n, B));
+    FG_TRY(D_backward(n, n->D_dlogit, true, false));
+    FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_D));
+    FG_TRY(prep(n, FG_NET_D, h, B, j > 0));
+    // optim.adam / optim.adagrad / optim.sgd (adversarial_c2f.lua:153-161, :177-185): same rules as the interruptable ones
+    FG_TRY(pair_optim(c, n->net, FG_NET_D, h, inv_world));
+  }
+  for (int j = 0; j < nG; ++j) {
+    // ---- G iteration j (adversarial_c2f.lua:167-187) ----
+    const float* cg = condG + (size_t)j * B * img;
+    FG_TRY(pair_zero_grads(c, n->net, FG_NET_G));
+    FG_TRY(G_forward(n, noiseG + (size_t)j * B * n->HW, cg, B));
+    FG_TRY(k_nchw_to_nhwc(c, cg, n->D_cond, B, C, n->HW));
+    if (masksG)
+      FG_CUDA(cudaMemcpyAsync(n->D_masks, masksG + j * mask, sizeof(float) * mask, cudaMemcpyDeviceToDevice, c->stream));
+    else
+      FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)mask, 2, h->p_drop, c->seed_dev + j));
+    FG_TRY(D_forward(n, n->G_z[4], n->D_cond, B, true, h->p_drop));
+    FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_G, n->net.tailG, B, B));
+    FG_TRY(D_backward(n, n->D_dlogit, false, true));  // D's weight grads are zeroed before use (:45) -> skipped
+    FG_TRY(G_backward(n, n->D_dx));
+    FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_G));
+    FG_TRY(prep(n, FG_NET_G, h, B));
+    FG_TRY(pair_optim(c, n->net, FG_NET_G, h, inv_world));
+  }
   FG_CUDA(cudaMemcpyAsync(n->net.hstats, n->net.dstats, sizeof(DeviceStats), cudaMemcpyDeviceToHost, c->stream));
   return FG_OK;
 }
@@ -387,10 +400,12 @@ int train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_diff, cons
 // train_step on device inputs: eager the first time, then a captured CUDA graph of the step (net_graph_run); the seed
 // is read on the device
 int run_train_step(fg_c2f* n, const fg_hyper* h, int B, const float* rd, const float* cd, const float* nd, const float* cg,
-                   const float* ng, const float* md, const float* mg, uint64_t seed, fg_step_stats* stats) {
+                   const float* ng, const float* md, const float* mg, uint64_t seed, fg_step_stats* stats, int nD = 1,
+                   int nG = 1, const std::function<int()>* feed = nullptr, const void* feed_key = nullptr,
+                   int coarse_size = 0) {
   FG_TRY(net_graph_run(
-      n->c, n->net, B, h, {rd, cd, nd, cg, ng, md, mg}, seed,
-      [&]() { return train_step(n, h, B, rd, cd, nd, cg, ng, md, mg, 0); }, true));
+      n->c, n->net, B, h, {rd, cd, nd, cg, ng, md, mg, feed_key, (const void*)(intptr_t)coarse_size}, seed,
+      [&]() { return train_step(n, h, B, nD, nG, rd, cd, nd, cg, ng, md, mg, feed); }, true, nD, nG));
   return pair_step_stats(n->c, n->net, stats);
 }
 }  // namespace
@@ -615,6 +630,69 @@ int fg_c2f_train_step_dataset(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B
   FG_TRY(noise_uniform_dev(c, seed * 8 + 3, (int64_t)Bh * n->HW, n->in_c));
   FG_TRY(noise_uniform_dev(c, seed * 8 + 4, (int64_t)B * n->HW, n->in_e));
   return run_train_step(n, h, B, n->in_a, n->in_b, n->in_c, n->in_d, n->in_e, nullptr, nullptr, seed, stats);
+}
+
+// d_iters D iterations + g_iters G iterations of the c2f loop body on the fg_c2f_train_step inputs stacked per iteration
+int fg_c2f_train_step_iters(fg_c2f* n, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real_diff,
+                            const float* cond_D, const float* noise_D, const float* cond_G, const float* noise_G,
+                            const float* masks_D, const float* masks_G, uint64_t seed, fg_step_stats* stats) {
+  ENTER(n);
+  FG_TRY(iters_check(d_iters, g_iters, "fg_c2f_train_step_iters"));
+  FG_REQUIRE(h && real_diff && cond_D && noise_D && cond_G && noise_G, "fg_c2f_train_step_iters: null input");
+  FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= n->maxB, "fg_c2f_train_step_iters: batch %d must be even, >= 4 and <= max_batch %d",
+             B, n->maxB);
+  fg_ctx* c = n->c;
+  const size_t nd = d_iters, ng = g_iters, Bh = B / 2, M = n->maxB, img = (size_t)n->C * n->HW, hw = n->HW, mk = n->mask;
+  IterStage& s = n->iter_stage;
+  const float *rd, *cd, *zd, *cg, *zg, *md, *mg;
+  FG_TRY(s.in(c, n->allocs, 0, real_diff, nd * Bh * img, nd * M / 2 * img, &rd));
+  FG_TRY(s.in(c, n->allocs, 1, cond_D, nd * B * img, nd * M * img, &cd));
+  FG_TRY(s.in(c, n->allocs, 2, noise_D, nd * Bh * hw, nd * M / 2 * hw, &zd));
+  FG_TRY(s.in(c, n->allocs, 3, cond_G, ng * B * img, ng * M * img, &cg));
+  FG_TRY(s.in(c, n->allocs, 4, noise_G, ng * B * hw, ng * M * hw, &zg));
+  FG_TRY(s.in(c, n->allocs, 5, masks_D, nd * B * mk, nd * M * mk, &md));
+  FG_TRY(s.in(c, n->allocs, 6, masks_G, ng * B * mk, ng * M * mk, &mg));
+  return run_train_step(n, h, B, rd, cd, zd, cg, zg, md, mg, seed, stats, d_iters, g_iters);
+}
+
+// fg_c2f_train_step_iters fed on the device: D iteration j draws the streams 8*r_j .. 8*r_j+1 and 8*r_j+3, G iteration
+// j the streams 8*r_j+2 and 8*r_j+4, as fg_c2f_train_step_dataset does for r_0 = seed (r_j: fg_b200.h); the draws run
+// inside the step
+int fg_c2f_train_step_dataset_iters(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B, int d_iters, int g_iters,
+                                    int coarse_size, uint64_t seed, fg_step_stats* stats) {
+  ENTER(n);
+  fg_ctx* c = n->c;
+  FG_TRY(iters_check(d_iters, g_iters, "fg_c2f_train_step_dataset_iters"));
+  FG_TRY(dataset_check_feed(d, c, "fg_c2f_train_step_dataset_iters"));
+  FG_REQUIRE(h && B >= 4 && B % 2 == 0 && B <= n->maxB,
+             "fg_c2f_train_step_dataset_iters: batch %d must be even, >= 4 and <= max_batch %d", B, n->maxB);
+  FG_REQUIRE(coarse_size >= 1 && coarse_size <= n->S, "fg_c2f_train_step_dataset_iters: coarse size %d outside [1, %d]",
+             coarse_size, n->S);
+  const int Bh = B / 2, S = n->S;
+  const size_t M = n->maxB, img = (size_t)n->C * n->HW, hw = n->HW;
+  IterStage& s = n->iter_stage;
+  FG_TRY(s.reserve(c, n->allocs, 0, d_iters * M / 2 * img));
+  FG_TRY(s.reserve(c, n->allocs, 1, d_iters * M * img));
+  FG_TRY(s.reserve(c, n->allocs, 2, d_iters * M / 2 * hw));
+  FG_TRY(s.reserve(c, n->allocs, 3, g_iters * M * img));
+  FG_TRY(s.reserve(c, n->allocs, 4, g_iters * M * hw));
+  float *rd = s.p[0], *cd = s.p[1], *zd = s.p[2], *cg = s.p[3], *zg = s.p[4];
+  const std::function<int()> feed = [&]() -> int {
+    for (int j = 0; j < d_iters; ++j) {
+      const uint64_t* r = c->seed_dev + j;
+      float* cdj = cd + (size_t)j * B * img;
+      FG_TRY(dataset_draw_gather_c2f(d, 0, Bh, S, coarse_size, nullptr, cdj, rd + (size_t)j * Bh * img, r, 8));
+      FG_TRY(dataset_draw_gather_c2f(d, 1, Bh, S, coarse_size, nullptr, cdj + Bh * img, nullptr, r, 8));
+      FG_TRY(noise_uniform_dev(c, 3, (int64_t)Bh * hw, zd + (size_t)j * Bh * hw, r, 8));
+    }
+    for (int j = 0; j < g_iters; ++j) {
+      const uint64_t* r = c->seed_dev + j;
+      FG_TRY(dataset_draw_gather_c2f(d, 2, B, S, coarse_size, nullptr, cg + (size_t)j * B * img, nullptr, r, 8));
+      FG_TRY(noise_uniform_dev(c, 4, (int64_t)B * hw, zg + (size_t)j * B * hw, r, 8));
+    }
+    return FG_OK;
+  };
+  return run_train_step(n, h, B, rd, cd, zd, cg, zg, nullptr, nullptr, seed, stats, d_iters, g_iters, &feed, d, coarse_size);
 }
 
 int64_t fg_c2f_debug_tensor(fg_c2f* n, const char* name, float* dst, int64_t max_elems) {

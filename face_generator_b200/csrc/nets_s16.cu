@@ -119,6 +119,7 @@ struct fg_s16 {
   // shared scratch
   float *ga = nullptr, *gb = nullptr, *ws = nullptr;
   float *in_a = nullptr, *in_b = nullptr, *in_c = nullptr, *in_m1 = nullptr, *in_m2 = nullptr, *io = nullptr;
+  IterStage iter_stage;  // the stacked inputs of fg_s16_train_step_iters / fg_s16_train_step_dataset_iters
   int D_pack_impl = -1;
   int D_B = 0;
   bool D_valid = false, D_train = true;
@@ -374,43 +375,51 @@ int keep_dstep(fg_s16* n, int B) {
   return FG_OK;
 }
 
-// one iteration of the adversarial.lua loop body (D_iterations = G_iterations = 1) on the 16x16 nets
-int train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const float* noiseD, const float* noiseG,
-               const float* masksD, const float* masksG, uint64_t seed) {
+// the adversarial.lua loop body on the 16x16 nets: nD D iterations, then nG G iterations, on inputs stacked per
+// iteration; the dropout masks of iteration j come from the stream root c->seed_dev[j] (k_seed_roots).  feed (may be
+// null) draws the inputs on the device first.
+int train_step(fg_s16* n, const fg_hyper* h, int B, int nD, int nG, const float* real, const float* noiseD,
+               const float* noiseG, const float* masksD, const float* masksG, const std::function<int()>* feed) {
   fg_ctx* c = n->c;
   const int Bh = B / 2, C = n->C;
-  const size_t img = (size_t)C * 256;
+  const size_t img = (size_t)C * 256, mask = (size_t)B * kS16Mask;
   const float inv_world = 1.0f / (float)c->world;
-  // ---- D step (adversarial.lua:240-268) ----
-  FG_TRY(gen_forward(n->env, n->G, n->net, noiseD, Bh, true));  // createImages: G in training mode (nn_utils.lua:52)
-  FG_TRY(k_nchw_to_nhwc(c, real, n->D_x, Bh, C, 256));
-  FG_CUDA(cudaMemcpyAsync(n->D_x + Bh * img, n->G.y, sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
-  if (masksD)
-    FG_CUDA(cudaMemcpyAsync(n->D_masks, masksD, sizeof(float) * (size_t)B * kS16Mask, cudaMemcpyDeviceToDevice, c->stream));
-  else
-    FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * kS16Mask, 1, 0.5f, c->seed_dev));
-  FG_TRY(pair_zero_grads(c, n->net, FG_NET_D));
-  FG_TRY(D_forward(n, n->D_x, B, true));
-  FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_D, n->net.tailD, B, Bh));
-  if (c->debug_keep) FG_TRY(keep_dstep(n, B));
-  FG_TRY(D_backward(n, n->D_dlogit, true, false));
-  FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_D));
-  FG_TRY(pair_gate(c, n->net, FG_NET_D, h, B, (float)c->world));
-  FG_TRY(pair_optim(c, n->net, FG_NET_D, h, inv_world));
-  // ---- G step (adversarial.lua:275-288) ----
-  FG_TRY(pair_zero_grads(c, n->net, FG_NET_G));
-  FG_TRY(gen_forward(n->env, n->G, n->net, noiseG, B, true));
-  if (masksG)
-    FG_CUDA(cudaMemcpyAsync(n->D_masks, masksG, sizeof(float) * (size_t)B * kS16Mask, cudaMemcpyDeviceToDevice, c->stream));
-  else
-    FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)B * kS16Mask, 2, 0.5f, c->seed_dev));
-  FG_TRY(D_forward(n, n->G.y, B, true));
-  FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_G, n->net.tailG, B, B));
-  FG_TRY(D_backward(n, n->D_dlogit, false, true));  // D's weight grads are discarded by the reference (:209 vs :92)
-  FG_TRY(gen_backward(n->env, n->G, n->net, n->D_dx, nullptr));
-  FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_G));
-  FG_TRY(pair_gate(c, n->net, FG_NET_G, h, B, (float)c->world));
-  FG_TRY(pair_optim(c, n->net, FG_NET_G, h, inv_world));
+  if (nD > 1 || nG > 1) FG_TRY(k_seed_roots(c, c->seed_dev, std::max(nD, nG)));
+  if (feed && *feed) FG_TRY((*feed)());
+  for (int j = 0; j < nD; ++j) {
+    // ---- D iteration j (adversarial.lua:240-268) ----
+    FG_TRY(gen_forward(n->env, n->G, n->net, noiseD + (size_t)j * Bh * 100, Bh, true));  // createImages: training mode
+    FG_TRY(k_nchw_to_nhwc(c, real + (size_t)j * Bh * img, n->D_x, Bh, C, 256));
+    FG_CUDA(cudaMemcpyAsync(n->D_x + Bh * img, n->G.y, sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
+    if (masksD)
+      FG_CUDA(cudaMemcpyAsync(n->D_masks, masksD + j * mask, sizeof(float) * mask, cudaMemcpyDeviceToDevice, c->stream));
+    else
+      FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)mask, 1, 0.5f, c->seed_dev + j));
+    FG_TRY(pair_zero_grads(c, n->net, FG_NET_D));
+    FG_TRY(D_forward(n, n->D_x, B, true));
+    FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_D, n->net.tailD, B, Bh));
+    if (c->debug_keep) FG_TRY(keep_dstep(n, B));
+    FG_TRY(D_backward(n, n->D_dlogit, true, false));
+    FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_D));
+    FG_TRY(pair_gate(c, n->net, FG_NET_D, h, B, (float)c->world, j > 0));
+    FG_TRY(pair_optim(c, n->net, FG_NET_D, h, inv_world));
+  }
+  for (int j = 0; j < nG; ++j) {
+    // ---- G iteration j (adversarial.lua:275-288) ----
+    FG_TRY(pair_zero_grads(c, n->net, FG_NET_G));
+    FG_TRY(gen_forward(n->env, n->G, n->net, noiseG + (size_t)j * B * 100, B, true));
+    if (masksG)
+      FG_CUDA(cudaMemcpyAsync(n->D_masks, masksG + j * mask, sizeof(float) * mask, cudaMemcpyDeviceToDevice, c->stream));
+    else
+      FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)mask, 2, 0.5f, c->seed_dev + j));
+    FG_TRY(D_forward(n, n->G.y, B, true));
+    FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_G, n->net.tailG, B, B));
+    FG_TRY(D_backward(n, n->D_dlogit, false, true));  // D's weight grads are discarded by the reference (:209 vs :92)
+    FG_TRY(gen_backward(n->env, n->G, n->net, n->D_dx, nullptr));
+    FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_G));
+    FG_TRY(pair_gate(c, n->net, FG_NET_G, h, B, (float)c->world));
+    FG_TRY(pair_optim(c, n->net, FG_NET_G, h, inv_world));
+  }
   FG_CUDA(cudaMemcpyAsync(n->net.hstats, n->net.dstats, sizeof(DeviceStats), cudaMemcpyDeviceToHost, c->stream));
   return FG_OK;
 }
@@ -418,9 +427,11 @@ int train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const flo
 // train_step on device inputs: eager the first time, then a captured CUDA graph of the step (net_graph_run); the seed
 // is read on the device
 int run_train_step(fg_s16* n, const fg_hyper* h, int B, const float* rd, const float* nd, const float* ng, const float* md,
-                   const float* mg, uint64_t seed, fg_step_stats* stats) {
+                   const float* mg, uint64_t seed, fg_step_stats* stats, int nD = 1, int nG = 1,
+                   const std::function<int()>* feed = nullptr, const void* feed_key = nullptr) {
   FG_TRY(net_graph_run(
-      n->c, n->net, B, h, {rd, nd, ng, md, mg}, seed, [&]() { return train_step(n, h, B, rd, nd, ng, md, mg, 0); }, true));
+      n->c, n->net, B, h, {rd, nd, ng, md, mg, feed_key}, seed,
+      [&]() { return train_step(n, h, B, nD, nG, rd, nd, ng, md, mg, feed); }, true, nD, nG));
   return pair_step_stats(n->c, n->net, stats);
 }
 }  // namespace
@@ -609,6 +620,56 @@ int fg_s16_train_step_dataset(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B
   FG_TRY(noise_uniform_dev(c, seed * 4 + 1, (int64_t)(B / 2) * 100, n->in_b));
   FG_TRY(noise_uniform_dev(c, seed * 4 + 2, (int64_t)B * 100, n->in_c));
   return run_train_step(n, h, B, n->in_a, n->in_b, n->in_c, nullptr, nullptr, seed, stats);
+}
+
+// d_iters D iterations + g_iters G iterations on inputs stacked per iteration (fg_train_step_iters at 16x16)
+int fg_s16_train_step_iters(fg_s16* n, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,
+                            const float* noise_D, const float* noise_G, const float* masks_D, const float* masks_G,
+                            uint64_t seed, fg_step_stats* stats) {
+  ENTER(n);
+  FG_TRY(iters_check(d_iters, g_iters, "fg_s16_train_step_iters"));
+  FG_REQUIRE(h && real && noise_D && noise_G, "fg_s16_train_step_iters: null input");
+  FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= n->maxB, "fg_s16_train_step_iters: batch %d must be even, >= 4 and <= max_batch %d",
+             B, n->maxB);
+  fg_ctx* c = n->c;
+  const size_t nd = d_iters, ng = g_iters, Bh = B / 2, M = n->maxB, img = (size_t)n->C * 256;
+  IterStage& s = n->iter_stage;
+  const float *rd, *zd, *zg, *md, *mg;
+  FG_TRY(s.in(c, n->allocs, 0, real, nd * Bh * img, nd * M / 2 * img, &rd));
+  FG_TRY(s.in(c, n->allocs, 1, noise_D, nd * Bh * 100, nd * M / 2 * 100, &zd));
+  FG_TRY(s.in(c, n->allocs, 2, noise_G, ng * B * 100, ng * M * 100, &zg));
+  FG_TRY(s.in(c, n->allocs, 3, masks_D, nd * B * kS16Mask, nd * M * kS16Mask, &md));
+  FG_TRY(s.in(c, n->allocs, 4, masks_G, ng * B * kS16Mask, ng * M * kS16Mask, &mg));
+  return run_train_step(n, h, B, rd, zd, zg, md, mg, seed, stats, d_iters, g_iters);
+}
+
+// fg_s16_train_step_iters fed on the device: the streams of fg_train_step_dataset_iters, the real halves at 16x16;
+// the draws run inside the step
+int fg_s16_train_step_dataset_iters(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B, int d_iters, int g_iters,
+                                    uint64_t seed, fg_step_stats* stats) {
+  ENTER(n);
+  fg_ctx* c = n->c;
+  FG_TRY(iters_check(d_iters, g_iters, "fg_s16_train_step_dataset_iters"));
+  FG_TRY(dataset_check_feed(d, c, "fg_s16_train_step_dataset_iters"));
+  FG_REQUIRE(h && B >= 4 && B % 2 == 0 && B <= n->maxB,
+             "fg_s16_train_step_dataset_iters: batch %d must be even, >= 4 and <= max_batch %d", B, n->maxB);
+  const int Bh = B / 2;
+  const size_t M = n->maxB, img = (size_t)n->C * 256;
+  IterStage& s = n->iter_stage;
+  FG_TRY(s.reserve(c, n->allocs, 0, d_iters * M / 2 * img));
+  FG_TRY(s.reserve(c, n->allocs, 1, d_iters * M / 2 * 100));
+  FG_TRY(s.reserve(c, n->allocs, 2, g_iters * M * 100));
+  float *real = s.p[0], *zd = s.p[1], *zg = s.p[2];
+  const std::function<int()> feed = [&]() -> int {
+    for (int j = 0; j < d_iters; ++j) {
+      FG_TRY(dataset_draw_gather(d, 0, Bh, kSide, real + (size_t)j * Bh * img, c->seed_dev + j, 4));
+      FG_TRY(noise_uniform_dev(c, 1, (int64_t)Bh * 100, zd + (size_t)j * Bh * 100, c->seed_dev + j, 4));
+    }
+    for (int j = 0; j < g_iters; ++j)
+      FG_TRY(noise_uniform_dev(c, 2, (int64_t)B * 100, zg + (size_t)j * B * 100, c->seed_dev + j, 4));
+    return FG_OK;
+  };
+  return run_train_step(n, h, B, real, zd, zg, nullptr, nullptr, seed, stats, d_iters, g_iters, &feed, d);
 }
 
 int64_t fg_s16_debug_tensor(fg_s16* n, const char* name, float* dst, int64_t max_elems) {

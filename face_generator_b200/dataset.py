@@ -6,6 +6,7 @@
     real16 = ds.gather(indices, 16)               # the same at 16x16 (train.lua --scale 16)
     fine, coarse, diff = ds.gather_c2f(indices, 16)   # dataset_c2f.lua _toResult (train_c2f.lua --coarseSize 16)
     stats = ds.train_step(hyper, B, seed)         # adversarial.lua loop body with no host->device traffic
+    stats = ds.train_step_iters(hyper, B, 2, 1, seed)          # --D_iterations 2: two D iterations, one G iteration
     S16(ctx).train_step_dataset(ds, hyper, B, seed)            # the same for the --scale 16 nets
     C2f(ctx).train_step_dataset(ds, hyper, B, 16, seed)        # and for the coarse-to-fine nets
     C2f(ctx, 64).train_step_dataset(ds, hyper, B, 32, seed)    # the pyramid level 32x32 -> 64x64 (--fineSize 64)
@@ -14,7 +15,7 @@ import ctypes as C
 
 import numpy as np
 
-from .lib import Context, StepStats, _check, _stats
+from .lib import Context, StepStats, _check, _stats, check_iters
 
 
 class DeviceDataset:
@@ -73,6 +74,15 @@ class DeviceDataset:
         st = StepStats() if want_stats else None
         _check(self.lib.fg_train_step_dataset(self.ctx.h, self.h, C.byref(hyper), B, seed,
                                               C.byref(st) if st is not None else None), "fg_train_step_dataset")
+        return _stats(st)
+
+    def train_step_iters(self, hyper, B, D_iterations, G_iterations, seed, want_stats=True):
+        """D_iterations D iterations + G_iterations G iterations of the 32x32 nets in one call, every input drawn on
+        the device inside the step (fg_train_step_dataset_iters; the streams are in fg_b200.h)."""
+        d, g = check_iters(D_iterations, G_iterations)
+        st = StepStats() if want_stats else None
+        _check(self.lib.fg_train_step_dataset_iters(self.ctx.h, self.h, C.byref(hyper), B, d, g, seed,
+                                                    C.byref(st) if st is not None else None), "fg_train_step_dataset_iters")
         return _stats(st)
 
 

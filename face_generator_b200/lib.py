@@ -181,7 +181,35 @@ SYMBOLS = {
     "fg_event_elapsed_ms": (_I, [_P, _I, _I, C.POINTER(C.c_double)]),
     "fg_timing_enable": (_I, [_P, _I]),
     "fg_timing_get": (_I, [_P, C.c_char_p, C.POINTER(C.c_double), C.POINTER(_L)]),
+    "fg_train_step_iters": (_I, [_P, C.POINTER(Hyper), _I, _I, _I, _P, _P, _P, _P, _P, _U64, C.POINTER(StepStats)]),
+    "fg_s16_train_step_iters": (_I, [_P, C.POINTER(Hyper), _I, _I, _I, _P, _P, _P, _P, _P, _U64, C.POINTER(StepStats)]),
+    "fg_c2f_train_step_iters": (_I, [_P, C.POINTER(Hyper), _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _U64,
+                                     C.POINTER(StepStats)]),
+    "fg_train_step_dataset_iters": (_I, [_P, _P, C.POINTER(Hyper), _I, _I, _I, _U64, C.POINTER(StepStats)]),
+    "fg_s16_train_step_dataset_iters": (_I, [_P, _P, C.POINTER(Hyper), _I, _I, _I, _U64, C.POINTER(StepStats)]),
+    "fg_c2f_train_step_dataset_iters": (_I, [_P, _P, C.POINTER(Hyper), _I, _I, _I, _I, _U64, C.POINTER(StepStats)]),
 }
+
+MAX_ITERS = 16  # the most D or G iterations one call runs (fg_train_step_iters)
+
+
+def check_iters(D_iterations, G_iterations):
+    """train.lua --D_iterations / --G_iterations as the _iters entry points take them: integers in [1, 16].
+    D_iterations = 0 is not supported.  Raises ValueError before anything runs."""
+    for name, v in (("D_iterations", D_iterations), ("G_iterations", G_iterations)):
+        if int(v) != v or not 1 <= int(v) <= MAX_ITERS:
+            raise ValueError("%s = %r: must be an integer in [1, %d]" % (name, v, MAX_ITERS))
+    return int(D_iterations), int(G_iterations)
+
+
+def iteration_root(seed, j):
+    """The stream root of iteration j of a multi-iteration step with step seed `seed` (fg_b200.h): the seed itself for
+    j = 0, else 2^60 | seed << 8 | j (64-bit).  Dropout masks of iteration j use 2*root+1 (D) / 2*root+2 (G); the
+    device-fed steps draw from 4*root+k (8*root+k for c2f)."""
+    seed = int(seed) & (2 ** 64 - 1)
+    if j == 0:
+        return seed
+    return ((1 << 60) | (seed << 8) | int(j)) & (2 ** 64 - 1)
 
 _lib = None
 
@@ -424,6 +452,18 @@ class Context(_BatchNormNetPair):
                "fg_train_step")
         return _stats(st)
 
+    def train_step_iters(self, hyper, B, D_iterations, G_iterations, real, noise_D, noise_G, masks_D=None, masks_G=None,
+                         seed=0, want_stats=True):
+        """D_iterations D iterations + G_iterations G iterations in one call (fg_train_step_iters); the inputs of
+        train_step stacked per iteration: real [d][B/2][C][32][32], noise_D [d][B/2][100], noise_G [g][B][100],
+        masks_* [d|g][B][1984] or None."""
+        d, g = check_iters(D_iterations, G_iterations)
+        st = StepStats() if want_stats else None
+        _check(self.lib.fg_train_step_iters(self.h, C.byref(hyper), B, d, g, _ptr(real), _ptr(noise_D), _ptr(noise_G),
+                                            _ptr(masks_D), _ptr(masks_G), seed, C.byref(st) if st is not None else None),
+               "fg_train_step_iters")
+        return _stats(st)
+
     def sample(self, noise, chunk):
         noise = f32(noise)
         N = noise.shape[0]
@@ -647,6 +687,27 @@ class C2f(_NetPair):
                                                   C.byref(st) if st is not None else None), "fg_c2f_train_step_dataset")
         return _stats(st)
 
+    def train_step_iters(self, hyper, B, D_iterations, G_iterations, real_diff, cond_D, noise_D, cond_G, noise_G,
+                         masks_D=None, masks_G=None, seed=0, want_stats=True):
+        """D_iterations D iterations + G_iterations G iterations in one call (fg_c2f_train_step_iters); the train_step
+        inputs stacked per iteration: real_diff [d][B/2], cond_D [d][B], noise_D [d][B/2], cond_G / noise_G [g][B],
+        masks_* [d|g][B][mask_per_sample] or None."""
+        d, g = check_iters(D_iterations, G_iterations)
+        st = StepStats() if want_stats else None
+        _check(self.lib.fg_c2f_train_step_iters(self.h, C.byref(hyper), B, d, g, _ptr(real_diff), _ptr(cond_D),
+                                                _ptr(noise_D), _ptr(cond_G), _ptr(noise_G), _ptr(masks_D), _ptr(masks_G),
+                                                seed, C.byref(st) if st is not None else None), "fg_c2f_train_step_iters")
+        return _stats(st)
+
+    def train_step_dataset_iters(self, dataset, hyper, B, D_iterations, G_iterations, coarse_size, seed, want_stats=True):
+        """train_step_iters with every input drawn on the device, inside the step (fg_c2f_train_step_dataset_iters)."""
+        d, g = check_iters(D_iterations, G_iterations)
+        st = StepStats() if want_stats else None
+        _check(self.lib.fg_c2f_train_step_dataset_iters(self.h, dataset.h, C.byref(hyper), B, d, g, coarse_size, seed,
+                                                        C.byref(st) if st is not None else None),
+               "fg_c2f_train_step_dataset_iters")
+        return _stats(st)
+
 
 S16_MASK_PER_SAMPLE = 1024 + 128
 
@@ -715,4 +776,24 @@ class S16(_BatchNormNetPair):
         st = StepStats() if want_stats else None
         _check(self.lib.fg_s16_train_step_dataset(self.h, dataset.h, C.byref(hyper), B, seed,
                                                   C.byref(st) if st is not None else None), "fg_s16_train_step_dataset")
+        return _stats(st)
+
+    def train_step_iters(self, hyper, B, D_iterations, G_iterations, real, noise_D, noise_G, masks_D=None, masks_G=None,
+                         seed=0, want_stats=True):
+        """fg_s16_train_step_iters: train_step's inputs stacked per iteration (real [d][B/2][C][16][16], noise_D
+        [d][B/2][100], noise_G [g][B][100], masks_* [d|g][B][1152] or None)."""
+        d, g = check_iters(D_iterations, G_iterations)
+        st = StepStats() if want_stats else None
+        _check(self.lib.fg_s16_train_step_iters(self.h, C.byref(hyper), B, d, g, _ptr(real), _ptr(noise_D), _ptr(noise_G),
+                                                _ptr(masks_D), _ptr(masks_G), seed, C.byref(st) if st is not None else None),
+               "fg_s16_train_step_iters")
+        return _stats(st)
+
+    def train_step_dataset_iters(self, dataset, hyper, B, D_iterations, G_iterations, seed, want_stats=True):
+        """train_step_iters with every input drawn on the device, inside the step (fg_s16_train_step_dataset_iters)."""
+        d, g = check_iters(D_iterations, G_iterations)
+        st = StepStats() if want_stats else None
+        _check(self.lib.fg_s16_train_step_dataset_iters(self.h, dataset.h, C.byref(hyper), B, d, g, seed,
+                                                        C.byref(st) if st is not None else None),
+               "fg_s16_train_step_dataset_iters")
         return _stats(st)

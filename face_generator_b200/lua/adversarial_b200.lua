@@ -1,5 +1,6 @@
 -- adversarial_b200.lua -- drop-in for adversarial.lua's loop body (adversarial.lua:54-300): the whole
--- "1 D iteration + 1 G iteration" (batch assembly excluded) is ONE fg_train_step call.  Keeps the globals
+-- "OPT.D_iterations D iterations + OPT.G_iterations G iterations" (batch assembly excluded) is ONE call, fg_train_step
+-- for 1 + 1 and fg_train_step_iters otherwise.  Keeps the globals
 -- train.lua sets up (OPT, OPTSTATE, CONFUSION, NN_UTILS, IMG_DIMENSIONS) and the ADVERSARIAL.train signature.
 -- Delivered untested-by-execution (no LuaJIT/Torch7 in the build image); face_generator_b200/adversarial.py
 -- is the executable mirror.
@@ -66,25 +67,42 @@ function adversarial.train(dataset, maxAccuracyD, accsInterval)
   local stats = ffi.new('fg_step_stats[1]')
   local time = sys.clock()
   local seed = (EPOCH - 1) * 1000000
+  -- train.lua --D_iterations / --G_iterations (train.lua:33-34): D and G optimizer steps per batch, 1..16 each
+  local dIters, gIters = OPT.D_iterations or 1, OPT.G_iterations or 1
+  assert(dIters >= 1 and dIters <= 16 and gIters >= 1 and gIters <= 16, 'b200: --D_iterations / --G_iterations must lie in [1, 16]')
   for t = 1, N_epoch, dataBatchSize do
     local thisBatchSize = math.min(OPT.batchSize, N_epoch - t + 1)
     if thisBatchSize < 4 then break end                      -- adversarial.lua:73-76
     thisBatchSize = thisBatchSize - thisBatchSize % 2        -- even batches only (SURVEY appendix 13)
     local half = thisBatchSize / 2
-    -- (1.1) real half-batch (adversarial.lua:244-249)
-    local real = torch.FloatTensor(half, IMG_DIMENSIONS[1], IMG_DIMENSIONS[2], IMG_DIMENSIONS[3])
-    for i = 1, half do real[i] = dataset[math.random(dataset:size())] end
-    -- (1.2)/(2) noise for the D-step fakes and for the G step (nn_utils.lua:35-39)
-    local noiseD = NN_UTILS.createNoiseInputs(half)
-    local noiseG = NN_UTILS.createNoiseInputs(thisBatchSize)
+    local dims = IMG_DIMENSIONS
+    -- every D iteration draws its own real half-batch (1.1, adversarial.lua:244-249) and its own noise for the fakes
+    -- (1.2, nn_utils.lua:35-39); every G iteration its own noise (2, :276); stacked per iteration
+    local real = torch.FloatTensor(dIters, half, dims[1], dims[2], dims[3])
+    local noiseD = torch.FloatTensor(dIters, half, 100)
+    for j = 1, dIters do
+      for i = 1, half do real[j][i] = dataset[math.random(dataset:size())] end
+      noiseD[j]:copy(NN_UTILS.createNoiseInputs(half))
+    end
+    local noiseG = torch.FloatTensor(gIters, thisBatchSize, 100)
+    for j = 1, gIters do noiseG[j]:copy(NN_UTILS.createNoiseInputs(thisBatchSize)) end
     seed = seed + 1
-    if s16 then
-      F.check(C.fg_s16_train_step(s16, hyper, thisBatchSize, F.ptr(real), F.ptr(noiseD), F.ptr(noiseG), nil, nil, seed, stats), 'fg_s16_train_step')
+    if dIters == 1 and gIters == 1 then
+      if s16 then
+        F.check(C.fg_s16_train_step(s16, hyper, thisBatchSize, F.ptr(real), F.ptr(noiseD), F.ptr(noiseG), nil, nil, seed, stats), 'fg_s16_train_step')
+      else
+        F.check(C.fg_train_step(ctx, hyper, thisBatchSize, F.ptr(real), F.ptr(noiseD), F.ptr(noiseG), nil, nil, seed, stats), 'fg_train_step')
+      end
+    elseif s16 then
+      F.check(C.fg_s16_train_step_iters(s16, hyper, thisBatchSize, dIters, gIters, F.ptr(real), F.ptr(noiseD), F.ptr(noiseG),
+                                        nil, nil, seed, stats), 'fg_s16_train_step_iters')
     else
-      F.check(C.fg_train_step(ctx, hyper, thisBatchSize, F.ptr(real), F.ptr(noiseD), F.ptr(noiseG), nil, nil, seed, stats), 'fg_train_step')
+      F.check(C.fg_train_step_iters(ctx, hyper, thisBatchSize, dIters, gIters, F.ptr(real), F.ptr(noiseD), F.ptr(noiseG),
+                                    nil, nil, seed, stats), 'fg_train_step_iters')
     end
     local s = stats[0]
-    -- feed optim.ConfusionMatrix exactly like adversarial.lua:112-117 (rows = predicted class, cols = target)
+    -- feed optim.ConfusionMatrix exactly like adversarial.lua:112-117 (rows = predicted class, cols = target); conf
+    -- sums over the call's D iterations, as CONFUSION:add does once per fevalD
     CONFUSION.mat[2][2] = CONFUSION.mat[2][2] + s.conf[0]
     CONFUSION.mat[1][2] = CONFUSION.mat[1][2] + s.conf[1]
     CONFUSION.mat[2][1] = CONFUSION.mat[2][1] + s.conf[2]

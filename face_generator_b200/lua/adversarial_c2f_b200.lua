@@ -1,5 +1,6 @@
--- adversarial_c2f_b200.lua -- drop-in for adversarial_c2f.lua's loop body (adversarial_c2f.lua:121-187): one
--- "D iteration + G iteration" of the coarse-to-fine GAN is ONE fg_c2f_train_step call.  Keeps the globals
+-- adversarial_c2f_b200.lua -- drop-in for adversarial_c2f.lua's loop body (adversarial_c2f.lua:121-187): the
+-- "OPT.D_iterations D iterations + OPT.G_iterations G iterations" of the coarse-to-fine GAN are ONE call
+-- (fg_c2f_train_step for 1 + 1, fg_c2f_train_step_iters otherwise).  Keeps the globals
 -- train_c2f.lua sets up (OPT, OPTSTATE, CONFUSION, IMG_DIMENSIONS, NOISE_DIM, COND_DIM) and the
 -- adversarial.train(trainData) signature; batch assembly (random {diff, coarse} pairs, adversarial_c2f.lua:124-141,
 -- :168-174) stays in Lua exactly as in the reference.
@@ -39,30 +40,46 @@ function adversarial.train(trainData)
   local time = sys.clock()
   local seed = (EPOCH - 1) * 1000000
   local dims = IMG_DIMENSIONS
+  -- train_c2f.lua --D_iterations / --G_iterations (train_c2f.lua:31-32): 1..16 each
+  local dIters, gIters = OPT.D_iterations or 1, OPT.G_iterations or 1
+  assert(dIters >= 1 and dIters <= 16 and gIters >= 1 and gIters <= 16, 'b200: --D_iterations / --G_iterations must lie in [1, 16]')
   for t = 1, N_epoch, dataBatchSize do
     local B = math.min(OPT.batchSize, N_epoch - t + 1)
     if B < 4 then break end                                  -- adversarial_c2f.lua:33-36
     B = B - B % 2
     local half = B / 2
-    local realDiff = torch.FloatTensor(half, dims[1], dims[2], dims[3])
-    local condD = torch.FloatTensor(B, COND_DIM[1], COND_DIM[2], COND_DIM[3])
-    local condG = torch.FloatTensor(B, COND_DIM[1], COND_DIM[2], COND_DIM[3])
-    for i = 1, half do                                       -- (1.1) real pairs, :124-132
-      local ex = trainData[math.random(trainData:size())]
-      realDiff[i] = ex.diff
-      condD[i] = ex.coarse
+    -- every D iteration draws its own pairs, coarse images and noise, every G iteration its own coarse images and
+    -- noise (the reference's fevalD / fevalG_on_D draws, once per iteration); stacked per iteration
+    local realDiff = torch.FloatTensor(dIters, half, dims[1], dims[2], dims[3])
+    local condD = torch.FloatTensor(dIters, B, COND_DIM[1], COND_DIM[2], COND_DIM[3])
+    local noiseD = torch.FloatTensor(dIters, half, NOISE_DIM[1], NOISE_DIM[2], NOISE_DIM[3])
+    local condG = torch.FloatTensor(gIters, B, COND_DIM[1], COND_DIM[2], COND_DIM[3])
+    local noiseG = torch.FloatTensor(gIters, B, NOISE_DIM[1], NOISE_DIM[2], NOISE_DIM[3])
+    for j = 1, dIters do
+      for i = 1, half do                                     -- (1.1) real pairs, :124-132
+        local ex = trainData[math.random(trainData:size())]
+        realDiff[j][i] = ex.diff
+        condD[j][i] = ex.coarse
+      end
+      for i = half + 1, B do                                 -- (1.2) coarse images for the generated half, :136-141
+        condD[j][i] = trainData[math.random(trainData:size())].coarse
+      end
+      noiseD[j]:uniform(-1, 1)
     end
-    for i = half + 1, B do                                   -- (1.2) coarse images for the generated half, :136-141
-      condD[i] = trainData[math.random(trainData:size())].coarse
+    for j = 1, gIters do
+      for i = 1, B do                                        -- (2) fresh coarse images for the G step, :170-174
+        condG[j][i] = trainData[math.random(trainData:size())].coarse
+      end
+      noiseG[j]:uniform(-1, 1)
     end
-    for i = 1, B do                                          -- (2) fresh coarse images for the G step, :170-174
-      condG[i] = trainData[math.random(trainData:size())].coarse
-    end
-    local noiseD = torch.FloatTensor(half, NOISE_DIM[1], NOISE_DIM[2], NOISE_DIM[3]):uniform(-1, 1)
-    local noiseG = torch.FloatTensor(B, NOISE_DIM[1], NOISE_DIM[2], NOISE_DIM[3]):uniform(-1, 1)
     seed = seed + 1
-    F.check(C.fg_c2f_train_step(n, hyper, B, F.ptr(realDiff), F.ptr(condD), F.ptr(noiseD), F.ptr(condG), F.ptr(noiseG),
-                                nil, nil, seed, stats), 'fg_c2f_train_step')
+    if dIters == 1 and gIters == 1 then
+      F.check(C.fg_c2f_train_step(n, hyper, B, F.ptr(realDiff), F.ptr(condD), F.ptr(noiseD), F.ptr(condG), F.ptr(noiseG),
+                                  nil, nil, seed, stats), 'fg_c2f_train_step')
+    else
+      F.check(C.fg_c2f_train_step_iters(n, hyper, B, dIters, gIters, F.ptr(realDiff), F.ptr(condD), F.ptr(noiseD),
+                                        F.ptr(condG), F.ptr(noiseG), nil, nil, seed, stats), 'fg_c2f_train_step_iters')
+    end
     local s = stats[0]
     CONFUSION.mat[2][2] = CONFUSION.mat[2][2] + s.conf[0]    -- adversarial_c2f.lua:66-70
     CONFUSION.mat[1][2] = CONFUSION.mat[1][2] + s.conf[1]

@@ -157,6 +157,21 @@ int fg_s16_train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, co
 int fg_s16_train_step_dataset(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B, uint64_t seed, fg_step_stats* stats);
 int fg_c2f_train_step_dataset(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B, int coarse_size, uint64_t seed,
                               fg_step_stats* stats);
+int fg_train_step_iters(fg_ctx* ctx, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,
+                        const float* noise_D, const float* noise_G, const float* masks_D, const float* masks_G, uint64_t seed,
+                        fg_step_stats* stats);
+int fg_s16_train_step_iters(fg_s16* n, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,
+                            const float* noise_D, const float* noise_G, const float* masks_D, const float* masks_G,
+                            uint64_t seed, fg_step_stats* stats);
+int fg_c2f_train_step_iters(fg_c2f* n, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real_diff,
+                            const float* cond_D, const float* noise_D, const float* cond_G, const float* noise_G,
+                            const float* masks_D, const float* masks_G, uint64_t seed, fg_step_stats* stats);
+int fg_train_step_dataset_iters(fg_ctx* ctx, fg_dataset* d, const fg_hyper* h, int B, int d_iters, int g_iters, uint64_t seed,
+                                fg_step_stats* stats);
+int fg_s16_train_step_dataset_iters(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B, int d_iters, int g_iters,
+                                    uint64_t seed, fg_step_stats* stats);
+int fg_c2f_train_step_dataset_iters(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B, int d_iters, int g_iters,
+                                    int coarse_size, uint64_t seed, fg_step_stats* stats);
 int fg_c2f_dp_broadcast_params(fg_c2f* n);
 int fg_s16_dp_broadcast_params(fg_s16* n);
 int fg_dp_world(fg_ctx* ctx);

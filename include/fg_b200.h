@@ -340,6 +340,44 @@ int fg_s16_train_step_dataset(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B
 int fg_c2f_train_step_dataset(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B, int coarse_size, uint64_t seed,
                               fg_step_stats* stats);
 
+/* ---- several D and G iterations per call (train.lua / train_c2f.lua --D_iterations, --G_iterations) ---- */
+/* One call runs d_iters D iterations, then g_iters G iterations (adversarial.lua:240-288,
+ * adversarial_c2f.lua:121-187), as one captured step.  D iteration j draws its own fakes from a
+ * training-mode G forward (G's BatchNorm running statistics move once per D iteration), runs D
+ * forward/backward, BCE, penalty, clamp and, for the 32x32 and 16x16 nets, the accuracy gate on its own
+ * accuracy, then its own optimizer step; iteration j+1 sees the D that iteration j left.  G iteration j
+ * is a full G step with its own optimizer step.  Inputs are those of the single-iteration entries,
+ * stacked per iteration: real [d][B/2][C][S][S], noise_D [d][B/2][..], noise_G [g][B][..], masks_D
+ * [d][B][mask], masks_G [g][B][mask] (or NULL: drawn from the stream roots below), c2f cond_D [d][B][..],
+ * cond_G [g][B][..].  1 <= d_iters, g_iters <= 16, anything else is FG_ERR_UNSUPPORTED before any work
+ * (D_iterations = 0 is not supported).  The statistics of a call: conf sums over the D iterations,
+ * trained_D counts the D iterations that stepped, loss_D / acc_D are those of the last D iteration,
+ * loss_G that of the last G iteration, t_D / t_G the counters after the call.  With d_iters = g_iters = 1
+ * a call is bit for bit the single-iteration entry.
+ * Stream roots: iteration j of a call with step seed s draws from the root r_j, r_0 = s and
+ * r_j = 2^60 | s << 8 | j for j >= 1 (64-bit arithmetic; distinct from every r_0 while s < 2^52).
+ * Its dropout masks use the streams of seed r_j (2*r_j+1 for D iteration j, 2*r_j+2 for G iteration j);
+ * the _dataset_iters entries draw D iteration j's real half from fg_dataset_draw(4*r_j) and its noise
+ * from fg_noise_uniform(4*r_j+1), G iteration j's noise from fg_noise_uniform(4*r_j+2); c2f: real pairs
+ * 8*r_j, fake cond 8*r_j+1 and noise_D 8*r_j+3 for D iteration j, G cond 8*r_j+2 and noise_G 8*r_j+4 for
+ * G iteration j.  For j = 0 these are the streams of the single-iteration entries.                   */
+int fg_train_step_iters(fg_ctx* ctx, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,
+                        const float* noise_D, const float* noise_G, const float* masks_D, const float* masks_G, uint64_t seed,
+                        fg_step_stats* stats);
+int fg_s16_train_step_iters(fg_s16* n, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,
+                            const float* noise_D, const float* noise_G, const float* masks_D, const float* masks_G,
+                            uint64_t seed, fg_step_stats* stats);
+int fg_c2f_train_step_iters(fg_c2f* n, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real_diff,
+                            const float* cond_D, const float* noise_D, const float* cond_G, const float* noise_G,
+                            const float* masks_D, const float* masks_G, uint64_t seed, fg_step_stats* stats);
+/* every input drawn on the device, inside the step (one graph launch per call once captured)          */
+int fg_train_step_dataset_iters(fg_ctx* ctx, fg_dataset* d, const fg_hyper* h, int B, int d_iters, int g_iters, uint64_t seed,
+                                fg_step_stats* stats);
+int fg_s16_train_step_dataset_iters(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B, int d_iters, int g_iters,
+                                    uint64_t seed, fg_step_stats* stats);
+int fg_c2f_train_step_dataset_iters(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B, int d_iters, int g_iters,
+                                    int coarse_size, uint64_t seed, fg_step_stats* stats);
+
 /* ---- scoring helpers of the sampler / the c2f trainer ------------------------------------------ */
 /* device part of NN_UTILS.sortImagesByPrediction (utils/nn_utils.lua:90-98; sample.lua:84-85):
  * D's prediction for N images [N][C][32][32], `chunk` (= OPT.batchSize) at a time.  training=1 is
