@@ -176,3 +176,39 @@ def load_flat_checkpoint(ctx, path):
                                int(f.number("adam_%s_t" % name)))
         ctx.set_bn_state(f.tensor("bn_G"))
         return int(f.number("epoch"))
+
+
+def read_denoiser_checkpoint(path, channels, size):
+    """train_denoiser.lua's `denoiser_CxHxW.net` ({AE1_ENCODER, AE1_DECODER, AE2_DECODER}, :360-362) as flat vectors:
+    dict(P1, P2, bn1, bn2), the getParameters() order and BatchNorm running statistics of the two decoders (AE2_DECODER
+    may be absent: P2 / bn2 None).  Needs no GPU."""
+    from .denoiser import BN_STATE, param_count
+    n = param_count(channels, size)
+    out = {}
+    with T7File(path) as f:
+        for key, pk, bk in (("AE1_DECODER", "P1", "bn1"), ("AE2_DECODER", "P2", "bn2")):
+            if f.kind(key) is None:
+                if key == "AE1_DECODER":
+                    raise FGError("%s holds no AE1_DECODER" % path)
+                out[pk] = out[bk] = None
+                continue
+            p = f.net_params(key)
+            if p.size != n:
+                raise FGError("checkpoint %s has %d parameters (%s); the %dx%dx%d denoiser has %d"
+                              % (key, p.size, f.net_describe(key), channels, size, size, n))
+            bn = f.net_bn_state(key)
+            if bn.size != BN_STATE:
+                raise FGError("checkpoint %s carries %d BatchNorm running statistics, expected %d (8 + 8 + 2048 channels)"
+                              % (key, bn.size, BN_STATE))
+            out[pk], out[bk] = p, bn
+    return out
+
+
+def load_denoiser_checkpoint(dn, path):
+    """train.lua --denoise (:101-110): load `denoiser_CxHxW.net` into a Denoiser (both decoders when present)."""
+    ck = read_denoiser_checkpoint(path, dn.C, dn.S)
+    for net, pk, bk in ((0, "P1", "bn1"), (1, "P2", "bn2")):
+        if ck[pk] is not None:
+            dn.set_params(net, ck[pk])
+            dn.set_bn_state(net, ck[bk])
+    return ck

@@ -506,8 +506,13 @@ int pair_get_bn_state(fg_ctx* c, const NetPair& p, float* dst);
 // Runs `body` (launches on c->stream that read their seed from c->seed_dev) as a train step of pair p: eagerly, or as a
 // captured CUDA graph keyed on B, *h, `inputs`, the stream, the communicator, graph_epoch, pack_key and the iteration
 // counts nd / ng
-int net_graph_run(fg_ctx* c, NetPair& p, int B, const fg_hyper* h, std::initializer_list<const void*> inputs, uint64_t seed,
-                  const std::function<int()>& body, bool allow_graph, int nd = 1, int ng = 1);
+// (hyper, hyper_bytes): the hyper-parameter struct of the step, keyed by its bytes
+int net_graph_run(fg_ctx* c, NetPair& p, int B, const void* hyper, size_t hyper_bytes, std::initializer_list<const void*> inputs,
+                  uint64_t seed, const std::function<int()>& body, bool allow_graph, int nd = 1, int ng = 1);
+inline int net_graph_run(fg_ctx* c, NetPair& p, int B, const fg_hyper* h, std::initializer_list<const void*> inputs, uint64_t seed,
+                         const std::function<int()>& body, bool allow_graph, int nd = 1, int ng = 1) {
+  return net_graph_run(c, p, B, h, sizeof(*h), inputs, seed, body, allow_graph, nd, ng);
+}
 
 // ---- capi.cu: host or device pointers at the C ABI ----
 bool fg_is_dev(const void* p);

@@ -235,8 +235,8 @@ void key_add(std::vector<uint8_t>& k, const T& v) {
 
 // The packs are marked stale before the capture and after every replay: the captured sequence has to contain the pack
 // kernels whatever the flags said at capture time, and a replayed optimizer step invalidates them again.
-int net_graph_run(fg_ctx* c, NetPair& p, int B, const fg_hyper* h, std::initializer_list<const void*> inputs, uint64_t seed,
-                  const std::function<int()>& body, bool allow_graph, int nd, int ng) {
+int net_graph_run(fg_ctx* c, NetPair& p, int B, const void* hyper, size_t hyper_bytes, std::initializer_list<const void*> inputs,
+                  uint64_t seed, const std::function<int()>& body, bool allow_graph, int nd, int ng) {
   FG_TRY(k_set_u64(c, c->seed_dev, seed));
   static const bool env_off = getenv("FG_GRAPH") && atoi(getenv("FG_GRAPH")) == 0;
   if (!allow_graph || !c->use_graph || env_off || c->timing || c->debug_keep) return body();
@@ -246,7 +246,8 @@ int net_graph_run(fg_ctx* c, NetPair& p, int B, const fg_hyper* h, std::initiali
   key_add(key, nd);
   key_add(key, ng);
   key_add(key, pack_key(c));
-  key_add(key, *h);
+  const uint8_t* hb = static_cast<const uint8_t*>(hyper);
+  key.insert(key.end(), hb, hb + hyper_bytes);
   for (const void* q : inputs) key_add(key, q);
   key_add(key, (const void*)c->stream);
   key_add(key, c->nccl_comm);

@@ -32,6 +32,15 @@ class StepStats(C.Structure):
                 ("t_D", C.c_int32), ("t_G", C.c_int32), ("acc_D", C.c_float)]
 
 
+class DnHyper(C.Structure):
+    _fields_ = [("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float), ("L1", C.c_float),
+                ("L2", C.c_float), ("clamp", C.c_float), ("p_drop", C.c_float), ("noise_std", C.c_float)]
+
+
+class DnStats(C.Structure):
+    _fields_ = [("loss_AE1", C.c_float), ("loss_AE2", C.c_float), ("t", C.c_int32)]
+
+
 # every symbol include/fg_b200.h declares: name -> (restype, argtypes)
 _P, _F, _I, _L, _U64, _SZ = C.c_void_p, C.c_float, C.c_int, C.c_int64, C.c_uint64, C.c_size_t
 SYMBOLS = {
@@ -188,6 +197,24 @@ SYMBOLS = {
     "fg_train_step_dataset_iters": (_I, [_P, _P, C.POINTER(Hyper), _I, _I, _I, _U64, C.POINTER(StepStats)]),
     "fg_s16_train_step_dataset_iters": (_I, [_P, _P, C.POINTER(Hyper), _I, _I, _I, _U64, C.POINTER(StepStats)]),
     "fg_c2f_train_step_dataset_iters": (_I, [_P, _P, C.POINTER(Hyper), _I, _I, _I, _I, _U64, C.POINTER(StepStats)]),
+    "fg_dn_hyper_default": (None, [C.POINTER(DnHyper)]),
+    "fg_dn_create": (_I, [_P, _I, C.POINTER(_P)]),
+    "fg_dn_destroy": (_I, [_P]),
+    "fg_dn_param_count": (_L, [_I, _I]),
+    "fg_dn_mask_per_sample": (_I, [_I]),
+    "fg_dn_set_params": (_I, [_P, _I, _P]),
+    "fg_dn_get_params": (_I, [_P, _I, _P]),
+    "fg_dn_get_grads": (_I, [_P, _I, _P]),
+    "fg_dn_zero_grads": (_I, [_P, _I]),
+    "fg_dn_set_bn_state": (_I, [_P, _I, _P]),
+    "fg_dn_get_bn_state": (_I, [_P, _I, _P]),
+    "fg_dn_set_adam_state": (_I, [_P, _P, _P, _I]),
+    "fg_dn_get_adam_state": (_I, [_P, _P, _P, C.POINTER(_I)]),
+    "fg_dn_forward": (_I, [_P, _I, _P, _I, _I, _P, _P, _U64, _P]),
+    "fg_dn_backward": (_I, [_P, _I, _P]),
+    "fg_dn_train_step": (_I, [_P, C.POINTER(DnHyper), _I, _P, _P, _P, _U64, C.POINTER(DnStats)]),
+    "fg_dn_denoise": (_I, [_P, _P, _I, _I, _P]),
+    "fg_dn_debug_tensor": (_L, [_P, C.c_char_p, _P, _L]),
 }
 
 MAX_ITERS = 16  # the most D or G iterations one call runs (fg_train_step_iters)

@@ -463,4 +463,52 @@ function Sg:updateGradInput(input, gradOutput)
   return self.gradInput
 end
 
+-- train.lua --denoise (:101-110): DENOISER = AE1_DECODER:evaluate(), applied to G's images in
+-- NN_UTILS.visualizeProgress (nn_utils.lua:144-155).  b200.Denoiser(IMG_DIMENSIONS, file, OPT.gpu, OPT.batchSize)
+-- loads `denoiser_CxHxW.net` (AE1_DECODER's flat parameters and BatchNorm running statistics, read by the library's
+-- Torch7 reader) and forwards through fg_dn_denoise; :training() switches to the training-mode forward (WhiteNoise,
+-- batch statistics, drawn dropout).  It is built before the GAN's shims, so it creates the process's context: pass the
+-- device and batch size the GAN will use (b200.context keeps the first context it creates).
+local Denoiser, dparent = torch.class('b200.Denoiser', 'nn.Module')
+function Denoiser:__init(dimensions, filename, device, maxBatch)
+  dparent.__init(self)
+  self.ctx = b200.context(device or 0, maxBatch or 256, dimensions[1])
+  self.maxBatch = tonumber(C.fg_get_option(self.ctx, 'max_batch'))  -- the context's, whoever created it
+  self.C, self.S, self.train, self.seed = dimensions[1], dimensions[2], false, 0
+  local out = ffi.new('fg_dn*[1]')
+  F.check(C.fg_dn_create(self.ctx, self.S, out), 'fg_dn_create')
+  self.dn = ffi.gc(out[0], C.fg_dn_destroy)
+  if filename then self:load(filename) end
+  self.output = torch.FloatTensor()
+end
+function Denoiser:load(filename)
+  local f = ffi.new('fg_t7*[1]')
+  F.check(C.fg_t7_open(filename, f), 'fg_t7_open')
+  local n = tonumber(C.fg_dn_param_count(self.C, self.S))
+  local p, bn = torch.FloatTensor(n), torch.FloatTensor(2 * (8 + 8 + 2048))
+  local got = C.fg_t7_net_params(f[0], 'AE1_DECODER', F.ptr(p), n)
+  local gotbn = C.fg_t7_net_bn_state(f[0], 'AE1_DECODER', F.ptr(bn), bn:nElement())
+  C.fg_t7_close(f[0])
+  assert(tonumber(got) == n, 'b200.Denoiser: AE1_DECODER does not match the denoiser at this image size')
+  assert(tonumber(gotbn) == bn:nElement(), 'b200.Denoiser: AE1_DECODER lacks its BatchNorm running statistics')
+  F.check(C.fg_dn_set_params(self.dn, 0, F.ptr(p)), 'fg_dn_set_params')
+  F.check(C.fg_dn_set_bn_state(self.dn, 0, F.ptr(bn)), 'fg_dn_set_bn_state')
+end
+function Denoiser:training() self.train = true; return self end
+function Denoiser:evaluate() self.train = false; return self end
+function Denoiser:type() return self end
+function Denoiser:float() return self end
+function Denoiser:updateOutput(input)
+  input = input:float():contiguous()
+  local B = input:size(1)
+  self.output:resize(B, self.C, self.S, self.S)
+  if self.train then
+    self.seed = self.seed + 1
+    F.check(C.fg_dn_forward(self.dn, 0, F.ptr(input), B, 1, nil, nil, self.seed, F.ptr(self.output)), 'fg_dn_forward')
+  else
+    F.check(C.fg_dn_denoise(self.dn, F.ptr(input), B, math.min(B, self.maxBatch), F.ptr(self.output)), 'fg_dn_denoise')
+  end
+  return self.output
+end
+
 return b200

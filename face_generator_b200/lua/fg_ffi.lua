@@ -189,6 +189,29 @@ int fg_event_record(fg_ctx* ctx, int slot);
 int fg_event_elapsed_ms(fg_ctx* ctx, int slot_a, int slot_b, double* ms);
 int fg_timing_enable(fg_ctx* ctx, int on);
 int fg_timing_get(fg_ctx* ctx, const char* name, double* ms_total, int64_t* launches);
+typedef struct fg_dn fg_dn;
+typedef struct fg_dn_hyper { float lr, beta1, beta2, eps; float L1, L2; float clamp; float p_drop; float noise_std; } fg_dn_hyper;
+typedef struct fg_dn_stats { float loss_AE1, loss_AE2; int32_t t; } fg_dn_stats;
+void fg_dn_hyper_default(fg_dn_hyper* h);
+int fg_dn_create(fg_ctx* ctx, int size, fg_dn** out);
+int fg_dn_destroy(fg_dn* n);
+int64_t fg_dn_param_count(int channels, int size);
+int fg_dn_mask_per_sample(int size);
+int fg_dn_set_params(fg_dn* n, int net, const float* src);
+int fg_dn_get_params(fg_dn* n, int net, float* dst);
+int fg_dn_get_grads(fg_dn* n, int net, float* dst);
+int fg_dn_zero_grads(fg_dn* n, int net);
+int fg_dn_set_bn_state(fg_dn* n, int net, const float* src);
+int fg_dn_get_bn_state(fg_dn* n, int net, float* dst);
+int fg_dn_set_adam_state(fg_dn* n, const float* m, const float* v, int t);
+int fg_dn_get_adam_state(fg_dn* n, float* m, float* v, int* t);
+int fg_dn_forward(fg_dn* n, int net, const float* x, int B, int training, const float* noise, const float* masks,
+                  uint64_t seed, float* out);
+int fg_dn_backward(fg_dn* n, int net, const float* dout);
+int fg_dn_train_step(fg_dn* n, const fg_dn_hyper* h, int B, const float* images, const float* noise, const float* masks,
+                     uint64_t seed, fg_dn_stats* stats);
+int fg_dn_denoise(fg_dn* n, const float* images, int N, int chunk, float* out);
+int64_t fg_dn_debug_tensor(fg_dn* n, const char* name, float* dst, int64_t max_elems);
 ]]
 
 local M = {}

@@ -393,6 +393,64 @@ int fg_dataset_nearest(fg_dataset* d, const float* queries, int Q, int32_t* idx_
  * noise [K][1][S][S], coarse / fine [C][S][S]                                                       */
 int fg_c2f_parzen_dist(fg_c2f* n, const float* noise, const float* coarse, const float* fine, int K, float* dist_out);
 
+/* ---- the denoising autoencoders of train_denoiser.lua (train.lua --denoise) ------------------ */
+/* AE = WhiteNoise(0, noise_std) + DECODER, AE2 = a second DECODER fed with AE's output
+ * (train_denoiser.lua:83-117), images [B][C][S][S] with S = 16 or 32 and C = the ctx's channels.
+ * DECODER = conv(C,8,3) SpatialBN LeakyReLU(0.333) conv(8,8,3) SpatialBN LeakyReLU Dropout(p)
+ *           Linear(8(S-4)^2, 2048) BN LeakyReLU Dropout(p) Linear(2048, C S S) Sigmoid (no padding).
+ * `net` is 0 for AE1's decoder (AE1_DECODER), 1 for AE2's (AE2_DECODER).  Single GPU only: a data-
+ * parallel ctx gets FG_ERR_UNSUPPORTED.  Batches run from 2 (1 in evaluation) up to max_batch.     */
+typedef struct fg_dn fg_dn;
+typedef struct fg_dn_hyper {
+  float lr, beta1, beta2, eps;  /* optim.adam: 1e-3, 0.9, 0.999, 1e-8 (OPTSTATE.adam = {})          */
+  float L1, L2;                 /* --coefL1 / --coefL2: 0, 0 (loss, then grad += L1 sign(P) + L2 P)   */
+  float clamp;                  /* --AE_clamp: 1 (gradients clamped to +-clamp; 0 = off)             */
+  float p_drop;                 /* Dropout(0.2) of both dropout layers                                */
+  float noise_std;              /* WhiteNoise(0, 0.1)                                                 */
+} fg_dn_hyper;
+typedef struct fg_dn_stats {
+  float loss_AE1, loss_AE2;     /* BCE of the AE step and of the AE2 step (no penalty terms)          */
+  int32_t t;                    /* the shared Adam step counter: 2 per batch                          */
+} fg_dn_stats;
+void fg_dn_hyper_default(fg_dn_hyper* h);
+int fg_dn_create(fg_ctx* ctx, int size, fg_dn** out);     /* size 16 or 32, else FG_ERR_UNSUPPORTED */
+int fg_dn_destroy(fg_dn* n);
+int64_t fg_dn_param_count(int channels, int size);        /* one decoder; -1 for an unsupported shape */
+/* dropout keep flags per sample: 8(S-4)^2 of the conv block ([8][S-4][S-4] order), then 2048       */
+int fg_dn_mask_per_sample(int size);
+int fg_dn_set_params(fg_dn* n, int net, const float* src); /* getParameters() order of one decoder   */
+int fg_dn_get_params(fg_dn* n, int net, float* dst);
+int fg_dn_get_grads(fg_dn* n, int net, float* dst);
+int fg_dn_zero_grads(fg_dn* n, int net);
+/* running statistics of one decoder's three BatchNorm layers: [mean1 8][var1 8][mean2 8][var2 8]
+ * [mean3 2048][var3 2048] (4128 floats, the fg_t7_net_bn_state order)                             */
+int fg_dn_set_bn_state(fg_dn* n, int net, const float* src);
+int fg_dn_get_bn_state(fg_dn* n, int net, float* dst);
+/* the ONE Adam state both updates of a batch use (m, v: fg_dn_param_count floats; t)              */
+int fg_dn_set_adam_state(fg_dn* n, const float* m, const float* v, int t);
+int fg_dn_get_adam_state(fg_dn* n, float* m, float* v, int* t);
+/* forward of one decoder (net 0 with its WhiteNoise): x, out [B][C][S][S].  training != 0: batch
+ * statistics (running statistics updated), noise [B][C][S][S] (net 0 only) and keep flags masks
+ * [B][mps], each drawn from `seed` when NULL; 0: evaluate().  backward: dout = dL/d(out) of the last
+ * forward of that decoder; its parameter gradients are ACCUMULATED (fg_dn_zero_grads).  A train step
+ * leaves no forward to differentiate: call fg_dn_forward first (else FG_ERR_INVALID).              */
+int fg_dn_forward(fg_dn* n, int net, const float* x, int B, int training, const float* noise, const float* masks,
+                  uint64_t seed, float* out);
+int fg_dn_backward(fg_dn* n, int net, const float* dout);
+/* the per-batch body of train_denoiser.lua:247-341: fevalAE + adam, then fevalAE2 (AE forward again:
+ * fresh noise and masks, AE's updated parameters, running statistics updated) + adam, on ONE Adam
+ * state.  images [B][C][S][S] are inputs and targets; noise [2][B][C][S][S] (AE step, AE in the AE2
+ * step) and masks [3][B][mps] (the same two, then AE2) may each be NULL: drawn from `seed`, streams
+ * (8 seed + k) for noise k and (8 seed + 2 + k) for masks k.  Replays a captured CUDA graph.       */
+int fg_dn_train_step(fg_dn* n, const fg_dn_hyper* h, int B, const float* images, const float* noise, const float* masks,
+                     uint64_t seed, fg_dn_stats* stats);
+/* train.lua --denoise: AE1_DECODER:evaluate():forward(images) for N images, `chunk` at a time       */
+int fg_dn_denoise(fg_dn* n, const float* images, int N, int chunk, float* out);
+/* the fg_*debug_tensor contract: what the last forwards drew, "noise0", "noise1" (NCHW), "masks0".."masks2";
+ * each decoder's last forward "AE1.*" / "AE2.*": x z1 h1 z2 h2 z3 h3 z4 y (NHWC) and mean1..3 istd1..3; the
+ * last backward's gradients dz4 dh3 dz3 dh2 dz2 dh1 dz1 (NHWC)                                      */
+int64_t fg_dn_debug_tensor(fg_dn* n, const char* name, float* dst, int64_t max_elems);
+
 /* ---- Torch7 checkpoint files (host only, no GPU needed) --------------------------------------- */
 /* Reads the binary torch.save format of the reference's checkpoints -- torch.save(filename,
  * {D=MODEL_D, G=MODEL_G, opt=OPT, epoch=EPOCH}) at adversarial.lua:328 / adversarial_c2f.lua:216,
