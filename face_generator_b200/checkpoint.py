@@ -212,3 +212,52 @@ def load_denoiser_checkpoint(dn, path):
             dn.set_params(net, ck[pk])
             dn.set_bn_state(net, ck[bk])
     return ck
+
+
+def read_autoencoder_checkpoint(path, size, noise_dim):
+    """train_autoencoder.lua's `autoencoder.net` ({AE = MODEL_AE, optstate = OPTSTATE}, :234): MODEL_AE's parameters in
+    getParameters() order.  The script's Adam state is per-parameter-tensor tables inside optstate and is not read:
+    training resumes with fresh moments, as the script itself does after a restart.  Needs no GPU."""
+    from .autoencoder import param_count
+    n = param_count(size, noise_dim)
+    with T7File(path) as f:
+        if f.kind("AE") is None:
+            raise FGError("%s holds no AE" % path)
+        p = f.net_params("AE")
+        if p.size != n:
+            raise FGError("checkpoint AE has %d parameters (%s); the %dx%d autoencoder with noiseDim %d has %d"
+                          % (p.size, f.net_describe("AE"), size, size, noise_dim, n))
+        return p
+
+
+def load_autoencoder_checkpoint(ae, path):
+    """load the AE of an `autoencoder.net` into an Autoencoder of the same --scale and --noiseDim"""
+    p = read_autoencoder_checkpoint(path, ae.S, ae.d)
+    ae.set_params(p)
+    return p
+
+
+def save_autoencoder_flat(ae, path, epoch=0):
+    """Everything needed to resume an Autoencoder: parameters, Adam moments and step counter, as flat tensors in one root
+    table that stock torch.load reads."""
+    w = T7Writer(path)
+    w.add("AE", ae.get_params())
+    m, v, t = ae.get_adam_state()
+    w.add("adam_m", m)
+    w.add("adam_v", v)
+    w.add("adam_t", t)
+    w.add("scale", ae.S)
+    w.add("noiseDim", ae.d)
+    w.add("epoch", epoch)
+    w.add("format", "fg_b200 flat checkpoint: getParameters()-ordered vector of train_autoencoder.lua's MODEL_AE")
+    w.close()
+
+
+def load_autoencoder_flat(ae, path):
+    with T7File(path) as f:
+        if int(f.number("scale")) != ae.S or int(f.number("noiseDim")) != ae.d:
+            raise FGError("%s was saved at scale %d, noiseDim %d; this autoencoder has %d, %d"
+                          % (path, f.number("scale"), f.number("noiseDim"), ae.S, ae.d))
+        ae.set_params(f.tensor("AE"))
+        ae.set_adam_state(f.tensor("adam_m"), f.tensor("adam_v"), int(f.number("adam_t")))
+        return int(f.number("epoch"))

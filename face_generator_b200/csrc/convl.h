@@ -23,6 +23,14 @@ struct AmaxInto {
   ~AmaxInto() { c->amax_out = nullptr; }
 };
 
+// host side of a producer's launch: the word it reduces max|output| into (amax_commit, k_f16split.cuh), or null; says
+// so in *c->amax_done
+inline unsigned* take_amax(fg_ctx* c) {
+  unsigned* p = c->amax_out;
+  if (p) *c->amax_done = true;
+  return p;
+}
+
 // the split of x (n elements) into op, in the format `f16` chooses, minus whatever the producer already did
 int tc_op_split(fg_ctx* c, TcOp& op, const float* x, int64_t n, bool f16);
 

@@ -494,6 +494,9 @@ int pair_allreduce_grads(fg_ctx* c, NetPair& p, int net);  // gradient + tail (o
 // the accuracy gate (D), t += 1 and the step size of `net` on the pair's own statistics
 int pair_gate(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, int B, float world, bool accumulate = false);
 int pair_optim(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, float grad_scale);  // penalty -> clamp -> update
+// stock optim.adam without a gate: *t_dev += 1, *step_dev = lr sqrt(1 - beta2^t) / (1 - beta1^t) in double, for the
+// k_optim_update that follows
+int k_adam_prep(fg_ctx* c, int* t_dev, float* step_dev, float lr, float beta1, float beta2);
 int pair_broadcast(fg_ctx* c, NetPair& p);  // rank 0's parameters, moments, BatchNorm state, statistics, history
 int pair_step_stats(fg_ctx* c, const NetPair& p, fg_step_stats* stats);  // synchronise, then the last step's statistics
 int pair_set_params(fg_ctx* c, NetPair& p, int net, const float* src);
@@ -513,6 +516,19 @@ inline int net_graph_run(fg_ctx* c, NetPair& p, int B, const fg_hyper* h, std::i
                          const std::function<int()>& body, bool allow_graph, int nd = 1, int ng = 1) {
   return net_graph_run(c, p, B, h, sizeof(*h), inputs, seed, body, allow_graph, nd, ng);
 }
+
+// ---- nets_ae.cu: the elementwise layers of the autoencoder (nn.ReLU, nn.Tanh + nn.Dropout, nn.AbsCriterion).  Each is
+// a producer in AmaxInto's sense (convl.h). ----
+int k_relu_fwd(fg_ctx* c, const float* z, float* h, int64_t n);
+int k_relu_bwd(fg_ctx* c, const float* dh, const float* z, float* dz, int64_t n);  // dz = dh [z > 0]
+// code = tanh(z), h (may be null) = Dropout(code): keep flags given (masks_in), drawn with probability 1 - p from
+// *seed_dev, or none (both null: h = code); flags_out (may be null) receives the flags used
+int k_tanh_dropout_fwd(fg_ctx* c, const float* z, const float* masks_in, const uint64_t* seed_dev, float p, float* code, float* h,
+                       float* flags_out, int64_t n);
+int k_tanh_dropout_bwd(fg_ctx* c, const float* dh, const float* masks, float p, const float* code, float* dz, int64_t n);
+// mean |y - t| -> *loss and its gradient -> dz, with y = sigmoid(z) (also stored) and dz taken through Sigmoid.backward
+// when `sigmoid`, else y = z; y, dz and loss may each be null
+int k_abs_criterion(fg_ctx* c, bool sigmoid, const float* z, const float* t, float* y, float* dz, int64_t n, float* loss);
 
 // ---- capi.cu: host or device pointers at the C ABI ----
 bool fg_is_dev(const void* p);

@@ -27,3 +27,22 @@ __device__ __forceinline__ float scale_for_amax(float amax) {
   const int e = max(-100, min(100, 15 - ex));
   return ldexpf(1.f, e);
 }
+
+// max|output| over the finite outputs of an elementwise producer (finite_abs) into a device word (option mma_f16: the
+// power-of-two scale of the FP16 split is derived from it, k_conv_tc.cu).  Non-negative floats order like their bit
+// patterns, so atomicMax on the bits is exact and order-independent (replicas stay identical).  Must be reached by all
+// 32 lanes.
+__device__ __forceinline__ void amax_commit(unsigned* amax, float m) {
+  if (!amax) return;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  // thousands of warps hit ONE word: an atomic per warp serialises at the L2 (measured 100+ us on the pooling kernels).
+  // A plain load first: only a warp that would actually raise the maximum issues the atomic (a handful per launch).
+  if ((threadIdx.x & 31) == 0 && m > 0.f) {
+    const unsigned bits = __float_as_uint(m);
+    if (bits > *reinterpret_cast<volatile unsigned*>(amax)) atomicMax(amax, bits);
+  }
+}
+__device__ __forceinline__ float amax4(float m, float a, float b, float c, float d) {
+  return fmaxf(fmaxf(m, fmaxf(finite_abs(a), finite_abs(b))), fmaxf(finite_abs(c), finite_abs(d)));
+}

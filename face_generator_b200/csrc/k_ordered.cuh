@@ -26,3 +26,15 @@ __device__ __forceinline__ double ordered_sum(const double* ws, int rows, int64_
 __device__ __forceinline__ void ordered_release(unsigned* ticket) {
   if (threadIdx.x == 0 && threadIdx.y == 0 && threadIdx.z == 0) *ticket = 0;
 }
+// sum over a block of 256 threads in a fixed order (lanes, then warps); valid in thread 0
+__device__ __forceinline__ double block_sum256(double v) {
+  __shared__ double red[8];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < 8; ++w) s += red[w];
+  return s;
+}

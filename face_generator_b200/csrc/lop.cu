@@ -458,4 +458,71 @@ int fg_sigmoid_backward(fg_ctx* c, const float* y, const float* dy, float* dx, i
   return out_done(c, dx, dxd, n);
 }
 
+
+// nn.ReLU, nn.Tanh and nn.AbsCriterion (the layers of train_autoencoder.lua's net), flat tensors of n floats
+int fg_relu_forward(fg_ctx* c, const float* x, float* y, int64_t n) {
+  ENTER(c);
+  FG_REQUIRE(x && y && n > 0, "fg_relu_forward: bad arguments");
+  const float* xd;
+  float* yd;
+  FG_TRY(in_dev(c, x, n, 0, &xd));
+  FG_TRY(out_dev(c, y, n, 6, &yd, false));
+  FG_TRY(k_relu_fwd(c, xd, yd, n));
+  return out_done(c, y, yd, n);
+}
+int fg_relu_backward(fg_ctx* c, const float* x, const float* dy, float* dx, int64_t n) {
+  ENTER(c);
+  FG_REQUIRE(x && dy && dx && n > 0, "fg_relu_backward: bad arguments");
+  const float *xd, *dyd;
+  float* dxd;
+  FG_TRY(in_dev(c, x, n, 0, &xd));
+  FG_TRY(in_dev(c, dy, n, 1, &dyd));
+  FG_TRY(out_dev(c, dx, n, 6, &dxd, false));
+  FG_TRY(k_relu_bwd(c, dyd, xd, dxd, n));
+  return out_done(c, dx, dxd, n);
+}
+int fg_tanh_forward(fg_ctx* c, const float* x, float* y, int64_t n) {
+  ENTER(c);
+  FG_REQUIRE(x && y && n > 0, "fg_tanh_forward: bad arguments");
+  const float* xd;
+  float* yd;
+  FG_TRY(in_dev(c, x, n, 0, &xd));
+  FG_TRY(out_dev(c, y, n, 6, &yd, false));
+  FG_TRY(k_tanh_dropout_fwd(c, xd, nullptr, nullptr, 0.f, yd, nullptr, nullptr, n));
+  return out_done(c, y, yd, n);
+}
+int fg_tanh_backward(fg_ctx* c, const float* y, const float* dy, float* dx, int64_t n) {
+  ENTER(c);
+  FG_REQUIRE(y && dy && dx && n > 0, "fg_tanh_backward: bad arguments");
+  const float *yd, *dyd;
+  float* dxd;
+  FG_TRY(in_dev(c, y, n, 0, &yd));
+  FG_TRY(in_dev(c, dy, n, 1, &dyd));
+  FG_TRY(out_dev(c, dx, n, 6, &dxd, false));
+  FG_TRY(k_tanh_dropout_bwd(c, dyd, nullptr, 0.f, yd, dxd, n));
+  return out_done(c, dx, dxd, n);
+}
+int fg_abs_forward(fg_ctx* c, const float* x, const float* t, int64_t n, float* loss_out) {
+  ENTER(c);
+  FG_REQUIRE(x && t && loss_out && n > 0, "fg_abs_forward: bad arguments");
+  const float *xd, *td;
+  float* ld;
+  FG_TRY(in_dev(c, x, n, 0, &xd));
+  FG_TRY(in_dev(c, t, n, 1, &td));
+  FG_TRY(out_dev(c, loss_out, 1, 6, &ld, false));
+  FG_TRY(k_abs_criterion(c, false, xd, td, nullptr, nullptr, n, ld));
+  return out_done(c, loss_out, ld, 1);
+}
+int fg_abs_backward(fg_ctx* c, const float* x, const float* t, int64_t n, float* dx) {
+  ENTER(c);
+  FG_REQUIRE(x && t && dx && n > 0, "fg_abs_backward: bad arguments");
+  const float *xd, *td;
+  float* dxd;
+  FG_TRY(in_dev(c, x, n, 0, &xd));
+  FG_TRY(in_dev(c, t, n, 1, &td));
+  FG_TRY(out_dev(c, dx, n, 6, &dxd, false));
+  FG_TRY(k_abs_criterion(c, false, xd, td, nullptr, dxd, n, nullptr));
+  return out_done(c, dx, dxd, n);
+}
+
 }  // extern "C"

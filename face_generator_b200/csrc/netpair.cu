@@ -123,6 +123,19 @@ int iters_check(int nd, int ng, const char* what) {
   return FG_OK;
 }
 
+namespace {
+__global__ void adam_prep_kernel(int* t_dev, float* step_dev, float lr, float beta1, float beta2) {
+  const int t = *t_dev + 1;
+  *t_dev = t;
+  *step_dev = (float)((double)lr * sqrt(1.0 - pow((double)beta2, (double)t)) / (1.0 - pow((double)beta1, (double)t)));
+}
+}  // namespace
+int k_adam_prep(fg_ctx* c, int* t_dev, float* step_dev, float lr, float beta1, float beta2) {
+  adam_prep_kernel<<<1, 1, 0, c->stream>>>(t_dev, step_dev, lr, beta1, beta2);
+  LAUNCH_CHECK(c);
+  return FG_OK;
+}
+
 // penalty -> clamp -> interruptable optimizer on the flat vectors (adversarial.lua:219-231, interruptable_optimizers.lua)
 int pair_optim(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, float grad_scale) {
   const bool isD = net == FG_NET_D;

@@ -17,6 +17,7 @@
 #include "convl.h"
 #include "fg_internal.h"
 #include "k_ordered.cuh"
+#include "k_stream.cuh"
 
 namespace {
 constexpr float kSlope = 0.333f;
@@ -25,16 +26,6 @@ constexpr int kBnDn = 2 * (8 + 8 + kHidden);  // [rm1 8][rv1 8][rm2 8][rv2 8][rm
 // random streams of a step (stream root = the step seed, *seed_dev): WhiteNoise of forward k (0: the AE step, 1: AE's
 // forward inside the AE2 step) and the dropout keep flags of forward k (0, 1: AE; 2: AE2)
 constexpr uint64_t kKindNoise = 0, kKindMask = 2;
-
-__device__ __forceinline__ uint64_t mix64(uint64_t x) {
-  x += 0x9E3779B97F4A7C15ull;
-  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-  return x ^ (x >> 31);
-}
-__device__ __forceinline__ uint64_t stream_bits(uint64_t root, uint64_t kind, int64_t i) {
-  return mix64((root * 8 + kind) * 0x100000001B3ull + (uint64_t)i);
-}
 
 // images NCHW -> x NHWC (+ WhiteNoise).  noise (NCHW, may be null) is added as given; else with seed_dev it is drawn:
 // std * N(0,1) by Box-Muller on the stream (seed, kind); noise_out (may be null) receives what was added.
@@ -311,17 +302,6 @@ __global__ void dn_bn_bwd_apply_kernel(const float* __restrict__ dh, const float
 }
 
 // ---- nn.Sigmoid + nn.BCECriterion against image targets: y, dlogit and the mean loss in one pass ----
-__device__ __forceinline__ double block_sum256(double v) {
-  __shared__ double red[8];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0;
-  if (threadIdx.x == 0)
-    for (int w = 0; w < 8; ++w) s += red[w];
-  return s;
-}
 // the 2015 Lua BCECriterion (eps = 1e-12, size-averaged), composed with Sigmoid.backward as k_sigmoid_bce does
 __global__ void __launch_bounds__(256) dn_sigmoid_bce_kernel(const float* __restrict__ z, const float* __restrict__ t,
                                                              float* __restrict__ y, float* __restrict__ dz, int64_t n,
@@ -346,14 +326,8 @@ __global__ void __launch_bounds__(256) dn_sigmoid_bce_kernel(const float* __rest
 struct DnStats {  // device; mirrored to fg_dn_stats
   float loss[2];
   int t;
-  float step;  // the Adam step size of the update that follows (dn_adam_prep_kernel)
+  float step;  // the Adam step size of the update that follows (k_adam_prep)
 };
-// optim.adam: t += 1, stepSize = lr sqrt(1 - beta2^t) / (1 - beta1^t) in double
-__global__ void dn_adam_prep_kernel(DnStats* st, float lr, float beta1, float beta2) {
-  const int t = st->t + 1;
-  st->t = t;
-  st->step = (float)((double)lr * sqrt(1.0 - pow((double)beta2, (double)t)) / (1.0 - pow((double)beta1, (double)t)));
-}
 }  // namespace
 
 // One decoder: its layers, activations (NHWC) and BatchNorm state
@@ -656,8 +630,7 @@ int sigmoid_bce(fg_dn* n, int net, int B, float* loss) {
 // penalty -> clamp -> Adam on the shared state (fevalAE / fevalAE2 + optim.adam, train_denoiser.lua:278-291, :335)
 int dn_optim(fg_dn* n, int net, const fg_dn_hyper* h) {
   fg_ctx* c = n->c;
-  dn_adam_prep_kernel<<<1, 1, 0, c->stream>>>(n->dstats, h->lr, h->beta1, h->beta2);
-  LAUNCH_CHECK(c);
+  FG_TRY(k_adam_prep(c, &n->dstats->t, &n->dstats->step, h->lr, h->beta1, h->beta2));
   NetPair& p = n->net;
   FG_TRY(k_optim_update(c, FG_OPT_ADAM, net ? p.PD : p.PG, grads(n, net), p.mG, p.vG, p.nG, h->beta1, h->beta2, h->eps, 0.f,
                         h->L1, h->L2, h->clamp, 1.0f, &n->dstats->step, nullptr, &n->dstats->t));

@@ -41,6 +41,15 @@ class DnStats(C.Structure):
     _fields_ = [("loss_AE1", C.c_float), ("loss_AE2", C.c_float), ("t", C.c_int32)]
 
 
+class AeHyper(C.Structure):
+    _fields_ = [("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float), ("L1", C.c_float),
+                ("L2", C.c_float), ("p_drop", C.c_float)]
+
+
+class AeStats(C.Structure):
+    _fields_ = [("loss", C.c_float), ("t", C.c_int32)]
+
+
 # every symbol include/fg_b200.h declares: name -> (restype, argtypes)
 _P, _F, _I, _L, _U64, _SZ = C.c_void_p, C.c_float, C.c_int, C.c_int64, C.c_uint64, C.c_size_t
 SYMBOLS = {
@@ -215,6 +224,28 @@ SYMBOLS = {
     "fg_dn_train_step": (_I, [_P, C.POINTER(DnHyper), _I, _P, _P, _P, _U64, C.POINTER(DnStats)]),
     "fg_dn_denoise": (_I, [_P, _P, _I, _I, _P]),
     "fg_dn_debug_tensor": (_L, [_P, C.c_char_p, _P, _L]),
+    "fg_ae_hyper_default": (None, [C.POINTER(AeHyper)]),
+    "fg_ae_create": (_I, [_P, _I, _I, C.POINTER(_P)]),
+    "fg_ae_destroy": (_I, [_P]),
+    "fg_ae_param_count": (_L, [_I, _I]),
+    "fg_ae_set_params": (_I, [_P, _P]),
+    "fg_ae_get_params": (_I, [_P, _P]),
+    "fg_ae_get_grads": (_I, [_P, _P]),
+    "fg_ae_zero_grads": (_I, [_P]),
+    "fg_ae_set_adam_state": (_I, [_P, _P, _P, _I]),
+    "fg_ae_get_adam_state": (_I, [_P, _P, _P, C.POINTER(_I)]),
+    "fg_ae_forward": (_I, [_P, _P, _I, _I, _P, _U64, _P, _P]),
+    "fg_ae_backward": (_I, [_P, _P]),
+    "fg_ae_train_step": (_I, [_P, C.POINTER(AeHyper), _I, _P, _P, _U64, C.POINTER(AeStats)]),
+    "fg_ae_train_step_dataset": (_I, [_P, _P, C.POINTER(AeHyper), _P, _I, _U64, C.POINTER(AeStats)]),
+    "fg_ae_reconstruct": (_I, [_P, _P, _L, _I, _I, _U64, _P]),
+    "fg_ae_debug_tensor": (_L, [_P, C.c_char_p, _P, _L]),
+    "fg_relu_forward": (_I, [_P, _P, _P, _L]),
+    "fg_relu_backward": (_I, [_P, _P, _P, _P, _L]),
+    "fg_tanh_forward": (_I, [_P, _P, _P, _L]),
+    "fg_tanh_backward": (_I, [_P, _P, _P, _P, _L]),
+    "fg_abs_forward": (_I, [_P, _P, _P, _L, _P]),
+    "fg_abs_backward": (_I, [_P, _P, _P, _L, _P]),
 }
 
 MAX_ITERS = 16  # the most D or G iterations one call runs (fg_train_step_iters)

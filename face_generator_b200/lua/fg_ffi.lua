@@ -212,6 +212,34 @@ int fg_dn_train_step(fg_dn* n, const fg_dn_hyper* h, int B, const float* images,
                      uint64_t seed, fg_dn_stats* stats);
 int fg_dn_denoise(fg_dn* n, const float* images, int N, int chunk, float* out);
 int64_t fg_dn_debug_tensor(fg_dn* n, const char* name, float* dst, int64_t max_elems);
+typedef struct fg_ae fg_ae;
+typedef struct fg_ae_hyper { float lr, beta1, beta2, eps; float L1, L2; float p_drop; } fg_ae_hyper;
+typedef struct fg_ae_stats { float loss; int32_t t; } fg_ae_stats;
+void fg_ae_hyper_default(fg_ae_hyper* h);
+int fg_ae_create(fg_ctx* ctx, int size, int noise_dim, fg_ae** out);
+int fg_ae_destroy(fg_ae* n);
+int64_t fg_ae_param_count(int size, int noise_dim);
+int fg_ae_set_params(fg_ae* n, const float* src);
+int fg_ae_get_params(fg_ae* n, float* dst);
+int fg_ae_get_grads(fg_ae* n, float* dst);
+int fg_ae_zero_grads(fg_ae* n);
+int fg_ae_set_adam_state(fg_ae* n, const float* m, const float* v, int t);
+int fg_ae_get_adam_state(fg_ae* n, float* m, float* v, int* t);
+int fg_ae_forward(fg_ae* n, const float* x, int B, int training, const float* masks, uint64_t seed, float* code_out,
+                  float* out);
+int fg_ae_backward(fg_ae* n, const float* dout);
+int fg_ae_train_step(fg_ae* n, const fg_ae_hyper* h, int B, const float* images, const float* masks, uint64_t seed,
+                     fg_ae_stats* stats);
+int fg_ae_train_step_dataset(fg_ae* n, fg_dataset* d, const fg_ae_hyper* h, const int32_t* idx, int B, uint64_t seed,
+                             fg_ae_stats* stats);
+int fg_ae_reconstruct(fg_ae* n, const float* images, int64_t N, int chunk, int training, uint64_t seed, float* out);
+int64_t fg_ae_debug_tensor(fg_ae* n, const char* name, float* dst, int64_t max_elems);
+int fg_relu_forward(fg_ctx* ctx, const float* x, float* y, int64_t n);
+int fg_relu_backward(fg_ctx* ctx, const float* x, const float* dy, float* dx, int64_t n);
+int fg_tanh_forward(fg_ctx* ctx, const float* x, float* y, int64_t n);
+int fg_tanh_backward(fg_ctx* ctx, const float* y, const float* dy, float* dx, int64_t n);
+int fg_abs_forward(fg_ctx* ctx, const float* x, const float* t, int64_t n, float* loss_out);
+int fg_abs_backward(fg_ctx* ctx, const float* x, const float* t, int64_t n, float* dx);
 ]]
 
 local M = {}

@@ -451,6 +451,69 @@ int fg_dn_denoise(fg_dn* n, const float* images, int N, int chunk, float* out);
  * last backward's gradients dz4 dh3 dz3 dh2 dz2 dh1 dz1 (NHWC)                                      */
 int64_t fg_dn_debug_tensor(fg_dn* n, const char* name, float* dst, int64_t max_elems);
 
+/* ---- the autoencoder of train_autoencoder.lua ------------------------------------------------- */
+/* MODEL_AE = View(I) Linear(I,512) ReLU Linear(512,d) Tanh Dropout(0.5) Linear(d,256) ReLU
+ * Linear(256,I) Sigmoid View(1,S,S) (train_autoencoder.lua:80-92): grayscale images [B][1][S][S],
+ * S = 16 or 32, I = S^2, d = --noiseDim (a multiple of 8 in [8, 1024]; a multiple of 64 keeps all four
+ * Linear layers on the tensor cores).  Parameters in getParameters() order [L1W L1b .. L4W L4b],
+ * weights [out][in].  The object borrows the ctx (destroy it before the ctx), which must have 1
+ * channel and be single-GPU (else FG_ERR_UNSUPPORTED).  No BatchNorm: batches run from 1 to max_batch. */
+typedef struct fg_ae fg_ae;
+typedef struct fg_ae_hyper {
+  float lr, beta1, beta2, eps;  /* optim.adam with OPTSTATE.adam = {}: 1e-3, 0.9, 0.999, 1e-8         */
+  float L1, L2;                 /* --coefL1 / --coefL2: 0, 0 (grad += L1 sign(P) + L2 P)               */
+  float p_drop;                 /* Dropout(0.5)                                                        */
+} fg_ae_hyper;
+typedef struct fg_ae_stats {
+  float loss;                   /* nn.AbsCriterion: mean |output - input| (no penalty terms)           */
+  int32_t t;                    /* the Adam step counter                                               */
+} fg_ae_stats;
+void fg_ae_hyper_default(fg_ae_hyper* h);
+int fg_ae_create(fg_ctx* ctx, int size, int noise_dim, fg_ae** out);
+int fg_ae_destroy(fg_ae* n);
+int64_t fg_ae_param_count(int size, int noise_dim);       /* -1 for an unsupported shape              */
+int fg_ae_set_params(fg_ae* n, const float* src);
+int fg_ae_get_params(fg_ae* n, float* dst);
+int fg_ae_get_grads(fg_ae* n, float* dst);
+int fg_ae_zero_grads(fg_ae* n);
+int fg_ae_set_adam_state(fg_ae* n, const float* m, const float* v, int t);
+int fg_ae_get_adam_state(fg_ae* n, float* m, float* v, int* t);
+/* forward: x [B][1][S][S] -> out (same shape) and the encoder's output code_out [B][d] (tanh, before
+ * Dropout); either may be NULL.  training != 0: Dropout with the keep flags masks [B][d], drawn from
+ * `seed` when NULL; 0: evaluate().  backward: dout = dL/d(out) of the last forward; the parameter
+ * gradients are ACCUMULATED (fg_ae_zero_grads).  A train step or fg_ae_reconstruct leaves no forward
+ * to differentiate: FG_ERR_STATE.                                                                   */
+int fg_ae_forward(fg_ae* n, const float* x, int B, int training, const float* masks, uint64_t seed, float* code_out,
+                  float* out);
+int fg_ae_backward(fg_ae* n, const float* dout);
+/* the per-batch body of train_autoencoder.lua:178-209: zero gradients, forward, nn.AbsCriterion with
+ * the images as their own targets, backward, penalty gradients, optim.adam; no gradient clamp.  The
+ * criterion's gradient is +1/n where output >= target (a tie counts as positive), -1/n elsewhere.
+ * masks [B][d] keep flags or NULL (drawn from `seed`).  Replays a captured CUDA graph; with stats ==
+ * NULL the call does not wait for the GPU.                                                          */
+int fg_ae_train_step(fg_ae* n, const fg_ae_hyper* h, int B, const float* images, const float* masks, uint64_t seed,
+                     fg_ae_stats* stats);
+/* the same on images idx[0..B) (int32, host or device) of a dataset on the same ctx, gathered at S x S
+ * on the device (fg_dataset_gather_sized); keep flags drawn from `seed`.  Nothing synchronises unless
+ * stats != NULL: an epoch over a host-owned permutation can be enqueued without waiting.            */
+int fg_ae_train_step_dataset(fg_ae* n, fg_dataset* d, const fg_ae_hyper* h, const int32_t* idx, int B, uint64_t seed,
+                             fg_ae_stats* stats);
+/* MODEL_AE:forward of N images, `chunk` (<= max_batch) at a time.  training != 0 keeps Dropout live, as
+ * getSamples (train_autoencoder.lua:137-145) does; chunk k then draws its keep flags from seed + k.    */
+int fg_ae_reconstruct(fg_ae* n, const float* images, int64_t N, int chunk, int training, uint64_t seed, float* out);
+/* the fg_*debug_tensor contract over the last forward (x z1 h1 z2 code h2 z3 h3 z4 y, and "masks" after
+ * a training-mode one) and the last backward (dz4 dz3 dz2 dz1), each [B][features]; "loss": the last
+ * step's criterion value, one float (into device memory the copy is asynchronous)                  */
+int64_t fg_ae_debug_tensor(fg_ae* n, const char* name, float* dst, int64_t max_elems);
+/* the same layers one at a time, flat tensors of n floats (host or device pointers): nn.ReLU (backward
+ * from the input x), nn.Tanh (backward from the output y), nn.AbsCriterion size-averaged              */
+int fg_relu_forward(fg_ctx* ctx, const float* x, float* y, int64_t n);
+int fg_relu_backward(fg_ctx* ctx, const float* x, const float* dy, float* dx, int64_t n);
+int fg_tanh_forward(fg_ctx* ctx, const float* x, float* y, int64_t n);
+int fg_tanh_backward(fg_ctx* ctx, const float* y, const float* dy, float* dx, int64_t n);
+int fg_abs_forward(fg_ctx* ctx, const float* x, const float* t, int64_t n, float* loss_out);
+int fg_abs_backward(fg_ctx* ctx, const float* x, const float* t, int64_t n, float* dx);
+
 /* ---- Torch7 checkpoint files (host only, no GPU needed) --------------------------------------- */
 /* Reads the binary torch.save format of the reference's checkpoints -- torch.save(filename,
  * {D=MODEL_D, G=MODEL_G, opt=OPT, epoch=EPOCH}) at adversarial.lua:328 / adversarial_c2f.lua:216,

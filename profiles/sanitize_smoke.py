@@ -85,6 +85,28 @@ for C, B, impl in ((3, 12, 2), (1, 6, 0)):  # ragged batches on purpose (not mul
     dxs, dws = np.empty_like(xs), np.zeros_like(ws)
     assert ctx.lib.fg_scu_backward_data(ctx.h, _ptr(ys), _ptr(ws), _ptr(dxs), 2, 64, 8, 8, 16, 3, 2) == 0
     assert ctx.lib.fg_scu_backward_filter(ctx.h, _ptr(xs), _ptr(ys), _ptr(dws), None, 2, 64, 8, 8, 16, 3, 2) == 0
+    if C == 1:  # the autoencoder of train_autoencoder.lua is grayscale: three steps (eager, captured, replayed), host- and
+        # device-fed with a ragged last batch, both forwards, the backward and the layer ops
+        from face_generator_b200 import autoencoder as A
+        ae = A.Autoencoder(ctx, 16, 64)
+        ae.set_params(A.init_params(16, 64, rng) * 10)
+        im = rng.random((B, 1, 16, 16)).astype(np.float32)
+        for i in range(3):
+            assert np.isfinite(ae.train_step(A.ae_hyper_default(L2=1e-4), im, seed=60 + i)["loss"])
+            assert np.isfinite(ae.train_step_dataset(ds, A.ae_hyper_default(), np.arange(B - i, dtype=np.int32), seed=i)["loss"])
+        ae.zero_grads()
+        ae.backward(ae.forward(im, training=True, seed=3)[1])
+        ae.reconstruct(im, chunk=4, training=True, seed=1)
+        ae.encode(im, chunk=5)
+        ae.close()
+        from face_generator_b200.lib import _ptr
+        v, o = rng.standard_normal(1000).astype(np.float32), np.empty(1000, np.float32)
+        for fn in (ctx.lib.fg_relu_forward, ctx.lib.fg_tanh_forward):
+            assert fn(ctx.h, _ptr(v), _ptr(o), v.size) == 0
+        for fn in (ctx.lib.fg_relu_backward, ctx.lib.fg_tanh_backward):
+            assert fn(ctx.h, _ptr(v), _ptr(v), _ptr(o), v.size) == 0
+        assert ctx.lib.fg_abs_forward(ctx.h, _ptr(v), _ptr(o), v.size, _ptr(o[:1].copy())) == 0
+        assert ctx.lib.fg_abs_backward(ctx.h, _ptr(v), _ptr(v), v.size, _ptr(o)) == 0
     ds.close()
     ctx.close()
     print("ok", C, B, impl, flush=True)
