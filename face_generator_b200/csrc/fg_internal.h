@@ -268,8 +268,8 @@ struct fg_ctx {
   double* red_ws_opt = nullptr;  // [kOptRedRows]: the penalty-loss sum of the optimizer, which may run on comm_stream
   unsigned* red_ticket = nullptr;  // [0]: red_ws, [1]: red_ws_opt
   // workspaces of the BatchNorm kernels, shared by the generators on this ctx's stream
-  double* bn_slice_acc = nullptr;  // workspace of k_bn_finalize_parts: 32 slices x 2 x 256 doubles + tickets
-  float* bn_parts = nullptr;  // [m-tile][2][C] BatchNorm partials written by the tensor-core conv epilogue
+  double* bn_slice_acc = nullptr;  // workspace of k_bn_finalize_parts: 32 slices x 4 x 256 doubles + tickets
+  float* bn_parts = nullptr;  // [m-tile][3][C] BatchNorm partials written by the tensor-core conv epilogue
   int edge_impl = 1;          // option "edge_impl": 0 = the round-1 small-channel kernels (k_conv_small.cu) for G.C3 / D.C1
   int bn_epilogue = 1;        // option "bn_epilogue": 0 = separate statistics pass over z (the round-1 path)
   int mma_f16 = 1;            // option "mma_f16": 1 (default) = tensor-core operands in the 3xFP16 split (f16 MMAs); 0 = 3xTF32
@@ -375,8 +375,10 @@ int k_bn_bwd_reduce4(fg_ctx* c, const float* dh, const float* z, const float* me
                      const float* beta, const float* slope, double* acc, float* dslope, int64_t P, int C);
 int k_bn_finalize(fg_ctx* c, double* acc2C, float* mean, float* istd, float* run_mean, float* run_var, int64_t P,
                   int C);
-int k_bn_finalize_parts(fg_ctx* c, const float* part, int nparts, float* mean, float* istd, float* run_mean, float* run_var,
-                        int64_t P, int C);  // statistics from the conv epilogue's per-tile partials
+// statistics from the conv epilogue's per-tile partials (sum z, sum z^2, squared deviations from the tile mean) of a
+// convolution with nphase output phases
+int k_bn_finalize_parts(fg_ctx* c, const float* part, int nparts, int nphase, float* mean, float* istd, float* run_mean,
+                        float* run_var, int64_t P, int C);
 int k_bn_eval_prep(fg_ctx* c, const float* run_mean, const float* run_var, float* mean, float* istd, int C);
 int k_bn_prelu_apply(fg_ctx* c, const float* z, const float* mean, const float* istd, const float* gamma,
                      const float* beta, const float* slope, float* h, int64_t P, int C, float* hi = nullptr,

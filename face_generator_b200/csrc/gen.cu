@@ -109,7 +109,7 @@ int bn_stats(fg_ctx* c, UpsGen& G, NetPair& p, int i, const float* z, int B, boo
   if (!training) return k_bn_eval_prep(c, rm, rv, G.bn_mean[i], G.bn_istd[i], Cc);
   if (parts) {
     ScopedTimer tm(c, t_finalize);
-    return k_bn_finalize_parts(c, c->bn_parts, parts, G.bn_mean[i], G.bn_istd[i], rm, rv, P, Cc);
+    return k_bn_finalize_parts(c, c->bn_parts, parts, 4, G.bn_mean[i], G.bn_istd[i], rm, rv, P, Cc);  // 4 upsampling phases
   }
   {
     ScopedTimer tm(c, t_stats);

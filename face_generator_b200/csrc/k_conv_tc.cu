@@ -433,7 +433,7 @@ bool pick_box(int H, int W, int npix, int* bw, int* bh, int* bb) {
 }
 
 template <int BN>
-constexpr size_t fwd_smem() { return (size_t)kStages * (2 * kABytes + 2 * BN * 128) + 256 + 2 * 8 * BN * 4 + 1024; }
+constexpr size_t fwd_smem() { return (size_t)kStages * (2 * kABytes + 2 * BN * 128) + 256 + 5 * 8 * BN * 4 + 1024; }
 // F16: 3 TMA stages; TF32: 2 TMA stages + the K-major copy of one (same bytes per stage)
 template <int BN>
 constexpr size_t wg_smem() { return (size_t)3 * (2 * 4 * 4096 + 2 * (BN / 32) * 4096) + 128 + 1024; }

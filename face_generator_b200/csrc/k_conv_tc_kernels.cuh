@@ -182,39 +182,70 @@ __device__ __forceinline__ void tapconv_mma_tile(const TcFwdParams& p, int tile,
     for (int i = 0; i < BN / 2; ++i) o[i] += p.bias[t.n0 + 8 * (i >> 2) + 2 * tq + (i & 1)];
   }
   if (p.stats) {
-    // BatchNorm statistics from the convolution epilogue (nn.SpatialBatchNormalization, models.lua:65,70): per
-    // tile the column sums of z and z^2 over its (valid) 128 pixels.  Each warp reduces its 16 rows with shuffles,
-    // the 8 warps meet in shared memory and one thread per column writes the tile's partial.  Every sum has a fixed
-    // order => replicas stay identical.
+    // BatchNorm statistics from the convolution epilogue (nn.SpatialBatchNormalization, models.lua:65,70), three
+    // partials per tile and column over its valid pixels: the sums of z and of z^2 and the sum of squared deviations
+    // from the tile's mean.  bn_finalize_parts_kernel forms the variance from the first two (one pass) unless that
+    // cancels: a channel whose mean is large against its spread, or whose variance is below eps, loses ~2^-24 mean^2 of
+    // its variance there, and then combines the third in double.  For the third each warp sums z - s and (z - s)^2
+    // over its 16 rows, s = z of its first row (a sample of the same column, so the sums no longer carry the mean), and
+    // one thread per column moves the 8 warps' sums to warp 0's shift.  Each warp reduces its rows with shuffles, the
+    // 8 warps meet in shared memory; every sum has a fixed order => replicas stay identical.
     const bool v0 = b[0] < p.B, v1 = b[1] < p.B;
+    const int nvalid = p.bb == 1 ? 128 : min(p.bb, p.B - t.b0) * p.bw * p.bh;  // = bn_tile_count in k_elem.cu
+    const int gi = ((g & 1) << 2) | (g & 2) | ((g & 4) >> 2);  // which of the 8 values lane g is left with (below)
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
+      // this lane's 2 columns x {z, z^2, z - s, (z - s)^2} summed over its 2 rows: v[2 q + e], q = the quantity
+      float v[8];
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const float z0 = v0 ? o[4 * j + e] : 0.f, z1 = v1 ? o[4 * j + 2 + e] : 0.f;
-        float x = z0 + z1, y = z0 * z0 + z1 * z1;
+        v[e] = z0 + z1;
+        v[2 + e] = z0 * z0 + z1 * z1;
+        const float s = __shfl_sync(0xffffffffu, o[4 * j + e], tq);  // row 16 warp (g = 0, h = 0) of this column
+        const float d0 = v0 ? o[4 * j + e] - s : 0.f, d1 = v1 ? o[4 * j + 2 + e] - s : 0.f;
+        v[4 + e] = d0 + d1;
+        v[6 + e] = fmaf(d0, d0, d1 * d1);
+        if (g == 0) stat_sm[(4 * 8 + warp) * BN + 8 * j + 2 * tq + e] = s;
+      }
+      // sum over the 8 lanes of equal tq (xor 4, 8, 16), halving the values each lane holds at every step: the
+      // lane whose mask bit is 0 keeps the lower half.  Each value sees the additions of a plain xor-shuffle tree,
+      // in the same pairs.
 #pragma unroll
-        for (int sft = 4; sft < 32; sft <<= 1) {
-          x += __shfl_xor_sync(0xffffffffu, x, sft);
-          y += __shfl_xor_sync(0xffffffffu, y, sft);
-        }
-        if (g == 0) {
-          stat_sm[(0 * 8 + warp) * BN + 8 * j + 2 * tq + e] = x;
-          stat_sm[(1 * 8 + warp) * BN + 8 * j + 2 * tq + e] = y;
+      for (int L = 8, m = 4; L > 1; L >>= 1, m <<= 1) {
+        const bool up = (lane & m) != 0;
+#pragma unroll
+        for (int k = 0; k < L / 2; ++k) {
+          const float send = up ? v[k] : v[k + L / 2], keep = up ? v[k + L / 2] : v[k];
+          v[k] = keep + __shfl_xor_sync(0xffffffffu, send, m);
         }
       }
+      stat_sm[((gi >> 1) * 8 + warp) * BN + 8 * j + 2 * tq + (gi & 1)] = v[0];
     }
     consumer_sync();
     const int et = threadIdx.x;
-    if (et < BN) {
+    const int mt = tile / (p.Cout / BN);
+    if (et < BN) {  // threads [0, BN): the sums of z and z^2
       float s0 = 0.f, s1 = 0.f;
       for (int w = 0; w < 8; ++w) {
         s0 += stat_sm[(0 * 8 + w) * BN + et];
         s1 += stat_sm[(1 * 8 + w) * BN + et];
       }
-      const int mt = tile / (p.Cout / BN);
-      p.stats[((int64_t)mt * 2 + 0) * p.Cout + t.n0 + et] = s0;
-      p.stats[((int64_t)mt * 2 + 1) * p.Cout + t.n0 + et] = s1;
+      p.stats[((int64_t)mt * 3 + 0) * p.Cout + t.n0 + et] = s0;
+      p.stats[((int64_t)mt * 3 + 1) * p.Cout + t.n0 + et] = s1;
+    } else if (et < 2 * BN) {  // threads [BN, 2 BN): the squared deviations from the tile mean
+      // sum over the valid rows of (z - r) and (z - r)^2, r = warp 0's shift: warp w's n rows moved by d = s_w - r
+      const int col = et - BN;
+      const float r = stat_sm[(4 * 8 + 0) * BN + col];
+      float t1 = 0.f, t2 = 0.f;
+      for (int w = 0; w < 8; ++w) {
+        const float n = (float)max(0, min(16, nvalid - 16 * w));
+        const float xs = stat_sm[(2 * 8 + w) * BN + col], ys = stat_sm[(3 * 8 + w) * BN + col];
+        const float d = stat_sm[(4 * 8 + w) * BN + col] - r;
+        t1 += fmaf(n, d, xs);
+        t2 += fmaf(d, fmaf(n, d, 2.f * xs), ys);
+      }
+      p.stats[((int64_t)mt * 3 + 2) * p.Cout + t.n0 + col] = fmaxf(0.f, fmaf(-t1 / (float)nvalid, t1, t2));
     }
     consumer_sync();
   }
@@ -235,7 +266,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tapconv_tc_kernel(const __grid_
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
   uint64_t* empty = full + kStages;
-  float* stat_sm = reinterpret_cast<float*>(smem + kStages * kStageBytes + 256);  // [2][8 warps][BN] (p.stats only)
+  float* stat_sm = reinterpret_cast<float*>(smem + kStages * kStageBytes + 256);  // [5][8 warps][BN] (p.stats only)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ntiles = p.ntiles;

@@ -303,37 +303,61 @@ int k_bn_finalize(fg_ctx* c, double* acc, float* mean, float* istd, float* run_m
   return FG_OK;
 }
 // BatchNorm statistics from the per-tile partials the tensor-core convolution wrote in its epilogue
-// (part[tile][2][C]: sum z, sum z^2 over the tile's pixels).  Grid (C/32, S slices): a block of 32 channels x 8
-// thread groups sums its slice of the tiles with double accumulators in a fixed order and writes a per-slice partial;
-// the block that finishes LAST (atomic ticket per channel group) adds the S slice partials in slice order and
-// finalises.  Every sum has a fixed order whatever the scheduling => data-parallel replicas stay bit-identical.
+// (part[tile][3][C]: over the tile's n_i valid pixels the sums s_i of z and q_i of z^2, and the sum m2_i of squared
+// deviations from the tile's mean s_i / n_i).  The one-pass variance sum q_i / n - mean^2 is exact enough while the
+// channel's mean square is within kBnOnePassRatio of var + eps: it then loses less than 4 of fp32's bits of the
+// variance to cancellation.  Beyond that (a mean far from 0 against the spread, or a variance below eps) the variance
+// comes from the third partial instead: with r = tile 0's mean, sum (s_i - n_i r) and sum m2_i + (s_i - n_i r)^2 / n_i
+// are double sums without cancellation.  Grid (C/32, S slices): a block of 32 channels x 8 thread groups sums its slice
+// of the tiles in a fixed order and writes a per-slice partial; the block that finishes LAST (atomic ticket per channel
+// group) adds the S slice partials in slice order and finalises.  Every sum has a fixed order whatever the
+// scheduling => data-parallel replicas stay bit-identical.
 constexpr int kBnSlices = 32;
-__global__ void __launch_bounds__(256) bn_finalize_parts_kernel(const float* __restrict__ part, int nparts, double* __restrict__ slice_acc,
+constexpr double kBnOnePassRatio = 16.0;
+// valid pixels of epilogue tile i: tiles are 128 pixels of one output phase (nphase phases, phase fastest); only the
+// last tile of each phase can be short, when its box holds several images and the batch ends inside it
+__device__ __forceinline__ double bn_tile_count(int i, int nphase, int64_t phase_pixels) {
+  return (double)min((int64_t)128, phase_pixels - (int64_t)(i / nphase) * 128);
+}
+__global__ void __launch_bounds__(256) bn_finalize_parts_kernel(const float* __restrict__ part, int nparts, int nphase,
+                                                                double* __restrict__ slice_acc,
                                                                 unsigned int* __restrict__ ticket, float* __restrict__ mean,
                                                                 float* __restrict__ istd, float* __restrict__ run_mean,
                                                                 float* __restrict__ run_var, int64_t P, int C) {
-  __shared__ double sm[2][8][32];
+  __shared__ double sm[4][8][32];
   __shared__ bool last;
   const int lane = threadIdx.x & 31, g = threadIdx.x >> 5;
   const int ch = blockIdx.x * 32 + lane;
   const int per = (nparts + kBnSlices - 1) / kBnSlices;
   const int i0 = blockIdx.y * per, i1 = min(nparts, i0 + per);
-  double s = 0, q = 0;
+  const int64_t pp = P / nphase;
+  const double r = ch < C ? (double)part[ch] / bn_tile_count(0, nphase, pp) : 0.0;
+  double s = 0, q = 0, ds = 0, dq = 0;
   if (ch < C)
     for (int i = i0 + g; i < i1; i += 8) {
-      s += (double)part[((int64_t)i * 2 + 0) * C + ch];
-      q += (double)part[((int64_t)i * 2 + 1) * C + ch];
+      const double si = (double)part[((int64_t)i * 3 + 0) * C + ch];
+      s += si;
+      q += (double)part[((int64_t)i * 3 + 1) * C + ch];
+      const double n = bn_tile_count(i, nphase, pp), d = si - n * r;
+      ds += d;
+      dq += (double)part[((int64_t)i * 3 + 2) * C + ch] + d * d * (n == 128.0 ? 1.0 / 128 : 1.0 / n);
     }
   sm[0][g][lane] = s;
   sm[1][g][lane] = q;
+  sm[2][g][lane] = ds;
+  sm[3][g][lane] = dq;
   __syncthreads();
   if (g == 0 && ch < C) {
     for (int k = 1; k < 8; ++k) {
       s += sm[0][k][lane];
       q += sm[1][k][lane];
+      ds += sm[2][k][lane];
+      dq += sm[3][k][lane];
     }
-    slice_acc[((int64_t)blockIdx.y * 2 + 0) * C + ch] = s;
-    slice_acc[((int64_t)blockIdx.y * 2 + 1) * C + ch] = q;
+    slice_acc[((int64_t)blockIdx.y * 4 + 0) * C + ch] = s;
+    slice_acc[((int64_t)blockIdx.y * 4 + 1) * C + ch] = q;
+    slice_acc[((int64_t)blockIdx.y * 4 + 2) * C + ch] = ds;
+    slice_acc[((int64_t)blockIdx.y * 4 + 3) * C + ch] = dq;
   }
   __threadfence();
   __syncthreads();
@@ -343,28 +367,30 @@ __global__ void __launch_bounds__(256) bn_finalize_parts_kernel(const float* __r
   __threadfence();
   if (threadIdx.x == 0) ticket[blockIdx.x] = 0;  // ready for the next launch
   if (g != 0 || ch >= C) return;
-  s = 0;
-  q = 0;
+  s = q = ds = dq = 0;
   for (int k = 0; k < kBnSlices; ++k) {
-    s += slice_acc[((int64_t)k * 2 + 0) * C + ch];
-    q += slice_acc[((int64_t)k * 2 + 1) * C + ch];
+    s += slice_acc[((int64_t)k * 4 + 0) * C + ch];
+    q += slice_acc[((int64_t)k * 4 + 1) * C + ch];
+    ds += slice_acc[((int64_t)k * 4 + 2) * C + ch];
+    dq += slice_acc[((int64_t)k * 4 + 3) * C + ch];
   }
   const double n = (double)P;
   const double m = s / n;
   double var = q / n - m * m;
   if (var < 0) var = 0;
+  if (q / n > kBnOnePassRatio * (var + 1e-5)) var = fmax(0.0, (dq - ds * (ds / n)) / n);  // the one pass cancelled
   mean[ch] = (float)m;
   istd[ch] = (float)(1.0 / sqrt(var + 1e-5));
   if (run_mean) run_mean[ch] = 0.9f * run_mean[ch] + 0.1f * (float)m;
   if (run_var) run_var[ch] = 0.9f * run_var[ch] + 0.1f * (float)(P > 1 ? var * n / (n - 1.0) : var);
 }
-// slice_ws: kBnSlices * 2 * C doubles + (C/32) tickets (zeroed once at allocation)
-int k_bn_finalize_parts(fg_ctx* c, const float* part, int nparts, float* mean, float* istd, float* run_mean, float* run_var,
-                        int64_t P, int C) {
+// slice_ws: kBnSlices * 4 * C doubles + (C/32) tickets (zeroed once at allocation)
+int k_bn_finalize_parts(fg_ctx* c, const float* part, int nparts, int nphase, float* mean, float* istd, float* run_mean,
+                        float* run_var, int64_t P, int C) {
   double* acc = c->bn_slice_acc;
-  unsigned int* ticket = reinterpret_cast<unsigned int*>(acc + (size_t)kBnSlices * 2 * 256);
-  bn_finalize_parts_kernel<<<dim3((C + 31) / 32, kBnSlices), 256, 0, c->stream>>>(part, nparts, acc, ticket, mean, istd, run_mean,
-                                                                                run_var, P, C);
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(acc + (size_t)kBnSlices * 4 * 256);
+  bn_finalize_parts_kernel<<<dim3((C + 31) / 32, kBnSlices), 256, 0, c->stream>>>(part, nparts, nphase, acc, ticket, mean, istd,
+                                                                                run_mean, run_var, P, C);
   LAUNCH_CHECK(c);
   return FG_OK;
 }

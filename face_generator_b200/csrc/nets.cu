@@ -65,9 +65,9 @@ int net_alloc(fg_ctx* c) {
   FG_TRY(dalloc(c, &c->small_ws, (size_t)kSmallMaxParts * 9 * 4 * 128));
   FG_TRY(dalloc(c, &tmp, 4 * 256 * 2));  // doubles
   c->bn_acc = (double*)tmp;
-  FG_TRY(dalloc(c, &tmp, 32 * 2 * 256 * 2 + 64));  // doubles + tickets (zero-initialised)
+  FG_TRY(dalloc(c, &tmp, 32 * 4 * 256 * 2 + 64));  // doubles + tickets (zero-initialised)
   c->bn_slice_acc = (double*)tmp;
-  FG_TRY(dalloc(c, &c->bn_parts, B * 2048));  // G.C2: 8 tiles/image x 2 x 128 ch; G.C1: 2 tiles/image x 2 x 256 ch
+  FG_TRY(dalloc(c, &c->bn_parts, B * 3072));  // G.C2: 8 tiles/image x 3 x 128 ch; G.C1: 2 tiles/image x 3 x 256 ch
   // D activations
   FG_TRY(dalloc(c, &c->D_x, B * 1024 * C));
   for (int i = 0; i < 4; ++i) {
