@@ -251,6 +251,11 @@ int64_t fg_get_option(fg_ctx* c, const char* key) {
   if (!strcmp(key, "bwd_merge_ctas")) return c->bwd_merge_ctas;
   if (!strcmp(key, "optimizer_D")) return c->opt_D;
   if (!strcmp(key, "optimizer_G")) return c->opt_G;
+  if (!strcmp(key, "last_conv_kind")) return c->last_conv_kind;
+  if (!strcmp(key, "last_conv_tile_m")) return c->last_conv_tile_m;
+  if (!strcmp(key, "last_conv_tile_n")) return c->last_conv_tile_n;
+  if (!strcmp(key, "last_conv_format")) return c->last_conv_format;
+  if (!strcmp(key, "last_conv_splits")) return c->last_conv_splits;
   return -1;
 }
 

@@ -304,6 +304,10 @@ struct fg_ctx {
   // stream already runs the G step's G forward (which only needs G's parameters); joined before D is used again
   int dp_overlap = 1;
   int reserve_sms = 0;  // SMs the persistent convolution kernels leave free while a collective runs next to them
+  // the convolution kernel launched last (fg_get_option "last_conv_*", include/fg_b200.h): FG_KERNEL_*, its tile, its
+  // operand format (0 fp32 FFMA, 1 3xTF32, 2 3xFP16) and its K splits.  Set by the launchers where they choose the
+  // kernel (note_conv), cleared on entry to every fg_conv2d_* / fg_scu_* / fg_linear_* call.  Host integers only.
+  int last_conv_kind = 0, last_conv_tile_m = 0, last_conv_tile_n = 0, last_conv_format = 0, last_conv_splits = 0;
   // option "bwd_merge": the weight and data gradients of G's upsampled layers run as one persistent launch
   // (k_conv_tc.cu tc_conv_bwd_ups).  1 (default): where its schedule estimate beats two launches (tc_bwd_pair_pays:
   // G.C2 at batch 256, not G.C1); 2: wherever the shapes allow it; 0: two launches.  Option "bwd_merge_ctas"
@@ -332,6 +336,15 @@ struct fg_ctx {
   ConvL Dc[4], DL1, DL2;
   ScalePairs D_pairs;
 };
+
+// record the convolution kernel a launcher is about to run (fg_ctx::last_conv_*)
+inline void note_conv(fg_ctx* c, int kind, int tile_m, int tile_n, int format, int splits) {
+  c->last_conv_kind = kind;
+  c->last_conv_tile_m = tile_m;
+  c->last_conv_tile_n = tile_n;
+  c->last_conv_format = format;
+  c->last_conv_splits = splits;
+}
 
 struct ScopedTimer {
   fg_ctx* c;

@@ -274,6 +274,7 @@ int launch_reduce(fg_ctx* c, const float* in, const float* Wp, const float* bias
     FG_CUDA(cudaFuncSetAttribute(conv_reduce_kernel<NS, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_done = true;
   }
+  note_conv(c, FG_KERNEL_EDGE_REDUCE, NS, VEC, 0, 1);
   conv_reduce_kernel<NS, VEC><<<std::min(nunits, c->sm_count), 256, smem, c->stream>>>(tmap, Wp, bias, out, g.H, nunits);
   LAUNCH_CHECK(c);
   return FG_OK;
@@ -281,6 +282,7 @@ int launch_reduce(fg_ctx* c, const float* in, const float* Wp, const float* bias
 template <int CS, int N>
 int launch_expand(fg_ctx* c, const float* in, const float* Wp, const float* bias, float* out, const ConvGeom& g) {
   const int nunits = g.B * (g.H / kExpRows);
+  note_conv(c, FG_KERNEL_EDGE_EXPAND, CS, N, 0, 1);
   conv_expand_kernel<CS, N><<<std::min(nunits, c->sm_count), 256, 0, c->stream>>>(in, Wp, bias, out, g.H, nunits);
   LAUNCH_CHECK(c);
   return FG_OK;

@@ -255,7 +255,9 @@ __global__ void __launch_bounds__(256) wgrad_simt_kernel(const float* __restrict
 
 int k_conv_simt(fg_ctx* c, const float* in, const float* Wp, const float* bias, float* out, ConvGeom g) {
   const int P = g.B * g.H * g.W;
+  const int tn = g.Cout > 64 ? 8 : (g.Cout > 16 ? 4 : 1);
   if (g.Cin < 16 && g.ups == 1 && g.k > 1) {
+    note_conv(c, FG_KERNEL_SIMT_FLATK, 8, tn, 0, 1);
     if (g.Cout > 64) {
       dim3 grid((P + 127) / 128, (g.Cout + 127) / 128);
       conv_simt_flatk_kernel<8, 8><<<grid, 256, 0, c->stream>>>(in, Wp, bias, out, g);
@@ -269,6 +271,7 @@ int k_conv_simt(fg_ctx* c, const float* in, const float* Wp, const float* bias, 
     LAUNCH_CHECK(c);
     return FG_OK;
   }
+  note_conv(c, FG_KERNEL_SIMT, 8, tn, 0, 1);
   if (g.Cout > 64) {
     dim3 grid((P + 127) / 128, (g.Cout + 127) / 128);
     conv_simt_kernel<8, 8><<<grid, 256, 0, c->stream>>>(in, Wp, bias, out, g);
@@ -302,6 +305,7 @@ int k_wgrad_simt(fg_ctx* c, const float* in, const float* dY, float* dWp, ConvGe
   splits = (P + pps - 1) / pps;
   float* dst = splits > 1 ? c->splitk_ws : dWp;
   dim3 grid(gx, gy, KK * splits);
+  note_conv(c, FG_KERNEL_WGRAD_SIMT, tm, tn, 0, splits);
 #define WG(TM_, TN_) wgrad_simt_kernel<TM_, TN_><<<grid, 256, 0, c->stream>>>(in, dY, dst, g, splits, pps)
   if (tm == 8 && tn == 8) WG(8, 8);
   else if (tm == 8 && tn == 4) WG(8, 4);

@@ -648,6 +648,7 @@ static int tc_chunk(bool forward_type = false) {
 
 static int launch_tapconv(fg_ctx* c, const TcFwdParams& p, int BN, int f16 = 0) {
   dim3 grid(std::min(p.ntiles, std::max(1, c->sm_count - c->reserve_sms)));
+  note_conv(c, FG_KERNEL_TAPCONV, 128, BN, f16 ? 2 : 1, 1);
   if (f16) {
     if (BN == 128) tapconv_tc_kernel<128, true><<<grid, kTcThreads, fwd_smem<128>(), c->stream>>>(p);
     else tapconv_tc_kernel<64, true><<<grid, kTcThreads, fwd_smem<64>(), c->stream>>>(p);
@@ -909,6 +910,7 @@ int tc_conv_wgrad(fg_ctx* c, const float* x_hi, const float* x_lo, const float* 
     return FG_ERR_UNSUPPORTED;
   }
   dim3 grid(ntt, (g.Cout / 128) * (g.Cin / BN), splits);
+  note_conv(c, FG_KERNEL_WGRAD_TC, 128, BN, f16 ? 2 : 1, splits);
   if (f16) {
     if (BN == 128) wgrad_tc_kernel<128, true><<<grid, kTcThreads, wg_smem<128>(), c->stream>>>(p);
     else wgrad_tc_kernel<64, true><<<grid, kTcThreads, wg_smem<64>(), c->stream>>>(p);

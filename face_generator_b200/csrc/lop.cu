@@ -58,14 +58,17 @@ int out_done(fg_ctx* c, float* user, const float* dev, size_t n) {
       return FG_ERR_INVALID;                          \
     }                                                 \
     FG_CUDA(cudaSetDevice((c)->device));              \
+    note_conv((c), FG_KERNEL_NONE, 0, 0, 0, 0);       \
   } while (0)
+// the shape every convolution entry point accepts: positive sizes, an odd kernel ("same" padding (k-1)/2)
+#define CONV_SHAPE_OK (N > 0 && Cin > 0 && Cout > 0 && H > 0 && W > 0 && k >= 1 && (k & 1))
 
 extern "C" {
 
 int fg_conv2d_forward(fg_ctx* c, const float* x, const float* w, const float* b, float* y, int N, int Cin, int H, int W,
                       int Cout, int k) {
   ENTER(c);
-  FG_REQUIRE(x && w && y && N > 0 && Cin > 0 && Cout > 0 && H > 0 && W > 0 && k >= 1 && (k & 1),
+  FG_REQUIRE(x && w && y && CONV_SHAPE_OK,
              "fg_conv2d_forward: bad arguments (odd kernel sizes only: same padding (k-1)/2)");
   const size_t nx = (size_t)N * Cin * H * W, ny = (size_t)N * Cout * H * W, nw = (size_t)Cout * Cin * k * k;
   const float *xd, *wd, *bd = nullptr;
@@ -106,7 +109,8 @@ int fg_conv2d_forward(fg_ctx* c, const float* x, const float* w, const float* b,
 int fg_conv2d_backward_data(fg_ctx* c, const float* dy, const float* w, float* dx, int N, int Cin, int H, int W, int Cout,
                             int k) {
   ENTER(c);
-  FG_REQUIRE(dy && w && dx && N > 0 && (k & 1), "fg_conv2d_backward_data: bad arguments");
+  FG_REQUIRE(dy && w && dx && CONV_SHAPE_OK, "fg_conv2d_backward_data: bad arguments (N %d, Cin %d, %dx%d, Cout %d, k %d)",
+             N, Cin, H, W, Cout, k);
   const size_t nx = (size_t)N * Cin * H * W, ny = (size_t)N * Cout * H * W, nw = (size_t)Cout * Cin * k * k;
   const float *dyd, *wd;
   FG_TRY(in_dev(c, dy, ny, 0, &dyd));
@@ -145,7 +149,8 @@ int fg_conv2d_backward_data(fg_ctx* c, const float* dy, const float* w, float* d
 int fg_conv2d_backward_filter(fg_ctx* c, const float* x, const float* dy, float* dw, float* db, int N, int Cin, int H,
                               int W, int Cout, int k) {
   ENTER(c);
-  FG_REQUIRE(x && dy && dw && N > 0 && (k & 1), "fg_conv2d_backward_filter: bad arguments");
+  FG_REQUIRE(x && dy && dw && CONV_SHAPE_OK, "fg_conv2d_backward_filter: bad arguments (N %d, Cin %d, %dx%d, Cout %d, k %d)",
+             N, Cin, H, W, Cout, k);
   const size_t nx = (size_t)N * Cin * H * W, ny = (size_t)N * Cout * H * W, nw = (size_t)Cout * Cin * k * k;
   const float *xd, *dyd;
   FG_TRY(in_dev(c, x, nx, 0, &xd));
@@ -192,7 +197,8 @@ int fg_conv2d_backward_filter(fg_ctx* c, const float* x, const float* dy, float*
 // nOutputPlane*factor*factor, ...) at :14-15, and every pass only re-views the contiguous output / gradOutput between
 // [N][nOut*f*f][h][w] and [N][nOut][h*f][w*f] (:18-30, :32-58) -- the bytes do not move, so the layer IS the
 // convolution with nOut*f*f planes on the caller's buffer.
-static int scu_planes(int nOutputPlane, int factor, int* planes) {
+static int scu_planes(fg_ctx* c, int nOutputPlane, int factor, int* planes) {
+  if (c) note_conv(c, FG_KERNEL_NONE, 0, 0, 0, 0);  // a refusal here does not report the previous call's kernel
   FG_REQUIRE(nOutputPlane > 0 && factor >= 1 && (int64_t)nOutputPlane * factor * factor < (1 << 20),
              "SpatialConvolutionUpsample: bad nOutputPlane %d / factor %d", nOutputPlane, factor);
   *planes = nOutputPlane * factor * factor;
@@ -201,19 +207,19 @@ static int scu_planes(int nOutputPlane, int factor, int* planes) {
 int fg_scu_forward(fg_ctx* c, const float* x, const float* w, const float* b, float* y, int N, int Cin, int H, int W,
                    int nOutputPlane, int k, int factor) {
   int planes;
-  FG_TRY(scu_planes(nOutputPlane, factor, &planes));
+  FG_TRY(scu_planes(c, nOutputPlane, factor, &planes));
   return fg_conv2d_forward(c, x, w, b, y, N, Cin, H, W, planes, k);
 }
 int fg_scu_backward_data(fg_ctx* c, const float* dy, const float* w, float* dx, int N, int Cin, int H, int W,
                          int nOutputPlane, int k, int factor) {
   int planes;
-  FG_TRY(scu_planes(nOutputPlane, factor, &planes));
+  FG_TRY(scu_planes(c, nOutputPlane, factor, &planes));
   return fg_conv2d_backward_data(c, dy, w, dx, N, Cin, H, W, planes, k);
 }
 int fg_scu_backward_filter(fg_ctx* c, const float* x, const float* dy, float* dw, float* db, int N, int Cin, int H, int W,
                            int nOutputPlane, int k, int factor) {
   int planes;
-  FG_TRY(scu_planes(nOutputPlane, factor, &planes));
+  FG_TRY(scu_planes(c, nOutputPlane, factor, &planes));
   return fg_conv2d_backward_filter(c, x, dy, dw, db, N, Cin, H, W, planes, k);
 }
 
@@ -233,7 +239,7 @@ int fg_linear_forward(fg_ctx* c, const float* x, const float* w, const float* b,
 int fg_linear_backward(fg_ctx* c, const float* x, const float* w, const float* dy, float* dx, float* dw, float* db, int N,
                        int in, int out) {
   ENTER(c);
-  FG_REQUIRE(x && w && dy && N > 0, "fg_linear_backward: bad arguments");
+  FG_REQUIRE(x && w && dy && N > 0 && in > 0 && out > 0, "fg_linear_backward: bad arguments");
   const float *xd, *wd, *dyd;
   FG_TRY(in_dev(c, x, (size_t)N * in, 0, &xd));
   FG_TRY(in_dev(c, w, (size_t)out * in, 1, &wd));

@@ -88,7 +88,29 @@ int fg_sync(fg_ctx* ctx);
  * step's pre-activations of fg_train_step as "Dstep.*" debug tensors), "edge_impl" / "bn_epilogue"
  * (0 selects the round-1 kernels for the 3-channel convolutions / a separate BatchNorm statistics
  * pass: cross-checks), "params_dirty" (re-pack weights
- * after writing through fg_params_ptr); unknown keys return FG_ERR_INVALID                        */
+ * after writing through fg_params_ptr); unknown keys return FG_ERR_INVALID
+ *
+ * Read-only keys of fg_get_option: which kernel the last fg_conv2d_* / fg_scu_* / fg_linear_* call launched
+ * (a call launches one: forward, data gradient or weight gradient; fg_linear_backward with both dx and dw
+ * records the weight gradient).  All 0 after a call that launched none (a refused one).
+ *   "last_conv_kind"     FG_KERNEL_*
+ *   "last_conv_tile_m"   TAPCONV: 128 (pixels)  WGRAD_TC: 128 (Cout)  EDGE_REDUCE: NS (outputs)
+ *                        EDGE_EXPAND: CS (inputs)  SIMT / SIMT_FLATK / WGRAD_SIMT: TM (rows per thread)
+ *   "last_conv_tile_n"   TAPCONV / WGRAD_TC: BN  EDGE_REDUCE: VEC (channels per lane)
+ *                        EDGE_EXPAND: N (outputs)  SIMT / SIMT_FLATK / WGRAD_SIMT: TN (columns per thread)
+ *   "last_conv_format"   0 fp32 FFMA, 1 3xTF32 tensor cores, 2 3xFP16 tensor cores
+ *   "last_conv_splits"   K splits of a weight gradient (1: unsplit, written straight to its output);
+ *                        1 for every other kernel                                                   */
+enum {
+  FG_KERNEL_NONE = 0,
+  FG_KERNEL_TAPCONV = 1,      /* wgmma forward / data gradient (tapconv_tc_kernel)                   */
+  FG_KERNEL_WGRAD_TC = 2,     /* wgmma weight gradient (wgrad_tc_kernel)                             */
+  FG_KERNEL_EDGE_REDUCE = 3,  /* 3x3, W = 32, 64 / 128 -> 1 / 3 channels (conv_reduce_kernel)         */
+  FG_KERNEL_EDGE_EXPAND = 4,  /* 3x3, W = 32, 1 / 3 / 4 -> 64 / 128 channels (conv_expand_kernel)     */
+  FG_KERNEL_SIMT = 5,         /* FFMA implicit GEMM (conv_simt_kernel)                               */
+  FG_KERNEL_SIMT_FLATK = 6,   /* FFMA, taps x channels flattened for Cin < 16 (conv_simt_flatk_kernel) */
+  FG_KERNEL_WGRAD_SIMT = 7    /* FFMA weight gradient (wgrad_simt_kernel)                            */
+};
 int fg_set_option(fg_ctx* ctx, const char* key, int64_t value);
 int64_t fg_get_option(fg_ctx* ctx, const char* key);
 int fg_set_option_f(fg_ctx* ctx, const char* key, double value);    /* "sgd_momentum_D", "sgd_momentum_G"     */
