@@ -151,6 +151,81 @@ def load_reference_checkpoint(ctx, path, want_D=True):
         return int(f.number("epoch")) if f.kind("epoch") == "number" else None
 
 
+def _c2f_fit(n_params, count):
+    """' (the count of a c2f D with C channels at fine size S)' for the (C, S) whose count(C, S) is n_params, else ''"""
+    fits = ["%d channels at fine size %d" % (c, s) for c in (1, 3) for s in (16, 32, 64) if count(c, s) == n_params]
+    return " (that of %s)" % " or ".join(fits) if fits else ""
+
+
+def read_c2f_checkpoint(path, channels, fine_size):
+    """adversarial_c2f.lua:207-216's `adversarial_c2f_<cs>_to_<S>.net` ({D, G, opt, epoch}) as flat vectors:
+    dict(PG, PD, epoch) in getParameters() order.  Refuses a G or D that does not fit the c2f nets with `channels`
+    channels at fine size `fine_size` (D's Linear reads 256*(S/4)^2 features).  Needs no GPU."""
+    lib = load_library()
+    nG = int(lib.fg_c2f_param_count_sized(NET_G, channels, fine_size))
+    nD = int(lib.fg_c2f_param_count_sized(NET_D, channels, fine_size))
+    if nG < 0:
+        raise FGError("fine size %d is not supported (16, 32 or 64)" % fine_size)
+    with T7File(path) as f:
+        pg = f.net_params("G")
+        if pg.size != nG:
+            fit = _c2f_fit(pg.size, lambda c, s: int(lib.fg_c2f_param_count_sized(NET_G, c, s)))
+            raise FGError("checkpoint G has %d parameters%s (%s); the c2f G with %d channels has %d"
+                          % (pg.size, fit, f.net_describe("G"), channels, nG))
+        pd = f.net_params("D")
+        if pd.size != nD:
+            fit = _c2f_fit(pd.size, lambda c, s: int(lib.fg_c2f_param_count_sized(NET_D, c, s)))
+            raise FGError("checkpoint D has %d parameters%s (%s); the c2f D with %d channels at fine size %d has %d"
+                          % (pd.size, fit, f.net_describe("D"), channels, fine_size, nD))
+        epoch = int(f.number("epoch")) if f.kind("epoch") == "number" else None
+    return dict(PG=pg, PD=pd, epoch=epoch)
+
+
+def load_c2f_checkpoint(net, path):
+    """load G and D of an `adversarial_c2f_<cs>_to_<S>.net` into a C2f of the same channels and fine size; returns the
+    epoch (None when the file has none)"""
+    ck = read_c2f_checkpoint(path, net.C, net.S)
+    net.set_params(NET_G, ck["PG"])
+    net.set_params(NET_D, ck["PD"])
+    return ck["epoch"]
+
+
+def read_s16_checkpoint(path, channels):
+    """an `adversarial.net` trained with train.lua --scale 16 (create_G_decoder_upsampling16 / create_D16_d) as flat
+    vectors: dict(PG, bn, PD, epoch); bn = G's 768 BatchNorm running statistics, PD None when the file has no D.
+    Needs no GPU."""
+    lib = load_library()
+    nG, nD = int(lib.fg_s16_param_count(NET_G, channels)), int(lib.fg_s16_param_count(NET_D, channels))
+    with T7File(path) as f:
+        pg = f.net_params("G")
+        if pg.size != nG:
+            raise FGError("checkpoint G has %d parameters (%s); the --scale 16 G with %d channels has %d"
+                          % (pg.size, f.net_describe("G"), channels, nG))
+        bn = f.net_bn_state("G")
+        if bn.size != 768:
+            raise FGError("checkpoint G carries %d BatchNorm running statistics, expected 768 (2 layers: 256 + 128 channels)"
+                          % bn.size)
+        pd = None
+        if f.kind("D") is not None:
+            pd = f.net_params("D")
+            if pd.size != nD:
+                raise FGError("checkpoint D has %d parameters (%s); the --scale 16 D with %d channels has %d"
+                              % (pd.size, f.net_describe("D"), channels, nD))
+        epoch = int(f.number("epoch")) if f.kind("epoch") == "number" else None
+    return dict(PG=pg, bn=bn, PD=pd, epoch=epoch)
+
+
+def load_s16_checkpoint(net, path):
+    """load G (with its BatchNorm running statistics) and, when present, D of a --scale 16 `adversarial.net` into an
+    S16; returns the epoch (None when the file has none)"""
+    ck = read_s16_checkpoint(path, net.C)
+    net.set_params(NET_G, ck["PG"])
+    net.set_bn_state(ck["bn"])
+    if ck["PD"] is not None:
+        net.set_params(NET_D, ck["PD"])
+    return ck["epoch"]
+
+
 def save_flat_checkpoint(ctx, path, epoch=0, extra=None):
     """Everything needed to resume: parameters, Adam moments and step counters, BN running statistics."""
     w = T7Writer(path)

@@ -10,17 +10,14 @@
 // kernel; fg_train_step_dataset draws the indices and both noise tensors on the device too, so a train step
 // needs no host->device traffic at all.
 //
-// image.scale(src, w, h) [third-party `image` rock, un-pinned; default mode 'bilinear'] is separable; along one
-// axis (generic/image.c, Main_scaleLinear_rowcol) it
-//   - shrinks by area averaging: output i covers source [i*s, (i+1)*s), s = src_len/dst_len (float), partial
-//     coverage of the first/last source pixel weighted by the covered fraction, divided by the total weight;
-//   - enlarges by linear interpolation with s = (src_len-1)/(dst_len-1), last output = last source pixel;
-//   - copies when the sizes match.
-// image.load(..., "float") is byte/255; nbChannels = 1 on a colour file is image.rgb2y: 0.299 R + 0.587 G + 0.114 B.
-// The oracle restates the same in numpy (oracle/oracle_data.py).  PARITY UNPINNED (no `image` rock here).
+// image.scale(src, w, h) is scale_pixel of k_scale.cuh.  image.load(..., "float") is byte/255; nbChannels = 1 on a
+// colour file is image.rgb2y: 0.299 R + 0.587 G + 0.114 B.  The oracle restates the same in numpy
+// (oracle/oracle_data.py).  PARITY UNPINNED (no `image` rock here).
 #include <algorithm>
 
 #include "fg_internal.h"
+#include "k_rng.cuh"
+#include "k_scale.cuh"
 
 struct fg_dataset {
   fg_ctx* c = nullptr;
@@ -31,79 +28,6 @@ struct fg_dataset {
 };
 
 namespace {
-__device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
-  x += 0x9E3779B97F4A7C15ull;
-  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-  return x ^ (x >> 31);
-}
-// weight of source index si for output index di along one axis (see the file header); *norm = total weight
-struct Span {
-  int i0, i1;      // source range [i0, i1]
-  float w0, w1;    // weights of i0 and i1 (everything strictly between weighs 1)
-  float norm;
-};
-__device__ __forceinline__ Span axis_span(int di, int src_len, int dst_len) {
-  Span s;
-  if (dst_len < src_len) {
-    const float scale = (float)src_len / (float)dst_len;
-    float f0 = (float)di * scale;
-    const int a = (int)f0;
-    f0 -= (float)a;
-    float f1 = (float)(di + 1) * scale;
-    int b = (int)f1;
-    f1 -= (float)b;
-    s.i0 = a;
-    s.w0 = 1.f - f0;
-    s.norm = (1.f - f0) + (float)(b - a - 1);
-    if (b < src_len) {
-      s.i1 = b;
-      s.w1 = f1;
-      s.norm += f1;
-    } else {
-      s.i1 = b - 1;
-      s.w1 = (b - 1 == a) ? s.w0 : 1.f;
-    }
-  } else if (dst_len > src_len) {
-    if (src_len == 1 || di == dst_len - 1) {
-      s.i0 = s.i1 = src_len - 1;
-      s.w0 = s.w1 = 1.f;
-      s.norm = 1.f;
-      if (src_len == 1) s.i0 = s.i1 = 0;
-    } else {
-      const float scale = (float)(src_len - 1) / (float)(dst_len - 1);
-      float f = (float)di * scale;
-      const int a = (int)f;
-      f -= (float)a;
-      s.i0 = a;
-      s.i1 = a + 1;
-      s.w0 = 1.f - f;
-      s.w1 = f;
-      s.norm = 1.f;
-    }
-  } else {
-    s.i0 = s.i1 = di;
-    s.w0 = s.w1 = 1.f;
-    s.norm = 1.f;
-  }
-  return s;
-}
-__device__ __forceinline__ float span_w(const Span& s, int i) { return i == s.i0 ? s.w0 : (i == s.i1 ? s.w1 : 1.f); }
-
-// image.scale's output pixel (y, x) of an Ho x Wo image from an Hs x Ws source, src(yy, xx) = source value: pass 1
-// (width) then pass 2 (height), like image.scale's two-pass implementation.  Every rescale of the input side goes
-// through here, so the scaling rule lives in one place.
-template <class Src>
-__device__ __forceinline__ float scale_pixel(const Src& src, int y, int x, int Hs, int Ws, int Ho, int Wo) {
-  const Span sy = axis_span(y, Hs, Ho), sx = axis_span(x, Ws, Wo);
-  float acc_y = 0.f;
-  for (int yy = sy.i0; yy <= sy.i1; ++yy) {
-    float acc_x = 0.f;
-    for (int xx = sx.i0; xx <= sx.i1; ++xx) acc_x += span_w(sx, xx) * src(yy, xx);
-    acc_y += span_w(sy, yy) * (acc_x / sx.norm);
-  }
-  return acc_y / sy.norm;
-}
 // image.load(..., "float") of channel ch of one cached image: byte/255, image.rgb2y when gray
 struct U8Src {
   const uint8_t* base;
@@ -118,13 +42,6 @@ struct U8Src {
     return base[((int64_t)ch * Hs + yy) * Ws + xx] * (1.f / 255.f);
   }
 };
-// one fp32 plane [H][W] (shared memory)
-struct PlaneSrc {
-  const float* p;
-  int W;
-  __device__ __forceinline__ float operator()(int yy, int xx) const { return p[yy * W + xx]; }
-};
-
 // out[b][c][y][x] (C channels, Ho x Wo) from u8 data[idx[b]][Cs][Hs][Ws]; gray = Cs==3 && C==1 (rgb2y)
 __global__ void gather_kernel(const uint8_t* __restrict__ data, const int32_t* __restrict__ idx, float* __restrict__ out,
                               int B, int C, int Cs, int Hs, int Ws, int Ho, int Wo, int64_t N) {
@@ -185,6 +102,18 @@ __global__ void __launch_bounds__(kPairThreads) c2f_pairs_kernel(const uint8_t* 
     if (diff) diff[o + i] = sfine[i] - v;
   }
 }
+// fg_image_scale: dst [NC][Ho][Wo] = image.scale of each plane of src [NC][Hs][Ws], one output pixel per thread
+__global__ void image_scale_kernel(const float* __restrict__ src, float* __restrict__ dst, int64_t NC, int Hs, int Ws, int Ho,
+                                   int Wo) {
+  const int64_t n = NC * Ho * Wo;
+  GRID_STRIDE(i, n) {
+    const int x = (int)(i % Wo);
+    const int64_t r = i / Wo;
+    const int y = (int)(r % Ho);
+    const int64_t plane = r / Ho;
+    dst[i] = scale_pixel(PlaneSrc{src + plane * Hs * Ws, Ws}, y, x, Hs, Ws, Ho, Wo);
+  }
+}
 // root (optional): the stream is *root * kinds + seed, read on the device (the per-iteration stream roots of a captured
 // multi-iteration step, k_seed_roots)
 __global__ void draw_indices_kernel(int32_t* __restrict__ idx, int B, uint64_t seed, int64_t N, const uint64_t* root = nullptr,
@@ -197,8 +126,7 @@ __global__ void uniform_pm1_kernel(float* __restrict__ out, int64_t n, uint64_t 
                                    uint64_t kinds = 0) {
   if (root) seed += *root * kinds;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const uint64_t r = splitmix64(seed * 0x100000001B3ull + (uint64_t)i);
-    out[i] = (float)(r >> 40) * (2.0f / 16777216.0f) - 1.0f;  // 24-bit uniform in [-1, 1)
+    out[i] = uniform_pm1_at(seed, (uint64_t)i);
   }
 }
 // ---- nearest neighbour by torch.dist (2-norm), brute force, HBM-bound ------------------------------------
@@ -520,6 +448,39 @@ int fg_noise_uniform(fg_ctx* c, uint64_t seed, int64_t n, float* out) {
   cudaFree(tmp);
   if (e != cudaSuccess) {
     fg_set_error("fg_noise_uniform: %s", cudaGetErrorString(e));
+    return FG_ERR_CUDA;
+  }
+  return FG_OK;
+}
+// image.scale(x, Wo, Ho) on fp32 NCHW images, host or device.  Host buffers go through temporary device memory (this
+// entry is not on a hot path; fg_c2f_refine scales inside its own kernel).
+int fg_image_scale(fg_ctx* c, const float* src, int64_t N, int C, int Hs, int Ws, int Ho, int Wo, float* dst) {
+  if (!c) {
+    fg_set_error("null fg_ctx");
+    return FG_ERR_INVALID;
+  }
+  FG_REQUIRE(src && dst && N >= 1 && C >= 1, "fg_image_scale: bad arguments");
+  FG_REQUIRE(Hs >= 1 && Ws >= 1 && Ho >= 1 && Wo >= 1 && Hs <= 256 && Ws <= 256 && Ho <= 256 && Wo <= 256,
+             "fg_image_scale: sizes %dx%d -> %dx%d outside [1, 256]", Hs, Ws, Ho, Wo);
+  FG_CUDA(cudaSetDevice(c->device));
+  const int64_t NC = N * C;
+  const size_t n_src = (size_t)NC * Hs * Ws, n_dst = (size_t)NC * Ho * Wo;
+  const bool src_dev = fg_is_dev(src), dst_dev = fg_is_dev(dst);
+  float* tmp = nullptr;
+  if (!src_dev || !dst_dev) FG_CUDA(cudaMalloc((void**)&tmp, sizeof(float) * ((src_dev ? 0 : n_src) + (dst_dev ? 0 : n_dst))));
+  const float* s = src_dev ? src : tmp;
+  float* d = dst_dev ? dst : tmp + (src_dev ? 0 : n_src);
+  cudaError_t e = src_dev ? cudaSuccess : cudaMemcpyAsync(tmp, src, sizeof(float) * n_src, cudaMemcpyHostToDevice, c->stream);
+  if (e == cudaSuccess) {
+    image_scale_kernel<<<grid_for((int64_t)n_dst, 256), 256, 0, c->stream>>>(s, d, NC, Hs, Ws, Ho, Wo);
+    c->launches++;
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess && !dst_dev) e = cudaMemcpyAsync(dst, d, sizeof(float) * n_dst, cudaMemcpyDeviceToHost, c->stream);
+  if (e == cudaSuccess && tmp) e = cudaStreamSynchronize(c->stream);
+  cudaFree(tmp);
+  if (e != cudaSuccess) {
+    fg_set_error("fg_image_scale: %s", cudaGetErrorString(e));
     return FG_ERR_CUDA;
   }
   return FG_OK;

@@ -92,11 +92,12 @@ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
   x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
   return x ^ (x >> 31);
 }
+// out[i] = element offset + i of stream `seed`
 __global__ void bernoulli_keep_kernel(float* __restrict__ out, int64_t n, uint64_t seed, float p_drop,
-                                      const uint64_t* __restrict__ seed_dev) {
+                                      const uint64_t* __restrict__ seed_dev, int64_t offset) {
   if (seed_dev) seed += *seed_dev * 2;  // the step seed lives in device memory (captured steps), see k_masks_generate
   GRID_STRIDE(i, n) {
-    const uint64_t r = splitmix64(seed * 0x100000001B3ull + (uint64_t)i);
+    const uint64_t r = splitmix64(seed * 0x100000001B3ull + (uint64_t)(offset + i));
     const float u = (float)(r >> 40) * (1.0f / 16777216.0f);
     out[i] = u >= p_drop ? 1.f : 0.f;
   }
@@ -351,8 +352,8 @@ int k_dropout_nhwc(fg_ctx* c, const float* x, const float* masks, int64_t stride
   LAUNCH_CHECK(c);
   return FG_OK;
 }
-int k_bernoulli_keep(fg_ctx* c, float* out, int64_t n, uint64_t seed, float p_drop, const uint64_t* seed_dev) {
-  bernoulli_keep_kernel<<<grid_for(n, 256), 256, 0, c->stream>>>(out, n, seed, p_drop, seed_dev);
+int k_bernoulli_keep(fg_ctx* c, float* out, int64_t n, uint64_t seed, float p_drop, const uint64_t* seed_dev, int64_t offset) {
+  bernoulli_keep_kernel<<<grid_for(n, 256), 256, 0, c->stream>>>(out, n, seed, p_drop, seed_dev, offset);
   LAUNCH_CHECK(c);
   return FG_OK;
 }

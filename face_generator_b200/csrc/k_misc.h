@@ -10,8 +10,10 @@ int k_maxpool2_bwd(fg_ctx* c, const float* dp, const float* h, float* dh, int B,
 // y = x * mask * scale; mask element order is the reference's NCHW flattening: masks[b*stride + moff + ch*HW + q]
 int k_dropout_nhwc(fg_ctx* c, const float* x, const float* masks, int64_t stride, int moff, int HW, int C, float scale,
                    float* y, int B);
-// 1 with probability 1-p_drop; seed_dev (optional): effective seed = *seed_dev * 2 + seed
-int k_bernoulli_keep(fg_ctx* c, float* out, int64_t n, uint64_t seed, float p_drop, const uint64_t* seed_dev = nullptr);
+// 1 with probability 1-p_drop; seed_dev (optional): effective seed = *seed_dev * 2 + seed.  out[i] is element
+// offset + i of the stream, so a slice of a longer draw can be drawn on its own.
+int k_bernoulli_keep(fg_ctx* c, float* out, int64_t n, uint64_t seed, float p_drop, const uint64_t* seed_dev = nullptr,
+                     int64_t offset = 0);
 // channel padding around the tensor-core kernels (layers with a narrow output side)
 int k_pad_split(fg_ctx* c, const float* src, float* hi, float* lo, int64_t P, int Cs, int Cp);       // [P][Cs] -> TF32 hi/lo [P][Cp]
 int k_compact_bias(fg_ctx* c, const float* src, const float* bias, float* dst, int64_t P, int Cs, int Cp);

@@ -19,6 +19,8 @@
 #include "fg_internal.h"
 #include "k_conv_tc.h"
 #include "k_misc.h"
+#include "k_rng.cuh"
+#include "k_scale.cuh"
 
 namespace {
 bool c2f_size_ok(int S) { return S == 16 || S == 32 || S == 64; }
@@ -40,6 +42,7 @@ struct fg_c2f {
   int64_t Gca[4] = {0, 0, 0, 0}, Dca[4] = {0, 0, 0, 0}, Da5 = 0, DL2W = 0, DL2b = 0;
   ConvL Gc[5], Dc[4], DL1;
   const char* D_L2_timer = "";
+  const char *t_refine_prep = "", *t_refine_pick = "";  // fg_c2f_refine's own kernels
   int G_pack_impl = -1, D_pack_impl = -1;
   float *G_x = nullptr, *G_z[5] = {}, *G_h[4] = {};
   float *D_x = nullptr, *D_cond = nullptr, *D_z[4] = {}, *D_h[4] = {}, *D_p2 = nullptr, *D_p4 = nullptr, *D_d4 = nullptr;
@@ -117,6 +120,8 @@ void make_layouts(fg_c2f* n) {
     L.b_off = o; o += 512;
     L.tf = timer_name(n, "D.L1.fwd"); L.td = timer_name(n, "D.L1.dgrad"); L.tw = timer_name(n, "D.L1.wgrad");
     n->D_L2_timer = timer_name(n, "D.L2.fwd");
+  n->t_refine_prep = timer_name(n, "refine_prep");
+  n->t_refine_pick = timer_name(n, "refine_pick");
     n->Da5 = o; o += 1;
     n->DL2W = o; o += 512;
     n->DL2b = o; o += 1;
@@ -196,12 +201,11 @@ int pack_D(fg_c2f* n) {
   return FG_OK;
 }
 
-// noise [B][1][S][S] and cond [B][C][S][S] are NCHW device pointers; the diff lands in G_z[4] (NHWC)
-int G_forward(fg_c2f* n, const float* noise, const float* cond, int B) {
+// G on the joined NHWC input already in G_x (nn.JoinTable order: the noise channel, then the C condition channels);
+// the diff lands in G_z[4] (NHWC)
+int G_forward_joined(fg_c2f* n, int B) {
   fg_ctx* c = n->c;
-  FG_REQUIRE(B >= 1 && B <= n->maxB, "c2f G forward: batch %d out of range [1,%d]", B, n->maxB);
   FG_TRY(pack_G(n));
-  FG_TRY(k_join_to_nhwc(c, noise, cond, n->G_x, B, n->C, n->HW));
   const float* cur = n->G_x;
   for (int i = 0; i < 5; ++i) {
     FG_TRY(convl_fwd(n, n->Gc[i], cur, n->net.PG, n->G_z[i], B));
@@ -213,6 +217,13 @@ int G_forward(fg_c2f* n, const float* noise, const float* cond, int B) {
   n->G_B = B;
   n->G_valid = true;
   return FG_OK;
+}
+// noise [B][1][S][S] and cond [B][C][S][S] are NCHW device pointers; the diff lands in G_z[4] (NHWC)
+int G_forward(fg_c2f* n, const float* noise, const float* cond, int B) {
+  FG_REQUIRE(B >= 1 && B <= n->maxB, "c2f G forward: batch %d out of range [1,%d]", B, n->maxB);
+  FG_TRY(pack_G(n));
+  FG_TRY(k_join_to_nhwc(n->c, noise, cond, n->G_x, B, n->C, n->HW));
+  return G_forward_joined(n, B);
 }
 // ddiff: NHWC [B][S][S][C]; accumulates into gG
 int G_backward(fg_c2f* n, const float* ddiff) {
@@ -408,6 +419,80 @@ int run_train_step(fg_c2f* n, const fg_hyper* h, int B, const float* rd, const f
       [&]() { return train_step(n, h, B, nD, nG, rd, cd, nd, cg, ng, md, mg, feed); }, true, nD, nG));
   return pair_step_stats(n->c, n->net, stats);
 }
+
+// ---- fg_c2f_refine: sample.lua:176-214 c2f() around the G and D forwards ----------------------------------------
+constexpr int kRefineThreads = 256;
+// The input side of one chunk, one CTA per base image i (global image i0 + i):
+//   up        = image.scale(image i, S, S), from the image staged in shared memory (C*in*in floats, <= 48 KB)
+//   G_x       [r][p] = {noise, up[0..C)} for the chunk rows r = i*tries + t (NHWC, nn.JoinTable(2,2) order), noise =
+//             noise[r*S*S + p] (the caller's, offset to the chunk) or element ((i0+i)*tries + t)*S*S + p of the uniform
+//             stream noise_seed (fg_noise_uniform's formula, so the draw does not depend on the chunking)
+//   D_cond    [r][p][ch] = up[ch][p]  (D's condition, NHWC)
+//   up_out    [i][ch][p] = up[ch][p]  (NCHW, for the final add)
+__global__ void __launch_bounds__(kRefineThreads) refine_prep_kernel(const float* __restrict__ images, int C, int in, int S,
+                                                                     int tries, int64_t i0, const float* __restrict__ noise,
+                                                                     uint64_t noise_seed, float* __restrict__ G_x,
+                                                                     float* __restrict__ D_cond, float* __restrict__ up_out) {
+  extern __shared__ float img_s[];
+  const int i = blockIdx.x, HW = S * S, plane = in * in, n_in = C * plane;
+  const float* src = images + (int64_t)i * n_in;
+  for (int k = threadIdx.x; k < n_in; k += blockDim.x) img_s[k] = src[k];
+  __syncthreads();
+  for (int p = threadIdx.x; p < HW; p += blockDim.x) {
+    const int y = p / S, x = p - y * S;
+    float up[3];
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+      if (ch < C) {
+        up[ch] = scale_pixel(PlaneSrc{img_s + ch * plane, in}, y, x, in, in, S, S);
+        up_out[((int64_t)i * C + ch) * HW + p] = up[ch];
+      }
+    }
+    for (int t = 0; t < tries; ++t) {
+      const int64_t r = (int64_t)i * tries + t, e = r * HW + p;
+      const float z = noise ? noise[e] : uniform_pm1_at(noise_seed, (uint64_t)(((i0 + i) * tries + t) * HW + p));
+      float* gx = G_x + e * (C + 1);
+      float* dc = D_cond + e * C;
+      gx[0] = z;
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) {
+        if (ch < C) {
+          gx[1 + ch] = up[ch];
+          dc[ch] = up[ch];
+        }
+      }
+    }
+  }
+}
+// The output side, one CTA per base image i: pick = the first try with the largest prediction (the strict > of
+// sample.lua:201-207, so a NaN wins only at t = 0), out[i] = up[i] + diff[i*tries + pick] (NCHW; diff is G's NHWC
+// output, transposed in the same pass).
+__global__ void __launch_bounds__(kRefineThreads) refine_pick_kernel(const float* __restrict__ pred, const float* __restrict__ diff,
+                                                                     const float* __restrict__ up, int C, int HW, int tries,
+                                                                     float* __restrict__ out, int32_t* __restrict__ pick_out) {
+  __shared__ int pick_s;
+  const int i = blockIdx.x;
+  if (threadIdx.x == 0) {
+    const float* pr = pred + (int64_t)i * tries;
+    int best = 0;
+    float m = pr[0];
+    for (int t = 1; t < tries; ++t) {
+      if (pr[t] > m) {
+        m = pr[t];
+        best = t;
+      }
+    }
+    pick_s = best;
+    if (pick_out) pick_out[i] = best;
+  }
+  __syncthreads();
+  const int n = C * HW;
+  const float* d = diff + ((int64_t)i * tries + pick_s) * n;
+  for (int k = threadIdx.x; k < n; k += blockDim.x) {
+    const int ch = k / HW, p = k - ch * HW;
+    out[(int64_t)i * n + k] = up[(int64_t)i * n + k] + d[(int64_t)p * C + ch];
+  }
+}
 }  // namespace
 
 #define ENTER(n)                                         \
@@ -578,6 +663,61 @@ int fg_c2f_parzen_dist(fg_c2f* n, const float* noise, const float* coarse, const
   FG_TRY(k_nchw_to_nhwc(c, fd, n->in_d, 1, n->C, n->HW));
   int32_t idx = 0;
   return fg_nearest(c, n->in_d, 1, n->io, K, (int)img, &idx, dist_out);
+}
+
+// sample.lua:176-214 c2f(images, G, D, fineSize), `chunk` base images (chunk * tries rows of G and D) per pass; see
+// fg_b200.h.  Host inputs and outputs are staged through the net's buffers:
+//   gb    the chunk's images (C*in*in <= 256*S*S floats per image)     in_c  the caller's noise rows
+//   in_a  up (NCHW)      io  out on its way to the host      in_e  pick on its way to the host (int32 storage)
+// Nothing synchronises per chunk: host copies are ordered on the stream behind the kernels that fill their source.
+int fg_c2f_refine(fg_c2f* n, const float* images, int64_t N, int in_size, int tries, int chunk, int training, const float* noise,
+                  const float* masks, uint64_t seed, float* out, int32_t* pick_out, float* pred_out) {
+  ENTER(n);
+  FG_REQUIRE(images && out && N >= 1, "fg_c2f_refine: need images, out and N >= 1");
+  FG_REQUIRE(tries >= 1 && chunk >= 1 && (int64_t)chunk * tries <= n->maxB,
+             "fg_c2f_refine: chunk %d x tries %d rows must be in [1, max_batch %d]", chunk, tries, n->maxB);
+  FG_REQUIRE(in_size >= 1 && in_size <= 64, "fg_c2f_refine: input size %d outside [1, 64]", in_size);
+  fg_ctx* c = n->c;
+  const int C = n->C, HW = n->HW;
+  const size_t img_in = (size_t)C * in_size * in_size, img = (size_t)C * HW, mask = n->mask;
+  const size_t smem = sizeof(float) * img_in;  // <= 3 x 64 x 64 floats: the default 48 KB
+  const bool out_dev = fg_is_dev(out), pick_dev = pick_out && fg_is_dev(pick_out);
+  const bool pred_dev = pred_out && fg_is_dev(pred_out);
+  for (int64_t s0 = 0; s0 < N; s0 += chunk) {
+    const int b = (int)std::min<int64_t>(chunk, N - s0), R = b * tries;
+    const int64_t r0 = s0 * tries;
+    const float *imd, *nz = nullptr;
+    FG_TRY(fg_to_dev(c, images + s0 * img_in, b * img_in, n->gb, &imd));
+    if (noise) FG_TRY(fg_to_dev(c, noise + r0 * HW, (size_t)R * HW, n->in_c, &nz));
+    {
+      ScopedTimer tm(c, n->t_refine_prep);
+      refine_prep_kernel<<<b, kRefineThreads, smem, c->stream>>>(imd, C, in_size, n->S, tries, s0, nz, 2 * seed, n->G_x, n->D_cond,
+                                                                 n->in_a);
+      LAUNCH_CHECK(c);
+    }
+    FG_TRY(G_forward_joined(n, R));
+    if (training) {
+      if (masks)
+        FG_CUDA(cudaMemcpyAsync(n->D_masks, masks + r0 * mask, sizeof(float) * R * mask, cudaMemcpyDefault, c->stream));
+      else
+        FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)R * mask, 2 * seed + 1, 0.5f, nullptr, r0 * (int64_t)mask));
+    }
+    FG_TRY(D_forward(n, n->G_z[4], n->D_cond, R, training != 0, 0.5f));
+    FG_TRY(k_sigmoid_fwd(c, n->D_logit, n->D_out, R));
+    float* od = out_dev ? out + s0 * img : n->io;
+    int32_t* pk = pick_dev ? pick_out + s0 : (pick_out ? reinterpret_cast<int32_t*>(n->in_e) : nullptr);
+    {
+      ScopedTimer tm(c, n->t_refine_pick);
+      refine_pick_kernel<<<b, kRefineThreads, 0, c->stream>>>(n->D_out, n->G_z[4], n->in_a, C, HW, tries, od, pk);
+      LAUNCH_CHECK(c);
+    }
+    if (!out_dev) FG_CUDA(cudaMemcpyAsync(out + s0 * img, od, sizeof(float) * b * img, cudaMemcpyDeviceToHost, c->stream));
+    if (pick_out && !pick_dev)
+      FG_CUDA(cudaMemcpyAsync(pick_out + s0, pk, sizeof(int32_t) * b, cudaMemcpyDeviceToHost, c->stream));
+    if (pred_out) FG_CUDA(cudaMemcpyAsync(pred_out + r0, n->D_out, sizeof(float) * R, cudaMemcpyDefault, c->stream));
+  }
+  if (!out_dev || (pick_out && !pick_dev) || (pred_out && !pred_dev)) FG_CUDA(cudaStreamSynchronize(c->stream));
+  return FG_OK;
 }
 
 // data parallel: rank 0's c2f parameters, optimizer moments, step counters and accuracy history (the nets have no

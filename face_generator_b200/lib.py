@@ -144,6 +144,8 @@ SYMBOLS = {
     "fg_nearest": (_I, [_P, _P, _I, _P, _L, _I, _P, _P]),
     "fg_dataset_nearest": (_I, [_P, _P, _I, _P, _P]),
     "fg_c2f_parzen_dist": (_I, [_P, _P, _P, _P, _I, _P]),
+    "fg_image_scale": (_I, [_P, _P, _L, _I, _I, _I, _I, _I, _P]),
+    "fg_c2f_refine": (_I, [_P, _P, _L, _I, _I, _I, _I, _P, _P, _U64, _P, _P, _P]),
     "fg_t7_open": (_I, [C.c_char_p, C.POINTER(_P)]),
     "fg_t7_close": (_I, [_P]),
     "fg_t7_kind": (_I, [_P, C.c_char_p]),

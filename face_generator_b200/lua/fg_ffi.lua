@@ -111,6 +111,9 @@ int fg_D_score(fg_ctx* ctx, const float* images, int64_t N, int chunk, int train
 int fg_nearest(fg_ctx* ctx, const float* queries, int Q, const float* cands, int64_t N, int D, int32_t* idx_out, float* dist_out);
 int fg_dataset_nearest(fg_dataset* d, const float* queries, int Q, int32_t* idx_out, float* dist_out);
 int fg_c2f_parzen_dist(fg_c2f* n, const float* noise, const float* coarse, const float* fine, int K, float* dist_out);
+int fg_image_scale(fg_ctx* ctx, const float* src, int64_t N, int C, int Hs, int Ws, int Ho, int Wo, float* dst);
+int fg_c2f_refine(fg_c2f* n, const float* images, int64_t N, int in_size, int tries, int chunk, int training,
+                  const float* noise, const float* masks, uint64_t seed, float* out, int32_t* pick_out, float* pred_out);
 typedef struct fg_t7 fg_t7;
 int fg_t7_open(const char* path, fg_t7** out);
 int fg_t7_close(fg_t7* f);

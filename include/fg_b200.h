@@ -414,6 +414,24 @@ int fg_dataset_nearest(fg_dataset* d, const float* queries, int Q, int32_t* idx_
 /* one sample of adversarial_c2f.lua:305-325 approxParzen: min_k || G({noise_k, coarse}) + coarse - fine ||,
  * noise [K][1][S][S], coarse / fine [C][S][S]                                                       */
 int fg_c2f_parzen_dist(fg_c2f* n, const float* noise, const float* coarse, const float* fine, int K, float* dist_out);
+/* image.scale(x, Wo, Ho) (default 'bilinear' mode) on fp32 NCHW: src [N][C][Hs][Ws] -> dst [N][C][Ho][Wo],
+ * host or device; 1 <= Hs, Ws, Ho, Wo <= 256                                                        */
+int fg_image_scale(fg_ctx* ctx, const float* src, int64_t N, int C, int Hs, int Ws, int Ho, int Wo, float* dst);
+/* sample.lua:176-214 c2f(images, G, D, fineSize) on the net's fine size S (the coarse-to-fine pyramid step):
+ *   up[i]     = image.scale(images[i], S, S)                     (a copy when in_size == S)
+ *   diff[i,t] = G({noise[i,t], up[i]}),  pred[i,t] = D({diff[i,t], up[i]})   t < tries
+ *   pick[i]   = the first t with the largest float32 pred (strict >, as the reference's loop; a NaN never
+ *               wins except at t = 0)
+ *   out[i]    = up[i] + diff[i, pick[i]]                          (no clamp, as torch.add)
+ * images [N][C][in_size][in_size], 1 <= in_size <= 64; out [N][C][S][S]; pick_out [N] (0-based) and
+ * pred_out [N][tries] may be NULL; every buffer host or device.  `chunk` images (chunk*tries rows <=
+ * max_batch) per pass.  training = 1 is what sample.lua does (D's dropout live), 0 = evaluate().
+ * noise [N][tries][1][S][S] or NULL = fg_noise_uniform(ctx, 2*seed, N*tries*S*S) (same element order);
+ * masks [N][tries][fg_c2f_mask_per_sample_sized(S)] or NULL = fg_dropout_mask(.., N*tries*mask, 0.5,
+ * 2*seed+1).  Both streams are indexed by the global row i*tries+t and neither net has a BatchNorm
+ * layer, so the result does not depend on `chunk`.  Argument errors return before any launch.      */
+int fg_c2f_refine(fg_c2f* n, const float* images, int64_t N, int in_size, int tries, int chunk, int training,
+                  const float* noise, const float* masks, uint64_t seed, float* out, int32_t* pick_out, float* pred_out);
 
 /* ---- the denoising autoencoders of train_denoiser.lua (train.lua --denoise) ------------------ */
 /* AE = WhiteNoise(0, noise_std) + DECODER, AE2 = a second DECODER fed with AE's output
