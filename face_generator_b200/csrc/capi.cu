@@ -70,6 +70,26 @@ int64_t debug_tensor_copy(fg_ctx* c, const char* what, const DebugTensor* ents, 
   return -1;
 }
 
+namespace {
+// d_iters D iterations + g_iters G iterations of the loop body on inputs stacked per iteration, for the entry `what`
+int train_step_iters(fg_ctx* c, const char* what, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,
+                     const float* noise_D, const float* noise_G, const float* masks_D, const float* masks_G, uint64_t seed,
+                     fg_step_stats* stats) {
+  ENTER(c);
+  FG_TRY(step_check(c, what, B, d_iters, g_iters, h && real && noise_D && noise_G));
+  const size_t nd = d_iters, ng = g_iters, Bh = B / 2, M = c->maxB, img = (size_t)c->C * 1024;
+  IterStage& s = c->iter_stage;
+  const float *r, *zd, *zg, *md, *mg;
+  FG_TRY(s.in(c, c->allocs, 0, real, nd * Bh * img, nd * M / 2 * img, &r));
+  FG_TRY(s.in(c, c->allocs, 1, noise_D, nd * Bh * kNoiseDim, nd * M / 2 * kNoiseDim, &zd));
+  FG_TRY(s.in(c, c->allocs, 2, noise_G, ng * B * kNoiseDim, ng * M * kNoiseDim, &zg));
+  FG_TRY(s.in(c, c->allocs, 3, masks_D, nd * B * kMaskPerSample, nd * M * kMaskPerSample, &md));
+  FG_TRY(s.in(c, c->allocs, 4, masks_G, ng * B * kMaskPerSample, ng * M * kMaskPerSample, &mg));
+  NetStep st(c, h, B, r, zd, zg);
+  return pair_train_step(st, d_iters, g_iters, md, mg, seed, {r, zd, zg, md, mg, nullptr}, nullptr, stats);
+}
+}  // namespace
+
 extern "C" {
 
 const char* fg_version(void) { return "fg_b200 0.1 (sm_90a)"; }
@@ -427,38 +447,13 @@ int fg_adam_step(fg_ctx* c, float* p, const float* g, float* m, float* v, int64_
 // ---- L-step -----------------------------------------------------------------------------------------
 int fg_train_step(fg_ctx* c, const fg_hyper* h, int B, const float* real, const float* noise_D, const float* noise_G,
                   const float* masks_D, const float* masks_G, uint64_t seed, fg_step_stats* stats) {
-  ENTER(c);
-  FG_REQUIRE(h && real && noise_D && noise_G, "fg_train_step: null input");
-  FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= c->maxB, "fg_train_step: batch %d must be even, >= 4 and <= max_batch %d", B,
-             c->maxB);
-  const float *r, *nd, *ng, *md = nullptr, *mg = nullptr;
-  FG_TRY(fg_to_dev(c, real, (size_t)(B / 2) * c->C * 1024, c->in_real, &r));
-  FG_TRY(fg_to_dev(c, noise_D, (size_t)(B / 2) * kNoiseDim, c->in_noiseD, &nd));
-  FG_TRY(fg_to_dev(c, noise_G, (size_t)B * kNoiseDim, c->in_noiseG, &ng));
-  if (masks_D) FG_TRY(fg_to_dev(c, masks_D, (size_t)B * kMaskPerSample, c->in_masksD, &md));
-  if (masks_G) FG_TRY(fg_to_dev(c, masks_G, (size_t)B * kMaskPerSample, c->in_masksG, &mg));
-  FG_TRY(net_train_step(c, h, B, r, nd, ng, md, mg, seed, true));
-  return pair_step_stats(c, c->net, stats);
+  return train_step_iters(c, "fg_train_step", h, B, 1, 1, real, noise_D, noise_G, masks_D, masks_G, seed, stats);
 }
-// d_iters D iterations + g_iters G iterations of the loop body on inputs stacked per iteration
 int fg_train_step_iters(fg_ctx* c, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,
                         const float* noise_D, const float* noise_G, const float* masks_D, const float* masks_G, uint64_t seed,
                         fg_step_stats* stats) {
-  ENTER(c);
-  FG_TRY(iters_check(d_iters, g_iters, "fg_train_step_iters"));
-  FG_REQUIRE(h && real && noise_D && noise_G, "fg_train_step_iters: null input");
-  FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= c->maxB, "fg_train_step_iters: batch %d must be even, >= 4 and <= max_batch %d", B,
-             c->maxB);
-  const size_t nd = d_iters, ng = g_iters, Bh = B / 2, M = c->maxB, img = (size_t)c->C * 1024;
-  IterStage& s = c->iter_stage;
-  const float *r, *zd, *zg, *md, *mg;
-  FG_TRY(s.in(c, c->allocs, 0, real, nd * Bh * img, nd * M / 2 * img, &r));
-  FG_TRY(s.in(c, c->allocs, 1, noise_D, nd * Bh * kNoiseDim, nd * M / 2 * kNoiseDim, &zd));
-  FG_TRY(s.in(c, c->allocs, 2, noise_G, ng * B * kNoiseDim, ng * M * kNoiseDim, &zg));
-  FG_TRY(s.in(c, c->allocs, 3, masks_D, nd * B * kMaskPerSample, nd * M * kMaskPerSample, &md));
-  FG_TRY(s.in(c, c->allocs, 4, masks_G, ng * B * kMaskPerSample, ng * M * kMaskPerSample, &mg));
-  FG_TRY(net_train_step_iters(c, h, B, d_iters, g_iters, r, zd, zg, md, mg, seed, nullptr, nullptr));
-  return pair_step_stats(c, c->net, stats);
+  return train_step_iters(c, "fg_train_step_iters", h, B, d_iters, g_iters, real, noise_D, noise_G, masks_D, masks_G, seed,
+                          stats);
 }
 
 int fg_sample(fg_ctx* c, const float* noise, int N, int chunk, float* images_out) {
@@ -529,11 +524,8 @@ int64_t fg_debug_tensor(fg_ctx* c, const char* name, float* dst, int64_t max_ele
       {"D.z1", c->D_z[0], 65536, db}, {"D.z2", c->D_z[1], 32768, db}, {"D.z3", c->D_z[2], 16384, db},
       {"D.z4", c->D_z[3], 8192, db}, {"D.p4", c->D_p[3], 2048, db}, {"D.logit", c->D_logit, 1, db},
       {"D.out", c->D_out, 1, db}, {"D.dx", c->D_dx, 1024 * c->C, db}, {"D.masks", c->D_masks, kMaskPerSample, db},
-      {"D.zl1", c->D_zl1, 512, db}, {"D.zl2", c->D_zl2, 512, db},
-      {"Dstep.z1", c->keep_D[0], 65536, c->keep_B}, {"Dstep.z2", c->keep_D[1], 32768, c->keep_B},
-      {"Dstep.z3", c->keep_D[2], 16384, c->keep_B}, {"Dstep.z4", c->keep_D[3], 8192, c->keep_B},
-      {"Dstep.zl1", c->keep_D[4], 512, c->keep_B}, {"Dstep.zl2", c->keep_D[5], 512, c->keep_B},
-      {"Dstep.logit", c->keep_D[6], 1, c->keep_B}, {"Dstep.out", c->keep_D[7], 1, c->keep_B}};
+      {"D.zl1", c->D_zl1, 512, db}, {"D.zl2", c->D_zl2, 512, db}};
+  pair_keep_rows(c->net, ents);
   gen_debug_rows(c->G, ents);
   return debug_tensor_copy(c, "fg_debug_tensor", ents.data(), ents.size(), name, dst, max_elems);
 }

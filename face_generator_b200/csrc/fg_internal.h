@@ -112,6 +112,16 @@ struct NetPair {
   bool G_packed = false, D_packed = false;  // the weight packs match the parameters
   std::vector<StepGraph> graphs;
   const char* optim_timer[2] = {nullptr, nullptr};  // ScopedTimer names of the G / D optimizer update (none: untimed)
+  // option "debug_keep" (tests): the D iteration's tensors that the G iteration's D forward overwrites, copied by the
+  // loop body (pair_train_step) and read back as the "Dstep.*" debug tensors.  The trainer fills the table at alloc.
+  struct Keep {
+    const char* name;       // "Dstep.<tensor>"
+    const float* src;
+    int64_t per;            // floats per sample
+    float* copy = nullptr;  // maxB * per floats, allocated by the first kept step
+  };
+  std::vector<Keep> keep;
+  int keep_B = 0;
 };
 
 // ---- layer types (dispatch in convl.cu) ------------------------------------------------------------------
@@ -293,8 +303,8 @@ struct fg_ctx {
   float* io_dev = nullptr;  // device staging for NCHW images / misc
   size_t io_dev_elems = 0;
   float* io_dev2 = nullptr;
-  float *in_real = nullptr, *in_noiseD = nullptr, *in_noiseG = nullptr, *in_masksD = nullptr, *in_masksG = nullptr;
-  IterStage iter_stage;  // the stacked inputs of fg_train_step_iters / fg_train_step_dataset_iters
+  float *in_noiseD = nullptr, *in_noiseG = nullptr;
+  IterStage iter_stage;  // the inputs of the host-fed and device-fed train steps, stacked per iteration
   float* scratch[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   size_t scratch_elems[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   // data parallel
@@ -320,11 +330,9 @@ struct fg_ctx {
   uint64_t* seed_dev = nullptr;
   cudaStream_t comm_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  // debug (tests): "debug_keep" = 1 keeps a copy of the D step's pre-activations of fg_train_step, which the G
-  // step's D forward overwrites (the strict gradient-parity tests read PReLU branch decisions from them)
+  // debug (tests): "debug_keep" = 1 keeps a copy of the D step's pre-activations of every train step (NetPair::keep),
+  // which the G step's D forward overwrites (the strict gradient-parity tests read PReLU branch decisions from them)
   bool debug_keep = false;
-  int keep_B = 0;
-  float* keep_D[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // D_z[0..3], D_zl1, D_zl2, D_logit, D_out
   // timing
   cudaEvent_t events[16] = {};
   bool timing = false;
@@ -481,17 +489,6 @@ void net_free(fg_ctx* c);
 int net_pack_D(fg_ctx* c);
 int net_D_forward(fg_ctx* c, const float* x_nhwc, int B, bool training, const fg_hyper* h);  // masks in c->D_masks
 int net_D_backward(fg_ctx* c, const float* dlogit_dev, bool want_wgrad, bool want_dx);       // -> c->D_dx (NHWC)
-int net_train_step(fg_ctx* c, const fg_hyper* h, int B, const float* real_nchw_dev, const float* noiseD_dev,
-                   const float* noiseG_dev, const float* masksD_dev, const float* masksG_dev, uint64_t seed,
-                   bool allow_graph = false);
-// nd D iterations + ng G iterations on inputs stacked per iteration (fg_train_step_iters).  feed (may be empty) runs
-// first inside the step, after the stream roots are set: the device-fed step draws its inputs there; feed_key names
-// what the feed reads (the dataset), for the graph key.
-int net_train_step_iters(fg_ctx* c, const fg_hyper* h, int B, int nd, int ng, const float* real, const float* noiseD,
-                         const float* noiseG, const float* masksD, const float* masksG, uint64_t seed,
-                         const std::function<int()>& feed, const void* feed_key);
-// 1 <= nd, ng <= kMaxIters, else FG_ERR_UNSUPPORTED
-int iters_check(int nd, int ng, const char* what);
 int net_allreduce(fg_ctx* c, float* buf, int64_t n);
 int net_broadcast(fg_ctx* c, void* buf, size_t bytes);  // rank 0 -> all (dp.cu)
 int net_group(bool start);                                // ncclGroupStart / ncclGroupEnd
@@ -522,15 +519,62 @@ int pair_get_adam_state(fg_ctx* c, const NetPair& p, int net, float* m, float* v
 int pair_set_bn_state(fg_ctx* c, NetPair& p, const float* src);
 int pair_get_bn_state(fg_ctx* c, const NetPair& p, float* dst);
 // Runs `body` (launches on c->stream that read their seed from c->seed_dev) as a train step of pair p: eagerly, or as a
-// captured CUDA graph keyed on B, *h, `inputs`, the stream, the communicator, graph_epoch, pack_key and the iteration
-// counts nd / ng
-// (hyper, hyper_bytes): the hyper-parameter struct of the step, keyed by its bytes
+// captured CUDA graph keyed on B, the hyper-parameter struct's bytes, `inputs`, the stream, the communicator,
+// graph_epoch, pack_key and the iteration counts nd / ng
 int net_graph_run(fg_ctx* c, NetPair& p, int B, const void* hyper, size_t hyper_bytes, std::initializer_list<const void*> inputs,
-                  uint64_t seed, const std::function<int()>& body, bool allow_graph, int nd = 1, int ng = 1);
-inline int net_graph_run(fg_ctx* c, NetPair& p, int B, const fg_hyper* h, std::initializer_list<const void*> inputs, uint64_t seed,
-                         const std::function<int()>& body, bool allow_graph, int nd = 1, int ng = 1) {
-  return net_graph_run(c, p, B, h, sizeof(*h), inputs, seed, body, allow_graph, nd, ng);
-}
+                  uint64_t seed, const std::function<int()>& body, int nd = 1, int ng = 1);
+
+// ---- the adversarial.lua loop body (adversarial_c2f.lua for the coarse-to-fine nets), netpair.cu ----
+// the checks of a train-step entry `what`, made before it stages anything: the iteration counts (1 <= nd, ng <=
+// kMaxIters, else FG_ERR_UNSUPPORTED), the feeding dataset d when `fed`, the inputs (`inputs`: none is null) and the batch
+int step_check(fg_ctx* c, const char* what, int B, int nd, int ng, bool inputs, const fg_dataset* d = nullptr, bool fed = false);
+// What one trainer contributes to the loop body: the calls on its nets and its D's output buffers.  It holds its own
+// inputs (device pointers, stacked per iteration).
+struct StepNets {
+  StepNets(fg_ctx* c, NetPair& pair, const fg_hyper* h, int B, float* logit, float* out, float* dlogit, float* masks,
+           int64_t mask, bool gate, bool overlap)
+      : c(c), pair(&pair), h(h), B(B), logit(logit), out(out), dlogit(dlogit), masks(masks), mask(mask), gate(gate),
+        overlap(overlap) {}
+  fg_ctx* c;
+  NetPair* pair;
+  const fg_hyper* h;
+  int B;
+  float *logit, *out, *dlogit;  // D's output buffers
+  float* masks;                 // D's dropout keep flags, `mask` floats per sample
+  int64_t mask;
+  bool gate;     // the accuracy gate decides whether D trains; false: it always does (adversarial_c2f.lua)
+  bool overlap;  // option dp_overlap may run D's all-reduce, gate and optimizer next to the following G forward
+  // G in training mode: the B/2 fakes of D iteration j (d_iter), or the B samples of G iteration j; with the
+  // condition rows D reads next, if any
+  virtual int g_forward(int j, bool d_iter) = 0;
+  virtual int d_input(int j) = 0;                              // D's input of D iteration j: the real half, then the fakes
+  virtual int draw_masks(int kind, const uint64_t* root) = 0;  // D's keep flags of kind 1 (D iteration) or 2 (G iteration)
+  virtual int d_forward(bool on_g) = 0;                        // D in training mode on its input, or on G's output
+  virtual int d_backward(bool want_wgrad, bool want_dx) = 0;   // from dlogit
+  virtual int g_backward() = 0;                                // from D's input gradient
+};
+// nd D iterations, then ng G iterations, then the statistics to `stats` (may be null).  masksD / masksG (may be null:
+// drawn from the stream root of each iteration) are stacked per iteration; feed (may be null) runs first inside the
+// step, after the stream roots are set: a device-fed step draws its inputs there.  The step is keyed (net_graph_run) on
+// `inputs`, which name every input pointer and what the feed reads.
+int pair_train_step(StepNets& s, int nd, int ng, const float* masksD, const float* masksG, uint64_t seed,
+                    std::initializer_list<const void*> inputs, const std::function<int()>* feed, fg_step_stats* stats);
+// the "Dstep.*" rows of a debug-tensor table
+struct DebugTensor;
+void pair_keep_rows(const NetPair& p, std::vector<DebugTensor>& ents);
+
+// the 32x32 nets' part of the loop body (nets.cu): real [B/2][C][32][32], noiseD [B/2][100], noiseG [B][100] per
+// iteration
+struct NetStep final : StepNets {
+  const float *real, *noiseD, *noiseG;
+  NetStep(fg_ctx* c, const fg_hyper* h, int B, const float* real, const float* noiseD, const float* noiseG);
+  int g_forward(int j, bool d_iter) override;
+  int d_input(int j) override;
+  int draw_masks(int kind, const uint64_t* root) override;
+  int d_forward(bool on_g) override;
+  int d_backward(bool want_wgrad, bool want_dx) override;
+  int g_backward() override;
+};
 
 // ---- nets_ae.cu: the elementwise layers of the autoencoder (nn.ReLU, nn.Tanh + nn.Dropout, nn.AbsCriterion).  Each is
 // a producer in AmaxInto's sense (convl.h). ----

@@ -1,7 +1,7 @@
 // The trainable state of a G/D pair (NetPair, fg_internal.h) and what every train step does with it: allocation,
 // zeroing and all-reducing the gradients, the accuracy gate and optimizer, the data-parallel broadcast, the statistics
-// mirror, the C ABI's set / get bodies and the CUDA-graph replay of the step.  Shared by the 32x32 nets (nets.cu), the
-// coarse-to-fine nets (nets_c2f.cu) and the --scale 16 nets (nets_s16.cu).
+// mirror, the C ABI's set / get bodies, the CUDA-graph replay of the step and the adversarial.lua loop body itself.
+// Shared by the 32x32 nets (nets.cu), the coarse-to-fine nets (nets_c2f.cu) and the --scale 16 nets (nets_s16.cu).
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -68,6 +68,10 @@ void pair_free(NetPair& p) {
   pair_clear_graphs(p);
   if (p.hstats) cudaFreeHost(p.hstats);
   p.hstats = nullptr;
+  for (NetPair::Keep& k : p.keep) {
+    if (k.copy) cudaFree(k.copy);
+    k.copy = nullptr;
+  }
 }
 
 int pair_zero_grads(fg_ctx* c, NetPair& p, int net) {
@@ -115,11 +119,14 @@ int IterStage::in(fg_ctx* c, std::vector<void*>& allocs, int k, const float* q, 
   return fg_to_dev(c, q, n, p[k], out);
 }
 
-int iters_check(int nd, int ng, const char* what) {
+int step_check(fg_ctx* c, const char* what, int B, int nd, int ng, bool inputs, const fg_dataset* d, bool fed) {
   if (nd < 1 || nd > kMaxIters || ng < 1 || ng > kMaxIters) {
     fg_set_error("%s: %d D and %d G iterations; each count must lie in [1, %d]", what, nd, ng, kMaxIters);
     return FG_ERR_UNSUPPORTED;
   }
+  if (fed) FG_TRY(dataset_check_feed(d, c, what));
+  FG_REQUIRE(inputs, "%s: null input", what);
+  FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= c->maxB, "%s: batch %d must be even, >= 4 and <= max_batch %d", what, B, c->maxB);
   return FG_OK;
 }
 
@@ -249,10 +256,10 @@ void key_add(std::vector<uint8_t>& k, const T& v) {
 // The packs are marked stale before the capture and after every replay: the captured sequence has to contain the pack
 // kernels whatever the flags said at capture time, and a replayed optimizer step invalidates them again.
 int net_graph_run(fg_ctx* c, NetPair& p, int B, const void* hyper, size_t hyper_bytes, std::initializer_list<const void*> inputs,
-                  uint64_t seed, const std::function<int()>& body, bool allow_graph, int nd, int ng) {
+                  uint64_t seed, const std::function<int()>& body, int nd, int ng) {
   FG_TRY(k_set_u64(c, c->seed_dev, seed));
   static const bool env_off = getenv("FG_GRAPH") && atoi(getenv("FG_GRAPH")) == 0;
-  if (!allow_graph || !c->use_graph || env_off || c->timing || c->debug_keep) return body();
+  if (!c->use_graph || env_off || c->timing || c->debug_keep) return body();
   std::vector<uint8_t> key;
   key_add(key, c->graph_epoch);
   key_add(key, B);
@@ -305,4 +312,117 @@ int net_graph_run(fg_ctx* c, NetPair& p, int B, const void* hyper, size_t hyper_
   c->launches += e->launches;
   p.G_packed = p.D_packed = false;
   return FG_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// The adversarial.lua loop body (:240-288; adversarial_c2f.lua:121-187) on the nets of one trainer: nd D iterations,
+// then ng G iterations.  The dropout masks of iteration j are drawn from the stream root c->seed_dev[j] (k_seed_roots;
+// [0] is the step seed).
+// ---------------------------------------------------------------------------------------------------
+namespace {
+int keep_dstep(fg_ctx* c, NetPair& p, int B) {
+  for (NetPair::Keep& k : p.keep) {
+    if (!k.copy) FG_CUDA(cudaMalloc((void**)&k.copy, sizeof(float) * c->maxB * k.per));
+    FG_CUDA(cudaMemcpyAsync(k.copy, k.src, sizeof(float) * B * k.per, cudaMemcpyDeviceToDevice, c->stream));
+  }
+  p.keep_B = B;
+  return FG_OK;
+}
+
+int step_body(StepNets& s, int nd, int ng, const float* masksD, const float* masksG, const std::function<int()>* feed) {
+  fg_ctx* c = s.c;
+  NetPair& p = *s.pair;
+  const fg_hyper* h = s.h;
+  const int B = s.B, Bh = B / 2;
+  const size_t mask = (size_t)B * s.mask;
+  const float world = (float)c->world;
+  fg_hyper hg = *h;  // the gate's: without the accuracy gate D trains at any accuracy
+  if (!s.gate) hg.D_maxAcc = 1e30f;
+  if (nd > 1 || ng > 1) FG_TRY(k_seed_roots(c, c->seed_dev, std::max(nd, ng)));
+  if (feed) FG_TRY((*feed)());
+  // with dp_overlap, D's gradient all-reduce, gate and optimizer run on the communication stream while the next G
+  // forward (it depends on G's parameters only: the fakes of the next D iteration or the first G iteration's samples)
+  // proceeds on the compute stream; D is joined right after it.  The replicas stay bit-identical: the same reductions
+  // in the same order, only on another stream.
+  const bool overlap = s.overlap && c->world > 1 && c->dp_overlap && !c->timing;
+  bool forked = false;
+  auto g_forward = [&](int j, bool d_iter) -> int {
+    // while the collective is in flight the persistent convolution kernels leave a few SMs to it (FG_DP_RESERVE_SMS)
+    static const int reserve = getenv("FG_DP_RESERVE_SMS") ? atoi(getenv("FG_DP_RESERVE_SMS")) : 0;
+    c->reserve_sms = forked ? reserve : 0;
+    const int r = s.g_forward(j, d_iter);
+    c->reserve_sms = 0;
+    FG_TRY(r);
+    if (forked) FG_CUDA(cudaStreamWaitEvent(c->stream, c->ev_join, 0));
+    forked = false;
+    return FG_OK;
+  };
+  auto masks = [&](const float* given, int j, int kind) -> int {
+    if (given)
+      FG_CUDA(cudaMemcpyAsync(s.masks, given + j * mask, sizeof(float) * mask, cudaMemcpyDeviceToDevice, c->stream));
+    else
+      FG_TRY(s.draw_masks(kind, c->seed_dev + j));
+    return FG_OK;
+  };
+  for (int j = 0; j < nd; ++j) {
+    // ---- D iteration j (adversarial.lua:240-268) ----
+    FG_TRY(g_forward(j, true));  // createImages
+    FG_TRY(s.d_input(j));
+    FG_TRY(masks(masksD, j, 1));
+    FG_TRY(pair_zero_grads(c, p, FG_NET_D));
+    FG_TRY(s.d_forward(false));
+    FG_TRY(k_sigmoid_bce(c, s.logit, s.out, s.dlogit, &p.dstats->loss_D, p.tailD, B, Bh));
+    if (c->debug_keep) FG_TRY(keep_dstep(c, p, B));
+    FG_TRY(s.d_backward(true, false));
+    const bool acc = j > 0;  // conf / trained_D add up over the step's D iterations
+    if (overlap) {
+      if (!c->comm_stream) {
+        FG_CUDA(cudaStreamCreateWithFlags(&c->comm_stream, cudaStreamNonBlocking));
+        FG_CUDA(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
+        FG_CUDA(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
+      }
+      FG_CUDA(cudaEventRecord(c->ev_fork, c->stream));
+      FG_CUDA(cudaStreamWaitEvent(c->comm_stream, c->ev_fork, 0));
+      cudaStream_t compute = c->stream;
+      c->stream = c->comm_stream;
+      int r = pair_allreduce_grads(c, p, FG_NET_D);
+      if (r == FG_OK) r = pair_gate(c, p, FG_NET_D, &hg, B, world, acc);
+      if (r == FG_OK) r = pair_optim(c, p, FG_NET_D, h, 1.0f / world);
+      if (r == FG_OK && cudaEventRecord(c->ev_join, c->comm_stream) != cudaSuccess) r = FG_ERR_CUDA;
+      c->stream = compute;
+      FG_TRY(r);
+      forked = true;
+    } else {
+      FG_TRY(pair_allreduce_grads(c, p, FG_NET_D));
+      FG_TRY(pair_gate(c, p, FG_NET_D, &hg, B, world, acc));
+      FG_TRY(pair_optim(c, p, FG_NET_D, h, 1.0f / world));
+    }
+  }
+  for (int j = 0; j < ng; ++j) {
+    // ---- G iteration j (adversarial.lua:275-288) ----
+    FG_TRY(pair_zero_grads(c, p, FG_NET_G));
+    FG_TRY(g_forward(j, false));
+    FG_TRY(masks(masksG, j, 2));
+    FG_TRY(s.d_forward(true));
+    FG_TRY(k_sigmoid_bce(c, s.logit, s.out, s.dlogit, &p.dstats->loss_G, p.tailG, B, B));
+    FG_TRY(s.d_backward(false, true));  // D's weight grads are discarded by the reference (:209 vs :92)
+    FG_TRY(s.g_backward());
+    FG_TRY(pair_allreduce_grads(c, p, FG_NET_G));
+    FG_TRY(pair_gate(c, p, FG_NET_G, &hg, B, world));
+    FG_TRY(pair_optim(c, p, FG_NET_G, h, 1.0f / world));
+  }
+  FG_CUDA(cudaMemcpyAsync(p.hstats, p.dstats, sizeof(DeviceStats), cudaMemcpyDeviceToHost, c->stream));
+  return FG_OK;
+}
+}  // namespace
+
+int pair_train_step(StepNets& s, int nd, int ng, const float* masksD, const float* masksG, uint64_t seed,
+                    std::initializer_list<const void*> inputs, const std::function<int()>* feed, fg_step_stats* stats) {
+  FG_TRY(net_graph_run(
+      s.c, *s.pair, s.B, s.h, sizeof(*s.h), inputs, seed, [&]() { return step_body(s, nd, ng, masksD, masksG, feed); }, nd, ng));
+  return pair_step_stats(s.c, *s.pair, stats);
+}
+
+void pair_keep_rows(const NetPair& p, std::vector<DebugTensor>& ents) {
+  for (const NetPair::Keep& k : p.keep) ents.push_back({k.name, k.copy, k.per, p.keep_B});
 }

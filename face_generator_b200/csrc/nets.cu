@@ -1,5 +1,5 @@
-// Orchestration of G (models.lua:57-81; gen.cu), D (models.lua:382-416) and the adversarial.lua loop body
-// (adversarial.lua:54-300) on one stream.  Kernels live in k_elem.cu / k_conv_simt.cu / k_conv_tc.cu.
+// Orchestration of G (models.lua:57-81; gen.cu), D (models.lua:382-416) and their part of the adversarial.lua loop body
+// (adversarial.lua:54-300; the loop itself is pair_train_step in netpair.cu) on one stream.  Kernels live in k_elem.cu / k_conv_simt.cu / k_conv_tc.cu.
 #include <algorithm>
 
 #include "convl.h"
@@ -125,11 +125,11 @@ int net_alloc(fg_ctx* c) {
       FG_TRY(convl_alloc(e, *L));
     }
   }
-  FG_TRY(dalloc(c, &c->in_real, B * 1024 * C));
   FG_TRY(dalloc(c, &c->in_noiseD, B * kNoiseDim));
   FG_TRY(dalloc(c, &c->in_noiseG, B * kNoiseDim));
-  FG_TRY(dalloc(c, &c->in_masksD, B * kMaskPerSample));
-  FG_TRY(dalloc(c, &c->in_masksG, B * kMaskPerSample));
+  p.keep = {{"Dstep.z1", c->D_z[0], 65536}, {"Dstep.z2", c->D_z[1], 32768}, {"Dstep.z3", c->D_z[2], 16384},
+            {"Dstep.z4", c->D_z[3], 8192},  {"Dstep.zl1", c->D_zl1, 512},    {"Dstep.zl2", c->D_zl2, 512},
+            {"Dstep.logit", c->D_logit, 1}, {"Dstep.out", c->D_out, 1}};
   FG_CUDA(cudaStreamSynchronize(c->stream));
   return FG_OK;
 }
@@ -250,114 +250,23 @@ int net_D_backward(fg_ctx* c, const float* dlogit, bool want_wgrad, bool want_dx
 }
 
 // ---------------------------------------------------------------------------------------------------
-// the adversarial.lua loop body: nd D iterations (:240-268), then ng G iterations (:275-288)
+// the 32x32 nets in the adversarial.lua loop body (pair_train_step, netpair.cu)
 // ---------------------------------------------------------------------------------------------------
-// the step proper; inputs are stacked per iteration, the dropout masks of iteration j are drawn from the stream root
-// c->seed_dev[j] (k_seed_roots; [0] is the step seed).  feed (may be null) draws the inputs on the device first.
-static int train_step_body(fg_ctx* c, const fg_hyper* h, int B, int nd, int ng, const float* real, const float* noiseD,
-                           const float* noiseG, const float* masksD, const float* masksG, const std::function<int()>* feed) {
-  const int Bh = B / 2, C = c->C;
-  const size_t img = (size_t)C * 1024, mask = (size_t)B * kMaskPerSample;
-  const float world = (float)c->world;
-  if (nd > 1 || ng > 1) FG_TRY(k_seed_roots(c, c->seed_dev, std::max(nd, ng)));
-  if (feed && *feed) FG_TRY((*feed)());
-  // with dp_overlap, D's gradient all-reduce, gate and optimizer run on the communication stream while the next G
-  // forward (it depends on G's parameters only: the fakes of the next D iteration or the first G iteration's samples)
-  // proceeds on the compute stream; D is joined right after it.  The replicas stay bit-identical: the same reductions
-  // in the same order, only on another stream.
-  const bool overlap = c->world > 1 && c->dp_overlap && !c->timing;
-  bool forked = false;
-  auto g_forward = [&](const float* noise, int n) -> int {
-    // while the collective is in flight the persistent convolution kernels leave a few SMs to it (FG_DP_RESERVE_SMS)
-    static const int reserve = getenv("FG_DP_RESERVE_SMS") ? atoi(getenv("FG_DP_RESERVE_SMS")) : 0;
-    c->reserve_sms = forked ? reserve : 0;
-    const int r = gen_forward(c->env, c->G, c->net, noise, n, true);  // G in training mode (nn_utils.lua:52)
-    c->reserve_sms = 0;
-    FG_TRY(r);
-    if (forked) FG_CUDA(cudaStreamWaitEvent(c->stream, c->ev_join, 0));
-    forked = false;
-    return FG_OK;
-  };
-  for (int j = 0; j < nd; ++j) {
-    // ---- D iteration j (adversarial.lua:240-268) ----
-    FG_TRY(g_forward(noiseD + (size_t)j * Bh * kNoiseDim, Bh));  // createImages
-    FG_TRY(k_nchw_to_nhwc(c, real + (size_t)j * Bh * img, c->D_x, Bh, C, 1024));
-    FG_CUDA(cudaMemcpyAsync(c->D_x + Bh * img, c->G.y, sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
-    if (masksD)
-      FG_CUDA(cudaMemcpyAsync(c->D_masks, masksD + j * mask, sizeof(float) * mask, cudaMemcpyDeviceToDevice, c->stream));
-    else
-      FG_TRY(k_masks_generate(c, c->D_masks, B, 1, h->p_spatial, h->p_drop, c->seed_dev + j));
-    FG_TRY(pair_zero_grads(c, c->net, FG_NET_D));
-    FG_TRY(net_D_forward(c, c->D_x, B, true, h));
-    FG_TRY(k_sigmoid_bce(c, c->D_logit, c->D_out, c->D_dlogit, &c->net.dstats->loss_D, c->net.tailD, B, Bh));
-    if (c->debug_keep) {  // tests: the G step's D forward overwrites these
-      const float* src[8] = {c->D_z[0], c->D_z[1], c->D_z[2], c->D_z[3], c->D_zl1, c->D_zl2, c->D_logit, c->D_out};
-      const size_t per[8] = {65536, 32768, 16384, 8192, 512, 512, 1, 1};
-      for (int i = 0; i < 8; ++i) {
-        if (!c->keep_D[i]) FG_TRY(dalloc(c, &c->keep_D[i], (size_t)c->maxB * per[i]));
-        FG_CUDA(cudaMemcpyAsync(c->keep_D[i], src[i], sizeof(float) * B * per[i], cudaMemcpyDeviceToDevice, c->stream));
-      }
-      c->keep_B = B;
-    }
-    FG_TRY(net_D_backward(c, c->D_dlogit, true, false));
-    const bool acc = j > 0;  // conf / trained_D add up over the step's D iterations
-    if (overlap) {
-      if (!c->comm_stream) {
-        FG_CUDA(cudaStreamCreateWithFlags(&c->comm_stream, cudaStreamNonBlocking));
-        FG_CUDA(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
-        FG_CUDA(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
-      }
-      FG_CUDA(cudaEventRecord(c->ev_fork, c->stream));
-      FG_CUDA(cudaStreamWaitEvent(c->comm_stream, c->ev_fork, 0));
-      cudaStream_t compute = c->stream;
-      c->stream = c->comm_stream;
-      int r = pair_allreduce_grads(c, c->net, FG_NET_D);
-      if (r == FG_OK) r = pair_gate(c, c->net, FG_NET_D, h, B, world, acc);
-      if (r == FG_OK) r = pair_optim(c, c->net, FG_NET_D, h, 1.0f / world);
-      if (r == FG_OK && cudaEventRecord(c->ev_join, c->comm_stream) != cudaSuccess) r = FG_ERR_CUDA;
-      c->stream = compute;
-      FG_TRY(r);
-      forked = true;
-    } else {
-      FG_TRY(pair_allreduce_grads(c, c->net, FG_NET_D));
-      FG_TRY(pair_gate(c, c->net, FG_NET_D, h, B, world, acc));
-      FG_TRY(pair_optim(c, c->net, FG_NET_D, h, 1.0f / world));
-    }
-  }
-  for (int j = 0; j < ng; ++j) {
-    // ---- G iteration j (adversarial.lua:275-288) ----
-    FG_TRY(pair_zero_grads(c, c->net, FG_NET_G));
-    FG_TRY(g_forward(noiseG + (size_t)j * B * kNoiseDim, B));
-    if (masksG)
-      FG_CUDA(cudaMemcpyAsync(c->D_masks, masksG + j * mask, sizeof(float) * mask, cudaMemcpyDeviceToDevice, c->stream));
-    else
-      FG_TRY(k_masks_generate(c, c->D_masks, B, 2, h->p_spatial, h->p_drop, c->seed_dev + j));
-    FG_TRY(net_D_forward(c, c->G.y, B, true, h));
-    FG_TRY(k_sigmoid_bce(c, c->D_logit, c->D_out, c->D_dlogit, &c->net.dstats->loss_G, c->net.tailG, B, B));
-    FG_TRY(net_D_backward(c, c->D_dlogit, false, true));  // D's weight grads are discarded by the reference (:209 vs :92)
-    FG_TRY(gen_backward(c->env, c->G, c->net, c->D_dx, nullptr));
-    FG_TRY(pair_allreduce_grads(c, c->net, FG_NET_G));
-    FG_TRY(pair_gate(c, c->net, FG_NET_G, h, B, world));
-    FG_TRY(pair_optim(c, c->net, FG_NET_G, h, 1.0f / world));
-  }
-  FG_CUDA(cudaMemcpyAsync(c->net.hstats, c->net.dstats, sizeof(DeviceStats), cudaMemcpyDeviceToHost, c->stream));
+NetStep::NetStep(fg_ctx* c, const fg_hyper* h, int B, const float* real, const float* noiseD, const float* noiseG)
+    : StepNets(c, c->net, h, B, c->D_logit, c->D_out, c->D_dlogit, c->D_masks, kMaskPerSample, true, true),
+      real(real), noiseD(noiseD), noiseG(noiseG) {}
+int NetStep::g_forward(int j, bool d_iter) {
+  const int n = d_iter ? B / 2 : B;
+  return gen_forward(c->env, c->G, c->net, (d_iter ? noiseD : noiseG) + (size_t)j * n * kNoiseDim, n, true);
+}
+int NetStep::d_input(int j) {
+  const int Bh = B / 2;
+  const size_t img = (size_t)c->C * 1024;
+  FG_TRY(k_nchw_to_nhwc(c, real + (size_t)j * Bh * img, c->D_x, Bh, c->C, 1024));
+  FG_CUDA(cudaMemcpyAsync(c->D_x + Bh * img, c->G.y, sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
   return FG_OK;
 }
-
-int net_train_step(fg_ctx* c, const fg_hyper* h, int B, const float* real, const float* noiseD, const float* noiseG,
-                   const float* masksD, const float* masksG, uint64_t seed, bool allow_graph) {
-  FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= c->maxB, "train step: batch %d must be even, >=4 and <= %d", B, c->maxB);
-  return net_graph_run(
-      c, c->net, B, h, {real, noiseD, noiseG, masksD, masksG}, seed,
-      [&]() { return train_step_body(c, h, B, 1, 1, real, noiseD, noiseG, masksD, masksG, nullptr); }, allow_graph);
-}
-
-int net_train_step_iters(fg_ctx* c, const fg_hyper* h, int B, int nd, int ng, const float* real, const float* noiseD,
-                         const float* noiseG, const float* masksD, const float* masksG, uint64_t seed,
-                         const std::function<int()>& feed, const void* feed_key) {
-  FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= c->maxB, "train step: batch %d must be even, >=4 and <= %d", B, c->maxB);
-  FG_TRY(iters_check(nd, ng, "train step"));
-  return net_graph_run(
-      c, c->net, B, h, {real, noiseD, noiseG, masksD, masksG, feed_key}, seed,
-      [&]() { return train_step_body(c, h, B, nd, ng, real, noiseD, noiseG, masksD, masksG, &feed); }, true, nd, ng);
-}
+int NetStep::draw_masks(int kind, const uint64_t* root) { return k_masks_generate(c, c->D_masks, B, kind, h->p_spatial, h->p_drop, root); }
+int NetStep::d_forward(bool on_g) { return net_D_forward(c, on_g ? c->G.y : c->D_x, B, true, h); }
+int NetStep::d_backward(bool want_wgrad, bool want_dx) { return net_D_backward(c, c->D_dlogit, want_wgrad, want_dx); }
+int NetStep::g_backward() { return gen_backward(c->env, c->G, c->net, c->D_dx, nullptr); }

@@ -325,7 +325,7 @@ int run_train_step(fg_ae* n, const fg_ae_hyper* h, int B, const float* img_dev, 
                    fg_ae_stats* stats) {
   fg_ctx* c = n->c;
   FG_TRY(net_graph_run(c, n->net, B, h, sizeof(*h), {img_dev, masks_dev}, seed,
-                       [&]() { return train_step(n, h, B, img_dev, masks_dev); }, true));
+                       [&]() { return train_step(n, h, B, img_dev, masks_dev); }));
   // a replayed step does not run the host side of its body: set what it would have set.  The optimizer has moved the
   // parameters away from the activations, so fg_ae_backward needs a new forward.
   n->x = img_dev;

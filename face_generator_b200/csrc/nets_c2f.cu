@@ -49,15 +49,11 @@ struct fg_c2f {
   float *D_zl1 = nullptr, *D_al1 = nullptr, *D_hl1 = nullptr, *D_logit = nullptr, *D_out = nullptr, *D_masks = nullptr,
         *D_dlogit = nullptr, *D_dx = nullptr;
   float *ga = nullptr, *gb = nullptr, *ws = nullptr;
-  float *in_a = nullptr, *in_b = nullptr, *in_c = nullptr, *in_d = nullptr, *in_e = nullptr, *in_m1 = nullptr,
-        *in_m2 = nullptr, *io = nullptr;
-  IterStage iter_stage;  // the stacked inputs of fg_c2f_train_step_iters / fg_c2f_train_step_dataset_iters
+  float *in_a = nullptr, *in_b = nullptr, *in_c = nullptr, *in_d = nullptr, *in_e = nullptr, *io = nullptr;
+  IterStage iter_stage;  // the inputs of the host-fed and device-fed train steps, stacked per iteration
   int G_B = 0, D_B = 0;
   bool G_valid = false, D_valid = false, D_train = true;
   float D_scale = 2.f;
-  // option "debug_keep" (tests): the D step's D_z[0..3], D_zl1, D_logit, D_out, which the G step's D forward overwrites
-  float* keep_D[7] = {};
-  int keep_B = 0;
   std::vector<void*> allocs;
   ConvLEnv env;  // shared scratch of the ConvL layers (filled by c2f_alloc)
 };
@@ -176,9 +172,12 @@ int c2f_alloc(fg_c2f* n) {
   FG_TRY(dalloc(n, &n->in_c, B * HW));
   FG_TRY(dalloc(n, &n->in_d, B * HW * C));
   FG_TRY(dalloc(n, &n->in_e, B * HW));
-  FG_TRY(dalloc(n, &n->in_m1, B * mask));
-  FG_TRY(dalloc(n, &n->in_m2, B * mask));
   FG_TRY(dalloc(n, &n->io, B * HW * C));
+  int64_t dz[4];
+  for (int i = 0; i < 4; ++i) dz[i] = (int64_t)n->Dc[i].H * n->Dc[i].H * n->Dc[i].Cout;
+  n->net.keep = {{"Dstep.z1", n->D_z[0], dz[0]}, {"Dstep.z2", n->D_z[1], dz[1]}, {"Dstep.z3", n->D_z[2], dz[2]},
+                 {"Dstep.z4", n->D_z[3], dz[3]}, {"Dstep.zl1", n->D_zl1, 512},  {"Dstep.logit", n->D_logit, 1},
+                 {"Dstep.out", n->D_out, 1}};
   FG_CUDA(cudaStreamSynchronize(n->c->stream));
   return FG_OK;
 }
@@ -332,93 +331,41 @@ int D_backward(fg_c2f* n, const float* dlogit, bool want_wgrad, bool want_dx) {
   return FG_OK;
 }
 
-// t += 1 and the Adam step size on the device (shares the kernel of the 32x32 loop; no accuracy gate here)
-int prep(fg_c2f* n, int net, const fg_hyper* h, int B, bool accumulate = false) {
-  fg_hyper hh = *h;
-  hh.D_maxAcc = 1e30f;
-  return pair_gate(n->c, n->net, net, &hh, B, (float)n->c->world, accumulate);
-}
-
-// option "debug_keep": copy the D step's pre-activations and outputs to keep_D ("Dstep.*" debug tensors)
-int keep_dstep(fg_c2f* n, int B) {
-  fg_ctx* c = n->c;
-  const float* src[7] = {n->D_z[0], n->D_z[1], n->D_z[2], n->D_z[3], n->D_zl1, n->D_logit, n->D_out};
-  size_t per[7] = {0, 0, 0, 0, 512, 1, 1};
-  for (int i = 0; i < 4; ++i) per[i] = (size_t)n->Dc[i].H * n->Dc[i].H * n->Dc[i].Cout;
-  for (int i = 0; i < 7; ++i) {
-    if (!n->keep_D[i]) FG_TRY(dalloc(n, &n->keep_D[i], (size_t)n->maxB * per[i]));
-    FG_CUDA(cudaMemcpyAsync(n->keep_D[i], src[i], sizeof(float) * B * per[i], cudaMemcpyDeviceToDevice, c->stream));
-  }
-  n->keep_B = B;
-  return FG_OK;
-}
-
-// nD D iterations (adversarial_c2f.lua:121-163), then nG G iterations (:167-187), on inputs stacked per iteration; the
-// dropout masks of iteration j come from the stream root c->seed_dev[j] (k_seed_roots).  feed (may be null) draws the
-// inputs on the device first.
-int train_step(fg_c2f* n, const fg_hyper* h, int B, int nD, int nG, const float* real_diff, const float* condD,
-               const float* noiseD, const float* condG, const float* noiseG, const float* masksD, const float* masksG,
-               const std::function<int()>* feed) {
-  fg_ctx* c = n->c;
-  const int Bh = B / 2, C = n->C;
-  const size_t img = (size_t)C * n->HW, mask = (size_t)B * n->mask;
-  const float inv_world = 1.0f / (float)c->world;
-  if (nD > 1 || nG > 1) FG_TRY(k_seed_roots(c, c->seed_dev, std::max(nD, nG)));
-  if (feed && *feed) FG_TRY((*feed)());
-  for (int j = 0; j < nD; ++j) {
-    // ---- D iteration j (adversarial_c2f.lua:121-163) ----
-    const float* cd = condD + (size_t)j * B * img;
-    FG_TRY(G_forward(n, noiseD + (size_t)j * Bh * n->HW, cd + Bh * img, Bh));
-    FG_TRY(k_nchw_to_nhwc(c, real_diff + (size_t)j * Bh * img, n->io, Bh, C, n->HW));
-    FG_CUDA(cudaMemcpyAsync(n->io + Bh * img, n->G_z[4], sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
-    FG_TRY(k_nchw_to_nhwc(c, cd, n->D_cond, B, C, n->HW));
-    if (masksD)
-      FG_CUDA(cudaMemcpyAsync(n->D_masks, masksD + j * mask, sizeof(float) * mask, cudaMemcpyDeviceToDevice, c->stream));
-    else
-      FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)mask, 1, h->p_drop, c->seed_dev + j));
-    FG_TRY(pair_zero_grads(c, n->net, FG_NET_D));
-    FG_TRY(D_forward(n, n->io, n->D_cond, B, true, h->p_drop));
-    FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_D, n->net.tailD, B, Bh));
-    if (c->debug_keep) FG_TRY(keep_dstep(n, B));
-    FG_TRY(D_backward(n, n->D_dlogit, true, false));
-    FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_D));
-    FG_TRY(prep(n, FG_NET_D, h, B, j > 0));
-    // optim.adam / optim.adagrad / optim.sgd (adversarial_c2f.lua:153-161, :177-185): same rules as the interruptable ones
-    FG_TRY(pair_optim(c, n->net, FG_NET_D, h, inv_world));
-  }
-  for (int j = 0; j < nG; ++j) {
-    // ---- G iteration j (adversarial_c2f.lua:167-187) ----
-    const float* cg = condG + (size_t)j * B * img;
-    FG_TRY(pair_zero_grads(c, n->net, FG_NET_G));
+// the c2f nets in the loop body of adversarial_c2f.lua:121-187 (pair_train_step, netpair.cu): D iteration j reads
+// real_diff [B/2][C][S][S], condD [B][C][S][S] (the real pairs' condition, then the fakes') and noiseD [B/2][1][S][S],
+// G iteration j condG [B][C][S][S] and noiseG [B][1][S][S].  optim.adam / adagrad / sgd (:153-161, :177-185) follow
+// the same rules as the interruptable optimizers, without the accuracy gate.
+struct C2fStep final : StepNets {
+  fg_c2f* n;
+  const float *real_diff, *condD, *noiseD, *condG, *noiseG;
+  C2fStep(fg_c2f* n, const fg_hyper* h, int B, const float* real_diff, const float* condD, const float* noiseD,
+          const float* condG, const float* noiseG)
+      : StepNets(n->c, n->net, h, B, n->D_logit, n->D_out, n->D_dlogit, n->D_masks, n->mask, false, false), n(n),
+        real_diff(real_diff), condD(condD), noiseD(noiseD), condG(condG), noiseG(noiseG) {}
+  size_t img() const { return (size_t)n->C * n->HW; }
+  int g_forward(int j, bool d_iter) override {
+    if (d_iter) {  // the fakes take the second half of D's condition rows
+      const float* cd = condD + (size_t)j * B * img();
+      return G_forward(n, noiseD + (size_t)j * (B / 2) * n->HW, cd + (B / 2) * img(), B / 2);
+    }
+    const float* cg = condG + (size_t)j * B * img();
     FG_TRY(G_forward(n, noiseG + (size_t)j * B * n->HW, cg, B));
-    FG_TRY(k_nchw_to_nhwc(c, cg, n->D_cond, B, C, n->HW));
-    if (masksG)
-      FG_CUDA(cudaMemcpyAsync(n->D_masks, masksG + j * mask, sizeof(float) * mask, cudaMemcpyDeviceToDevice, c->stream));
-    else
-      FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)mask, 2, h->p_drop, c->seed_dev + j));
-    FG_TRY(D_forward(n, n->G_z[4], n->D_cond, B, true, h->p_drop));
-    FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_G, n->net.tailG, B, B));
-    FG_TRY(D_backward(n, n->D_dlogit, false, true));  // D's weight grads are zeroed before use (:45) -> skipped
-    FG_TRY(G_backward(n, n->D_dx));
-    FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_G));
-    FG_TRY(prep(n, FG_NET_G, h, B));
-    FG_TRY(pair_optim(c, n->net, FG_NET_G, h, inv_world));
+    return k_nchw_to_nhwc(c, cg, n->D_cond, B, n->C, n->HW);
   }
-  FG_CUDA(cudaMemcpyAsync(n->net.hstats, n->net.dstats, sizeof(DeviceStats), cudaMemcpyDeviceToHost, c->stream));
-  return FG_OK;
-}
-
-// train_step on device inputs: eager the first time, then a captured CUDA graph of the step (net_graph_run); the seed
-// is read on the device
-int run_train_step(fg_c2f* n, const fg_hyper* h, int B, const float* rd, const float* cd, const float* nd, const float* cg,
-                   const float* ng, const float* md, const float* mg, uint64_t seed, fg_step_stats* stats, int nD = 1,
-                   int nG = 1, const std::function<int()>* feed = nullptr, const void* feed_key = nullptr,
-                   int coarse_size = 0) {
-  FG_TRY(net_graph_run(
-      n->c, n->net, B, h, {rd, cd, nd, cg, ng, md, mg, feed_key, (const void*)(intptr_t)coarse_size}, seed,
-      [&]() { return train_step(n, h, B, nD, nG, rd, cd, nd, cg, ng, md, mg, feed); }, true, nD, nG));
-  return pair_step_stats(n->c, n->net, stats);
-}
+  int d_input(int j) override {
+    const int Bh = B / 2;
+    FG_TRY(k_nchw_to_nhwc(c, real_diff + (size_t)j * Bh * img(), n->io, Bh, n->C, n->HW));
+    FG_CUDA(cudaMemcpyAsync(n->io + Bh * img(), n->G_z[4], sizeof(float) * Bh * img(), cudaMemcpyDeviceToDevice, c->stream));
+    return k_nchw_to_nhwc(c, condD + (size_t)j * B * img(), n->D_cond, B, n->C, n->HW);
+  }
+  int draw_masks(int kind, const uint64_t* root) override {
+    return k_bernoulli_keep(c, n->D_masks, (int64_t)B * n->mask, kind, h->p_drop, root);
+  }
+  int d_forward(bool on_g) override { return D_forward(n, on_g ? n->G_z[4] : n->io, n->D_cond, B, true, h->p_drop); }
+  // D's weight grads of the G iteration are zeroed before use (:45): skipped
+  int d_backward(bool want_wgrad, bool want_dx) override { return D_backward(n, n->D_dlogit, want_wgrad, want_dx); }
+  int g_backward() override { return G_backward(n, n->D_dx); }
+};
 
 // ---- fg_c2f_refine: sample.lua:176-214 c2f() around the G and D forwards ----------------------------------------
 constexpr int kRefineThreads = 256;
@@ -503,6 +450,67 @@ __global__ void __launch_bounds__(kRefineThreads) refine_pick_kernel(const float
     }                                                    \
     FG_CUDA(cudaSetDevice((n)->c->device));              \
   } while (0)
+
+namespace {
+// d_iters D iterations + g_iters G iterations of the c2f loop body on the fg_c2f_train_step inputs stacked per
+// iteration, for the entry `what`
+int train_step_iters(fg_c2f* n, const char* what, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real_diff,
+                     const float* cond_D, const float* noise_D, const float* cond_G, const float* noise_G, const float* masks_D,
+                     const float* masks_G, uint64_t seed, fg_step_stats* stats) {
+  ENTER(n);
+  fg_ctx* c = n->c;
+  FG_TRY(step_check(c, what, B, d_iters, g_iters, h && real_diff && cond_D && noise_D && cond_G && noise_G));
+  const size_t nd = d_iters, ng = g_iters, Bh = B / 2, M = n->maxB, img = (size_t)n->C * n->HW, hw = n->HW, mk = n->mask;
+  IterStage& s = n->iter_stage;
+  const float *rd, *cd, *zd, *cg, *zg, *md, *mg;
+  FG_TRY(s.in(c, n->allocs, 0, real_diff, nd * Bh * img, nd * M / 2 * img, &rd));
+  FG_TRY(s.in(c, n->allocs, 1, cond_D, nd * B * img, nd * M * img, &cd));
+  FG_TRY(s.in(c, n->allocs, 2, noise_D, nd * Bh * hw, nd * M / 2 * hw, &zd));
+  FG_TRY(s.in(c, n->allocs, 3, cond_G, ng * B * img, ng * M * img, &cg));
+  FG_TRY(s.in(c, n->allocs, 4, noise_G, ng * B * hw, ng * M * hw, &zg));
+  FG_TRY(s.in(c, n->allocs, 5, masks_D, nd * B * mk, nd * M * mk, &md));
+  FG_TRY(s.in(c, n->allocs, 6, masks_G, ng * B * mk, ng * M * mk, &mg));
+  C2fStep st(n, h, B, rd, cd, zd, cg, zg);
+  return pair_train_step(st, d_iters, g_iters, md, mg, seed, {rd, cd, zd, cg, zg, md, mg, nullptr, nullptr}, nullptr, stats);
+}
+
+// the same fed on the device: D iteration j draws the streams 8*r_j .. 8*r_j+1 and 8*r_j+3, G iteration j the streams
+// 8*r_j+2 and 8*r_j+4 (r_j: fg_b200.h; r_0 = seed); the draws run inside the step
+int train_step_dataset_iters(fg_c2f* n, fg_dataset* d, const char* what, const fg_hyper* h, int B, int d_iters, int g_iters,
+                             int coarse_size, uint64_t seed, fg_step_stats* stats) {
+  ENTER(n);
+  fg_ctx* c = n->c;
+  FG_TRY(step_check(c, what, B, d_iters, g_iters, h, d, true));
+  FG_REQUIRE(coarse_size >= 1 && coarse_size <= n->S, "%s: coarse size %d outside [1, %d]", what, coarse_size, n->S);
+  const int Bh = B / 2, S = n->S;
+  const size_t M = n->maxB, img = (size_t)n->C * n->HW, hw = n->HW;
+  IterStage& s = n->iter_stage;
+  FG_TRY(s.reserve(c, n->allocs, 0, d_iters * M / 2 * img));
+  FG_TRY(s.reserve(c, n->allocs, 1, d_iters * M * img));
+  FG_TRY(s.reserve(c, n->allocs, 2, d_iters * M / 2 * hw));
+  FG_TRY(s.reserve(c, n->allocs, 3, g_iters * M * img));
+  FG_TRY(s.reserve(c, n->allocs, 4, g_iters * M * hw));
+  float *rd = s.p[0], *cd = s.p[1], *zd = s.p[2], *cg = s.p[3], *zg = s.p[4];
+  const std::function<int()> feed = [&]() -> int {
+    for (int j = 0; j < d_iters; ++j) {
+      const uint64_t* r = c->seed_dev + j;
+      float* cdj = cd + (size_t)j * B * img;
+      FG_TRY(dataset_draw_gather_c2f(d, 0, Bh, S, coarse_size, nullptr, cdj, rd + (size_t)j * Bh * img, r, 8));
+      FG_TRY(dataset_draw_gather_c2f(d, 1, Bh, S, coarse_size, nullptr, cdj + Bh * img, nullptr, r, 8));
+      FG_TRY(noise_uniform_dev(c, 3, (int64_t)Bh * hw, zd + (size_t)j * Bh * hw, r, 8));
+    }
+    for (int j = 0; j < g_iters; ++j) {
+      const uint64_t* r = c->seed_dev + j;
+      FG_TRY(dataset_draw_gather_c2f(d, 2, B, S, coarse_size, nullptr, cg + (size_t)j * B * img, nullptr, r, 8));
+      FG_TRY(noise_uniform_dev(c, 4, (int64_t)B * hw, zg + (size_t)j * B * hw, r, 8));
+    }
+    return FG_OK;
+  };
+  C2fStep st(n, h, B, rd, cd, zd, cg, zg);
+  return pair_train_step(st, d_iters, g_iters, nullptr, nullptr, seed,
+                         {rd, cd, zd, cg, zg, nullptr, nullptr, d, (const void*)(intptr_t)coarse_size}, &feed, stats);
+}
+}  // namespace
 
 extern "C" {
 
@@ -730,21 +738,8 @@ int fg_c2f_dp_broadcast_params(fg_c2f* n) {
 int fg_c2f_train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_diff, const float* cond_D,
                       const float* noise_D, const float* cond_G, const float* noise_G, const float* masks_D,
                       const float* masks_G, uint64_t seed, fg_step_stats* stats) {
-  ENTER(n);
-  FG_REQUIRE(h && real_diff && cond_D && noise_D && cond_G && noise_G, "fg_c2f_train_step: null input");
-  FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= n->maxB, "fg_c2f_train_step: batch %d must be even, >= 4 and <= max_batch %d", B,
-             n->maxB);
-  fg_ctx* c = n->c;
-  const size_t img = (size_t)n->C * n->HW;
-  const float *rd, *cd, *nd, *cg, *ng, *md = nullptr, *mg = nullptr;
-  FG_TRY(fg_to_dev(c, real_diff, (size_t)(B / 2) * img, n->in_a, &rd));
-  FG_TRY(fg_to_dev(c, cond_D, (size_t)B * img, n->in_b, &cd));
-  FG_TRY(fg_to_dev(c, noise_D, (size_t)(B / 2) * n->HW, n->in_c, &nd));
-  FG_TRY(fg_to_dev(c, cond_G, (size_t)B * img, n->in_d, &cg));
-  FG_TRY(fg_to_dev(c, noise_G, (size_t)B * n->HW, n->in_e, &ng));
-  if (masks_D) FG_TRY(fg_to_dev(c, masks_D, (size_t)B * n->mask, n->in_m1, &md));
-  if (masks_G) FG_TRY(fg_to_dev(c, masks_G, (size_t)B * n->mask, n->in_m2, &mg));
-  return run_train_step(n, h, B, rd, cd, nd, cg, ng, md, mg, seed, stats);
+  return train_step_iters(n, "fg_c2f_train_step", h, B, 1, 1, real_diff, cond_D, noise_D, cond_G, noise_G, masks_D, masks_G,
+                          seed, stats);
 }
 
 // one adversarial_c2f.lua:121-187 loop body fed on the device (the draws of :124-141 and :168-174):
@@ -752,87 +747,24 @@ int fg_c2f_train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_dif
 //   fake cond   = gather_c2f(draw(8*seed+1, B/2)) -> cond_D rows [B/2, B)
 //   G-step cond = gather_c2f(draw(8*seed+2, B))   -> cond_G
 //   noise_D = uniform(8*seed+3), noise_G = uniform(8*seed+4), dropout masks from `seed`.
-// The inputs land in the staging buffers a host-fed fg_c2f_train_step copies into, so both run the same step on the
-// same bits.
 int fg_c2f_train_step_dataset(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B, int coarse_size, uint64_t seed,
                               fg_step_stats* stats) {
-  ENTER(n);
-  fg_ctx* c = n->c;
-  FG_TRY(dataset_check_feed(d, c, "fg_c2f_train_step_dataset"));
-  FG_REQUIRE(h && B >= 4 && B % 2 == 0 && B <= n->maxB, "fg_c2f_train_step_dataset: batch %d must be even, >= 4 and <= max_batch %d",
-             B, n->maxB);
-  FG_REQUIRE(coarse_size >= 1 && coarse_size <= n->S, "fg_c2f_train_step_dataset: coarse size %d outside [1, %d]", coarse_size, n->S);
-  const int Bh = B / 2, S = n->S;
-  const size_t img = (size_t)n->C * n->HW;
-  FG_TRY(dataset_draw_gather_c2f(d, seed * 8, Bh, S, coarse_size, nullptr, n->in_b, n->in_a));
-  FG_TRY(dataset_draw_gather_c2f(d, seed * 8 + 1, Bh, S, coarse_size, nullptr, n->in_b + Bh * img, nullptr));
-  FG_TRY(dataset_draw_gather_c2f(d, seed * 8 + 2, B, S, coarse_size, nullptr, n->in_d, nullptr));
-  FG_TRY(noise_uniform_dev(c, seed * 8 + 3, (int64_t)Bh * n->HW, n->in_c));
-  FG_TRY(noise_uniform_dev(c, seed * 8 + 4, (int64_t)B * n->HW, n->in_e));
-  return run_train_step(n, h, B, n->in_a, n->in_b, n->in_c, n->in_d, n->in_e, nullptr, nullptr, seed, stats);
+  return train_step_dataset_iters(n, d, "fg_c2f_train_step_dataset", h, B, 1, 1, coarse_size, seed, stats);
 }
 
 // d_iters D iterations + g_iters G iterations of the c2f loop body on the fg_c2f_train_step inputs stacked per iteration
 int fg_c2f_train_step_iters(fg_c2f* n, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real_diff,
                             const float* cond_D, const float* noise_D, const float* cond_G, const float* noise_G,
                             const float* masks_D, const float* masks_G, uint64_t seed, fg_step_stats* stats) {
-  ENTER(n);
-  FG_TRY(iters_check(d_iters, g_iters, "fg_c2f_train_step_iters"));
-  FG_REQUIRE(h && real_diff && cond_D && noise_D && cond_G && noise_G, "fg_c2f_train_step_iters: null input");
-  FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= n->maxB, "fg_c2f_train_step_iters: batch %d must be even, >= 4 and <= max_batch %d",
-             B, n->maxB);
-  fg_ctx* c = n->c;
-  const size_t nd = d_iters, ng = g_iters, Bh = B / 2, M = n->maxB, img = (size_t)n->C * n->HW, hw = n->HW, mk = n->mask;
-  IterStage& s = n->iter_stage;
-  const float *rd, *cd, *zd, *cg, *zg, *md, *mg;
-  FG_TRY(s.in(c, n->allocs, 0, real_diff, nd * Bh * img, nd * M / 2 * img, &rd));
-  FG_TRY(s.in(c, n->allocs, 1, cond_D, nd * B * img, nd * M * img, &cd));
-  FG_TRY(s.in(c, n->allocs, 2, noise_D, nd * Bh * hw, nd * M / 2 * hw, &zd));
-  FG_TRY(s.in(c, n->allocs, 3, cond_G, ng * B * img, ng * M * img, &cg));
-  FG_TRY(s.in(c, n->allocs, 4, noise_G, ng * B * hw, ng * M * hw, &zg));
-  FG_TRY(s.in(c, n->allocs, 5, masks_D, nd * B * mk, nd * M * mk, &md));
-  FG_TRY(s.in(c, n->allocs, 6, masks_G, ng * B * mk, ng * M * mk, &mg));
-  return run_train_step(n, h, B, rd, cd, zd, cg, zg, md, mg, seed, stats, d_iters, g_iters);
+  return train_step_iters(n, "fg_c2f_train_step_iters", h, B, d_iters, g_iters, real_diff, cond_D, noise_D, cond_G, noise_G,
+                          masks_D, masks_G, seed, stats);
 }
 
 // fg_c2f_train_step_iters fed on the device: D iteration j draws the streams 8*r_j .. 8*r_j+1 and 8*r_j+3, G iteration
-// j the streams 8*r_j+2 and 8*r_j+4, as fg_c2f_train_step_dataset does for r_0 = seed (r_j: fg_b200.h); the draws run
-// inside the step
+// j the streams 8*r_j+2 and 8*r_j+4, as fg_c2f_train_step_dataset does for r_0 = seed (r_j: fg_b200.h)
 int fg_c2f_train_step_dataset_iters(fg_c2f* n, fg_dataset* d, const fg_hyper* h, int B, int d_iters, int g_iters,
                                     int coarse_size, uint64_t seed, fg_step_stats* stats) {
-  ENTER(n);
-  fg_ctx* c = n->c;
-  FG_TRY(iters_check(d_iters, g_iters, "fg_c2f_train_step_dataset_iters"));
-  FG_TRY(dataset_check_feed(d, c, "fg_c2f_train_step_dataset_iters"));
-  FG_REQUIRE(h && B >= 4 && B % 2 == 0 && B <= n->maxB,
-             "fg_c2f_train_step_dataset_iters: batch %d must be even, >= 4 and <= max_batch %d", B, n->maxB);
-  FG_REQUIRE(coarse_size >= 1 && coarse_size <= n->S, "fg_c2f_train_step_dataset_iters: coarse size %d outside [1, %d]",
-             coarse_size, n->S);
-  const int Bh = B / 2, S = n->S;
-  const size_t M = n->maxB, img = (size_t)n->C * n->HW, hw = n->HW;
-  IterStage& s = n->iter_stage;
-  FG_TRY(s.reserve(c, n->allocs, 0, d_iters * M / 2 * img));
-  FG_TRY(s.reserve(c, n->allocs, 1, d_iters * M * img));
-  FG_TRY(s.reserve(c, n->allocs, 2, d_iters * M / 2 * hw));
-  FG_TRY(s.reserve(c, n->allocs, 3, g_iters * M * img));
-  FG_TRY(s.reserve(c, n->allocs, 4, g_iters * M * hw));
-  float *rd = s.p[0], *cd = s.p[1], *zd = s.p[2], *cg = s.p[3], *zg = s.p[4];
-  const std::function<int()> feed = [&]() -> int {
-    for (int j = 0; j < d_iters; ++j) {
-      const uint64_t* r = c->seed_dev + j;
-      float* cdj = cd + (size_t)j * B * img;
-      FG_TRY(dataset_draw_gather_c2f(d, 0, Bh, S, coarse_size, nullptr, cdj, rd + (size_t)j * Bh * img, r, 8));
-      FG_TRY(dataset_draw_gather_c2f(d, 1, Bh, S, coarse_size, nullptr, cdj + Bh * img, nullptr, r, 8));
-      FG_TRY(noise_uniform_dev(c, 3, (int64_t)Bh * hw, zd + (size_t)j * Bh * hw, r, 8));
-    }
-    for (int j = 0; j < g_iters; ++j) {
-      const uint64_t* r = c->seed_dev + j;
-      FG_TRY(dataset_draw_gather_c2f(d, 2, B, S, coarse_size, nullptr, cg + (size_t)j * B * img, nullptr, r, 8));
-      FG_TRY(noise_uniform_dev(c, 4, (int64_t)B * hw, zg + (size_t)j * B * hw, r, 8));
-    }
-    return FG_OK;
-  };
-  return run_train_step(n, h, B, rd, cd, zd, cg, zg, nullptr, nullptr, seed, stats, d_iters, g_iters, &feed, d, coarse_size);
+  return train_step_dataset_iters(n, d, "fg_c2f_train_step_dataset_iters", h, B, d_iters, g_iters, coarse_size, seed, stats);
 }
 
 int64_t fg_c2f_debug_tensor(fg_c2f* n, const char* name, float* dst, int64_t max_elems) {
@@ -841,20 +773,19 @@ int64_t fg_c2f_debug_tensor(fg_c2f* n, const char* name, float* dst, int64_t max
     return -1;
   }
   cudaSetDevice(n->c->device);
-  const int gb = n->G_B, db = n->D_B, kb = n->keep_B, C = n->C, HW = n->HW;
+  const int gb = n->G_B, db = n->D_B, C = n->C, HW = n->HW;
   auto g = [&](const float* p) { return n->G_valid ? p : nullptr; };
   auto d = [&](const float* p) { return n->D_valid ? p : nullptr; };
   auto dz = [&](int i) { return (int64_t)n->Dc[i].H * n->Dc[i].H * n->Dc[i].Cout; };
-  const DebugTensor ents[] = {
+  std::vector<DebugTensor> ents = {
       {"G.x", g(n->G_x), HW * (C + 1), gb}, {"G.z1", g(n->G_z[0]), HW * 64, gb}, {"G.z2", g(n->G_z[1]), HW * 64, gb},
       {"G.z3", g(n->G_z[2]), HW * 128, gb}, {"G.z4", g(n->G_z[3]), HW * 256, gb}, {"G.z5", g(n->G_z[4]), HW * C, gb},
       {"D.x", d(n->D_x), HW * C, db}, {"D.z1", d(n->D_z[0]), dz(0), db}, {"D.z2", d(n->D_z[1]), dz(1), db},
       {"D.z3", d(n->D_z[2]), dz(2), db}, {"D.z4", d(n->D_z[3]), dz(3), db}, {"D.p2", d(n->D_p2), HW / 4 * 64, db},
       {"D.p4", d(n->D_p4), n->flat, db}, {"D.zl1", d(n->D_zl1), 512, db}, {"D.logit", d(n->D_logit), 1, db},
-      {"D.out", d(n->D_out), 1, db}, {"Dstep.z1", n->keep_D[0], dz(0), kb}, {"Dstep.z2", n->keep_D[1], dz(1), kb},
-      {"Dstep.z3", n->keep_D[2], dz(2), kb}, {"Dstep.z4", n->keep_D[3], dz(3), kb}, {"Dstep.zl1", n->keep_D[4], 512, kb},
-      {"Dstep.logit", n->keep_D[5], 1, kb}, {"Dstep.out", n->keep_D[6], 1, kb}};
-  return debug_tensor_copy(n->c, "fg_c2f_debug_tensor", ents, sizeof(ents) / sizeof(ents[0]), name, dst, max_elems);
+      {"D.out", d(n->D_out), 1, db}};
+  pair_keep_rows(n->net, ents);
+  return debug_tensor_copy(n->c, "fg_c2f_debug_tensor", ents.data(), ents.size(), name, dst, max_elems);
 }
 
 }  // extern "C"

@@ -859,7 +859,7 @@ int fg_dn_train_step(fg_dn* n, const fg_dn_hyper* h, int B, const float* images,
   if (noise) FG_TRY(fg_to_dev(c, noise, 2 * im, n->in_noise, &nd));
   if (masks) FG_TRY(fg_to_dev(c, masks, 3 * (size_t)B * n->mps, n->in_masks, &md));
   n->p_drop = h->p_drop;
-  FG_TRY(net_graph_run(c, n->net, B, h, sizeof(*h), {id, nd, md}, seed, [&]() { return train_step(n, h, B, id, nd, md); }, true));
+  FG_TRY(net_graph_run(c, n->net, B, h, sizeof(*h), {id, nd, md}, seed, [&]() { return train_step(n, h, B, id, nd, md); }));
   // A replayed step does not run the host side of its body: set what it would have set.  The step leaves AE1's
   // activations of its second forward beside the sigmoid output of its first, so fg_dn_backward needs a new forward.
   for (DnDec& d : n->dec) {

@@ -118,15 +118,11 @@ struct fg_s16 {
         *D_dx2 = nullptr, *D_djoint = nullptr, *D_dhf = nullptr, *D_dhe2 = nullptr;
   // shared scratch
   float *ga = nullptr, *gb = nullptr, *ws = nullptr;
-  float *in_a = nullptr, *in_b = nullptr, *in_c = nullptr, *in_m1 = nullptr, *in_m2 = nullptr, *io = nullptr;
-  IterStage iter_stage;  // the stacked inputs of fg_s16_train_step_iters / fg_s16_train_step_dataset_iters
+  float *in_a = nullptr, *in_b = nullptr, *in_c = nullptr, *io = nullptr;
+  IterStage iter_stage;  // the inputs of the host-fed and device-fed train steps, stacked per iteration
   int D_pack_impl = -1;
   int D_B = 0;
   bool D_valid = false, D_train = true;
-  // option "debug_keep" (tests): the D step's D_z[0..3], D_zf, D_ze1, D_ze2, D_logit, D_out, which the G step's D
-  // forward overwrites
-  float* keep_D[9] = {};
-  int keep_B = 0;
   std::vector<void*> allocs;
   ConvLEnv env;
 };
@@ -228,9 +224,10 @@ int s16_alloc(fg_s16* n) {
   FG_TRY(dalloc(n, &n->in_a, B * 256 * C));
   FG_TRY(dalloc(n, &n->in_b, B * 100));
   FG_TRY(dalloc(n, &n->in_c, B * 100));
-  FG_TRY(dalloc(n, &n->in_m1, B * kS16Mask));
-  FG_TRY(dalloc(n, &n->in_m2, B * kS16Mask));
   FG_TRY(dalloc(n, &n->io, B * 256 * C));
+  n->net.keep = {{"Dstep.z1", n->D_z[0], 256 * 128}, {"Dstep.z2", n->D_z[1], 256 * 128}, {"Dstep.z3", n->D_z[2], 16 * 512},
+                 {"Dstep.z4", n->D_z[3], 4 * 1024},  {"Dstep.zf", n->D_zf, 1024},        {"Dstep.ze1", n->D_ze1, 128},
+                 {"Dstep.ze2", n->D_ze2, 128},       {"Dstep.logit", n->D_logit, 1},     {"Dstep.out", n->D_out, 1}};
   FG_CUDA(cudaStreamSynchronize(n->c->stream));
   return FG_OK;
 }
@@ -362,78 +359,33 @@ int D_backward(fg_s16* n, const float* dlogit, bool want_wgrad, bool want_dx) {
   return FG_OK;
 }
 
-// option "debug_keep": copy the D step's pre-activations and outputs to keep_D ("Dstep.*" debug tensors)
-int keep_dstep(fg_s16* n, int B) {
-  fg_ctx* c = n->c;
-  const float* src[9] = {n->D_z[0], n->D_z[1], n->D_z[2], n->D_z[3], n->D_zf, n->D_ze1, n->D_ze2, n->D_logit, n->D_out};
-  const size_t per[9] = {256 * 128, 256 * 128, 16 * 512, 4 * 1024, 1024, 128, 128, 1, 1};
-  for (int i = 0; i < 9; ++i) {
-    if (!n->keep_D[i]) FG_TRY(dalloc(n, &n->keep_D[i], (size_t)n->maxB * per[i]));
-    FG_CUDA(cudaMemcpyAsync(n->keep_D[i], src[i], sizeof(float) * B * per[i], cudaMemcpyDeviceToDevice, c->stream));
+// the 16x16 nets in the loop body (pair_train_step, netpair.cu): real [B/2][C][16][16], noiseD [B/2][100] and noiseG
+// [B][100] per iteration
+struct S16Step final : StepNets {
+  fg_s16* n;
+  const float *real, *noiseD, *noiseG;
+  S16Step(fg_s16* n, const fg_hyper* h, int B, const float* real, const float* noiseD, const float* noiseG)
+      : StepNets(n->c, n->net, h, B, n->D_logit, n->D_out, n->D_dlogit, n->D_masks, kS16Mask, true, false), n(n), real(real),
+        noiseD(noiseD), noiseG(noiseG) {}
+  int g_forward(int j, bool d_iter) override {
+    const int rows = d_iter ? B / 2 : B;
+    return gen_forward(n->env, n->G, n->net, (d_iter ? noiseD : noiseG) + (size_t)j * rows * 100, rows, true);
   }
-  n->keep_B = B;
-  return FG_OK;
-}
-
-// the adversarial.lua loop body on the 16x16 nets: nD D iterations, then nG G iterations, on inputs stacked per
-// iteration; the dropout masks of iteration j come from the stream root c->seed_dev[j] (k_seed_roots).  feed (may be
-// null) draws the inputs on the device first.
-int train_step(fg_s16* n, const fg_hyper* h, int B, int nD, int nG, const float* real, const float* noiseD,
-               const float* noiseG, const float* masksD, const float* masksG, const std::function<int()>* feed) {
-  fg_ctx* c = n->c;
-  const int Bh = B / 2, C = n->C;
-  const size_t img = (size_t)C * 256, mask = (size_t)B * kS16Mask;
-  const float inv_world = 1.0f / (float)c->world;
-  if (nD > 1 || nG > 1) FG_TRY(k_seed_roots(c, c->seed_dev, std::max(nD, nG)));
-  if (feed && *feed) FG_TRY((*feed)());
-  for (int j = 0; j < nD; ++j) {
-    // ---- D iteration j (adversarial.lua:240-268) ----
-    FG_TRY(gen_forward(n->env, n->G, n->net, noiseD + (size_t)j * Bh * 100, Bh, true));  // createImages: training mode
-    FG_TRY(k_nchw_to_nhwc(c, real + (size_t)j * Bh * img, n->D_x, Bh, C, 256));
+  int d_input(int j) override {
+    const int Bh = B / 2;
+    const size_t img = (size_t)n->C * 256;
+    FG_TRY(k_nchw_to_nhwc(c, real + (size_t)j * Bh * img, n->D_x, Bh, n->C, 256));
     FG_CUDA(cudaMemcpyAsync(n->D_x + Bh * img, n->G.y, sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
-    if (masksD)
-      FG_CUDA(cudaMemcpyAsync(n->D_masks, masksD + j * mask, sizeof(float) * mask, cudaMemcpyDeviceToDevice, c->stream));
-    else
-      FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)mask, 1, 0.5f, c->seed_dev + j));
-    FG_TRY(pair_zero_grads(c, n->net, FG_NET_D));
-    FG_TRY(D_forward(n, n->D_x, B, true));
-    FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_D, n->net.tailD, B, Bh));
-    if (c->debug_keep) FG_TRY(keep_dstep(n, B));
-    FG_TRY(D_backward(n, n->D_dlogit, true, false));
-    FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_D));
-    FG_TRY(pair_gate(c, n->net, FG_NET_D, h, B, (float)c->world, j > 0));
-    FG_TRY(pair_optim(c, n->net, FG_NET_D, h, inv_world));
+    return FG_OK;
   }
-  for (int j = 0; j < nG; ++j) {
-    // ---- G iteration j (adversarial.lua:275-288) ----
-    FG_TRY(pair_zero_grads(c, n->net, FG_NET_G));
-    FG_TRY(gen_forward(n->env, n->G, n->net, noiseG + (size_t)j * B * 100, B, true));
-    if (masksG)
-      FG_CUDA(cudaMemcpyAsync(n->D_masks, masksG + j * mask, sizeof(float) * mask, cudaMemcpyDeviceToDevice, c->stream));
-    else
-      FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)mask, 2, 0.5f, c->seed_dev + j));
-    FG_TRY(D_forward(n, n->G.y, B, true));
-    FG_TRY(k_sigmoid_bce(c, n->D_logit, n->D_out, n->D_dlogit, &n->net.dstats->loss_G, n->net.tailG, B, B));
-    FG_TRY(D_backward(n, n->D_dlogit, false, true));  // D's weight grads are discarded by the reference (:209 vs :92)
-    FG_TRY(gen_backward(n->env, n->G, n->net, n->D_dx, nullptr));
-    FG_TRY(pair_allreduce_grads(c, n->net, FG_NET_G));
-    FG_TRY(pair_gate(c, n->net, FG_NET_G, h, B, (float)c->world));
-    FG_TRY(pair_optim(c, n->net, FG_NET_G, h, inv_world));
+  int draw_masks(int kind, const uint64_t* root) override {
+    return k_bernoulli_keep(c, n->D_masks, (int64_t)B * kS16Mask, kind, 0.5f, root);
   }
-  FG_CUDA(cudaMemcpyAsync(n->net.hstats, n->net.dstats, sizeof(DeviceStats), cudaMemcpyDeviceToHost, c->stream));
-  return FG_OK;
-}
+  int d_forward(bool on_g) override { return D_forward(n, on_g ? n->G.y : n->D_x, B, true); }
+  int d_backward(bool want_wgrad, bool want_dx) override { return D_backward(n, n->D_dlogit, want_wgrad, want_dx); }
+  int g_backward() override { return gen_backward(n->env, n->G, n->net, n->D_dx, nullptr); }
+};
 
-// train_step on device inputs: eager the first time, then a captured CUDA graph of the step (net_graph_run); the seed
-// is read on the device
-int run_train_step(fg_s16* n, const fg_hyper* h, int B, const float* rd, const float* nd, const float* ng, const float* md,
-                   const float* mg, uint64_t seed, fg_step_stats* stats, int nD = 1, int nG = 1,
-                   const std::function<int()>* feed = nullptr, const void* feed_key = nullptr) {
-  FG_TRY(net_graph_run(
-      n->c, n->net, B, h, {rd, nd, ng, md, mg, feed_key}, seed,
-      [&]() { return train_step(n, h, B, nD, nG, rd, nd, ng, md, mg, feed); }, true, nD, nG));
-  return pair_step_stats(n->c, n->net, stats);
-}
 }  // namespace
 
 #define ENTER(n)                                         \
@@ -444,6 +396,55 @@ int run_train_step(fg_s16* n, const fg_hyper* h, int B, const float* rd, const f
     }                                                    \
     FG_CUDA(cudaSetDevice((n)->c->device));              \
   } while (0)
+
+namespace {
+// d_iters D iterations + g_iters G iterations on inputs stacked per iteration (fg_train_step_iters at 16x16), for the
+// entry `what`
+int train_step_iters(fg_s16* n, const char* what, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,
+                     const float* noise_D, const float* noise_G, const float* masks_D, const float* masks_G, uint64_t seed,
+                     fg_step_stats* stats) {
+  ENTER(n);
+  fg_ctx* c = n->c;
+  FG_TRY(step_check(c, what, B, d_iters, g_iters, h && real && noise_D && noise_G));
+  const size_t nd = d_iters, ng = g_iters, Bh = B / 2, M = n->maxB, img = (size_t)n->C * 256;
+  IterStage& s = n->iter_stage;
+  const float *rd, *zd, *zg, *md, *mg;
+  FG_TRY(s.in(c, n->allocs, 0, real, nd * Bh * img, nd * M / 2 * img, &rd));
+  FG_TRY(s.in(c, n->allocs, 1, noise_D, nd * Bh * 100, nd * M / 2 * 100, &zd));
+  FG_TRY(s.in(c, n->allocs, 2, noise_G, ng * B * 100, ng * M * 100, &zg));
+  FG_TRY(s.in(c, n->allocs, 3, masks_D, nd * B * kS16Mask, nd * M * kS16Mask, &md));
+  FG_TRY(s.in(c, n->allocs, 4, masks_G, ng * B * kS16Mask, ng * M * kS16Mask, &mg));
+  S16Step st(n, h, B, rd, zd, zg);
+  return pair_train_step(st, d_iters, g_iters, md, mg, seed, {rd, zd, zg, md, mg, nullptr}, nullptr, stats);
+}
+
+// the same fed on the device: the streams of fg_train_step_dataset_iters, the real halves at 16x16; the draws run
+// inside the step
+int train_step_dataset_iters(fg_s16* n, fg_dataset* d, const char* what, const fg_hyper* h, int B, int d_iters, int g_iters,
+                             uint64_t seed, fg_step_stats* stats) {
+  ENTER(n);
+  fg_ctx* c = n->c;
+  FG_TRY(step_check(c, what, B, d_iters, g_iters, h, d, true));
+  const int Bh = B / 2;
+  const size_t M = n->maxB, img = (size_t)n->C * 256;
+  IterStage& s = n->iter_stage;
+  FG_TRY(s.reserve(c, n->allocs, 0, d_iters * M / 2 * img));
+  FG_TRY(s.reserve(c, n->allocs, 1, d_iters * M / 2 * 100));
+  FG_TRY(s.reserve(c, n->allocs, 2, g_iters * M * 100));
+  float *real = s.p[0], *zd = s.p[1], *zg = s.p[2];
+  const std::function<int()> feed = [&]() -> int {
+    for (int j = 0; j < d_iters; ++j) {
+      FG_TRY(dataset_draw_gather(d, 0, Bh, kSide, real + (size_t)j * Bh * img, c->seed_dev + j, 4));
+      FG_TRY(noise_uniform_dev(c, 1, (int64_t)Bh * 100, zd + (size_t)j * Bh * 100, c->seed_dev + j, 4));
+    }
+    for (int j = 0; j < g_iters; ++j)
+      FG_TRY(noise_uniform_dev(c, 2, (int64_t)B * 100, zg + (size_t)j * B * 100, c->seed_dev + j, 4));
+    return FG_OK;
+  };
+  S16Step st(n, h, B, real, zd, zg);
+  return pair_train_step(st, d_iters, g_iters, nullptr, nullptr, seed, {real, zd, zg, nullptr, nullptr, d}, &feed, stats);
+}
+}  // namespace
 
 extern "C" {
 
@@ -593,83 +594,27 @@ int fg_s16_dp_broadcast_params(fg_s16* n) {
 
 int fg_s16_train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const float* noise_D, const float* noise_G,
                       const float* masks_D, const float* masks_G, uint64_t seed, fg_step_stats* stats) {
-  ENTER(n);
-  FG_REQUIRE(h && real && noise_D && noise_G, "fg_s16_train_step: null input");
-  FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= n->maxB, "fg_s16_train_step: batch %d must be even, >= 4 and <= max_batch %d", B,
-             n->maxB);
-  fg_ctx* c = n->c;
-  const float *rd, *nd, *ng, *md = nullptr, *mg = nullptr;
-  FG_TRY(fg_to_dev(c, real, (size_t)(B / 2) * n->C * 256, n->in_a, &rd));
-  FG_TRY(fg_to_dev(c, noise_D, (size_t)(B / 2) * 100, n->in_b, &nd));
-  FG_TRY(fg_to_dev(c, noise_G, (size_t)B * 100, n->in_c, &ng));
-  if (masks_D) FG_TRY(fg_to_dev(c, masks_D, (size_t)B * kS16Mask, n->in_m1, &md));
-  if (masks_G) FG_TRY(fg_to_dev(c, masks_G, (size_t)B * kS16Mask, n->in_m2, &mg));
-  return run_train_step(n, h, B, rd, nd, ng, md, mg, seed, stats);
+  return train_step_iters(n, "fg_s16_train_step", h, B, 1, 1, real, noise_D, noise_G, masks_D, masks_G, seed, stats);
 }
 
 // train.lua --scale 16 fed on the device: real = gather at 16x16 of draw(4*seed, B/2), noise_D = uniform(4*seed+1),
-// noise_G = uniform(4*seed+2), dropout masks from `seed` (the streams of fg_train_step_dataset).  The inputs land in
-// the staging buffers a host-fed fg_s16_train_step copies into, so both run the same step on the same bits.
+// noise_G = uniform(4*seed+2), dropout masks from `seed` (the streams of fg_train_step_dataset)
 int fg_s16_train_step_dataset(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B, uint64_t seed, fg_step_stats* stats) {
-  ENTER(n);
-  fg_ctx* c = n->c;
-  FG_TRY(dataset_check_feed(d, c, "fg_s16_train_step_dataset"));
-  FG_REQUIRE(h && B >= 4 && B % 2 == 0 && B <= n->maxB, "fg_s16_train_step_dataset: batch %d must be even, >= 4 and <= max_batch %d",
-             B, n->maxB);
-  FG_TRY(dataset_draw_gather(d, seed * 4, B / 2, kSide, n->in_a));
-  FG_TRY(noise_uniform_dev(c, seed * 4 + 1, (int64_t)(B / 2) * 100, n->in_b));
-  FG_TRY(noise_uniform_dev(c, seed * 4 + 2, (int64_t)B * 100, n->in_c));
-  return run_train_step(n, h, B, n->in_a, n->in_b, n->in_c, nullptr, nullptr, seed, stats);
+  return train_step_dataset_iters(n, d, "fg_s16_train_step_dataset", h, B, 1, 1, seed, stats);
 }
 
 // d_iters D iterations + g_iters G iterations on inputs stacked per iteration (fg_train_step_iters at 16x16)
 int fg_s16_train_step_iters(fg_s16* n, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,
                             const float* noise_D, const float* noise_G, const float* masks_D, const float* masks_G,
                             uint64_t seed, fg_step_stats* stats) {
-  ENTER(n);
-  FG_TRY(iters_check(d_iters, g_iters, "fg_s16_train_step_iters"));
-  FG_REQUIRE(h && real && noise_D && noise_G, "fg_s16_train_step_iters: null input");
-  FG_REQUIRE(B >= 4 && B % 2 == 0 && B <= n->maxB, "fg_s16_train_step_iters: batch %d must be even, >= 4 and <= max_batch %d",
-             B, n->maxB);
-  fg_ctx* c = n->c;
-  const size_t nd = d_iters, ng = g_iters, Bh = B / 2, M = n->maxB, img = (size_t)n->C * 256;
-  IterStage& s = n->iter_stage;
-  const float *rd, *zd, *zg, *md, *mg;
-  FG_TRY(s.in(c, n->allocs, 0, real, nd * Bh * img, nd * M / 2 * img, &rd));
-  FG_TRY(s.in(c, n->allocs, 1, noise_D, nd * Bh * 100, nd * M / 2 * 100, &zd));
-  FG_TRY(s.in(c, n->allocs, 2, noise_G, ng * B * 100, ng * M * 100, &zg));
-  FG_TRY(s.in(c, n->allocs, 3, masks_D, nd * B * kS16Mask, nd * M * kS16Mask, &md));
-  FG_TRY(s.in(c, n->allocs, 4, masks_G, ng * B * kS16Mask, ng * M * kS16Mask, &mg));
-  return run_train_step(n, h, B, rd, zd, zg, md, mg, seed, stats, d_iters, g_iters);
+  return train_step_iters(n, "fg_s16_train_step_iters", h, B, d_iters, g_iters, real, noise_D, noise_G, masks_D, masks_G, seed,
+                          stats);
 }
 
-// fg_s16_train_step_iters fed on the device: the streams of fg_train_step_dataset_iters, the real halves at 16x16;
-// the draws run inside the step
+// fg_s16_train_step_iters fed on the device: the streams of fg_train_step_dataset_iters, the real halves at 16x16
 int fg_s16_train_step_dataset_iters(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B, int d_iters, int g_iters,
                                     uint64_t seed, fg_step_stats* stats) {
-  ENTER(n);
-  fg_ctx* c = n->c;
-  FG_TRY(iters_check(d_iters, g_iters, "fg_s16_train_step_dataset_iters"));
-  FG_TRY(dataset_check_feed(d, c, "fg_s16_train_step_dataset_iters"));
-  FG_REQUIRE(h && B >= 4 && B % 2 == 0 && B <= n->maxB,
-             "fg_s16_train_step_dataset_iters: batch %d must be even, >= 4 and <= max_batch %d", B, n->maxB);
-  const int Bh = B / 2;
-  const size_t M = n->maxB, img = (size_t)n->C * 256;
-  IterStage& s = n->iter_stage;
-  FG_TRY(s.reserve(c, n->allocs, 0, d_iters * M / 2 * img));
-  FG_TRY(s.reserve(c, n->allocs, 1, d_iters * M / 2 * 100));
-  FG_TRY(s.reserve(c, n->allocs, 2, g_iters * M * 100));
-  float *real = s.p[0], *zd = s.p[1], *zg = s.p[2];
-  const std::function<int()> feed = [&]() -> int {
-    for (int j = 0; j < d_iters; ++j) {
-      FG_TRY(dataset_draw_gather(d, 0, Bh, kSide, real + (size_t)j * Bh * img, c->seed_dev + j, 4));
-      FG_TRY(noise_uniform_dev(c, 1, (int64_t)Bh * 100, zd + (size_t)j * Bh * 100, c->seed_dev + j, 4));
-    }
-    for (int j = 0; j < g_iters; ++j)
-      FG_TRY(noise_uniform_dev(c, 2, (int64_t)B * 100, zg + (size_t)j * B * 100, c->seed_dev + j, 4));
-    return FG_OK;
-  };
-  return run_train_step(n, h, B, real, zd, zg, nullptr, nullptr, seed, stats, d_iters, g_iters, &feed, d);
+  return train_step_dataset_iters(n, d, "fg_s16_train_step_dataset_iters", h, B, d_iters, g_iters, seed, stats);
 }
 
 int64_t fg_s16_debug_tensor(fg_s16* n, const char* name, float* dst, int64_t max_elems) {
@@ -678,16 +623,14 @@ int64_t fg_s16_debug_tensor(fg_s16* n, const char* name, float* dst, int64_t max
     return -1;
   }
   cudaSetDevice(n->c->device);
-  const int db = n->D_B, kb = n->keep_B;
+  const int db = n->D_B;
   auto d = [&](const float* p) { return n->D_valid ? p : nullptr; };
   std::vector<DebugTensor> ents = {
       {"D.z1", d(n->D_z[0]), 256 * 128, db}, {"D.z2", d(n->D_z[1]), 256 * 128, db}, {"D.z3", d(n->D_z[2]), 16 * 512, db},
       {"D.z4", d(n->D_z[3]), 4 * 1024, db}, {"D.p1", d(n->D_p1), 64 * 128, db}, {"D.zf", d(n->D_zf), 1024, db},
       {"D.ze1", d(n->D_ze1), 128, db}, {"D.ze2", d(n->D_ze2), 128, db}, {"D.logit", d(n->D_logit), 1, db},
-      {"D.out", d(n->D_out), 1, db}, {"Dstep.z1", n->keep_D[0], 256 * 128, kb}, {"Dstep.z2", n->keep_D[1], 256 * 128, kb},
-      {"Dstep.z3", n->keep_D[2], 16 * 512, kb}, {"Dstep.z4", n->keep_D[3], 4 * 1024, kb}, {"Dstep.zf", n->keep_D[4], 1024, kb},
-      {"Dstep.ze1", n->keep_D[5], 128, kb}, {"Dstep.ze2", n->keep_D[6], 128, kb}, {"Dstep.logit", n->keep_D[7], 1, kb},
-      {"Dstep.out", n->keep_D[8], 1, kb}};
+      {"D.out", d(n->D_out), 1, db}};
+  pair_keep_rows(n->net, ents);
   gen_debug_rows(n->G, ents);
   return debug_tensor_copy(n->c, "fg_s16_debug_tensor", ents.data(), ents.size(), name, dst, max_elems);
 }

@@ -1,11 +1,14 @@
 """Bit-for-bit A/B of two builds of libfg_b200.so.
 
-`run` loads the library at --lib, and for each case (net, batch, options) runs 3 host-fed and 3 device-fed seeded train
-steps, then one G forward / G backward / D forward / D backward call.  It writes every piece of state as .npy under
+`run` loads the library at --lib, and for each case (net, batch, options, step mode) runs 3 host-fed and 3 device-fed
+seeded train steps, then one G forward / G backward / D forward / D backward call.  The step modes are the
+single-iteration entries, the *_iters / *_dataset_iters entries at 2 D and 2 G iterations ("iters2x2"), and the single
+entries with option debug_keep, saving every Dstep.* tensor after each step ("debug_keep").  The coarse-to-fine nets
+also run at fine sizes 16 and 64.  It writes every piece of state as .npy under
 --out/<case>/: parameters, gradients, optimizer m / v / t, BatchNorm running state, the step statistics, the outputs
 of those calls and the generator's debug tensors, plus the kernel launches of each step (launches.json).  The L-op
 convolutions (fg_conv2d_*) with the 3xFP16 split are one more case.  `compare A B` reports, per case, the first array
-that differs and the launches per step of both builds.
+that differs and the launches per step of both builds; a case differs when either does.
 
 One build per process: both libraries export the same symbols.
 
@@ -29,6 +32,10 @@ OPTS_S16 = OPTS_32[:4]
 G_DEBUG_32 = ["G." + n for n in ("z0", "h0", "z1", "h1", "z2", "h2", "z3", "y", "dz2", "dz1", "dz0",
                                  "bn_mean1", "bn_istd1", "bn_mean2", "bn_istd2")]
 G_DEBUG_S16 = ["G." + n for n in ("z0", "z1", "z2", "z3", "bn_mean1", "bn_istd1", "bn_mean2", "bn_istd2")]
+DSTEP = {"32": ("z1", "z2", "z3", "z4", "zl1", "zl2", "logit", "out"),
+         "s16": ("z1", "z2", "z3", "z4", "zf", "ze1", "ze2", "logit", "out"),
+         "c2f": ("z1", "z2", "z3", "z4", "zl1", "logit", "out")}
+ITERS = 2  # D and G iterations of the "iters2x2" mode
 
 
 def f32(a):
@@ -51,8 +58,9 @@ def stats_array(st):
     return np.concatenate([np.ravel(np.asarray(st[k], np.float64)) for k in sorted(st)])
 
 
-def steps(ctx, out, host_step, dev_step):
-    """3 host-fed, then 3 device-fed steps (eager, captured, replayed where the net captures graphs)"""
+def steps(ctx, out, host_step, dev_step, net=None, kind=None):
+    """3 host-fed, then 3 device-fed steps (eager, captured, replayed where the net captures graphs).  With `kind`
+    (debug_keep set), the Dstep.* tensors of `net` after each step too."""
     launches = []
     for i in range(6):
         l0 = ctx.launches()
@@ -60,10 +68,17 @@ def steps(ctx, out, host_step, dev_step):
         ctx.sync()
         launches.append(ctx.launches() - l0)
         out["stats_%d" % i] = stats_array(st)
+        for n in DSTEP.get(kind, ()):
+            out["Dstep.%s_%d" % (n, i)] = net.debug_tensor("Dstep." + n)
     return launches
 
 
-def case_32(B, opts, imgs):
+def n_rows(mode):
+    """the stacked iterations of one host-fed input ([] for the single-iteration entries)"""
+    return [ITERS] if mode == "iters2x2" else []
+
+
+def case_32(B, opts, imgs, mode="step"):
     import face_generator_b200 as fg
     from face_generator_b200 import layouts as LY
     from face_generator_b200.dataset import DeviceDataset
@@ -72,18 +87,27 @@ def case_32(B, opts, imgs):
     ctx = fg.Context(0, max_batch=B, channels=C)
     for k, v in opts.items():
         ctx.set_option(k, v)
+    if mode == "debug_keep":
+        ctx.set_option("debug_keep", 1)
     ctx.set_params(NET_G, LY.trained_like_init(LY.G_layout(C), rng))
     ctx.set_params(NET_D, LY.trained_like_init(LY.D_layout(C), rng, 1.4))
     ds = DeviceDataset(ctx, imgs)
     h = fg.hyper_default()
     out = {}
 
-    def host(seed):
-        real = f32(rng.random((B // 2, C, 32, 32)))
-        return ctx.train_step(h, B, real, f32(rng.uniform(-1, 1, (B // 2, 100))), f32(rng.uniform(-1, 1, (B, 100))),
-                              None, None, seed)
+    r = n_rows(mode)
 
-    launches = steps(ctx, out, host, lambda seed: ds.train_step(h, B, seed))
+    def host(seed):
+        real = f32(rng.random(r + [B // 2, C, 32, 32]))
+        zD, zG = f32(rng.uniform(-1, 1, r + [B // 2, 100])), f32(rng.uniform(-1, 1, r + [B, 100]))
+        if r:
+            return ctx.train_step_iters(h, B, ITERS, ITERS, real, zD, zG, None, None, seed)
+        return ctx.train_step(h, B, real, zD, zG, None, None, seed)
+
+    def dev(seed):
+        return ds.train_step_iters(h, B, ITERS, ITERS, seed) if r else ds.train_step(h, B, seed)
+
+    launches = steps(ctx, out, host, dev, ctx, "32" if mode == "debug_keep" else None)
     out.update(pair_state(ctx, True))
     out["G_forward"] = ctx.G_forward(f32(rng.uniform(-1, 1, (B, 100))), training=True)
     out["G_backward.dnoise"] = ctx.G_backward(f32(rng.standard_normal((B, C, 32, 32)) * 1e-2), want_dnoise=True)
@@ -98,7 +122,7 @@ def case_32(B, opts, imgs):
     return out, launches
 
 
-def case_s16(B, opts, imgs):
+def case_s16(B, opts, imgs, mode="step"):
     import face_generator_b200 as fg
     from face_generator_b200.dataset import DeviceDataset
     from face_generator_b200.lib import NET_D, NET_G
@@ -106,6 +130,8 @@ def case_s16(B, opts, imgs):
     ctx = fg.Context(0, max_batch=B, channels=C)
     for k, v in opts.items():
         ctx.set_option(k, v)
+    if mode == "debug_keep":
+        ctx.set_option("debug_keep", 1)
     net = fg.S16(ctx)
     net.set_params(NET_G, f32(rng.standard_normal(net.count(NET_G)) * 0.02))
     net.set_params(NET_D, f32(rng.standard_normal(net.count(NET_D)) * 0.02))
@@ -113,12 +139,19 @@ def case_s16(B, opts, imgs):
     h = fg.hyper_default()
     out = {}
 
-    def host(seed):
-        real = f32(rng.random((B // 2, C, 16, 16)))
-        return net.train_step(h, B, real, f32(rng.uniform(-1, 1, (B // 2, 100))), f32(rng.uniform(-1, 1, (B, 100))),
-                              None, None, seed)
+    r = n_rows(mode)
 
-    launches = steps(ctx, out, host, lambda seed: net.train_step_dataset(ds, h, B, seed))
+    def host(seed):
+        real = f32(rng.random(r + [B // 2, C, 16, 16]))
+        zD, zG = f32(rng.uniform(-1, 1, r + [B // 2, 100])), f32(rng.uniform(-1, 1, r + [B, 100]))
+        if r:
+            return net.train_step_iters(h, B, ITERS, ITERS, real, zD, zG, None, None, seed)
+        return net.train_step(h, B, real, zD, zG, None, None, seed)
+
+    def dev(seed):
+        return net.train_step_dataset_iters(ds, h, B, ITERS, ITERS, seed) if r else net.train_step_dataset(ds, h, B, seed)
+
+    launches = steps(ctx, out, host, dev, net, "s16" if mode == "debug_keep" else None)
     out.update(pair_state(net, True))
     out["G_forward"] = net.G_forward(f32(rng.uniform(-1, 1, (B, 100))), training=True)
     out["G_backward.dnoise"] = net.G_backward(f32(rng.standard_normal((B, C, 16, 16)) * 1e-2), want_dnoise=True)
@@ -133,33 +166,49 @@ def case_s16(B, opts, imgs):
     return out, launches
 
 
-def case_c2f(B, imgs, cs=16):
+def case_c2f(B, imgs, S=32, mode="step"):
     import face_generator_b200 as fg
     from face_generator_b200 import layouts as LY
     from face_generator_b200.dataset import DeviceDataset, noise_uniform
     from face_generator_b200.lib import NET_D, NET_G
     rng = np.random.default_rng(51)
+    cs = S // 2  # train_c2f.lua --coarseSize
     ctx = fg.Context(0, max_batch=B, channels=C)
-    net = fg.C2f(ctx)
+    if mode == "debug_keep":
+        ctx.set_option("debug_keep", 1)
+    net = fg.C2f(ctx, S)
     net.set_params(NET_G, LY.trained_like_init(LY.c2f_G_layout(C), rng, 1.2))
-    net.set_params(NET_D, LY.trained_like_init(LY.c2f_D_layout(C), rng, 1.0))
+    net.set_params(NET_D, LY.trained_like_init(LY.c2f_D_layout(C, S), rng, 1.0))
     ds = DeviceDataset(ctx, imgs)
     h = fg.hyper_default()
     out = {}
     Bh = B // 2
+    r = n_rows(mode)
+
+    def inputs(seed):
+        _, cr, dr = ds.gather_c2f(ds.draw(8 * seed, Bh), cs, S)
+        _, cf, _ = ds.gather_c2f(ds.draw(8 * seed + 1, Bh), cs, S)
+        _, cg, _ = ds.gather_c2f(ds.draw(8 * seed + 2, B), cs, S)
+        nD, nG = noise_uniform(ctx, 8 * seed + 3, (Bh, 1, S, S)), noise_uniform(ctx, 8 * seed + 4, (B, 1, S, S))
+        return dr, np.concatenate([cr, cf]), nD, cg, nG
 
     def host(seed):
-        _, cr, dr = ds.gather_c2f(ds.draw(8 * seed, Bh), cs)
-        _, cf, _ = ds.gather_c2f(ds.draw(8 * seed + 1, Bh), cs)
-        _, cg, _ = ds.gather_c2f(ds.draw(8 * seed + 2, B), cs)
-        nD, nG = noise_uniform(ctx, 8 * seed + 3, (Bh, 1, 32, 32)), noise_uniform(ctx, 8 * seed + 4, (B, 1, 32, 32))
-        return net.train_step(h, B, dr, np.concatenate([cr, cf]), nD, cg, nG, None, None, seed)
+        if not r:
+            return net.train_step(h, B, *inputs(seed), None, None, seed)
+        # the iterations' inputs stacked: any rows do, these are the single step's of seeds 1000 * seed + j
+        x = [f32(np.stack(a)) for a in zip(*(inputs(1000 * seed + j) for j in range(ITERS)))]
+        return net.train_step_iters(h, B, ITERS, ITERS, *x, None, None, seed)
 
-    launches = steps(ctx, out, host, lambda seed: net.train_step_dataset(ds, h, B, cs, seed))
+    def dev(seed):
+        if r:
+            return net.train_step_dataset_iters(ds, h, B, ITERS, ITERS, cs, seed)
+        return net.train_step_dataset(ds, h, B, cs, seed)
+
+    launches = steps(ctx, out, host, dev, net, "c2f" if mode == "debug_keep" else None)
     out.update(pair_state(net, False))
-    _, cond, diff = ds.gather_c2f(ds.draw(99, B), cs)
-    out["G_forward"] = net.G_forward(f32(rng.uniform(-1, 1, (B, 1, 32, 32))), cond)
-    net.G_backward(f32(rng.standard_normal((B, C, 32, 32)) * 1e-2))
+    _, cond, diff = ds.gather_c2f(ds.draw(99, B), cs, S)
+    out["G_forward"] = net.G_forward(f32(rng.uniform(-1, 1, (B, 1, S, S))), cond)
+    net.G_backward(f32(rng.standard_normal((B, C, S, S)) * 1e-2))
     out["D_forward"] = net.D_forward(diff, cond, None, True, 3)
     out["D_backward.ddiff"] = net.D_backward(f32(rng.standard_normal(B)), True, True)
     out["grads_G_after_calls"], out["grads_D_after_calls"] = net.get_grads(NET_G), net.get_grads(NET_D)
@@ -202,8 +251,16 @@ def run(args):
             cases += [("32.B%d.%s" % (B, n), lambda B=B, o=o: case_32(B, o, imgs)) for n, o in OPTS_32]
         if "s16" in only:
             cases += [("s16.B%d.%s" % (B, n), lambda B=B, o=o: case_s16(B, o, imgs)) for n, o in OPTS_S16]
+    for mode in ("iters2x2", "debug_keep"):
+        if "32" in only:
+            cases.append(("32.B256.%s" % mode, lambda m=mode: case_32(256, {}, imgs, m)))
+        if "s16" in only:
+            cases.append(("s16.B256.%s" % mode, lambda m=mode: case_s16(256, {}, imgs, m)))
+        if "c2f" in only:
+            cases.append(("c2f.B256.%s" % mode, lambda m=mode: case_c2f(256, imgs, 32, m)))
     if "c2f" in only:
         cases.append(("c2f.B256.default", lambda: case_c2f(256, imgs)))
+        cases += [("c2f%d.B256.default" % S, lambda S=S: case_c2f(256, imgs, S)) for S in (16, 64)]
     if "lop" in only:
         cases.append(("lop.conv2d_f16", case_lop))
     for name, fn in cases:
@@ -235,7 +292,7 @@ def compare(args):
                 n = int(np.sum(a != b)) if a.shape == b.shape else -1
                 first = "%s: %d elements differ" % (k, n)
                 break
-        bad += first is not None
+        bad += first is not None or la != lb
         print("%-28s %-34s launches/step A %s  B %s" % (name, first or "identical (%d arrays)" % len(keys), la, lb))
     print("%d case(s) differ" % bad)
     return 1 if bad else 0

@@ -75,7 +75,8 @@ def make_pairs(B, C, rng, fine_size):
 
 
 def rank_step(case, st, B, C, world, allreduce, fine_size, hyper=None):
-    """dp_ref_c2f.rank_step at fine size S (nets_c2f.cu::train_step for world > 1, restated with the CPU oracle)"""
+    """dp_ref_c2f.rank_step at fine size S (netpair.cu::pair_train_step on the c2f nets for world > 1, restated with
+    the CPU oracle)"""
     hp = hyper or CU.HYPER
     Bh = B // 2
     G, D = OS.f64.G(fine_size), OS.f64.D(fine_size)

@@ -1,7 +1,7 @@
 """Data-parallel semantics of the train step, restated with the CPU oracle (test infrastructure).
 
-Mirrors face_generator_b200/csrc/nets.cu::net_train_step for world > 1: every rank computes the gradient
-of ITS shard (BatchNorm statistics stay per replica), the flat gradient (+ confusion counts in the tail)
+Mirrors face_generator_b200/csrc/netpair.cu::pair_train_step on the 32x32 nets for world > 1: every rank computes the
+gradient of ITS shard (BatchNorm statistics stay per replica), the flat gradient (+ confusion counts in the tail)
 is sum-all-reduced, scaled by 1/N, then penalty -> clamp -> Adam run identically on every rank
 (SURVEY.md section 8e)."""
 import numpy as np

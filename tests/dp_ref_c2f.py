@@ -1,6 +1,6 @@
 """Data-parallel semantics of the coarse-to-fine train step, restated with the CPU oracle (test infrastructure).
-Mirrors face_generator_b200/csrc/nets_c2f.cu::train_step for world > 1: per-shard gradients, one sum-all-reduce of
-the flat gradient (+ the confusion counts in its tail) per optimizer step, 1/N, then penalty -> clamp -> Adam
+Mirrors face_generator_b200/csrc/netpair.cu::pair_train_step on the c2f nets for world > 1: per-shard gradients, one
+sum-all-reduce of the flat gradient (+ the confusion counts in its tail) per optimizer step, 1/N, then penalty -> clamp -> Adam
 identically on every rank (adversarial_c2f.lua:56-76, :104-112; SURVEY.md section 8e)."""
 import numpy as np
 

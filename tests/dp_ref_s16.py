@@ -1,6 +1,6 @@
 """Data-parallel semantics of fg_s16_train_step restated with the CPU oracle (test infrastructure): the same scheme as
 dp_ref.py (per-rank gradient of the rank's shard, sum-all-reduce of the flat gradient + confusion counts, 1/N, then
-penalty -> clamp -> Adam identically on every rank) on the --scale 16 nets (nets_s16.cu::train_step)."""
+penalty -> clamp -> Adam identically on every rank) on the --scale 16 nets (netpair.cu::pair_train_step)."""
 import numpy as np
 
 from oracle import oracle as O
