@@ -4,7 +4,7 @@
 //   dataset.lua:80-117  loadRandomImages: image.load(path, nbChannels, "float") then image.scale(img, 32, 32)
 //   adversarial.lua:244-249 / :276  the per-sample Lua loop that copies math.random(dataset:size()) images into
 //                       `inputs`, and NN_UTILS.createNoiseInputs (utils/nn_utils.lua:35-39: uniform(-1,1))
-// Decoding stays on the host (it happens once, at load time); what is kept on the GPU is the DECODED uint8 image
+// Decoding happens once, at load time (JPEG files on the GPU too, jpeg.cu); what is kept on the GPU is the DECODED uint8 image
 // at its original scale (dataset.originalScale = 64, dataset.lua:10), 4x smaller than the float tensors the
 // reference keeps.  fg_dataset_gather turns B indices into the normalised, down-scaled fp32 NCHW batch in one
 // kernel; fg_train_step_dataset draws the indices and both noise tensors on the device too, so a train step
@@ -18,14 +18,6 @@
 #include "fg_internal.h"
 #include "k_rng.cuh"
 #include "k_scale.cuh"
-
-struct fg_dataset {
-  fg_ctx* c = nullptr;
-  int64_t N = 0;
-  int Cs = 3, Hs = 64, Ws = 64;
-  uint8_t* data = nullptr;  // [N][Cs][Hs][Ws]
-  int32_t* idx = nullptr;   // [maxB] staging for host index lists / drawn indices
-};
 
 namespace {
 // image.load(..., "float") of channel ch of one cached image: byte/255, image.rgb2y when gray
@@ -368,6 +360,7 @@ int fg_dataset_destroy(fg_dataset* d) {
     // even if a later dataset is allocated at the same host address
     d->c->graph_epoch++;
   }
+  jpeg_scratch_free(d->jpeg);
   cudaFree(d->data);
   cudaFree(d->idx);
   delete d;

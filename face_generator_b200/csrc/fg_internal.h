@@ -606,6 +606,17 @@ struct DebugTensor {
 int64_t debug_tensor_copy(fg_ctx* c, const char* what, const DebugTensor* ents, size_t n_ents, const char* name, float* dst,
                           int64_t max_elems);
 
+// ---- dataset.cu / jpeg.cu: the device-resident dataset ----
+struct JpegScratch;                     // fg_dataset_upload_jpeg's chunk buffers (jpeg.cu), made on first use
+void jpeg_scratch_free(JpegScratch* s);
+struct fg_dataset {
+  fg_ctx* c = nullptr;
+  int64_t N = 0;
+  int Cs = 3, Hs = 64, Ws = 64;
+  uint8_t* data = nullptr;  // [N][Cs][Hs][Ws]
+  int32_t* idx = nullptr;   // [maxB] staging for host index lists / drawn indices
+  JpegScratch* jpeg = nullptr;
+};
 // ---- dataset.cu: inputs of the device-fed --scale 16 / coarse-to-fine steps (launches on the ctx stream) ----
 // root (optional): the stream is *root * kinds + seed, read on the device (a captured step replays with a new seed)
 int dataset_check_feed(const fg_dataset* d, const fg_ctx* c, const char* what);  // same ctx, compatible channels

@@ -5,6 +5,7 @@
     real = ds.gather(indices)                     # == image.scale(image.load(...), 32, 32) for those images
     real16 = ds.gather(indices, 16)               # the same at 16x16 (train.lua --scale 16)
     fine, coarse, diff = ds.gather_c2f(indices, 16)   # dataset_c2f.lua _toResult (train_c2f.lua --coarseSize 16)
+    ds = DeviceDataset.from_dirs(ctx, ["faces/"])  # dataset.loadImagesFromDirs: .jpg files decoded on the GPU
     stats = ds.train_step(hyper, B, seed)         # adversarial.lua loop body with no host->device traffic
     stats = ds.train_step_iters(hyper, B, 2, 1, seed)          # --D_iterations 2: two D iterations, one G iteration
     S16(ctx).train_step_dataset(ds, hyper, B, seed)            # the same for the --scale 16 nets
@@ -12,24 +13,144 @@
     C2f(ctx, 64).train_step_dataset(ds, hyper, B, 32, seed)    # the pyramid level 32x32 -> 64x64 (--fineSize 64)
 """
 import ctypes as C
+import os
 
 import numpy as np
 
-from .lib import Context, StepStats, _check, _stats, check_iters
+from .lib import Context, FGError, StepStats, _check, _stats, check_iters, load_library
+
+
+def list_image_files(dirs, ext="jpg", start_at=1, count=None):
+    """dataset.lua:156-190 loadImagesFromDirs' file list: the files of each directory whose name ends in `ext`, in the
+    order the directories are given, sorted by full path (byte order, as Lua's `<` on strings), then the 1-based
+    range [start_at, start_at + count)."""
+    files = []
+    for d in dirs:
+        files += [os.path.join(d, f) for f in os.listdir(d) if f.endswith(ext)]
+        if not files:
+            raise FileNotFoundError("given directory doesnt contain any files of type: " + ext)
+    files.sort(key=os.fsencode)
+    end = len(files) if count is None else min(start_at + count - 1, len(files))
+    return files[start_at - 1:end]
+
+
+def read_pgm(data):
+    """Binary (P5) 8-bit PGM bytes -> [1][H][W] uint8 (train_autoencoder.lua's lfwcrop_grey set)."""
+    fields, p = [], 2
+    if data[:2] != b"P5":
+        raise ValueError("not a binary PGM (P5) file")
+    while len(fields) < 3:
+        while p < len(data) and data[p:p + 1].isspace():
+            p += 1
+        if data[p:p + 1] == b"#":
+            while p < len(data) and data[p:p + 1] not in (b"\n", b"\r"):
+                p += 1
+            continue
+        q = p
+        while q < len(data) and not data[q:q + 1].isspace():
+            q += 1
+        if q == p:
+            raise ValueError("truncated PGM header")
+        fields.append(int(data[p:q]))
+        p = q
+    W, H, maxval = fields
+    if not 0 < maxval < 256:
+        raise ValueError("PGM maxval %d: only 8-bit PGM is supported" % maxval)
+    p += 1  # the single whitespace byte after maxval
+    if len(data) < p + W * H:
+        raise ValueError("truncated PGM data")
+    return np.frombuffer(data, np.uint8, W * H, p).reshape(1, H, W)
+
+
+def jpeg_info(data):
+    """(C, H, W) of JPEG bytes from their markers (fg_jpeg_info; host only)."""
+    lib = load_library()
+    c, h, w = C.c_int(), C.c_int(), C.c_int()
+    buf = np.frombuffer(data, np.uint8)
+    _check(lib.fg_jpeg_info(buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(c), C.byref(h), C.byref(w)), "fg_jpeg_info")
+    return c.value, h.value, w.value
 
 
 class DeviceDataset:
-    def __init__(self, ctx: Context, images_u8, chunk=8192):
-        images_u8 = np.ascontiguousarray(images_u8, np.uint8)
-        assert images_u8.ndim == 4, "[N][Cs][Hs][Ws] uint8"
-        N, Cs, Hs, Ws = images_u8.shape
+    def __init__(self, ctx: Context, images_u8=None, chunk=8192, shape=None):
+        """From decoded images [N][Cs][Hs][Ws] uint8, or an empty cache of `shape` = (N, Cs, Hs, Ws) to fill with
+        upload / upload_jpeg."""
+        if images_u8 is not None:
+            images_u8 = np.ascontiguousarray(images_u8, np.uint8)
+            assert images_u8.ndim == 4, "[N][Cs][Hs][Ws] uint8"
+            shape = images_u8.shape
+        N, Cs, Hs, Ws = shape
         self.ctx, self.lib, self.N = ctx, ctx.lib, N
+        self.shape = (N, Cs, Hs, Ws)
         h = C.c_void_p()
         _check(self.lib.fg_dataset_create(ctx.h, N, Cs, Hs, Ws, C.byref(h)), "fg_dataset_create")
         self.h = h
-        for s in range(0, N, chunk):  # dataset.loadImages(startAt, count) granularity
-            part = images_u8[s:s + chunk]
-            _check(self.lib.fg_dataset_upload(self.h, s, part.shape[0], part.ctypes.data_as(C.c_void_p)), "fg_dataset_upload")
+        if images_u8 is not None:
+            for s in range(0, N, chunk):  # dataset.loadImages(startAt, count) granularity
+                self.upload(s, images_u8[s:s + chunk])
+
+    @classmethod
+    def from_dirs(cls, ctx: Context, dirs, ext="jpg", start_at=1, count=None, channels=None, chunk=16384):
+        """dataset.loadImagesFromDirs(dirs, ext, startAt, count, doSort = true) into a device cache at the files'
+        own size (image.load(path, nbChannels, 'byte')): the cache is sized from the first file, every file must
+        match it.  JPEG files are decoded on the GPU, `chunk` files per call; ext "pgm" reads binary PGM on the host
+        (nothing to decode).  channels = the cache's Cs: default 3 for colour JPEG files (a 1-channel context then
+        gathers image.rgb2y of them), else the context's channel count."""
+        files = list_image_files(dirs, ext, start_at, count)
+        if not files:
+            raise FileNotFoundError("no %s files in the requested range" % ext)
+        pgm = ext.lower().endswith("pgm")
+        with open(files[0], "rb") as f:
+            head = f.read()
+        C0, Hs, Ws = read_pgm(head).shape if pgm else jpeg_info(head)
+        Cs = channels if channels is not None else (3 if C0 == 3 else ctx.C)
+        ds = cls(ctx, shape=(len(files), Cs, Hs, Ws))
+        try:
+            for s in range(0, len(files), chunk):
+                blobs = []
+                for fn in files[s:s + chunk]:
+                    with open(fn, "rb") as f:
+                        blobs.append(f.read())
+                if pgm:
+                    imgs = np.stack([read_pgm(b) for b in blobs])
+                    if imgs.shape[2:] != (Hs, Ws):
+                        raise ValueError("PGM files of different sizes in %s" % dirs)
+                    ds.upload(s, np.repeat(imgs, Cs, axis=1) if Cs == 3 else imgs)
+                else:
+                    try:
+                        ds.upload_jpeg(s, blobs)
+                    except FGError as e:
+                        raise FGError("%s (%s)" % (e, files[s + e.index] if e.index is not None else dirs)) from None
+        except Exception:
+            ds.close()
+            raise
+        return ds
+
+    def upload(self, first, images_u8):
+        """fg_dataset_upload: decoded images [n][Cs][Hs][Ws] uint8 into rows [first, first + n)."""
+        a = np.ascontiguousarray(images_u8, np.uint8)
+        _check(self.lib.fg_dataset_upload(self.h, first, a.shape[0], a.ctypes.data_as(C.c_void_p)), "fg_dataset_upload")
+
+    def upload_jpeg(self, first, files):
+        """fg_dataset_upload_jpeg: a list of JPEG files (bytes) decoded on the GPU into rows [first, first + n).
+        On failure the FGError carries .index, the position in `files` of the first failing file."""
+        offsets = np.zeros(len(files) + 1, np.int64)
+        offsets[1:] = np.cumsum([len(b) for b in files])
+        data = np.frombuffer(b"".join(files), np.uint8) if offsets[-1] else np.zeros(1, np.uint8)
+        failed = C.c_int64(-1)
+        rc = self.lib.fg_dataset_upload_jpeg(self.h, first, len(files), data.ctypes.data_as(C.c_void_p),
+                                             offsets.ctypes.data_as(C.c_void_p), C.byref(failed))
+        if rc != 0:
+            err = FGError("fg_dataset_upload_jpeg failed (%d): %s" % (rc, self.lib.fg_last_error().decode()))
+            err.rc, err.index = rc, (failed.value if failed.value >= 0 else None)
+            raise err
+
+    def download(self, first=0, count=None):
+        """fg_dataset_download: rows [first, first + count) of the cache, [count][Cs][Hs][Ws] uint8."""
+        count = self.N - first if count is None else count
+        out = np.empty((count,) + self.shape[1:], np.uint8)
+        _check(self.lib.fg_dataset_download(self.h, first, count, out.ctypes.data_as(C.c_void_p)), "fg_dataset_download")
+        return out
 
     def close(self):
         if self.h:

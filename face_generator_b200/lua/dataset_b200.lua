@@ -1,0 +1,126 @@
+-- dataset_b200.lua -- dataset.lua's loadImagesFromDirs (dataset.lua:156-211) straight into the device-resident
+-- training set: the .jpg files are read with io.open and decoded on the GPU (fg_dataset_upload_jpeg), so no image
+-- is decoded on the host.  .pgm files (train_autoencoder.lua's lfwcrop_grey set) are parsed here and uploaded as
+-- decoded planes (fg_dataset_upload).  The Python mirror is DeviceDataset.from_dirs (face_generator_b200/dataset.py).
+-- Delivered untested-by-execution (no LuaJIT/Torch7 in the build image).
+--
+--   local ds = b200.loadImagesToDevice(ctx, DATASET.dirs, 'jpg', 3, 1, 250000)
+--   F.check(C.fg_train_step_dataset(ctx, ds, hyper, B, seed, stats), 'fg_train_step_dataset')
+require 'paths'
+local ffi = require 'ffi'
+local F = require 'fg_ffi'
+local C = F.C
+
+b200 = b200 or {}
+
+local CHUNK = 16384  -- files per fg_dataset_upload_jpeg call: bounds the host bytes held at once
+
+-- the file list of loadImagesFromDirs with doSort = true: every file of each dir whose name ends in ext, sorted by
+-- full path, then files[startAt .. min(startAt+count-1, #files)]
+function b200.listImageFiles(dirs, ext, startAt, count)
+  local files = {}
+  for i = 1, #dirs do
+    for file in paths.files(dirs[i]) do
+      if file:find(ext .. '$') then
+        table.insert(files, paths.concat(dirs[i], file))
+      end
+    end
+    if #files == 0 then
+      error('given directory doesnt contain any files of type: ' .. ext)
+    end
+  end
+  table.sort(files, function (a, b) return a < b end)
+  local out = {}
+  for i = startAt, math.min(startAt + count - 1, #files) do
+    out[#out + 1] = files[i]
+  end
+  return out
+end
+
+local function readFile(path)
+  local f = assert(io.open(path, 'rb'))
+  local s = f:read('*a')
+  f:close()
+  return s
+end
+
+-- binary (P5) 8-bit PGM -> width, height, offset of the pixel bytes (1-based)
+local function pgmHeader(s, path)
+  assert(s:sub(1, 2) == 'P5', path .. ': not a binary PGM (P5) file')
+  local fields, p = {}, 3
+  while #fields < 3 do
+    local a, b = s:find('^%s+', p)
+    if a then p = b + 1 end
+    if s:sub(p, p) == '#' then
+      p = (s:find('[\r\n]', p) or #s) + 1
+    else
+      local num = s:match('^%d+', p)
+      assert(num, path .. ': bad PGM header')
+      fields[#fields + 1] = tonumber(num)
+      p = p + #num
+    end
+  end
+  assert(fields[3] > 0 and fields[3] < 256, path .. ': only 8-bit PGM is supported')
+  assert(#s >= p + fields[1] * fields[2], path .. ': truncated PGM data')
+  return fields[1], fields[2], p + 1
+end
+
+-- dataset.loadImagesFromDirs(dirs, ext, startAt, count, true) as an fg_dataset* of nbChannels planes at the files'
+-- own size (image.load(path, nbChannels, 'byte')), sized from the first file; every file must have that size.
+-- A colour JPEG under nbChannels = 1 is refused: load it with nbChannels = 3, a 1-channel ctx gathers rgb2y of it.
+function b200.loadImagesToDevice(ctx, dirs, ext, nbChannels, startAt, count)
+  ext = ext or 'jpg'
+  startAt = startAt or 1
+  count = count or math.huge
+  local files = b200.listImageFiles(dirs, ext, startAt, count)
+  assert(#files > 0, 'no ' .. ext .. ' files in the requested range')
+  local pgm = ext:lower():find('pgm$') ~= nil
+  local first = readFile(files[1])
+  local H, W
+  if pgm then
+    W, H = pgmHeader(first, files[1])
+  else
+    local c, h, w = ffi.new('int[1]'), ffi.new('int[1]'), ffi.new('int[1]')
+    F.check(C.fg_jpeg_info(ffi.cast('const uint8_t*', first), #first, c, h, w), 'fg_jpeg_info ' .. files[1])
+    H, W = h[0], w[0]
+  end
+  local out = ffi.new('fg_dataset*[1]')
+  F.check(C.fg_dataset_create(ctx, #files, nbChannels, H, W, out), 'fg_dataset_create')
+  local ds = ffi.gc(out[0], C.fg_dataset_destroy)
+  local failed = ffi.new('int64_t[1]')
+  for s = 1, #files, CHUNK do
+    local n = math.min(CHUNK, #files - s + 1)
+    if pgm then
+      local plane = H * W
+      local buf = ffi.new('uint8_t[?]', n * nbChannels * plane)
+      for i = 0, n - 1 do
+        local data = readFile(files[s + i])
+        local w, h, p = pgmHeader(data, files[s + i])
+        assert(w == W and h == H, files[s + i] .. ': PGM files of different sizes')
+        for c = 0, nbChannels - 1 do
+          ffi.copy(buf + (i * nbChannels + c) * plane, ffi.cast('const uint8_t*', data) + p - 1, plane)
+        end
+      end
+      F.check(C.fg_dataset_upload(ds, s - 1, n, buf), 'fg_dataset_upload')
+    else
+      local parts, offsets, total = {}, ffi.new('int64_t[?]', n + 1), 0
+      for i = 1, n do
+        parts[i] = readFile(files[s + i - 1])
+        offsets[i - 1] = total
+        total = total + #parts[i]
+      end
+      offsets[n] = total
+      local bytes = table.concat(parts)
+      parts = nil
+      local rc = C.fg_dataset_upload_jpeg(ds, s - 1, n, ffi.cast('const uint8_t*', bytes), offsets, failed)
+      if rc ~= 0 then
+        local where = failed[0] >= 0 and files[s + tonumber(failed[0])] or ''
+        error(string.format('fg_dataset_upload_jpeg failed (%d): %s %s', rc, ffi.string(C.fg_last_error()), where))
+      end
+      collectgarbage()
+    end
+  end
+  return ds
+end
+
+return b200

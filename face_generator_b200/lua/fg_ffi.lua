@@ -99,6 +99,9 @@ int fg_dataset_create(fg_ctx* ctx, int64_t N, int Cs, int Hs, int Ws, fg_dataset
 int fg_dataset_destroy(fg_dataset* d);
 int64_t fg_dataset_size(fg_dataset* d);
 int fg_dataset_upload(fg_dataset* d, int64_t first, int64_t count, const uint8_t* images);
+int fg_dataset_download(fg_dataset* d, int64_t first, int64_t count, uint8_t* out);
+int fg_jpeg_info(const uint8_t* bytes, int64_t len, int* C, int* H, int* W);
+int fg_dataset_upload_jpeg(fg_dataset* d, int64_t first, int64_t count, const uint8_t* bytes, const int64_t* offsets, int64_t* failed_out);
 int fg_dataset_gather(fg_dataset* d, const int32_t* idx, int B, float* out);
 int fg_dataset_draw(fg_dataset* d, uint64_t seed, int B, int32_t* idx_out);
 int fg_noise_uniform(fg_ctx* ctx, uint64_t seed, int64_t n, float* out);

@@ -326,6 +326,27 @@ int fg_dataset_create(fg_ctx* ctx, int64_t N, int Cs, int Hs, int Ws, fg_dataset
 int fg_dataset_destroy(fg_dataset* d);
 int64_t fg_dataset_size(fg_dataset* d);
 int fg_dataset_upload(fg_dataset* d, int64_t first, int64_t count, const uint8_t* images);
+/* the inverse of fg_dataset_upload: rows [first, first+count) into out (host or device), [count][Cs][Hs][Ws]  */
+int fg_dataset_download(fg_dataset* d, int64_t first, int64_t count, uint8_t* out);
+/* JPEG files straight into the cache (dataset.lua loadImagesFromDirs' image.load(path, Cs, 'byte')).
+ * Supported: baseline / extended sequential Huffman (SOF0, SOF1), 8-bit, one scan holding every
+ * component, 1 or 3 components, luma sampled 1x1, 2x1 or 2x2 with 1x1 chroma (4:4:4, 4:2:2, 4:2:0),
+ * DRI restarts; APPn / COM segments are skipped.  The output equals libjpeg-turbo's default
+ * decompression (islow IDCT, fancy upsampling) bit for bit.
+ * fg_jpeg_info: host only, needs no GPU; C, H, W of a file from its markers (any may be NULL).  A
+ * file outside the scope above is FG_ERR_UNSUPPORTED, a malformed header FG_ERR_INVALID, and
+ * fg_last_error names the reason.
+ * fg_dataset_upload_jpeg: file i = bytes[offsets[i] .. offsets[i+1]) (offsets has count+1 entries,
+ * host memory) goes to row first+i, planar [Cs][Hs][Ws]; a 1-component file under Cs = 3 is
+ * replicated to three planes, a 3-component file under Cs = 1 is refused.  Every header is checked
+ * before anything is launched; a size other than Hs x Ws, an unsupported format or corrupt /
+ * truncated entropy-coded data returns an error with *failed_out (may be NULL) = the index i of the
+ * first failing file (a header failure is reported before any decode), else -1.  After an error the
+ * rows [first, first+count) are unspecified.  Runs in bounded chunks on the ctx stream; returns once
+ * the host buffers may be reused.                                                                  */
+int fg_jpeg_info(const uint8_t* bytes, int64_t len, int* C, int* H, int* W);
+int fg_dataset_upload_jpeg(fg_dataset* d, int64_t first, int64_t count, const uint8_t* bytes, const int64_t* offsets,
+                           int64_t* failed_out);
 /* out [B][C][32][32] (host or device) for B 0-based indices (host or device int32)              */
 int fg_dataset_gather(fg_dataset* d, const int32_t* idx, int B, float* out);
 /* the counter-based streams fg_train_step_dataset draws from: B indices in [0,N) / n floats in
