@@ -6,6 +6,7 @@
     real16 = ds.gather(indices, 16)               # the same at 16x16 (train.lua --scale 16)
     fine, coarse, diff = ds.gather_c2f(indices, 16)   # dataset_c2f.lua _toResult (train_c2f.lua --coarseSize 16)
     ds = DeviceDataset.from_dirs(ctx, ["faces/"])  # dataset.loadImagesFromDirs: .jpg files decoded on the GPU
+    ds = DeviceDataset.from_lfw(ctx, ["lfw/"])     # generate_dataset.py's out_aug_64x64, built on the GPU from LFW
     stats = ds.train_step(hyper, B, seed)         # adversarial.lua loop body with no host->device traffic
     stats = ds.train_step_iters(hyper, B, 2, 1, seed)          # --D_iterations 2: two D iterations, one G iteration
     S16(ctx).train_step_dataset(ds, hyper, B, seed)            # the same for the --scale 16 nets
@@ -32,6 +33,35 @@ def list_image_files(dirs, ext="jpg", start_at=1, count=None):
     files.sort(key=os.fsencode)
     end = len(files) if count is None else min(start_at + count - 1, len(files))
     return files[start_at - 1:end]
+
+
+def list_lfw_files(dirs):
+    """dataset/generate_dataset.py's walk: the files of each given directory and of its direct subdirectories whose
+    name matches `.jpg$`, sorted by full path in byte order (as list_image_files).  The reference took the files in
+    the order of a set() of directories and os.listdir, which is unspecified; sorting makes the row order, and with
+    it every augmentation drawn for a photo, reproducible."""
+    files = []
+    for d in dirs:
+        subs = [d] + sorted(os.path.join(d, s) for s in os.listdir(d) if os.path.isdir(os.path.join(d, s)))
+        for sd in subs:
+            files += [os.path.join(sd, f) for f in os.listdir(sd)
+                      if f.endswith(".jpg") and os.path.isfile(os.path.join(sd, f))]
+    files = sorted(set(files), key=os.fsencode)
+    return files
+
+
+# fg_aug (include/fg_b200.h)
+AUG_DTYPE = np.dtype([("src", "<i8"), ("warp", "<i4"), ("hflip", "<i4"), ("brightness", "<f8"), ("m", "<f8", (9,))])
+
+
+def lfw_aug_params(seed, first_src, n_src, n_aug, src_h, src_w):
+    """fg_lfw_aug_params (host only): the n_src * (1 + n_aug) descriptors of photos [first_src, first_src + n_src),
+    photo-major, as an AUG_DTYPE array; src is the global photo index."""
+    out = np.zeros(n_src * (1 + n_aug), AUG_DTYPE)
+    lib = load_library()
+    _check(lib.fg_lfw_aug_params(seed, first_src, n_src, n_aug, src_h, src_w, out.ctypes.data_as(C.c_void_p)),
+           "fg_lfw_aug_params")
+    return out
 
 
 def read_pgm(data):
@@ -125,6 +155,51 @@ class DeviceDataset:
             ds.close()
             raise
         return ds
+
+    @classmethod
+    def from_lfw(cls, ctx: Context, dirs, augmentations=19, seed=43, size=64, chunk=2048):
+        """dataset/generate_dataset.py on the GPU: the augmented LFW training set (out_aug_64x64 with the defaults,
+        out_unaug_64x64 with augmentations=0) straight into a device cache of len(files) * (1 + augmentations) rows,
+        3 planes (a 1-channel context gathers image.rgb2y of them), size x size.  Row i * (1 + augmentations) + a is
+        augmentation a of photo i of list_lfw_files(dirs), a = 0 the photo itself: the order of the reference's file
+        names {i:06}_{a:03}.jpg.  The photos are decoded on the GPU `chunk` at a time into a scratch cache that the
+        chunk's rows are built from (fg_dataset_upload_jpeg, fg_dataset_augment); the descriptors come from
+        fg_lfw_aug_params(seed), so the result does not depend on `chunk`."""
+        files = list_lfw_files(dirs)
+        if not files:
+            raise FileNotFoundError("no .jpg files in %s or their direct subdirectories" % (dirs,))
+        with open(files[0], "rb") as f:
+            _, Hs, Ws = jpeg_info(f.read())
+        per = 1 + augmentations
+        ds = cls(ctx, shape=(len(files) * per, 3, size, size))
+        try:
+            for s in range(0, len(files), chunk):
+                blobs = []
+                for fn in files[s:s + chunk]:
+                    with open(fn, "rb") as f:
+                        blobs.append(f.read())
+                scratch = cls(ctx, shape=(len(blobs), 3, Hs, Ws))
+                try:
+                    try:
+                        scratch.upload_jpeg(0, blobs)
+                    except FGError as e:
+                        raise FGError("%s (%s)" % (e, files[s + e.index] if e.index is not None else dirs)) from None
+                    augs = lfw_aug_params(seed, s, len(blobs), augmentations, Hs, Ws)
+                    augs["src"] -= s  # rows of the scratch cache
+                    ds.augment(scratch, s * per, augs)
+                finally:
+                    scratch.close()
+        except Exception:
+            ds.close()
+            raise
+        return ds
+
+    def augment(self, src, first, augs):
+        """fg_dataset_augment: rows [first, first + len(augs)) of this cache from rows of `src` (a cache on the same
+        context), one AUG_DTYPE descriptor per row."""
+        a = np.ascontiguousarray(augs, AUG_DTYPE)
+        _check(self.lib.fg_dataset_augment(src.h, self.h, first, a.ctypes.data_as(C.c_void_p), a.size),
+               "fg_dataset_augment")
 
     def upload(self, first, images_u8):
         """fg_dataset_upload: decoded images [n][Cs][Hs][Ws] uint8 into rows [first, first + n)."""

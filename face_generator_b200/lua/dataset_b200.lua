@@ -4,7 +4,10 @@
 -- decoded planes (fg_dataset_upload).  The Python mirror is DeviceDataset.from_dirs (face_generator_b200/dataset.py).
 -- Delivered untested-by-execution (no LuaJIT/Torch7 in the build image).
 --
+-- b200.loadLFWToDevice builds the augmented LFW set those trainers read (dataset/generate_dataset.py) from LFW itself.
+--
 --   local ds = b200.loadImagesToDevice(ctx, DATASET.dirs, 'jpg', 3, 1, 250000)
+--   local ds = b200.loadLFWToDevice(ctx, {'/data/lfw'}, 19, 43)   -- out_aug_64x64, on the GPU
 --   F.check(C.fg_train_step_dataset(ctx, ds, hyper, B, seed, stats), 'fg_train_step_dataset')
 require 'paths'
 local ffi = require 'ffi'
@@ -119,6 +122,89 @@ function b200.loadImagesToDevice(ctx, dirs, ext, nbChannels, startAt, count)
       end
       collectgarbage()
     end
+  end
+  return ds
+end
+
+-- dataset/generate_dataset.py's walk: the .jpg files of each dir and of its direct subdirectories, sorted by full path
+-- (the reference's order came from a set() and os.listdir, which is unspecified)
+function b200.listLFWFiles(dirs)
+  local files, seen = {}, {}
+  local function add(dir)
+    for file in paths.files(dir) do
+      local p = paths.concat(dir, file)
+      if file:find('%.jpg$') and paths.filep(p) and not seen[p] then
+        seen[p] = true
+        files[#files + 1] = p
+      end
+    end
+  end
+  for i = 1, #dirs do
+    add(dirs[i])
+    for sub in paths.files(dirs[i]) do
+      if sub ~= '.' and sub ~= '..' and paths.dirp(paths.concat(dirs[i], sub)) then
+        add(paths.concat(dirs[i], sub))
+      end
+    end
+  end
+  table.sort(files, function (a, b) return a < b end)
+  return files
+end
+
+-- generate_dataset.py on the GPU (the Python mirror is DeviceDataset.from_lfw): an fg_dataset* of
+-- #files * (1 + augmentations) rows of 3 x size x size, row i * (1 + augmentations) + a = augmentation a of photo i
+-- (a = 0: the photo itself), the order of the reference's {i:06}_{a:03}.jpg names.  augmentations = 19 (default) is
+-- out_aug_64x64, 0 is out_unaug_64x64; seed defaults to generate_dataset.py's 43.  Photos are decoded on the GPU
+-- `chunk` at a time into a scratch cache and augmented from there (fg_dataset_upload_jpeg, fg_lfw_aug_params,
+-- fg_dataset_augment).
+function b200.loadLFWToDevice(ctx, dirs, augmentations, seed, size, chunk)
+  augmentations = augmentations or 19
+  seed = seed or 43
+  size = size or 64
+  chunk = chunk or 2048
+  local files = b200.listLFWFiles(dirs)
+  assert(#files > 0, 'no .jpg files in the given directories or their direct subdirectories')
+  local first = readFile(files[1])
+  local c, h, w = ffi.new('int[1]'), ffi.new('int[1]'), ffi.new('int[1]')
+  F.check(C.fg_jpeg_info(ffi.cast('const uint8_t*', first), #first, c, h, w), 'fg_jpeg_info ' .. files[1])
+  local H, W = h[0], w[0]
+  local per = 1 + augmentations
+  local out = ffi.new('fg_dataset*[1]')
+  F.check(C.fg_dataset_create(ctx, #files * per, 3, size, size, out), 'fg_dataset_create')
+  local ds = ffi.gc(out[0], C.fg_dataset_destroy)
+  local failed = ffi.new('int64_t[1]')
+  for s = 1, #files, chunk do
+    local n = math.min(chunk, #files - s + 1)
+    local parts, offsets, total = {}, ffi.new('int64_t[?]', n + 1), 0
+    for i = 1, n do
+      parts[i] = readFile(files[s + i - 1])
+      offsets[i - 1] = total
+      total = total + #parts[i]
+    end
+    offsets[n] = total
+    local bytes = table.concat(parts)
+    parts = nil
+    local sc = ffi.new('fg_dataset*[1]')
+    F.check(C.fg_dataset_create(ctx, n, 3, H, W, sc), 'fg_dataset_create')
+    local rc = C.fg_dataset_upload_jpeg(sc[0], 0, n, ffi.cast('const uint8_t*', bytes), offsets, failed)
+    if rc ~= 0 then
+      local msg = ffi.string(C.fg_last_error())
+      C.fg_dataset_destroy(sc[0])
+      local where = failed[0] >= 0 and files[s + tonumber(failed[0])] or ''
+      error(string.format('fg_dataset_upload_jpeg failed (%d): %s %s', rc, msg, where))
+    end
+    local augs = ffi.new('fg_aug[?]', n * per)
+    rc = C.fg_lfw_aug_params(seed, s - 1, n, augmentations, H, W, augs)
+    if rc == 0 then
+      for k = 0, n * per - 1 do
+        augs[k].src = augs[k].src - (s - 1)  -- rows of the scratch cache
+      end
+      rc = C.fg_dataset_augment(sc[0], ds, (s - 1) * per, augs, n * per)
+    end
+    local msg = rc ~= 0 and ffi.string(C.fg_last_error()) or nil
+    C.fg_dataset_destroy(sc[0])
+    if msg then error(string.format('LFW augmentation failed (%d): %s', rc, msg)) end
+    collectgarbage()
   end
   return ds
 end

@@ -347,6 +347,36 @@ int fg_dataset_download(fg_dataset* d, int64_t first, int64_t count, uint8_t* ou
 int fg_jpeg_info(const uint8_t* bytes, int64_t len, int* C, int* H, int* W);
 int fg_dataset_upload_jpeg(fg_dataset* d, int64_t first, int64_t count, const uint8_t* bytes, const int64_t* offsets,
                            int64_t* failed_out);
+/* The augmented LFW training set (dataset/generate_dataset.py + ImageAugmenter.py): each output row
+ * is LFW-crop's 84x84 box (rows 92..175, cols 83..166) of a source row, resized to the destination's
+ * Ho x Wo as Pillow's Image.resize(BILINEAR) does (scipy.misc.imresize).  A descriptor with warp = 1
+ * first flips the source horizontally (hflip = 1), scales it by `brightness` with truncation to
+ * uint8, and warps it as skimage.transform.warp(img, m, mode="constant") at order 1: m is the
+ * row-major 3x3 INVERSE map from output (x = col, y = row) to input coordinates, evaluated in
+ * float64 without FMA contraction, bilinear taps outside the image read 0, the result is clipped to
+ * the brightened source's [min, max] (exact zeros kept when min > 0) and truncated to uint8.  warp = 0
+ * is the photo itself: crop and resize only (hflip, brightness and m are ignored).
+ * fg_lfw_aug_params: host only, needs no GPU.  Fills n_src * (1 + n_aug) descriptors: row
+ * (i - first_src) * (1 + n_aug) + a for source photo i in [first_src, first_src + n_src) and a in
+ * [0, n_aug]; src = i, a = 0 is warp = 0, a >= 1 draws generate_dataset.py's distributions (scale
+ * U[0.82, 1.10) on both axes, integer degrees in [-8, 8], integer translations in [-5, 5], hflip
+ * with p = 1/2, brightness U[0.9, 1.1)) from counter-based streams keyed by (seed, i, a), so a slice
+ * gives the same descriptors as the whole.  m = inverse of T(+shift) A T(-shift) with shift =
+ * (src_h / 2, src_w / 2) for (x, y) (the reference's width/height swap), third row [0, 0, 1].
+ * fg_dataset_augment: rows [dst_first, dst_first + n) of dst from the descriptors augs[0..n) (host
+ * memory), on the ctx stream; returns when the rows are written.  Refused before anything is
+ * launched (FG_ERR_INVALID, fg_last_error names the reason): caches on different contexts,
+ * different channel counts, a source smaller than 176 x 167, a destination side outside [1, 84], a
+ * descriptor whose src is out of range, whose warp / hflip is not 0 or 1, whose brightness is not
+ * finite and >= 0 or whose m is not finite.                                                          */
+typedef struct fg_aug {
+  int64_t src;
+  int32_t warp, hflip;
+  double brightness;
+  double m[9];
+} fg_aug;
+int fg_lfw_aug_params(uint64_t seed, int64_t first_src, int64_t n_src, int n_aug, int src_h, int src_w, fg_aug* out);
+int fg_dataset_augment(fg_dataset* src, fg_dataset* dst, int64_t dst_first, const fg_aug* augs, int64_t n);
 /* out [B][C][32][32] (host or device) for B 0-based indices (host or device int32)              */
 int fg_dataset_gather(fg_dataset* d, const int32_t* idx, int B, float* out);
 /* the counter-based streams fg_train_step_dataset draws from: B indices in [0,N) / n floats in
