@@ -429,10 +429,8 @@ int fg_bce_backward(fg_ctx* c, const float* x, const float* t, int n, float* dx)
 int fg_optim_step(fg_ctx* c, int net, const fg_hyper* h, float grad_scale) {
   ENTER(c);
   FG_REQUIRE(h && (net == FG_NET_G || net == FG_NET_D), "fg_optim_step: bad arguments");
-  // no accuracy information at this level: force the gate open by clearing the history influence
-  fg_hyper hh = *h;
-  hh.D_maxAcc = 2.0f;
-  FG_TRY(pair_gate(c, c->net, net, &hh, 1, 1.0f));
+  // no accuracy information at this level: no gate, and the fused steps' accuracy history is not touched
+  FG_TRY(k_optim_prep(c, c->net.dstats, net, h));
   return pair_optim(c, c->net, net, h, grad_scale);
 }
 int fg_adam_step(fg_ctx* c, float* p, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2,

@@ -442,6 +442,8 @@ int k_penalty_loss(fg_ctx* c, const float* p, int64_t n, float l1, float l2, flo
 // accumulate: conf and trained_D add to the values of the earlier D iterations of the same step instead of replacing them
 int k_gate_and_prep(fg_ctx* c, DeviceStats* st, float* acc_hist, int net, const fg_hyper* h, const float* tail4, int B,
                     float world, bool accumulate = false);
+// no gate: t += 1 and the step size of `net` for its update rule (fg_optim_step); the accuracy state is left alone
+int k_optim_prep(fg_ctx* c, DeviceStats* st, int net, const fg_hyper* h);
 int k_gemv_fwd(fg_ctx* c, const float* x, const float* w, const float* bias, float* out, int B, int K);
 int k_gemv_dgrad(fg_ctx* c, const float* dy, const float* w, float* dx, int B, int K);
 int k_gemv_wgrad_add(fg_ctx* c, const float* x, const float* dy, float* dw, float* db, int B, int K);

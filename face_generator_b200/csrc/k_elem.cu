@@ -1121,6 +1121,26 @@ int k_gate_and_prep(fg_ctx* c, DeviceStats* st, float* acc_hist, int net, const 
   LAUNCH_CHECK(c);
   return FG_OK;
 }
+// fg_optim_step: a module-level step has no batch accuracy, so it opens the update and advances t / the step size of
+// `net` only.  The accuracy history, conf, acc_D and trained_D belong to the fused steps' D iterations and stay as
+// they are.
+__global__ void optim_prep_kernel(DeviceStats* st, int net, fg_hyper h, int opt) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  if (net == FG_NET_D) {
+    st->do_train_D = 1;
+    st->t_D += 1;
+    st->step_D = step_size(h, opt, h.lr_D, (double)st->t_D);
+  } else {
+    st->do_train_G = 1;
+    st->t_G += 1;
+    st->step_G = step_size(h, opt, h.lr_G, (double)st->t_G);
+  }
+}
+int k_optim_prep(fg_ctx* c, DeviceStats* st, int net, const fg_hyper* h) {
+  optim_prep_kernel<<<1, 32, 0, c->stream>>>(st, net, *h, net == FG_NET_D ? c->opt_D : c->opt_G);
+  LAUNCH_CHECK(c);
+  return FG_OK;
+}
 // g = grad*scale; g += l1_grad*sign(p) + l2*p; clamp; m,v EMA; p -= step*m/(sqrt(v)+eps); grads written back
 __global__ void adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
                             int64_t n, float beta1, float beta2, float eps, float l1_grad, float l2, float clampv,

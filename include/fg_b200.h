@@ -157,7 +157,11 @@ int fg_bce_forward(fg_ctx* ctx, const float* x, const float* t, int n, float* lo
 int fg_bce_backward(fg_ctx* ctx, const float* x, const float* t, int n, float* dx);
 /* penalty + clamp + interruptableAdam (or the optimizer chosen with "optimizer_D"/"optimizer_G")
  * on the ctx's own buffers (adversarial.lua:103-123, interruptable_optimizers.lua:7-167).
- * grad_scale multiplies the gradient first (1/N for DP).                                         */
+ * grad_scale multiplies the gradient first (1/N for DP).  The step is never gated: it advances t
+ * of `net` and steps it, and leaves D's accuracy history, conf, acc_D and trained_D as the last
+ * fused step left them (a module-level step has no batch accuracy; adversarial.lua's gate only
+ * sees the fused steps' accuracies).  The clamp is fminf(fmaxf(g, -c), c): a NaN gradient element
+ * becomes -c under a clamp (Torch's CPU clamp keeps the NaN) and stays NaN without one.          */
 int fg_optim_step(fg_ctx* ctx, int net, const fg_hyper* h, float grad_scale);
 
 /* ---- L-op: raw-pointer optimizer for b200.Adam (DEVICE pointers) ----------------------------- */
