@@ -1,10 +1,11 @@
-// C ABI of libfg_b200.so (include/fg_b200.h).  Thin: argument checking, host/device pointer
-// classification, NCHW<->NHWC at the boundary, then nets.cu / kernels.
+// C ABI of libfg_b200.so (include/fg_b200.h): the context (fg_ctx: its stream, options and shared workspaces), the
+// last error, host/device pointer classification, events and timers.  The entry points of each net sit next to its code
+// (nets.cu, nets_s16.cu, nets_c2f.cu, ...).
+#include <algorithm>
 #include <cstdarg>
 #include <cstdlib>
 #include <cstring>
 
-#include "convl.h"
 #include "fg_internal.h"
 #include "k_conv_tc.h"
 
@@ -71,22 +72,32 @@ int64_t debug_tensor_copy(fg_ctx* c, const char* what, const DebugTensor* ents, 
 }
 
 namespace {
-// d_iters D iterations + g_iters G iterations of the loop body on inputs stacked per iteration, for the entry `what`
-int train_step_iters(fg_ctx* c, const char* what, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,
-                     const float* noise_D, const float* noise_G, const float* masks_D, const float* masks_G, uint64_t seed,
-                     fg_step_stats* stats) {
-  ENTER(c);
-  FG_TRY(step_check(c, what, B, d_iters, g_iters, h && real && noise_D && noise_G));
-  const size_t nd = d_iters, ng = g_iters, Bh = B / 2, M = c->maxB, img = (size_t)c->C * 1024;
-  IterStage& s = c->iter_stage;
-  const float *r, *zd, *zg, *md, *mg;
-  FG_TRY(s.in(c, c->allocs, 0, real, nd * Bh * img, nd * M / 2 * img, &r));
-  FG_TRY(s.in(c, c->allocs, 1, noise_D, nd * Bh * kNoiseDim, nd * M / 2 * kNoiseDim, &zd));
-  FG_TRY(s.in(c, c->allocs, 2, noise_G, ng * B * kNoiseDim, ng * M * kNoiseDim, &zg));
-  FG_TRY(s.in(c, c->allocs, 3, masks_D, nd * B * kMaskPerSample, nd * M * kMaskPerSample, &md));
-  FG_TRY(s.in(c, c->allocs, 4, masks_G, ng * B * kMaskPerSample, ng * M * kMaskPerSample, &mg));
-  NetStep st(c, h, B, r, zd, zg);
-  return pair_train_step(st, d_iters, g_iters, md, mg, seed, {r, zd, zg, md, mg, nullptr}, nullptr, stats);
+// the workspaces every net on the context shares
+int ctx_alloc(fg_ctx* c) {
+  const size_t B = c->maxB, C = c->C;
+  auto dalloc = [c](auto** p, size_t n) { return fg_dalloc(c, c->allocs, reinterpret_cast<float**>(p), n); };
+  FG_TRY(dalloc(&c->lop_sx, 2));
+  FG_TRY(dalloc(&c->lop_sy, 2));
+  FG_TRY(dalloc(&c->seed_dev, 2 * kMaxIters));  // one stream root per iteration (k_seed_roots)
+  c->splitk_ws_elems = (size_t)c->sm_count * 4 * 128 * 128;  // >= splits x output of every split-K weight gradient
+  FG_TRY(dalloc(&c->splitk_ws, c->splitk_ws_elems));
+  c->red_ws_elems = (size_t)4 << 20;  // >= blocks x partials of every ordered reduction (checked at each launch)
+  FG_TRY(dalloc(&c->red_ws, 2 * c->red_ws_elems));
+  FG_TRY(dalloc(&c->red_ws_opt, 2 * kOptRedRows));
+  FG_TRY(dalloc(&c->red_ticket, 2));  // zeroed; every ordered reduction resets its ticket
+  FG_TRY(dalloc(&c->bwd_claim, 1));
+  FG_TRY(dalloc(&c->small_ws, (size_t)kSmallMaxParts * 9 * 4 * 128));
+  FG_TRY(dalloc(&c->bn_acc, 4 * 256 * 2));  // doubles
+  FG_TRY(dalloc(&c->bn_slice_acc, 32 * 4 * 256 * 2 + 64));  // doubles + tickets (zero-initialised)
+  FG_TRY(dalloc(&c->bn_parts, B * 3072));  // G.C2: 8 tiles/image x 3 x 128 ch; G.C1: 2 tiles/image x 3 x 256 ch
+  c->io_dev_elems = std::max<size_t>(B * 1024 * C, B * kMaskPerSample);
+  return dalloc(&c->io_dev, c->io_dev_elems);
+}
+void ctx_free(fg_ctx* c) {
+  for (void* p : c->allocs) cudaFree(p);
+  c->allocs.clear();
+  for (int i = 0; i < 8; ++i)
+    if (c->scratch[i]) cudaFree(c->scratch[i]);
 }
 }  // namespace
 
@@ -135,10 +146,12 @@ int fg_create(fg_ctx** out, int device, int max_batch, int channels) {
     delete c;
     return FG_ERR_CUDA;
   }
-  int r = net_alloc(c);
+  int r = ctx_alloc(c);
+  if (r == FG_OK) r = net32_alloc(c);
   if (r == FG_OK) r = tc_init(c);
   if (r != FG_OK) {
-    net_free(c);
+    net32_free(c);
+    ctx_free(c);
     cudaStreamDestroy(c->stream);
     delete c;
     return r;
@@ -158,7 +171,8 @@ int fg_destroy(fg_ctx* c) {
     cudaEventDestroy(c->ev_join);
   }
   tc_destroy(c);
-  net_free(c);
+  net32_free(c);
+  ctx_free(c);
   for (auto& kv : c->timers)
     for (auto& pr : kv.second.pending) {
       cudaEventDestroy(pr.first);
@@ -194,11 +208,11 @@ int fg_set_option(fg_ctx* c, const char* key, int64_t v) {
   if (!strcmp(key, "conv_impl")) {
     FG_REQUIRE(v >= 0 && v <= 2, "conv_impl must be 0 (simt), 1 (tc dense) or 2 (tc collapsed)");
     c->conv_impl = (int)v;
-    c->net.G_packed = c->net.D_packed = false;
     return FG_OK;
   }
   if (!strcmp(key, "params_dirty")) {
-    c->net.G_packed = c->net.D_packed = false;
+    NetPair& p = net32_pair(c);
+    p.G_pack = p.D_pack = -1;
     return FG_OK;
   }
   if (!strcmp(key, "edge_impl")) {  // 1 (default): k_conv_edge.cu for the 3-channel-side convolutions; 0: k_conv_small.cu
@@ -211,7 +225,6 @@ int fg_set_option(fg_ctx* c, const char* key, int64_t v) {
   }
   if (!strcmp(key, "mma_f16")) {  // 1: K-major tensor-core kernels (forward, dgrad) use the 3xFP16 split + f16 MMAs
     c->mma_f16 = v != 0;
-    c->net.G_packed = c->net.D_packed = false;
     return FG_OK;
   }
   if (!strcmp(key, "use_graph")) {  // 1 (default): fg_train_step replays a captured CUDA graph of the step
@@ -279,160 +292,6 @@ int64_t fg_get_option(fg_ctx* c, const char* key) {
   return -1;
 }
 
-int64_t fg_param_count(int net, int channels) {
-  if (channels != 1 && channels != 3) return -1;
-  return net == FG_NET_G ? make_g_layout(channels, 32).total : net == FG_NET_D ? make_d_layout(channels).total : -1;
-}
-int fg_set_params(fg_ctx* c, int net, const float* src) {
-  ENTER(c);
-  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
-  return pair_set_params(c, c->net, net, src);
-}
-int fg_get_params(fg_ctx* c, int net, float* dst) {
-  ENTER(c);
-  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
-  return pair_get_params(c, c->net, net, dst);
-}
-int fg_get_grads(fg_ctx* c, int net, float* dst) {
-  ENTER(c);
-  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
-  return pair_get_grads(c, c->net, net, dst);
-}
-int fg_zero_grads(fg_ctx* c, int net) {
-  ENTER(c);
-  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
-  return pair_zero_grads(c, c->net, net);
-}
-// Borrow caller-owned DEVICE buffers as the flat parameter / gradient vectors of `net` (see include/fg_b200.h).
-int fg_bind_params(fg_ctx* c, int net, float* params_dev, float* grads_dev) {
-  ENTER(c);
-  c->graph_epoch++;
-  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
-  for (const float* p : {params_dev, grads_dev}) {
-    if (!p) continue;
-    FG_REQUIRE(fg_is_dev(p), "fg_bind_params: buffers must be DEVICE memory (CudaTensor:data())");
-    FG_REQUIRE(reinterpret_cast<uintptr_t>(p) % 16 == 0, "fg_bind_params: buffers must be 16-byte aligned");
-  }
-  FG_CUDA(cudaStreamSynchronize(c->stream));
-  NetPair& np = c->net;
-  const bool d = net == FG_NET_D;
-  (d ? np.PD : np.PG) = params_dev ? params_dev : (d ? c->ownPD : c->ownPG);
-  float* own_g = d ? c->ownGD : c->ownGG;
-  const int64_t n = d ? np.nD : np.nG;
-  (d ? np.gD : np.gG) = grads_dev ? grads_dev : own_g;
-  (d ? np.tailD : np.tailG) = grads_dev ? c->tail_sep + (d ? kGradTail : 0) : own_g + n;
-  np.G_packed = np.D_packed = false;
-  return FG_OK;
-}
-float* fg_params_ptr(fg_ctx* c, int net) { return !c ? nullptr : net == FG_NET_D ? c->net.PD : net == FG_NET_G ? c->net.PG : nullptr; }
-float* fg_grads_ptr(fg_ctx* c, int net) { return !c ? nullptr : net == FG_NET_D ? c->net.gD : net == FG_NET_G ? c->net.gG : nullptr; }
-
-int fg_set_adam_state(fg_ctx* c, int net, const float* m, const float* v, int t) {
-  ENTER(c);
-  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
-  return pair_set_adam_state(c, c->net, net, m, v, t);
-}
-int fg_get_adam_state(fg_ctx* c, int net, float* m, float* v, int* t) {
-  ENTER(c);
-  FG_REQUIRE(net == FG_NET_G || net == FG_NET_D, "net must be FG_NET_G or FG_NET_D");
-  return pair_get_adam_state(c, c->net, net, m, v, t);
-}
-int fg_set_bn_state(fg_ctx* c, const float* src) {
-  ENTER(c);
-  return pair_set_bn_state(c, c->net, src);
-}
-int fg_get_bn_state(fg_ctx* c, float* dst) {
-  ENTER(c);
-  return pair_get_bn_state(c, c->net, dst);
-}
-
-// ---- L-net ------------------------------------------------------------------------------------------
-int fg_G_forward(fg_ctx* c, const float* noise, int B, int training, float* images_out) {
-  ENTER(c);
-  FG_REQUIRE(noise && B >= 1 && B <= c->maxB, "fg_G_forward: bad arguments (B=%d, max %d)", B, c->maxB);
-  c->net.G_packed = false;  // parameters may have been edited through fg_params_ptr()
-  const float* nd;
-  FG_TRY(fg_to_dev(c, noise, (size_t)B * kNoiseDim, c->in_noiseG, &nd));
-  FG_TRY(gen_forward(c->env, c->G, c->net, nd, B, training != 0));
-  if (images_out) {
-    FG_TRY(k_nhwc_to_nchw(c, c->G.y, c->io_dev, B, c->C, 1024));
-    FG_TRY(fg_to_user(c, images_out, c->io_dev, (size_t)B * c->C * 1024));
-  }
-  return FG_OK;
-}
-int fg_G_backward(fg_ctx* c, const float* d_images, float* d_noise) {
-  ENTER(c);
-  FG_REQUIRE(d_images, "fg_G_backward: d_images is null");
-  const int B = c->G.B;
-  const float* dd;
-  FG_TRY(fg_to_dev(c, d_images, (size_t)B * c->C * 1024, c->io_dev, &dd));
-  FG_TRY(k_nchw_to_nhwc(c, dd, c->io_dev2, B, c->C, 1024));
-  float* dn = nullptr;
-  if (d_noise) dn = fg_is_dev(d_noise) ? d_noise : c->in_noiseD;
-  FG_TRY(gen_backward(c->env, c->G, c->net, c->io_dev2, dn));
-  if (d_noise && dn != d_noise) FG_TRY(fg_to_user(c, d_noise, dn, (size_t)B * kNoiseDim));
-  return FG_OK;
-}
-int fg_D_forward(fg_ctx* c, const float* images, int B, int training, const float* masks, uint64_t seed, float* out) {
-  ENTER(c);
-  FG_REQUIRE(images && B >= 1 && B <= c->maxB, "fg_D_forward: bad arguments (B=%d, max %d)", B, c->maxB);
-  c->net.D_packed = false;
-  fg_hyper h;
-  fg_hyper_default(&h);
-  const float* xd;
-  FG_TRY(fg_to_dev(c, images, (size_t)B * c->C * 1024, c->io_dev, &xd));
-  FG_TRY(k_nchw_to_nhwc(c, xd, c->D_x, B, c->C, 1024));
-  if (training) {
-    if (masks) {
-      FG_CUDA(cudaMemcpyAsync(c->D_masks, masks, sizeof(float) * (size_t)B * kMaskPerSample, cudaMemcpyDefault, c->stream));
-    } else {
-      FG_TRY(k_masks_generate(c, c->D_masks, B, seed, h.p_spatial, h.p_drop));
-    }
-  }
-  FG_TRY(net_D_forward(c, c->D_x, B, training != 0, &h));
-  FG_TRY(k_sigmoid_fwd(c, c->D_logit, c->D_out, B));
-  if (out) FG_TRY(fg_to_user(c, out, c->D_out, B));
-  return FG_OK;
-}
-int fg_D_backward(fg_ctx* c, const float* d_out, int want_wgrad, float* d_images) {
-  ENTER(c);
-  FG_REQUIRE(d_out, "fg_D_backward: d_out is null");
-  const int B = c->D_B;
-  const float* dd;
-  FG_TRY(fg_to_dev(c, d_out, B, c->D_targets, &dd));
-  FG_TRY(k_sigmoid_grad_mul(c, dd, c->D_out, c->D_dlogit, B));
-  FG_TRY(net_D_backward(c, c->D_dlogit, want_wgrad != 0, d_images != nullptr));
-  if (d_images) {
-    FG_TRY(k_nhwc_to_nchw(c, c->D_dx, c->io_dev, B, c->C, 1024));
-    FG_TRY(fg_to_user(c, d_images, c->io_dev, (size_t)B * c->C * 1024));
-  }
-  return FG_OK;
-}
-int fg_bce_forward(fg_ctx* c, const float* x, const float* t, int n, float* loss_out) {
-  ENTER(c);
-  FG_REQUIRE(x && t && loss_out && n > 0 && n <= c->maxB, "fg_bce_forward: bad arguments");
-  const float *xd, *td;
-  FG_TRY(fg_to_dev(c, x, n, c->io_dev, &xd));
-  FG_TRY(fg_to_dev(c, t, n, c->io_dev2, &td));
-  FG_TRY(k_bce_fwd(c, xd, td, n, c->D_targets));
-  return fg_to_user(c, loss_out, c->D_targets, 1);
-}
-int fg_bce_backward(fg_ctx* c, const float* x, const float* t, int n, float* dx) {
-  ENTER(c);
-  FG_REQUIRE(x && t && dx && n > 0 && n <= c->maxB, "fg_bce_backward: bad arguments");
-  const float *xd, *td;
-  FG_TRY(fg_to_dev(c, x, n, c->io_dev, &xd));
-  FG_TRY(fg_to_dev(c, t, n, c->io_dev2, &td));
-  FG_TRY(k_bce_bwd(c, xd, td, n, c->D_targets));
-  return fg_to_user(c, dx, c->D_targets, n);
-}
-int fg_optim_step(fg_ctx* c, int net, const fg_hyper* h, float grad_scale) {
-  ENTER(c);
-  FG_REQUIRE(h && (net == FG_NET_G || net == FG_NET_D), "fg_optim_step: bad arguments");
-  // no accuracy information at this level: no gate, and the fused steps' accuracy history is not touched
-  FG_TRY(k_optim_prep(c, c->net.dstats, net, h));
-  return pair_optim(c, c->net, net, h, grad_scale);
-}
 int fg_adam_step(fg_ctx* c, float* p, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2,
                  float eps, int t, float l1_grad, float l2, float clampv, float grad_scale) {
   ENTER(c);
@@ -440,44 +299,6 @@ int fg_adam_step(fg_ctx* c, float* p, const float* g, float* m, float* v, int64_
   const double step = (double)lr * sqrt(1.0 - pow((double)beta2, t)) / (1.0 - pow((double)beta1, t));
   return k_adam(c, p, g, m, v, n, beta1, beta2, eps, l1_grad, l2, clampv, grad_scale, nullptr, nullptr, (float)step,
                 nullptr);
-}
-
-// ---- L-step -----------------------------------------------------------------------------------------
-int fg_train_step(fg_ctx* c, const fg_hyper* h, int B, const float* real, const float* noise_D, const float* noise_G,
-                  const float* masks_D, const float* masks_G, uint64_t seed, fg_step_stats* stats) {
-  return train_step_iters(c, "fg_train_step", h, B, 1, 1, real, noise_D, noise_G, masks_D, masks_G, seed, stats);
-}
-int fg_train_step_iters(fg_ctx* c, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,
-                        const float* noise_D, const float* noise_G, const float* masks_D, const float* masks_G, uint64_t seed,
-                        fg_step_stats* stats) {
-  return train_step_iters(c, "fg_train_step_iters", h, B, d_iters, g_iters, real, noise_D, noise_G, masks_D, masks_G, seed,
-                          stats);
-}
-
-int fg_sample(fg_ctx* c, const float* noise, int N, int chunk, float* images_out) {
-  ENTER(c);
-  FG_REQUIRE(noise && images_out && N >= 1 && chunk >= 1 && chunk <= c->maxB, "fg_sample: bad arguments (chunk %d, max %d)",
-             chunk, c->maxB);
-  const bool out_dev = fg_is_dev(images_out);
-  const size_t img = (size_t)c->C * 1024;
-  c->net.G_packed = false;
-  for (int s = 0; s < N; s += chunk) {
-    const int b = std::min(chunk, N - s);
-    const float* nd;
-    FG_TRY(fg_to_dev(c, noise + (size_t)s * kNoiseDim, (size_t)b * kNoiseDim, c->in_noiseG, &nd));
-    // sample.lua never calls :evaluate() => BatchNorm uses the statistics of each chunk (SURVEY 3.4)
-    FG_TRY(gen_forward(c->env, c->G, c->net, nd, b, true));
-    float* dst = images_out + (size_t)s * img;
-    if (out_dev) {
-      FG_TRY(k_nhwc_to_nchw(c, c->G.y, dst, b, c->C, 1024));
-    } else {
-      FG_TRY(k_nhwc_to_nchw(c, c->G.y, c->io_dev, b, c->C, 1024));
-      FG_CUDA(cudaMemcpyAsync(dst, c->io_dev, b * img * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-      if (s + chunk < N) FG_CUDA(cudaStreamSynchronize(c->stream));  // io_dev is reused by the next chunk
-    }
-  }
-  if (!out_dev) FG_CUDA(cudaStreamSynchronize(c->stream));
-  return FG_OK;
 }
 
 // ---- helpers ----------------------------------------------------------------------------------------
@@ -513,20 +334,6 @@ int fg_memcpy(fg_ctx* c, void* dst, const void* src, size_t bytes) {
 }
 
 int64_t fg_kernel_launches(fg_ctx* c) { return c ? c->launches : -1; }
-
-int64_t fg_debug_tensor(fg_ctx* c, const char* name, float* dst, int64_t max_elems) {
-  if (!c || !name) return -1;
-  cudaSetDevice(c->device);
-  const int db = c->D_B;
-  std::vector<DebugTensor> ents = {
-      {"D.z1", c->D_z[0], 65536, db}, {"D.z2", c->D_z[1], 32768, db}, {"D.z3", c->D_z[2], 16384, db},
-      {"D.z4", c->D_z[3], 8192, db}, {"D.p4", c->D_p[3], 2048, db}, {"D.logit", c->D_logit, 1, db},
-      {"D.out", c->D_out, 1, db}, {"D.dx", c->D_dx, 1024 * c->C, db}, {"D.masks", c->D_masks, kMaskPerSample, db},
-      {"D.zl1", c->D_zl1, 512, db}, {"D.zl2", c->D_zl2, 512, db}};
-  pair_keep_rows(c->net, ents);
-  gen_debug_rows(c->G, ents);
-  return debug_tensor_copy(c, "fg_debug_tensor", ents.data(), ents.size(), name, dst, max_elems);
-}
 
 int fg_bench_tf32_peak(fg_ctx* c, int iters, double* tflops) {
   ENTER(c);

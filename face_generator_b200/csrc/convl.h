@@ -56,9 +56,9 @@ int upsl_fwd(ConvLEnv& e, UpsL& U, const float* h, const float* P, float* z, int
 // the upsample backward); otherwise dh is the full-resolution gradient the consumer still sums 2x2.
 int upsl_bwd(ConvLEnv& e, UpsL& U, TcOp& dy, const float* h, const float* dz, float* G, float* dh, int B, bool* pooled);
 
-// ---- gen.cu: UpsGen on the owner's layer scratch (ConvLEnv) and parameters (NetPair: PG, gG, bnG, G_packed) ----
+// ---- gen.cu: UpsGen on the owner's layer scratch (ConvLEnv) and parameters (NetPair: PG, gG, bnG, G_pack) ----
 int gen_alloc(ConvLEnv& e, UpsGen& G, const GenDesc& d);
-int gen_pack(fg_ctx* c, UpsGen& G, NetPair& p);  // unless p.G_packed under the current pack_key()
+int gen_pack(fg_ctx* c, UpsGen& G, NetPair& p);  // unless p.G_pack is the current pack_key()
 // noise: device [B][100] -> G.y (NHWC [B][S][S][C]).  training: batch statistics + running statistics update
 int gen_forward(ConvLEnv& e, UpsGen& G, NetPair& p, const float* noise, int B, bool training);
 // dy: NHWC [B][S][S][C] of the last (training-mode) forward; accumulates into p.gG; dnoise (device [B][100]) may be null

@@ -291,36 +291,6 @@ int nearest_run(fg_ctx* c, const float* cands, const fg_dataset* d, int64_t N, i
     FG_CUDA(cudaSetDevice((d)->c->device));              \
   } while (0)
 
-namespace {
-// d_iters D iterations + g_iters G iterations of the loop body fed on the device, for the entry `what`: the inputs of D
-// iteration j are gather(draw(4*r_j)) and uniform(4*r_j+1), those of G iteration j uniform(4*r_j+2), r_j the stream root
-// of iteration j (fg_b200.h; r_0 = seed).  The draws run inside the step (one graph launch per call once captured), each
-// reading its root from c->seed_dev.
-int train_step_dataset_iters(fg_ctx* c, fg_dataset* d, const char* what, const fg_hyper* h, int B, int d_iters, int g_iters,
-                             uint64_t seed, fg_step_stats* stats) {
-  ENTER(d);
-  FG_TRY(step_check(c, what, B, d_iters, g_iters, h, d, true));
-  const int Bh = B / 2;
-  const size_t M = c->maxB, img = (size_t)c->C * 1024;
-  IterStage& s = c->iter_stage;
-  FG_TRY(s.reserve(c, c->allocs, 0, d_iters * M / 2 * img));
-  FG_TRY(s.reserve(c, c->allocs, 1, d_iters * M / 2 * kNoiseDim));
-  FG_TRY(s.reserve(c, c->allocs, 2, g_iters * M * kNoiseDim));
-  float *real = s.p[0], *zd = s.p[1], *zg = s.p[2];
-  const std::function<int()> feed = [&]() -> int {
-    for (int j = 0; j < d_iters; ++j) {
-      FG_TRY(dataset_draw_gather(d, 0, Bh, 32, real + (size_t)j * Bh * img, c->seed_dev + j, 4));
-      FG_TRY(noise_uniform_dev(c, 1, (int64_t)Bh * kNoiseDim, zd + (size_t)j * Bh * kNoiseDim, c->seed_dev + j, 4));
-    }
-    for (int j = 0; j < g_iters; ++j)
-      FG_TRY(noise_uniform_dev(c, 2, (int64_t)B * kNoiseDim, zg + (size_t)j * B * kNoiseDim, c->seed_dev + j, 4));
-    return FG_OK;
-  };
-  NetStep st(c, h, B, real, zd, zg);
-  return pair_train_step(st, d_iters, g_iters, nullptr, nullptr, seed, {real, zd, zg, nullptr, nullptr, d}, &feed, stats);
-}
-}  // namespace
-
 extern "C" {
 
 int fg_dataset_create(fg_ctx* ctx, int64_t N, int Cs, int Hs, int Ws, fg_dataset** out) {
@@ -540,16 +510,6 @@ int fg_nearest(fg_ctx* c, const float* queries, int Q, const float* cands, int64
 int fg_dataset_nearest(fg_dataset* d, const float* queries, int Q, int32_t* idx_out, float* dist_out) {
   ENTER(d);
   return nearest_run(d->c, nullptr, d, d->N, d->c->C * 1024, queries, Q, idx_out, dist_out);
-}
-
-// One adversarial.lua loop body fed entirely on the device: real half-batch = gather(draw(4*seed)), noise for the
-// D step = uniform(4*seed+1), for the G step = uniform(4*seed+2), dropout masks from `seed` as in fg_train_step.
-int fg_train_step_dataset(fg_ctx* c, fg_dataset* d, const fg_hyper* h, int B, uint64_t seed, fg_step_stats* stats) {
-  return train_step_dataset_iters(c, d, "fg_train_step_dataset", h, B, 1, 1, seed, stats);
-}
-int fg_train_step_dataset_iters(fg_ctx* c, fg_dataset* d, const fg_hyper* h, int B, int d_iters, int g_iters, uint64_t seed,
-                                fg_step_stats* stats) {
-  return train_step_dataset_iters(c, d, "fg_train_step_dataset_iters", h, B, d_iters, g_iters, seed, stats);
 }
 
 }  // extern "C"

@@ -97,7 +97,7 @@ int fg_dp_init(fg_ctx* c, const void* id128, int nranks, int rank) {
     return FG_ERR_INVALID;
   }
   FG_CUDA(cudaSetDevice(c->device));
-  pair_clear_graphs(c->net);  // captured steps reference the old communicator
+  pair_clear_graphs(net32_pair(c));  // captured steps reference the old communicator
   c->graph_epoch++;
   if (c->nccl_comm) {
     g_nccl.CommDestroy((ncclComm_t)c->nccl_comm);
@@ -120,7 +120,7 @@ int fg_dp_broadcast_params(fg_ctx* c) {
   if (!c) return FG_ERR_INVALID;
   if (c->world <= 1) return FG_OK;
   FG_CUDA(cudaSetDevice(c->device));
-  return pair_broadcast(c, c->net);
+  return pair_broadcast(c, net32_pair(c));
 }
 int fg_dp_world(fg_ctx* c) { return c ? c->world : 0; }
 }

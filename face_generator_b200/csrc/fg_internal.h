@@ -54,8 +54,8 @@ inline int grid_for(int64_t n, int block, int cap = 132 * 16) {
 constexpr int kMaskPerSample = 1984;  // 64+128+256+512 SpatialDropout + 512+512 Dropout keep flags
 constexpr int kNoiseDim = 100;
 constexpr int kSmallMaxParts = 2048;  // partial rows of the small-channel wgrad workspace
-constexpr int kGradTail = 8;
-constexpr int kOptRedRows = 132 * 2;  // blocks of the penalty-loss reduction          // extra floats behind each flat gradient (DP-reduced scalars)
+constexpr int kGradTail = 8;           // extra floats behind each flat gradient (DP-reduced scalars)
+constexpr int kOptRedRows = 132 * 2;  // blocks of the penalty-loss reduction
 
 // Geometry of one stride-1 "same" convolution seen as a sum over taps of shifted GEMMs.
 // Output pixels p = (b,y,x) in [0,B)x[0,H)x[0,W); the stored input is [B][H/ups][W/ups][Cin]
@@ -68,11 +68,7 @@ struct ConvGeom {
 struct GLayout {
   int64_t L1W, L1b, a1, C1W, C1b, g1, be1, a2, C2W, C2b, g2, be2, a3, C3W, C3b, total;
 };
-struct DLayout {
-  int64_t cW[4], cb[4], ca[4], L1W, L1b, a5, L2W, L2b, a6, L3W, L3b, total;
-};
 GLayout make_g_layout(int C, int side);  // the generator of models.lua at side 32 (upsampling32) or 16 (upsampling16)
-DLayout make_d_layout(int C);
 
 struct DeviceStats {  // lives in device memory; mirrored to fg_step_stats
   float loss_D, loss_G;
@@ -99,7 +95,7 @@ struct StepGraph {
   bool failed = false;
 };
 
-// The trainable state of one G/D pair (the 32x32 nets of fg_ctx, the coarse-to-fine nets, the --scale 16 nets)
+// The trainable state of one G/D pair (the 32x32 nets, the coarse-to-fine nets, the --scale 16 nets)
 struct NetPair {
   int64_t nG = 0, nD = 0;
   float *PG = nullptr, *PD = nullptr, *gG = nullptr, *gD = nullptr;  // flat parameters and gradients
@@ -109,7 +105,8 @@ struct NetPair {
   DeviceStats* dstats = nullptr;
   DeviceStats* hstats = nullptr;  // pinned mirror
   float* acc_hist = nullptr;      // [kAccHistMax]
-  bool G_packed = false, D_packed = false;  // the weight packs match the parameters
+  // the pack_key() (convl.h) each half's weight packs were made under; -1: stale, the parameters changed since
+  int G_pack = -1, D_pack = -1;
   std::vector<StepGraph> graphs;
   const char* optim_timer[2] = {nullptr, nullptr};  // ScopedTimer names of the G / D optimizer update (none: untimed)
   // option "debug_keep" (tests): the D iteration's tensors that the G iteration's D forward overwrites, copied by the
@@ -223,7 +220,6 @@ struct UpsGen {
   float *bn_mean[2] = {nullptr, nullptr}, *bn_istd[2] = {nullptr, nullptr}, *bn_mg = nullptr;
   int B = 0;
   bool train = true, valid = false;
-  int pack_key = -1;  // pack_key() of the weight packs
   std::deque<std::string> names;  // prefixed timer names (stable storage: the layers point into it)
   const char *t_bn2_finalize = nullptr, *t_bn2_stats = nullptr, *t_bn2_apply = nullptr, *t_bn2_bwd_reduce = nullptr,
              *t_bn2_bwd_apply = nullptr;
@@ -246,6 +242,10 @@ struct IterStage {
   int in(fg_ctx* c, std::vector<void*>& allocs, int k, const float* p, size_t n, size_t cap_n, const float** out);
 };
 
+struct Net32;  // the 32x32 nets (nets.cu)
+
+// What every net on one device stream shares: the stream, the options, the data-parallel state and the workspaces of
+// the kernels.  Each net owns its own parameters, activations and layer scratch.
 struct fg_ctx {
   int device = 0, maxB = 0, C = 3;
   cudaStream_t stream = nullptr;
@@ -256,17 +256,9 @@ struct fg_ctx {
   // OPT.D_optmethod / OPT.G_optmethod (train.lua:38-39): FG_OPT_ADAM | FG_OPT_ADAGRAD | FG_OPT_SGD, and SGD momentum
   int opt_D = 0, opt_G = 0;
   float sgd_mom_D = 0.f, sgd_mom_G = 0.f;
-  DLayout dl;
-  std::vector<void*> allocs;  // every cudaMalloc of net_alloc(), released by net_free()
-  NetPair net;
-  // the library's own allocations (net.PG.. point here unless fg_bind_params borrowed caller-owned buffers) and the 8
-  // DP-reduced scalars behind a bound gradient (behind the own gradient buffer they are contiguous with it)
-  float *ownPG = nullptr, *ownPD = nullptr, *ownGG = nullptr, *ownGD = nullptr;
-  float* tail_sep = nullptr;
-  // packed weights (forward packs [tap][n][c], dgrad packs [tap'][c][n])
+  std::vector<void*> allocs;  // the workspaces below, allocated by fg_create
+  Net32* n32 = nullptr;       // allocated by fg_create too, freed by fg_destroy before the workspaces
   float* small_ws = nullptr;  // per-block partials of the small-channel wgrad (k_conv_small.cu)
-  float* wgrad_ws = nullptr;  // packed weight-gradient workspace (largest layer)
-  size_t wgrad_ws_elems = 0;
   // Cross-block sums are never accumulated with float / double atomics, whose order varies from run to run: split-K
   // weight gradients write one partial per split into splitk_ws and k_splitk_reduce adds them in split order; the
   // reduction kernels write one row of partials per block into red_ws and the last block to finish (red_ticket)
@@ -288,23 +280,8 @@ struct fg_ctx {
   unsigned* amax_out = nullptr;  // when set (AmaxInto, convl.h), the next elementwise producer also reduces max|output| there ...
   bool* amax_done = nullptr;     // ... and sets *amax_done (a TcOp's amax_ready): its consumer skips its own reduction
   double* bn_acc = nullptr;  // [4][256] double accumulators (sum, sumsq / sum g, sum g xhat)
-  // D activations (NHWC)
-  int D_B = 0;
-  bool D_train = true, D_fwd_valid = false;
-  float *D_x = nullptr, *D_z[4] = {nullptr, nullptr, nullptr, nullptr}, *D_p[4] = {nullptr, nullptr, nullptr, nullptr};
-  float *D_zl1 = nullptr, *D_hl1 = nullptr, *D_zl2 = nullptr, *D_hl2 = nullptr, *D_logit = nullptr, *D_out = nullptr;
-  float* D_masks = nullptr;
-  float D_drop_scale = 2.0f, D_spatial_eval = 0.8f;  // 1/(1-p_drop), 1-p_spatial of the last forward
-  float *D_dlogit = nullptr, *D_dh = nullptr, *D_dzl = nullptr, *D_dz = nullptr, *D_dp = nullptr, *D_dx = nullptr;
-  float* D_targets = nullptr;
-  // staging
-  float* stage_pinned = nullptr;
-  size_t stage_pinned_bytes = 0;
   float* io_dev = nullptr;  // device staging for NCHW images / misc
   size_t io_dev_elems = 0;
-  float* io_dev2 = nullptr;
-  float *in_noiseD = nullptr, *in_noiseG = nullptr;
-  IterStage iter_stage;  // the inputs of the host-fed and device-fed train steps, stacked per iteration
   float* scratch[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   size_t scratch_elems[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   // data parallel
@@ -337,12 +314,6 @@ struct fg_ctx {
   cudaEvent_t events[16] = {};
   bool timing = false;
   std::map<std::string, TimerRec> timers;
-  // G, the layers of D (D.L3 runs on the GEMV kernels) and the scratch they share: env.dy is the split of the current
-  // dY, env.ws = wgrad_ws.  D's FP16 scale pairs, env.dy's included, live in D_pairs.
-  ConvLEnv env;
-  UpsGen G;
-  ConvL Dc[4], DL1, DL2;
-  ScalePairs D_pairs;
 };
 
 // record the convolution kernel a launcher is about to run (fg_ctx::last_conv_*)
@@ -485,14 +456,14 @@ int k_splitk_reduce(fg_ctx* c, const float* parts, int splits, int64_t n, float*
 int tc_init(fg_ctx* c);
 void tc_destroy(fg_ctx* c);
 
-// ---- nets.cu ---------------------------------------------------------------------------------------
-int net_alloc(fg_ctx* c);
-void net_free(fg_ctx* c);
-int net_pack_D(fg_ctx* c);
-int net_D_forward(fg_ctx* c, const float* x_nhwc, int B, bool training, const fg_hyper* h);  // masks in c->D_masks
-int net_D_backward(fg_ctx* c, const float* dlogit_dev, bool want_wgrad, bool want_dx);       // -> c->D_dx (NHWC)
+// ---- nets.cu: the 32x32 nets of fg_ctx::n32 ---------------------------------------------------------
+int net32_alloc(fg_ctx* c);
+void net32_free(fg_ctx* c);
+NetPair& net32_pair(fg_ctx* c);  // their trainable state
+
+// ---- dp.cu ------------------------------------------------------------------------------------------
 int net_allreduce(fg_ctx* c, float* buf, int64_t n);
-int net_broadcast(fg_ctx* c, void* buf, size_t bytes);  // rank 0 -> all (dp.cu)
+int net_broadcast(fg_ctx* c, void* buf, size_t bytes);  // rank 0 -> all
 int net_group(bool start);                                // ncclGroupStart / ncclGroupEnd
 
 // ---- netpair.cu: the lifecycle of a NetPair, on the ctx stream.  `net` is FG_NET_G or FG_NET_D (anything else: G) ----
@@ -564,19 +535,6 @@ int pair_train_step(StepNets& s, int nd, int ng, const float* masksD, const floa
 // the "Dstep.*" rows of a debug-tensor table
 struct DebugTensor;
 void pair_keep_rows(const NetPair& p, std::vector<DebugTensor>& ents);
-
-// the 32x32 nets' part of the loop body (nets.cu): real [B/2][C][32][32], noiseD [B/2][100], noiseG [B][100] per
-// iteration
-struct NetStep final : StepNets {
-  const float *real, *noiseD, *noiseG;
-  NetStep(fg_ctx* c, const fg_hyper* h, int B, const float* real, const float* noiseD, const float* noiseG);
-  int g_forward(int j, bool d_iter) override;
-  int d_input(int j) override;
-  int draw_masks(int kind, const uint64_t* root) override;
-  int d_forward(bool on_g) override;
-  int d_backward(bool want_wgrad, bool want_dx) override;
-  int g_backward() override;
-};
 
 // ---- nets_ae.cu: the elementwise layers of the autoencoder (nn.ReLU, nn.Tanh + nn.Dropout, nn.AbsCriterion).  Each is
 // a producer in AmaxInto's sense (convl.h). ----

@@ -89,12 +89,11 @@ int gen_alloc(ConvLEnv& e, UpsGen& G, const GenDesc& d) {
 }
 
 int gen_pack(fg_ctx* c, UpsGen& G, NetPair& p) {
-  if (p.G_packed && G.pack_key == pack_key(c)) return FG_OK;
+  if (p.G_pack == pack_key(c)) return FG_OK;
   FG_TRY(convl_pack(c, G.GL1, p.PG));
   for (int i = 0; i < 2; ++i) FG_TRY(upsl_pack(c, G.GU[i], p.PG));
   FG_TRY(convl_pack(c, G.GC3, p.PG));
-  p.G_packed = true;
-  G.pack_key = pack_key(c);
+  p.G_pack = pack_key(c);
   return FG_OK;
 }
 

@@ -157,7 +157,7 @@ int pair_optim(fg_ctx* c, NetPair& p, int net, const fg_hyper* h, float grad_sca
   FG_TRY(k_optim_update(c, isD ? c->opt_D : c->opt_G, x.P, x.g, x.m, x.v, x.n, h->beta1, h->beta2, h->eps,
                         isD ? c->sgd_mom_D : c->sgd_mom_G, l1_grad, pen ? l2 : 0.f, isD ? h->D_clamp : h->G_clamp, grad_scale,
                         isD ? &s->step_D : &s->step_G, isD ? &s->do_train_D : &s->do_train_G, step_count(s, net)));
-  (isD ? p.D_packed : p.G_packed) = false;
+  (isD ? p.D_pack : p.G_pack) = -1;
   return FG_OK;
 }
 
@@ -179,7 +179,7 @@ int pair_broadcast(fg_ctx* c, NetPair& p) {
   FG_TRY(net_broadcast(c, p.acc_hist, kAccHistMax * sizeof(float)));
   FG_TRY(net_group(false));
   FG_CUDA(cudaStreamSynchronize(c->stream));
-  p.G_packed = p.D_packed = false;
+  p.G_pack = p.D_pack = -1;
   return FG_OK;
 }
 
@@ -202,7 +202,7 @@ int pair_set_params(fg_ctx* c, NetPair& p, int net, const float* src) {
   const Half h = half(p, net);
   FG_CUDA(cudaMemcpyAsync(h.P, src, h.n * sizeof(float), cudaMemcpyDefault, c->stream));
   FG_CUDA(cudaStreamSynchronize(c->stream));
-  (net == FG_NET_D ? p.D_packed : p.G_packed) = false;
+  (net == FG_NET_D ? p.D_pack : p.G_pack) = -1;
   return FG_OK;
 }
 int pair_get_params(fg_ctx* c, const NetPair& p, int net, float* dst) {
@@ -286,7 +286,7 @@ int net_graph_run(fg_ctx* c, NetPair& p, int B, const void* hyper, size_t hyper_
   }
   if (e->failed) return body();
   if (!e->exec) {
-    p.G_packed = p.D_packed = false;
+    p.G_pack = p.D_pack = -1;
     const int64_t l0 = c->launches;
     FG_CUDA(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeRelaxed));
     const int r = body();
@@ -310,7 +310,7 @@ int net_graph_run(fg_ctx* c, NetPair& p, int B, const void* hyper, size_t hyper_
   }
   FG_CUDA(cudaGraphLaunch(e->exec, c->stream));
   c->launches += e->launches;
-  p.G_packed = p.D_packed = false;
+  p.G_pack = p.D_pack = -1;
   return FG_OK;
 }
 

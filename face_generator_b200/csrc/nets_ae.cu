@@ -165,7 +165,7 @@ struct fg_ae {
         *h3 = nullptr, *z4 = nullptr, *y = nullptr, *masks = nullptr;
   float *dz4 = nullptr, *dz3 = nullptr, *dz2 = nullptr, *dz1 = nullptr, *dh = nullptr;
   float *in_img = nullptr, *in_masks = nullptr;  // staging of host inputs
-  int B = 0, grad_B = 0, pack_key = -1;
+  int B = 0, grad_B = 0;
   bool train = true, valid = false;
   float p_drop = 0.5f;  // Dropout probability of the last training forward
   std::vector<void*> allocs;
@@ -237,10 +237,9 @@ int ae_alloc(fg_ae* n) {
 }
 
 int ae_pack(fg_ae* n) {
-  if (n->net.G_packed && n->pack_key == pack_key(n->c)) return FG_OK;
+  if (n->net.G_pack == pack_key(n->c)) return FG_OK;
   for (ConvL& L : n->L) FG_TRY(convl_pack(n->c, L, n->net.PG));
-  n->net.G_packed = true;
-  n->pack_key = pack_key(n->c);
+  n->net.G_pack = pack_key(n->c);
   return FG_OK;
 }
 
@@ -316,7 +315,7 @@ int train_step(fg_ae* n, const fg_ae_hyper* h, int B, const float* img, const fl
   FG_TRY(k_adam_prep(c, &n->dstats->t, &n->dstats->step, h->lr, h->beta1, h->beta2));
   FG_TRY(k_optim_update(c, FG_OPT_ADAM, p.PG, p.gG, p.mG, p.vG, p.nG, h->beta1, h->beta2, h->eps, 0.f, h->L1, h->L2, 0.f, 1.0f,
                         &n->dstats->step, nullptr, &n->dstats->t));
-  p.G_packed = false;
+  p.G_pack = -1;
   FG_CUDA(cudaMemcpyAsync(n->hstats, n->dstats, sizeof(AeStats), cudaMemcpyDeviceToHost, c->stream));
   return FG_OK;
 }

@@ -43,7 +43,6 @@ struct fg_c2f {
   ConvL Gc[5], Dc[4], DL1;
   const char* D_L2_timer = "";
   const char *t_refine_prep = "", *t_refine_pick = "";  // fg_c2f_refine's own kernels
-  int G_pack_impl = -1, D_pack_impl = -1;
   float *G_x = nullptr, *G_z[5] = {}, *G_h[4] = {};
   float *D_x = nullptr, *D_cond = nullptr, *D_z[4] = {}, *D_h[4] = {}, *D_p2 = nullptr, *D_p4 = nullptr, *D_d4 = nullptr;
   float *D_zl1 = nullptr, *D_al1 = nullptr, *D_hl1 = nullptr, *D_logit = nullptr, *D_out = nullptr, *D_masks = nullptr,
@@ -185,18 +184,16 @@ int c2f_alloc(fg_c2f* n) {
 // packs are rebuilt after every optimizer step / set_params, and when the ctx's "conv_impl" changed since the last
 // pack (the TF32 splits are only produced for the tensor-core implementations)
 int pack_G(fg_c2f* n) {
-  if (n->net.G_packed && n->G_pack_impl == pack_key(n->c)) return FG_OK;
+  if (n->net.G_pack == pack_key(n->c)) return FG_OK;
   for (int i = 0; i < 5; ++i) FG_TRY(convl_pack(n->c, n->Gc[i], n->net.PG));
-  n->net.G_packed = true;
-  n->G_pack_impl = pack_key(n->c);
+  n->net.G_pack = pack_key(n->c);
   return FG_OK;
 }
 int pack_D(fg_c2f* n) {
-  if (n->net.D_packed && n->D_pack_impl == pack_key(n->c)) return FG_OK;
+  if (n->net.D_pack == pack_key(n->c)) return FG_OK;
   for (int i = 0; i < 4; ++i) FG_TRY(convl_pack(n->c, n->Dc[i], n->net.PD));
   FG_TRY(convl_pack(n->c, n->DL1, n->net.PD));
-  n->net.D_packed = true;
-  n->D_pack_impl = pack_key(n->c);
+  n->net.D_pack = pack_key(n->c);
   return FG_OK;
 }
 

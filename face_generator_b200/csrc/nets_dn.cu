@@ -339,7 +339,7 @@ struct DnDec {
   float *mean[3] = {}, *istd[3] = {};
   float* bn = nullptr;  // [kBnDn] running statistics
   const float* masks = nullptr;  // keep flags of the last training forward ([B][mps]); null: evaluation
-  int B = 0, pack_key = -1;
+  int B = 0;
   bool train = true, valid = false;
 };
 
@@ -465,17 +465,16 @@ int dn_alloc(fg_dn* n) {
   return FG_OK;
 }
 
-bool& packed_flag(fg_dn* n, int net) { return net ? n->net.D_packed : n->net.G_packed; }
+int& pack_state(fg_dn* n, int net) { return net ? n->net.D_pack : n->net.G_pack; }
 const float* params(fg_dn* n, int net) { return net ? n->net.PD : n->net.PG; }
 float* grads(fg_dn* n, int net) { return net ? n->net.gD : n->net.gG; }
 
 int pack(fg_dn* n, int net) {
   DnDec& d = n->dec[net];
-  if (packed_flag(n, net) && d.pack_key == pack_key(n->c)) return FG_OK;
+  if (pack_state(n, net) == pack_key(n->c)) return FG_OK;
   FG_TRY(convl_pack(n->c, d.L1, params(n, net)));
   FG_TRY(convl_pack(n->c, d.L2, params(n, net)));
-  packed_flag(n, net) = true;
-  d.pack_key = pack_key(n->c);
+  pack_state(n, net) = pack_key(n->c);
   return FG_OK;
 }
 
@@ -634,7 +633,7 @@ int dn_optim(fg_dn* n, int net, const fg_dn_hyper* h) {
   NetPair& p = n->net;
   FG_TRY(k_optim_update(c, FG_OPT_ADAM, net ? p.PD : p.PG, grads(n, net), p.mG, p.vG, p.nG, h->beta1, h->beta2, h->eps, 0.f,
                         h->L1, h->L2, h->clamp, 1.0f, &n->dstats->step, nullptr, &n->dstats->t));
-  packed_flag(n, net) = false;
+  pack_state(n, net) = -1;
   return FG_OK;
 }
 

@@ -120,7 +120,6 @@ struct fg_s16 {
   float *ga = nullptr, *gb = nullptr, *ws = nullptr;
   float *in_a = nullptr, *in_b = nullptr, *in_c = nullptr, *io = nullptr;
   IterStage iter_stage;  // the inputs of the host-fed and device-fed train steps, stacked per iteration
-  int D_pack_impl = -1;
   int D_B = 0;
   bool D_valid = false, D_train = true;
   std::vector<void*> allocs;
@@ -234,13 +233,12 @@ int s16_alloc(fg_s16* n) {
 
 int pack_D(fg_s16* n) {
   fg_ctx* c = n->c;
-  if (n->net.D_packed && n->D_pack_impl == pack_key(c)) return FG_OK;
+  if (n->net.D_pack == pack_key(c)) return FG_OK;
   for (int i = 0; i < 4; ++i) FG_TRY(convl_pack(c, n->Dc[i], n->net.PD));
   FG_TRY(convl_pack(c, n->DF1, n->net.PD));
   FG_TRY(convl_pack(c, n->DE1, n->net.PD));
   FG_TRY(convl_pack(c, n->DE2, n->net.PD));
-  n->net.D_packed = true;
-  n->D_pack_impl = pack_key(c);
+  n->net.D_pack = pack_key(c);
   return FG_OK;
 }
 

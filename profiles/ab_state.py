@@ -7,12 +7,14 @@ entries with option debug_keep, saving every Dstep.* tensor after each step ("de
 also run at fine sizes 16 and 64.  It writes every piece of state as .npy under
 --out/<case>/: parameters, gradients, optimizer m / v / t, BatchNorm running state, the step statistics, the outputs
 of those calls and the generator's debug tensors, plus the kernel launches of each step (launches.json).  The L-op
-convolutions (fg_conv2d_*) with the 3xFP16 split are one more case.  `compare A B` reports, per case, the first array
+convolutions (fg_conv2d_*) with the 3xFP16 split are one more case.  The denoiser and the autoencoder run 6 seeded train
+steps with option mma_f16 switched off for the middle two, then save parameters, gradients, Adam and BatchNorm state and
+forward outputs.  Each run also records the free device memory after fg_create at batch 256 (free_after_create.json).  `compare A B` reports, per case, the first array
 that differs and the launches per step of both builds; a case differs when either does.
 
 One build per process: both libraries export the same symbols.
 
-usage:  python profiles/ab_state.py run --lib face_generator_b200/libfg_b200.so --out /tmp/ab/new [--only 32,s16,c2f,lop]
+usage:  python profiles/ab_state.py run --lib face_generator_b200/libfg_b200.so --out /tmp/ab/new [--only 32,s16,c2f,lop,dn,ae]
         python profiles/ab_state.py compare /tmp/ab/old /tmp/ab/new
 """
 import argparse
@@ -240,6 +242,75 @@ def case_lop(N=16, Cin=128, H=16, Cout=128, k=3):
     return {"y": y, "dx": dx, "dw": dw, "db": db}, launches
 
 
+def toggled_steps(ctx, step):
+    """6 seeded steps, the middle two with mma_f16 0: the weight packs are remade under each key"""
+    launches, stats = [], []
+    for i in range(6):
+        if i in (2, 4):
+            ctx.set_option("mma_f16", 0 if i == 2 else 1)
+        l0 = ctx.launches()
+        st = step(20 + i)
+        ctx.sync()
+        launches.append(ctx.launches() - l0)
+        stats.append(np.array([st[k] for k in sorted(st)], np.float64))
+    return launches, np.stack(stats)
+
+
+def case_dn(B=128, S=16):
+    import face_generator_b200 as fg
+    from face_generator_b200 import denoiser as DN
+    rng = np.random.default_rng(61)
+    ctx = fg.Context(0, max_batch=B, channels=C)
+    dn = DN.Denoiser(ctx, S)
+    for net in (0, 1):
+        dn.set_params(net, DN.init_params(C, S, rng))
+    h = DN.dn_hyper_default()
+    imgs = f32(rng.random((B, C, S, S)))
+    launches, stats = toggled_steps(ctx, lambda seed: dn.train_step(h, imgs, seed=seed))
+    m, v, t = dn.get_adam_state()
+    out = {"stats": stats, "adam_m": m, "adam_v": v, "adam_t": np.array([t])}
+    for net in (0, 1):
+        out.update({"params_%d" % net: dn.get_params(net), "grads_%d" % net: dn.get_grads(net),
+                    "bn_state_%d" % net: dn.get_bn_state(net), "forward_eval_%d" % net: dn.forward(net, imgs, False)})
+    out["denoise"] = dn.denoise(f32(rng.random((B, C, S, S))))
+    dn.close()
+    ctx.close()
+    return out, launches
+
+
+def case_ae(B=128, S=32, d=256):
+    import face_generator_b200 as fg
+    from face_generator_b200 import autoencoder as AE
+    rng = np.random.default_rng(71)
+    ctx = fg.Context(0, max_batch=B, channels=1)
+    ae = AE.Autoencoder(ctx, S, d)
+    ae.set_params(AE.init_params(S, d, rng))
+    h = AE.ae_hyper_default()
+    imgs = f32(rng.random((B, 1, S, S)))
+    launches, stats = toggled_steps(ctx, lambda seed: ae.train_step(h, imgs, seed=seed))
+    m, v, t = ae.get_adam_state()
+    code, y = ae.forward(imgs, training=False)
+    out = {"stats": stats, "params": ae.get_params(), "grads": ae.get_grads(), "adam_m": m, "adam_v": v,
+           "adam_t": np.array([t]), "forward_code": code, "forward_out": y,
+           "reconstruct": ae.reconstruct(f32(rng.random((B, 1, S, S))))}
+    ae.close()
+    ctx.close()
+    return out, launches
+
+
+def free_after_create(B=256):
+    """free device memory (bytes) right after fg_create(max_batch B, 3 channels), and before it"""
+    import face_generator_b200 as fg
+    import torch
+    torch.cuda.synchronize()
+    before = torch.cuda.mem_get_info()[0]
+    ctx = fg.Context(0, max_batch=B, channels=C)
+    ctx.sync()
+    after = torch.cuda.mem_get_info()[0]
+    ctx.close()
+    return {"before": before, "after": after, "used_by_create": before - after}
+
+
 def run(args):
     from face_generator_b200.lib import load_library
     load_library(os.path.abspath(args.lib))
@@ -263,6 +334,15 @@ def run(args):
         cases += [("c2f%d.B256.default" % S, lambda S=S: case_c2f(256, imgs, S)) for S in (16, 64)]
     if "lop" in only:
         cases.append(("lop.conv2d_f16", case_lop))
+    if "dn" in only:
+        cases.append(("dn.S16.B128", case_dn))
+    if "ae" in only:
+        cases.append(("ae.S32.B128", case_ae))
+    os.makedirs(args.out, exist_ok=True)
+    mem = free_after_create()
+    with open(os.path.join(args.out, "free_after_create.json"), "w") as f:
+        json.dump(mem, f)
+    print("free memory after fg_create(256, 3): %s" % mem, flush=True)
     for name, fn in cases:
         out, launches = fn()
         d = os.path.join(args.out, name)
@@ -277,6 +357,9 @@ def run(args):
 def compare(args):
     bad = 0
     for name in sorted(os.listdir(args.A)):
+        if name.endswith(".json"):
+            print("%-28s A %s  B %s" % (name, *(open(os.path.join(d, name)).read() for d in (args.A, args.B))))
+            continue
         da, db = os.path.join(args.A, name), os.path.join(args.B, name)
         la, lb = (json.load(open(os.path.join(d, "launches.json"))) for d in (da, db))
         keys = sorted(f[:-4] for f in os.listdir(da) if f.endswith(".npy"))
@@ -304,7 +387,7 @@ def main():
     r = sub.add_parser("run")
     r.add_argument("--lib", required=True)
     r.add_argument("--out", required=True)
-    r.add_argument("--only", default="32,s16,c2f,lop")
+    r.add_argument("--only", default="32,s16,c2f,lop,dn,ae")
     c = sub.add_parser("compare")
     c.add_argument("A")
     c.add_argument("B")
