@@ -58,7 +58,7 @@ int64_t debug_tensor_copy(fg_ctx* c, const char* what, const DebugTensor* ents, 
     if (strcmp(e.name, name)) continue;
     const int64_t n = e.per * e.B;
     if (!e.p) {
-      fg_set_error("%s: '%s' has not been produced (Dstep.*: option \"debug_keep\" + a train step)", what, name);
+      fg_set_error("%s: '%s' has not been produced (Dstep.* / Dbwd.*: option \"debug_keep\" + a train step / D backward)", what, name);
       return -1;
     }
     if (dst) {

@@ -60,6 +60,10 @@ struct Net32 {
   float D_drop_scale = 2.0f, D_spatial_eval = 0.8f;  // 1/(1-p_drop), 1-p_spatial of the last forward
   float *D_dlogit = nullptr, *D_dh = nullptr, *D_dzl = nullptr, *D_dz = nullptr, *D_dp = nullptr, *D_dx = nullptr;
   float* D_targets = nullptr;
+  // option "debug_keep" (tests): the backward reuses D_dh / D_dzl / D_dp / D_dz across layers, so D_backward copies
+  // each one as a kernel wrote it ("Dbwd.*" debug tensors, the last D backward; Keep::src is unused here)
+  std::vector<NetPair::Keep> bwd_keep;
+  int bwd_keep_B = 0;
   // staging
   float* io_dev2 = nullptr;
   float *in_noiseD = nullptr, *in_noiseG = nullptr;
@@ -144,6 +148,10 @@ int n32_alloc(Net32* n) {
   p.keep = {{"Dstep.z1", n->D_z[0], 65536}, {"Dstep.z2", n->D_z[1], 32768}, {"Dstep.z3", n->D_z[2], 16384},
             {"Dstep.z4", n->D_z[3], 8192},  {"Dstep.zl1", n->D_zl1, 512},    {"Dstep.zl2", n->D_zl2, 512},
             {"Dstep.logit", n->D_logit, 1}, {"Dstep.out", n->D_out, 1}};
+  n->bwd_keep = {{"Dbwd.dh3", nullptr, 512},    {"Dbwd.dzl2", nullptr, 512},  {"Dbwd.dh2", nullptr, 512},
+                 {"Dbwd.dzl1", nullptr, 512},   {"Dbwd.dp4", nullptr, 2048},  {"Dbwd.dz4", nullptr, 8192},
+                 {"Dbwd.dp3", nullptr, 4096},   {"Dbwd.dz3", nullptr, 16384}, {"Dbwd.dp2", nullptr, 8192},
+                 {"Dbwd.dz2", nullptr, 32768},  {"Dbwd.dp1", nullptr, 16384}, {"Dbwd.dz1", nullptr, 65536}};
   FG_CUDA(cudaStreamSynchronize(c->stream));
   return FG_OK;
 }
@@ -206,6 +214,17 @@ int D_forward(Net32* n, const float* x, int B, bool training, const fg_hyper* h)
   return FG_OK;
 }
 
+// option "debug_keep": bwd_keep[k].copy = the first B samples of src, bit for bit (allocated by the first use)
+int keep_bwd(Net32* n, int k, const float* src, int B) {
+  fg_ctx* c = n->c;
+  if (!c->debug_keep) return FG_OK;
+  NetPair::Keep& e = n->bwd_keep[k];
+  if (!e.copy) FG_CUDA(cudaMalloc((void**)&e.copy, sizeof(float) * c->maxB * e.per));
+  FG_CUDA(cudaMemcpyAsync(e.copy, src, sizeof(float) * B * e.per, cudaMemcpyDeviceToDevice, c->stream));
+  n->bwd_keep_B = B;
+  return FG_OK;
+}
+
 // dlogit [B]; want_dx: the image gradient into D_dx (NHWC)
 int D_backward(Net32* n, const float* dlogit, bool want_wgrad, bool want_dx) {
   fg_ctx* c = n->c;
@@ -228,6 +247,7 @@ int D_backward(Net32* n, const float* dlogit, bool want_wgrad, bool want_dx) {
     ScopedTimer tm(c, "D.L3.dgrad");
     FG_TRY(k_gemv_dgrad(c, dlogit, P + L.L3W, n->D_dh, B, 512));
   }
+  FG_TRY(keep_bwd(n, 0, n->D_dh, B));
   TcOp& dy = n->env.dy;  // the producers below say in its flags what they already did for the layer that follows
   float* GD = want_wgrad ? G : nullptr;
   {
@@ -235,15 +255,19 @@ int D_backward(Net32* n, const float* dlogit, bool want_wgrad, bool want_dx) {
     FG_TRY(k_lin_act_drop_bwd(c, n->D_dh, n->D_zl2, P + L.a6, masks, 1472, scale, n->D_dzl, want_wgrad ? G + L.a6 : nullptr, B,
                               512));
   }
+  FG_TRY(keep_bwd(n, 1, n->D_dzl, B));
   FG_TRY(convl_bwd(n->env, n->DL2, n->D_hl1, n->D_dzl, GD, n->D_dh, B));
+  FG_TRY(keep_bwd(n, 2, n->D_dh, B));
   {
     AmaxInto am(c, n->DL1.sdy, &dy.amax_ready);
     FG_TRY(k_lin_act_drop_bwd(c, n->D_dh, n->D_zl1, P + L.a5, masks, 960, scale, n->D_dzl, want_wgrad ? G + L.a5 : nullptr, B,
                               512));
   }
+  FG_TRY(keep_bwd(n, 3, n->D_dzl, B));
   FG_TRY(convl_bwd(n->env, n->DL1, n->D_p[3], n->D_dzl, GD, n->D_dp, B));
   for (int i = 3; i >= 0; --i) {
     const int H = kDhw[i];
+    FG_TRY(keep_bwd(n, 4 + 2 * (3 - i), n->D_dp, B));  // "Dbwd.dp<i+1>": the input of layer i's act/pool backward
     // dz and, for the tensor-core layers, its TF32 split in one pass, + the conv bias gradient (column sums of dz)
     dy.split_ready = convl_tc_bwd(c, n->Dc[i]) && !tc_f16(c);
     dy.bias_ready = want_wgrad;
@@ -253,6 +277,7 @@ int D_backward(Net32* n, const float* dlogit, bool want_wgrad, bool want_dx) {
                               want_wgrad ? G + L.ca[i] : nullptr, B, H, H, kDcout[i], dy.split_ready ? dy.hi : nullptr,
                               dy.split_ready ? dy.lo : nullptr, want_wgrad ? G + L.cb[i] : nullptr));
     }
+    FG_TRY(keep_bwd(n, 5 + 2 * (3 - i), n->D_dz, B));
     float* din = i > 0 ? n->D_dp : want_dx ? n->D_dx : nullptr;
     FG_TRY(convl_bwd(n->env, n->Dc[i], i == 0 ? n->D_x : n->D_p[i - 1], n->D_dz, GD, din, B));
   }
@@ -298,6 +323,8 @@ void net32_free(fg_ctx* c) {
   Net32* n = c->n32;
   if (!n) return;
   pair_free(n->net);
+  for (NetPair::Keep& k : n->bwd_keep)
+    if (k.copy) cudaFree(k.copy);
   for (void* p : n->allocs) cudaFree(p);
   delete n;
   c->n32 = nullptr;
@@ -587,9 +614,12 @@ int64_t fg_debug_tensor(fg_ctx* c, const char* name, float* dst, int64_t max_ele
   const int db = n->D_B;
   std::vector<DebugTensor> ents = {
       {"D.z1", n->D_z[0], 65536, db}, {"D.z2", n->D_z[1], 32768, db}, {"D.z3", n->D_z[2], 16384, db},
-      {"D.z4", n->D_z[3], 8192, db}, {"D.p4", n->D_p[3], 2048, db}, {"D.logit", n->D_logit, 1, db},
+      {"D.z4", n->D_z[3], 8192, db}, {"D.p1", n->D_p[0], 16384, db}, {"D.p2", n->D_p[1], 8192, db},
+      {"D.p3", n->D_p[2], 4096, db}, {"D.p4", n->D_p[3], 2048, db}, {"D.logit", n->D_logit, 1, db},
       {"D.out", n->D_out, 1, db}, {"D.dx", n->D_dx, 1024 * c->C, db}, {"D.masks", n->D_masks, kMaskPerSample, db},
-      {"D.zl1", n->D_zl1, 512, db}, {"D.zl2", n->D_zl2, 512, db}};
+      {"D.zl1", n->D_zl1, 512, db}, {"D.hl1", n->D_hl1, 512, db}, {"D.zl2", n->D_zl2, 512, db},
+      {"D.hl2", n->D_hl2, 512, db}, {"D.dlogit", n->D_dlogit, 1, db}};
+  for (const NetPair::Keep& k : n->bwd_keep) ents.push_back({k.name, k.copy, k.per, n->bwd_keep_B});
   pair_keep_rows(n->net, ents);
   gen_debug_rows(n->G, ents);
   return debug_tensor_copy(c, "fg_debug_tensor", ents.data(), ents.size(), name, dst, max_elems);
