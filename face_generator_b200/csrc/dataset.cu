@@ -331,6 +331,7 @@ int fg_dataset_destroy(fg_dataset* d) {
     d->c->graph_epoch++;
   }
   jpeg_scratch_free(d->jpeg);
+  jpeg_enc_scratch_free(d->jpeg_enc);
   cudaFree(d->data);
   cudaFree(d->idx);
   delete d;

@@ -569,6 +569,8 @@ int64_t debug_tensor_copy(fg_ctx* c, const char* what, const DebugTensor* ents, 
 // ---- dataset.cu / jpeg.cu: the device-resident dataset ----
 struct JpegScratch;                     // fg_dataset_upload_jpeg's chunk buffers (jpeg.cu), made on first use
 void jpeg_scratch_free(JpegScratch* s);
+struct JpegEncScratch;                  // fg_dataset_encode_jpeg / fg_dataset_jpeg_roundtrip's chunk buffers (jpeg_enc.cu)
+void jpeg_enc_scratch_free(JpegEncScratch* s);
 struct fg_dataset {
   fg_ctx* c = nullptr;
   int64_t N = 0;
@@ -576,6 +578,7 @@ struct fg_dataset {
   uint8_t* data = nullptr;  // [N][Cs][Hs][Ws]
   int32_t* idx = nullptr;   // [maxB] staging for host index lists / drawn indices
   JpegScratch* jpeg = nullptr;
+  JpegEncScratch* jpeg_enc = nullptr;
 };
 // ---- dataset.cu: inputs of the device-fed --scale 16 / coarse-to-fine steps (launches on the ctx stream) ----
 // root (optional): the stream is *root * kinds + seed, read on the device (a captured step replays with a new seed)

@@ -24,6 +24,7 @@
 
 #include "fg_internal.h"
 #include "k_jpeg.cuh"
+#include "k_jpeg_enc.cuh"
 
 using jpg::BandDesc;
 using jpg::ImageDesc;
@@ -443,6 +444,22 @@ int64_t finish(Slot& s, int* rc) {
 }
 
 }  // namespace
+
+int jpeg_idct_band_rows(const ImageDesc& m, int* smem) {
+  int rows = 1;
+  while (rows < m.mcuy && jpg::band_bytes(m, 0, rows + 1) <= kBandBudget) ++rows;
+  *smem = 0;
+  for (int r0 = 0; r0 < m.mcuy; r0 += rows) *smem = std::max(*smem, jpg::band_bytes(m, r0, std::min(m.mcuy, r0 + rows)));
+  return rows;
+}
+
+int jpeg_idct_launch(fg_ctx* c, const TableSet* sets, const ImageDesc* imgs, const BandDesc* bands, int n_bands, int smem,
+                     const int16_t* coef, uint8_t* data) {
+  if (smem > 48 * 1024) FG_CUDA(cudaFuncSetAttribute(jpeg_idct_color_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  jpeg_idct_color_kernel<<<n_bands, kIdctThreads, smem, c->stream>>>(sets, imgs, bands, coef, data);
+  LAUNCH_CHECK(c);
+  return FG_OK;
+}
 
 extern "C" {
 

@@ -7,6 +7,8 @@
     fine, coarse, diff = ds.gather_c2f(indices, 16)   # dataset_c2f.lua _toResult (train_c2f.lua --coarseSize 16)
     ds = DeviceDataset.from_dirs(ctx, ["faces/"])  # dataset.loadImagesFromDirs: .jpg files decoded on the GPU
     ds = DeviceDataset.from_lfw(ctx, ["lfw/"])     # generate_dataset.py's out_aug_64x64, built on the GPU from LFW
+    ds = DeviceDataset.from_lfw(ctx, ["lfw/"], jpeg_quality=75)  # ... as its quality-75 .jpg files decode
+    ds.save_jpeg("out_aug_64x64/")                # and those files themselves, {i:06}_{a:03}.jpg, encoded on the GPU
     stats = ds.train_step(hyper, B, seed)         # adversarial.lua loop body with no host->device traffic
     stats = ds.train_step_iters(hyper, B, 2, 1, seed)          # --D_iterations 2: two D iterations, one G iteration
     S16(ctx).train_step_dataset(ds, hyper, B, seed)            # the same for the --scale 16 nets
@@ -157,14 +159,16 @@ class DeviceDataset:
         return ds
 
     @classmethod
-    def from_lfw(cls, ctx: Context, dirs, augmentations=19, seed=43, size=64, chunk=2048):
+    def from_lfw(cls, ctx: Context, dirs, augmentations=19, seed=43, size=64, chunk=2048, jpeg_quality=None):
         """dataset/generate_dataset.py on the GPU: the augmented LFW training set (out_aug_64x64 with the defaults,
         out_unaug_64x64 with augmentations=0) straight into a device cache of len(files) * (1 + augmentations) rows,
         3 planes (a 1-channel context gathers image.rgb2y of them), size x size.  Row i * (1 + augmentations) + a is
         augmentation a of photo i of list_lfw_files(dirs), a = 0 the photo itself: the order of the reference's file
         names {i:06}_{a:03}.jpg.  The photos are decoded on the GPU `chunk` at a time into a scratch cache that the
         chunk's rows are built from (fg_dataset_upload_jpeg, fg_dataset_augment); the descriptors come from
-        fg_lfw_aug_params(seed), so the result does not depend on `chunk`."""
+        fg_lfw_aug_params(seed), so the result does not depend on `chunk`.  jpeg_quality = q (75 for the reference's
+        misc.imsave) then passes every row through jpeg_roundtrip(q): the rows are what the reference's files decode
+        to.  save_jpeg writes those files."""
         files = list_lfw_files(dirs)
         if not files:
             raise FileNotFoundError("no .jpg files in %s or their direct subdirectories" % (dirs,))
@@ -172,6 +176,7 @@ class DeviceDataset:
             _, Hs, Ws = jpeg_info(f.read())
         per = 1 + augmentations
         ds = cls(ctx, shape=(len(files) * per, 3, size, size))
+        ds.per = per
         try:
             for s in range(0, len(files), chunk):
                 blobs = []
@@ -189,6 +194,8 @@ class DeviceDataset:
                     ds.augment(scratch, s * per, augs)
                 finally:
                     scratch.close()
+            if jpeg_quality is not None:
+                ds.jpeg_roundtrip(quality=jpeg_quality)
         except Exception:
             ds.close()
             raise
@@ -219,6 +226,47 @@ class DeviceDataset:
             err = FGError("fg_dataset_upload_jpeg failed (%d): %s" % (rc, self.lib.fg_last_error().decode()))
             err.rc, err.index = rc, (failed.value if failed.value >= 0 else None)
             raise err
+
+    def encode_jpeg(self, first=0, count=None, quality=75):
+        """fg_dataset_encode_jpeg: rows [first, first + count) as JPEG files (list of bytes), byte for byte what
+        Pillow's Image.save(f, "JPEG", quality=quality) writes (3 planes: YCbCr 4:2:0, 1 plane: grayscale).  The
+        output buffer is sized from a guess first and, when that is short, once more from the sizes reported."""
+        count = self.N - first if count is None else count
+        offsets = np.zeros(count + 1, np.int64)
+        _, Cs, Hs, Ws = self.shape
+        cap = count * (700 + Cs * Hs * Ws // 2)
+        for attempt in range(2):
+            out = np.empty(max(cap, 1), np.uint8)
+            rc = self.lib.fg_dataset_encode_jpeg(self.h, first, count, quality, out.ctypes.data_as(C.c_void_p), cap,
+                                                 offsets.ctypes.data_as(C.c_void_p))
+            if rc == 0:
+                break
+            if attempt or offsets[-1] <= cap:
+                _check(rc, "fg_dataset_encode_jpeg")
+            cap = int(offsets[-1])
+        data = out.tobytes()
+        return [data[offsets[i]:offsets[i + 1]] for i in range(count)]
+
+    def jpeg_roundtrip(self, first=0, count=None, quality=75):
+        """fg_dataset_jpeg_roundtrip: rows [first, first + count) replaced in place by what upload_jpeg gives on
+        encode_jpeg's files, without leaving the device."""
+        count = self.N - first if count is None else count
+        _check(self.lib.fg_dataset_jpeg_roundtrip(self.h, first, count, quality), "fg_dataset_jpeg_roundtrip")
+
+    def save_jpeg(self, directory, quality=75, names=None, per=None, chunk=16384):
+        """Every row as a JPEG file in `directory` (created if missing), encoded on the GPU `chunk` rows at a time.
+        names: one file name per row; by default generate_dataset.py's {i:06}_{a:03}.jpg for a cache of `per` rows
+        per photo (row i * per + a), `per` defaulting to the 1 + augmentations of from_lfw, else 1."""
+        per = per or getattr(self, "per", 1)
+        if names is None:
+            names = ["%06d_%03d.jpg" % (r // per, r % per) for r in range(self.N)]
+        if len(names) != self.N:
+            raise ValueError("%d names for %d rows" % (len(names), self.N))
+        os.makedirs(directory, exist_ok=True)
+        for s in range(0, self.N, chunk):
+            for name, b in zip(names[s:s + chunk], self.encode_jpeg(s, min(chunk, self.N - s), quality)):
+                with open(os.path.join(directory, name), "wb") as f:
+                    f.write(b)
 
     def download(self, first=0, count=None):
         """fg_dataset_download: rows [first, first + count) of the cache, [count][Cs][Hs][Ws] uint8."""

@@ -134,6 +134,8 @@ SYMBOLS = {
     "fg_dataset_download": (_I, [_P, _L, _L, _P]),
     "fg_jpeg_info": (_I, [_P, _L, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)]),
     "fg_dataset_upload_jpeg": (_I, [_P, _L, _L, _P, _P, C.POINTER(_L)]),
+    "fg_dataset_encode_jpeg": (_I, [_P, _L, _L, _I, _P, _L, _P]),
+    "fg_dataset_jpeg_roundtrip": (_I, [_P, _L, _L, _I]),
     "fg_lfw_aug_params": (_I, [_U64, _L, _L, _I, _I, _I, _P]),
     "fg_dataset_augment": (_I, [_P, _P, _L, _P, _L]),
     "fg_dataset_gather": (_I, [_P, _P, _I, _P]),

@@ -8,6 +8,8 @@
 --
 --   local ds = b200.loadImagesToDevice(ctx, DATASET.dirs, 'jpg', 3, 1, 250000)
 --   local ds = b200.loadLFWToDevice(ctx, {'/data/lfw'}, 19, 43)   -- out_aug_64x64, on the GPU
+--   local ds = b200.loadLFWToDevice(ctx, {'/data/lfw'}, 19, 43, 64, 2048, 75)   -- ... as its .jpg files decode
+--   b200.saveDatasetJPEG(ds, 'out_aug_64x64', 75, 20)               -- and those files, encoded on the GPU
 --   F.check(C.fg_train_step_dataset(ctx, ds, hyper, B, seed, stats), 'fg_train_step_dataset')
 require 'paths'
 local ffi = require 'ffi'
@@ -157,7 +159,9 @@ end
 -- out_aug_64x64, 0 is out_unaug_64x64; seed defaults to generate_dataset.py's 43.  Photos are decoded on the GPU
 -- `chunk` at a time into a scratch cache and augmented from there (fg_dataset_upload_jpeg, fg_lfw_aug_params,
 -- fg_dataset_augment).
-function b200.loadLFWToDevice(ctx, dirs, augmentations, seed, size, chunk)
+-- quality (optional, last): pass every row through fg_dataset_jpeg_roundtrip(quality) -- 75 gives the rows the
+-- reference's quality-75 files decode to; nil keeps the rows before any JPEG encoding
+function b200.loadLFWToDevice(ctx, dirs, augmentations, seed, size, chunk, quality)
   augmentations = augmentations or 19
   seed = seed or 43
   size = size or 64
@@ -206,7 +210,34 @@ function b200.loadLFWToDevice(ctx, dirs, augmentations, seed, size, chunk)
     if msg then error(string.format('LFW augmentation failed (%d): %s', rc, msg)) end
     collectgarbage()
   end
+  if quality then
+    F.check(C.fg_dataset_jpeg_roundtrip(ds, 0, #files * per, quality), 'fg_dataset_jpeg_roundtrip')
+  end
   return ds
+end
+
+-- every row of ds as a JPEG file in dir (which must exist), encoded on the GPU at quality (default 75): byte for byte
+-- what generate_dataset.py's misc.imsave wrote, named {i:06}_{a:03}.jpg for per (default 20) rows per photo
+function b200.saveDatasetJPEG(ds, dir, quality, per)
+  quality = quality or 75
+  per = per or 20
+  local N = tonumber(C.fg_dataset_size(ds))
+  for s = 0, N - 1, CHUNK do
+    local n = math.min(CHUNK, N - s)
+    local offsets = ffi.new('int64_t[?]', n + 1)
+    F.check(C.fg_dataset_encode_jpeg(ds, s, n, quality, nil, 0, offsets), 'fg_dataset_encode_jpeg (sizes)')
+    local total = tonumber(offsets[n])
+    local out = ffi.new('uint8_t[?]', math.max(total, 1))
+    F.check(C.fg_dataset_encode_jpeg(ds, s, n, quality, out, total, offsets), 'fg_dataset_encode_jpeg')
+    for i = 0, n - 1 do
+      local r = s + i
+      local f = assert(io.open(paths.concat(dir, string.format('%06d_%03d.jpg', math.floor(r / per), r % per)), 'wb'))
+      f:write(ffi.string(out + offsets[i], tonumber(offsets[i + 1] - offsets[i])))
+      f:close()
+    end
+    out = nil
+    collectgarbage()
+  end
 end
 
 return b200

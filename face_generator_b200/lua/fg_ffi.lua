@@ -102,6 +102,8 @@ int fg_dataset_upload(fg_dataset* d, int64_t first, int64_t count, const uint8_t
 int fg_dataset_download(fg_dataset* d, int64_t first, int64_t count, uint8_t* out);
 int fg_jpeg_info(const uint8_t* bytes, int64_t len, int* C, int* H, int* W);
 int fg_dataset_upload_jpeg(fg_dataset* d, int64_t first, int64_t count, const uint8_t* bytes, const int64_t* offsets, int64_t* failed_out);
+int fg_dataset_encode_jpeg(fg_dataset* d, int64_t first, int64_t count, int quality, uint8_t* out, int64_t cap, int64_t* offsets);
+int fg_dataset_jpeg_roundtrip(fg_dataset* d, int64_t first, int64_t count, int quality);
 typedef struct fg_aug { int64_t src; int32_t warp, hflip; double brightness; double m[9]; } fg_aug;
 int fg_lfw_aug_params(uint64_t seed, int64_t first_src, int64_t n_src, int n_aug, int src_h, int src_w, fg_aug* out);
 int fg_dataset_augment(fg_dataset* src, fg_dataset* dst, int64_t dst_first, const fg_aug* augs, int64_t n);

@@ -351,6 +351,22 @@ int fg_dataset_download(fg_dataset* d, int64_t first, int64_t count, uint8_t* ou
 int fg_jpeg_info(const uint8_t* bytes, int64_t len, int* C, int* H, int* W);
 int fg_dataset_upload_jpeg(fg_dataset* d, int64_t first, int64_t count, const uint8_t* bytes, const int64_t* offsets,
                            int64_t* failed_out);
+/* The other direction (dataset/generate_dataset.py's misc.imsave): rows [first, first+count) as
+ * baseline JFIF files, byte for byte what Pillow's Image.save(f, "JPEG", quality=quality) writes for
+ * them (3 planes: YCbCr 4:2:0; 1 plane: grayscale; standard Huffman tables, no restart markers).
+ * quality 1..100; any size the cache holds.
+ * fg_dataset_encode_jpeg: offsets[count+1] (host) is always filled: file i = out[offsets[i] ..
+ * offsets[i+1]).  If offsets[count] > cap, nothing is written to out and the call returns
+ * FG_ERR_INVALID (the caller retries with that size); out may be NULL to ask for the sizes only.
+ * out may be host or device memory.
+ * fg_dataset_jpeg_roundtrip: rows [first, first+count) replaced in place by decode(encode(row,
+ * quality)), what fg_dataset_upload_jpeg gives on fg_dataset_encode_jpeg's files, without leaving
+ * the device.
+ * An out-of-range span, a quality outside 1..100 or a NULL offsets is FG_ERR_INVALID and launches
+ * nothing.  Both run in bounded chunks on the ctx stream and return once the work is done.          */
+int fg_dataset_encode_jpeg(fg_dataset* d, int64_t first, int64_t count, int quality, uint8_t* out, int64_t cap,
+                           int64_t* offsets);
+int fg_dataset_jpeg_roundtrip(fg_dataset* d, int64_t first, int64_t count, int quality);
 /* The augmented LFW training set (dataset/generate_dataset.py + ImageAugmenter.py): each output row
  * is LFW-crop's 84x84 box (rows 92..175, cols 83..166) of a source row, resized to the destination's
  * Ho x Wo as Pillow's Image.resize(BILINEAR) does (scipy.misc.imresize).  A descriptor with warp = 1
