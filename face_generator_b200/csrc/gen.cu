@@ -1,6 +1,6 @@
 // UpsGen: the generator of models.lua at side S, create_G_decoder_upsampling32 (models.lua:57-81, S = 32) or
-// create_G_decoder_upsampling16 (models.lua:27-51, S = 16: the same layers with every spatial size halved).  The 32x32
-// nets (nets.cu) and the --scale 16 nets (nets_s16.cu) own one each; what differs between them is data (GenDesc).
+// create_G_decoder_upsampling16 (models.lua:27-51, S = 16: the same layers with every spatial size halved).  The trainer
+// of the 32x32 and --scale 16 nets (UpsGan, ups_gan.cu) owns one; what differs between the sizes is data (GenDesc).
 #include "convl.h"
 
 GLayout make_g_layout(int C, int side) {

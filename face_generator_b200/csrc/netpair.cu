@@ -1,7 +1,7 @@
 // The trainable state of a G/D pair (NetPair, fg_internal.h) and what every train step does with it: allocation,
 // zeroing and all-reducing the gradients, the accuracy gate and optimizer, the data-parallel broadcast, the statistics
 // mirror, the C ABI's set / get bodies, the CUDA-graph replay of the step and the adversarial.lua loop body itself.
-// Shared by the 32x32 nets (nets.cu), the coarse-to-fine nets (nets_c2f.cu) and the --scale 16 nets (nets_s16.cu).
+// Shared by the trainer of the 32x32 and --scale 16 nets (ups_gan.cu) and the coarse-to-fine nets (nets_c2f.cu).
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
