@@ -90,6 +90,12 @@ int ctx_alloc(fg_ctx* c) {
   FG_TRY(dalloc(&c->bn_acc, 4 * 256 * 2));  // doubles
   FG_TRY(dalloc(&c->bn_slice_acc, 32 * 4 * 256 * 2 + 64));  // doubles + tickets (zero-initialised)
   FG_TRY(dalloc(&c->bn_parts, B * 3072));  // G.C2: 8 tiles/image x 3 x 128 ch; G.C1: 2 tiles/image x 3 x 256 ch
+  fg_ctx::Workspaces& s = c->side_ws;  // the same for a generator forward on side_stream
+  FG_TRY(dalloc(&s.red_ws, 2 * c->red_ws_elems));
+  FG_TRY(dalloc(&s.red_ticket, 2));
+  FG_TRY(dalloc(&s.bn_acc, 4 * 256 * 2));
+  FG_TRY(dalloc(&s.bn_slice_acc, 32 * 4 * 256 * 2 + 64));
+  FG_TRY(dalloc(&s.bn_parts, B * 3072));
   c->io_dev_elems = std::max<size_t>(B * 1024 * C, B * kMaskPerSample);
   return dalloc(&c->io_dev, c->io_dev_elems);
 }
@@ -164,12 +170,13 @@ int fg_destroy(fg_ctx* c) {
   if (!c) return FG_OK;
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
-  if (c->comm_stream) {
-    cudaStreamSynchronize(c->comm_stream);
-    cudaStreamDestroy(c->comm_stream);
-    cudaEventDestroy(c->ev_fork);
-    cudaEventDestroy(c->ev_join);
-  }
+  for (cudaStream_t s : {c->comm_stream, c->side_stream})
+    if (s) {
+      cudaStreamSynchronize(s);
+      cudaStreamDestroy(s);
+    }
+  if (c->ev_fork) cudaEventDestroy(c->ev_fork);
+  if (c->ev_join) cudaEventDestroy(c->ev_join);
   tc_destroy(c);
   net32_free(c);
   ctx_free(c);

@@ -55,19 +55,13 @@ int convl_alloc(ConvLEnv& e, ConvL& L) {
   FG_TRY(convl_dalloc(e, &L.Wp, nw));
   FG_TRY(convl_dalloc(e, &L.Wpd, nw));
   if (L.nA) FG_TRY(convl_dalloc(e, &L.bp, L.Cout));
-  if (!L.x.s) FG_TRY(convl_dalloc(e, &L.x.s, 2));
   if (!e.dy.s) FG_TRY(convl_dalloc(e, &e.dy.s, 2));
-  if (tc_conv_eligible(L.geom_k(e.maxB))) {
-    const int K = L.geom_k(e.maxB).Cin;
-    const size_t nk = (size_t)L.k * L.k * L.Cout * K, nx = (size_t)e.maxB * L.H * L.H * K;
+  const bool tc = tc_conv_eligible(L.geom_k(e.maxB));
+  if (tc) {
+    const size_t nk = (size_t)L.k * L.k * L.Cout * L.geom_k(e.maxB).Cin;
     FG_TRY(convl_dalloc(e, &L.Wf_hi, nk));
     FG_TRY(convl_dalloc(e, &L.Wf_lo, nk));
-    FG_TRY(convl_dalloc(e, &L.x.hi, nx));
-    FG_TRY(convl_dalloc(e, &L.x.lo, nx));
-    if (L.kpad) {  // zero-filled: the pad columns stay zero
-      FG_TRY(convl_dalloc(e, &L.Wpad, nk));
-      FG_TRY(convl_dalloc(e, &L.xpad, nx));
-    }
+    if (L.kpad) FG_TRY(convl_dalloc(e, &L.Wpad, nk));  // zero-filled: the pad columns stay zero
   }
   if (L.need_dgrad && tc_conv_eligible(L.geom_d(e.maxB))) {
     FG_TRY(convl_dalloc(e, &L.Wd_hi, nw));
@@ -78,16 +72,25 @@ int convl_alloc(ConvLEnv& e, ConvL& L) {
   if (L.pad_out && !(tc_conv_eligible(ConvGeom{B, L.H, L.H, L.Cin, L.pad_out, L.k, 1}) &&
                      tc_conv_eligible(ConvGeom{B, L.H, L.H, L.pad_out, L.Cin, L.k, 1}) && L.Cin % 128 == 0))
     L.pad_out = 0;
-  if (L.pad_dy && !(L.x.hi && tc_conv_eligible(ConvGeom{B, L.H, L.H, L.Cin, L.pad_dy, L.k, 1}) && L.Cin % 64 == 0))
+  if (L.pad_dy && !(tc && tc_conv_eligible(ConvGeom{B, L.H, L.H, L.Cin, L.pad_dy, L.k, 1}) && L.Cin % 64 == 0))
     L.pad_dy = 0;
   if (L.pad_out) {
     const size_t nq = (size_t)L.k * L.k * L.pad_out * L.Cin;
     FG_TRY(convl_dalloc(e, &L.Wq_hi, nq));  // zero-initialised: the padding rows stay zero
     FG_TRY(convl_dalloc(e, &L.Wq_lo, nq));
-    const size_t nx = (size_t)B * L.H * L.H * L.Cin;
-    FG_TRY(convl_dalloc(e, &L.x.hi, nx));
-    FG_TRY(convl_dalloc(e, &L.x.lo, nx));
   }
+  return convl_alloc_x(e, L);
+}
+
+int convl_alloc_x(ConvLEnv& e, ConvL& L) {
+  if (!L.x.s) FG_TRY(convl_dalloc(e, &L.x.s, 2));
+  const bool tc = tc_conv_eligible(L.geom_k(e.maxB));
+  if (!tc && !L.pad_out) return FG_OK;
+  // a pad_out layer (Cout <= 4) is never eligible itself: its split holds the Cin input channels
+  const size_t nx = (size_t)e.maxB * L.H * L.H * L.geom_k(e.maxB).Cin;
+  FG_TRY(convl_dalloc(e, &L.x.hi, nx));
+  FG_TRY(convl_dalloc(e, &L.x.lo, nx));
+  if (tc && L.kpad) FG_TRY(convl_dalloc(e, &L.xpad, nx));  // zero-filled: the pad columns stay zero
   return FG_OK;
 }
 
@@ -229,6 +232,10 @@ int upsl_alloc(ConvLEnv& e, UpsL& U) {
   FG_TRY(convl_dalloc(e, &U.Wd_lo, nw36));
   FG_TRY(convl_dalloc(e, &U.Wx_hi, nw25));
   FG_TRY(convl_dalloc(e, &U.Wx_lo, nw25));
+  return upsl_alloc_x(e, U);
+}
+
+int upsl_alloc_x(ConvLEnv& e, UpsL& U) {
   const size_t nx = (size_t)e.maxB * (U.H / 2) * (U.H / 2) * U.Cin;
   FG_TRY(convl_dalloc(e, &U.x.hi, nx));
   FG_TRY(convl_dalloc(e, &U.x.lo, nx));

@@ -38,6 +38,9 @@ int tc_op_split(fg_ctx* c, TcOp& op, const float* x, int64_t n, bool f16);
 inline int pack_key(const fg_ctx* c) { return c->conv_impl | (c->mma_f16 << 4); }
 int convl_dalloc(ConvLEnv& e, float** p, size_t elems);  // zero-filled device buffer, owned by *e.allocs
 int convl_alloc(ConvLEnv& e, ConvL& L);
+// the buffers of L's input operand only (x.s unless set, x's split, xpad): what a copy of the layer that shares its
+// weight packs needs for a forward of its own (gen_alloc_fwd)
+int convl_alloc_x(ConvLEnv& e, ConvL& L);
 bool convl_tc_fwd(const fg_ctx* c, const ConvL& L);  // the forward runs on the tensor cores (it reads the input's split)
 bool convl_tc_bwd(const fg_ctx* c, const ConvL& L);  // ... and so does the data gradient
 int convl_pack(fg_ctx* c, ConvL& L, const float* P);
@@ -48,6 +51,7 @@ int convl_bwd(ConvLEnv& e, ConvL& L, const float* in, const float* dy, float* G,
 
 bool upsl_tc(const fg_ctx* c, const UpsL& U);  // the layer runs on the tensor cores
 int upsl_alloc(ConvLEnv& e, UpsL& U);
+int upsl_alloc_x(ConvLEnv& e, UpsL& U);  // the same share of upsl_alloc (x's split, x.s unless set)
 int upsl_pack(fg_ctx* c, UpsL& U, const float* P);
 // *parts (optional, in: want BatchNorm partials; out: how many tiles wrote one into c->bn_parts, 0 = none)
 int upsl_fwd(ConvLEnv& e, UpsL& U, const float* h, const float* P, float* z, int B, int* parts = nullptr);
@@ -58,6 +62,9 @@ int upsl_bwd(ConvLEnv& e, UpsL& U, TcOp& dy, const float* h, const float* dz, fl
 
 // ---- gen.cu: UpsGen on the owner's layer scratch (ConvLEnv) and parameters (NetPair: PG, gG, bnG, G_pack) ----
 int gen_alloc(ConvLEnv& e, UpsGen& G, const GenDesc& d);
+// a forward-only instance F of an allocated G (F.owner): G's weight packs, its own input operands, scale pairs,
+// activations and batch statistics for batches up to e.maxB
+int gen_alloc_fwd(ConvLEnv& e, UpsGen& F, UpsGen& G);
 int gen_pack(fg_ctx* c, UpsGen& G, NetPair& p);  // unless p.G_pack is the current pack_key()
 // noise: device [B][100] -> G.y (NHWC [B][S][S][C]).  training: batch statistics + running statistics update
 int gen_forward(ConvLEnv& e, UpsGen& G, NetPair& p, const float* noise, int B, bool training);

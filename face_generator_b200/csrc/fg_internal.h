@@ -220,6 +220,7 @@ struct UpsGen {
   float *bn_mean[2] = {nullptr, nullptr}, *bn_istd[2] = {nullptr, nullptr}, *bn_mg = nullptr;
   int B = 0;
   bool train = true, valid = false;
+  UpsGen* owner = nullptr;  // a forward-only instance (gen_alloc_fwd): the instance whose weight packs it reads
   std::deque<std::string> names;  // prefixed timer names (stable storage: the layers point into it)
   const char *t_bn2_finalize = nullptr, *t_bn2_stats = nullptr, *t_bn2_apply = nullptr, *t_bn2_bwd_reduce = nullptr,
              *t_bn2_bwd_apply = nullptr;
@@ -290,7 +291,9 @@ struct fg_ctx {
   // option "dp_overlap" (default 1): D's all-reduce + accuracy gate + optimizer run on comm_stream while the compute
   // stream already runs the G step's G forward (which only needs G's parameters); joined before D is used again
   int dp_overlap = 1;
-  int reserve_sms = 0;  // SMs the persistent convolution kernels leave free while a collective runs next to them
+  // SMs the persistent convolution kernels leave free while a collective, or the D iterations (step_body), run next
+  // to them
+  int reserve_sms = 0;
   // the convolution kernel launched last (fg_get_option "last_conv_*", include/fg_b200.h): FG_KERNEL_*, its tile, its
   // operand format (0 fp32 FFMA, 1 3xTF32, 2 3xFP16) and its K splits.  Set by the launchers where they choose the
   // kernel (note_conv), cleared on entry to every fg_conv2d_* / fg_scu_* / fg_linear_* call.  Host integers only.
@@ -307,6 +310,16 @@ struct fg_ctx {
   uint64_t* seed_dev = nullptr;
   cudaStream_t comm_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  // with one GPU the loop body (step_body) runs the first G iteration's generator forward on side_stream, next to the
+  // D iterations.  side_ws holds a second copy of each workspace above that the generator forward's kernels use;
+  // ctx_swap_side exchanges it and the stream with the context's own.
+  cudaStream_t side_stream = nullptr;
+  struct Workspaces {
+    double* red_ws = nullptr;
+    unsigned* red_ticket = nullptr;
+    double *bn_acc = nullptr, *bn_slice_acc = nullptr;
+    float* bn_parts = nullptr;
+  } side_ws;
   // debug (tests): "debug_keep" = 1 keeps a copy of the D step's pre-activations of every train step (NetPair::keep),
   // which the G step's D forward overwrites (the strict gradient-parity tests read PReLU branch decisions from them)
   bool debug_keep = false;
@@ -517,6 +530,9 @@ struct StepNets {
   int64_t mask;
   bool gate;     // the accuracy gate decides whether D trains; false: it always does (adversarial_c2f.lua)
   bool overlap;  // option dp_overlap may run D's all-reduce, gate and optimizer next to the following G forward
+  // the D iterations take their fakes from a generator of their own, so the first G iteration's generator forward
+  // may run next to the last D iteration's D forward, backward and update (step_body)
+  virtual bool g_side() const { return false; }
   // G in training mode: the B/2 fakes of D iteration j (d_iter), or the B samples of G iteration j; with the
   // condition rows D reads next, if any
   virtual int g_forward(int j, bool d_iter) = 0;
@@ -526,6 +542,8 @@ struct StepNets {
   virtual int d_backward(bool want_wgrad, bool want_dx) = 0;   // from dlogit
   virtual int g_backward() = 0;                                // from D's input gradient
 };
+// c->stream and the workspaces in c->side_ws change places with c->side_stream and the context's own (twice: back)
+void ctx_swap_side(fg_ctx* c);
 // nd D iterations, then ng G iterations, then the statistics to `stats` (may be null).  masksD / masksG (may be null:
 // drawn from the stream root of each iteration) are stacked per iteration; feed (may be null) runs first inside the
 // step, after the stream roots are set: a device-fed step draws its inputs there.  The step is keyed (net_graph_run) on

@@ -26,6 +26,23 @@ GLayout make_g_layout(int C, int side) {
   return L;
 }
 
+namespace {
+// what a forward writes besides the layers' input operands: noise, activations and batch statistics
+int alloc_fwd(ConvLEnv& e, UpsGen& G) {
+  const int S = G.S;
+  const size_t B = e.maxB, n0 = G.GL1.Cout, n1 = (size_t)256 * (S / 2) * (S / 2), n2 = (size_t)128 * S * S,
+               n3 = (size_t)G.C * S * S;
+  for (auto [p, n] : {std::pair<float**, size_t>{&G.noise, kNoiseDim}, {&G.z0, n0}, {&G.h0, n0}, {&G.z1, n1}, {&G.h1, n1},
+                      {&G.z2, n2}, {&G.h2, n2}, {&G.z3, n3}, {&G.y, n3}})
+    FG_TRY(convl_dalloc(e, p, B * n));
+  for (int i = 0; i < 2; ++i) {
+    FG_TRY(convl_dalloc(e, &G.bn_mean[i], G.GU[i].Cout));
+    FG_TRY(convl_dalloc(e, &G.bn_istd[i], G.GU[i].Cout));
+  }
+  return FG_OK;
+}
+}  // namespace
+
 int gen_alloc(ConvLEnv& e, UpsGen& G, const GenDesc& d) {
   fg_ctx* c = e.c;
   const int S = d.side, C = c->C;
@@ -75,17 +92,44 @@ int gen_alloc(ConvLEnv& e, UpsGen& G, const GenDesc& d) {
   G.t_bn2_apply = timer("hbm.G.bn2.apply");
   G.t_bn2_bwd_reduce = timer("hbm.G.bn2.bwd_reduce");
   G.t_bn2_bwd_apply = timer("hbm.G.bn2.bwd_apply");
+  FG_TRY(alloc_fwd(e, G));
   const size_t B = e.maxB, n0 = L1.Cout, n1 = (size_t)256 * (S / 2) * (S / 2), n2 = (size_t)128 * S * S, n3 = (size_t)C * S * S;
-  for (auto [p, n] : {std::pair<float**, size_t>{&G.noise, kNoiseDim}, {&G.z0, n0}, {&G.h0, n0}, {&G.z1, n1}, {&G.h1, n1},
-                      {&G.z2, n2}, {&G.h2, n2}, {&G.z3, n3}, {&G.y, n3}, {&G.dz3, n3},
+  for (auto [p, n] : {std::pair<float**, size_t>{&G.dz3, n3},
                       {&G.dfull, (size_t)256 * S * S},  // full-resolution dgrad of G.C2 on the FFMA path: [B][S][S][256]
                       {&G.dz2, n2}, {&G.dz1, n1}, {&G.dz0, n0}})
     FG_TRY(convl_dalloc(e, p, B * n));
-  for (int i = 0; i < 2; ++i) {
-    FG_TRY(convl_dalloc(e, &G.bn_mean[i], co[i]));
-    FG_TRY(convl_dalloc(e, &G.bn_istd[i], co[i]));
-  }
   return convl_dalloc(e, &G.bn_mg, 512);
+}
+
+int gen_alloc_fwd(ConvLEnv& e, UpsGen& F, UpsGen& G) {
+  F.S = G.S;
+  F.C = G.C;
+  F.gl = G.gl;
+  F.owner = &G;
+  // the layers as G's: its weight packs and timer names; the input operands are replaced below
+  F.GL1 = G.GL1;
+  F.GC3 = G.GC3;
+  F.GU[0] = G.GU[0];
+  F.GU[1] = G.GU[1];
+  F.t_bn2_finalize = G.t_bn2_finalize;
+  F.t_bn2_stats = G.t_bn2_stats;
+  F.t_bn2_apply = G.t_bn2_apply;
+  F.t_bn2_bwd_reduce = G.t_bn2_bwd_reduce;
+  F.t_bn2_bwd_apply = G.t_bn2_bwd_apply;
+  FG_TRY(F.pairs.alloc(e.c, *e.allocs, 4));  // x of G.L1, G.C1, G.C2 and G.C3
+  for (ConvL* L : {&F.GL1, &F.GC3}) {
+    L->x = TcOp{};
+    L->xpad = nullptr;
+    L->sdy = nullptr;
+    FG_TRY(F.pairs.take(&L->x.s));
+    FG_TRY(convl_alloc_x(e, *L));
+  }
+  for (UpsL& U : F.GU) {
+    U.x = TcOp{};
+    FG_TRY(F.pairs.take(&U.x.s));
+    FG_TRY(upsl_alloc_x(e, U));
+  }
+  return alloc_fwd(e, F);
 }
 
 int gen_pack(fg_ctx* c, UpsGen& G, NetPair& p) {
@@ -121,7 +165,13 @@ int bn_stats(fg_ctx* c, UpsGen& G, NetPair& p, int i, const float* z, int B, boo
 int gen_forward(ConvLEnv& e, UpsGen& G, NetPair& p, const float* noise, int B, bool training) {
   fg_ctx* c = e.c;
   FG_REQUIRE(B >= 1 && B <= e.maxB, "G forward: batch %d out of range [1,%d]", B, e.maxB);
-  FG_TRY(gen_pack(c, G, p));
+  if (G.owner) {  // forward-only: the owner's packs, read in the format they were made in
+    FG_TRY(gen_pack(c, *G.owner, p));
+    G.GL1.packed_f16 = G.owner->GL1.packed_f16;
+    G.GC3.packed_f16 = G.owner->GC3.packed_f16;
+  } else {
+    FG_TRY(gen_pack(c, G, p));
+  }
   const GLayout& L = G.gl;
   const float* P = p.PG;
   const int S = G.S;

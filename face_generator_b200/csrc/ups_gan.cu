@@ -1,6 +1,6 @@
 // UpsGan (ups_gan.h): the 32x32 and --scale 16 trainers of train.lua, an UpsGen generator (gen.cu) and a discriminator
 // (GanD) in the adversarial.lua loop body (adversarial.lua:54-300; the loop itself is pair_train_step in netpair.cu), and
-// the bodies of their C entry points, on one stream.
+// the bodies of their C entry points.
 #include "ups_gan.h"
 
 namespace {
@@ -12,15 +12,17 @@ struct GanStep final : StepNets {
   GanStep(UpsGan& n, const fg_hyper* h, int B, const float* real, const float* noiseD, const float* noiseG)
       : StepNets(n.c, n.net, h, B, n.D->logit, n.D->out, n.D->dlogit, n.D->masks, n.d.mask, true, n.d.overlap), n(n),
         D(*n.D), real(real), noiseD(noiseD), noiseG(noiseG) {}
+  bool g_side() const override { return true; }
   int g_forward(int j, bool d_iter) override {
     const int rows = d_iter ? B / 2 : B;
-    return gen_forward(n.env, n.G, n.net, (d_iter ? noiseD : noiseG) + (size_t)j * rows * kNoiseDim, rows, true);
+    return gen_forward(d_iter ? n.env_f : n.env, d_iter ? n.F : n.G, n.net,
+                       (d_iter ? noiseD : noiseG) + (size_t)j * rows * kNoiseDim, rows, true);
   }
   int d_input(int j) override {
     const int Bh = B / 2, HW = n.G.S * n.G.S;
     const size_t img = (size_t)c->C * HW;
     FG_TRY(k_nchw_to_nhwc(c, real + (size_t)j * Bh * img, D.x, Bh, c->C, HW));
-    FG_CUDA(cudaMemcpyAsync(D.x + Bh * img, n.G.y, sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
+    FG_CUDA(cudaMemcpyAsync(D.x + Bh * img, n.F.y, sizeof(float) * Bh * img, cudaMemcpyDeviceToDevice, c->stream));
     return FG_OK;
   }
   int draw_masks(int kind, const uint64_t* root) override { return D.draw_masks(B, kind, h, root); }
@@ -42,6 +44,10 @@ int gan_alloc(UpsGan& n, fg_ctx* c, const GanDesc& d, std::unique_ptr<GanD> D, f
   FG_TRY(pair_alloc(c, n.allocs, n.net, make_g_layout(c->C, d.g.side).total, n.D->layout(c->C), true));
   FG_TRY(n.D->alloc());
   FG_TRY(gen_alloc(e, n.G, d.g));
+  n.env_f.c = c;
+  n.env_f.maxB = c->maxB / 2;
+  n.env_f.allocs = &n.allocs;
+  FG_TRY(gen_alloc_fwd(n.env_f, n.F, n.G));
   const size_t B = c->maxB, img = B * d.g.side * d.g.side * c->C;
   n.img[0] = io;
   if (!io) FG_TRY(convl_dalloc(e, &n.img[0], img));

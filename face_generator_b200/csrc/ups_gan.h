@@ -39,6 +39,11 @@ struct UpsGan {
   GanDesc d{};
   NetPair net;
   UpsGen G;
+  // the generator of the D iterations' fakes: forward only, on G's weight packs, at maxB / 2 (gen_alloc_fwd).  Everything
+  // read from G after a step (its outputs, the "G.*" debug rows) is the G iteration's, and the first G iteration's
+  // forward may run next to the last D iteration (step_body).  env_f: its allocation context
+  UpsGen F;
+  ConvLEnv env_f;
   std::unique_ptr<GanD> D;
   // staging at the C ABI: NCHW images from / to the caller and their NHWC conversion; noise rows (or D's output
   // gradient) from the caller and the noise gradient to it
