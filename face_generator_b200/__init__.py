@@ -7,4 +7,4 @@ tests and bench.py; the reference-side binding is the LuaJIT FFI shim under face
 There is NO CPU fallback: importing works anywhere, but every compute call needs an H100 (sm_90).
 """
 from .lib import FGError, load_library, Context, C2f, S16, hyper_default, MASK_PER_SAMPLE, NOISE_DIM  # noqa: F401
-from . import nn, adversarial, adversarial_c2f, denoiser, autoencoder, pyramid  # noqa: F401
+from . import nn, adversarial, adversarial_c2f, denoiser, autoencoder, pyramid, sheets  # noqa: F401

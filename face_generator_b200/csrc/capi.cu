@@ -179,6 +179,7 @@ int fg_destroy(fg_ctx* c) {
   if (c->ev_join) cudaEventDestroy(c->ev_join);
   tc_destroy(c);
   net32_free(c);
+  jpeg_enc_scratch_free(c->jpeg_enc);
   ctx_free(c);
   for (auto& kv : c->timers)
     for (auto& pr : kv.second.pending) {
@@ -253,6 +254,11 @@ int fg_set_option(fg_ctx* c, const char* key, int64_t v) {
     c->bwd_merge_ctas = v > (1 << 20) ? (1 << 20) : (int)v;
     return FG_OK;
   }
+  if (!strcmp(key, "jpeg_route")) {  // tests only: 0 (default) by file size, 1 one CTA per file, 2 many CTAs per file
+    FG_REQUIRE(v >= 0 && v <= 2, "jpeg_route must be 0 (by file size), 1 (one CTA per file) or 2 (many CTAs per file)");
+    c->jpeg_route = (int)v;
+    return FG_OK;
+  }
   if (!strcmp(key, "debug_keep")) {  // keep the D step's pre-activations of fg_train_step ("Dstep.*" debug tensors)
     c->debug_keep = v != 0;
     return FG_OK;
@@ -280,6 +286,7 @@ int64_t fg_get_option(fg_ctx* c, const char* key) {
   if (!c || !key) return -1;
   if (!strcmp(key, "conv_impl")) return c->conv_impl;
   if (!strcmp(key, "max_batch")) return c->maxB;
+  if (!strcmp(key, "jpeg_route")) return c->jpeg_route;
   if (!strcmp(key, "channels")) return c->C;
   if (!strcmp(key, "sm_count")) return c->sm_count;
   if (!strcmp(key, "bn_epilogue")) return c->bn_epilogue;

@@ -130,8 +130,8 @@ __global__ void uniform_pm1_kernel(float* __restrict__ out, int64_t n, uint64_t 
 constexpr int kQG = 4;
 template <bool U8>
 __global__ void __launch_bounds__(256) nearest_kernel(const float* __restrict__ cands, const uint8_t* __restrict__ data, int64_t N,
-                                                      int D, int C, int Cs, int Hs, int Ws, const float* __restrict__ queries, int Q,
-                                                      unsigned long long* __restrict__ best) {
+                                                      int D, int C, int Cs, int Hs, int Ws, int S, const float* __restrict__ queries,
+                                                      int Q, unsigned long long* __restrict__ best) {
   extern __shared__ float qs[];  // [kQG][D]
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   const bool gray = Cs == 3 && C == 1;
@@ -146,9 +146,9 @@ __global__ void __launch_bounds__(256) nearest_kernel(const float* __restrict__ 
         float v;
         if (!U8) {
           v = cands[cand * D + i];
-        } else {  // the 32x32 view of the cached image, same arithmetic as gather_kernel
-          const int x = i & 31, y = (i >> 5) & 31, ch = i >> 10;
-          const Span sy = axis_span(y, Hs, 32), sx = axis_span(x, Ws, 32);
+        } else {  // the S x S view of the cached image, same arithmetic as gather_kernel
+          const int x = i % S, y = (i / S) % S, ch = i / (S * S);
+          const Span sy = axis_span(y, Hs, S), sx = axis_span(x, Ws, S);
           const uint8_t* base = data + cand * (int64_t)Cs * Hs * Ws;
           float acc_y = 0.f;
           for (int yy = sy.i0; yy <= sy.i1; ++yy) {
@@ -220,9 +220,9 @@ int stage_indices(fg_dataset* d, const int32_t* idx, int B, const char* what, co
   *idx_dev = d->idx;
   return FG_OK;
 }
-// queries [Q][D] (host or device); candidates either fp32 [N][D] (host or device) or the dataset cache.
-// idx_out / dist_out: host or device, Q entries each.
-int nearest_run(fg_ctx* c, const float* cands, const fg_dataset* d, int64_t N, int D, const float* queries, int Q,
+// queries [Q][D] (host or device); candidates either fp32 [N][D] (host or device) or the dataset cache at S x S
+// (D = C*S*S).  idx_out / dist_out: host or device, Q entries each.
+int nearest_run(fg_ctx* c, const float* cands, const fg_dataset* d, int S, int64_t N, int D, const float* queries, int Q,
                 int32_t* idx_out, float* dist_out) {
   FG_REQUIRE(queries && idx_out && dist_out && Q >= 1 && N >= 1 && D >= 1 && D <= 12288 && N < ((int64_t)1 << 32),
              "nearest: need 1 <= D <= 12288 (3x64x64), Q >= 1, 1 <= N < 2^32");
@@ -262,9 +262,9 @@ int nearest_run(fg_ctx* c, const float* cands, const fg_dataset* d, int64_t N, i
       if (fail(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute")) break;
     }
     if (d)
-      nearest_kernel<true><<<grid, 32 * warps, smem, c->stream>>>(nullptr, d->data, N, D, c->C, d->Cs, d->Hs, d->Ws, qd, Q, best);
+      nearest_kernel<true><<<grid, 32 * warps, smem, c->stream>>>(nullptr, d->data, N, D, c->C, d->Cs, d->Hs, d->Ws, S, qd, Q, best);
     else
-      nearest_kernel<false><<<grid, 32 * warps, smem, c->stream>>>(cd, nullptr, N, D, 0, 0, 0, 0, qd, Q, best);
+      nearest_kernel<false><<<grid, 32 * warps, smem, c->stream>>>(cd, nullptr, N, D, 0, 0, 0, 0, 0, qd, Q, best);
     c->launches++;
     if (fail(cudaGetLastError(), "nearest_kernel")) break;
     nearest_unpack_kernel<<<(Q + 127) / 128, 128, 0, c->stream>>>(best, Q, idx_dev, dist_dev);
@@ -505,12 +505,18 @@ int fg_nearest(fg_ctx* c, const float* queries, int Q, const float* cands, int64
   }
   FG_CUDA(cudaSetDevice(c->device));
   FG_REQUIRE(cands, "fg_nearest: null candidates");
-  return nearest_run(c, cands, nullptr, N, D, queries, Q, idx_out, dist_out);
+  return nearest_run(c, cands, nullptr, 0, N, D, queries, Q, idx_out, dist_out);
 }
 // sample.lua:141-159 findClosestNeighboursOf against the device-resident training set (32x32 view of every image)
 int fg_dataset_nearest(fg_dataset* d, const float* queries, int Q, int32_t* idx_out, float* dist_out) {
+  return fg_dataset_nearest_sized(d, 32, queries, Q, idx_out, dist_out);
+}
+// the same against the size x size view of every image (DATASET.setScale(OPT.scale), then loadImages): queries
+// [Q][C][size][size]
+int fg_dataset_nearest_sized(fg_dataset* d, int size, const float* queries, int Q, int32_t* idx_out, float* dist_out) {
   ENTER(d);
-  return nearest_run(d->c, nullptr, d, d->N, d->c->C * 1024, queries, Q, idx_out, dist_out);
+  FG_REQUIRE(size >= 1 && size <= 64, "fg_dataset_nearest_sized: size %d outside [1, 64]", size);
+  return nearest_run(d->c, nullptr, d, size, d->N, d->c->C * size * size, queries, Q, idx_out, dist_out);
 }
 
 }  // extern "C"

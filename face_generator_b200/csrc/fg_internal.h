@@ -247,6 +247,7 @@ struct Net32;  // the 32x32 nets (nets.cu)
 
 // What every net on one device stream shares: the stream, the options, the data-parallel state and the workspaces of
 // the kernels.  Each net owns its own parameters, activations and layer scratch.
+struct JpegEncScratch;
 struct fg_ctx {
   int device = 0, maxB = 0, C = 3;
   cudaStream_t stream = nullptr;
@@ -283,6 +284,10 @@ struct fg_ctx {
   double* bn_acc = nullptr;  // [4][256] double accumulators (sum, sumsq / sum g, sum g xhat)
   float* io_dev = nullptr;  // device staging for NCHW images / misc
   size_t io_dev_elems = 0;
+  JpegEncScratch* jpeg_enc = nullptr;  // fg_jpeg_encode's chunk buffers (jpeg_enc.cu), made on first use
+  // option "jpeg_route" (tests only): the entropy coder of every JPEG encode on this ctx; 0 (default) = by the blocks
+  // per file, 1 = one CTA per file, 2 = many CTAs per file.  The bytes are the same.
+  int jpeg_route = 0;
   float* scratch[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   size_t scratch_elems[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   // data parallel

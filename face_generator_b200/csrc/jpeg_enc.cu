@@ -1,21 +1,32 @@
-// Baseline JPEG encode of the device-resident dataset (fg_dataset_encode_jpeg) and its round trip in place
-// (fg_dataset_jpeg_roundtrip).
+// Baseline JPEG encode of the device-resident dataset (fg_dataset_encode_jpeg), of caller images (fg_jpeg_encode), and
+// the dataset's round trip in place (fg_dataset_jpeg_roundtrip).
 //
-// Replaces dataset/generate_dataset.py's last step, misc.imsave(path, row): Pillow's Image.save at its defaults
-// (baseline JFIF 1.01, quality 75, YCbCr 4:2:0, standard Huffman tables, islow DCT, no restart markers), which every
-// file train.lua, train_c2f.lua and sample.lua read went through.  The arithmetic is k_jpeg_enc.cuh; the files equal
-// Pillow's byte for byte (tests/jpeg_enc_ref.py restates the rules, tests/test_gpu_jpeg_encode.py holds the kernels to
-// them).  A call runs in chunks of at most kChunkBlocks 8x8 blocks (at least one row), on the ctx stream:
-//   jpeg_fdct_kernel   one CTA per band of MCU rows (usually the whole row): colour conversion into shared memory,
+// Replaces dataset/generate_dataset.py's last step, misc.imsave(path, row), and image.save(path, grid) of sample.lua's
+// sheets: Pillow's Image.save at its defaults (baseline JFIF 1.01, quality 75, YCbCr 4:2:0, standard Huffman tables,
+// islow DCT, no restart markers), which every file train.lua, train_c2f.lua and sample.lua read or write went through.
+// The arithmetic is k_jpeg_enc.cuh; the files equal Pillow's byte for byte (tests/jpeg_enc_ref.py restates the rules,
+// tests/test_gpu_jpeg_encode.py and tests/test_gpu_sample_sheets.py hold the kernels to them).  A call runs in chunks
+// of at most kChunkBlocks 8x8 blocks (at least one image), on the ctx stream:
+//   jpeg_fdct_kernel   one CTA per band of MCU rows (usually the whole image): colour conversion into shared memory,
 //                      then one thread per block: edge expansion, 2x2 downsampling, forward DCT, quantisation, written
 //                      in the decoder's coefficient layout; then the dummy blocks
-//   jpeg_huff_kernel   one CTA per row: the bit length of every block (its DC predictor is already in the scratch),
-//                      a scan to bit offsets, every block's codes packed into the row's word buffer, the padding
-//                      1-bits, and the length after byte stuffing
-//   jpeg_stuff_kernel  one CTA per row: header, stuffed entropy bytes (0x00 after each 0xFF) and EOI at the file's
-//                      offset in the chunk's output, which goes to the host in one copy
+// then one of two entropy coders, chosen by the blocks per file (kMultiMinBlocks); both write the same bytes:
+//   one CTA per file (small files, many per chunk)
+//     jpeg_huff_kernel   the bit length of every block (its DC predictor is already in the scratch), a scan to bit
+//                        offsets, every block's codes packed into the file's word buffer, the padding 1-bits, and the
+//                        length after byte stuffing
+//     jpeg_stuff_kernel  header, stuffed entropy bytes (0x00 after each 0xFF) and EOI at the file's offset in the
+//                        chunk's output, which goes to the host in one copy
+//   many CTAs per file (large files, such as sample sheets: one file per chunk)
+//     jpeg_blen_kernel    kTileBlocks blocks per CTA: bit lengths, their scan within the tile, the tile's sum
+//     jpeg_scan_kernel    one CTA: exclusive scan of the tile sums -> tile bit offsets and the file's bit count
+//     jpeg_zero_kernel    zeroes the words the codes occupy
+//     jpeg_pack_kernel    kTileBlocks blocks per CTA: codes OR-ed into the words at their offsets, the padding 1-bits
+//     jpeg_ffcount_kernel kStuffSegs CTAs, one contiguous segment of words each: the 0xFF bytes of the segment
+//     jpeg_scan_kernel    the segments' 0xFF counts -> their shifts, and the stuffed byte count
+//     jpeg_scatter_kernel kStuffSegs CTAs: header, each segment's stuffed bytes at its shift, EOI
 // The sizes are known only once a chunk is coded, and nothing may be written to the caller's buffer unless every file
-// fits, so the encode codes the rows twice: once for the sizes (no stuffing, no copy), once to write (a call of one
+// fits, so the encode codes the images twice: once for the sizes (no stuffing, no copy), once to write (a call of one
 // chunk keeps its first pass).  The round trip runs jpeg_fdct_kernel and then the decoder's jpeg_idct_color_kernel on
 // the same coefficients: decode(encode(row)) without the entropy coding, which is lossless.
 #include <algorithm>
@@ -33,6 +44,13 @@ constexpr int64_t kChunkBlocks = 1 << 18;  // 32 MB of coefficients, 53 MB of wo
 constexpr int kBandBudget = 64 * 1024;     // shared memory a band of the forward kernel aims for; one MCU row may need more
 constexpr int kFdctThreads = 128, kHuffThreads = 128, kStuffThreads = 128;
 constexpr int kBlockWords = (jpg::kMaxBlockBits + 31) / 32;  // code words one block may need
+// Files of at least kMultiMinBlocks blocks are entropy-coded by many CTAs: one CTA of kHuffThreads would loop over
+// 16 or more blocks per thread, and a chunk holds at most a few dozen such files, so most SMs would idle (a 1024x1024
+// colour sheet has 24 576 blocks, 192 per thread).  Below it, files are small and a chunk holds many of them.
+constexpr int kMultiMinBlocks = 2048;
+constexpr int kTileBlocks = 128;  // blocks per CTA of jpeg_blen_kernel / jpeg_pack_kernel (one per thread)
+constexpr int kScanThreads = 1024;
+constexpr int kStuffSegs = 264;  // CTAs of jpeg_ffcount_kernel / jpeg_scatter_kernel: two per SM
 
 // ---- kernels ------------------------------------------------------------------------------------------------------
 // exclusive scan of v over the CTA (blockDim.x a multiple of 32, at most 1024); *total = the sum
@@ -262,6 +280,134 @@ __global__ void __launch_bounds__(kStuffThreads) jpeg_stuff_kernel(int nblk, con
   }
 }
 
+// ---- the multi-CTA coder of one file (the chunk's only image) ---------------------------------------------------------
+// kTileBlocks blocks per CTA: boff[s] = the bit offset of block s within its tile, tsum[tile] = the tile's bits
+__global__ void __launch_bounds__(kTileBlocks) jpeg_blen_kernel(const __grid_constant__ EncGeom g, const int16_t* __restrict__ coef,
+                                                                const uint32_t* __restrict__ codes, int* __restrict__ boff,
+                                                                int* __restrict__ tsum) {
+  __shared__ uint32_t s_codes[4][256];
+  for (int i = threadIdx.x; i < 4 * 256; i += blockDim.x) (&s_codes[0][0])[i] = codes[i];
+  __syncthreads();
+  const int s = blockIdx.x * kTileBlocks + threadIdx.x;
+  int len = 0;
+  if (s < g.nblk) {
+    int64_t off, prev;
+    const int comp = jpg::scan_block(g, s, &off, &prev);
+    jpg::BitCount bc;
+    jpg::huff_block(coef + off, prev < 0 ? 0 : coef[prev], s_codes[comp ? 2 : 0], s_codes[comp ? 3 : 1], bc);
+    len = bc.n;
+  }
+  int total;
+  const int ex = block_excl_scan(len, &total);
+  if (s < g.nblk) boff[s] = ex;
+  if (threadIdx.x == 0) tsum[blockIdx.x] = total;
+}
+
+// One CTA: v[0, n) replaced by its exclusive scan; *total = the sum, plus the whole bytes of *nbits bits when nbits is
+// given (the stuffed length: entropy bytes + one 0x00 per 0xFF)
+__global__ void __launch_bounds__(kScanThreads) jpeg_scan_kernel(int* __restrict__ v, int n, int* __restrict__ total,
+                                                                 const int* __restrict__ nbits) {
+  int carry = 0;
+  for (int t = 0; t < n; t += blockDim.x) {
+    const int i = t + threadIdx.x;
+    const int x = i < n ? v[i] : 0;
+    int sum;
+    const int ex = block_excl_scan(x, &sum);
+    if (i < n) v[i] = carry + ex;
+    carry += sum;
+  }
+  if (threadIdx.x == 0) *total = carry + (nbits ? (*nbits + 7) >> 3 : 0);
+}
+
+// the words the file's *nbits bits occupy, zeroed for jpeg_pack_kernel's OR-ing
+__global__ void jpeg_zero_kernel(const int* __restrict__ nbits, uint32_t* __restrict__ words) {
+  const int nw = (*nbits + 31) >> 5;
+  GRID_STRIDE(i, nw) words[i] = 0;
+}
+
+// kTileBlocks blocks per CTA: each block's codes at toff[tile] + boff[s], shared boundary words OR-ed atomically as
+// in jpeg_huff_kernel; the thread of the last block adds the padding 1-bits
+__global__ void __launch_bounds__(kTileBlocks) jpeg_pack_kernel(const __grid_constant__ EncGeom g, const int16_t* __restrict__ coef,
+                                                                const uint32_t* __restrict__ codes, const int* __restrict__ boff,
+                                                                const int* __restrict__ toff, const int* __restrict__ nbits,
+                                                                uint32_t* __restrict__ words) {
+  __shared__ uint32_t s_codes[4][256];
+  for (int i = threadIdx.x; i < 4 * 256; i += blockDim.x) (&s_codes[0][0])[i] = codes[i];
+  __syncthreads();
+  const int s = blockIdx.x * kTileBlocks + threadIdx.x;
+  if (s >= g.nblk) return;
+  int64_t off, prev;
+  const int comp = jpg::scan_block(g, s, &off, &prev);
+  WordSink ws(words, toff[blockIdx.x] + boff[s]);
+  jpg::huff_block(coef + off, prev < 0 ? 0 : coef[prev], s_codes[comp ? 2 : 0], s_codes[comp ? 3 : 1], ws);
+  ws.flush();
+  if (s == g.nblk - 1) {
+    const int T = *nbits, pad = ((T + 7) >> 3) * 8 - T;
+    if (pad) atomicOr(words + (T >> 5), ((1u << pad) - 1) << (32 - (T & 31) - pad));
+  }
+}
+
+// the words [w0, w1) of segment blockIdx.x of the file's entropy bytes (kStuffSegs equal segments)
+__device__ void stuff_segment(int nbytes, int* w0, int* w1) {
+  const int nw = (nbytes + 3) >> 2, per = (nw + gridDim.x - 1) / gridDim.x;
+  *w0 = min(nw, (int)blockIdx.x * per);
+  *w1 = min(nw, *w0 + per);
+}
+
+// sff[seg] = the 0xFF bytes among the entropy bytes of segment seg
+__global__ void __launch_bounds__(kStuffThreads) jpeg_ffcount_kernel(const uint32_t* __restrict__ words, const int* __restrict__ nbits,
+                                                                     int* __restrict__ sff) {
+  const int nbytes = (*nbits + 7) >> 3;
+  int w0, w1;
+  stuff_segment(nbytes, &w0, &w1);
+  int ff = 0;
+  for (int i = w0 + threadIdx.x; i < w1; i += blockDim.x) {
+    const uint32_t v = words[i];
+    for (int j = 0; j < 4 && 4 * i + j < nbytes; ++j) ff += ((v >> (24 - 8 * j)) & 0xff) == 0xff;
+  }
+  int total;
+  block_excl_scan(ff, &total);
+  if (threadIdx.x == 0) sff[blockIdx.x] = total;
+}
+
+// The file at out + off[0]: header (CTA 0), each segment's stuffed bytes shifted by the 0x00s of the segments before
+// it (soff[seg]), EOI after the *slen stuffed bytes
+__global__ void __launch_bounds__(kStuffThreads) jpeg_scatter_kernel(const uint32_t* __restrict__ words, const int* __restrict__ nbits,
+                                                                     const int* __restrict__ soff, const int* __restrict__ slen,
+                                                                     const uint8_t* __restrict__ hdr, int hdr_len,
+                                                                     const int64_t* __restrict__ off, uint8_t* __restrict__ out) {
+  uint8_t* dst = out + off[0];
+  if (blockIdx.x == 0)
+    for (int i = threadIdx.x; i < hdr_len; i += blockDim.x) dst[i] = hdr[i];
+  dst += hdr_len;
+  const int nbytes = (*nbits + 7) >> 3;
+  int w0, w1;
+  stuff_segment(nbytes, &w0, &w1);
+  int carry = soff[blockIdx.x];
+  for (int t = w0; t < w1; t += blockDim.x) {
+    const int i = t + threadIdx.x;
+    uint32_t v = 0;
+    int nb = 0, ff = 0;
+    if (i < w1) {
+      v = words[i];
+      nb = min(4, nbytes - 4 * i);
+      for (int j = 0; j < nb; ++j) ff += ((v >> (24 - 8 * j)) & 0xff) == 0xff;
+    }
+    int total;
+    int p = 4 * i + carry + block_excl_scan(ff, &total);
+    for (int j = 0; j < nb; ++j) {
+      const uint8_t b = (uint8_t)(v >> (24 - 8 * j));
+      dst[p++] = b;
+      if (b == 0xff) dst[p++] = 0;
+    }
+    carry += total;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    dst[*slen] = 0xff;
+    dst[*slen + 1] = 0xd9;
+  }
+}
+
 // ---- host side -----------------------------------------------------------------------------------------------------
 void put16(std::vector<uint8_t>& v, int x) {
   v.push_back((uint8_t)(x >> 8));
@@ -311,13 +457,13 @@ std::vector<uint8_t> jfif_header(const EncGeom& g) {
   return h;
 }
 
-EncGeom make_geom(const fg_dataset* d, int quality, int* smem) {
+EncGeom make_geom(int Cs, int H, int W, int quality, int* smem) {
   EncGeom g;
   memset(&g, 0, sizeof(g));
-  g.Cs = d->Cs;
-  g.H = d->Hs;
-  g.W = d->Ws;
-  g.hs = g.vs = d->Cs == 3 ? 2 : 1;
+  g.Cs = Cs;
+  g.H = H;
+  g.W = W;
+  g.hs = g.vs = Cs == 3 ? 2 : 1;
   g.mcux = (g.W + 8 * g.hs - 1) / (8 * g.hs);
   g.mcuy = (g.H + 8 * g.vs - 1) / (8 * g.vs);
   g.bwr = (g.W + 7) / 8;
@@ -356,7 +502,8 @@ int check_span(fg_dataset* d, const char* what, int64_t first, int64_t count, in
 
 }  // namespace
 
-// Chunk scratch of the encoder, grown to the largest chunk seen; freed with the dataset.
+// Chunk scratch of the encoder, grown to the largest chunk seen; freed with the dataset (fg_dataset_encode_jpeg,
+// fg_dataset_jpeg_roundtrip) or the ctx (fg_jpeg_encode).
 struct JpegEncScratch {
   int16_t* coef = nullptr;
   int64_t coef_cap = 0;
@@ -364,7 +511,7 @@ struct JpegEncScratch {
   int64_t words_cap = 0;
   int* boff = nullptr;
   int64_t boff_cap = 0;
-  int* lens = nullptr;  // [2][rows]: bit counts, stuffed byte counts
+  int* lens = nullptr;  // [2][images]: bit counts, stuffed byte counts
   int64_t lens_cap = 0;
   int* lens_host = nullptr;  // pinned mirror of the stuffed byte counts
   int64_t lens_host_cap = 0;
@@ -376,6 +523,10 @@ struct JpegEncScratch {
   int64_t consts_cap = 0;
   uint8_t* desc = nullptr;  // the round trip's ImageDesc / BandDesc arrays
   int64_t desc_cap = 0;
+  int* part = nullptr;  // the multi-CTA coder's tile sums, then its segment 0xFF counts
+  int64_t part_cap = 0;
+  uint8_t* src = nullptr;  // fg_jpeg_encode: the chunk's images when the caller's are in host memory
+  int64_t src_cap = 0;
 };
 
 void jpeg_enc_scratch_free(JpegEncScratch* s) {
@@ -389,28 +540,31 @@ void jpeg_enc_scratch_free(JpegEncScratch* s) {
   cudaFree(s->out);
   cudaFree(s->consts);
   cudaFree(s->desc);
+  cudaFree(s->part);
+  cudaFree(s->src);
   delete s;
 }
 
 namespace {
 
-// jpeg_fdct_kernel on rows [row0, row0 + n) into the coefficient scratch
-int run_fdct(fg_dataset* d, const EncGeom& g, int smem, int64_t row0, int n) {
-  fg_ctx* c = d->c;
-  JpegEncScratch& s = *d->jpeg_enc;
+// jpeg_fdct_kernel on n images at src (device, [n][Cs][H][W]) into the coefficient scratch
+int run_fdct(fg_ctx* c, JpegEncScratch& s, const EncGeom& g, int smem, const uint8_t* src, int n) {
   FG_TRY(dev_reserve(c, &s.coef, &s.coef_cap, (int64_t)n * g.nblk * 64));
   if (smem > 48 * 1024) FG_CUDA(cudaFuncSetAttribute(jpeg_fdct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  const int64_t per = (int64_t)g.Cs * g.H * g.W;
-  jpeg_fdct_kernel<<<n * g.bands, kFdctThreads, smem, c->stream>>>(g, d->data + row0 * per, s.coef);
+  jpeg_fdct_kernel<<<n * g.bands, kFdctThreads, smem, c->stream>>>(g, src, s.coef);
   LAUNCH_CHECK(c);
   return FG_OK;
 }
 
-// forward kernel and entropy coding of rows [row0, row0 + n): the stuffed byte count of each into s.lens_host
-int run_code(fg_dataset* d, const EncGeom& g, int smem, int64_t row0, int n) {
-  fg_ctx* c = d->c;
-  JpegEncScratch& s = *d->jpeg_enc;
-  FG_TRY(run_fdct(d, g, smem, row0, n));
+// the multi-CTA coder: one file per chunk
+bool multi_cta(const fg_ctx* c, const EncGeom& g) {
+  return c->jpeg_route == 2 || (c->jpeg_route == 0 && g.nblk >= kMultiMinBlocks);
+}
+
+// forward kernel and entropy coding of n images at src: the bit and stuffed byte counts in s.lens, the stuffed byte
+// count of each also in s.lens_host
+int run_code(fg_ctx* c, JpegEncScratch& s, const EncGeom& g, int smem, const uint8_t* src, int n) {
+  FG_TRY(run_fdct(c, s, g, smem, src, n));
   FG_TRY(dev_reserve(c, &s.words, &s.words_cap, (int64_t)n * g.nblk * kBlockWords));
   FG_TRY(dev_reserve(c, &s.boff, &s.boff_cap, (int64_t)n * g.nblk));
   FG_TRY(dev_reserve(c, &s.lens, &s.lens_cap, 2 * (int64_t)n));
@@ -421,11 +575,95 @@ int run_code(fg_dataset* d, const EncGeom& g, int smem, int64_t row0, int n) {
     FG_CUDA(cudaHostAlloc((void**)&s.lens_host, sizeof(int) * (size_t)n, cudaHostAllocDefault));
     s.lens_host_cap = n;
   }
-  jpeg_huff_kernel<<<n, kHuffThreads, 0, c->stream>>>(g, s.coef, reinterpret_cast<const uint32_t*>(s.consts), s.words, s.boff,
-                                                       s.lens, s.lens + n);
-  LAUNCH_CHECK(c);
+  const uint32_t* codes = reinterpret_cast<const uint32_t*>(s.consts);
+  if (multi_cta(c, g)) {
+    const int tiles = (g.nblk + kTileBlocks - 1) / kTileBlocks;
+    FG_TRY(dev_reserve(c, &s.part, &s.part_cap, (int64_t)std::max(tiles, kStuffSegs)));
+    jpeg_blen_kernel<<<tiles, kTileBlocks, 0, c->stream>>>(g, s.coef, codes, s.boff, s.part);
+    LAUNCH_CHECK(c);
+    jpeg_scan_kernel<<<1, kScanThreads, 0, c->stream>>>(s.part, tiles, s.lens, nullptr);
+    LAUNCH_CHECK(c);
+    jpeg_zero_kernel<<<grid_for((int64_t)g.nblk * kBlockWords, 256, c->sm_count * 4), 256, 0, c->stream>>>(s.lens, s.words);
+    LAUNCH_CHECK(c);
+    jpeg_pack_kernel<<<tiles, kTileBlocks, 0, c->stream>>>(g, s.coef, codes, s.boff, s.part, s.lens, s.words);
+    LAUNCH_CHECK(c);
+    jpeg_ffcount_kernel<<<kStuffSegs, kStuffThreads, 0, c->stream>>>(s.words, s.lens, s.part);
+    LAUNCH_CHECK(c);
+    jpeg_scan_kernel<<<1, kScanThreads, 0, c->stream>>>(s.part, kStuffSegs, s.lens + 1, s.lens);
+    LAUNCH_CHECK(c);
+  } else {
+    jpeg_huff_kernel<<<n, kHuffThreads, 0, c->stream>>>(g, s.coef, codes, s.words, s.boff, s.lens, s.lens + n);
+    LAUNCH_CHECK(c);
+  }
   FG_CUDA(cudaMemcpyAsync(s.lens_host, s.lens + n, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
   FG_CUDA(cudaStreamSynchronize(c->stream));
+  return FG_OK;
+}
+
+// The JFIF files of `count` images, each [Cs][H][W]: image i at images + i * Cs*H*W, device memory, or host memory
+// staged a chunk at a time.  offsets / out / cap as fg_dataset_encode_jpeg.
+int encode_files(fg_ctx* c, JpegEncScratch& s, const char* what, const uint8_t* images, bool host, int64_t count, int Cs,
+                 int H, int W, int quality, uint8_t* out, int64_t cap, int64_t* offsets) {
+  int smem;
+  const EncGeom g = make_geom(Cs, H, W, quality, &smem);
+  const int64_t per = (int64_t)Cs * H * W;
+  const std::vector<uint8_t> hdr = jfif_header(g);
+  std::vector<uint8_t> consts(4 * 256 * sizeof(uint32_t) + hdr.size());
+  for (int t = 0; t < 4; ++t) jpg::huff_codes(t, reinterpret_cast<uint32_t*>(consts.data()) + 256 * t);
+  memcpy(consts.data() + 4 * 256 * sizeof(uint32_t), hdr.data(), hdr.size());
+  FG_TRY(dev_reserve(c, &s.consts, &s.consts_cap, (int64_t)consts.size()));
+  FG_CUDA(cudaMemcpyAsync(s.consts, consts.data(), consts.size(), cudaMemcpyHostToDevice, c->stream));
+  const uint8_t* hdr_dev = s.consts + 4 * 256 * sizeof(uint32_t);
+  const int64_t fixed = (int64_t)hdr.size() + 2;  // header + EOI
+  const bool multi = multi_cta(c, g);
+  const int chunk = multi ? 1 : (int)std::max<int64_t>(1, std::min<int64_t>(count, kChunkBlocks / g.nblk));
+  // the chunk's images on the device
+  auto chunk_src = [&](int64_t i, int n, const uint8_t** src) -> int {
+    *src = images + i * per;
+    if (!host) return FG_OK;
+    FG_TRY(dev_reserve(c, &s.src, &s.src_cap, n * per));
+    FG_CUDA(cudaMemcpyAsync(s.src, *src, (size_t)(n * per), cudaMemcpyHostToDevice, c->stream));
+    *src = s.src;
+    return FG_OK;
+  };
+
+  // pass 1: every file's size
+  offsets[0] = 0;
+  for (int64_t i = 0; i < count; i += chunk) {
+    const int n = (int)std::min<int64_t>(chunk, count - i);
+    const uint8_t* src;
+    FG_TRY(chunk_src(i, n, &src));
+    FG_TRY(run_code(c, s, g, smem, src, n));
+    for (int k = 0; k < n; ++k) offsets[i + k + 1] = offsets[i + k] + fixed + s.lens_host[k];
+  }
+  if (!out) return FG_OK;
+  if (offsets[count] > cap) {
+    fg_set_error("%s: the files take %lld bytes, the buffer holds %lld", what, (long long)offsets[count], (long long)cap);
+    return FG_ERR_INVALID;
+  }
+  // pass 2: the files (a single chunk is still coded from pass 1)
+  std::vector<int64_t> off(chunk);
+  for (int64_t i = 0; i < count; i += chunk) {
+    const int n = (int)std::min<int64_t>(chunk, count - i);
+    if (count > chunk) {
+      const uint8_t* src;
+      FG_TRY(chunk_src(i, n, &src));
+      FG_TRY(run_code(c, s, g, smem, src, n));
+    }
+    for (int k = 0; k < n; ++k) off[k] = offsets[i + k] - offsets[i];
+    const int64_t bytes = offsets[i + n] - offsets[i];
+    FG_TRY(dev_reserve(c, &s.off, &s.off_cap, (int64_t)n));
+    FG_TRY(dev_reserve(c, &s.out, &s.out_cap, bytes));
+    FG_CUDA(cudaMemcpyAsync(s.off, off.data(), sizeof(int64_t) * n, cudaMemcpyHostToDevice, c->stream));
+    if (multi)
+      jpeg_scatter_kernel<<<kStuffSegs, kStuffThreads, 0, c->stream>>>(s.words, s.lens, s.part, s.lens + 1, hdr_dev,
+                                                                     (int)hdr.size(), s.off, s.out);
+    else
+      jpeg_stuff_kernel<<<n, kStuffThreads, 0, c->stream>>>(g.nblk, s.words, s.lens, hdr_dev, (int)hdr.size(), s.off, s.out);
+    LAUNCH_CHECK(c);
+    FG_CUDA(cudaMemcpyAsync(out + offsets[i], s.out, (size_t)bytes, cudaMemcpyDefault, c->stream));
+    FG_CUDA(cudaStreamSynchronize(c->stream));
+  }
   return FG_OK;
 }
 
@@ -441,48 +679,26 @@ int fg_dataset_encode_jpeg(fg_dataset* d, int64_t first, int64_t count, int qual
   fg_ctx* c = d->c;
   FG_CUDA(cudaSetDevice(c->device));
   if (!d->jpeg_enc) d->jpeg_enc = new JpegEncScratch();
-  JpegEncScratch& s = *d->jpeg_enc;
-  int smem;
-  const EncGeom g = make_geom(d, quality, &smem);
-  const std::vector<uint8_t> hdr = jfif_header(g);
-  std::vector<uint8_t> consts(4 * 256 * sizeof(uint32_t) + hdr.size());
-  for (int t = 0; t < 4; ++t) jpg::huff_codes(t, reinterpret_cast<uint32_t*>(consts.data()) + 256 * t);
-  memcpy(consts.data() + 4 * 256 * sizeof(uint32_t), hdr.data(), hdr.size());
-  FG_TRY(dev_reserve(c, &s.consts, &s.consts_cap, (int64_t)consts.size()));
-  FG_CUDA(cudaMemcpyAsync(s.consts, consts.data(), consts.size(), cudaMemcpyHostToDevice, c->stream));
-  const uint8_t* hdr_dev = s.consts + 4 * 256 * sizeof(uint32_t);
-  const int64_t fixed = (int64_t)hdr.size() + 2;  // header + EOI
-  const int chunk = (int)std::max<int64_t>(1, std::min<int64_t>(count, kChunkBlocks / g.nblk));
+  const int64_t per = (int64_t)d->Cs * d->Hs * d->Ws;
+  return encode_files(c, *d->jpeg_enc, "fg_dataset_encode_jpeg", d->data + first * per, false, count, d->Cs, d->Hs, d->Ws,
+                      quality, out, cap, offsets);
+}
 
-  // pass 1: every file's size
-  offsets[0] = 0;
-  for (int64_t i = 0; i < count; i += chunk) {
-    const int n = (int)std::min<int64_t>(chunk, count - i);
-    FG_TRY(run_code(d, g, smem, first + i, n));
-    for (int k = 0; k < n; ++k) offsets[i + k + 1] = offsets[i + k] + fixed + s.lens_host[k];
-  }
-  if (!out) return FG_OK;
-  if (offsets[count] > cap) {
-    fg_set_error("fg_dataset_encode_jpeg: the files take %lld bytes, the buffer holds %lld", (long long)offsets[count],
-                 (long long)cap);
+int fg_jpeg_encode(fg_ctx* c, const uint8_t* images, int count, int C, int H, int W, int quality, uint8_t* out, int64_t cap,
+                   int64_t* offsets) {
+  if (!c) {
+    fg_set_error("null fg_ctx");
     return FG_ERR_INVALID;
   }
-  // pass 2: the files (a single chunk is still coded from pass 1)
-  std::vector<int64_t> off(chunk);
-  for (int64_t i = 0; i < count; i += chunk) {
-    const int n = (int)std::min<int64_t>(chunk, count - i);
-    if (count > chunk) FG_TRY(run_code(d, g, smem, first + i, n));
-    for (int k = 0; k < n; ++k) off[k] = offsets[i + k] - offsets[i];
-    const int64_t bytes = offsets[i + n] - offsets[i];
-    FG_TRY(dev_reserve(c, &s.off, &s.off_cap, (int64_t)n));
-    FG_TRY(dev_reserve(c, &s.out, &s.out_cap, bytes));
-    FG_CUDA(cudaMemcpyAsync(s.off, off.data(), sizeof(int64_t) * n, cudaMemcpyHostToDevice, c->stream));
-    jpeg_stuff_kernel<<<n, kStuffThreads, 0, c->stream>>>(g.nblk, s.words, s.lens, hdr_dev, (int)hdr.size(), s.off, s.out);
-    LAUNCH_CHECK(c);
-    FG_CUDA(cudaMemcpyAsync(out + offsets[i], s.out, (size_t)bytes, cudaMemcpyDefault, c->stream));
-    FG_CUDA(cudaStreamSynchronize(c->stream));
-  }
-  return FG_OK;
+  FG_REQUIRE(images && offsets && count >= 1, "fg_jpeg_encode: need images, offsets and count >= 1");
+  FG_REQUIRE(C == 1 || C == 3, "fg_jpeg_encode: %d channels (1 or 3)", C);
+  FG_REQUIRE(H >= 1 && W >= 1 && H <= 4096 && W <= 4096, "fg_jpeg_encode: size %dx%d outside [1, 4096]", H, W);
+  FG_REQUIRE(quality >= 1 && quality <= 100, "fg_jpeg_encode: quality %d outside 1..100", quality);
+  FG_REQUIRE(!out || cap >= 0, "fg_jpeg_encode: negative capacity");
+  FG_CUDA(cudaSetDevice(c->device));
+  if (!c->jpeg_enc) c->jpeg_enc = new JpegEncScratch();
+  return encode_files(c, *c->jpeg_enc, "fg_jpeg_encode", images, !fg_is_dev(images), count, C, H, W, quality, out, cap,
+                      offsets);
 }
 
 int fg_dataset_jpeg_roundtrip(fg_dataset* d, int64_t first, int64_t count, int quality) {
@@ -492,7 +708,7 @@ int fg_dataset_jpeg_roundtrip(fg_dataset* d, int64_t first, int64_t count, int q
   if (!d->jpeg_enc) d->jpeg_enc = new JpegEncScratch();
   JpegEncScratch& s = *d->jpeg_enc;
   int smem;
-  const EncGeom g = make_geom(d, quality, &smem);
+  const EncGeom g = make_geom(d->Cs, d->Hs, d->Ws, quality, &smem);
   // the decoder's view of one file: its quantisation tables (the Huffman tables are not read by the IDCT kernel)
   jpg::TableSet ts;
   memset(&ts, 0, sizeof(ts));
@@ -522,7 +738,7 @@ int fg_dataset_jpeg_roundtrip(fg_dataset* d, int64_t first, int64_t count, int q
   FG_TRY(dev_reserve(c, &s.desc, &s.desc_cap, (int64_t)(o_band + sizeof(jpg::BandDesc) * bds.size())));
   for (int64_t i = 0; i < count; i += chunk) {
     const int n = (int)std::min<int64_t>(chunk, count - i);
-    FG_TRY(run_fdct(d, g, smem, first + i, n));
+    FG_TRY(run_fdct(c, s, g, smem, d->data + (first + i) * per, n));
     for (int k = 0; k < n; ++k) {
       imgs[k] = m;
       imgs[k].coef = (int64_t)k * g.nblk * 64;

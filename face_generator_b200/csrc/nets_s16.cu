@@ -444,6 +444,19 @@ int fg_s16_D_forward(fg_s16* n, const float* img, int B, int training, const flo
   FG_REQUIRE(img && B >= 1 && B <= n->c->maxB, "fg_s16_D_forward: bad arguments (batch %d, max %d)", B, n->c->maxB);
   return gan_D_forward(*n, img, B, training != 0, masks, seed, out);
 }
+// fg_D_score on D16_d: predictions for N 16x16 images in chunks of `chunk`, dropout masks of chunk s drawn from
+// seed + s when training (sample.lua --scale 16 never calls evaluate())
+int fg_s16_D_score(fg_s16* n, const float* images, int64_t N, int chunk, int training, uint64_t seed, float* preds_out) {
+  ENTER(n);
+  FG_REQUIRE(images && preds_out && N >= 1 && chunk >= 1 && chunk <= n->c->maxB, "fg_s16_D_score: bad arguments (chunk %d, max %d)",
+             chunk, n->c->maxB);
+  const size_t img = (size_t)n->c->C * 256;
+  for (int64_t s = 0; s < N; s += chunk) {
+    const int b = (int)std::min<int64_t>(chunk, N - s);
+    FG_TRY(fg_s16_D_forward(n, images + (size_t)s * img, b, training, nullptr, seed + (uint64_t)s, preds_out + s));
+  }
+  return FG_OK;
+}
 int fg_s16_D_backward(fg_s16* n, const float* d_out, int want_wgrad, float* d_img) {
   ENTER(n);
   FG_REQUIRE(d_out, "fg_s16_D_backward: null gradient");

@@ -136,6 +136,8 @@ SYMBOLS = {
     "fg_dataset_upload_jpeg": (_I, [_P, _L, _L, _P, _P, C.POINTER(_L)]),
     "fg_dataset_encode_jpeg": (_I, [_P, _L, _L, _I, _P, _L, _P]),
     "fg_dataset_jpeg_roundtrip": (_I, [_P, _L, _L, _I]),
+    "fg_jpeg_encode": (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _L, _P]),
+    "fg_image_grid": (_I, [_P, _P, _L, _I, _I, _I, _P, _I, _I, _I, _P, _P, _P]),
     "fg_lfw_aug_params": (_I, [_U64, _L, _L, _I, _I, _I, _P]),
     "fg_dataset_augment": (_I, [_P, _P, _L, _P, _L]),
     "fg_dataset_gather": (_I, [_P, _P, _I, _P]),
@@ -150,6 +152,8 @@ SYMBOLS = {
     "fg_D_score": (_I, [_P, _P, _L, _I, _I, _U64, _P]),
     "fg_nearest": (_I, [_P, _P, _I, _P, _L, _I, _P, _P]),
     "fg_dataset_nearest": (_I, [_P, _P, _I, _P, _P]),
+    "fg_dataset_nearest_sized": (_I, [_P, _I, _P, _I, _P, _P]),
+    "fg_s16_D_score": (_I, [_P, _P, _L, _I, _I, _U64, _P]),
     "fg_c2f_parzen_dist": (_I, [_P, _P, _P, _P, _I, _P]),
     "fg_image_scale": (_I, [_P, _P, _L, _I, _I, _I, _I, _I, _P]),
     "fg_c2f_refine": (_I, [_P, _P, _L, _I, _I, _I, _I, _P, _P, _U64, _P, _P, _P]),

@@ -103,6 +103,8 @@ int fg_dataset_download(fg_dataset* d, int64_t first, int64_t count, uint8_t* ou
 int fg_jpeg_info(const uint8_t* bytes, int64_t len, int* C, int* H, int* W);
 int fg_dataset_upload_jpeg(fg_dataset* d, int64_t first, int64_t count, const uint8_t* bytes, const int64_t* offsets, int64_t* failed_out);
 int fg_dataset_encode_jpeg(fg_dataset* d, int64_t first, int64_t count, int quality, uint8_t* out, int64_t cap, int64_t* offsets);
+int fg_jpeg_encode(fg_ctx* ctx, const uint8_t* images, int count, int C, int H, int W, int quality, uint8_t* out, int64_t cap, int64_t* offsets);
+int fg_image_grid(fg_ctx* ctx, const float* images, int64_t N, int C, int H, int W, const int32_t* order, int count, int nrow, int padding, uint8_t* out, int* Hg_out, int* Wg_out);
 int fg_dataset_jpeg_roundtrip(fg_dataset* d, int64_t first, int64_t count, int quality);
 typedef struct fg_aug { int64_t src; int32_t warp, hflip; double brightness; double m[9]; } fg_aug;
 int fg_lfw_aug_params(uint64_t seed, int64_t first_src, int64_t n_src, int n_aug, int src_h, int src_w, fg_aug* out);
@@ -118,6 +120,7 @@ int fg_dataset_gather_c2f_sized(fg_dataset* d, const int32_t* idx, int B, int fi
 int fg_D_score(fg_ctx* ctx, const float* images, int64_t N, int chunk, int training, uint64_t seed, float* preds_out);
 int fg_nearest(fg_ctx* ctx, const float* queries, int Q, const float* cands, int64_t N, int D, int32_t* idx_out, float* dist_out);
 int fg_dataset_nearest(fg_dataset* d, const float* queries, int Q, int32_t* idx_out, float* dist_out);
+int fg_dataset_nearest_sized(fg_dataset* d, int size, const float* queries, int Q, int32_t* idx_out, float* dist_out);
 int fg_c2f_parzen_dist(fg_c2f* n, const float* noise, const float* coarse, const float* fine, int K, float* dist_out);
 int fg_image_scale(fg_ctx* ctx, const float* src, int64_t N, int C, int Hs, int Ws, int Ho, int Wo, float* dst);
 int fg_c2f_refine(fg_c2f* n, const float* images, int64_t N, int in_size, int tries, int chunk, int training,
@@ -163,6 +166,7 @@ int fg_s16_G_forward(fg_s16* n, const float* noise, int B, int training, float* 
 int fg_s16_G_backward(fg_s16* n, const float* d_img, float* d_noise);
 int fg_s16_D_forward(fg_s16* n, const float* img, int B, int training, const float* masks, uint64_t seed, float* out);
 int fg_s16_D_backward(fg_s16* n, const float* d_out, int want_wgrad, float* d_img);
+int fg_s16_D_score(fg_s16* n, const float* images, int64_t N, int chunk, int training, uint64_t seed, float* preds_out);
 int fg_s16_train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const float* noise_D, const float* noise_G,
                       const float* masks_D, const float* masks_G, uint64_t seed, fg_step_stats* stats);
 int fg_s16_train_step_dataset(fg_s16* n, fg_dataset* d, const fg_hyper* h, int B, uint64_t seed, fg_step_stats* stats);

@@ -367,6 +367,26 @@ int fg_dataset_upload_jpeg(fg_dataset* d, int64_t first, int64_t count, const ui
 int fg_dataset_encode_jpeg(fg_dataset* d, int64_t first, int64_t count, int quality, uint8_t* out, int64_t cap,
                            int64_t* offsets);
 int fg_dataset_jpeg_roundtrip(fg_dataset* d, int64_t first, int64_t count, int quality);
+/* The same encoder on caller images (image.save(path, img) of sample.lua's sheets): count images
+ * planar uint8 [count][C][H][W] (host or device), C = 1 or 3, 1 <= H, W <= 4096, quality 1..100 ->
+ * baseline JFIF files byte for byte what Pillow's Image.save(f, "JPEG", quality=quality) writes
+ * (4:2:0 colour, grayscale for C = 1).  offsets / cap / out: fg_dataset_encode_jpeg's contract.
+ * Bad arguments are FG_ERR_INVALID and launch nothing.  Files of 2048 blocks or more (about 256x256
+ * colour) are entropy-coded by many CTAs each, smaller ones by one CTA each; fg_set_option(ctx,
+ * "jpeg_route", 1 | 2) forces one route for every encode on the ctx (tests only: same bytes).      */
+int fg_jpeg_encode(fg_ctx* ctx, const uint8_t* images, int count, int C, int H, int W, int quality, uint8_t* out,
+                   int64_t cap, int64_t* offsets);
+/* image.toDisplayTensor{input=images[order[0..count)], nrow=nrow, padding=padding} followed by
+ * image.saveJPG's clampImage (saturate to [0,1], *255, to bytes): planar uint8 [C][Hg][Wg] with
+ * Hg = ceil(count / xmaps) * (H + padding), Wg = xmaps * (W + padding), xmaps = min(nrow, count).
+ * images [N][C][H][W] float, host or device; order int32 [count] (host or device, NULL = 0..count-1;
+ * host entries are range-checked, device ones clamped to [0, N)); out host or device, or NULL to ask
+ * for Hg / Wg only (Hg_out / Wg_out may be NULL).  Cells outside an image hold the largest value of
+ * the selected images; the grid is then normalised by image.minmax over those images.  NaN values
+ * take no part in the minimum and maximum and give byte 0.  1 <= C <= 3, padding even and >= 0,
+ * Hg, Wg <= 4096, nrow >= 1; anything else is FG_ERR_INVALID and launches nothing.               */
+int fg_image_grid(fg_ctx* ctx, const float* images, int64_t N, int C, int H, int W, const int32_t* order, int count,
+                  int nrow, int padding, uint8_t* out, int* Hg_out, int* Wg_out);
 /* The augmented LFW training set (dataset/generate_dataset.py + ImageAugmenter.py): each output row
  * is LFW-crop's 84x84 box (rows 92..175, cols 83..166) of a source row, resized to the destination's
  * Ho x Wo as Pillow's Image.resize(BILINEAR) does (scipy.misc.imresize).  A descriptor with warp = 1
@@ -482,6 +502,12 @@ int fg_nearest(fg_ctx* ctx, const float* queries, int Q, const float* cands, int
                float* dist_out);
 /* findClosestNeighboursOf (sample.lua:141-159) against the device-resident training set            */
 int fg_dataset_nearest(fg_dataset* d, const float* queries, int Q, int32_t* idx_out, float* dist_out);
+/* the same against the size x size view of every cached image (1 <= size <= 64; DATASET.setScale
+ * then loadImages: fg_dataset_gather_sized's arithmetic), queries [Q][C][size][size];
+ * fg_dataset_nearest is fg_dataset_nearest_sized(d, 32, ...)                                         */
+int fg_dataset_nearest_sized(fg_dataset* d, int size, const float* queries, int Q, int32_t* idx_out, float* dist_out);
+/* fg_D_score on the --scale 16 discriminator: images [N][C][16][16], same chunking and seeds        */
+int fg_s16_D_score(fg_s16* n, const float* images, int64_t N, int chunk, int training, uint64_t seed, float* preds_out);
 /* one sample of adversarial_c2f.lua:305-325 approxParzen: min_k || G({noise_k, coarse}) + coarse - fine ||,
  * noise [K][1][S][S], coarse / fine [C][S][S]                                                       */
 int fg_c2f_parzen_dist(fg_c2f* n, const float* noise, const float* coarse, const float* fine, int K, float* dist_out);
