@@ -10,7 +10,7 @@ import ctypes as C
 
 import numpy as np
 
-from .lib import FGError, NET_D, NET_G, load_library
+from .lib import FGError, NET_D, NET_G, disc_param_count, load_library
 
 KINDS = {0: "nil", 1: "number", 2: "string", 3: "table", 4: "object", 5: "boolean", 6: "function", 16: "tensor",
          17: "storage", -1: None}
@@ -121,9 +121,60 @@ class T7Writer:
                 _err("fg_t7_writer_close")
 
 
+# models.lua's discriminators as module lists (nn.Module class names, containers with their children in braces), one
+# letter per leaf: C SpatialConvolution, P PReLU, M SpatialMaxPooling, A SpatialAveragePooling, S SpatialDropout,
+# V View, L Linear, D Dropout, J JoinTable, G Sigmoid
+_LEAF = dict(C="nn.SpatialConvolution", P="nn.PReLU", M="nn.SpatialMaxPooling", A="nn.SpatialAveragePooling",
+             S="nn.SpatialDropout", V="nn.View", L="nn.Linear", D="nn.Dropout", J="nn.JoinTable", G="nn.Sigmoid")
+_DENSE = "VLPDLP"
+_DISC_TREES = {  # (branches of the ConcatTable or None, modules of the Sequential after it)
+    "create_D32b": (None, "CPSA" * 4 + "VLPDLPDLG"),
+    "create_D16_d": (["CPCPACPCPSVLP", "VLPDLP"], "JLG"),
+    "create_D32": (["CPCPMSVLP", "CPCPMCPCPMSVLPDLP", _DENSE], "JLPDLG"),
+    "create_D16": (["CPCPMSVLPD", "CPCPMSVLPD", _DENSE], "JLPDLG"),
+    "create_D16_b": (["CPCPCPCPSVLPD", "CPCPCPCPSVLPD", _DENSE], "JLPDLG"),
+    "create_D16_c": (["CPCPCPCPCPSVLP", "CPCPCPCPCPSVLP", _DENSE], "JLPDLG"),
+}
+
+
+def disc_module_list(name):
+    """the fg_t7_net_describe skeleton of models.lua's discriminator `name` (without the CUDA-mode Copy wrapper)"""
+    branches, tail = _DISC_TREES[name]
+    seq = lambda letters: "nn.Sequential{%s}" % ",".join(_LEAF[c] for c in letters)
+    mods = ([] if branches is None else ["nn.ConcatTable{%s}" % ",".join(seq(b) for b in branches)])
+    return "nn.Sequential{%s}" % ",".join(mods + [_LEAF[c] for c in tail])
+
+
+def recognise_disc(describe):
+    """the models.lua discriminator whose module list `describe` (fg_t7_net_describe) is, or None.  The CUDA-mode
+    wrapper nn.Sequential{nn.Copy, net, nn.Copy} (utils/nn_utils.lua:328-363) and cudnn.* classes are accepted."""
+    d = describe.replace("cudnn.", "nn.")
+    pre, post = "nn.Sequential{nn.Copy,", ",nn.Copy}"
+    if d.startswith(pre) and d.endswith(post):
+        d = d[len(pre):-len(post)]
+    for name in _DISC_TREES:
+        if d == disc_module_list(name):
+            return name
+    return None
+
+
+def _check_disc(f, want, channels, what):
+    """D of checkpoint f against the net's discriminator `want`: a recognised other D is refused naming both; any D
+    whose length is not `want`'s is refused"""
+    desc = f.net_describe("D")
+    have = recognise_disc(desc)
+    if have is not None and have != want:
+        raise FGError("checkpoint D is %s; %s has %s" % (have, what, want))
+    pd = f.net_params("D")
+    n = disc_param_count(want, channels)
+    if pd.size != n:
+        raise FGError("checkpoint D has %d parameters (%s); %s has %s with %d" % (pd.size, desc, what, want, n))
+    return pd
+
+
 def load_reference_checkpoint(ctx, path, want_D=True):
     """sample.lua:247-258 `loadModels`: upload G (and D) of a reference `adversarial.net` into a Context.
-    Raises if the stored nets are not the default 32x32 architectures this library implements."""
+    Raises if G is not the 32x32 generator or D is not the discriminator the Context was created with."""
     with T7File(path) as f:
         pg = f.net_params("G")
         if pg.size != ctx.count(NET_G):
@@ -143,11 +194,7 @@ def load_reference_checkpoint(ctx, path, want_D=True):
             warnings.warn("checkpoint G holds no BatchNorm running statistics: evaluate()-mode forwards will use the "
                           "context's current ones (training-mode forwards, incl. sample.lua's, are unaffected)")
         if want_D and f.kind("D") is not None:
-            pd = f.net_params("D")
-            if pd.size != ctx.count(NET_D):
-                raise FGError("checkpoint D has %d parameters (%s); this build implements create_D32b with %d"
-                              % (pd.size, f.net_describe("D"), ctx.count(NET_D)))
-            ctx.set_params(NET_D, pd)
+            ctx.set_params(NET_D, _check_disc(f, ctx.discriminator, ctx.C, "this 32x32 net"))
         return int(f.number("epoch")) if f.kind("epoch") == "number" else None
 
 
@@ -190,12 +237,12 @@ def load_c2f_checkpoint(net, path):
     return ck["epoch"]
 
 
-def read_s16_checkpoint(path, channels):
-    """an `adversarial.net` trained with train.lua --scale 16 (create_G_decoder_upsampling16 / create_D16_d) as flat
-    vectors: dict(PG, bn, PD, epoch); bn = G's 768 BatchNorm running statistics, PD None when the file has no D.
-    Needs no GPU."""
+def read_s16_checkpoint(path, channels, discriminator="create_D16_d"):
+    """an `adversarial.net` trained with train.lua --scale 16 (create_G_decoder_upsampling16 and `discriminator`:
+    create_D16_d, or create_D16 / _b / _c) as flat vectors: dict(PG, bn, PD, epoch); bn = G's 768 BatchNorm running
+    statistics, PD None when the file has no D.  Needs no GPU."""
     lib = load_library()
-    nG, nD = int(lib.fg_s16_param_count(NET_G, channels)), int(lib.fg_s16_param_count(NET_D, channels))
+    nG = int(lib.fg_s16_param_count(NET_G, channels))
     with T7File(path) as f:
         pg = f.net_params("G")
         if pg.size != nG:
@@ -207,10 +254,7 @@ def read_s16_checkpoint(path, channels):
                           % bn.size)
         pd = None
         if f.kind("D") is not None:
-            pd = f.net_params("D")
-            if pd.size != nD:
-                raise FGError("checkpoint D has %d parameters (%s); the --scale 16 D with %d channels has %d"
-                              % (pd.size, f.net_describe("D"), channels, nD))
+            pd = _check_disc(f, discriminator, channels, "the --scale 16 D with %d channels" % channels)
         epoch = int(f.number("epoch")) if f.kind("epoch") == "number" else None
     return dict(PG=pg, bn=bn, PD=pd, epoch=epoch)
 
@@ -218,7 +262,7 @@ def read_s16_checkpoint(path, channels):
 def load_s16_checkpoint(net, path):
     """load G (with its BatchNorm running statistics) and, when present, D of a --scale 16 `adversarial.net` into an
     S16; returns the epoch (None when the file has none)"""
-    ck = read_s16_checkpoint(path, net.C)
+    ck = read_s16_checkpoint(path, net.C, net.discriminator)
     net.set_params(NET_G, ck["PG"])
     net.set_bn_state(ck["bn"])
     if ck["PD"] is not None:

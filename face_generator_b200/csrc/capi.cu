@@ -8,6 +8,7 @@
 
 #include "fg_internal.h"
 #include "k_conv_tc.h"
+#include "ups_gan.h"
 
 static thread_local char g_err[1024] = "";
 void fg_set_error(const char* fmt, ...) {
@@ -125,8 +126,35 @@ void fg_hyper_default(fg_hyper* h) {
 }
 
 int fg_create(fg_ctx** out, int device, int max_batch, int channels) {
+  return fg_create_disc(out, device, max_batch, channels, FG_DISC_D32B);
+}
+
+int64_t fg_disc_param_count(int disc, int channels) {
+  if (channels != 1 && channels != 3) return -1;
+  if (disc == FG_DISC_D32B) return fg_param_count(FG_NET_D, channels);
+  if (disc == FG_DISC_D16_D) return fg_s16_param_count(FG_NET_D, channels);
+  return dbr_param_count(disc, channels);
+}
+int fg_disc_mask_per_sample(int disc) {
+  if (disc == FG_DISC_D32B) return kMaskPerSample;
+  if (disc == FG_DISC_D16_D) return fg_s16_mask_per_sample();
+  return dbr_mask_per_sample(disc);
+}
+int fg_disc_side(int disc) {
+  if (disc == FG_DISC_D32B) return 32;
+  if (disc == FG_DISC_D16_D) return 16;
+  return dbr_side(disc);
+}
+
+int fg_create_disc(fg_ctx** out, int device, int max_batch, int channels, int disc) {
   if (!out) { fg_set_error("fg_create: out is null"); return FG_ERR_INVALID; }
   *out = nullptr;
+  if (disc == FG_DISC_DEFAULT) disc = FG_DISC_D32B;
+  FG_REQUIRE(fg_disc_side(disc), "fg_create_disc: unknown discriminator %d", disc);
+  if (fg_disc_side(disc) != 32) {
+    fg_set_error("fg_create_disc: discriminator %d is a 16x16 net; the 32x32 nets take FG_DISC_D32B or FG_DISC_D32", disc);
+    return FG_ERR_UNSUPPORTED;
+  }
   FG_REQUIRE(channels == 1 || channels == 3, "fg_create: channels must be 1 or 3 (got %d)", channels);
   FG_REQUIRE(max_batch >= 4 && max_batch % 2 == 0, "fg_create: max_batch must be even and >= 4 (got %d)", max_batch);
   int ndev = 0;
@@ -153,7 +181,7 @@ int fg_create(fg_ctx** out, int device, int max_batch, int channels) {
     return FG_ERR_CUDA;
   }
   int r = ctx_alloc(c);
-  if (r == FG_OK) r = net32_alloc(c);
+  if (r == FG_OK) r = net32_alloc(c, disc);
   if (r == FG_OK) r = tc_init(c);
   if (r != FG_OK) {
     net32_free(c);

@@ -475,7 +475,7 @@ int tc_init(fg_ctx* c);
 void tc_destroy(fg_ctx* c);
 
 // ---- nets.cu: the 32x32 nets of fg_ctx::n32 ---------------------------------------------------------
-int net32_alloc(fg_ctx* c);
+int net32_alloc(fg_ctx* c, int disc);  // disc: FG_DISC_D32B or a branched D at side 32 (nets_dbr.cu)
 void net32_free(fg_ctx* c);
 NetPair& net32_pair(fg_ctx* c);  // their trainable state
 

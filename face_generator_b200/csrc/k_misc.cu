@@ -27,16 +27,6 @@ __global__ void add_kernel(const float* __restrict__ a, const float* __restrict_
   GRID_STRIDE(i, n) out[i] = a[i] + b[i];
 }
 
-// first strict maximum in row-major window order (THNN SpatialMaxPooling: `val > maxval`)
-__device__ __forceinline__ int argmax4(float v0, float v1, float v2, float v3, float* best) {
-  int j = 0;
-  float m = v0;
-  if (v1 > m) { m = v1; j = 1; }
-  if (v2 > m) { m = v2; j = 2; }
-  if (v3 > m) { m = v3; j = 3; }
-  *best = m;
-  return j;
-}
 __global__ void maxpool2_fwd_nhwc_kernel(const float* __restrict__ h, float* __restrict__ p, int B, int H, int W, int C) {
   const int Ho = H / 2, Wo = W / 2;
   const int64_t n = (int64_t)B * Ho * Wo * C;

@@ -2,11 +2,27 @@
 #pragma once
 #include "fg_internal.h"
 
+// first strict maximum of a 2x2 window in row-major order (THNN SpatialMaxPooling: `val > maxval`); a NaN in the first
+// position passes through
+__device__ __forceinline__ int argmax4(float v0, float v1, float v2, float v3, float* best) {
+  int j = 0;
+  float m = v0;
+  if (v1 > m) { m = v1; j = 1; }
+  if (v2 > m) { m = v2; j = 2; }
+  if (v3 > m) { m = v3; j = 3; }
+  *best = m;
+  return j;
+}
+
 // NHWC (fused nets)
 int k_join_to_nhwc(fg_ctx* c, const float* noise_nchw, const float* cond_nchw, float* out_nhwc, int B, int C, int HW);
 int k_add(fg_ctx* c, const float* a, const float* b, float* out, int64_t n);
 int k_maxpool2_fwd(fg_ctx* c, const float* h, float* p, int B, int H, int W, int C);                  // H,W: input size
 int k_maxpool2_bwd(fg_ctx* c, const float* dp, const float* h, float* dh, int B, int H, int W, int C);
+// a stride-2 "same" convolution as the stride-1 one sampled at the even pixels (nets_s16.cu): x [B][H][W][C] ->
+// y [B][H/2][W/2][C], and its adjoint (zeros at the odd pixels); H, W: the stride-1 size
+int k_subsample2(fg_ctx* c, const float* x, float* y, int B, int H, int W, int C);
+int k_zero_insert2(fg_ctx* c, const float* dy, float* dx, int B, int H, int W, int C);
 // y = x * mask * scale; mask element order is the reference's NCHW flattening: masks[b*stride + moff + ch*HW + q]
 int k_dropout_nhwc(fg_ctx* c, const float* x, const float* masks, int64_t stride, int moff, int HW, int C, float scale,
                    float* y, int B);

@@ -261,11 +261,13 @@ struct Net32 : UpsGan {
   float* tail_sep = nullptr;
 };
 
-int net32_alloc(fg_ctx* c) {
+int net32_alloc(fg_ctx* c, int disc) {
   Net32* n = c->n32 = new Net32();
+  n->disc = disc;
   // G.L1 padded to K = 128 for the tensor cores; G.C1 / G.C2 may merge
-  static const GanDesc k32{{32, "", 128, true}, kMaskPerSample, true};
-  FG_TRY(gan_alloc(*n, c, k32, std::make_unique<D32>(), c->io_dev));
+  const bool b = disc == FG_DISC_D32B;
+  const GanDesc k32{{32, "", 128, true}, b ? kMaskPerSample : dbr_mask_per_sample(disc), true};
+  FG_TRY(gan_alloc(*n, c, k32, b ? std::make_unique<D32>() : dbr_make(disc), c->io_dev));
   NetPair& p = n->net;
   p.optim_timer[0] = "hbm.optim.G";
   p.optim_timer[1] = "hbm.optim.D";
@@ -315,6 +317,13 @@ int train_step_dataset_iters(fg_ctx* c, fg_dataset* d, const char* what, const f
 
 extern "C" {
 
+int fg_get_disc(fg_ctx* c) {
+  if (!c) {
+    fg_set_error("null fg_ctx");
+    return FG_ERR_INVALID;
+  }
+  return c->n32->disc;
+}
 int64_t fg_param_count(int net, int channels) {
   if (channels != 1 && channels != 3) return -1;
   return net == FG_NET_G ? make_g_layout(channels, 32).total : net == FG_NET_D ? make_d_layout(channels).total : -1;

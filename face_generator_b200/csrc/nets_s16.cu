@@ -105,6 +105,16 @@ __global__ void split2_kernel(const float* __restrict__ in, float* __restrict__ 
 }
 }  // namespace
 
+int k_subsample2(fg_ctx* c, const float* x, float* y, int B, int H, int W, int C) {
+  subsample2_kernel<<<grid_for((int64_t)B * (H / 2) * (W / 2) * C, 256), 256, 0, c->stream>>>(x, y, B, H, W, C);
+  LAUNCH_CHECK(c);
+  return FG_OK;
+}
+int k_zero_insert2(fg_ctx* c, const float* dy, float* dx, int B, int H, int W, int C) {
+  zero_insert2_kernel<<<grid_for((int64_t)B * H * W * C, 256), 256, 0, c->stream>>>(dy, dx, B, H, W, C);
+  LAUNCH_CHECK(c);
+  return FG_OK;
+}
 
 namespace {
 // D16: every layer a ConvL, activations NHWC
@@ -351,17 +361,28 @@ struct fg_s16 : UpsGan {};
 
 extern "C" {
 
-int fg_s16_create(fg_ctx* ctx, fg_s16** out) {
+int fg_s16_create(fg_ctx* ctx, fg_s16** out) { return fg_s16_create_disc(ctx, FG_DISC_D16_D, out); }
+
+int fg_s16_create_disc(fg_ctx* ctx, int disc, fg_s16** out) {
   if (!ctx || !out) {
     fg_set_error("fg_s16_create: null argument");
     return FG_ERR_INVALID;
   }
   *out = nullptr;
+  if (disc == FG_DISC_DEFAULT) disc = FG_DISC_D16_D;
+  FG_REQUIRE(fg_disc_side(disc), "fg_s16_create_disc: unknown discriminator %d", disc);
+  if (fg_disc_side(disc) != kSide) {
+    fg_set_error("fg_s16_create_disc: discriminator %d is a 32x32 net; the --scale 16 nets take FG_DISC_D16_D, "
+                 "FG_DISC_D16, FG_DISC_D16_B or FG_DISC_D16_C", disc);
+    return FG_ERR_UNSUPPORTED;
+  }
   FG_CUDA(cudaSetDevice(ctx->device));
   fg_s16* n = new fg_s16();
+  n->disc = disc;
   // G.L1 keeps K = 100 (on the FFMA kernels): padding it would change its bits.  Two backward launches per 5x5 layer.
-  static const GanDesc k16{{kSide, "s16.", 0, false}, kS16Mask, false};
-  const int r = gan_alloc(*n, ctx, k16, std::make_unique<D16>(), nullptr);
+  const bool d = disc == FG_DISC_D16_D;
+  const GanDesc k16{{kSide, "s16.", 0, false}, d ? kS16Mask : dbr_mask_per_sample(disc), false};
+  const int r = gan_alloc(*n, ctx, k16, d ? std::make_unique<D16>() : dbr_make(disc), nullptr);
   if (r != FG_OK) {
     fg_s16_destroy(n);
     return r;
@@ -384,6 +405,10 @@ int64_t fg_s16_param_count(int net, int channels) {
   return D16().layout(channels);
 }
 int fg_s16_mask_per_sample(void) { return kS16Mask; }
+int fg_s16_get_disc(fg_s16* n) {
+  ENTER(n);
+  return n->disc;
+}
 
 int fg_s16_set_params(fg_s16* n, int net, const float* src) {
   ENTER(n);

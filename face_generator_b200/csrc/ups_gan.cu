@@ -3,6 +3,8 @@
 // the bodies of their C entry points.
 #include "ups_gan.h"
 
+#include <algorithm>
+
 namespace {
 // the nets in the loop body: real [B/2][C][S][S], noiseD [B/2][100] and noiseG [B][100] per iteration
 struct GanStep final : StepNets {
@@ -42,6 +44,11 @@ int gan_alloc(UpsGan& n, fg_ctx* c, const GanDesc& d, std::unique_ptr<GanD> D, f
   e.maxB = c->maxB;
   e.allocs = &n.allocs;
   FG_TRY(pair_alloc(c, n.allocs, n.net, make_g_layout(c->C, d.g.side).total, n.D->layout(c->C), true));
+  // G's share of the scratch: the split of its largest dY (G.C2's [maxB][S][S][128]) and its largest weight gradient
+  // (the collapsed 5x5 packs, or G.L1 padded to K = l1_kpad on the tensor cores: (S/4)^2 * 128 rows x (kpad + 100))
+  const size_t S = d.g.side;
+  n.g_dy = (size_t)c->maxB * S * S * 128;
+  n.g_ws = std::max<size_t>(36 * 256 * 128, d.g.l1_kpad ? S * S / 16 * 128 * (d.g.l1_kpad + kNoiseDim) : 0);
   FG_TRY(n.D->alloc());
   FG_TRY(gen_alloc(e, n.G, d.g));
   n.env_f.c = c;

@@ -34,8 +34,16 @@ struct GanDesc {
   bool overlap;   // StepNets::overlap: option dp_overlap may run D's update next to the following G forward
 };
 
+// The branched discriminators of models.lua (nets_dbr.cu): create_D32 at side 32, create_D16 / _b / _c at side 16.
+// disc is FG_DISC_*; every function refuses (side 0, count / width -1, null D) a value that is not one of those four.
+int dbr_side(int disc);
+int64_t dbr_param_count(int disc, int C);
+int dbr_mask_per_sample(int disc);
+std::unique_ptr<GanD> dbr_make(int disc);
+
 struct UpsGan {
   fg_ctx* c = nullptr;
+  int disc = 0;  // FG_DISC_* of D
   GanDesc d{};
   NetPair net;
   UpsGen G;
@@ -51,8 +59,10 @@ struct UpsGan {
   IterStage iter_stage;  // the inputs of the host-fed and device-fed train steps, stacked per iteration
   std::vector<void*> allocs;
   // the scratch G's and D's layers share: env.dy is the split of the current dY, env.ws the packed weight-gradient
-  // workspace (largest layer of either net)
+  // workspace (largest layer of either net).  D allocates both; g_dy / g_ws (floats) are G's needs, set by gan_alloc
+  // before D's alloc()
   ConvLEnv env;
+  size_t g_dy = 0, g_ws = 0;
 };
 
 // n's pair, D, G and staging on ctx c.  io: a buffer of at least maxB * side^2 * C floats to borrow as img[0], or null

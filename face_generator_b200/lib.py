@@ -64,6 +64,11 @@ SYMBOLS = {
     "fg_get_option": (_L, [_P, C.c_char_p]),
     "fg_set_option_f": (_I, [_P, C.c_char_p, C.c_double]),
     "fg_param_count": (_L, [_I, _I]),
+    "fg_create_disc": (_I, [C.POINTER(_P), _I, _I, _I, _I]),
+    "fg_get_disc": (_I, [_P]),
+    "fg_disc_param_count": (_L, [_I, _I]),
+    "fg_disc_mask_per_sample": (_I, [_I]),
+    "fg_disc_side": (_I, [_I]),
     "fg_set_params": (_I, [_P, _I, _P]),
     "fg_get_params": (_I, [_P, _I, _P]),
     "fg_get_grads": (_I, [_P, _I, _P]),
@@ -182,6 +187,8 @@ SYMBOLS = {
     "fg_s16_destroy": (_I, [_P]),
     "fg_s16_param_count": (_L, [_I, _I]),
     "fg_s16_mask_per_sample": (_I, []),
+    "fg_s16_create_disc": (_I, [_P, _I, C.POINTER(_P)]),
+    "fg_s16_get_disc": (_I, [_P]),
     "fg_s16_set_params": (_I, [_P, _I, _P]),
     "fg_s16_get_params": (_I, [_P, _I, _P]),
     "fg_s16_get_grads": (_I, [_P, _I, _P]),
@@ -379,6 +386,18 @@ class _NetPair:
             raise FGError("%s%s: expected %d floats, got %d" % (self._what, what, n, a.size))
         return a
 
+    def _masks(self, what, m, rows):
+        """host keep flags for `rows` samples of this pair's D: the C ABI reads rows * mask_per_sample floats, so a
+        shorter array (flags of another discriminator) is refused.  Raw addresses pass as they are."""
+        if m is None or not hasattr(m, "shape"):
+            return m
+        m = f32(m)
+        n = rows * self.mask_per_sample
+        if m.size < n:
+            raise FGError("%s%s: %d keep flags for %d samples of %d, got %d"
+                          % (self._what, what, n, rows, self.mask_per_sample, m.size))
+        return m
+
     def set_params(self, net, p):
         self._call("set_params", net, _ptr(self._sized("set_params", p, self.count(net))))
 
@@ -433,16 +452,42 @@ class _BatchNormNetPair(_NetPair):
         return out
 
 
-class Context(_BatchNormNetPair):
-    """One fg_ctx (one GPU).  Mirrors face_generator_b200/lua/b200.lua's `b200.Context`."""
+# models.lua's discriminators by the name of the function that builds them (include/fg_b200.h FG_DISC_*)
+DISCRIMINATORS = {"create_D32b": 1, "create_D16_d": 2, "create_D32": 3, "create_D16": 4, "create_D16_b": 5,
+                  "create_D16_c": 6}
 
-    def __init__(self, device=0, max_batch=256, channels=3):
+
+def disc_id(name):
+    """FG_DISC_* of a models.lua discriminator name ("create_D32", ...)"""
+    if name not in DISCRIMINATORS:
+        raise FGError("unknown discriminator %r: models.lua defines %s" % (name, ", ".join(sorted(DISCRIMINATORS))))
+    return DISCRIMINATORS[name]
+
+
+def disc_param_count(name, channels):
+    """length of the discriminator's getParameters() vector"""
+    return int(load_library().fg_disc_param_count(disc_id(name), channels))
+
+
+def disc_mask_per_sample(name):
+    """the discriminator's (Spatial)Dropout keep flags per sample, in module order"""
+    return int(load_library().fg_disc_mask_per_sample(disc_id(name)))
+
+
+class Context(_BatchNormNetPair):
+    """One fg_ctx (one GPU).  Mirrors face_generator_b200/lua/b200.lua's `b200.Context`.  discriminator: the 32x32
+    D, "create_D32b" (models.lua's choice) or "create_D32"."""
+
+    def __init__(self, device=0, max_batch=256, channels=3, discriminator="create_D32b"):
         self.lib = load_library()
         h = C.c_void_p()
-        _check(self.lib.fg_create(C.byref(h), device, max_batch, channels), "fg_create")
+        disc = disc_id(discriminator)
+        _check(self.lib.fg_create_disc(C.byref(h), device, max_batch, channels, disc), "fg_create_disc")
         self.h, self.C, self.max_batch, self.device = h, channels, max_batch, device
+        self.discriminator = discriminator
         self.nG = int(self.lib.fg_param_count(NET_G, channels))
-        self.nD = int(self.lib.fg_param_count(NET_D, channels))
+        self.nD = int(self.lib.fg_disc_param_count(disc, channels))
+        self.mask_per_sample = int(self.lib.fg_disc_mask_per_sample(disc))
 
     def close(self):
         if self.h:
@@ -487,7 +532,7 @@ class Context(_BatchNormNetPair):
     def D_forward(self, images, masks=None, training=True, seed=0):
         images = f32(images)
         B = images.shape[0]
-        masks = f32(masks) if masks is not None else None
+        masks = self._masks("D_forward", masks, B)
         out = np.empty(B, np.float32)
         _check(self.lib.fg_D_forward(self.h, _ptr(images), B, int(training), _ptr(masks), seed, _ptr(out)), "fg_D_forward")
         return out
@@ -517,6 +562,7 @@ class Context(_BatchNormNetPair):
     # ---- L-step ----
     def train_step(self, hyper, B, real, noise_D, noise_G, masks_D=None, masks_G=None, seed=0, want_stats=True):
         """Pointers may be numpy float32 arrays (host) or raw addresses (device / pinned)."""
+        masks_D, masks_G = self._masks("train_step masks_D", masks_D, B), self._masks("train_step masks_G", masks_G, B)
         st = StepStats() if want_stats else None
         _check(self.lib.fg_train_step(self.h, C.byref(hyper), B, _ptr(real), _ptr(noise_D), _ptr(noise_G),
                                       _ptr(masks_D), _ptr(masks_G), seed, C.byref(st) if st is not None else None),
@@ -527,8 +573,10 @@ class Context(_BatchNormNetPair):
                          seed=0, want_stats=True):
         """D_iterations D iterations + G_iterations G iterations in one call (fg_train_step_iters); the inputs of
         train_step stacked per iteration: real [d][B/2][C][32][32], noise_D [d][B/2][100], noise_G [g][B][100],
-        masks_* [d|g][B][1984] or None."""
+        masks_* [d|g][B][mask_per_sample] or None (mask_per_sample: 1984 for create_D32b)."""
         d, g = check_iters(D_iterations, G_iterations)
+        masks_D = self._masks("train_step_iters masks_D", masks_D, d * B)
+        masks_G = self._masks("train_step_iters masks_G", masks_G, g * B)
         st = StepStats() if want_stats else None
         _check(self.lib.fg_train_step_iters(self.h, C.byref(hyper), B, d, g, _ptr(real), _ptr(noise_D), _ptr(noise_G),
                                             _ptr(masks_D), _ptr(masks_G), seed, C.byref(st) if st is not None else None),
@@ -784,16 +832,20 @@ S16_MASK_PER_SAMPLE = 1024 + 128
 
 
 class S16(_BatchNormNetPair):
-    """The --scale 16 nets (models.lua:27-51 G16, :279-316 D16_d) + the adversarial.lua loop on a Context."""
+    """The --scale 16 nets (models.lua:27-51 G16, :279-316 D16_d) + the adversarial.lua loop on a Context.
+    discriminator: "create_D16_d" (models.lua's choice), "create_D16", "create_D16_b" or "create_D16_c"."""
     _prefix, _what = "fg_s16_", "s16 "
 
-    def __init__(self, ctx):
+    def __init__(self, ctx, discriminator="create_D16_d"):
         self.ctx, self.lib, self.C = ctx, ctx.lib, ctx.C
         h = C.c_void_p()
-        _check(self.lib.fg_s16_create(ctx.h, C.byref(h)), "fg_s16_create")
+        disc = disc_id(discriminator)
+        _check(self.lib.fg_s16_create_disc(ctx.h, disc, C.byref(h)), "fg_s16_create_disc")
         self.h = h
+        self.discriminator = discriminator
         self.nG = int(self.lib.fg_s16_param_count(NET_G, self.C))
-        self.nD = int(self.lib.fg_s16_param_count(NET_D, self.C))
+        self.nD = int(self.lib.fg_disc_param_count(disc, self.C))
+        self.mask_per_sample = int(self.lib.fg_disc_mask_per_sample(disc))
 
     def close(self):
         if self.h:
@@ -823,7 +875,7 @@ class S16(_BatchNormNetPair):
     def D_forward(self, img, masks=None, training=True, seed=0):
         img = f32(img)
         B = img.shape[0]
-        masks = f32(masks) if masks is not None else None
+        masks = self._masks("D_forward", masks, B)
         out = np.empty(B, np.float32)
         _check(self.lib.fg_s16_D_forward(self.h, _ptr(img), B, int(training), _ptr(masks), seed, _ptr(out)), "fg_s16_D_forward")
         return out
@@ -836,6 +888,7 @@ class S16(_BatchNormNetPair):
 
     def train_step(self, hyper, B, real, noise_D, noise_G, masks_D=None, masks_G=None, seed=0, want_stats=True):
         """Pointers may be numpy float32 arrays (host) or raw addresses (device / pinned)."""
+        masks_D, masks_G = self._masks("train_step masks_D", masks_D, B), self._masks("train_step masks_G", masks_G, B)
         st = StepStats() if want_stats else None
         _check(self.lib.fg_s16_train_step(self.h, C.byref(hyper), B, _ptr(real), _ptr(noise_D), _ptr(noise_G), _ptr(masks_D),
                                           _ptr(masks_G), seed, C.byref(st) if st is not None else None), "fg_s16_train_step")
@@ -852,8 +905,10 @@ class S16(_BatchNormNetPair):
     def train_step_iters(self, hyper, B, D_iterations, G_iterations, real, noise_D, noise_G, masks_D=None, masks_G=None,
                          seed=0, want_stats=True):
         """fg_s16_train_step_iters: train_step's inputs stacked per iteration (real [d][B/2][C][16][16], noise_D
-        [d][B/2][100], noise_G [g][B][100], masks_* [d|g][B][1152] or None)."""
+        [d][B/2][100], noise_G [g][B][100], masks_* [d|g][B][mask_per_sample] or None; 1152 for create_D16_d)."""
         d, g = check_iters(D_iterations, G_iterations)
+        masks_D = self._masks("train_step_iters masks_D", masks_D, d * B)
+        masks_G = self._masks("train_step_iters masks_G", masks_G, g * B)
         st = StepStats() if want_stats else None
         _check(self.lib.fg_s16_train_step_iters(self.h, C.byref(hyper), B, d, g, _ptr(real), _ptr(noise_D), _ptr(noise_G),
                                                 _ptr(masks_D), _ptr(masks_G), seed, C.byref(st) if st is not None else None),

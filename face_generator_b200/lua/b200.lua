@@ -10,11 +10,22 @@ local C = F.C
 
 b200 = b200 or {}
 
--- one context per process/GPU, created lazily from OPT (train.lua:16-50)
-function b200.context(device, maxBatch, channels)
+-- models.lua's discriminators by the name of the function that builds them (FG_DISC_*, include/fg_b200.h)
+b200.DISCRIMINATORS = {create_D32b = 1, create_D16_d = 2, create_D32 = 3, create_D16 = 4, create_D16_b = 5,
+                       create_D16_c = 6}
+local function disc_id(name, default)
+  local d = b200.DISCRIMINATORS[name or default]
+  assert(d, 'unknown discriminator ' .. tostring(name))
+  return d
+end
+
+-- one context per process/GPU, created lazily from OPT (train.lua:16-50); discriminator: 'create_D32b' (default)
+-- or 'create_D32'
+function b200.context(device, maxBatch, channels, discriminator)
   if not b200._ctx then
     local out = ffi.new('fg_ctx*[1]')
-    F.check(C.fg_create(out, device or 0, maxBatch or 256, channels or 3), 'fg_create')
+    F.check(C.fg_create_disc(out, device or 0, maxBatch or 256, channels or 3, disc_id(discriminator, 'create_D32b')),
+            'fg_create_disc')
     b200._ctx = ffi.gc(out[0], C.fg_destroy)
     b200._hyper = ffi.new('fg_hyper[1]')
     C.fg_hyper_default(b200._hyper)
@@ -22,11 +33,12 @@ function b200.context(device, maxBatch, channels)
   return b200._ctx
 end
 
--- the --scale 16 nets (models.lua:87-104 pick create_G_decoder_upsampling16 / create_D16_d for 16x16 images)
-function b200.s16(ctx)
+-- the --scale 16 nets (models.lua:87-104 pick create_G_decoder_upsampling16 / create_D16_d for 16x16 images);
+-- discriminator: 'create_D16_d' (default), 'create_D16', 'create_D16_b' or 'create_D16_c'
+function b200.s16(ctx, discriminator)
   if not b200._s16 then
     local out = ffi.new('fg_s16*[1]')
-    F.check(C.fg_s16_create(ctx, out), 'fg_s16_create')
+    F.check(C.fg_s16_create_disc(ctx, disc_id(discriminator, 'create_D16_d'), out), 'fg_s16_create_disc')
     b200._s16 = ffi.gc(out[0], C.fg_s16_destroy)
   end
   return b200._s16
@@ -86,7 +98,9 @@ function Fused:__init(net, channels, layers)
 end
 function Fused:attach()
   self.ctx = b200.context()
-  self.n = tonumber(C.fg_param_count(self.net, self.channels))
+  -- D's length follows the discriminator the context holds (fg_create_disc), G's is fixed
+  self.n = self.net == F.NET_D and tonumber(C.fg_disc_param_count(C.fg_get_disc(self.ctx), self.channels))
+           or tonumber(C.fg_param_count(self.net, self.channels))
   self.train = true
   self.output, self.gradInput = torch.CudaTensor(), torch.CudaTensor()
   self.weight = b200.aliasCuda(C.fg_params_ptr(self.ctx, self.net), self.n)
@@ -177,11 +191,12 @@ function FusedG:backward(input, gradOutput)  -- updateGradInput + accGradParamet
 end
 FusedG.updateGradInput = FusedG.backward
 
--- MODELS.create_D(dimensions)  (models.lua:98-104 -> create_D32b :382-416)
-local FusedD = torch.class('b200.FusedD', 'b200.Fused')
-function FusedD:__init(dimensions)
-  assert(dimensions[2] == 32, 'b200.FusedD implements create_D32b')
-  local layers, cin = {}, dimensions[1]
+-- MODELS.create_D(dimensions)  (models.lua:98-104 -> create_D32b :382-416), or with `name` another 32x32
+-- discriminator of models.lua ('create_D32', :322-376).  The context is created with that D when this is its first
+-- use; a context that already holds another D is refused, naming both.  The proxies list the parameterised leaves
+-- in module order through the ConcatTable, which is getParameters() order.
+local function d32b_layers(c)
+  local layers, cin = {}, c
   for _, cout in ipairs({64, 128, 256, 512}) do
     for _, L in ipairs({{'nn.SpatialConvolution', {cout, cin, 3, 3}, {cout}}, {'nn.PReLU', {1}}, {'nn.SpatialDropout'},
                         {'nn.SpatialAveragePooling'}}) do layers[#layers + 1] = L end
@@ -190,6 +205,38 @@ function FusedD:__init(dimensions)
   for _, L in ipairs({{'nn.View'}, {'nn.Linear', {512, 2048}, {512}}, {'nn.PReLU', {1}}, {'nn.Dropout'},
                       {'nn.Linear', {512, 512}, {512}}, {'nn.PReLU', {1}}, {'nn.Dropout'}, {'nn.Linear', {1, 512}, {1}},
                       {'nn.Sigmoid'}}) do layers[#layers + 1] = L end
+  return layers
+end
+local function d32_layers(c)
+  local conv = function(o, i, k) return {'nn.SpatialConvolution', {o, i, k, k}, {o}} end
+  local lin = function(o, i) return {'nn.Linear', {o, i}, {o}} end
+  local P = {'nn.PReLU', {1}}
+  return {
+    -- fine branch
+    conv(64, c, 3), P, conv(64, 64, 3), P, {'nn.SpatialMaxPooling'}, {'nn.SpatialDropout'}, {'nn.View'}, lin(1024, 16384), P,
+    -- coarse branch
+    conv(32, c, 5), P, conv(32, 32, 5), P, {'nn.SpatialMaxPooling'}, conv(54, 32, 5), P, conv(54, 54, 5), P,
+    {'nn.SpatialMaxPooling'}, {'nn.SpatialDropout'}, {'nn.View'}, lin(1024, 3456), P, {'nn.Dropout'}, lin(1024, 1024), P,
+    -- dense branch
+    {'nn.View'}, lin(1024, c * 1024), P, {'nn.Dropout'}, lin(1024, 1024), P,
+    -- head
+    {'nn.JoinTable'}, lin(1024, 3072), P, {'nn.Dropout'}, lin(1, 1024), {'nn.Sigmoid'}}
+end
+local D32_LAYERS = {create_D32b = d32b_layers, create_D32 = d32_layers}
+local FusedD = torch.class('b200.FusedD', 'b200.Fused')
+function FusedD:__init(dimensions, name)
+  name = name or 'create_D32b'
+  assert(dimensions[2] == 32 and D32_LAYERS[name], 'b200.FusedD implements create_D32b and create_D32 (32x32), not '
+         .. tostring(name) .. ' at ' .. tostring(dimensions[2]))
+  local ctx = b200.context(nil, nil, dimensions[1], name)
+  local held = C.fg_get_disc(ctx)
+  if held ~= disc_id(name) then
+    local have = '?'
+    for k, v in pairs(b200.DISCRIMINATORS) do if v == held then have = k end end
+    error('b200.FusedD(' .. name .. '): the context already holds ' .. have .. '; create it with b200.context(..., \''
+          .. name .. '\') first')
+  end
+  local layers = D32_LAYERS[name](dimensions[1])
   b200.Fused.__init(self, F.NET_D, dimensions[1], layers)
   self.seed = 0
   self.wantWeightGrads = true   -- set false inside fevalG_on_D to skip the D weight gradients the reference discards

@@ -25,6 +25,11 @@ int fg_set_option(fg_ctx* ctx, const char* key, int64_t value);
 int64_t fg_get_option(fg_ctx* ctx, const char* key);
 int fg_set_option_f(fg_ctx* ctx, const char* key, double value);
 int64_t fg_param_count(int net, int channels);
+int fg_create_disc(fg_ctx** out, int device, int max_batch, int channels, int disc);
+int fg_get_disc(fg_ctx* ctx);
+int64_t fg_disc_param_count(int disc, int channels);
+int fg_disc_mask_per_sample(int disc);
+int fg_disc_side(int disc);
 int fg_set_params(fg_ctx* ctx, int net, const float* src);
 int fg_get_params(fg_ctx* ctx, int net, float* dst);
 int fg_get_grads(fg_ctx* ctx, int net, float* dst);
@@ -152,6 +157,8 @@ int fg_s16_create(fg_ctx* ctx, fg_s16** out);
 int fg_s16_destroy(fg_s16* n);
 int64_t fg_s16_param_count(int net, int channels);
 int fg_s16_mask_per_sample(void);
+int fg_s16_create_disc(fg_ctx* ctx, int disc, fg_s16** out);
+int fg_s16_get_disc(fg_s16* n);
 int fg_s16_set_params(fg_s16* n, int net, const float* src);
 int fg_s16_get_params(fg_s16* n, int net, float* dst);
 int fg_s16_get_grads(fg_s16* n, int net, float* dst);

@@ -115,6 +115,30 @@ int fg_set_option(fg_ctx* ctx, const char* key, int64_t value);
 int64_t fg_get_option(fg_ctx* ctx, const char* key);
 int fg_set_option_f(fg_ctx* ctx, const char* key, double value);    /* "sgd_momentum_D", "sgd_momentum_G"     */
 
+/* ---- discriminators: the D of the 32x32 nets (fg_create_disc) and of the --scale 16 nets (fg_s16_create_disc) ----
+ * models.lua defines six; create_D picks FG_DISC_D32B at 32x32 and FG_DISC_D16_D at 16x16 (the nets' defaults,
+ * which fg_create / fg_s16_create build).  The other four are the three-branch nets (3x3 conv branch, 5x5 conv branch,
+ * dense branch -> JoinTable(2) -> Linear -> PReLU -> Dropout -> Linear(1) -> Sigmoid) the author trained against
+ * before them.  All p = 0.5 dropouts; keep flags per sample in module order.  A D of the other side is refused with
+ * FG_ERR_UNSUPPORTED before anything is allocated.                                                            */
+enum {
+  FG_DISC_DEFAULT = 0,  /* the size's own: D32B at 32x32, D16_D at 16x16                             */
+  FG_DISC_D32B = 1,     /* models.lua:382-416 create_D32b  (32x32)                                    */
+  FG_DISC_D16_D = 2,    /* models.lua:279-316 create_D16_d (16x16)                                    */
+  FG_DISC_D32 = 3,      /* models.lua:322-376 create_D32   (32x32)                                    */
+  FG_DISC_D16 = 4,      /* models.lua:110-159 create_D16   (16x16)                                    */
+  FG_DISC_D16_B = 5,    /* models.lua:161-216 create_D16_b (16x16)                                    */
+  FG_DISC_D16_C = 6     /* models.lua:218-277 create_D16_c (16x16)                                    */
+};
+/* fg_create with discriminator `disc` (FG_DISC_DEFAULT / D32B / D32)                                    */
+int fg_create_disc(fg_ctx** out, int device, int max_batch, int channels, int disc);
+int fg_get_disc(fg_ctx* ctx);                      /* FG_DISC_* of the 32x32 D (never DEFAULT); < 0 on error */
+/* D's getParameters() length for 1 or 3 channels and its keep flags per sample; -1 for an unknown disc
+ * (or FG_DISC_DEFAULT, which names no net by itself) or channel count                                    */
+int64_t fg_disc_param_count(int disc, int channels);
+int fg_disc_mask_per_sample(int disc);
+int fg_disc_side(int disc);                        /* 32 or 16; 0 for an unknown disc                       */
+
 /* ---- parameters: replaces MODEL:getParameters() (train.lua:151-152) -------------------------- */
 int64_t fg_param_count(int net, int channels);
 int fg_set_params(fg_ctx* ctx, int net, const float* src);
@@ -145,7 +169,8 @@ int fg_G_forward(fg_ctx* ctx, const float* noise, int B, int training, float* im
 /* d_images [B][C][32][32]; accumulates into G's grad buffer; d_noise may be NULL.               */
 int fg_G_backward(fg_ctx* ctx, const float* d_images, float* d_noise);
 /* models.lua:382-416.  masks: [B][1984] keep flags (0/1) per sample =
- * [64|128|256|512] SpatialDropout + [512|512] Dropout; NULL => drawn in-kernel from `seed`.
+ * [64|128|256|512] SpatialDropout + [512|512] Dropout (another D: [B][fg_disc_mask_per_sample(D)], module order);
+ * NULL => drawn in-kernel from `seed`.
  * training=0 => evaluate() semantics.  out [B] sigmoid outputs (may be NULL).                   */
 int fg_D_forward(fg_ctx* ctx, const float* images, int B, int training, const float* masks, uint64_t seed,
                  float* out);
@@ -293,6 +318,10 @@ int fg_c2f_train_step(fg_c2f* n, const fg_hyper* h, int B, const float* real_dif
  * D [c1W c1b a1 .. c4W c4b a4 F1W F1b af E1W E1b ae1 E2W E2b ae2 JW Jb].                                  */
 typedef struct fg_s16 fg_s16;
 int fg_s16_create(fg_ctx* ctx, fg_s16** out);
+/* fg_s16_create with discriminator `disc` (FG_DISC_DEFAULT / D16_D / D16 / D16_B / D16_C); masks and D's parameter
+ * vector of every fg_s16_* entry point then follow that D (fg_disc_param_count / fg_disc_mask_per_sample)      */
+int fg_s16_create_disc(fg_ctx* ctx, int disc, fg_s16** out);
+int fg_s16_get_disc(fg_s16* n);                  /* FG_DISC_* of D (never DEFAULT); < 0 on error           */
 int fg_s16_destroy(fg_s16* n);
 int64_t fg_s16_param_count(int net, int channels);
 int fg_s16_mask_per_sample(void);                         /* 1152 = 1024 SpatialDropout planes + 128 Dropout */
@@ -310,11 +339,12 @@ int fg_s16_get_bn_state(fg_s16* n, float* dst768);
  * backward accumulates into G's grad buffer; d_noise [B][100] may be NULL.                                */
 int fg_s16_G_forward(fg_s16* n, const float* noise, int B, int training, float* img_out);
 int fg_s16_G_backward(fg_s16* n, const float* d_img, float* d_noise);
-/* images [B][C][16][16] -> [B] sigmoid outputs; masks [B][1152] keep flags or NULL (drawn from seed).     */
+/* images [B][C][16][16] -> [B] sigmoid outputs; masks [B][fg_disc_mask_per_sample(D)] keep flags (1152 for
+ * create_D16_d) or NULL (drawn from seed).                                                                */
 int fg_s16_D_forward(fg_s16* n, const float* img, int B, int training, const float* masks, uint64_t seed, float* out);
 int fg_s16_D_backward(fg_s16* n, const float* d_out, int want_wgrad, float* d_img);
 /* fg_train_step on the 16x16 nets: real [B/2][C][16][16], noise_D [B/2][100], noise_G [B][100],
- * masks_* [B][1152] or NULL.                                                                              */
+ * masks_* [B][fg_disc_mask_per_sample(D)] (1152 for create_D16_d) or NULL.                                 */
 int fg_s16_train_step(fg_s16* n, const fg_hyper* h, int B, const float* real, const float* noise_D, const float* noise_G,
                       const float* masks_D, const float* masks_G, uint64_t seed, fg_step_stats* stats);
 
