@@ -97,6 +97,11 @@ int ctx_alloc(fg_ctx* c) {
   FG_TRY(dalloc(&s.bn_acc, 4 * 256 * 2));
   FG_TRY(dalloc(&s.bn_slice_acc, 32 * 4 * 256 * 2 + 64));
   FG_TRY(dalloc(&s.bn_parts, B * 3072));
+  fg_ctx::WgradWorkspaces& w = c->wgrad_ws;  // and for the weight gradients on wgrad_stream
+  FG_TRY(dalloc(&w.splitk_ws, c->splitk_ws_elems));
+  FG_TRY(dalloc(&w.red_ws, 2 * c->red_ws_elems));
+  FG_TRY(dalloc(&w.red_ticket, 2));
+  FG_TRY(dalloc(&w.small_ws, (size_t)kSmallMaxParts * 9 * 4 * 128));
   c->io_dev_elems = std::max<size_t>(B * 1024 * C, B * kMaskPerSample);
   return dalloc(&c->io_dev, c->io_dev_elems);
 }
@@ -198,13 +203,15 @@ int fg_destroy(fg_ctx* c) {
   if (!c) return FG_OK;
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
-  for (cudaStream_t s : {c->comm_stream, c->side_stream})
+  for (cudaStream_t s : {c->comm_stream, c->side_stream, c->wgrad_stream})
     if (s) {
       cudaStreamSynchronize(s);
       cudaStreamDestroy(s);
     }
   if (c->ev_fork) cudaEventDestroy(c->ev_fork);
   if (c->ev_join) cudaEventDestroy(c->ev_join);
+  for (cudaEvent_t e : {c->ev_wfork, c->ev_wjoin})
+    if (e) cudaEventDestroy(e);
   tc_destroy(c);
   net32_free(c);
   jpeg_enc_scratch_free(c->jpeg_enc);
@@ -277,6 +284,11 @@ int fg_set_option(fg_ctx* c, const char* key, int64_t v) {
     c->bwd_merge = (int)v;
     return FG_OK;
   }
+  if (!strcmp(key, "bwd_streams")) {  // see fg_ctx::bwd_streams
+    FG_REQUIRE(v == 0 || v == 1, "bwd_streams must be 0 (one stream) or 1 (weight gradients on a stream of their own)");
+    c->bwd_streams = (int)v;
+    return FG_OK;
+  }
   if (!strcmp(key, "bwd_merge_ctas")) {
     FG_REQUIRE(v >= 0, "bwd_merge_ctas must be >= 0 (0: one CTA per SM)");
     c->bwd_merge_ctas = v > (1 << 20) ? (1 << 20) : (int)v;
@@ -324,6 +336,7 @@ int64_t fg_get_option(fg_ctx* c, const char* key) {
   if (!strcmp(key, "use_graph")) return c->use_graph;
   if (!strcmp(key, "bwd_merge")) return c->bwd_merge;
   if (!strcmp(key, "bwd_merge_ctas")) return c->bwd_merge_ctas;
+  if (!strcmp(key, "bwd_streams")) return c->bwd_streams;
   if (!strcmp(key, "optimizer_D")) return c->opt_D;
   if (!strcmp(key, "optimizer_G")) return c->opt_G;
   if (!strcmp(key, "last_conv_kind")) return c->last_conv_kind;

@@ -1,6 +1,8 @@
 // ConvL / UpsL: layer-level dispatch shared by the nets (see convl.h)
 #include "convl.h"
 
+#include <utility>
+
 #include "k_conv_tc.h"
 #include "k_misc.h"
 
@@ -36,6 +38,51 @@ inline bool tc_w(const fg_ctx* c, const ConvL& L, int B) { return tc_f(c, L, B) 
 
 bool convl_tc_fwd(const fg_ctx* c, const ConvL& L) { return tc_f(c, L, 1); }
 bool convl_tc_bwd(const fg_ctx* c, const ConvL& L) { return tc_f(c, L, 1) && tc_d(c, L, 1); }
+bool convl_tc_wgrad(const fg_ctx* c, const ConvL& L) { return tc_w(c, L, 1); }
+
+bool wgrad_async(const fg_ctx* c, const ConvLEnv& e) {
+  return c->bwd_streams && e.ws_w && c->world == 1 && !c->timing && !c->debug_keep;
+}
+
+namespace {
+void swap_wgrad(fg_ctx* c, ConvLEnv& e) {
+  fg_ctx::WgradWorkspaces& w = c->wgrad_ws;
+  std::swap(c->stream, c->wgrad_stream);
+  std::swap(c->splitk_ws, w.splitk_ws);
+  std::swap(c->red_ws, w.red_ws);
+  std::swap(c->red_ticket, w.red_ticket);
+  std::swap(c->small_ws, w.small_ws);
+  std::swap(e.ws, e.ws_w);
+}
+int wgrad_fork(fg_ctx* c) {
+  if (!c->wgrad_stream) FG_CUDA(cudaStreamCreateWithFlags(&c->wgrad_stream, cudaStreamNonBlocking));
+  if (!c->ev_wfork) FG_CUDA(cudaEventCreateWithFlags(&c->ev_wfork, cudaEventDisableTiming));
+  if (!c->ev_wjoin) FG_CUDA(cudaEventCreateWithFlags(&c->ev_wjoin, cudaEventDisableTiming));
+  FG_CUDA(cudaEventRecord(c->ev_wfork, c->stream));
+  FG_CUDA(cudaStreamWaitEvent(c->wgrad_stream, c->ev_wfork, 0));
+  c->wgrad_forked = true;
+  return FG_OK;
+}
+}  // namespace
+
+OnWgradStream::OnWgradStream(ConvLEnv& e_, bool on_) : e(e_), on(on_) {
+  if (!on) return;
+  r = wgrad_fork(e.c);
+  if (r != FG_OK) on = false;
+  else swap_wgrad(e.c, e);
+}
+OnWgradStream::~OnWgradStream() {
+  if (on) swap_wgrad(e.c, e);
+}
+
+int wgrad_join(ConvLEnv& e) {
+  fg_ctx* c = e.c;
+  if (!c->wgrad_forked) return FG_OK;
+  c->wgrad_forked = false;
+  FG_CUDA(cudaEventRecord(c->ev_wjoin, c->wgrad_stream));
+  FG_CUDA(cudaStreamWaitEvent(c->stream, c->ev_wjoin, 0));
+  return FG_OK;
+}
 
 int tc_op_split(fg_ctx* c, TcOp& op, const float* x, int64_t n, bool f16) {
   if (!f16) {
@@ -158,13 +205,14 @@ int convl_fwd(ConvLEnv& e, ConvL& L, const float* in, const float* P, float* out
   return k_small_eligible(g) ? k_conv_small(c, in, L.Wp, bias, out, g) : k_conv_simt(c, in, L.Wp, bias, out, g);
 }
 
-int convl_bwd(ConvLEnv& e, ConvL& L, const float* in, const float* dy, float* G, float* din, int B) {
+int convl_bwd(ConvLEnv& e, ConvL& L, const float* in, const float* dy, float* G, float* din, int B, bool wgrad_side) {
   fg_ctx* c = e.c;
   const ConvGeom g = L.geom(B), gd = L.geom_d(B);
   const bool w_tc = G && tc_w(c, L, B), d_tc = din && tc_d(c, L, B);
   const bool h = L.packed_f16;
   // what the producer of dY already did (TcOp): consumed here
   float* sdy = L.sdy ? L.sdy : e.dy.s;
+  float *dy_hi = L.dy_hi ? L.dy_hi : e.dy.hi, *dy_lo = L.dy_lo ? L.dy_lo : e.dy.lo;
   const bool split_ready = e.dy.split_ready, amax_ready = e.dy.amax_ready, bias_ready = e.dy.bias_ready;
   e.dy.split_ready = e.dy.amax_ready = e.dy.bias_ready = false;
   const float *osy = h ? sdy + 1 : nullptr, *osx = h ? L.x.s + 1 : nullptr;
@@ -172,8 +220,8 @@ int convl_bwd(ConvLEnv& e, ConvL& L, const float* in, const float* dy, float* G,
   const int64_t P = (int64_t)B * L.H * L.H;
   if (h && !amax_ready && (w_tc || d_tc || (G && tc_on && (L.pad_out || L.pad_dy)))) FG_TRY(tc_amax(c, dy, P * L.Cout, sdy));
   if (w_tc || d_tc) {
-    if (h) FG_TRY(tc_split_h(c, dy, e.dy.hi, e.dy.lo, P * L.Cout, sdy));
-    else if (!split_ready) FG_TRY(tc_split(c, dy, e.dy.hi, e.dy.lo, P * L.Cout));
+    if (h) FG_TRY(tc_split_h(c, dy, dy_hi, dy_lo, P * L.Cout, sdy));
+    else if (!split_ready) FG_TRY(tc_split(c, dy, dy_hi, dy_lo, P * L.Cout));
   }
   if (G && tc_on && L.pad_out) {
     // swapped roles: Gt[t'][c][n] = sum_p X[p][c] * dYpad[p + off(t')][n]  ==  dW[KK-1-t'][n][c]
@@ -195,11 +243,13 @@ int convl_bwd(ConvLEnv& e, ConvL& L, const float* in, const float* dy, float* G,
     FG_TRY(k_unpack_wgrad_pad(c, e.ws, G + L.w_off, L.Cout, L.pad_dy, L.Cin, L.k * L.k));
     if (!bias_ready) FG_TRY(k_colsum_add(c, dy, G + L.b_off, P, L.Cout, 0, 0));
   } else if (G) {
+    OnWgradStream side(e, wgrad_side);
+    FG_TRY(side.r);
     // kpad: the [Cout][kpad] gradient lands behind the [Cout][Cin] one, whose pad columns are dropped by the copy
     const int64_t koff = L.kpad && w_tc ? (int64_t)L.Cout * L.Cin : 0;
     {
       ScopedTimer t(c, L.tw);
-      if (w_tc) FG_TRY(tc_conv_wgrad(c, L.x.hi, L.x.lo, e.dy.hi, e.dy.lo, e.ws + koff, L.geom_k(B), h, osy, osx));
+      if (w_tc) FG_TRY(tc_conv_wgrad(c, L.x.hi, L.x.lo, dy_hi, dy_lo, e.ws + koff, L.geom_k(B), h, osy, osx));
       else if (k_small_eligible(g)) FG_TRY(k_wgrad_small(c, in, dy, e.ws, g));
       else FG_TRY(k_wgrad_simt(c, in, dy, e.ws, g));
     }
@@ -211,7 +261,7 @@ int convl_bwd(ConvLEnv& e, ConvL& L, const float* in, const float* dy, float* G,
   }
   if (din) {
     ScopedTimer t(c, L.td);
-    if (d_tc) return tc_conv_fwd(c, e.dy.hi, e.dy.lo, L.Wd_hi, L.Wd_lo, nullptr, din, gd, 0, nullptr, nullptr, h, osy);
+    if (d_tc) return tc_conv_fwd(c, dy_hi, dy_lo, L.Wd_hi, L.Wd_lo, nullptr, din, gd, 0, nullptr, nullptr, h, osy);
     if (c->edge_impl && k_edge_eligible(gd)) return k_conv_edge(c, dy, L.Wpd, nullptr, din, gd);
     return k_small_eligible(gd) ? k_conv_small(c, dy, L.Wpd, nullptr, din, gd) : k_conv_simt(c, dy, L.Wpd, nullptr, din, gd);
   }
@@ -272,7 +322,8 @@ int upsl_fwd(ConvLEnv& e, UpsL& U, const float* h, const float* P, float* z, int
                      st ? parts : nullptr, f16, f16 ? U.x.s + 1 : nullptr);
 }
 
-int upsl_bwd(ConvLEnv& e, UpsL& U, TcOp& dy, const float* h, const float* dz, float* G, float* dh, int B, bool* pooled) {
+int upsl_bwd(ConvLEnv& e, UpsL& U, TcOp& dy, const float* h, const float* dz, float* G, float* dh, int B, bool* pooled,
+             bool wgrad_side) {
   fg_ctx* c = e.c;
   const ConvGeom g = U.geom(B);
   float* dW = G + U.w_off;
@@ -299,10 +350,16 @@ int upsl_bwd(ConvLEnv& e, UpsL& U, TcOp& dy, const float* h, const float* dz, fl
     return tc_combine_collapsed_wgrad(c, e.ws, dW, U.Cout, U.Cin);
   }
   {
-    ScopedTimer t(c, U.tw);
-    FG_TRY(tc_conv_wgrad(c, U.x.hi, U.x.lo, dy.hi, dy.lo, e.ws, g, f16, sy, sx));
+    // wgrad_side: the weight gradient and its combine on the wgrad stream, beside the data gradient (G.C1's 72 CTAs
+    // leave 60 SMs to the data-gradient tiles)
+    OnWgradStream side(e, wgrad_side);
+    FG_TRY(side.r);
+    {
+      ScopedTimer t(c, U.tw);
+      FG_TRY(tc_conv_wgrad(c, U.x.hi, U.x.lo, dy.hi, dy.lo, e.ws, g, f16, sy, sx));
+    }
+    FG_TRY(tc_combine_collapsed_wgrad(c, e.ws, dW, U.Cout, U.Cin));
   }
-  FG_TRY(tc_combine_collapsed_wgrad(c, e.ws, dW, U.Cout, U.Cin));
   ScopedTimer t(c, U.td);
   return tc_conv_dgrad_ups(c, dy.hi, dy.lo, U.Wd_hi, U.Wd_lo, dh, g, f16, sy);
 }

@@ -45,9 +45,27 @@ bool convl_tc_fwd(const fg_ctx* c, const ConvL& L);  // the forward runs on the 
 bool convl_tc_bwd(const fg_ctx* c, const ConvL& L);  // ... and so does the data gradient
 int convl_pack(fg_ctx* c, ConvL& L, const float* P);
 int convl_fwd(ConvLEnv& e, ConvL& L, const float* in, const float* P, float* out, int B);
+bool convl_tc_wgrad(const fg_ctx* c, const ConvL& L);  // the weight gradient runs on the tensor cores (reads the splits)
 // G (may be null): dW += wgrad, db += colsum(dy).  din (may be null) = dgrad.  The flags of e.dy say what dY's producer
-// already did (split into e.dy, max|dY| into L.sdy, bias gradient added); they are cleared.
-int convl_bwd(ConvLEnv& e, ConvL& L, const float* in, const float* dy, float* G, float* din, int B);
+// already did (split into L's dY split, max|dY| into L.sdy, bias gradient added); they are cleared.  wgrad_side: the
+// weight gradient of a layer without pad_out / pad_dy goes to the wgrad stream (OnWgradStream); the caller keeps
+// what it reads (in, dy or L's splits) unchanged until wgrad_join.
+int convl_bwd(ConvLEnv& e, ConvL& L, const float* in, const float* dy, float* G, float* din, int B, bool wgrad_side = false);
+
+// option "bwd_streams": whether a backward on e may put weight gradients on c->wgrad_stream.  Timing runs (per-launch
+// timers on one stream would misattribute the overlap), debug_keep runs and data-parallel steps stay on one stream.
+bool wgrad_async(const fg_ctx* c, const ConvLEnv& e);
+// While one lives (with `on`), launches go to c->wgrad_stream, after everything enqueued on c->stream so far, with that
+// stream's own copy of each workspace a weight gradient writes (c->wgrad_ws, e.ws_w).  r: the fork's error, if any.
+struct OnWgradStream {
+  ConvLEnv& e;
+  bool on;
+  int r = FG_OK;
+  OnWgradStream(ConvLEnv& e, bool on);
+  ~OnWgradStream();
+};
+// c->stream waits for every launch made on c->wgrad_stream so far (nothing to do when none was made since the last join)
+int wgrad_join(ConvLEnv& e);
 
 bool upsl_tc(const fg_ctx* c, const UpsL& U);  // the layer runs on the tensor cores
 int upsl_alloc(ConvLEnv& e, UpsL& U);
@@ -58,7 +76,8 @@ int upsl_fwd(ConvLEnv& e, UpsL& U, const float* h, const float* P, float* z, int
 // G: dW += wgrad (the bias gradient is the producer's: k_bn_prelu_bwd_apply's dbias); dh = dgrad; dy: the operand dz is
 // split into.  *pooled: dh already is the gradient of the LOW-RES input (the tensor-core dgrad folds in the 2x2 sum of
 // the upsample backward); otherwise dh is the full-resolution gradient the consumer still sums 2x2.
-int upsl_bwd(ConvLEnv& e, UpsL& U, TcOp& dy, const float* h, const float* dz, float* G, float* dh, int B, bool* pooled);
+int upsl_bwd(ConvLEnv& e, UpsL& U, TcOp& dy, const float* h, const float* dz, float* G, float* dh, int B, bool* pooled,
+             bool wgrad_side = false);
 
 // ---- gen.cu: UpsGen on the owner's layer scratch (ConvLEnv) and parameters (NetPair: PG, gG, bnG, G_pack) ----
 int gen_alloc(ConvLEnv& e, UpsGen& G, const GenDesc& d);

@@ -155,6 +155,9 @@ struct ConvL {  // NHWC, stride 1, "same" padding (a strided layer runs at strid
   float *Wf_hi = nullptr, *Wf_lo = nullptr, *Wd_hi = nullptr, *Wd_lo = nullptr;   // TF32 splits of the packs
   TcOp x;                    // split of the input (fwd -> wgrad); x.s may be set before convl_alloc
   float* sdy = nullptr;      // (max|dY|, 1/scale) of this layer's dY split; nullptr: the shared ConvLEnv::dy.s
+  // this layer's own dY split (a weight gradient on the wgrad stream still reads it while the next layer splits its
+  // dY); nullptr: the shared ConvLEnv::dy.hi / lo
+  float *dy_hi = nullptr, *dy_lo = nullptr;
   // kpad (Linear only): K zero-padded Cin -> kpad so that the layer runs on the tensor cores (xpad: [B][kpad] input,
   // Wpad: [Cout][kpad] weights, both with zero pad columns); its weight gradient needs Cout * (kpad + Cin) floats of ws
   int kpad = 0;
@@ -194,6 +197,8 @@ struct ConvLEnv {
   TcOp dy;              // split of the current dY (largest layer output); dy.s: (max|dY|, 1/scale) of its FP16 split
   TcOp pad;             // channel-padded split of dY (pad_out / pad_dy layers); scaled by dy.s
   float* ws = nullptr;  // packed weight-gradient workspace (largest layer)
+  // the same for the weight gradients on fg_ctx::wgrad_stream; nullptr: a backward on this scratch stays on one stream
+  float* ws_w = nullptr;
 };
 
 // What differs between the generator sizes, as data: the generator code never asks which net it serves
@@ -325,6 +330,20 @@ struct fg_ctx {
     double *bn_acc = nullptr, *bn_slice_acc = nullptr;
     float* bn_parts = nullptr;
   } side_ws;
+  // option "bwd_streams" (default 1): the backward of the 32x32 D and of G (D32::backward, gen_backward) enqueues the
+  // weight gradients that nothing downstream reads before the optimizer on wgrad_stream, next to the data-gradient
+  // chain on `stream` (OnWgradStream, convl.h); 0: one stream, in layer order.  wgrad_ws holds the stream's own copy of
+  // each workspace a weight gradient writes; wgrad_forked: launches went there since the last wgrad_join.
+  int bwd_streams = 1;
+  cudaStream_t wgrad_stream = nullptr;
+  cudaEvent_t ev_wfork = nullptr, ev_wjoin = nullptr;
+  bool wgrad_forked = false;
+  struct WgradWorkspaces {
+    float* splitk_ws = nullptr;
+    double* red_ws = nullptr;
+    unsigned* red_ticket = nullptr;
+    float* small_ws = nullptr;
+  } wgrad_ws;
   // debug (tests): "debug_keep" = 1 keeps a copy of the D step's pre-activations of every train step (NetPair::keep),
   // which the G step's D forward overwrites (the strict gradient-parity tests read PReLU branch decisions from them)
   bool debug_keep = false;

@@ -70,6 +70,10 @@ int gen_alloc(ConvLEnv& e, UpsGen& G, const GenDesc& d) {
     FG_TRY(G.pairs.take(&L->sdy));
     FG_TRY(convl_alloc(e, *L));
   }
+  // G.L1 splits its dY into buffers of its own: with option bwd_streams G.C1's weight gradient on the wgrad stream still
+  // reads G.C1's split in the shared ConvLEnv::dy while G.L1 splits
+  FG_TRY(convl_dalloc(e, &L1.dy_hi, (size_t)e.maxB * L1.Cout));
+  FG_TRY(convl_dalloc(e, &L1.dy_lo, (size_t)e.maxB * L1.Cout));
   static const char* uf[2] = {"G.C1.fwd", "G.C2.fwd"};
   static const char* ud[2] = {"G.C1.dgrad", "G.C2.dgrad"};
   static const char* uw[2] = {"G.C1.wgrad", "G.C2.wgrad"};
@@ -120,7 +124,7 @@ int gen_alloc_fwd(ConvLEnv& e, UpsGen& F, UpsGen& G) {
   for (ConvL* L : {&F.GL1, &F.GC3}) {
     L->x = TcOp{};
     L->xpad = nullptr;
-    L->sdy = nullptr;
+    L->sdy = L->dy_hi = L->dy_lo = nullptr;
     FG_TRY(F.pairs.take(&L->x.s));
     FG_TRY(convl_alloc_x(e, *L));
   }
@@ -221,7 +225,10 @@ int gen_backward(ConvLEnv& e, UpsGen& G, NetPair& p, const float* dy, float* dno
   const int B = G.B, S = G.S, h = S / 2;
   FG_TRY(G.pairs.reset(c));
   FG_TRY(k_sigmoid_bwd(c, dy, G.y, G.dz3, (int64_t)B * S * S * G.C));
-  FG_TRY(convl_bwd(e, G.GC3, G.h2, G.dz3, g, G.dfull, B));
+  // option bwd_streams: G.C3's weight gradient (a read of all of h2) beside its data gradient and the BN2 backward; it
+  // reads h2 and dz3, which nothing below writes.  G.L1's stays here: with no noise gradient it is the last launch of
+  // the pass, so on another stream it would overlap nothing (it runs beside G.C1's instead).
+  FG_TRY(convl_bwd(e, G.GC3, G.h2, G.dz3, g, G.dfull, B, wgrad_async(c, e)));
   // BN2 + PReLU
   {
     ScopedTimer tm(c, G.t_bn2_bwd_reduce);
@@ -257,12 +264,16 @@ int gen_backward(ConvLEnv& e, UpsGen& G, NetPair& p, const float* dy, float* dno
                                 dz1.split_ready ? dz1.lo : nullptr, g + L.C1b));
   }
   // C1
-  FG_TRY(upsl_bwd(e, G.GU[0], dz1, G.h0, G.dz1, g, G.dfull, B, &pooled));
+  // option bwd_streams: G.C1's weight gradient beside its data gradient and the G.L1 tail; it reads h0's split and dz1's
+  // in ConvLEnv::dy, which G.L1 (splitting into its own buffers) leaves alone.  Where the merged launch runs (bwd_merge)
+  // there is no separate weight gradient to move.
+  FG_TRY(upsl_bwd(e, G.GU[0], dz1, G.h0, G.dz1, g, G.dfull, B, &pooled, wgrad_async(c, e)));
   {
     AmaxInto am(c, G.GL1.sdy, &e.dy.amax_ready);
     FG_TRY(k_prelu_bwd(c, G.dfull, G.z0, P + L.a1, G.dz0, g + L.a1, B, S / 4, S / 4, 128, pooled ? 0 : 1));
   }
-  return convl_bwd(e, G.GL1, G.noise, G.dz0, g, dnoise, B);
+  FG_TRY(convl_bwd(e, G.GL1, G.noise, G.dz0, g, dnoise, B));
+  return wgrad_join(e);
 }
 
 void gen_debug_rows(const UpsGen& G, std::vector<DebugTensor>& rows) {

@@ -47,8 +47,9 @@ struct D32 final : GanD {
   float *z[4] = {nullptr, nullptr, nullptr, nullptr}, *p[4] = {nullptr, nullptr, nullptr, nullptr};
   float *zl1 = nullptr, *hl1 = nullptr, *zl2 = nullptr, *hl2 = nullptr;
   float drop_scale = 2.0f, spatial_eval = 0.8f;  // 1/(1-p_drop), 1-p_spatial of the last forward
-  float *dh = nullptr, *dzl = nullptr, *dz = nullptr, *dp = nullptr;
-  // option "debug_keep" (tests): the backward reuses dh / dzl / dp / dz across layers, so backward() copies each one as
+  float *dh = nullptr, *dz = nullptr, *dp = nullptr;
+  float *dzl2 = nullptr, *dzl1 = nullptr;  // D.L2's and D.L1's dY: their bias gradients may still read them (bwd_streams)
+  // option "debug_keep" (tests): the backward reuses dh / dp / dz across layers, so backward() copies each one as
   // a kernel wrote it ("Dbwd.*" debug tensors, the last D backward; Keep::src is unused here)
   std::vector<NetPair::Keep> bwd_keep;
   int bwd_keep_B = 0;
@@ -93,7 +94,8 @@ int D32::alloc() {
   FG_TRY(dalloc(&masks, B * kMaskPerSample));
   FG_TRY(dalloc(&dlogit, B));
   FG_TRY(dalloc(&dh, B * 512));
-  FG_TRY(dalloc(&dzl, B * 512));
+  FG_TRY(dalloc(&dzl2, B * 512));
+  FG_TRY(dalloc(&dzl1, B * 512));
   FG_TRY(dalloc(&dz, B * 65536));
   FG_TRY(dalloc(&dp, B * 16384));
   FG_TRY(dalloc(&dx, B * 1024 * C));
@@ -119,6 +121,13 @@ int D32::alloc() {
     FG_TRY(pairs.take(&L->x.s));
     FG_TRY(pairs.take(&L->sdy));
     FG_TRY(convl_alloc(e, *L));
+  }
+  // the tensor-core layers split their dY into buffers of their own: with option bwd_streams a weight gradient on the
+  // wgrad stream still reads a layer's split while the chain splits the next layer's dY
+  for (ConvL* L : {&Dc[1], &Dc[2], &Dc[3], &DL1, &DL2}) {
+    const size_t n_dy = B * (size_t)L->H * L->H * L->Cout;
+    FG_TRY(dalloc(&L->dy_hi, n_dy));
+    FG_TRY(dalloc(&L->dy_lo, n_dy));
   }
   n->net.keep = {{"Dstep.z1", z[0], 65536}, {"Dstep.z2", z[1], 32768}, {"Dstep.z3", z[2], 16384},
                  {"Dstep.z4", z[3], 8192},  {"Dstep.zl1", zl1, 512},    {"Dstep.zl2", zl2, 512},
@@ -197,8 +206,14 @@ int D32::backward(bool want_wgrad, bool want_dx) {
   const float scale = drop_scale, eval_scale = spatial_eval;
   ConvLEnv& e = n->env;
   FG_TRY(pairs.reset(c));
+  // option bwd_streams: the weight gradients of D.L3 to D.C2 (and the bias gradients of the Linear layers) on the wgrad
+  // stream, beside the data-gradient chain; each reads only its layer's input split and own dY (dY split, dzl2 /
+  // dzl1), which the chain leaves alone until the join at the end.  D.C1's stays on the chain: nothing follows it there.
+  const bool side = want_wgrad && wgrad_async(c, e);
   // L3
   if (want_wgrad) {
+    OnWgradStream ws(e, side);
+    FG_TRY(ws.r);
     ScopedTimer tm(c, "D.L3.wgrad");
     FG_TRY(k_gemv_wgrad_add(c, hl2, dlogit, G + L.L3W, G + L.L3b, B, 512));
   }
@@ -211,34 +226,37 @@ int D32::backward(bool want_wgrad, bool want_dx) {
   float* GD = want_wgrad ? G : nullptr;
   {
     AmaxInto am(c, DL2.sdy, &dy.amax_ready);
-    FG_TRY(k_lin_act_drop_bwd(c, dh, zl2, P + L.a6, m, 1472, scale, dzl, want_wgrad ? G + L.a6 : nullptr, B, 512));
+    FG_TRY(k_lin_act_drop_bwd(c, dh, zl2, P + L.a6, m, 1472, scale, dzl2, want_wgrad ? G + L.a6 : nullptr, B, 512));
   }
-  FG_TRY(keep_bwd(1, dzl, B));
-  FG_TRY(convl_bwd(e, DL2, hl1, dzl, GD, dh, B));
+  FG_TRY(keep_bwd(1, dzl2, B));
+  FG_TRY(convl_bwd(e, DL2, hl1, dzl2, GD, dh, B, side));
   FG_TRY(keep_bwd(2, dh, B));
   {
     AmaxInto am(c, DL1.sdy, &dy.amax_ready);
-    FG_TRY(k_lin_act_drop_bwd(c, dh, zl1, P + L.a5, m, 960, scale, dzl, want_wgrad ? G + L.a5 : nullptr, B, 512));
+    FG_TRY(k_lin_act_drop_bwd(c, dh, zl1, P + L.a5, m, 960, scale, dzl1, want_wgrad ? G + L.a5 : nullptr, B, 512));
   }
-  FG_TRY(keep_bwd(3, dzl, B));
-  FG_TRY(convl_bwd(e, DL1, p[3], dzl, GD, dp, B));
+  FG_TRY(keep_bwd(3, dzl1, B));
+  FG_TRY(convl_bwd(e, DL1, p[3], dzl1, GD, dp, B, side));
   for (int i = 3; i >= 0; --i) {
     const int H = kDhw[i];
     FG_TRY(keep_bwd(4 + 2 * (3 - i), dp, B));  // "Dbwd.dp<i+1>": the input of layer i's act/pool backward
     // dz and, for the tensor-core layers, its TF32 split in one pass, + the conv bias gradient (column sums of dz)
-    dy.split_ready = convl_tc_bwd(c, Dc[i]) && !tc_f16(c);
+    ConvL& Li = Dc[i];
+    dy.split_ready = convl_tc_bwd(c, Li) && !tc_f16(c);
     dy.bias_ready = want_wgrad;
+    float *dy_hi = Li.dy_hi ? Li.dy_hi : dy.hi, *dy_lo = Li.dy_lo ? Li.dy_lo : dy.lo;
     {
-      AmaxInto am(c, Dc[i].sdy, &dy.amax_ready);
+      AmaxInto am(c, Li.sdy, &dy.amax_ready);
       FG_TRY(k_d_act_pool_bwd(c, dp, z[i], P + L.ca[i], m, kDmoff[i], eval_scale, dz, want_wgrad ? G + L.ca[i] : nullptr, B,
-                              H, H, kDcout[i], dy.split_ready ? dy.hi : nullptr, dy.split_ready ? dy.lo : nullptr,
+                              H, H, kDcout[i], dy.split_ready ? dy_hi : nullptr, dy.split_ready ? dy_lo : nullptr,
                               want_wgrad ? G + L.cb[i] : nullptr));
     }
     FG_TRY(keep_bwd(5 + 2 * (3 - i), dz, B));
     float* din = i > 0 ? dp : want_dx ? dx : nullptr;
-    FG_TRY(convl_bwd(e, Dc[i], i == 0 ? x : p[i - 1], dz, GD, din, B));
+    // off the tensor cores the weight gradient reads dz, which the next layer overwrites: on the chain then
+    FG_TRY(convl_bwd(e, Li, i == 0 ? x : p[i - 1], dz, GD, din, B, side && i > 0 && convl_tc_wgrad(c, Li)));
   }
-  return FG_OK;
+  return wgrad_join(e);
 }
 
 void D32::debug_rows(std::vector<DebugTensor>& ents) const {

@@ -51,6 +51,9 @@ int gan_alloc(UpsGan& n, fg_ctx* c, const GanDesc& d, std::unique_ptr<GanD> D, f
   n.g_ws = std::max<size_t>(36 * 256 * 128, d.g.l1_kpad ? S * S / 16 * 128 * (d.g.l1_kpad + kNoiseDim) : 0);
   FG_TRY(n.D->alloc());
   FG_TRY(gen_alloc(e, n.G, d.g));
+  // the layer scratch of the weight gradients on the wgrad stream (option bwd_streams): G.C3's and those of the 32x32
+  // D's tensor-core layers, the largest D.C4's 9 x 512 x 256
+  FG_TRY(convl_dalloc(e, &e.ws_w, std::max<size_t>(n.g_ws, 9 * 512 * 256)));
   n.env_f.c = c;
   n.env_f.maxB = c->maxB / 2;
   n.env_f.allocs = &n.allocs;

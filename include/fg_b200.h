@@ -88,7 +88,9 @@ int fg_sync(fg_ctx* ctx);
  * step's pre-activations of fg_train_step as "Dstep.*" debug tensors), "edge_impl" / "bn_epilogue"
  * (0 selects the round-1 kernels for the 3-channel convolutions / a separate BatchNorm statistics
  * pass: cross-checks), "params_dirty" (re-pack weights
- * after writing through fg_params_ptr); unknown keys return FG_ERR_INVALID
+ * after writing through fg_params_ptr), "bwd_streams" (1, the default: the weight gradients of the 32x32 D
+ * and of G.C3 and G.C1 run on a second stream beside the data-gradient chain of the backward, same bits; 0: one
+ * stream); unknown keys return FG_ERR_INVALID
  *
  * Read-only keys of fg_get_option: which kernel the last fg_conv2d_* / fg_scu_* / fg_linear_* call launched
  * (a call launches one: forward, data gradient or weight gradient; fg_linear_backward with both dx and dw
