@@ -344,6 +344,7 @@ int64_t fg_get_option(fg_ctx* c, const char* key) {
   if (!strcmp(key, "last_conv_tile_n")) return c->last_conv_tile_n;
   if (!strcmp(key, "last_conv_format")) return c->last_conv_format;
   if (!strcmp(key, "last_conv_splits")) return c->last_conv_splits;
+  if (!strcmp(key, "step_graph_launches")) return c->graph_launches;
   return -1;
 }
 

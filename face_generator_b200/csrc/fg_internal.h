@@ -317,6 +317,7 @@ struct fg_ctx {
   // option "use_graph" (default 1): fg_train_step replays a captured CUDA graph of the step (launch overhead of ~200
   // kernels); keyed on everything a captured step bakes in, the seed is read from device memory
   int use_graph = 1, graph_epoch = 0;
+  int64_t graph_launches = 0;  // steps run as a launch of a captured graph (fg_get_option "step_graph_launches")
   uint64_t* seed_dev = nullptr;
   cudaStream_t comm_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;

@@ -320,6 +320,7 @@ int net_graph_run(fg_ctx* c, NetPair& p, int B, const void* hyper, size_t hyper_
   }
   FG_CUDA(cudaGraphLaunch(e->exec, c->stream));
   c->launches += e->launches;
+  c->graph_launches++;
   p.G_pack = p.D_pack = -1;
   return FG_OK;
 }

@@ -102,7 +102,9 @@ int fg_sync(fg_ctx* ctx);
  *                        EDGE_EXPAND: N (outputs)  SIMT / SIMT_FLATK / WGRAD_SIMT: TN (columns per thread)
  *   "last_conv_format"   0 fp32 FFMA, 1 3xTF32 tensor cores, 2 3xFP16 tensor cores
  *   "last_conv_splits"   K splits of a weight gradient (1: unsplit, written straight to its output);
- *                        1 for every other kernel                                                   */
+ *                        1 for every other kernel
+ * and how many train steps on this context, of any of its nets, ran as a launch of a captured CUDA graph:
+ *   "step_graph_launches"                                                                             */
 enum {
   FG_KERNEL_NONE = 0,
   FG_KERNEL_TAPCONV = 1,      /* wgmma forward / data gradient (tapconv_tc_kernel)                   */
