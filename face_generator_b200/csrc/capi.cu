@@ -137,17 +137,14 @@ int fg_create(fg_ctx** out, int device, int max_batch, int channels) {
 int64_t fg_disc_param_count(int disc, int channels) {
   if (channels != 1 && channels != 3) return -1;
   if (disc == FG_DISC_D32B) return fg_param_count(FG_NET_D, channels);
-  if (disc == FG_DISC_D16_D) return fg_s16_param_count(FG_NET_D, channels);
   return dbr_param_count(disc, channels);
 }
 int fg_disc_mask_per_sample(int disc) {
   if (disc == FG_DISC_D32B) return kMaskPerSample;
-  if (disc == FG_DISC_D16_D) return fg_s16_mask_per_sample();
   return dbr_mask_per_sample(disc);
 }
 int fg_disc_side(int disc) {
   if (disc == FG_DISC_D32B) return 32;
-  if (disc == FG_DISC_D16_D) return 16;
   return dbr_side(disc);
 }
 

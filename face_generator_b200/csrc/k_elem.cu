@@ -17,25 +17,6 @@ __device__ __forceinline__ int perm_idx(int j, int A, int S) {
   return (j % S) * A + (j / S);
 }
 
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-// block-wide sum (blockDim.x multiple of 32, <= 1024); result valid in thread 0
-__device__ __forceinline__ double block_sum(double v) {
-  __shared__ double red[32];
-  __syncthreads();
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    v = threadIdx.x < (blockDim.x + 31) / 32 ? red[threadIdx.x] : 0.0;
-    v = warp_sum(v);
-  }
-  return v;
-}
-
 __global__ void fill_kernel(float* p, float v, int64_t n) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = v;
 }

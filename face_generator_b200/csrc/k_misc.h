@@ -19,10 +19,6 @@ int k_join_to_nhwc(fg_ctx* c, const float* noise_nchw, const float* cond_nchw, f
 int k_add(fg_ctx* c, const float* a, const float* b, float* out, int64_t n);
 int k_maxpool2_fwd(fg_ctx* c, const float* h, float* p, int B, int H, int W, int C);                  // H,W: input size
 int k_maxpool2_bwd(fg_ctx* c, const float* dp, const float* h, float* dh, int B, int H, int W, int C);
-// a stride-2 "same" convolution as the stride-1 one sampled at the even pixels (nets_s16.cu): x [B][H][W][C] ->
-// y [B][H/2][W/2][C], and its adjoint (zeros at the odd pixels); H, W: the stride-1 size
-int k_subsample2(fg_ctx* c, const float* x, float* y, int B, int H, int W, int C);
-int k_zero_insert2(fg_ctx* c, const float* dy, float* dx, int B, int H, int W, int C);
 // y = x * mask * scale; mask element order is the reference's NCHW flattening: masks[b*stride + moff + ch*HW + q]
 int k_dropout_nhwc(fg_ctx* c, const float* x, const float* masks, int64_t stride, int moff, int HW, int C, float scale,
                    float* y, int B);

@@ -26,6 +26,25 @@ __device__ __forceinline__ double ordered_sum(const double* ws, int rows, int64_
 __device__ __forceinline__ void ordered_release(unsigned* ticket) {
   if (threadIdx.x == 0 && threadIdx.y == 0 && threadIdx.z == 0) *ticket = 0;
 }
+__device__ __forceinline__ double warp_sum(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+// block-wide sum (blockDim.x multiple of 32, <= 1024): a xor tree over the lanes, then over the warp partials; result
+// valid in thread 0
+__device__ __forceinline__ double block_sum(double v) {
+  __shared__ double red[32];
+  __syncthreads();
+  v = warp_sum(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    v = threadIdx.x < (blockDim.x + 31) / 32 ? red[threadIdx.x] : 0.0;
+    v = warp_sum(v);
+  }
+  return v;
+}
 // sum over a block of 256 threads in a fixed order (lanes, then warps); valid in thread 0
 __device__ __forceinline__ double block_sum256(double v) {
   __shared__ double red[8];

@@ -1,14 +1,18 @@
-// The branched discriminators of models.lua that create_D does not pick: create_D32 (:322-376) at 32x32 and
-// create_D16 (:110-159), create_D16_b (:161-216), create_D16_c (:218-277) at 16x16.  Each is
-//   ConcatTable{fine conv branch (3x3), coarse conv branch (5x5), dense branch} -> JoinTable(2) -> Linear -> PReLU
-//   -> Dropout -> Linear(1) -> Sigmoid
+// The branched discriminators of models.lua: create_D32 (:322-376) at 32x32 and create_D16_d (:279-316, the --scale 16
+// default), create_D16 (:110-159), create_D16_b (:161-216), create_D16_c (:218-277) at 16x16.  Each is
+//   ConcatTable{branch, ...} -> JoinTable(2) [-> Linear -> PReLU -> Dropout] -> Linear(1) -> Sigmoid
 // and differs from the others only in data: one descriptor (DbrDesc) per net, one GanD type (DBr) built from it.
-//   conv branch : conv (PReLU) [MaxPool(2,2)] ... SpatialDropout View Linear PReLU [Dropout] [Linear PReLU]
-//   dense branch: View(C*S*S) Linear(.., 1024) PReLU Dropout Linear(1024, 1024) PReLU
-// Every convolution and Linear is a ConvL (convl.h) through the shared dispatch; a stride-2 convolution runs at stride 1
-// and is subsampled, as D16_d does (nets_s16.cu).  The elementwise stages are one kernel pair: PReLU -> optional 2x2
-// max pooling -> optional (spatial) dropout forward, writing the window's arg-max, and its backward, which reduces
-// the PReLU slope gradient in a fixed order (k_ordered.cuh), so a step stays bit-reproducible.
+//   conv branch : conv (PReLU) [MaxPool(2,2) | AvgPool(2,2)] ... SpatialDropout View Linear PReLU [Dropout] [Linear PReLU]
+//   dense branch: View(C*S*S) Linear PReLU Dropout Linear PReLU
+// create_D32 and create_D16 / _b / _c have a fine (3x3) and a coarse (5x5) conv branch, a dense branch and a hidden
+// head; create_D16_d has one conv branch, a dense branch and no hidden head.
+// Every convolution and Linear is a ConvL (convl.h) through the shared dispatch.  A stride-2 "same" convolution is the
+// stride-1 one sampled at the even pixels: forward = stride-1 kernel + subsample, backward = the stride-1 dgrad / wgrad
+// of dY with zeros inserted at the odd pixels.  That is exact (the inserted zeros contribute nothing) and keeps the
+// layer on the tensor cores.  The elementwise stages are one kernel pair: PReLU -> optional 2x2 max pooling -> optional
+// (spatial) dropout forward, writing the window's arg-max, and its backward, which reduces the PReLU slope gradient in
+// a fixed order (k_ordered.cuh), so a step stays bit-reproducible.  A 2x2 average pooling runs after its stage's PReLU
+// as a kernel of its own.
 #include <deque>
 #include <string>
 
@@ -21,13 +25,21 @@ namespace {
 constexpr float kP = 0.5f;  // nn.SpatialDropout() / nn.Dropout() default probability
 
 // ---- descriptor --------------------------------------------------------------------------------------------------
+// the names a layer's timers and debug rows take instead of the generated "D.<branch>.*" ones (each may be null):
+// timer stem t (t.fwd / .dgrad / .wgrad), pre-activation z ("D.z", "Dstep.z"), stage output h ("D.h")
+struct DbrNames {
+  const char *t, *z, *h;
+};
+enum DbrPool { kNoPool, kMaxPool, kAvgPool };  // nn.SpatialMaxPooling(2, 2) / nn.SpatialAveragePooling(2, 2) after the PReLU
 struct DbrConvDesc {
   int cout, k, stride;
-  bool pool;  // nn.SpatialMaxPooling(2, 2) after the PReLU
+  DbrPool pool;
+  DbrNames nm;
 };
 struct DbrLinDesc {
   int out;
   bool drop;  // nn.Dropout() after the PReLU
+  DbrNames nm;
 };
 // a conv branch ends in nn.SpatialDropout() + View; a branch without convolutions is the dense branch (View of the image)
 struct DbrBranchDesc {
@@ -38,32 +50,45 @@ struct DbrBranchDesc {
   DbrLinDesc lin[2];
 };
 struct DbrDesc {
-  int disc, side;
+  int disc, side, nbr;
   DbrBranchDesc br[3];  // ConcatTable order
-  DbrLinDesc head;      // Linear(joint, head.out) PReLU Dropout; then Linear(head.out, 1)
+  // Linear(joint, head.out) PReLU Dropout, then Linear(head.out, 1); head.out 0: Linear(joint, 1) on the joint row
+  DbrLinDesc head;
 };
 
 constexpr DbrBranchDesc kDense = {"dense", 0, {}, 2, {{1024, true}, {1024, false}}};
 const DbrDesc kDescs[] = {
-    {FG_DISC_D32, 32,
-     {{"fine", 2, {{64, 3, 1, false}, {64, 3, 1, true}}, 1, {{1024, false}}},
-      {"coarse", 4, {{32, 5, 1, false}, {32, 5, 1, true}, {54, 5, 1, false}, {54, 5, 1, true}}, 2, {{1024, true}, {1024, false}}},
+    {FG_DISC_D32, 32, 3,
+     {{"fine", 2, {{64, 3, 1, kNoPool}, {64, 3, 1, kMaxPool}}, 1, {{1024, false}}},
+      {"coarse", 4, {{32, 5, 1, kNoPool}, {32, 5, 1, kMaxPool}, {54, 5, 1, kNoPool}, {54, 5, 1, kMaxPool}}, 2,
+       {{1024, true}, {1024, false}}},
       kDense},
      {1024, true}},
-    {FG_DISC_D16, 16,
-     {{"fine", 2, {{64, 3, 1, false}, {64, 3, 1, true}}, 1, {{1024, true}}},
-      {"coarse", 2, {{32, 5, 1, false}, {64, 5, 1, true}}, 1, {{1024, true}}},
+    {FG_DISC_D16_D, 16, 2,
+     {{"conv", 4,
+       {{128, 3, 1, kNoPool, {"s16.D.c1", "z1"}},
+        {128, 3, 1, kAvgPool, {"s16.D.c2", "z2", "p1"}},
+        {512, 3, 2, kNoPool, {"s16.D.c3", "z3"}},
+        {1024, 3, 2, kNoPool, {"s16.D.c4", "z4"}}},
+       1, {{1024, false, {"s16.D.F1", "zf"}}}},
+      {"dense", 0, {}, 2, {{128, true, {"s16.D.E1", "ze1"}}, {128, false, {"s16.D.E2", "ze2"}}}}},
+     {0, false}},
+    {FG_DISC_D16, 16, 3,
+     {{"fine", 2, {{64, 3, 1, kNoPool}, {64, 3, 1, kMaxPool}}, 1, {{1024, true}}},
+      {"coarse", 2, {{32, 5, 1, kNoPool}, {64, 5, 1, kMaxPool}}, 1, {{1024, true}}},
       kDense},
      {1024, true}},
-    {FG_DISC_D16_B, 16,
-     {{"fine", 4, {{64, 3, 1, false}, {64, 3, 1, false}, {128, 3, 1, false}, {128, 3, 2, false}}, 1, {{512, true}}},
-      {"coarse", 4, {{64, 5, 1, false}, {64, 5, 1, false}, {128, 5, 1, false}, {128, 5, 2, false}}, 1, {{512, true}}},
+    {FG_DISC_D16_B, 16, 3,
+     {{"fine", 4, {{64, 3, 1, kNoPool}, {64, 3, 1, kNoPool}, {128, 3, 1, kNoPool}, {128, 3, 2, kNoPool}}, 1, {{512, true}}},
+      {"coarse", 4, {{64, 5, 1, kNoPool}, {64, 5, 1, kNoPool}, {128, 5, 1, kNoPool}, {128, 5, 2, kNoPool}}, 1, {{512, true}}},
       kDense},
      {1024, true}},
-    {FG_DISC_D16_C, 16,
-     {{"fine", 5, {{64, 3, 1, false}, {64, 3, 1, false}, {128, 3, 1, false}, {128, 3, 2, false}, {512, 3, 2, false}}, 1,
+    {FG_DISC_D16_C, 16, 3,
+     {{"fine", 5,
+       {{64, 3, 1, kNoPool}, {64, 3, 1, kNoPool}, {128, 3, 1, kNoPool}, {128, 3, 2, kNoPool}, {512, 3, 2, kNoPool}}, 1,
        {{1024, false}}},
-      {"coarse", 5, {{64, 5, 1, false}, {64, 5, 1, false}, {128, 5, 1, false}, {128, 5, 2, false}, {512, 5, 2, false}}, 1,
+      {"coarse", 5,
+       {{64, 5, 1, kNoPool}, {64, 5, 1, kNoPool}, {128, 5, 1, kNoPool}, {128, 5, 2, kNoPool}, {512, 5, 2, kNoPool}}, 1,
        {{1024, false}}},
       kDense},
      {1024, true}},
@@ -169,7 +194,7 @@ __global__ void __launch_bounds__(256) dbr_act_bwd_kernel(const float* __restric
     }
   }
   if (!dslope) return;
-  s = block_sum256(s);
+  s = block_sum(s);
   if (threadIdx.x == 0) ws[blockIdx.x] = s;
   if (ordered_last_block(ticket)) {
     if (threadIdx.x == 0) *dslope += (float)ordered_sum(ws, gridDim.x, 1, 0);
@@ -177,7 +202,60 @@ __global__ void __launch_bounds__(256) dbr_act_bwd_kernel(const float* __restric
   }
 }
 
-// nn.JoinTable(2) of up to kMaxJoin inputs [B][w_k] -> [B][sum w_k], and the split of its gradient
+// nn.SpatialAveragePooling(2,2,2,2): x [B][H][W][C] -> y [B][H/2][W/2][C], and its adjoint
+__global__ void __launch_bounds__(256) avgpool2_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H,
+                                                           int W, int C) {
+  const int Ho = H / 2, Wo = W / 2;
+  GRID_STRIDE(i, (int64_t)B * Ho * Wo * C) {
+    const int ch = (int)(i % C);
+    int64_t r = i / C;
+    const int xo = (int)(r % Wo); r /= Wo;
+    const int yo = (int)(r % Ho);
+    const int64_t b = r / Ho;
+    const float* p = x + (((b * H + 2 * yo) * W + 2 * xo) * (int64_t)C + ch);
+    y[i] = 0.25f * ((p[0] + p[C]) + (p[(int64_t)W * C] + p[(int64_t)W * C + C]));
+  }
+}
+__global__ void __launch_bounds__(256) avgpool2_bwd_kernel(const float* __restrict__ dy, float* __restrict__ dx, int B, int H,
+                                                           int W, int C) {
+  const int Ho = H / 2, Wo = W / 2;
+  GRID_STRIDE(i, (int64_t)B * H * W * C) {
+    const int ch = (int)(i % C);
+    int64_t r = i / C;
+    const int xx = (int)(r % W); r /= W;
+    const int yy = (int)(r % H);
+    const int64_t b = r / H;
+    dx[i] = 0.25f * dy[((b * Ho + yy / 2) * Wo + xx / 2) * (int64_t)C + ch];
+  }
+}
+// the stride-2 sampling of a stride-1 "same" convolution output: y[b][yo][xo][c] = x[b][2yo][2xo][c] (H, W: the
+// stride-1 size), and its adjoint: dx[b][y][x][c] = (y, x both even) ? dy[b][y/2][x/2][c] : 0
+__global__ void __launch_bounds__(256) subsample2_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H,
+                                                         int W, int C) {
+  const int Ho = H / 2, Wo = W / 2;
+  GRID_STRIDE(i, (int64_t)B * Ho * Wo * C) {
+    const int ch = (int)(i % C);
+    int64_t r = i / C;
+    const int xo = (int)(r % Wo); r /= Wo;
+    const int yo = (int)(r % Ho);
+    const int64_t b = r / Ho;
+    y[i] = x[((b * H + 2 * yo) * W + 2 * xo) * (int64_t)C + ch];
+  }
+}
+__global__ void __launch_bounds__(256) zero_insert2_kernel(const float* __restrict__ dy, float* __restrict__ dx, int B, int H,
+                                                           int W, int C) {
+  const int Ho = H / 2, Wo = W / 2;
+  GRID_STRIDE(i, (int64_t)B * H * W * C) {
+    const int ch = (int)(i % C);
+    int64_t r = i / C;
+    const int xx = (int)(r % W); r /= W;
+    const int yy = (int)(r % H);
+    const int64_t b = r / H;
+    dx[i] = ((xx | yy) & 1) ? 0.f : dy[((b * Ho + yy / 2) * Wo + xx / 2) * (int64_t)C + ch];
+  }
+}
+
+// nn.JoinTable(2) of two or three inputs [B][w_k] -> [B][sum w_k] (w[2] = 0 for two), and the split of its gradient
 constexpr int kMaxJoin = 3;
 struct JoinArgs {
   float* p[kMaxJoin];
@@ -199,11 +277,12 @@ __global__ void __launch_bounds__(256) splitN_kernel(JoinArgs a, const float* __
 }
 
 // ---- the net -----------------------------------------------------------------------------------------------------
-// one PReLU [-> MaxPool(2,2)] [-> (spatial) dropout] stage on a [B][H][W][C] pre-activation z
+// one PReLU [-> MaxPool(2,2) | AvgPool(2,2)] [-> (spatial) dropout] stage on a [B][H][W][C] pre-activation z
 struct Act {
   int64_t a_off = 0;  // slope
   int H = 1, W = 1, C = 0, pool = 1;
-  int moff = -1;  // keep-flag offset in the sample's row; -1: no dropout
+  bool avg = false;  // pool 2 is an average: the PReLU (and dropout) into DBr::full, then the average into h
+  int moff = -1;     // keep-flag offset in the sample's row; -1: no dropout
   float train_scale = 1.f, eval_scale = 1.f;
   float *z = nullptr, *h = nullptr;
   uint8_t* code = nullptr;
@@ -225,10 +304,11 @@ struct DBr final : GanD {
   const DbrDesc& dd;
   int mask = 0;
   Branch br[3];
-  Layer head;
-  int64_t JW = 0, Jb = 0;  // the last Linear(head.out, 1)
-  int joint_w = 0;
-  float *zfull = nullptr, *joint = nullptr, *djoint = nullptr, *ga = nullptr, *gb = nullptr;
+  Layer head;             // when dd.head.out
+  int64_t JW = 0, Jb = 0;  // the last Linear(top_w, 1)
+  int joint_w = 0, top_w = 0;  // widths of the joint row and of the last Linear's input
+  // full: the stride-1 output of a stride-2 convolution, or the PReLU of an average-pooled stage before its pooling
+  float *full = nullptr, *joint = nullptr, *djoint = nullptr, *ga = nullptr, *gb = nullptr;
   bool train = true, valid = false;
   std::deque<std::string> names;  // timer and debug names (stable storage)
   std::vector<DebugTensor> rows;   // "D.*" of fg_*debug_tensor
@@ -240,11 +320,11 @@ struct DBr final : GanD {
   }
   std::vector<Layer*> layers() {
     std::vector<Layer*> v;
-    for (Branch& b : br) {
-      for (Layer& l : b.conv) v.push_back(&l);
-      for (Layer& l : b.lin) v.push_back(&l);
+    for (int k = 0; k < dd.nbr; ++k) {
+      for (Layer& l : br[k].conv) v.push_back(&l);
+      for (Layer& l : br[k].lin) v.push_back(&l);
     }
-    v.push_back(&head);
+    if (dd.head.out) v.push_back(&head);
     return v;
   }
   int64_t layout(int C) override;
@@ -267,24 +347,29 @@ int64_t DBr::layout(int C) {
   names.clear();
   int64_t o = 0;
   int m = 0;
-  auto linear = [&](Layer& l, const char* pre, int j, int cin, int cout, int cA, int cS) {
-    ConvL& L = l.L;
-    L.Cin = cin; L.Cout = cout; L.k = 1; L.H = 1;
-    L.cA = cA; L.cS = cS;  // View flattens [C][H][W]; ours is [H][W][C]
-    L.w_off = o; o += (int64_t)cout * cin;
-    L.b_off = o; o += cout;
-    l.act.a_off = o; o += 1;
-    l.act.C = cout;
-    L.tf = name(std::string(pre) + ".L" + std::to_string(j + 1) + ".fwd");
-    L.td = name(std::string(pre) + ".L" + std::to_string(j + 1) + ".dgrad");
-    L.tw = name(std::string(pre) + ".L" + std::to_string(j + 1) + ".wgrad");
+  auto timers = [&](ConvL& L, const char* t, const std::string& gen) {
+    const std::string s = t ? t : gen;
+    L.tf = name(s + ".fwd");
+    L.td = name(s + ".dgrad");
+    L.tw = name(s + ".wgrad");
   };
-  auto dropout = [&](Act& a, int width) {
-    a.moff = m;
-    m += width;
+  auto linear = [&](Layer& l, const std::string& pre, int j, int cin, const DbrLinDesc& ld, int cA, int cS) {
+    ConvL& L = l.L;
+    L.Cin = cin; L.Cout = ld.out; L.k = 1; L.H = 1;
+    L.cA = cA; L.cS = cS;  // View flattens [C][H][W]; ours is [H][W][C]
+    L.w_off = o; o += (int64_t)ld.out * cin;
+    L.b_off = o; o += ld.out;
+    l.act.a_off = o; o += 1;
+    l.act.C = ld.out;
+    timers(L, ld.nm.t, pre + ".L" + std::to_string(j + 1));
+    if (ld.drop) {  // nn.Dropout(): 1/(1-p) in training, identity in evaluation
+      l.act.moff = m;
+      m += ld.out;
+      l.act.train_scale = 1.f / (1.f - kP);
+    }
   };
   joint_w = 0;
-  for (int k = 0; k < 3; ++k) {
+  for (int k = 0; k < dd.nbr; ++k) {
     const DbrBranchDesc& bd = dd.br[k];
     Branch& b = br[k];
     const std::string pre = std::string("D.") + bd.name;
@@ -299,40 +384,31 @@ int64_t DBr::layout(int C) {
       L.w_off = o; o += (int64_t)cd.cout * cin * cd.k * cd.k;
       L.b_off = o; o += cd.cout;
       l.act.a_off = o; o += 1;
-      L.tf = name(pre + ".c" + std::to_string(i + 1) + ".fwd");
-      L.td = name(pre + ".c" + std::to_string(i + 1) + ".dgrad");
-      L.tw = name(pre + ".c" + std::to_string(i + 1) + ".wgrad");
+      timers(L, cd.nm.t, pre + ".c" + std::to_string(i + 1));
       l.stride = cd.stride;
       s /= cd.stride;
       l.act.H = l.act.W = s;
       l.act.C = cd.cout;
-      l.act.pool = cd.pool ? 2 : 1;
+      l.act.pool = cd.pool == kNoPool ? 1 : 2;
+      l.act.avg = cd.pool == kAvgPool;
       s /= l.act.pool;
       cin = cd.cout;
     }
     if (bd.nconv) {  // nn.SpatialDropout(): one flag per plane, no rescale in training, 1-p in evaluation
       Act& a = b.conv.back().act;
-      dropout(a, cin);
+      a.moff = m;
+      m += cin;
       a.eval_scale = 1.f - kP;
     }
-    for (int j = 0; j < bd.nlin; ++j) {
-      const int in = j ? bd.lin[j - 1].out : cin * s * s;
-      linear(b.lin[j], pre.c_str(), j, in, bd.lin[j].out, j ? 0 : cin, j ? 0 : s * s);
-      if (bd.lin[j].drop) {  // nn.Dropout(): 1/(1-p) in training, identity in evaluation
-        dropout(b.lin[j].act, bd.lin[j].out);
-        b.lin[j].act.train_scale = 1.f / (1.f - kP);
-      }
-    }
+    for (int j = 0; j < bd.nlin; ++j)
+      linear(b.lin[j], pre, j, j ? bd.lin[j - 1].out : cin * s * s, bd.lin[j], j ? 0 : cin, j ? 0 : s * s);
     b.out = bd.lin[bd.nlin - 1].out;
     joint_w += b.out;
   }
   head = Layer{};
-  linear(head, "D.head", 0, joint_w, dd.head.out, 0, 0);
-  if (dd.head.drop) {
-    dropout(head.act, dd.head.out);
-    head.act.train_scale = 1.f / (1.f - kP);
-  }
-  JW = o; o += dd.head.out;
+  if (dd.head.out) linear(head, "D.head", 0, joint_w, dd.head, 0, 0);
+  top_w = dd.head.out ? dd.head.out : joint_w;
+  JW = o; o += top_w;
   Jb = o; o += 1;
   mask = m;
   return o;
@@ -343,14 +419,15 @@ int DBr::alloc() {
   ConvLEnv& e = n->env;
   const size_t B = e.maxB, C = c->C, S = dd.side;
   // the scratch both nets share: the largest dY split and weight gradient of either net (G's needs from the trainer)
-  size_t dy = n->g_dy, ws = n->g_ws, g = B * S * S * C, full = 0;
+  size_t dy = n->g_dy, ws = n->g_ws, g = B * S * S * C, nfull = 0;
   for (Layer* l : layers()) {
     ConvL& L = l->L;
     const size_t P = B * L.H * L.H;
     dy = std::max(dy, P * L.Cout);
     ws = std::max(ws, (size_t)L.k * L.k * L.Cout * L.Cin);
     g = std::max(g, std::max(P * L.Cout, P * L.Cin));
-    if (l->stride == 2) full = std::max(full, P * L.Cout);
+    if (l->stride == 2) nfull = std::max(nfull, P * L.Cout);
+    if (l->act.avg) nfull = std::max(nfull, B * l->act.H * l->act.W * l->act.C);
     FG_TRY(convl_alloc(e, L));
   }
   FG_TRY(dalloc(&e.ws, ws));
@@ -358,41 +435,45 @@ int DBr::alloc() {
   FG_TRY(dalloc(&e.dy.lo, dy));
   FG_TRY(dalloc(&ga, g));
   FG_TRY(dalloc(&gb, g));
-  if (full) FG_TRY(dalloc(&zfull, full));
+  if (nfull) FG_TRY(dalloc(&full, nfull));
   FG_TRY(dalloc(&x, B * S * S * C));
   FG_TRY(dalloc(&dx, B * S * S * C));
   rows.clear();
   n->net.keep.clear();
-  for (int k = 0; k < 3; ++k) {
+  // a pre-activation's "D.*" row and "Dstep.*" keep entry: nm.z, else the generated name
+  auto zrow = [&](const DbrNames& nm, const std::string& gen, float* p, int64_t per) {
+    const std::string zn = nm.z ? nm.z : gen;
+    rows.push_back({name("D." + zn), p, per, 0});
+    n->net.keep.push_back({name("Dstep." + zn), p, per});
+  };
+  for (int k = 0; k < dd.nbr; ++k) {
+    const DbrBranchDesc& bd = dd.br[k];
     Branch& b = br[k];
-    const std::string pre = std::string("D.") + dd.br[k].name;
+    const std::string pre = std::string(bd.name) + ".";
     const float* in = x;
-    for (size_t i = 0; i < b.conv.size(); ++i) {
+    for (int i = 0; i < bd.nconv; ++i) {
       Layer& l = b.conv[i];
       Act& a = l.act;
       const int64_t zper = (int64_t)a.H * a.W * a.C;
+      const DbrNames& nm = bd.conv[i].nm;
       l.in = in;
       FG_TRY(dalloc(&a.z, B * zper));
       FG_TRY(dalloc(&a.h, B * a.out_per()));
-      if (a.pool == 2) {
+      if (a.pool == 2 && !a.avg) {
         float* q;
         FG_TRY(dalloc(&q, (B * a.out_per() + 3) / 4));
         a.code = reinterpret_cast<uint8_t*>(q);
       }
-      const std::string zn = pre + ".z" + std::to_string(i + 1);
-      rows.push_back({name(zn), a.z, zper, 0});
-      rows.push_back({name(pre + ".h" + std::to_string(i + 1)), a.h, a.out_per(), 0});
-      n->net.keep.push_back({name("Dstep." + zn.substr(2)), a.z, zper});
+      zrow(nm, pre + "z" + std::to_string(i + 1), a.z, zper);
+      rows.push_back({name("D." + (nm.h ? std::string(nm.h) : pre + "h" + std::to_string(i + 1))), a.h, a.out_per(), 0});
       in = a.h;
     }
-    for (size_t j = 0; j < b.lin.size(); ++j) {
+    for (int j = 0; j < bd.nlin; ++j) {
       Layer& l = b.lin[j];
       l.in = in;
       FG_TRY(dalloc(&l.act.z, B * l.act.C));
       FG_TRY(dalloc(&l.act.h, B * l.act.C));
-      const std::string zn = pre + ".zl" + std::to_string(j + 1);
-      rows.push_back({name(zn), l.act.z, l.act.C, 0});
-      n->net.keep.push_back({name("Dstep." + zn.substr(2)), l.act.z, l.act.C});
+      zrow(bd.lin[j].nm, pre + "zl" + std::to_string(j + 1), l.act.z, l.act.C);
       in = l.act.h;
     }
     FG_TRY(dalloc(&b.dsplit, B * b.out));
@@ -401,18 +482,20 @@ int DBr::alloc() {
   br[0].dxb = dx;
   FG_TRY(dalloc(&joint, B * joint_w));
   FG_TRY(dalloc(&djoint, B * joint_w));
-  head.in = joint;
-  FG_TRY(dalloc(&head.act.z, B * head.act.C));
-  FG_TRY(dalloc(&head.act.h, B * head.act.C));
+  rows.push_back({"D.joint", joint, joint_w, 0});
+  if (dd.head.out) {
+    head.in = joint;
+    FG_TRY(dalloc(&head.act.z, B * head.act.C));
+    FG_TRY(dalloc(&head.act.h, B * head.act.C));
+    zrow({}, "head.z", head.act.z, head.act.C);
+  }
   FG_TRY(dalloc(&logit, B));
   FG_TRY(dalloc(&out, B));
   FG_TRY(dalloc(&dlogit, B));
   FG_TRY(dalloc(&masks, B * mask));
-  rows.insert(rows.end(), {{"D.joint", joint, joint_w, 0}, {"D.head.z", head.act.z, head.act.C, 0},
-                           {"D.logit", logit, 1, 0}, {"D.out", out, 1, 0}, {"D.masks", masks, mask, 0},
+  rows.insert(rows.end(), {{"D.logit", logit, 1, 0}, {"D.out", out, 1, 0}, {"D.masks", masks, mask, 0},
                            {"D.dx", dx, (int64_t)(S * S * C), 0}});
-  n->net.keep.insert(n->net.keep.end(), {{"Dstep.head.z", head.act.z, head.act.C}, {"Dstep.logit", logit, 1},
-                                         {"Dstep.out", out, 1}});
+  n->net.keep.insert(n->net.keep.end(), {{"Dstep.logit", logit, 1}, {"Dstep.out", out, 1}});
   return FG_OK;
 }
 
@@ -421,27 +504,36 @@ int DBr::act_fwd(const Act& A, int Bn, bool training) {
   const float* keep = training && A.moff >= 0 ? masks : nullptr;
   const float es = training ? 1.f : A.eval_scale;
   const float* P = n->net.PD;
-  const int64_t nout = (int64_t)Bn * A.out_per();
-  if (A.pool == 2)
+  if (A.pool == 2 && !A.avg) {
+    const int64_t nout = (int64_t)Bn * A.out_per();
     dbr_act_fwd_kernel<2><<<grid_for(nout, 256), 256, 0, c->stream>>>(A.z, P + A.a_off, keep, mask, A.moff, A.train_scale,
                                                                        es, A.h, A.code, Bn, A.H, A.W, A.C);
-  else
-    dbr_act_fwd_kernel<1><<<grid_for(nout, 256), 256, 0, c->stream>>>(A.z, P + A.a_off, keep, mask, A.moff, A.train_scale,
-                                                                       es, A.h, nullptr, Bn, A.H, A.W, A.C);
+    LAUNCH_CHECK(c);
+    return FG_OK;
+  }
+  const int64_t nz = (int64_t)Bn * A.H * A.W * A.C;
+  dbr_act_fwd_kernel<1><<<grid_for(nz, 256), 256, 0, c->stream>>>(A.z, P + A.a_off, keep, mask, A.moff, A.train_scale, es,
+                                                                   A.avg ? full : A.h, nullptr, Bn, A.H, A.W, A.C);
   LAUNCH_CHECK(c);
+  if (A.avg) {
+    avgpool2_fwd_kernel<<<grid_for((int64_t)Bn * A.out_per(), 256), 256, 0, c->stream>>>(full, A.h, Bn, A.H, A.W, A.C);
+    LAUNCH_CHECK(c);
+  }
   return FG_OK;
 }
 
+// dy: the gradient of A.h, or of the PReLU's full-size output on an average-pooled stage
 int DBr::act_bwd(const Act& A, const float* dy, float* dz, float* G, int Bn) {
   fg_ctx* c = n->c;
   const float* keep = train && A.moff >= 0 ? masks : nullptr;
   const float es = train ? 1.f : A.eval_scale;
   const float* P = n->net.PD;
   float* ds = G ? G + A.a_off : nullptr;
-  const int64_t nout = (int64_t)Bn * A.out_per();
+  const bool max2 = A.pool == 2 && !A.avg;
+  const int64_t nout = (int64_t)Bn * (max2 ? A.out_per() : (int64_t)A.H * A.W * A.C);
   const int grid = grid_for(nout, 256, 132 * 8);
   FG_TRY(red_check(c, grid, 1));
-  if (A.pool == 2)
+  if (max2)
     dbr_act_bwd_kernel<2><<<grid, 256, 0, c->stream>>>(dy, A.z, A.code, P + A.a_off, keep, mask, A.moff, A.train_scale, es,
                                                        dz, ds, Bn, A.H, A.W, A.C, c->red_ws, c->red_ticket);
   else
@@ -455,20 +547,22 @@ int DBr::forward(const float* xin, int Bn, bool training, const fg_hyper*) {
   fg_ctx* c = n->c;
   ConvLEnv& e = n->env;
   FG_REQUIRE(Bn >= 1 && Bn <= e.maxB, "D forward: batch %d out of range [1,%d]", Bn, e.maxB);
+  std::vector<ConvL*> Ls;
+  for (Layer* l : layers()) Ls.push_back(&l->L);
+  FG_TRY(gan_pack_D(*n, Ls));
   const float* P = n->net.PD;
-  if (n->net.D_pack != pack_key(c)) {
-    for (Layer* l : layers()) FG_TRY(convl_pack(c, l->L, P));
-    n->net.D_pack = pack_key(c);
-  }
   const int S = dd.side;
   if (xin != x) FG_CUDA(cudaMemcpyAsync(x, xin, sizeof(float) * (size_t)Bn * S * S * c->C, cudaMemcpyDeviceToDevice, c->stream));
   JoinArgs ja{};
-  for (int k = 0; k < 3; ++k) {
+  for (int k = 0; k < dd.nbr; ++k) {
     Branch& b = br[k];
     for (Layer& l : b.conv) {
       if (l.stride == 2) {  // stride 1, then every other pixel
-        FG_TRY(convl_fwd(e, l.L, l.in, P, zfull, Bn));
-        FG_TRY(k_subsample2(c, zfull, l.act.z, Bn, l.L.H, l.L.H, l.L.Cout));
+        const int H = l.L.H, Co = l.L.Cout;
+        FG_TRY(convl_fwd(e, l.L, l.in, P, full, Bn));
+        subsample2_kernel<<<grid_for((int64_t)Bn * (H / 2) * (H / 2) * Co, 256), 256, 0, c->stream>>>(full, l.act.z, Bn, H,
+                                                                                                      H, Co);
+        LAUNCH_CHECK(c);
       } else {
         FG_TRY(convl_fwd(e, l.L, l.in, P, l.act.z, Bn));
       }
@@ -483,16 +577,20 @@ int DBr::forward(const float* xin, int Bn, bool training, const fg_hyper*) {
   }
   joinN_kernel<<<grid_for((int64_t)Bn * joint_w, 256), 256, 0, c->stream>>>(ja, joint, Bn, joint_w);
   LAUNCH_CHECK(c);
-  FG_TRY(convl_fwd(e, head.L, joint, P, head.act.z, Bn));
-  FG_TRY(act_fwd(head.act, Bn, training));
-  FG_TRY(k_gemv_fwd(c, head.act.h, P + JW, P + Jb, logit, Bn, head.act.C));
+  const float* top = joint;
+  if (dd.head.out) {
+    FG_TRY(convl_fwd(e, head.L, joint, P, head.act.z, Bn));
+    FG_TRY(act_fwd(head.act, Bn, training));
+    top = head.act.h;
+  }
+  FG_TRY(k_gemv_fwd(c, top, P + JW, P + Jb, logit, Bn, top_w));
   B = Bn;
   train = training;
   valid = true;
   return FG_OK;
 }
 
-// want_dx: the image gradient is the sum of the three branches' (nn.ConcatTable backward), in branch order
+// want_dx: the image gradient is the sum of the branches' (nn.ConcatTable backward), in branch order
 int DBr::backward(bool want_wgrad, bool want_dx) {
   fg_ctx* c = n->c;
   ConvLEnv& e = n->env;
@@ -502,19 +600,23 @@ int DBr::backward(bool want_wgrad, bool want_dx) {
   }
   const float* P = n->net.PD;
   float* G = want_wgrad ? n->net.gD : nullptr;
-  const int hw = head.act.C;
-  if (G) FG_TRY(k_gemv_wgrad_add(c, head.act.h, dlogit, G + JW, G + Jb, B, hw));
-  FG_TRY(k_gemv_dgrad(c, dlogit, P + JW, ga, B, hw));
-  FG_TRY(act_bwd(head.act, ga, gb, G, B));
-  FG_TRY(convl_bwd(e, head.L, joint, gb, G, djoint, B));
+  if (dd.head.out) {
+    if (G) FG_TRY(k_gemv_wgrad_add(c, head.act.h, dlogit, G + JW, G + Jb, B, top_w));
+    FG_TRY(k_gemv_dgrad(c, dlogit, P + JW, ga, B, top_w));
+    FG_TRY(act_bwd(head.act, ga, gb, G, B));
+    FG_TRY(convl_bwd(e, head.L, joint, gb, G, djoint, B));
+  } else {
+    if (G) FG_TRY(k_gemv_wgrad_add(c, joint, dlogit, G + JW, G + Jb, B, top_w));
+    FG_TRY(k_gemv_dgrad(c, dlogit, P + JW, djoint, B, top_w));
+  }
   JoinArgs ja{};
-  for (int k = 0; k < 3; ++k) {
+  for (int k = 0; k < dd.nbr; ++k) {
     ja.p[k] = br[k].dsplit;
     ja.w[k] = br[k].out;
   }
   splitN_kernel<<<grid_for((int64_t)B * joint_w, 256), 256, 0, c->stream>>>(ja, djoint, B, joint_w);
   LAUNCH_CHECK(c);
-  for (int k = 0; k < 3; ++k) {
+  for (int k = 0; k < dd.nbr; ++k) {
     Branch& b = br[k];
     const float* cur = b.dsplit;  // the gradient of the current stage's output
     float *t0 = ga, *t1 = gb;     // ping-pong: a stage reads cur and writes the other buffer
@@ -530,23 +632,29 @@ int DBr::backward(bool want_wgrad, bool want_dx) {
     }
     for (int i = (int)b.conv.size() - 1; i >= 0; --i) {
       Layer& l = b.conv[i];
+      const Act& a = l.act;
+      if (a.avg) {  // the average's adjoint: the gradient of the PReLU's full-size output
+        float* dfull = next();
+        avgpool2_bwd_kernel<<<grid_for((int64_t)B * a.H * a.W * a.C, 256), 256, 0, c->stream>>>(cur, dfull, B, a.H, a.W, a.C);
+        LAUNCH_CHECK(c);
+        cur = dfull;
+      }
       float* dz = next();
-      FG_TRY(act_bwd(l.act, cur, dz, G, B));
+      FG_TRY(act_bwd(a, cur, dz, G, B));
       if (l.stride == 2) {  // the adjoint of the subsample: zeros at the odd pixels
-        float* full = dz == t0 ? t1 : t0;
-        FG_TRY(k_zero_insert2(c, dz, full, B, l.L.H, l.L.H, l.L.Cout));
-        dz = full;
+        const int H = l.L.H, Co = l.L.Cout;
+        float* dzfull = dz == t0 ? t1 : t0;
+        zero_insert2_kernel<<<grid_for((int64_t)B * H * H * Co, 256), 256, 0, c->stream>>>(dz, dzfull, B, H, H, Co);
+        LAUNCH_CHECK(c);
+        dz = dzfull;
       }
       float* din = i == 0 ? (want_dx ? b.dxb : nullptr) : (dz == t0 ? t1 : t0);
       FG_TRY(convl_bwd(e, l.L, l.in, dz, G, din, B));
       cur = din;
     }
   }
-  if (want_dx) {
-    const int64_t nx = (int64_t)B * dd.side * dd.side * c->C;
-    FG_TRY(k_add(c, dx, br[1].dxb, dx, nx));
-    FG_TRY(k_add(c, dx, br[2].dxb, dx, nx));
-  }
+  if (want_dx)
+    for (int k = 1; k < dd.nbr; ++k) FG_TRY(k_add(c, dx, br[k].dxb, dx, (int64_t)B * dd.side * dd.side * c->C));
   return FG_OK;
 }
 }  // namespace
@@ -557,8 +665,7 @@ int dbr_side(int disc) {
 }
 int64_t dbr_param_count(int disc, int C) {
   const DbrDesc* d = find_desc(disc);
-  if (!d || (C != 1 && C != 3)) return -1;
-  return DBr(*d).layout(C);
+  return d ? DBr(*d).layout(C) : -1;
 }
 int dbr_mask_per_sample(int disc) {
   const DbrDesc* d = find_desc(disc);

@@ -75,7 +75,7 @@ void gan_free(UpsGan& n) {
   n.allocs.clear();
 }
 
-int gan_pack_D(UpsGan& n, std::initializer_list<ConvL*> layers) {
+int gan_pack_D(UpsGan& n, const std::vector<ConvL*>& layers) {
   if (n.net.D_pack == pack_key(n.c)) return FG_OK;
   for (ConvL* L : layers) FG_TRY(convl_pack(n.c, *L, n.net.PD));
   n.net.D_pack = pack_key(n.c);

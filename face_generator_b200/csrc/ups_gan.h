@@ -34,8 +34,9 @@ struct GanDesc {
   bool overlap;   // StepNets::overlap: option dp_overlap may run D's update next to the following G forward
 };
 
-// The branched discriminators of models.lua (nets_dbr.cu): create_D32 at side 32, create_D16 / _b / _c at side 16.
-// disc is FG_DISC_*; every function refuses (side 0, count / width -1, null D) a value that is not one of those four.
+// The branched discriminators of models.lua (nets_dbr.cu): create_D32 at side 32, create_D16_d and create_D16 / _b / _c
+// at side 16.  disc is FG_DISC_*; every function refuses (side 0, count / width -1, null D) a value that is not one of
+// those five.  dbr_param_count takes any channel count C.
 int dbr_side(int disc);
 int64_t dbr_param_count(int disc, int C);
 int dbr_mask_per_sample(int disc);
@@ -69,7 +70,7 @@ struct UpsGan {
 // for one of n's own
 int gan_alloc(UpsGan& n, fg_ctx* c, const GanDesc& d, std::unique_ptr<GanD> D, float* io);
 void gan_free(UpsGan& n);  // the pair's graphs and mirror, D, and every buffer on n.allocs
-int gan_pack_D(UpsGan& n, std::initializer_list<ConvL*> layers);  // D's layers, unless net.D_pack is the current pack_key()
+int gan_pack_D(UpsGan& n, const std::vector<ConvL*>& layers);  // D's layers, unless net.D_pack is the current pack_key()
 // d_iters D iterations + g_iters G iterations of the loop body (pair_train_step) on inputs stacked per iteration:
 // real [B/2][C][S][S], noise_D [B/2][100] and noise_G [B][100], masks_D / masks_G [B][mask] (may be null), for entry `what`
 int gan_train_step_iters(UpsGan& n, const char* what, const fg_hyper* h, int B, int d_iters, int g_iters, const float* real,

@@ -4,7 +4,8 @@
 seeded train steps, then one G forward / G backward / D forward / D backward call.  The step modes are the
 single-iteration entries, the *_iters / *_dataset_iters entries at 2 D and 2 G iterations ("iters2x2"), and the single
 entries with option debug_keep, saving every Dstep.* tensor after each step ("debug_keep").  The coarse-to-fine nets
-also run at fine sizes 16 and 64.  It writes every piece of state as .npy under
+also run at fine sizes 16 and 64.  The dbr group runs models.lua's other discriminators at batch 256: create_D32 on
+the 32x32 nets, create_D16 / _b / _c on the --scale 16 nets.  It writes every piece of state as .npy under
 --out/<case>/: parameters, gradients, optimizer m / v / t, BatchNorm running state, the step statistics, the outputs
 of those calls and the generator's debug tensors, plus the kernel launches of each step (launches.json).  The L-op
 convolutions (fg_conv2d_*) with the 3xFP16 split are one more case.  The denoiser and the autoencoder run 6 seeded train
@@ -14,7 +15,7 @@ that differs and the launches per step of both builds; a case differs when eithe
 
 One build per process: both libraries export the same symbols.
 
-usage:  python profiles/ab_state.py run --lib face_generator_b200/libfg_b200.so --out /tmp/ab/new [--only 32,s16,c2f,lop,dn,ae]
+usage:  python profiles/ab_state.py run --lib face_generator_b200/libfg_b200.so --out /tmp/ab/new [--only 32,s16,dbr,c2f,lop,dn,ae]
         python profiles/ab_state.py compare /tmp/ab/old /tmp/ab/new
 """
 import argparse
@@ -80,19 +81,22 @@ def n_rows(mode):
     return [ITERS] if mode == "iters2x2" else []
 
 
-def case_32(B, opts, imgs, mode="step"):
+def case_32(B, opts, imgs, mode="step", discriminator=None):
     import face_generator_b200 as fg
     from face_generator_b200 import layouts as LY
     from face_generator_b200.dataset import DeviceDataset
     from face_generator_b200.lib import NET_D, NET_G
     rng = np.random.default_rng(7)
-    ctx = fg.Context(0, max_batch=B, channels=C)
+    ctx = fg.Context(0, max_batch=B, channels=C, **({"discriminator": discriminator} if discriminator else {}))
     for k, v in opts.items():
         ctx.set_option(k, v)
     if mode == "debug_keep":
         ctx.set_option("debug_keep", 1)
     ctx.set_params(NET_G, LY.trained_like_init(LY.G_layout(C), rng))
-    ctx.set_params(NET_D, LY.trained_like_init(LY.D_layout(C), rng, 1.4))
+    if discriminator:
+        ctx.set_params(NET_D, f32(rng.standard_normal(ctx.count(NET_D)) * 0.02))
+    else:
+        ctx.set_params(NET_D, LY.trained_like_init(LY.D_layout(C), rng, 1.4))
     ds = DeviceDataset(ctx, imgs)
     h = fg.hyper_default()
     out = {}
@@ -124,7 +128,7 @@ def case_32(B, opts, imgs, mode="step"):
     return out, launches
 
 
-def case_s16(B, opts, imgs, mode="step"):
+def case_s16(B, opts, imgs, mode="step", discriminator=None):
     import face_generator_b200 as fg
     from face_generator_b200.dataset import DeviceDataset
     from face_generator_b200.lib import NET_D, NET_G
@@ -134,7 +138,7 @@ def case_s16(B, opts, imgs, mode="step"):
         ctx.set_option(k, v)
     if mode == "debug_keep":
         ctx.set_option("debug_keep", 1)
-    net = fg.S16(ctx)
+    net = fg.S16(ctx, **({"discriminator": discriminator} if discriminator else {}))
     net.set_params(NET_G, f32(rng.standard_normal(net.count(NET_G)) * 0.02))
     net.set_params(NET_D, f32(rng.standard_normal(net.count(NET_D)) * 0.02))
     ds = DeviceDataset(ctx, imgs)
@@ -329,6 +333,10 @@ def run(args):
             cases.append(("s16.B256.%s" % mode, lambda m=mode: case_s16(256, {}, imgs, m)))
         if "c2f" in only:
             cases.append(("c2f.B256.%s" % mode, lambda m=mode: case_c2f(256, imgs, 32, m)))
+    if "dbr" in only:  # models.lua's other discriminators, on the 32x32 and the --scale 16 nets
+        cases.append(("dbr.D32.B256", lambda: case_32(256, {}, imgs, discriminator="create_D32")))
+        cases += [("dbr.%s.B256" % d[7:], lambda d=d: case_s16(256, {}, imgs, discriminator=d))
+                  for d in ("create_D16", "create_D16_b", "create_D16_c")]
     if "c2f" in only:
         cases.append(("c2f.B256.default", lambda: case_c2f(256, imgs)))
         cases += [("c2f%d.B256.default" % S, lambda S=S: case_c2f(256, imgs, S)) for S in (16, 64)]
@@ -387,7 +395,7 @@ def main():
     r = sub.add_parser("run")
     r.add_argument("--lib", required=True)
     r.add_argument("--out", required=True)
-    r.add_argument("--only", default="32,s16,c2f,lop,dn,ae")
+    r.add_argument("--only", default="32,s16,dbr,c2f,lop,dn,ae")
     c = sub.add_parser("compare")
     c.add_argument("A")
     c.add_argument("B")
