@@ -10,7 +10,8 @@ import ctypes as C
 
 import numpy as np
 
-from .lib import FGError, NET_D, NET_G, disc_param_count, load_library
+from .lib import (FGError, NET_D, NET_G, c2f_disc_param_count, c2f_gen_param_count, disc_param_count,
+                  load_library)
 
 KINDS = {0: "nil", 1: "number", 2: "string", 3: "table", 4: "object", 5: "boolean", 6: "function", 16: "tensor",
          17: "storage", -1: None}
@@ -198,40 +199,140 @@ def load_reference_checkpoint(ctx, path, want_D=True):
         return int(f.number("epoch")) if f.kind("epoch") == "number" else None
 
 
+# models_c2f.lua's nets: G's "same" SpatialConvolutionUpsample layers (Cout, k) after the C+1 joined planes, Cout 0 =
+# the C image channels; D's 3x3 convolutions (Cout, 2x2 max pool after) (include/fg_b200.h FG_C2F_G_* / FG_C2F_D_*)
+C2F_G_LAYERS = {
+    "create_G_d": [(64, 3), (64, 3), (128, 5), (256, 5), (0, 7)],
+    "create_G_a": [(64, 3), (128, 7), (0, 5)],
+    "create_G_b": [(64, 3), (64, 3), (256, 5), (0, 7)],
+    "create_G_c": [(64, 3), (128, 3), (256, 5), (0, 7)],
+}
+C2F_D_LAYERS = {
+    "create_D_c": [(64, False), (64, True), (128, False), (256, True)],
+    "create_D_a": [(64, False), (64, True)],
+    "create_D_b": [(64, False), (64, True), (128, False), (128, True)],
+}
+
+
+def c2f_G_module_list(name):
+    """the fg_t7_net_describe skeleton of models_c2f.lua's generator `name` (cuda = false: no Copy layers)"""
+    inner = ["nn.SpatialConvolutionUpsample", "nn.PReLU"] * (len(C2F_G_LAYERS[name]) - 1)
+    return "nn.Sequential{nn.JoinTable,nn.Sequential{%s}}" % ",".join(inner + ["nn.SpatialConvolutionUpsample", "nn.View"])
+
+
+def c2f_D_module_list(name):
+    """the fg_t7_net_describe skeleton of models_c2f.lua's discriminator `name` (cuda = false: no Copy layers)"""
+    inner = []
+    for _, pool in C2F_D_LAYERS[name]:
+        inner += ["nn.SpatialConvolution", "nn.PReLU"] + (["nn.SpatialMaxPooling"] if pool else [])
+    inner += ["nn.Dropout", "nn.View", "nn.Linear", "nn.PReLU", "nn.Dropout", "nn.Linear", "nn.Sigmoid"]
+    return "nn.Sequential{nn.CAddTable,nn.Sequential{%s}}" % ",".join(inner)
+
+
+def c2f_G_conv_shapes(name, channels):
+    """the weight shapes (Cout, Cin, k, k) of the generator's convolutions in module order"""
+    out, cin = [], channels + 1
+    for cout, k in C2F_G_LAYERS[name]:
+        cout = cout or channels
+        out.append((cout, cin, k, k))
+        cin = cout
+    return out
+
+
+def c2f_D_conv_shapes(name, channels):
+    out, cin = [], channels
+    for cout, _ in C2F_D_LAYERS[name]:
+        out.append((cout, cin, 3, 3))
+        cin = cout
+    return out
+
+
+def _c2f_plain(describe):
+    """describe without the CUDA-mode Copy layers models_c2f.lua inserts (cuda = true) and with cudnn.* as nn.*"""
+    return describe.replace("cudnn.", "nn.").replace(",nn.Copy", "")
+
+
+def _recognise(describe, conv_shapes, names, module_list, shapes):
+    d = _c2f_plain(describe)
+    for name in names:
+        if d != module_list(name):
+            continue
+        for C in (1, 3):
+            if [tuple(s) for s in conv_shapes] == shapes(name, C):
+                return name
+    return None
+
+
+def recognise_c2f_G(describe, conv_shapes):
+    """the models_c2f.lua generator whose module list `describe` (fg_t7_net_describe) and convolution weight shapes
+    `conv_shapes` (module order) these are, or None.  The CUDA-mode Copy layers and cudnn.* classes are accepted."""
+    return _recognise(describe, conv_shapes, C2F_G_LAYERS, c2f_G_module_list, c2f_G_conv_shapes)
+
+
+def recognise_c2f_D(describe, conv_shapes):
+    """the models_c2f.lua discriminator of `describe` and `conv_shapes`, as recognise_c2f_G"""
+    return _recognise(describe, conv_shapes, C2F_D_LAYERS, c2f_D_module_list, c2f_D_conv_shapes)
+
+
+def conv_weight_shapes(f, path, limit=256):
+    """the weight shapes of every (Spatial)Convolution* leaf of the module tree at `path`, in module order (at most
+    `limit` modules are visited, so a cyclic or huge tree ends the walk)"""
+    out, seen = [], [0]
+
+    def walk(p, depth):
+        seen[0] += 1
+        if seen[0] > limit or depth > 16:
+            raise FGError("%s is not a plausible module tree" % path)
+        if f.kind(p + ".modules") == "table":
+            i = 1
+            while f.kind("%s.modules.%d" % (p, i)) is not None:
+                walk("%s.modules.%d" % (p, i), depth + 1)
+                i += 1
+        elif "Convolution" in f.string(p) and f.kind(p + ".weight") == "tensor":
+            out.append(f.tensor(p + ".weight").shape)
+
+    walk(path, 0)
+    return out
+
+
 def _c2f_fit(n_params, count):
     """' (the count of a c2f D with C channels at fine size S)' for the (C, S) whose count(C, S) is n_params, else ''"""
     fits = ["%d channels at fine size %d" % (c, s) for c in (1, 3) for s in (16, 32, 64) if count(c, s) == n_params]
     return " (that of %s)" % " or ".join(fits) if fits else ""
 
 
-def read_c2f_checkpoint(path, channels, fine_size):
+def read_c2f_checkpoint(path, channels, fine_size, generator="create_G_d", discriminator="create_D_c"):
     """adversarial_c2f.lua:207-216's `adversarial_c2f_<cs>_to_<S>.net` ({D, G, opt, epoch}) as flat vectors:
-    dict(PG, PD, epoch) in getParameters() order.  Refuses a G or D that does not fit the c2f nets with `channels`
-    channels at fine size `fine_size` (D's Linear reads 256*(S/4)^2 features).  Needs no GPU."""
-    lib = load_library()
-    nG = int(lib.fg_c2f_param_count_sized(NET_G, channels, fine_size))
-    nD = int(lib.fg_c2f_param_count_sized(NET_D, channels, fine_size))
-    if nG < 0:
+    dict(PG, PD, epoch) in getParameters() order.  Refuses a G or D that does not fit the c2f nets `generator` /
+    `discriminator` with `channels` channels at fine size `fine_size` (create_D_c's Linear reads 256*(S/4)^2
+    features): a recognised other models_c2f.lua net is named, any other tree is refused by its length.  Needs no
+    GPU."""
+    if fine_size not in (16, 32, 64):
         raise FGError("fine size %d is not supported (16, 32 or 64)" % fine_size)
+    nG = c2f_gen_param_count(generator, channels)
+    nD = c2f_disc_param_count(discriminator, channels, fine_size)
     with T7File(path) as f:
+        for key, want, recognise in (("G", generator, recognise_c2f_G), ("D", discriminator, recognise_c2f_D)):
+            have = recognise(f.net_describe(key), conv_weight_shapes(f, key))
+            if have is not None and have != want:
+                raise FGError("checkpoint %s is %s; the c2f net has %s" % (key, have, want))
         pg = f.net_params("G")
         if pg.size != nG:
-            fit = _c2f_fit(pg.size, lambda c, s: int(lib.fg_c2f_param_count_sized(NET_G, c, s)))
-            raise FGError("checkpoint G has %d parameters%s (%s); the c2f G with %d channels has %d"
-                          % (pg.size, fit, f.net_describe("G"), channels, nG))
+            raise FGError("checkpoint G has %d parameters (%s); the c2f G with %d channels has %d (%s)"
+                          % (pg.size, f.net_describe("G"), channels, nG, generator))
         pd = f.net_params("D")
         if pd.size != nD:
-            fit = _c2f_fit(pd.size, lambda c, s: int(lib.fg_c2f_param_count_sized(NET_D, c, s)))
-            raise FGError("checkpoint D has %d parameters%s (%s); the c2f D with %d channels at fine size %d has %d"
-                          % (pd.size, fit, f.net_describe("D"), channels, fine_size, nD))
+            fit = _c2f_fit(pd.size, lambda c, s: c2f_disc_param_count(discriminator, c, s))
+            raise FGError("checkpoint D has %d parameters%s (%s); the c2f D with %d channels at fine size %d has %d (%s)"
+                          % (pd.size, fit, f.net_describe("D"), channels, fine_size, nD, discriminator))
         epoch = int(f.number("epoch")) if f.kind("epoch") == "number" else None
     return dict(PG=pg, PD=pd, epoch=epoch)
 
 
 def load_c2f_checkpoint(net, path):
-    """load G and D of an `adversarial_c2f_<cs>_to_<S>.net` into a C2f of the same channels and fine size; returns the
-    epoch (None when the file has none)"""
-    ck = read_c2f_checkpoint(path, net.C, net.S)
+    """load G and D of an `adversarial_c2f_<cs>_to_<S>.net` into a C2f of the same nets, channels and fine size;
+    returns the epoch (None when the file has none)"""
+    ck = read_c2f_checkpoint(path, net.C, net.S, net.generator, net.discriminator)
     net.set_params(NET_G, ck["PG"])
     net.set_params(NET_D, ck["PD"])
     return ck["epoch"]

@@ -1,16 +1,19 @@
 // Coarse-to-fine GAN (BASELINE configs[3], train_c2f.lua) on the same kernels as the 32x32 nets, at fine size
-// S = train_c2f.lua --fineSize in {16, 32, 64} (the pyramid levels a 64x64 training set feeds):
-//   G = models_c2f.lua:113-145 create_G_d : JoinTable{noise[1xSxS], coarse[CxSxS]} -> SCU(C+1->64,3) PReLU
-//       SCU(64->64,3) PReLU SCU(64->128,5) PReLU SCU(128->256,5) PReLU SCU(256->C,7)            (all at SxS)
-//   D = models_c2f.lua:237-278 create_D_c : CAddTable{diff, coarse} -> conv(C->64,3) PReLU conv(64->64,3) PReLU
-//       MaxPool2 conv(64->128,3) PReLU conv(128->256,3) PReLU MaxPool2 Dropout View(256*(S/4)^2) Linear(512) PReLU
-//       Dropout Linear(1) Sigmoid
+// S = train_c2f.lua --fineSize in {16, 32, 64} (the pyramid levels a 64x64 training set feeds), with any of
+// models_c2f.lua's generators and discriminators (the default pair: create_G_d / create_D_c):
+//   G = JoinTable{noise[1xSxS], coarse[CxSxS]} -> SCU(C+1->c1,k1) PReLU ... SCU(->C,kn)          (all at SxS)
+//       create_G_d (:113-145) (64,3) (64,3) (128,5) (256,5) (C,7); create_G_a (:16-45) (64,3) (128,7) (C,5);
+//       create_G_b (:47-78) (64,3) (64,3) (256,5) (C,7); create_G_c (:80-111) (64,3) (128,3) (256,5) (C,7)
+//   D = CAddTable{diff, coarse} -> conv(C->c1,3) PReLU [MaxPool2] ... Dropout View Linear(512) PReLU Dropout Linear(1)
+//       Sigmoid; create_D_c (:237-278) (64,-) (64,pool) (128,-) (256,pool); create_D_a (:156-192) (64,-) (64,pool);
+//       create_D_b (:194-235) (64,-) (64,pool) (128,-) (128,pool)
 //   loop = adversarial_c2f.lua:121-187 (fevalD :40-81, fevalG_on_D :85-116, optim.adam)
 // cudnn.SpatialConvolutionUpsample with factor 1 (layers/cudnnSpatialConvolutionUpsample.lua:4-28) is a "same"
-// convolution whose output view is the identity, so every layer maps onto the tap-GEMM convolution kernels:
-// wgmma (3xTF32, chunk-promoted) where the channel counts make a dense contraction (64->64, 64->128,
-// 128->256 and the 256*(S/4)^2 -> 512 Linear), the bandwidth-shaped small-channel kernels for (C+1)->64 / C->64 and the
-// fp32 FFMA tile kernel for the 256->C 7x7 output layer (N = 3 is not a tensor-core shape).
+// convolution whose output view is the identity, so every layer maps onto the tap-GEMM convolution kernels through
+// ConvL: wgmma (chunk-promoted 3xFP16 / 3xTF32) where the channel counts make a dense contraction (64->64, 64->128,
+// 128->128, 64/128->256 and the Linear), the bandwidth-shaped small-channel kernels for (C+1)->64 / C->64 and, for the
+// ->C output layers, a wgmma forward and weight gradient with the output channels zero-padded to a 64-row tile
+// (ConvL::pad_out) and an FFMA data gradient.
 #include <algorithm>
 #include <deque>
 #include <string>
@@ -23,11 +26,46 @@
 #include "k_scale.cuh"
 
 namespace {
+constexpr int kMaxGL = 5, kMaxDL = 4;
+// a generator: its "same" convolutions after the C+1 joined input planes; Cout 0 is the C image channels of the last
+// layer (no activation after it), every other layer is followed by a one-slope PReLU
+struct C2fGDesc {
+  const char* name;
+  const char* tag;  // of the timer names of a pair other than the default one
+  int n;
+  struct { int Cout, k; } L[kMaxGL];
+};
+// a discriminator: 3x3 convolutions, each followed by a one-slope PReLU and optionally a 2x2 max pool; the last pooled
+// map ([view_c][S/view_div][S/view_div]) goes through Dropout and View into Linear(512)
+struct C2fDDesc {
+  const char* name;
+  const char* tag;
+  int n;
+  struct { int Cout; bool pool; } L[kMaxDL];
+  int view_c, view_div;
+};
+// indexed by FG_C2F_G_* / FG_C2F_D_* (DEFAULT is the models_c2f.lua create_G / create_D default)
+const C2fGDesc kGens[] = {
+    {"create_G_d", "Gd", 5, {{64, 3}, {64, 3}, {128, 5}, {256, 5}, {0, 7}}},
+    {"create_G_d", "Gd", 5, {{64, 3}, {64, 3}, {128, 5}, {256, 5}, {0, 7}}},
+    {"create_G_a", "Ga", 3, {{64, 3}, {128, 7}, {0, 5}}},
+    {"create_G_b", "Gb", 4, {{64, 3}, {64, 3}, {256, 5}, {0, 7}}},
+    {"create_G_c", "Gc", 4, {{64, 3}, {128, 3}, {256, 5}, {0, 7}}},
+};
+const C2fDDesc kDiscs[] = {
+    {"create_D_c", "Dc", 4, {{64, false}, {64, true}, {128, false}, {256, true}}, 256, 4},
+    {"create_D_c", "Dc", 4, {{64, false}, {64, true}, {128, false}, {256, true}}, 256, 4},
+    {"create_D_a", "Da", 2, {{64, false}, {64, true}}, 64, 2},
+    {"create_D_b", "Db", 4, {{64, false}, {64, true}, {128, false}, {128, true}}, 128, 4},
+};
+constexpr int kNGens = sizeof(kGens) / sizeof(kGens[0]), kNDiscs = sizeof(kDiscs) / sizeof(kDiscs[0]);
 bool c2f_size_ok(int S) { return S == 16 || S == 32 || S == 64; }
-// View(256*(S/4)^2) of D's last pooled map [256][S/4][S/4]: D.L1's input width
-int c2f_flat(int S) { return 256 * (S / 4) * (S / 4); }
-// nn.Dropout keep flags per sample: [256][S/4][S/4] then [512]
-int c2f_mask(int S) { return c2f_flat(S) + 512; }
+bool c2f_gen_ok(int g) { return g >= 0 && g < kNGens; }
+bool c2f_disc_ok(int d) { return d >= 0 && d < kNDiscs; }
+// View(view_c*(S/view_div)^2) of D's last pooled map: D.L1's input width
+int c2f_flat(const C2fDDesc& d, int S) { return d.view_c * (S / d.view_div) * (S / d.view_div); }
+// nn.Dropout keep flags per sample: the pooled map (NCHW order) then [512]
+int c2f_mask(const C2fDDesc& d, int S) { return c2f_flat(d, S) + 512; }
 }  // namespace
 
 struct fg_c2f {
@@ -35,16 +73,22 @@ struct fg_c2f {
   int maxB = 0, C = 3;
   int S = 32;           // fine size: every image, noise and activation of G and D's first stage is S x S
   int HW = 1024;        // S * S
-  int flat = 16384;     // c2f_flat(S)
-  int mask = 16896;     // c2f_mask(S)
+  int gen = FG_C2F_G_D, disc = FG_C2F_D_C;      // never DEFAULT
+  const C2fGDesc* gd = &kGens[FG_C2F_G_D];
+  const C2fDDesc* dd = &kDiscs[FG_C2F_D_C];
+  int flat = 16384;     // c2f_flat(*dd, S)
+  int mask = 16896;     // c2f_mask(*dd, S)
+  int nGc = 5, nDc = 4;  // layer counts of the descriptors
   std::deque<std::string> names;  // timer names (stable storage: the layers point into it)
   NetPair net;  // no BatchNorm
-  int64_t Gca[4] = {0, 0, 0, 0}, Dca[4] = {0, 0, 0, 0}, Da5 = 0, DL2W = 0, DL2b = 0;
-  ConvL Gc[5], Dc[4], DL1;
+  int64_t Gca[kMaxGL] = {}, Dca[kMaxDL] = {}, Da5 = 0, DL2W = 0, DL2b = 0;
+  ConvL Gc[kMaxGL], Dc[kMaxDL], DL1;
   const char* D_L2_timer = "";
   const char *t_refine_prep = "", *t_refine_pick = "";  // fg_c2f_refine's own kernels
-  float *G_x = nullptr, *G_z[5] = {}, *G_h[4] = {};
-  float *D_x = nullptr, *D_cond = nullptr, *D_z[4] = {}, *D_h[4] = {}, *D_p2 = nullptr, *D_p4 = nullptr, *D_d4 = nullptr;
+  float *G_x = nullptr, *G_z[kMaxGL] = {}, *G_h[kMaxGL] = {};
+  // D_p[i]: the 2x2 max pool of D_h[i] (layers with a pool only); D_pv = the last of them, the map View flattens
+  float *D_x = nullptr, *D_cond = nullptr, *D_z[kMaxDL] = {}, *D_h[kMaxDL] = {}, *D_p[kMaxDL] = {}, *D_pv = nullptr,
+        *D_d4 = nullptr;
   float *D_zl1 = nullptr, *D_al1 = nullptr, *D_hl1 = nullptr, *D_logit = nullptr, *D_out = nullptr, *D_masks = nullptr,
         *D_dlogit = nullptr, *D_dx = nullptr;
   float *ga = nullptr, *gb = nullptr, *ws = nullptr;
@@ -55,6 +99,7 @@ struct fg_c2f {
   float D_scale = 2.f;
   std::vector<void*> allocs;
   ConvLEnv env;  // shared scratch of the ConvL layers (filled by c2f_alloc)
+  float* G_y() const { return G_z[nGc - 1]; }  // G's output (the diff), NHWC
 };
 
 namespace {
@@ -66,57 +111,81 @@ inline int convl_bwd(fg_c2f* n, ConvL& L, const float* in, const float* dy, floa
 }
 
 // "c2f.<layer>" at S = 32 (the names profiles/bench_configs.py reads), "c2f16.<layer>" / "c2f64.<layer>" otherwise, so
-// that nets of two sizes on one ctx keep their timings apart
+// that nets of two sizes on one ctx keep their timings apart; a pair other than create_G_d / create_D_c adds its nets'
+// tags ("c2f32.Ga.Dc.<layer>"), so that two pairs of one size keep theirs apart too
 const char* timer_name(fg_c2f* n, const char* layer) {
-  n->names.push_back((n->S == 32 ? std::string("c2f.") : "c2f" + std::to_string(n->S) + ".") + layer);
+  std::string p = n->S == 32 ? std::string("c2f.") : "c2f" + std::to_string(n->S) + ".";
+  if (n->gen != FG_C2F_G_D || n->disc != FG_C2F_D_C)
+    p = "c2f" + std::to_string(n->S) + "." + n->gd->tag + "." + n->dd->tag + ".";
+  n->names.push_back(p + layer);
   return n->names.back().c_str();
+}
+
+// the pad rules of the ConvL dispatch (DESIGN.md §7.2): a ->C output layer runs its forward and weight gradient with the
+// output channels padded to a 64-row tile, a 64 -> 64 layer its weight gradient with dY padded to 128 rows
+void set_pads(ConvL& L) {
+  if (L.Cout <= 4 && L.Cin % 128 == 0) L.pad_out = 64;
+  if (L.Cout == 64 && L.Cin % 64 == 0) L.pad_dy = 128;
 }
 
 void make_layouts(fg_c2f* n) {
   const int C = n->C, S = n->S;
+  const C2fGDesc& gd = *n->gd;
+  const C2fDDesc& dd = *n->dd;
   n->HW = S * S;
-  n->flat = c2f_flat(S);
-  n->mask = c2f_mask(S);
+  n->flat = c2f_flat(dd, S);
+  n->mask = c2f_mask(dd, S);
+  n->nGc = gd.n;
+  n->nDc = dd.n;
   n->names.clear();
   {
-    const int ci[5] = {C + 1, 64, 64, 128, 256}, co[5] = {64, 64, 128, 256, C}, kk[5] = {3, 3, 5, 5, 7};
     int64_t o = 0;
-    for (int i = 0; i < 5; ++i) {
+    int ci = C + 1;
+    for (int i = 0; i < gd.n; ++i) {
+      const bool last = i == gd.n - 1;
+      const int co = last ? C : gd.L[i].Cout, k = gd.L[i].k;
       ConvL& L = n->Gc[i];
-      L.Cin = ci[i]; L.Cout = co[i]; L.k = kk[i]; L.H = S;
-      L.w_off = o; o += (int64_t)co[i] * ci[i] * kk[i] * kk[i];
-      L.b_off = o; o += co[i];
-      if (i < 4) { n->Gca[i] = o; o += 1; }
+      L = ConvL{};
+      L.Cin = ci; L.Cout = co; L.k = k; L.H = S;
+      L.w_off = o; o += (int64_t)co * ci * k * k;
+      L.b_off = o; o += co;
+      if (!last) { n->Gca[i] = o; o += 1; }
       L.need_dgrad = i > 0;
       const std::string l = "G.c" + std::to_string(i + 1);
       L.tf = timer_name(n, (l + ".fwd").c_str()); L.td = timer_name(n, (l + ".dgrad").c_str()); L.tw = timer_name(n, (l + ".wgrad").c_str());
-      if (co[i] <= 4 && ci[i] % 128 == 0) L.pad_out = 64;  // c5: 256 -> C, 7x7
-      if (co[i] == 64 && ci[i] % 64 == 0) L.pad_dy = 128;  // c2: 64 -> 64
+      set_pads(L);
+      ci = co;
     }
     n->net.nG = o;
   }
   {
-    const int ci[4] = {C, 64, 64, 128}, co[4] = {64, 64, 128, 256}, hw[4] = {S, S, S / 2, S / 2};
     int64_t o = 0;
-    for (int i = 0; i < 4; ++i) {
+    int ci = C, H = S;
+    for (int i = 0; i < dd.n; ++i) {
+      const int co = dd.L[i].Cout;
       ConvL& L = n->Dc[i];
-      L.Cin = ci[i]; L.Cout = co[i]; L.k = 3; L.H = hw[i];
-      L.w_off = o; o += (int64_t)co[i] * ci[i] * 9;
-      L.b_off = o; o += co[i];
+      L = ConvL{};
+      L.Cin = ci; L.Cout = co; L.k = 3; L.H = H;
+      L.w_off = o; o += (int64_t)co * ci * 9;
+      L.b_off = o; o += co;
       n->Dca[i] = o; o += 1;
       const std::string l = "D.c" + std::to_string(i + 1);
       L.tf = timer_name(n, (l + ".fwd").c_str()); L.td = timer_name(n, (l + ".dgrad").c_str()); L.tw = timer_name(n, (l + ".wgrad").c_str());
-      if (co[i] == 64 && ci[i] % 64 == 0) L.pad_dy = 128;  // c2: 64 -> 64
+      set_pads(L);
+      ci = co;
+      if (dd.L[i].pool) H /= 2;
     }
     ConvL& L = n->DL1;
+    L = ConvL{};
     L.Cin = n->flat; L.Cout = 512; L.k = 1; L.H = 1;
-    L.cA = 256; L.cS = (S / 4) * (S / 4);  // View(256*(S/4)^2) flattens [256][S/4][S/4]; ours is [S/4][S/4][256]
+    // View(view_c*(S/view_div)^2) flattens [view_c][S/view_div][S/view_div]; ours is [S/view_div][S/view_div][view_c]
+    L.cA = dd.view_c; L.cS = (S / dd.view_div) * (S / dd.view_div);
     L.w_off = o; o += (int64_t)512 * n->flat;
     L.b_off = o; o += 512;
     L.tf = timer_name(n, "D.L1.fwd"); L.td = timer_name(n, "D.L1.dgrad"); L.tw = timer_name(n, "D.L1.wgrad");
     n->D_L2_timer = timer_name(n, "D.L2.fwd");
-  n->t_refine_prep = timer_name(n, "refine_prep");
-  n->t_refine_pick = timer_name(n, "refine_pick");
+    n->t_refine_prep = timer_name(n, "refine_prep");
+    n->t_refine_pick = timer_name(n, "refine_pick");
     n->Da5 = o; o += 1;
     n->DL2W = o; o += 512;
     n->DL2b = o; o += 1;
@@ -131,23 +200,41 @@ int c2f_alloc(fg_c2f* n) {
   n->env.maxB = n->maxB;
   n->env.allocs = &n->allocs;
   FG_TRY(pair_alloc(n->c, n->allocs, n->net, n->net.nG, n->net.nD, false));
-  for (int i = 0; i < 5; ++i) FG_TRY(convl_alloc(n, n->Gc[i]));
-  for (int i = 0; i < 4; ++i) FG_TRY(convl_alloc(n, n->Dc[i]));
+  // per-sample scratch sizes, the maximum over the layers of both nets:
+  //   act  the largest activation / gradient map (the gradient ping-pong, the dY split, a pad_out forward's padded
+  //        output); G's first layer (64 channels at S x S) keeps it above fg_c2f_refine's C x 64 x 64 image staging
+  //   pad  the largest channel-padded dY (pad_out / pad_dy layers)
+  //   wsz  the largest packed weight gradient (whole, not per sample)
+  size_t act = 0, pad = 0, wsz = (size_t)512 * flat;
+  auto visit = [&](const ConvL& L) {
+    const size_t hw = (size_t)L.H * L.H, KK = (size_t)L.k * L.k;
+    act = std::max(act, hw * std::max({L.Cin, L.Cout, L.pad_out}));
+    pad = std::max(pad, hw * std::max(L.pad_out, L.pad_dy));
+    wsz = std::max(wsz, KK * L.Cin * (L.pad_out ? L.pad_out : L.pad_dy ? L.pad_dy : L.Cout));
+  };
+  for (int i = 0; i < n->nGc; ++i) visit(n->Gc[i]);
+  for (int i = 0; i < n->nDc; ++i) visit(n->Dc[i]);
+  act = std::max(act, (size_t)flat);
+  for (int i = 0; i < n->nGc; ++i) FG_TRY(convl_alloc(n, n->Gc[i]));
+  for (int i = 0; i < n->nDc; ++i) FG_TRY(convl_alloc(n, n->Dc[i]));
   FG_TRY(convl_alloc(n, n->DL1));
   FG_TRY(dalloc(n, &n->G_x, B * HW * (C + 1)));
-  for (int i = 0; i < 5; ++i) {
+  for (int i = 0; i < n->nGc; ++i) {
     FG_TRY(dalloc(n, &n->G_z[i], B * HW * n->Gc[i].Cout));
-    if (i < 4) FG_TRY(dalloc(n, &n->G_h[i], B * HW * n->Gc[i].Cout));
+    if (i < n->nGc - 1) FG_TRY(dalloc(n, &n->G_h[i], B * HW * n->Gc[i].Cout));
   }
   FG_TRY(dalloc(n, &n->D_x, B * HW * C));
   FG_TRY(dalloc(n, &n->D_cond, B * HW * C));
-  for (int i = 0; i < 4; ++i) {
-    const size_t e = B * (size_t)n->Dc[i].H * n->Dc[i].H * n->Dc[i].Cout;
+  for (int i = 0; i < n->nDc; ++i) {
+    const ConvL& L = n->Dc[i];
+    const size_t e = B * (size_t)L.H * L.H * L.Cout;
     FG_TRY(dalloc(n, &n->D_z[i], e));
     FG_TRY(dalloc(n, &n->D_h[i], e));
+    if (n->dd->L[i].pool) {
+      FG_TRY(dalloc(n, &n->D_p[i], e / 4));
+      n->D_pv = n->D_p[i];
+    }
   }
-  FG_TRY(dalloc(n, &n->D_p2, B * (HW / 4) * 64));
-  FG_TRY(dalloc(n, &n->D_p4, B * flat));
   FG_TRY(dalloc(n, &n->D_d4, B * flat));
   FG_TRY(dalloc(n, &n->D_zl1, B * 512));
   FG_TRY(dalloc(n, &n->D_al1, B * 512));
@@ -157,14 +244,14 @@ int c2f_alloc(fg_c2f* n) {
   FG_TRY(dalloc(n, &n->D_dlogit, B));
   FG_TRY(dalloc(n, &n->D_masks, B * mask));
   FG_TRY(dalloc(n, &n->D_dx, B * HW * C));
-  const size_t big = B * HW * 256;  // largest activation: G conv4 output
+  const size_t big = B * act;
   FG_TRY(dalloc(n, &n->ga, big));
   FG_TRY(dalloc(n, &n->gb, big));
   FG_TRY(dalloc(n, &n->env.dy.hi, big));
   FG_TRY(dalloc(n, &n->env.dy.lo, big));
-  FG_TRY(dalloc(n, &n->env.pad.hi, big / 2));  // up to 128 padded channels at S x S
-  FG_TRY(dalloc(n, &n->env.pad.lo, big / 2));
-  FG_TRY(dalloc(n, &n->ws, std::max<size_t>((size_t)512 * flat, (size_t)25 * 256 * 128)));
+  FG_TRY(dalloc(n, &n->env.pad.hi, B * pad));
+  FG_TRY(dalloc(n, &n->env.pad.lo, B * pad));
+  FG_TRY(dalloc(n, &n->ws, wsz));
   n->env.ga = n->ga; n->env.ws = n->ws;
   FG_TRY(dalloc(n, &n->in_a, B * HW * C));
   FG_TRY(dalloc(n, &n->in_b, B * HW * C));
@@ -172,11 +259,14 @@ int c2f_alloc(fg_c2f* n) {
   FG_TRY(dalloc(n, &n->in_d, B * HW * C));
   FG_TRY(dalloc(n, &n->in_e, B * HW));
   FG_TRY(dalloc(n, &n->io, B * HW * C));
-  int64_t dz[4];
-  for (int i = 0; i < 4; ++i) dz[i] = (int64_t)n->Dc[i].H * n->Dc[i].H * n->Dc[i].Cout;
-  n->net.keep = {{"Dstep.z1", n->D_z[0], dz[0]}, {"Dstep.z2", n->D_z[1], dz[1]}, {"Dstep.z3", n->D_z[2], dz[2]},
-                 {"Dstep.z4", n->D_z[3], dz[3]}, {"Dstep.zl1", n->D_zl1, 512},  {"Dstep.logit", n->D_logit, 1},
-                 {"Dstep.out", n->D_out, 1}};
+  n->net.keep.clear();
+  for (int i = 0; i < n->nDc; ++i) {
+    n->names.push_back("Dstep.z" + std::to_string(i + 1));
+    n->net.keep.push_back({n->names.back().c_str(), n->D_z[i], (int64_t)n->Dc[i].H * n->Dc[i].H * n->Dc[i].Cout});
+  }
+  n->net.keep.push_back({"Dstep.zl1", n->D_zl1, 512});
+  n->net.keep.push_back({"Dstep.logit", n->D_logit, 1});
+  n->net.keep.push_back({"Dstep.out", n->D_out, 1});
   FG_CUDA(cudaStreamSynchronize(n->c->stream));
   return FG_OK;
 }
@@ -185,27 +275,27 @@ int c2f_alloc(fg_c2f* n) {
 // pack (the TF32 splits are only produced for the tensor-core implementations)
 int pack_G(fg_c2f* n) {
   if (n->net.G_pack == pack_key(n->c)) return FG_OK;
-  for (int i = 0; i < 5; ++i) FG_TRY(convl_pack(n->c, n->Gc[i], n->net.PG));
+  for (int i = 0; i < n->nGc; ++i) FG_TRY(convl_pack(n->c, n->Gc[i], n->net.PG));
   n->net.G_pack = pack_key(n->c);
   return FG_OK;
 }
 int pack_D(fg_c2f* n) {
   if (n->net.D_pack == pack_key(n->c)) return FG_OK;
-  for (int i = 0; i < 4; ++i) FG_TRY(convl_pack(n->c, n->Dc[i], n->net.PD));
+  for (int i = 0; i < n->nDc; ++i) FG_TRY(convl_pack(n->c, n->Dc[i], n->net.PD));
   FG_TRY(convl_pack(n->c, n->DL1, n->net.PD));
   n->net.D_pack = pack_key(n->c);
   return FG_OK;
 }
 
 // G on the joined NHWC input already in G_x (nn.JoinTable order: the noise channel, then the C condition channels);
-// the diff lands in G_z[4] (NHWC)
+// the diff lands in G_y() (NHWC)
 int G_forward_joined(fg_c2f* n, int B) {
   fg_ctx* c = n->c;
   FG_TRY(pack_G(n));
   const float* cur = n->G_x;
-  for (int i = 0; i < 5; ++i) {
+  for (int i = 0; i < n->nGc; ++i) {
     FG_TRY(convl_fwd(n, n->Gc[i], cur, n->net.PG, n->G_z[i], B));
-    if (i < 4) {
+    if (i < n->nGc - 1) {
       FG_TRY(k_prelu_fwd(c, n->G_z[i], n->net.PG + n->Gca[i], n->G_h[i], (int64_t)B * n->HW * n->Gc[i].Cout));
       cur = n->G_h[i];
     }
@@ -214,7 +304,7 @@ int G_forward_joined(fg_c2f* n, int B) {
   n->G_valid = true;
   return FG_OK;
 }
-// noise [B][1][S][S] and cond [B][C][S][S] are NCHW device pointers; the diff lands in G_z[4] (NHWC)
+// noise [B][1][S][S] and cond [B][C][S][S] are NCHW device pointers; the diff lands in G_y() (NHWC)
 int G_forward(fg_c2f* n, const float* noise, const float* cond, int B) {
   FG_REQUIRE(B >= 1 && B <= n->maxB, "c2f G forward: batch %d out of range [1,%d]", B, n->maxB);
   FG_TRY(pack_G(n));
@@ -230,7 +320,7 @@ int G_backward(fg_c2f* n, const float* ddiff) {
   }
   const int B = n->G_B;
   const float* dcur = ddiff;
-  for (int i = 4; i >= 0; --i) {
+  for (int i = n->nGc - 1; i >= 0; --i) {
     const float* in = i == 0 ? n->G_x : n->G_h[i - 1];
     FG_TRY(convl_bwd(n, n->Gc[i], in, dcur, n->net.gG, i > 0 ? n->ga : nullptr, B));
     if (i > 0) {
@@ -250,22 +340,20 @@ int D_forward(fg_c2f* n, const float* diff, const float* cond, int B, bool train
   const float* P = n->net.PD;
   FG_TRY(k_add(c, diff, cond, n->D_x, (int64_t)B * n->HW * n->C));  // nn.CAddTable
   const float* cur = n->D_x;
-  for (int i = 0; i < 4; ++i) {
+  for (int i = 0; i < n->nDc; ++i) {
     const ConvL& L = n->Dc[i];
     FG_TRY(convl_fwd(n, n->Dc[i], cur, P, n->D_z[i], B));
     FG_TRY(k_prelu_fwd(c, n->D_z[i], P + n->Dca[i], n->D_h[i], (int64_t)B * L.H * L.H * L.Cout));
     cur = n->D_h[i];
-    if (i == 1) {
-      FG_TRY(k_maxpool2_fwd(c, n->D_h[1], n->D_p2, B, n->S, n->S, 64));
-      cur = n->D_p2;
-    } else if (i == 3) {
-      FG_TRY(k_maxpool2_fwd(c, n->D_h[3], n->D_p4, B, n->S / 2, n->S / 2, 256));
+    if (n->D_p[i]) {
+      FG_TRY(k_maxpool2_fwd(c, n->D_h[i], n->D_p[i], B, L.H, L.H, L.Cout));
+      cur = n->D_p[i];
     }
   }
   n->D_scale = 1.0f / (1.0f - p_drop);
-  const float* d4 = n->D_p4;
+  const float* d4 = n->D_pv;
   if (training) {  // nn.Dropout (v2): mask/(1-p) in training, identity in evaluation
-    FG_TRY(k_dropout_nhwc(c, n->D_p4, n->D_masks, n->mask, 0, n->HW / 16, 256, n->D_scale, n->D_d4, B));
+    FG_TRY(k_dropout_nhwc(c, n->D_pv, n->D_masks, n->mask, 0, n->DL1.cS, n->DL1.cA, n->D_scale, n->D_d4, B));
     d4 = n->D_d4;
   }
   FG_TRY(convl_fwd(n, n->DL1, d4, P, n->D_zl1, B));
@@ -296,7 +384,7 @@ int D_backward(fg_c2f* n, const float* dlogit, bool want_wgrad, bool want_dx) {
   float* G = want_wgrad ? n->net.gD : nullptr;
   const bool tr = n->D_train;
   const float* hl1 = tr ? n->D_hl1 : n->D_al1;
-  const float* d4 = tr ? n->D_d4 : n->D_p4;
+  const float* d4 = tr ? n->D_d4 : n->D_pv;
   if (G) FG_TRY(k_gemv_wgrad_add(c, hl1, dlogit, G + n->DL2W, G + n->DL2b, B, 512));
   float *cur = n->ga, *oth = n->gb;  // gradient ping-pong: every stage reads `cur`, writes `oth`, then they swap
   FG_TRY(k_gemv_dgrad(c, dlogit, P + n->DL2W, cur, B, 512));
@@ -306,21 +394,21 @@ int D_backward(fg_c2f* n, const float* dlogit, bool want_wgrad, bool want_dx) {
   }
   FG_TRY(k_prelu_bwd(c, cur, n->D_zl1, P + n->Da5, oth, G ? G + n->Da5 : nullptr, B, 1, 1, 512, 0));
   std::swap(cur, oth);
-  FG_TRY(convl_bwd(n, n->DL1, d4, cur, G, oth, B));  // -> gradient of the View input, [B][S/4][S/4][256]
+  FG_TRY(convl_bwd(n, n->DL1, d4, cur, G, oth, B));  // -> gradient of the View input, NHWC
   std::swap(cur, oth);
   if (tr) {
-    FG_TRY(k_dropout_nhwc(c, cur, n->D_masks, n->mask, 0, n->HW / 16, 256, n->D_scale, oth, B));
+    FG_TRY(k_dropout_nhwc(c, cur, n->D_masks, n->mask, 0, n->DL1.cS, n->DL1.cA, n->D_scale, oth, B));
     std::swap(cur, oth);
   }
-  for (int i = 3; i >= 0; --i) {
+  for (int i = n->nDc - 1; i >= 0; --i) {
     ConvL& L = n->Dc[i];
-    if (i == 3 || i == 1) {  // cur is the gradient of the pooled map
+    if (n->D_p[i]) {  // cur is the gradient of the pooled map
       FG_TRY(k_maxpool2_bwd(c, cur, n->D_h[i], oth, B, L.H, L.H, L.Cout));
       std::swap(cur, oth);
     }
     FG_TRY(k_prelu_bwd(c, cur, n->D_z[i], P + n->Dca[i], oth, G ? G + n->Dca[i] : nullptr, B, L.H, L.H, L.Cout, 0));
     std::swap(cur, oth);
-    const float* in = i == 0 ? n->D_x : (i == 2 ? n->D_p2 : n->D_h[i - 1]);
+    const float* in = i == 0 ? n->D_x : (n->D_p[i - 1] ? n->D_p[i - 1] : n->D_h[i - 1]);
     float* din = i > 0 ? oth : (want_dx ? n->D_dx : nullptr);
     FG_TRY(convl_bwd(n, L, in, cur, G, din, B));
     if (i > 0) std::swap(cur, oth);
@@ -352,13 +440,13 @@ struct C2fStep final : StepNets {
   int d_input(int j) override {
     const int Bh = B / 2;
     FG_TRY(k_nchw_to_nhwc(c, real_diff + (size_t)j * Bh * img(), n->io, Bh, n->C, n->HW));
-    FG_CUDA(cudaMemcpyAsync(n->io + Bh * img(), n->G_z[4], sizeof(float) * Bh * img(), cudaMemcpyDeviceToDevice, c->stream));
+    FG_CUDA(cudaMemcpyAsync(n->io + Bh * img(), n->G_y(), sizeof(float) * Bh * img(), cudaMemcpyDeviceToDevice, c->stream));
     return k_nchw_to_nhwc(c, condD + (size_t)j * B * img(), n->D_cond, B, n->C, n->HW);
   }
   int draw_masks(int kind, const uint64_t* root) override {
     return k_bernoulli_keep(c, n->D_masks, (int64_t)B * n->mask, kind, h->p_drop, root);
   }
-  int d_forward(bool on_g) override { return D_forward(n, on_g ? n->G_z[4] : n->io, n->D_cond, B, true, h->p_drop); }
+  int d_forward(bool on_g) override { return D_forward(n, on_g ? n->G_y() : n->io, n->D_cond, B, true, h->p_drop); }
   // D's weight grads of the G iteration are zeroed before use (:45): skipped
   int d_backward(bool want_wgrad, bool want_dx) override { return D_backward(n, n->D_dlogit, want_wgrad, want_dx); }
   int g_backward() override { return G_backward(n, n->D_dx); }
@@ -439,6 +527,19 @@ __global__ void __launch_bounds__(kRefineThreads) refine_pick_kernel(const float
 }
 }  // namespace
 
+namespace {
+// getParameters() length of G (net FG_NET_G) or D of the pair (gen, disc) with C channels at fine size S
+int64_t c2f_count(int gen, int disc, int C, int S, int net) {
+  fg_c2f tmp;
+  tmp.C = C;
+  tmp.S = S;
+  tmp.gd = &kGens[gen];
+  tmp.dd = &kDiscs[disc];
+  make_layouts(&tmp);
+  return net == FG_NET_D ? tmp.net.nD : tmp.net.nG;
+}
+}  // namespace
+
 #define ENTER(n)                                         \
   do {                                                   \
     if (!(n) || !(n)->c) {                               \
@@ -513,19 +614,31 @@ extern "C" {
 
 int fg_c2f_create(fg_ctx* ctx, fg_c2f** out) { return fg_c2f_create_sized(ctx, 32, out); }
 int fg_c2f_create_sized(fg_ctx* ctx, int fine_size, fg_c2f** out) {
+  return fg_c2f_create_nets(ctx, fine_size, FG_C2F_G_DEFAULT, FG_C2F_D_DEFAULT, out);
+}
+int fg_c2f_create_nets(fg_ctx* ctx, int fine_size, int gen, int disc, fg_c2f** out) {
   if (!ctx || !out) {
-    fg_set_error("fg_c2f_create_sized: null argument");
+    fg_set_error("fg_c2f_create_nets: null argument");
     return FG_ERR_INVALID;
   }
   *out = nullptr;
   if (!c2f_size_ok(fine_size)) {
-    fg_set_error("fg_c2f_create_sized: fine size %d is not supported (16, 32 or 64)", fine_size);
+    fg_set_error("fg_c2f_create_nets: fine size %d is not supported (16, 32 or 64)", fine_size);
+    return FG_ERR_UNSUPPORTED;
+  }
+  if (!c2f_gen_ok(gen) || !c2f_disc_ok(disc)) {
+    fg_set_error("fg_c2f_create_nets: unknown generator %d or discriminator %d (FG_C2F_G_* 0..%d, FG_C2F_D_* 0..%d)", gen,
+                 disc, kNGens - 1, kNDiscs - 1);
     return FG_ERR_UNSUPPORTED;
   }
   FG_CUDA(cudaSetDevice(ctx->device));
   fg_c2f* n = new fg_c2f();
   n->c = ctx;
   n->S = fine_size;
+  n->gen = gen == FG_C2F_G_DEFAULT ? FG_C2F_G_D : gen;
+  n->disc = disc == FG_C2F_D_DEFAULT ? FG_C2F_D_C : disc;
+  n->gd = &kGens[n->gen];
+  n->dd = &kDiscs[n->disc];
   n->maxB = ctx->maxB;
   n->C = ctx->C;
   const int r = c2f_alloc(n);
@@ -536,6 +649,8 @@ int fg_c2f_create_sized(fg_ctx* ctx, int fine_size, fg_c2f** out) {
   *out = n;
   return FG_OK;
 }
+int fg_c2f_get_gen(fg_c2f* n) { return n ? n->gen : -1; }
+int fg_c2f_get_disc(fg_c2f* n) { return n ? n->disc : -1; }
 int fg_c2f_destroy(fg_c2f* n) {
   if (!n) return FG_OK;
   if (n->c) {
@@ -550,14 +665,20 @@ int fg_c2f_destroy(fg_c2f* n) {
 int64_t fg_c2f_param_count(int net, int channels) { return fg_c2f_param_count_sized(net, channels, 32); }
 int64_t fg_c2f_param_count_sized(int net, int channels, int fine_size) {
   if (!c2f_size_ok(fine_size)) return -1;
-  fg_c2f tmp;
-  tmp.C = channels;
-  tmp.S = fine_size;
-  make_layouts(&tmp);
-  return net == FG_NET_D ? tmp.net.nD : tmp.net.nG;
+  return c2f_count(FG_C2F_G_DEFAULT, FG_C2F_D_DEFAULT, channels, fine_size, net);
 }
-int fg_c2f_mask_per_sample(void) { return c2f_mask(32); }
-int fg_c2f_mask_per_sample_sized(int fine_size) { return c2f_size_ok(fine_size) ? c2f_mask(fine_size) : -1; }
+int64_t fg_c2f_gen_param_count(int gen, int channels) {
+  return c2f_gen_ok(gen) && channels >= 1 ? c2f_count(gen, FG_C2F_D_DEFAULT, channels, 32, FG_NET_G) : -1;
+}
+int64_t fg_c2f_disc_param_count(int disc, int channels, int fine_size) {
+  return c2f_disc_ok(disc) && channels >= 1 && c2f_size_ok(fine_size)
+             ? c2f_count(FG_C2F_G_DEFAULT, disc, channels, fine_size, FG_NET_D) : -1;
+}
+int fg_c2f_mask_per_sample(void) { return c2f_mask(kDiscs[FG_C2F_D_DEFAULT], 32); }
+int fg_c2f_mask_per_sample_sized(int fine_size) { return fg_c2f_disc_mask_per_sample(FG_C2F_D_DEFAULT, fine_size); }
+int fg_c2f_disc_mask_per_sample(int disc, int fine_size) {
+  return c2f_disc_ok(disc) && c2f_size_ok(fine_size) ? c2f_mask(kDiscs[disc], fine_size) : -1;
+}
 int fg_c2f_fine_size(fg_c2f* n) { return n ? n->S : 0; }
 
 int fg_c2f_set_params(fg_c2f* n, int net, const float* src) {
@@ -599,7 +720,7 @@ int fg_c2f_G_forward(fg_c2f* n, const float* noise, const float* cond, int B, fl
   FG_TRY(fg_to_dev(n->c, cond, (size_t)B * n->C * n->HW, n->in_b, &cd));
   FG_TRY(G_forward(n, nd, cd, B));
   if (diff_out) {
-    FG_TRY(k_nhwc_to_nchw(n->c, n->G_z[4], n->io, B, n->C, n->HW));
+    FG_TRY(k_nhwc_to_nchw(n->c, n->G_y(), n->io, B, n->C, n->HW));
     FG_TRY(fg_to_user(n->c, diff_out, n->io, (size_t)B * n->C * n->HW));
   }
   return FG_OK;
@@ -663,7 +784,7 @@ int fg_c2f_parzen_dist(fg_c2f* n, const float* noise, const float* coarse, const
     FG_CUDA(cudaMemcpyAsync(n->in_b + (size_t)k * img, coarse, img * sizeof(float), cudaMemcpyDefault, c->stream));
   FG_TRY(G_forward(n, nd, n->in_b, K));
   FG_TRY(k_nchw_to_nhwc(c, n->in_b, n->D_cond, K, n->C, n->HW));
-  FG_TRY(k_add(c, n->G_z[4], n->D_cond, n->io, (int64_t)K * img));  // neighbors:add(condInputs)  (:322)
+  FG_TRY(k_add(c, n->G_y(), n->D_cond, n->io, (int64_t)K * img));  // neighbors:add(condInputs)  (:322)
   FG_TRY(fg_to_dev(c, fine, img, n->in_a, &fd));
   FG_TRY(k_nchw_to_nhwc(c, fd, n->in_d, 1, n->C, n->HW));
   int32_t idx = 0;
@@ -672,7 +793,8 @@ int fg_c2f_parzen_dist(fg_c2f* n, const float* noise, const float* coarse, const
 
 // sample.lua:176-214 c2f(images, G, D, fineSize), `chunk` base images (chunk * tries rows of G and D) per pass; see
 // fg_b200.h.  Host inputs and outputs are staged through the net's buffers:
-//   gb    the chunk's images (C*in*in <= 256*S*S floats per image)     in_c  the caller's noise rows
+//   gb    the chunk's images (C*in*in <= 3*64*64 floats per image; gb holds at least 64*S*S >= 3*64*64 per
+//         row at S >= 16, G's first layer having 64 channels)          in_c  the caller's noise rows
 //   in_a  up (NCHW)      io  out on its way to the host      in_e  pick on its way to the host (int32 storage)
 // Nothing synchronises per chunk: host copies are ordered on the stream behind the kernels that fill their source.
 int fg_c2f_refine(fg_c2f* n, const float* images, int64_t N, int in_size, int tries, int chunk, int training, const float* noise,
@@ -707,13 +829,13 @@ int fg_c2f_refine(fg_c2f* n, const float* images, int64_t N, int in_size, int tr
       else
         FG_TRY(k_bernoulli_keep(c, n->D_masks, (int64_t)R * mask, 2 * seed + 1, 0.5f, nullptr, r0 * (int64_t)mask));
     }
-    FG_TRY(D_forward(n, n->G_z[4], n->D_cond, R, training != 0, 0.5f));
+    FG_TRY(D_forward(n, n->G_y(), n->D_cond, R, training != 0, 0.5f));
     FG_TRY(k_sigmoid_fwd(c, n->D_logit, n->D_out, R));
     float* od = out_dev ? out + s0 * img : n->io;
     int32_t* pk = pick_dev ? pick_out + s0 : (pick_out ? reinterpret_cast<int32_t*>(n->in_e) : nullptr);
     {
       ScopedTimer tm(c, n->t_refine_pick);
-      refine_pick_kernel<<<b, kRefineThreads, 0, c->stream>>>(n->D_out, n->G_z[4], n->in_a, C, HW, tries, od, pk);
+      refine_pick_kernel<<<b, kRefineThreads, 0, c->stream>>>(n->D_out, n->G_y(), n->in_a, C, HW, tries, od, pk);
       LAUNCH_CHECK(c);
     }
     if (!out_dev) FG_CUDA(cudaMemcpyAsync(out + s0 * img, od, sizeof(float) * b * img, cudaMemcpyDeviceToHost, c->stream));
@@ -773,14 +895,25 @@ int64_t fg_c2f_debug_tensor(fg_c2f* n, const char* name, float* dst, int64_t max
   const int gb = n->G_B, db = n->D_B, C = n->C, HW = n->HW;
   auto g = [&](const float* p) { return n->G_valid ? p : nullptr; };
   auto d = [&](const float* p) { return n->D_valid ? p : nullptr; };
-  auto dz = [&](int i) { return (int64_t)n->Dc[i].H * n->Dc[i].H * n->Dc[i].Cout; };
-  std::vector<DebugTensor> ents = {
-      {"G.x", g(n->G_x), HW * (C + 1), gb}, {"G.z1", g(n->G_z[0]), HW * 64, gb}, {"G.z2", g(n->G_z[1]), HW * 64, gb},
-      {"G.z3", g(n->G_z[2]), HW * 128, gb}, {"G.z4", g(n->G_z[3]), HW * 256, gb}, {"G.z5", g(n->G_z[4]), HW * C, gb},
-      {"D.x", d(n->D_x), HW * C, db}, {"D.z1", d(n->D_z[0]), dz(0), db}, {"D.z2", d(n->D_z[1]), dz(1), db},
-      {"D.z3", d(n->D_z[2]), dz(2), db}, {"D.z4", d(n->D_z[3]), dz(3), db}, {"D.p2", d(n->D_p2), HW / 4 * 64, db},
-      {"D.p4", d(n->D_p4), n->flat, db}, {"D.zl1", d(n->D_zl1), 512, db}, {"D.logit", d(n->D_logit), 1, db},
-      {"D.out", d(n->D_out), 1, db}};
+  std::vector<DebugTensor> ents = {{"G.x", g(n->G_x), HW * (C + 1), gb}, {"D.x", d(n->D_x), HW * C, db}};
+  std::deque<std::string> rows;  // the names of the per-layer rows (stable storage)
+  for (int i = 0; i < n->nGc; ++i) {
+    rows.push_back("G.z" + std::to_string(i + 1));
+    ents.push_back({rows.back().c_str(), g(n->G_z[i]), HW * n->Gc[i].Cout, gb});
+  }
+  for (int i = 0; i < n->nDc; ++i) {
+    const ConvL& L = n->Dc[i];
+    const int64_t e = (int64_t)L.H * L.H * L.Cout;
+    rows.push_back("D.z" + std::to_string(i + 1));
+    ents.push_back({rows.back().c_str(), d(n->D_z[i]), e, db});
+    if (n->D_p[i]) {
+      rows.push_back("D.p" + std::to_string(i + 1));
+      ents.push_back({rows.back().c_str(), d(n->D_p[i]), e / 4, db});
+    }
+  }
+  ents.push_back({"D.zl1", d(n->D_zl1), 512, db});
+  ents.push_back({"D.logit", d(n->D_logit), 1, db});
+  ents.push_back({"D.out", d(n->D_out), 1, db});
   pair_keep_rows(n->net, ents);
   return debug_tensor_copy(n->c, "fg_c2f_debug_tensor", ents.data(), ents.size(), name, dst, max_elems);
 }

@@ -116,6 +116,12 @@ SYMBOLS = {
     "fg_c2f_fine_size": (_I, [_P]),
     "fg_c2f_param_count_sized": (_L, [_I, _I, _I]),
     "fg_c2f_mask_per_sample_sized": (_I, [_I]),
+    "fg_c2f_create_nets": (_I, [_P, _I, _I, _I, C.POINTER(_P)]),
+    "fg_c2f_get_gen": (_I, [_P]),
+    "fg_c2f_get_disc": (_I, [_P]),
+    "fg_c2f_gen_param_count": (_L, [_I, _I]),
+    "fg_c2f_disc_param_count": (_L, [_I, _I, _I]),
+    "fg_c2f_disc_mask_per_sample": (_I, [_I, _I]),
     "fg_c2f_destroy": (_I, [_P]),
     "fg_c2f_param_count": (_L, [_I, _I]),
     "fg_c2f_mask_per_sample": (_I, []),
@@ -732,25 +738,71 @@ C2F_MASK_PER_SAMPLE = 16384 + 512
 C2F_FINE_SIZES = (16, 32, 64)
 
 
-def c2f_mask_per_sample(fine_size=32):
-    """nn.Dropout keep flags per sample of the coarse-to-fine D at fine size S: [256][S/4][S/4] then [512]"""
-    return 256 * (fine_size // 4) ** 2 + 512
+# models_c2f.lua's generators and discriminators by the name of the function that builds them (include/fg_b200.h
+# FG_C2F_G_* / FG_C2F_D_*); create_G / create_D resolve to create_G_d / create_D_c
+C2F_GENERATORS = {"create_G_d": 1, "create_G_a": 2, "create_G_b": 3, "create_G_c": 4}
+C2F_DISCRIMINATORS = {"create_D_c": 1, "create_D_a": 2, "create_D_b": 3}
+
+
+def c2f_gen_id(name):
+    """FG_C2F_G_* of a models_c2f.lua generator name ("create_G_a", ...)"""
+    if name not in C2F_GENERATORS:
+        raise FGError("unknown c2f generator %r: models_c2f.lua defines %s" % (name, ", ".join(sorted(C2F_GENERATORS))))
+    return C2F_GENERATORS[name]
+
+
+def c2f_disc_id(name):
+    """FG_C2F_D_* of a models_c2f.lua discriminator name ("create_D_a", ...)"""
+    if name not in C2F_DISCRIMINATORS:
+        raise FGError("unknown c2f discriminator %r: models_c2f.lua defines %s"
+                      % (name, ", ".join(sorted(C2F_DISCRIMINATORS))))
+    return C2F_DISCRIMINATORS[name]
+
+
+def _c2f_size(n, what):
+    """a count of the C ABI, or FGError for its -1 (a channel count below 1 or a fine size other than 16, 32, 64)"""
+    n = int(n)
+    if n < 0:
+        raise FGError("%s is not supported (channels >= 1; fine size 16, 32 or 64)" % what)
+    return n
+
+
+def c2f_gen_param_count(name, channels):
+    """length of the c2f generator's getParameters() vector"""
+    n = load_library().fg_c2f_gen_param_count(c2f_gen_id(name), channels)
+    return _c2f_size(n, "%s with %d channels" % (name, channels))
+
+
+def c2f_disc_param_count(name, channels, fine_size):
+    """length of the c2f discriminator's getParameters() vector at fine size S"""
+    n = load_library().fg_c2f_disc_param_count(c2f_disc_id(name), channels, fine_size)
+    return _c2f_size(n, "%s with %d channels at fine size %d" % (name, channels, fine_size))
+
+
+def c2f_mask_per_sample(fine_size=32, discriminator="create_D_c"):
+    """nn.Dropout keep flags per sample of a coarse-to-fine D at fine size S: its last pooled map (create_D_c:
+    [256][S/4][S/4]) then [512]"""
+    n = load_library().fg_c2f_disc_mask_per_sample(c2f_disc_id(discriminator), fine_size)
+    return _c2f_size(n, "%s at fine size %d" % (discriminator, fine_size))
 
 
 class C2f(_NetPair):
     """Coarse-to-fine nets + loop (train_c2f.lua) on a Context at fine size S = train_c2f.lua --fineSize (16, 32 or
-    64).  Mirrors lua/adversarial_c2f_b200.lua."""
+    64).  generator / discriminator: models_c2f.lua's nets by name (C2F_GENERATORS, C2F_DISCRIMINATORS; the defaults
+    are models_c2f.lua's create_G / create_D).  Mirrors lua/adversarial_c2f_b200.lua."""
     _prefix, _what = "fg_c2f_", "c2f "
 
-    def __init__(self, ctx, fine_size=32):
+    def __init__(self, ctx, fine_size=32, generator="create_G_d", discriminator="create_D_c"):
         self.ctx, self.lib, self.C = ctx, ctx.lib, ctx.C
+        gen, disc = c2f_gen_id(generator), c2f_disc_id(discriminator)
         h = C.c_void_p()
-        _check(self.lib.fg_c2f_create_sized(ctx.h, fine_size, C.byref(h)), "fg_c2f_create_sized")
+        _check(self.lib.fg_c2f_create_nets(ctx.h, fine_size, gen, disc, C.byref(h)), "fg_c2f_create_nets")
         self.h = h
+        self.generator, self.discriminator = generator, discriminator
         self.S = int(self.lib.fg_c2f_fine_size(h))
-        self.mask_per_sample = int(self.lib.fg_c2f_mask_per_sample_sized(self.S))
-        self.nG = int(self.lib.fg_c2f_param_count_sized(NET_G, self.C, self.S))
-        self.nD = int(self.lib.fg_c2f_param_count_sized(NET_D, self.C, self.S))
+        self.mask_per_sample = int(self.lib.fg_c2f_disc_mask_per_sample(disc, self.S))
+        self.nG = int(self.lib.fg_c2f_gen_param_count(gen, self.C))
+        self.nD = int(self.lib.fg_c2f_disc_param_count(disc, self.C, self.S))
 
     def close(self):
         if self.h:
@@ -777,7 +829,7 @@ class C2f(_NetPair):
     def D_forward(self, diff, cond, masks=None, training=True, seed=0):
         diff, cond = f32(diff), f32(cond)
         B = diff.shape[0]
-        masks = f32(masks) if masks is not None else None
+        masks = self._masks("D_forward masks", masks, B)
         out = np.empty(B, np.float32)
         _check(self.lib.fg_c2f_D_forward(self.h, _ptr(diff), _ptr(cond), B, int(training), _ptr(masks), seed, _ptr(out)),
                "fg_c2f_D_forward")
@@ -792,6 +844,7 @@ class C2f(_NetPair):
     def train_step(self, hyper, B, real_diff, cond_D, noise_D, cond_G, noise_G, masks_D=None, masks_G=None, seed=0,
                    want_stats=True):
         """Pointers may be numpy float32 arrays (host) or raw addresses (device / pinned)."""
+        masks_D, masks_G = self._masks("train_step masks_D", masks_D, B), self._masks("train_step masks_G", masks_G, B)
         st = StepStats() if want_stats else None
         _check(self.lib.fg_c2f_train_step(self.h, C.byref(hyper), B, _ptr(real_diff), _ptr(cond_D), _ptr(noise_D),
                                           _ptr(cond_G), _ptr(noise_G), _ptr(masks_D), _ptr(masks_G), seed,
@@ -812,6 +865,8 @@ class C2f(_NetPair):
         inputs stacked per iteration: real_diff [d][B/2], cond_D [d][B], noise_D [d][B/2], cond_G / noise_G [g][B],
         masks_* [d|g][B][mask_per_sample] or None."""
         d, g = check_iters(D_iterations, G_iterations)
+        masks_D = self._masks("train_step_iters masks_D", masks_D, d * B)
+        masks_G = self._masks("train_step_iters masks_G", masks_G, g * B)
         st = StepStats() if want_stats else None
         _check(self.lib.fg_c2f_train_step_iters(self.h, C.byref(hyper), B, d, g, _ptr(real_diff), _ptr(cond_D),
                                                 _ptr(noise_D), _ptr(cond_G), _ptr(noise_G), _ptr(masks_D), _ptr(masks_G),

@@ -17,13 +17,10 @@ local net = nil   -- fg_c2f*, created on first use, parameters uploaded from PAR
 
 local function c2f(ctx)
   if net == nil then
-    local out = ffi.new('fg_c2f*[1]')
-    -- train_c2f.lua --fineSize (16, 32 or 64) sizes both nets; IMG_DIMENSIONS / NOISE_DIM / COND_DIM follow it
-    F.check(C.fg_c2f_create_sized(ctx, OPT.fineSize, out), 'fg_c2f_create_sized')
-    net = out[0]
-    -- flat vectors are already in getParameters() order (train_c2f.lua:131-132)
-    F.check(C.fg_c2f_set_params(net, 0, F.ptr(PARAMETERS_G)), 'fg_c2f_set_params(G)')
-    F.check(C.fg_c2f_set_params(net, 1, F.ptr(PARAMETERS_D)), 'fg_c2f_set_params(D)')
+    -- train_c2f.lua --fineSize (16, 32 or 64) sizes both nets; IMG_DIMENSIONS / NOISE_DIM / COND_DIM follow it.
+    -- MODEL_G / MODEL_D may be any of models_c2f.lua's nets (models_c2f.create_G / create_D); the flat vectors are
+    -- already in getParameters() order (train_c2f.lua:131-132) and are checked against the recognised nets' lengths
+    net = b200.c2fNets(ctx, MODEL_G, MODEL_D, PARAMETERS_G, PARAMETERS_D, OPT.fineSize, IMG_DIMENSIONS[1])
   end
   return net
 end

@@ -19,6 +19,103 @@ local function disc_id(name, default)
   return d
 end
 
+-- models_c2f.lua's nets by the name of the function that builds them (FG_C2F_G_* / FG_C2F_D_*, include/fg_b200.h):
+-- G's "same" SpatialConvolutionUpsample layers {planes out, kernel} after the C+1 joined planes (0 = the C image
+-- channels), D's 3x3 convolutions {planes out, 2x2 max pool after}
+b200.C2F_GENERATORS = {
+  create_G_d = {id = 1, layers = {{64, 3}, {64, 3}, {128, 5}, {256, 5}, {0, 7}}},
+  create_G_a = {id = 2, layers = {{64, 3}, {128, 7}, {0, 5}}},
+  create_G_b = {id = 3, layers = {{64, 3}, {64, 3}, {256, 5}, {0, 7}}},
+  create_G_c = {id = 4, layers = {{64, 3}, {128, 3}, {256, 5}, {0, 7}}},
+}
+b200.C2F_DISCRIMINATORS = {
+  create_D_c = {id = 1, layers = {{64, false}, {64, true}, {128, false}, {256, true}}},
+  create_D_a = {id = 2, layers = {{64, false}, {64, true}}},
+  create_D_b = {id = 3, layers = {{64, false}, {64, true}, {128, false}, {128, true}}},
+}
+
+-- the convolutions of a module tree in module order, {planes out, planes in, kernel width, max pool after}; the
+-- CUDA-mode nn.Copy layers and every other leaf are skipped
+local function c2f_convs(net)
+  local convs = {}
+  local function walk(m)
+    if m.modules then
+      for _, child in ipairs(m.modules) do walk(child) end
+      return
+    end
+    local t = torch.type(m)
+    if t:find('Convolution') then
+      table.insert(convs, {m.nOutputPlane, m.nInputPlane, m.kW, false})
+    elseif t:find('SpatialMaxPooling') and #convs > 0 then
+      convs[#convs][4] = true
+    end
+  end
+  walk(net)
+  return convs
+end
+
+local function c2f_describe(convs)
+  local parts = {}
+  for _, c in ipairs(convs) do
+    table.insert(parts, string.format('%d->%d %dx%d%s', c[2], c[1], c[3], c[3], c[4] and ' pool' or ''))
+  end
+  return #parts > 0 and table.concat(parts, ', ') or 'none'
+end
+
+-- the entry of `nets` (C2F_GENERATORS or C2F_DISCRIMINATORS) whose layers the convolutions are, for `channels`
+-- image channels: name, FG_C2F_* id
+local function c2f_recognise(convs, channels, nets, isG)
+  for name, e in pairs(nets) do
+    if #e.layers == #convs then
+      local ok, cin = true, isG and channels + 1 or channels
+      for i, l in ipairs(e.layers) do
+        local cout = (isG and l[1] == 0) and channels or l[1]
+        local k, pool = isG and l[2] or 3, (not isG) and l[2] or false
+        local c = convs[i]
+        if c[1] ~= cout or c[2] ~= cin or c[3] ~= k or c[4] ~= pool then
+          ok = false
+          break
+        end
+        cin = cout
+      end
+      if ok then return name, e.id end
+    end
+  end
+  return nil
+end
+
+-- the fg_c2f for the models_c2f.lua nets G and D (recognised from their convolutions' kernel sizes and plane counts)
+-- at fineSize on ctx, with their flat parameter vectors pG / pD (G:getParameters() order) uploaded.  A net that is
+-- none of models_c2f.lua's, or a vector of another length, is refused before anything is copied.
+function b200.c2fNets(ctx, G, D, pG, pD, fineSize, channels)
+  local gc, dc = c2f_convs(G), c2f_convs(D)
+  local gName, gId = c2f_recognise(gc, channels, b200.C2F_GENERATORS, true)
+  assert(gName, 'b200: G is not one of models_c2f.lua\'s generators for ' .. channels .. ' channels; its convolutions: '
+         .. c2f_describe(gc))
+  local dName, dId = c2f_recognise(dc, channels, b200.C2F_DISCRIMINATORS, false)
+  assert(dName, 'b200: D is not one of models_c2f.lua\'s discriminators for ' .. channels .. ' channels; its convolutions: '
+         .. c2f_describe(dc))
+  local nG = tonumber(C.fg_c2f_gen_param_count(gId, channels))
+  local nD = tonumber(C.fg_c2f_disc_param_count(dId, channels, fineSize))
+  assert(nD >= 0, 'b200: fine size ' .. tostring(fineSize) .. ' is not supported (16, 32 or 64)')
+  assert(pG:nElement() == nG, string.format('b200: G (%s) has %d parameters, the c2f net expects %d', gName,
+                                            pG:nElement(), nG))
+  assert(pD:nElement() == nD, string.format('b200: D (%s) has %d parameters, %s at fine size %d expects %d', dName,
+                                            pD:nElement(), dName, fineSize, nD))
+  local out = ffi.new('fg_c2f*[1]')
+  F.check(C.fg_c2f_create_nets(ctx, fineSize, gId, dId, out), 'fg_c2f_create_nets')
+  local net = out[0]
+  for i, p in ipairs({pG, pD}) do
+    local rc = C.fg_c2f_set_params(net, i - 1, F.ptr(p))
+    if rc ~= 0 then
+      local msg = ffi.string(C.fg_last_error())
+      C.fg_c2f_destroy(net)   -- a failed upload leaves no half-initialised net behind
+      error(string.format('fg_c2f_set_params(%s) failed (%d): %s', i == 1 and 'G' or 'D', rc, msg))
+    end
+  end
+  return net, gName, dName
+end
+
 -- one context per process/GPU, created lazily from OPT (train.lua:16-50); discriminator: 'create_D32b' (default)
 -- or 'create_D32'
 function b200.context(device, maxBatch, channels, discriminator)

@@ -81,6 +81,14 @@ int fg_c2f_create_sized(fg_ctx* ctx, int fine_size, fg_c2f** out);
 int fg_c2f_fine_size(fg_c2f* n);
 int64_t fg_c2f_param_count_sized(int net, int channels, int fine_size);
 int fg_c2f_mask_per_sample_sized(int fine_size);
+enum { FG_C2F_G_DEFAULT = 0, FG_C2F_G_D = 1, FG_C2F_G_A = 2, FG_C2F_G_B = 3, FG_C2F_G_C = 4 };
+enum { FG_C2F_D_DEFAULT = 0, FG_C2F_D_C = 1, FG_C2F_D_A = 2, FG_C2F_D_B = 3 };
+int fg_c2f_create_nets(fg_ctx* ctx, int fine_size, int gen, int disc, fg_c2f** out);
+int fg_c2f_get_gen(fg_c2f* n);
+int fg_c2f_get_disc(fg_c2f* n);
+int64_t fg_c2f_gen_param_count(int gen, int channels);
+int64_t fg_c2f_disc_param_count(int disc, int channels, int fine_size);
+int fg_c2f_disc_mask_per_sample(int disc, int fine_size);
 int fg_c2f_destroy(fg_c2f* n);
 int64_t fg_c2f_param_count(int net, int channels);
 int fg_c2f_mask_per_sample(void);

@@ -20,17 +20,17 @@ local TRIES = 10         -- sample.lua:177 triesPerImage
 local nets = {}          -- fineSize -> {net = fg_c2f*, G = G, D = D}
 local calls = 0
 
-local function c2f_net(ctx, G, D, fineSize)
+local function c2f_net(ctx, G, D, fineSize, channels)
   local e = nets[fineSize]
   if e == nil or e.G ~= G or e.D ~= D then
-    if e ~= nil then C.fg_c2f_destroy(e.net) end
-    local out = ffi.new('fg_c2f*[1]')
-    F.check(C.fg_c2f_create_sized(ctx, fineSize, out), 'fg_c2f_create_sized')
+    if e ~= nil then
+      C.fg_c2f_destroy(e.net)
+      nets[fineSize] = nil   -- if building the new net fails, no later call may get the destroyed one back
+    end
+    -- G and D may be any of models_c2f.lua's nets; their parameter vectors are checked against the recognised nets
     local pG = G:getParameters():float():contiguous()
     local pD = D:getParameters():float():contiguous()
-    F.check(C.fg_c2f_set_params(out[0], 0, F.ptr(pG)), 'fg_c2f_set_params(G)')
-    F.check(C.fg_c2f_set_params(out[0], 1, F.ptr(pD)), 'fg_c2f_set_params(D)')
-    e = {net = out[0], G = G, D = D}
+    e = {net = b200.c2fNets(ctx, G, D, pG, pD, fineSize, channels), G = G, D = D}
     nets[fineSize] = e
   end
   return e.net
@@ -41,7 +41,7 @@ function sample_b200.c2f(images, G, D, fineSize)
   local N = #images
   local channels, inSize = images[1]:size(1), images[1]:size(2)
   local ctx = b200.context(OPT and OPT.gpu or 0, TRIES * 16, channels)
-  local net = c2f_net(ctx, G, D, fineSize)
+  local net = c2f_net(ctx, G, D, fineSize, channels)
   -- as many images per pass as the ctx's batch holds (the result does not depend on it)
   local chunk = math.max(1, math.floor(tonumber(C.fg_get_option(ctx, 'max_batch')) / TRIES))
   local batch = torch.FloatTensor(N, channels, inSize, inSize)

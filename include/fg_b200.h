@@ -267,26 +267,55 @@ int fg_train_step(fg_ctx* ctx, const fg_hyper* h, int B, const float* real, cons
 int fg_sample(fg_ctx* ctx, const float* noise, int N, int chunk, float* images_out);
 
 /* ---- coarse-to-fine GAN (train_c2f.lua; BASELINE configs[3]) --------------------------------- */
-/* G = models_c2f.lua:113-145 create_G_d, D = models_c2f.lua:237-278 create_D_c, both at the fine
- * size S = train_c2f.lua --fineSize (16, 32 or 64; fg_c2f_create: 32) on the ctx's channel count.
+/* G = models_c2f.lua:113-145 create_G_d, D = models_c2f.lua:237-278 create_D_c (or another pair of
+ * models_c2f.lua's nets, fg_c2f_create_nets), both at the fine size S = train_c2f.lua --fineSize (16, 32
+ * or 64; fg_c2f_create: 32) on the ctx's channel count.
  * Every image, noise and mask buffer below is at the net's S: images [B][C][S][S], noise
- * [B][1][S][S], masks [B][fg_c2f_mask_per_sample_sized(S)].  cudnn.SpatialConvolutionUpsample with factor 1
- * (layers/cudnnSpatialConvolutionUpsample.lua) is a "same" convolution.  The object borrows the
+ * [B][1][S][S], masks [B][fg_c2f_disc_mask_per_sample(D, S)].  cudnn.SpatialConvolutionUpsample with
+ * factor 1 (layers/cudnnSpatialConvolutionUpsample.lua) is a "same" convolution.  The object borrows the
  * ctx (stream, device, DP communicator, "conv_impl"); destroy it before the ctx.  Flat parameter
  * vectors follow getParameters() order: G [c1W c1b a1 ... c4W c4b a4 c5W c5b], D [c1W c1b a1 ...
- * c4W c4b a4 L1W L1b a5 L2W L2b].                                                                 */
+ * c4W c4b a4 L1W L1b a5 L2W L2b] (create_G_d / create_D_c; the other nets the same per layer).       */
 typedef struct fg_c2f fg_c2f;
 int fg_c2f_create(fg_ctx* ctx, fg_c2f** out);            /* fg_c2f_create_sized(ctx, 32, out)      */
-/* any fine size other than 16, 32, 64 -> FG_ERR_UNSUPPORTED before anything is allocated          */
+/* fg_c2f_create_nets(ctx, fine_size, FG_C2F_G_DEFAULT, FG_C2F_D_DEFAULT, out); any fine size other
+ * than 16, 32, 64 -> FG_ERR_UNSUPPORTED before anything is allocated                               */
 int fg_c2f_create_sized(fg_ctx* ctx, int fine_size, fg_c2f** out);
 int fg_c2f_fine_size(fg_c2f* n);
 int fg_c2f_destroy(fg_c2f* n);
 int64_t fg_c2f_param_count(int net, int channels);        /* 1 101 319 / 8 797 382 for colour      */
 int fg_c2f_mask_per_sample(void);                         /* 16896 = [256][8][8] + [512] nn.Dropout */
 /* at fine size S: G unchanged, D's Linear 256*(S/4)^2 -> 512 (colour D: 2 505 926 at 16, 33 963 206
- * at 64); keep flags [256][S/4][S/4] + [512] (4608 / 16896 / 66048); -1 for an unsupported size    */
+ * at 64); keep flags [256][S/4][S/4] + [512] (4608 / 16896 / 66048); -1 for an unsupported size.
+ * These four always describe the default pair, create_G_d / create_D_c.                            */
 int64_t fg_c2f_param_count_sized(int net, int channels, int fine_size);
 int fg_c2f_mask_per_sample_sized(int fine_size);
+/* models_c2f.lua's generators and discriminators; create_G / create_D pick create_G_d / create_D_c     */
+enum {
+  FG_C2F_G_DEFAULT = 0, /* create_G_d                                                               */
+  FG_C2F_G_D = 1,       /* models_c2f.lua:113-145 create_G_d (64,3) (64,3) (128,5) (256,5) (C,7)    */
+  FG_C2F_G_A = 2,       /* models_c2f.lua:16-45   create_G_a (64,3) (128,7) (C,5)                   */
+  FG_C2F_G_B = 3,       /* models_c2f.lua:47-78   create_G_b (64,3) (64,3) (256,5) (C,7)            */
+  FG_C2F_G_C = 4        /* models_c2f.lua:80-111  create_G_c (64,3) (128,3) (256,5) (C,7)           */
+};
+enum {
+  FG_C2F_D_DEFAULT = 0, /* create_D_c                                                               */
+  FG_C2F_D_C = 1,       /* models_c2f.lua:237-278 create_D_c 64, 64 pool, 128, 256 pool             */
+  FG_C2F_D_A = 2,       /* models_c2f.lua:156-192 create_D_a 64, 64 pool                            */
+  FG_C2F_D_B = 3        /* models_c2f.lua:194-235 create_D_b 64, 64 pool, 128, 128 pool             */
+};
+/* the c2f nets with generator `gen` (FG_C2F_G_*) and discriminator `disc` (FG_C2F_D_*); an unknown net
+ * or fine size -> FG_ERR_UNSUPPORTED before anything is allocated.  Every fg_c2f_* entry point then
+ * follows that pair: parameter vectors fg_c2f_gen_param_count / fg_c2f_disc_param_count long, keep
+ * flags fg_c2f_disc_mask_per_sample wide.                                                           */
+int fg_c2f_create_nets(fg_ctx* ctx, int fine_size, int gen, int disc, fg_c2f** out);
+int fg_c2f_get_gen(fg_c2f* n);                   /* FG_C2F_G_* of G (never DEFAULT); < 0 on error       */
+int fg_c2f_get_disc(fg_c2f* n);                  /* FG_C2F_D_* of D (never DEFAULT); < 0 on error       */
+/* getParameters() lengths and D's keep flags per sample (the pooled map View flattens, in NCHW order,
+ * then [512]); no GPU needed; -1 for an unknown net, a channel count < 1 or an unsupported fine size  */
+int64_t fg_c2f_gen_param_count(int gen, int channels);
+int64_t fg_c2f_disc_param_count(int disc, int channels, int fine_size);
+int fg_c2f_disc_mask_per_sample(int disc, int fine_size);
 int fg_c2f_set_params(fg_c2f* n, int net, const float* src);
 int fg_c2f_get_params(fg_c2f* n, int net, float* dst);
 int fg_c2f_get_grads(fg_c2f* n, int net, float* dst);

@@ -15,6 +15,9 @@ that differs and the launches per step of both builds; a case differs when eithe
 
 One build per process: both libraries export the same symbols.
 
+The c2f group also runs the default pair at every fine size, batch 256 and 130, mma_f16 1 and 0; the c2fvar group (not
+in the default --only) runs models_c2f.lua's other generators and discriminators, for builds that have them.
+
 usage:  python profiles/ab_state.py run --lib face_generator_b200/libfg_b200.so --out /tmp/ab/new [--only 32,s16,dbr,c2f,lop,dn,ae]
         python profiles/ab_state.py compare /tmp/ab/old /tmp/ab/new
 """
@@ -172,7 +175,7 @@ def case_s16(B, opts, imgs, mode="step", discriminator=None):
     return out, launches
 
 
-def case_c2f(B, imgs, S=32, mode="step"):
+def case_c2f(B, imgs, S=32, mode="step", generator="create_G_d", discriminator="create_D_c", opts=None):
     import face_generator_b200 as fg
     from face_generator_b200 import layouts as LY
     from face_generator_b200.dataset import DeviceDataset, noise_uniform
@@ -180,11 +183,21 @@ def case_c2f(B, imgs, S=32, mode="step"):
     rng = np.random.default_rng(51)
     cs = S // 2  # train_c2f.lua --coarseSize
     ctx = fg.Context(0, max_batch=B, channels=C)
+    for k, v in (opts or {}).items():
+        ctx.set_option(k, v)
     if mode == "debug_keep":
         ctx.set_option("debug_keep", 1)
-    net = fg.C2f(ctx, S)
-    net.set_params(NET_G, LY.trained_like_init(LY.c2f_G_layout(C), rng, 1.2))
-    net.set_params(NET_D, LY.trained_like_init(LY.c2f_D_layout(C, S), rng, 1.0))
+    # the default pair through the two-argument form, which every build of C2f takes
+    default = (generator, discriminator) == ("create_G_d", "create_D_c")
+    net = fg.C2f(ctx, S) if default else fg.C2f(ctx, S, generator, discriminator)
+    if generator == "create_G_d":
+        net.set_params(NET_G, LY.trained_like_init(LY.c2f_G_layout(C), rng, 1.2))
+    else:
+        net.set_params(NET_G, f32(rng.standard_normal(net.count(NET_G)) * 0.02))
+    if discriminator == "create_D_c":
+        net.set_params(NET_D, LY.trained_like_init(LY.c2f_D_layout(C, S), rng, 1.0))
+    else:
+        net.set_params(NET_D, f32(rng.standard_normal(net.count(NET_D)) * 0.02))
     ds = DeviceDataset(ctx, imgs)
     h = fg.hyper_default()
     out = {}
@@ -340,6 +353,12 @@ def run(args):
     if "c2f" in only:
         cases.append(("c2f.B256.default", lambda: case_c2f(256, imgs)))
         cases += [("c2f%d.B256.default" % S, lambda S=S: case_c2f(256, imgs, S)) for S in (16, 64)]
+        cases += [("c2f%d.B%d.mma_f16=%d" % (S, B, f), lambda S=S, B=B, f=f: case_c2f(B, imgs, S, opts={"mma_f16": f}))
+                  for S in (16, 32, 64) for B in (256, 130) for f in (1, 0)]
+    if "c2fvar" in only:  # models_c2f.lua's other generators and discriminators (builds that have them)
+        cases += [("c2fvar.%s.%s.S%d" % (g[7:], d[7:], S), lambda g=g, d=d, S=S: case_c2f(256, imgs, S, "step", g, d))
+                  for g, d in (("create_G_a", "create_D_c"), ("create_G_b", "create_D_c"), ("create_G_c", "create_D_c"),
+                               ("create_G_d", "create_D_a"), ("create_G_d", "create_D_b")) for S in (16, 32, 64)]
     if "lop" in only:
         cases.append(("lop.conv2d_f16", case_lop))
     if "dn" in only:
